@@ -5,8 +5,12 @@
   python bench.py --impl reference --gpus N --steps K ...  (the reference algorithm on the host CPU cores)
 
 One "step" = one pass of the hot path over one batch of 32 synthetic frames per GPU (BASELINE.json configs[2] /
-configs[3]: batch 32 per B200, bf16, fused post-processing).  Weights: seeded He-normal (SURVEY.md 8c), inputs:
+configs[3]: batch 32 per GPU, bf16, fused post-processing).  Weights: seeded He-normal (SURVEY.md 8c), inputs:
 seeded uniform [-0.5, 0.5).  Prints ONE JSON line on rank 0.
+
+  --dump-outputs DIR   after the timed steps, write what the last timed step computed - per image the person rows and
+                       the peaks a caller of the path reads back - as DIR/<name>.npy (float32 / float64), so that two
+                       builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import datetime
@@ -37,13 +41,15 @@ def peaks(clocks):
     figure applies when the clock sampler saw sw_power_cap or a median clock well below the maximum."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     capped = (clocks is None or "sw_power_cap" in (clocks.get("reasons") or []) or not clocks.get("sm_mhz")
-              or clocks["sm_mhz"] < 0.97 * clocks.get("sm_max_mhz", 1965.0))
+              or clocks["sm_mhz"] < 0.97 * clocks.get("sm_max_mhz", 1980.0))
     if os.path.exists(p):
         d = json.load(open(p))
-        tf = d.get("bf16_tflops_sustained", 1400.0) if capped else d.get("bf16_tflops", 1590.0)
-        return tf, d.get("hbm_gbs", 6650.0), "of measured (MEASURED_PEAKS.json, %s)" % ("bf16_tflops_sustained: power cap / reduced clock seen"
+        tf = d.get("bf16_tflops_sustained", 989.0) if capped else d.get("bf16_tflops", 989.0)
+        return tf, d.get("hbm_gbs", 3350.0), "of measured (MEASURED_PEAKS.json, %s)" % ("bf16_tflops_sustained: power cap / reduced clock seen"
                                                                                      if capped else "bf16_tflops burst: max SM clock, no power cap seen")
-    return (1400.0 if capped else 1590.0), 6650.0, "of fallback (B200_PROFILING.md, %s)" % ("sustained" if capped else "burst")
+    return 989.0, 3350.0, "of the H100 SXM data sheet (dense BF16, HBM3; not a measured peak; %s)" % (
+        "sustained: power cap / reduced clock seen, the card runs below the data-sheet rate" if capped
+        else "burst: max SM clock, no power cap seen")
 
 
 class ClockSampler:
@@ -193,12 +199,12 @@ def run_ours(args):
     eng = engine.PoseEngine(arrays, local, mode=args.mode, batch_cap=BATCH, peak_cap=1024, human_cap=512)
 
     # Frames are uint8 HWC BGR (what cv2.imread / crop_with_factor hand to get_outputs); rtpose_preprocess is fused
-    # into the first convolution.  10 rotating device batches (10 x 13 MB > 126 MB L2) + 2 pinned host batches.
+    # into the first convolution.  10 rotating device batches (10 x 13 MB > 50 MB L2) + 2 pinned host batches.
     g = torch.Generator().manual_seed(1234 + rank)
     # --raw N: the frames are N x N "camera" frames and crop_with_factor (resize to 368 x 368) runs on the device too
     SH = SW = args.raw if args.raw else H          # (multi-scale: the raw frames are 368 x 368 unless --raw says otherwise)
     host = [torch.randint(0, 256, (BATCH, SH, SW, 3), generator=g, dtype=torch.uint8).pin_memory() for _ in range(2)]
-    # enough rotating device batches that one full rotation exceeds the 126 MB L2 (10 at batch 32)
+    # enough rotating device batches that one full rotation exceeds the 50 MB L2 several times over (10 at batch 32)
     n_rot = max(10, -(-130_000_000 // (BATCH * SH * SW * 3)))
     devin = [torch.randint(0, 256, (BATCH, SH, SW, 3), generator=g, dtype=torch.uint8).to(dev) for i in range(n_rot)]
     torch.cuda.synchronize()
@@ -222,7 +228,7 @@ def run_ours(args):
         infer_u8 = eng.infer_flip_async_u8 if args.flip else eng.infer_async_u8
 
     def step_device(i):
-        infer_u8(devin[i % n_rot].data_ptr(), True, BATCH, H, W, 0.1, sptr)
+        return infer_u8(devin[i % n_rot].data_ptr(), True, BATCH, H, W, 0.1, sptr)
 
     d2h_bytes = []
 
@@ -264,7 +270,7 @@ def run_ours(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(stream)
     for i in range(args.steps):
-        step_device(i)
+        last_ticket = step_device(i)
     eng.post.sync()          # the last step's assembly + result copy run on the engine's second stream
     e1.record(stream)
     torch.cuda.synchronize()
@@ -272,6 +278,8 @@ def run_ours(args):
     launches = nat.launch_count() - l0
     clocks = sampler.stop() if sampler else None
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, last_ticket)
 
     # ---- end-to-end timing through the public API with host buffers (e2e): every step copies its uint8 frames from
     # pinned host memory and its results back; two runs are kept in flight (submit i+1, then read i), K results are read
@@ -323,12 +331,10 @@ def run_ours(args):
             net_ms = tot_ms / 3 + first_ms
             net_fl = tot_fl / 3 + fl[0]
             step_ms = ms_dev / args.steps
-            roof = {"bound": "tensor", "kernel": "conv_tc_kernel (%d launches/step, all tcgen05 convs)" % (nl - 1),
+            roof = {"bound": "tensor", "kernel": "conv_tc_kernel (%d launches/step, all wgmma convs)" % (nl - 1),
                     "achieved": round(ach, 1), "peak": pk_tf, "unit": "TFLOP/s", "frac": round(ach / pk_tf, 4),
-                    # DRAM bytes per launch cannot be read inside a timed run (it needs ncu's replay); the figure of the
-                    # committed ncu capture of this command is in the file named below
+                    # DRAM bytes per launch cannot be read inside a timed run (it needs a profiler's replay)
                     "traffic": None,
-                    "traffic_source": "profiles/r02_conv_tc_dram.csv (ncu dram__bytes_read.sum + dram__bytes_write.sum per launch)",
                     "peak_source": pk_src,
                     "share_of_step": round(tot_ms / 3 / step_ms, 3),
                     # the same arithmetic over the whole network (conv1_1 included) and over the whole step
@@ -384,7 +390,7 @@ def run_ours(args):
         "scaling": "weak", "vs_baseline": None, "dtype": {"bf16": "bf16", "bf16x3": "bf16x3 (hi+lo bf16 planes, fp32 accumulate)", "fp32": "f32"}[args.mode],
         "data": "synthetic",
         "config": {"workload": "batch=%d per GPU, 368x368, rtpose VGG19 %s + fused NMS/PAF-match/assembly%s"
-                               % (BATCH, {"bf16": "bf16 (tcgen05)", "bf16x3": "bf16x3 (tcgen05, split precision)", "fp32": "fp32 (CUDA cores, parity mode)"}[args.mode],
+                               % (BATCH, {"bf16": "bf16 (wgmma)", "bf16x3": "bf16x3 (wgmma, split precision)", "fp32": "fp32 (CUDA cores, parity mode)"}[args.mode],
                                   (", multi-scale test-time averaging at scales %s%s (BASELINE.json configs[4]; %d forwards per frame; the "
                                    "composition has no reference counterpart: parity unpinned, DESIGN.md 2.7)"
                                    % (args.scales, " x left/right flip" if args.flip else "", len(scales) * (2 if args.flip else 1))) if scales else
@@ -393,7 +399,7 @@ def run_ours(args):
                    "global_batch": BATCH * world, "weights": "He-normal seed 1234 (random init)",
                    "input": ("uint8 HWC BGR %dx%d frames, crop_with_factor (bilinear resize to 368x368) and rtpose_preprocess on "
                              "the device" % (SH, SW)) if args.raw else "uint8 HWC BGR frames, rtpose_preprocess fused on the device",
-                   "l2": "inputs rotate over %d device batches (%d MB > 126 MB L2); ~%d MB of activations per step"
+                   "l2": "inputs rotate over %d device batches (%d MB > 50 MB L2); ~%d MB of activations per step"
                          % (n_rot, n_rot * BATCH * SH * SW * 3 // 1000000, 44 * BATCH * (2 if args.flip else 1)),
                    "parallelism": "dp%d (frames sharded, one NCCL weight broadcast)" % world,
                    "post_status_bits": int(status_bits),
@@ -408,6 +414,37 @@ def run_ours(args):
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, eng, ticket):
+    """The results of run `ticket` as the caller of the timed path reads them back: person rows (float32 [k, 73]: score,
+    18 x (x, y, peak score, peak id | -1)) and peaks (float32 [P, 5]: x, y, score, id, part) of every image, concatenated
+    in image order, with the per-image counts (float64).  Images beyond what fits in 64 MB are left out, the kept ones
+    chosen by a fixed seed."""
+    eng.post.select(ticket)
+    humans = [eng.post.humans(k).reshape(-1, 73) for k in range(BATCH)]
+    peaks = [eng.post.peaks(k).reshape(-1, 5) for k in range(BATCH)]
+    keep = list(range(BATCH))
+    size = lambda ks: sum(humans[k].nbytes + peaks[k].nbytes + 16 for k in ks)
+    if size(keep) > DUMP_LIMIT:
+        order = np.random.default_rng(0).permutation(BATCH).tolist()
+        keep = []
+        for k in order:
+            if size(keep + [k]) > DUMP_LIMIT:
+                break
+            keep.append(k)
+        keep.sort()
+    out = {"image_index": np.array(keep, np.float64),
+           "humans": np.concatenate([humans[k] for k in keep]).astype(np.float32),
+           "humans_per_image": np.array([len(humans[k]) for k in keep], np.float64),
+           "peaks": np.concatenate([peaks[k] for k in keep]).astype(np.float32),
+           "peaks_per_image": np.array([len(peaks[k]) for k in keep], np.float64)}
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def cpu_frame_fn():
@@ -502,6 +539,8 @@ def main():
                     help="multi-scale test-time averaging around 368 (BASELINE.json configs[4]: 0.5,1.0,1.5,2.0 with --flip --batch 8)")
     ap.add_argument("--raw", type=int, default=0, metavar="N",
                     help="feed N x N raw frames and run crop_with_factor (resize to 368 x 368) on the device as well")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's person rows and peaks as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     global BATCH

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Single-picture demo on the B200 path, with the command line, the files and the flow of the reference's
+"""Single-picture demo on the H100 path, with the command line, the files and the flow of the reference's
 demo/picture_demo.py (:30-65): `--cfg` (default ./experiments/vgg19_368x368_sgd.yaml), `--weight` (default
 pose_model.pth), trailing config overrides; reads ./readme/ski.jpg, prints im_scale, writes result.png.  Run from the
 repo root, like the reference.  The reference's own script runs unmodified against this repo as well (its imports are

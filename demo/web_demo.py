@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Camera front-end on the B200 path: the flow and command line of the reference's demo/web_demo.py (:29-71) - camera 0,
+"""Camera front-end on the H100 path: the flow and command line of the reference's demo/web_demo.py (:29-71) - camera 0,
 every frame through the network and the post-processing, the drawn frame shown until `q` is pressed - with the capture of
 frame i+1 overlapped with the inference of frame i (streaming.PoseStream, batch 1).  Extras: `--source` (a camera index
 or a file), `--no-window` (headless: count frames instead of cv2.imshow), `--max-frames`, `--synthetic-weights`.

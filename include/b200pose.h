@@ -1,4 +1,4 @@
-/* b200pose - C ABI of the B200-native OpenPose (rtpose VGG19) inference path.
+/* b200pose - C ABI of the H100-native OpenPose (rtpose VGG19) inference path.
  *
  * Plain pointers and sizes only; no torch / numpy types.  Every entry point returns 0 on success and a
  * non-zero code on failure (b200pose_last_error() gives the text) unless stated otherwise.
@@ -7,7 +7,7 @@
  * nothing themselves - use one object per host thread (or your own lock).  All work of a call is enqueued on the
  * cuda_stream argument (plus the post object's private second stream for the person assembly and result copies).
  *
- * Each declaration cites the reference interface it replaces (paths relative to /root/reference).
+ * Each declaration cites the reference interface it replaces (paths relative to the reference repository).
  * The reference-side bindings (ctypes) are shown in INTEGRATION.md.
  */
 #ifndef B200POSE_H

@@ -127,7 +127,7 @@ struct TcLayer {            // one grouped tensor-core launch
 }  // namespace
 
 struct b200pose_net {
-    int device = 0, num_sms = 148;
+    int device = 0, num_sms = 0;
     bool finalized = false;
     std::vector<std::vector<float>> host_w, host_b;   // per conv
     std::vector<bool> have;                            // per tensor
@@ -152,8 +152,6 @@ struct b200pose_net {
     };
     bool plan_cache_on = true;
     bool conv_pdl = true;             // programmatic dependent launch between the layers of small-batch plans (B200POSE_CONV_PDL=0: never)
-    bool conv_narrow = true;          // 8 x 16 pixel tiles for layers that fill less than half of the SMs (B200POSE_CONV_NARROW=0: never)
-    bool conv_pair = true;            // tcgen05 cta_group::2 CTA pairs for the N >= 64 layers (B200POSE_CONV_PAIR=0: single CTAs)
     // The 52 launches of a forward pass are captured at the second use of a (shape, mode, input pointer) into a CUDA graph and replayed
     // (B200POSE_GRAPH=0: plain launches).  Graphs embed the tensor maps, i.e. buffer addresses: every plan build drops them.
     // Capture needs a real stream: calls on the legacy default stream (0) launch directly.
@@ -211,9 +209,8 @@ struct b200pose_post {
     int hw_h = 0, hw_w = 0;
     // Peaks / limbs / assembly of run i all run on the second stream from a private copy of the maps (15 MB at batch 32),
     // so that the caller's stream is free for the convolutions of run i+1: the small kernels (peaks, assembly) co-reside
-    // with the conv CTAs and the limbs blocks fill the SMs the conv launches leave idle in their last wave
-    // (measured on B200, batch 32: 14.23 -> 13.52 ms per step device-resident, 14.26 -> 13.15 end to end;
-    // profiles/r02_variants.txt).  B200POSE_POST_OVERLAP=0 keeps everything on the caller's stream.
+    // with the conv CTAs and the limbs blocks fill the SMs the conv launches leave idle in their last wave.
+    // B200POSE_POST_OVERLAP=0 keeps everything on the caller's stream.
     bool overlap = true;
     DevBuf<float> ov_maps[2];                       // [heat | paf] copies, slot = run parity
     cudaEvent_t ev_maps = nullptr, ev_ld[2] = {nullptr, nullptr};   // maps copied (st) / limbs done with a slot (s2)
@@ -260,9 +257,9 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_id
     return 0;
 }
 
-// Small-batch plans: the 46 x 46 stage layers would fill less than half of the SMs with 16 x 16 tiles.  Their launches are the
-// launch-bound part of the product: they are chained by PDL and replayed as a CUDA graph; the large plans are GPU-bound and
-// get neither (PDL measured -2 % there; a capture only adds a CPU hiccup).
+// Small-batch plans: the 46 x 46 stage layers (two groups) would fill at most half of the SMs with one n-tile per group.
+// Their launches are the launch-bound part of the product: they are chained by PDL and replayed as a CUDA graph; the large
+// plans are GPU-bound and get neither (a capture only adds a CPU hiccup).
 bool small_plan(const b200pose_net* net, int n, int H, int W) {
     return 2 * n * ((H / 8 + kTileH - 1) / kTileH) * ((W / 8 + kTileW - 1) / kTileW) * 2 <= net->num_sms;
 }
@@ -275,20 +272,13 @@ int add_plan(b200pose_net* net, const TcLayer& L, int n, int H, int W, const __n
     a.n_img = n; a.H = H; a.W = W; a.ksize = L.ks; a.cin_blocks = L.cin_blocks;
     a.in_ch_base = in_ch_base; a.in_ch_group_stride = in_group_stride; a.groups = L.groups;
     a.n_tile = L.n_tile; a.n_tiles = L.n_tiles; a.bias = L.bias; a.relu = L.relu; a.pool = L.pool;
-    {   // small batches: while the layer's CTAs fill less than half of the SMs, halve the work per CTA - 128-wide n-tiles
-        // become 64-wide, then the 16 x 16 pixel tile becomes 8 x 16 (one UMMA sub-tile), then 64-wide n-tiles become
-        // 32-wide (the weight layout does not depend on the n-tile).  B200POSE_CONV_NARROW=0 keeps the 16 x 16 tiles.
-        auto ctas = [&](int narrow, int n_tiles) {
-            const int pix = n * ((H + kTileH - 1) / kTileH) * ((W + (narrow ? 8 : kTileW) - 1) / (narrow ? 8 : kTileW));
-            return (net->conv_pair ? (pix + 1) / 2 * 2 : pix) * L.groups * n_tiles;
-        };
-        if (L.n_tile == 128 && 2 * ctas(0, a.n_tiles) <= net->num_sms) { a.n_tile = 64; a.n_tiles = L.n_tiles * 2; }
-        if (net->conv_narrow && 2 * ctas(0, a.n_tiles) <= net->num_sms) {
-            a.narrow = 1;
-            if (a.n_tile == 64 && net->conv_pair && 2 * ctas(1, a.n_tiles) <= net->num_sms) { a.n_tile = 32; a.n_tiles *= 2; }
-        }
+    {   // small batches: while the layer's CTAs fill at most half of the SMs, halve the work per CTA - 128-wide n-tiles become
+        // 64-wide, then 32-wide (the weight layout does not depend on the n-tile)
+        const int pix = n * ((H + kTileH - 1) / kTileH) * ((W + kTileW - 1) / kTileW);
+        if (L.n_tile == 128 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 64; a.n_tiles = L.n_tiles * 2; }
+        if (a.n_tile == 64 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 32; a.n_tiles *= 2; }
     }
-    if (net->plan_split) {     // bf16x3: K-chunked accumulation, one 32-column chunk per epilogue warp, so N <= 64
+    if (net->plan_split) {     // bf16x3: K-chunked accumulation in a second register set, so N <= 64
         a.chunk = 1;
         if (a.n_tile > 64) { a.n_tile = 64; a.n_tiles = L.n_tiles * (L.n_tile / 64); }
     }
@@ -297,8 +287,6 @@ int add_plan(b200pose_net* net, const TcLayer& L, int n, int H, int W, const __n
     a.store_ch[0] = store0; a.store_ch[1] = store1;
     a.out_f32[0] = f32_0; a.out_f32[1] = f32_1;
     a.f32_ch[0] = f32c0; a.f32_ch[1] = f32c1;
-    a.use_base_offset = 0;
-    a.pair = (net->conv_pair && a.n_tile % 32 == 0) ? 1 : 0;    // heads (N = 48) stay single-CTA
     // small batches (the 46 x 46 layers fill less than half of the SMs with 16 x 16 tiles): chain the layers with programmatic
     // dependent launches; the first tensor-core layer follows conv1_1, which does not signal
     a.pdl = (net->conv_pdl && !net->plan.empty() && small_plan(net, n, H, W)) ? 1 : 0;
@@ -570,7 +558,8 @@ int b200pose_net_create(b200pose_net** out, int cuda_device) {
     CU(cudaSetDevice(cuda_device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, cuda_device));
-    if (prop.major != 10) return fail("b200pose: built for sm_100a (B200); device is sm_%d%d", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail("b200pose: built for sm_90a (H100); device is sm_%d%d", prop.major, prop.minor);
     b200pose_net* net = new b200pose_net();
     net->device = cuda_device;
     net->num_sms = prop.multiProcessorCount;
@@ -579,10 +568,6 @@ int b200pose_net_create(b200pose_net** out, int cuda_device) {
     net->have.assign(B200POSE_NUM_TENSORS, false);
     const char* pc = getenv("B200POSE_PLAN_CACHE");
     net->plan_cache_on = !(pc && pc[0] == '0');
-    const char* cp = getenv("B200POSE_CONV_PAIR");
-    net->conv_pair = !(cp && cp[0] == '0');
-    const char* nw = getenv("B200POSE_CONV_NARROW");
-    net->conv_narrow = !(nw && nw[0] == '0');
     const char* pd = getenv("B200POSE_CONV_PDL");
     net->conv_pdl = !(pd && pd[0] == '0');
     const char* gr = getenv("B200POSE_GRAPH");

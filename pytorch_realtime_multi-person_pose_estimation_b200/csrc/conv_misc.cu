@@ -1,6 +1,6 @@
-// CUDA-core kernels around the tcgen05 conv:
+// CUDA-core kernels around the wgmma conv:
 //   conv_first_kernel : conv1_1 (3 -> 64, 3x3, pad 1) + bias + ReLU, fp32 NCHW in -> bf16 NHWC out
-//                       (/root/reference/lib/network/rtpose_vgg.py:69).  K = 27 is too thin for UMMA tiles and the
+//                       (the reference's rtpose_vgg.py:69).  K = 27 is too thin for wgmma tiles and the
 //                       layer is HBM/LSU bound (AI ~ 26 FLOP/B), so it runs on the FP32 pipes.
 //   conv_f32_kernel   : generic stride-1 "same" conv, NHWC fp32 in/out, fp32 FMA accumulate - the fp32-parity mode
 //                       of every layer (heat/PAF within 1e-3 of the fp32 reference) and the GPU-side cross-check of
@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_kernel(const void* __re
 
 
 // ------------------------------------------------------------------ conv1_1 on the tensor cores (bf16 mode)
-// conv1_1 is a GEMM with K = 27: far too thin for a tcgen05 tile pipeline (one 128 x 64 x 32 MMA per 128 pixels), and its
+// conv1_1 is a GEMM with K = 27: far too thin for a wgmma tile pipeline (one 64 x 64 x 32 MMA per 64 pixels), and its
 // roofline is HBM (0.4 MB in, 17.7 MB out per frame: 0.09 ms per batch of 32 at the measured copy bandwidth) - the fp32
 // CUDA-core kernel above needs 0.50 ms for its 7.5 G fused multiply-adds.  Here every warp runs warp-level
 // mma.sync.m16n8k16 (bf16 x bf16 -> fp32) on im2col fragments gathered straight from the staged input tile: K is padded
@@ -400,7 +400,7 @@ __global__ void u8hwc_to_f32nchw_kernel(const unsigned char* __restrict__ in, fl
 cudaError_t u8hwc_to_f32nchw_launch(const unsigned char* in, float* out, int N, int H, int W, int mode, cudaStream_t s) {
     if (mode < kPreRtpose || mode > kPreSsd) return cudaErrorInvalidValue;
     const size_t total = (size_t)N * 3 * H * W;
-    const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     u8hwc_to_f32nchw_kernel<<<blocks, 256, 0, s>>>(in, out, N, H, W, mode);
     return cudaGetLastError();
 }
@@ -414,7 +414,7 @@ cudaError_t conv_f32_launch(const ConvF32Args& a, cudaStream_t s) {
 
 cudaError_t maxpool_f32_launch(const float* in, float* out, int N, int H, int W, int C, cudaStream_t s) {
     const size_t total = (size_t)N * (H / 2) * (W / 2) * C;
-    const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     maxpool_f32_kernel<<<blocks, 256, 0, s>>>(in, out, N, H, W, C);
     return cudaGetLastError();
 }
@@ -422,7 +422,7 @@ cudaError_t maxpool_f32_launch(const float* in, float* out, int N, int H, int W,
 cudaError_t nchw_to_nhwc_f32_launch(const float* in, float* out, int N, int C, int H, int W, int out_cstride,
                                     int out_ch_off, cudaStream_t s) {
     const size_t total = (size_t)N * C * H * W;
-    const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     nchw_to_nhwc_f32_kernel<<<blocks, 256, 0, s>>>(in, out, N, C, H, W, out_cstride, out_ch_off);
     return cudaGetLastError();
 }

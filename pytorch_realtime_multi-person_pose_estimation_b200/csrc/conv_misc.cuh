@@ -1,4 +1,4 @@
-// CUDA-core kernels around the tcgen05 conv (see conv_misc.cu).
+// CUDA-core kernels around the wgmma conv (see conv_misc.cu).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

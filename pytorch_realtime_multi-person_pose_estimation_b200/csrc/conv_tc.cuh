@@ -1,6 +1,6 @@
-// Host-side interface of the tcgen05 "halo-patch" implicit-GEMM convolution (conv_tc.cu).
-// Replaces the nn.Conv2d(+ReLU)(+MaxPool2d)(+torch.cat) sequences of
-// /root/reference/lib/network/rtpose_vgg.py:23-29,165 for every conv with Cin >= 64.
+// Host-side interface of the wgmma "halo-patch" implicit-GEMM convolution (conv_tc.cu).
+// Replaces the nn.Conv2d(+ReLU)(+MaxPool2d)(+torch.cat) sequences of the reference's
+// lib/network/rtpose_vgg.py for every conv with Cin >= 64.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -9,17 +9,15 @@
 
 namespace b2p {
 
-constexpr int kTileW = 16;        // CTA tile: 16 x 16 output pixels = two 8-wide x 16-high UMMA M=128 sub-tiles
+constexpr int kTileW = 8;         // CTA tile: 8 (w) x 16 (h) output pixels = two wgmma M=64 halves of 8 x 8 (one per consumer warpgroup)
 constexpr int kTileH = 16;
-constexpr int kPatchPitch = 24;   // patch row pitch in pixels (16 + 6 halo, rounded up to a multiple of 8)
+constexpr int kPatchPitch = 16;   // patch row pitch in pixels (8 + 6 halo, rounded up so that a patch is a multiple of 1024 B)
 constexpr int kMaxKs = 7;
-constexpr int kPatchBytes = kPatchPitch * (kTileH + kMaxKs - 1) * 128;  // 67,584 B per 64-channel block
+constexpr int kPatchBytes = kPatchPitch * (kTileH + kMaxKs - 1) * 128;  // 45,056 B per 64-channel block
 constexpr int kBStageBytes = 128 * 128;                                 // up to N=128 rows of 64 bf16
 #ifndef B2P_CONV_B_STAGES
-#define B2P_CONV_B_STAGES 3      // weight (B operand) ring: 48 KB, cut into stages of `tps` taps (conv_tc.cu): three stages of two 8 KB
-                                 // half-slices for a CTA pair with N = 128.  The shared memory a conv CTA leaves free decides which
-                                 // post-processing kernels of the previous batch can run NEXT to it: at 185 KB the small ones still
-                                 // fit; taking everything (four patch stages, 230 KB) cost 9 % of the step; see DESIGN.md 2.4
+#define B2P_CONV_B_STAGES 6      // weight (B operand) ring: 96 KB, cut into stages of `tps` taps (conv_tc.cu); with the two patch
+                                 // stages a CTA holds 185 KB of the 227 KB an H100 block may use
 #endif
 constexpr int kNumBStages = B2P_CONV_B_STAGES;
 #ifndef B2P_CONV_MIN_B_STAGES
@@ -28,7 +26,7 @@ constexpr int kNumBStages = B2P_CONV_B_STAGES;
 constexpr int kMinBStages = B2P_CONV_MIN_B_STAGES;     // a stage holds as many taps as still leave this many stages in the ring
 constexpr int kMaxBStages = 16;       // the ring is cut into stages of the size the layer's n-tile needs (conv_tc.cu)
 constexpr int kNumPatchStages = 2;
-constexpr int kConvTcThreads = 352;   // warps: 0 patch TMA, 1 MMA, 2-5 and 7-10 epilogue (two per TMEM lane quarter), 6 weight TMA
+constexpr int kConvTcThreads = 384;   // warpgroup 0: producers (warp 0 patch TMA, warp 1 weight TMA); warpgroups 1, 2: MMA + epilogue
 constexpr int kConvTcSmemBytes = kNumPatchStages * kPatchBytes + kNumBStages * kBStageBytes + 1024 /*align*/ + 512;
 
 struct ConvTcArgs {
@@ -39,7 +37,7 @@ struct ConvTcArgs {
     int in_ch_base;           // first input channel (in the NHWC buffer) of group 0
     int in_ch_group_stride;   // channel offset between groups in the input buffer (0 = groups share input)
     int groups;               // 1 or 2
-    int n_tile;               // UMMA N: multiple of 16, <= 128
+    int n_tile;               // wgmma N: 32, 48, 64 or 128
     int n_tiles;              // N tiles per group
     // ---- epilogue
     const float* bias;        // [groups * n_tiles * n_tile]
@@ -51,24 +49,18 @@ struct ConvTcArgs {
     int store_ch[2];          // channels (multiple of 8) stored per group *per n-tile*
     float* out_f32[2];        // optional NCHW fp32 copy per group (heads), may be null
     int f32_ch[2];            // valid channels of the fp32 copy
-    int use_base_offset;      // descriptor swizzle-phase field (see DESIGN.md)
     // ---- split-precision ("bf16x3") mode: operands are hi + lo bf16 planes, three MMA terms per K block
     int split;                // 0: plain bf16; 1: A_hi*W_hi + A_hi*W_lo + A_lo*W_hi
     __nv_bfloat16* out_lo;    // residual plane of the output (same geometry as `out`), split mode only
-    // ---- CTA-pair mode (tcgen05 cta_group::2): clusters of two CTAs share each weight slice; needs n_tile % 32 == 0
-    int pair;
     // ---- K-chunked accumulation (n_tile <= 64): see conv_tc_chunk_kernel
     int chunk;
-    // ---- narrow tiles (small batches): the CTA tile is 8 x 16 pixels (one UMMA M=128 sub-tile) instead of 16 x 16
-    int narrow;
     // ---- taps per weight stage (set by conv_tc_make_maps together with the weight map's box)
     int tps;
     // ---- programmatic dependent launch of this layer behind the previous one (small-batch plans)
     int pdl;
     // ---- tensor maps
-    CUtensorMap tm_in;        // 4D (C, W, H, N) bf16, box (64, 24, 16+ks-1, 1), SWIZZLE_128B
+    CUtensorMap tm_in;        // 4D (C, W, H, N) bf16, box (64, 16, 16+ks-1, 1), SWIZZLE_128B
     CUtensorMap tm_w;         // 3D (cin_pad, groups*n_tiles*n_tile, 2*taps) bf16 [hi taps | lo taps], box (64, n_tile, tps)
-                              // (pair mode: box (64, n_tile / 2, 1) - each CTA of a pair loads its half of the N rows)
     CUtensorMap tm_in_lo;     // residual plane of the input (split mode)
 };
 

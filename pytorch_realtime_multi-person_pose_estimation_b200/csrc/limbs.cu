@@ -822,7 +822,7 @@ cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long 
     }
     static DynSmemOptIn optin_score, optin_sort;
     B2P_TRY(optin_score.ensure(limb_score_kernel, smem));
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     B2P_TRY(cudaGetDevice(&dev));
     B2P_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb);
@@ -861,7 +861,7 @@ cudaError_t post_debug_sort(const PostBuffers& pb, const unsigned long long* key
     B2P_TRY(cudaGetLastError());
     static DynSmemOptIn optin_sort;
     B2P_TRY(optin_sort.ensure(range_sort_kernel, sizeof(SortSmem)));
-    range_sort_kernel<<<148 * 3, kSortThreads, sizeof(SortSmem), s>>>(pb);
+    range_sort_kernel<<<132 * 3, kSortThreads, sizeof(SortSmem), s>>>(pb);
     B2P_TRY(cudaGetLastError());
     B2P_TRY(cudaMemcpyAsync(out, pb.pool + pb.pool_cap / 2, (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);

@@ -1,4 +1,4 @@
-// Fused post-processing kernel family for sm_100a: heat-map NMS + bicubic refinement, PAF line-integral scoring
+// Fused post-processing kernel family for sm_90a: heat-map NMS + bicubic refinement, PAF line-integral scoring
 // + greedy bipartite matching, person assembly.  See postprocess.cuh for the reference lines each kernel replaces.
 // HBM-side this path touches 56 x h x w x 4 B per image once (18 heat + 38 PAF planes); it is latency bound, so
 // the design goal is: everything stays on the device, one block per (image, part) / (image, limb) / image, warp

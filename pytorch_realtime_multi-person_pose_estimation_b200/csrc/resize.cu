@@ -62,7 +62,7 @@ cudaError_t resize_cubic_accum_launch(const float* src, float* dst, long planes,
     if (planes < 1 || src_h < 1 || src_w < 1 || dst_h < 1 || dst_w < 1) return cudaErrorInvalidValue;
     const long total = planes * dst_h * dst_w;
     long b = (total + kThreads - 1) / kThreads;
-    if (b > 148L * 8) b = 148L * 8;
+    if (b > 132L * 8) b = 132L * 8;
     resize_cubic_accum_kernel<<<(unsigned)b, kThreads, 0, s>>>(src, dst, planes, src_h, src_w, dst_h, dst_w,
                                                              rs_step(dst_h, src_h), rs_step(dst_w, src_w), first, divide_by);
     return cudaGetLastError();
@@ -73,7 +73,7 @@ cudaError_t crop_with_factor_launch(const unsigned char* in, unsigned char* out,
     if (n < 1 || n > 65535) return cudaErrorInvalidValue;
     const long px = (long)g.pad_h * g.pad_w;
     long bx = (px + kThreads - 1) / kThreads;
-    const long cap = (148L * 8 + n - 1) / n;      // about one wave of 8 blocks per SM over the whole batch
+    const long cap = (132L * 8 + n - 1) / n;      // about one wave of 8 blocks per SM over the whole batch
     if (bx > cap) bx = cap;
     if (bx < 1) bx = 1;
     crop_with_factor_kernel<<<dim3((unsigned)bx, (unsigned)n), kThreads, 0, s>>>(in, out, src_h, src_w, g);

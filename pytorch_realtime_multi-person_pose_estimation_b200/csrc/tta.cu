@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(kThreads) flip_merge_kernel(const float* __res
 
 int grid_for(long total) {
     long b = (total + kThreads - 1) / kThreads;
-    const long cap = 148L * 8;          // 8 resident blocks of 256 threads per SM
+    const long cap = 132L * 8;          // 8 resident blocks of 256 threads per SM
     return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

@@ -1,5 +1,5 @@
 """Counterpart of /root/reference/evaluate/evaluation.py: load a checkpoint into the rtpose VGG19 model and run the
-COCO keypoint evaluation on the B200 path.  The reference hard-codes its paths (evaluation.py:12,31); here they are
+COCO keypoint evaluation on the H100 path.  The reference hard-codes its paths (evaluation.py:12,31); here they are
 arguments with the same defaults.  Run from the repository root:  python -m evaluate.evaluation --weight ... """
 import argparse
 from collections import OrderedDict

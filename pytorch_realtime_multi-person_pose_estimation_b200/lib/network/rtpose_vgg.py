@@ -4,10 +4,10 @@
 (model0.{0,2,5,...}, model{1..6}_{1,2}.{0,2,...}; rtpose_vgg.py:69-127, 140-156), so
 `model.load_state_dict(torch.load(w))`, `.cuda()`, `.float()`, `.eval()` and `torch.nn.DataParallel(model)`
 (demo/picture_demo.py:45-49) work unchanged.  `forward` (rtpose_vgg.py:158-198) does NOT run nn.Conv2d: it hands
-the input's device pointer to libb200pose.so, which runs the hand-written sm_100a kernels, and returns
+the input's device pointer to libb200pose.so, which runs the hand-written sm_90a kernels, and returns
 `((paf, heat), saved_for_loss[12])` as CUDA fp32 NCHW tensors.
 
-Precision: `model.precision = 'bf16x3'` (default: split-precision operands on the tcgen05 tensor cores with K-chunked
+Precision: `model.precision = 'bf16x3'` (default: split-precision operands on the wgmma tensor cores with K-chunked
 fp32 accumulation - maps within 1.4e-4 of the reference's fp32 network at 368x368, inside its 1e-3 tolerance), `'bf16'`
 (the fast mode of the batched engine and the benchmark: ~4.5x faster, maps within ~8e-2) or `'fp32'` (CUDA cores,
 bit-identical to the oracle's fp32 network); the environment variable B200POSE_MODE sets the default.
@@ -191,7 +191,7 @@ class rtpose_model(nn.Module):
 def get_model(trunk='vgg19'):
     """rtpose_vgg.py:60.  Only the VGG19 trunk exists on this path (BASELINE.json north_star)."""
     if trunk != 'vgg19':
-        raise NotImplementedError("only trunk='vgg19' is built for the B200 path")
+        raise NotImplementedError("only trunk='vgg19' is built for the H100 path")
     return rtpose_model()
 
 

@@ -23,7 +23,7 @@ def _post(device_index=None, peak_cap=2048, human_cap=2048):
 
 def _run(heatmaps, pafs, config):
     if config.MODEL.DOWNSAMPLE != 8:
-        raise ValueError("the B200 path supports MODEL.DOWNSAMPLE == 8 only")
+        raise ValueError("the H100 path supports MODEL.DOWNSAMPLE == 8 only")
     heat = np.ascontiguousarray(heatmaps, dtype=np.float32)
     paf = np.ascontiguousarray(pafs, dtype=np.float32)
     if heat.ndim != 3 or heat.shape[2] != 19 or paf.shape[:2] != heat.shape[:2] or paf.shape[2] != 38:

@@ -1,5 +1,5 @@
-// Standalone GPU check of the tcgen05 conv kernel against a plain CPU loop (bf16-rounded operands, double
-// accumulation).  Build: see __graft_entry__.build().  Run on the GPU box: build/test_conv_tc [quick|perf]
+// Standalone GPU check of the wgmma conv kernel against a plain CPU loop (bf16-rounded operands, double
+// accumulation).  Build: see __graft_entry__.build().  Run on an H100: build/test_conv_tc [perf]
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -32,7 +32,7 @@ struct Case {
 };
 
 // head: out_ch_off {0,40}, store {40,24}, f32 {38,19}; cout_g is the padded per-group Cout (n_tile).
-static int run_case(const Case& c, int use_bo, int num_sms, int pair, int chunk = 0, int narrow = 0) {
+static int run_case(const Case& c, int num_sms, int chunk = 0) {
     const int taps = c.ks * c.ks, pad = c.ks / 2;
     const int cin_blocks = c.cin_g / 64;
     const int in_c = (c.in_stride_g == 0) ? c.cin_g : c.cin_g * c.groups;
@@ -86,15 +86,12 @@ static int run_case(const Case& c, int use_bo, int num_sms, int pair, int chunk 
         a.out_f32[g] = d_f32[g];
         a.f32_ch[g] = c.head ? valid[g] : 0;
     }
-    a.use_base_offset = use_bo;
-    a.pair = pair;
     a.chunk = chunk;
-    a.narrow = narrow;
     CK(conv_tc_make_maps(a, d_in, in_c, d_w));
     CK(conv_tc_launch(a, num_sms, 0));
     cudaError_t e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
-        printf("case %-28s bo=%d pair=%d : KERNEL FAILED: %s\n", c.name, use_bo, pair, cudaGetErrorString(e));
+        printf("case %-28s chunk=%d : KERNEL FAILED: %s\n", c.name, chunk, cudaGetErrorString(e));
         return 100;
     }
 #ifdef B2P_CONV_TIMELINE
@@ -104,7 +101,7 @@ static int run_case(const Case& c, int use_bo, int num_sms, int pair, int chunk 
         const char* names[10] = {"entry", "prologue done", "patch cb0", "patch cb1", "first weights", "MMAs issued", "acc complete",
                                  "tile stored", "before final sync", "exit"};
         for (int cta = 0; cta < 4; ++cta) {
-            printf("  timeline %s pair=%d chunk=%d narrow=%d CTA %d (clk since entry):", c.name, pair, chunk, narrow, cta);
+            printf("  timeline %s chunk=%d CTA %d (clk since entry):", c.name, chunk, cta);
             for (int sl = 1; sl < 10; ++sl) {
                 const unsigned long long v = tl[cta * kTlSlots + sl], v0 = tl[cta * kTlSlots];
                 printf(" %s=%lld", names[sl], v ? (long long)(v - v0) : -1LL);
@@ -179,14 +176,14 @@ static int run_case(const Case& c, int use_bo, int num_sms, int pair, int chunk 
                         }
                     }
                 }
-    printf("case %-28s bo=%d pair=%d chunk=%d narrow=%d : max|err| bf16 %.5f  f32 %.3e  (max|ref| %.3f)  bad=%ld  %s\n", c.name, use_bo,
-           pair, chunk, narrow, max_err, max_err32, max_ref, bad, bad == 0 ? "OK" : "MISMATCH");
+    printf("case %-28s chunk=%d : max|err| bf16 %.5f  f32 %.3e  (max|ref| %.3f)  bad=%ld  %s\n", c.name, chunk, max_err,
+           max_err32, max_ref, bad, bad == 0 ? "OK" : "MISMATCH");
     cudaFree(d_in); cudaFree(d_w); cudaFree(d_bias); cudaFree(d_out);
     for (int g = 0; g < 2; ++g) if (d_f32[g]) cudaFree(d_f32[g]);
     return bad == 0 ? 0 : 1;
 }
 
-static void perf(int num_sms, int use_bo, int pair) {
+static void perf(int num_sms) {
     // Mconv{2..5}_stageX_L{1,2}: 7x7 128->128, both branches grouped, batch 32 @46x46.
     struct P { const char* name; int n, H, W, ks, groups, cin_g, stride_g, cout_g, n_tile, pool; };
     const P ps[] = {
@@ -216,8 +213,6 @@ static void perf(int num_sms, int use_bo, int pair) {
         a.in_ch_group_stride = p.stride_g; a.groups = p.groups; a.n_tile = p.n_tile; a.n_tiles = p.cout_g / p.n_tile;
         a.bias = d_bias; a.relu = 1; a.pool = p.pool; a.out = d_out; a.out_cstride = rows;
         for (int g = 0; g < 2; ++g) { a.out_ch_off[g] = g * p.cout_g; a.store_ch[g] = p.n_tile; }
-        a.use_base_offset = use_bo;
-        a.pair = (pair && p.n_tile % 32 == 0) ? 1 : 0;
         CK(conv_tc_make_maps(a, d_in, in_c, d_w));
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -232,7 +227,7 @@ static void perf(int num_sms, int use_bo, int pair) {
         cudaEventElapsedTime(&ms, e0, e1);
         ms /= iters;
         double flops = 2.0 * p.n * p.H * p.W * (double)rows * taps * p.cin_g;
-        printf("perf %-30s pair=%d : %8.3f ms  %8.1f TFLOP/s\n", p.name, a.pair, ms, flops / ms * 1e-9);
+        printf("perf %-30s : %8.3f ms  %8.1f TFLOP/s\n", p.name, ms, flops / ms * 1e-9);
         cudaFree(d_in); cudaFree(d_w); cudaFree(d_out); cudaFree(d_bias);
     }
 }
@@ -254,35 +249,25 @@ int main(int argc, char** argv) {
         {"7x7 2grp shared192->128 22x26", 1, 22, 26, 7, 2, 192, 0, 128, 128, 1, 0, 0},
         {"1x1 head 128->38|19 46x46", 2, 46, 46, 1, 2, 128, 128, 48, 48, 0, 0, 1},
         {"1x1 512->512 46x46 4 ntiles", 1, 46, 46, 1, 1, 512, 512, 512, 128, 1, 0, 0},
-        {"3x3 64->128 odd tiles 3x40x16", 3, 40, 16, 3, 1, 64, 64, 128, 128, 1, 0, 0},     // 3 images x 3 x 1 = 9 pixel tiles (odd)
-        {"7x7 2grp 128->128 1x16x16", 1, 16, 16, 7, 2, 128, 128, 128, 128, 1, 0, 0},        // ONE pixel tile: the odd CTA idles
+        {"3x3 64->128 odd tiles 3x40x16", 3, 40, 16, 3, 1, 64, 64, 128, 128, 1, 0, 0},     // 3 images x 3 x 2 = 18 pixel tiles
+        {"7x7 2grp 128->128 1x16x16", 1, 16, 16, 7, 2, 128, 128, 128, 128, 1, 0, 0},        // two pixel tiles
         {"7x7 2grp 128->128 nt64 30x30", 1, 30, 30, 7, 2, 128, 128, 128, 64, 1, 0, 0},      // two 64-wide n-tiles per group
         {"7x7 2grp 128->128 nt32 46x46", 1, 46, 46, 7, 2, 128, 128, 128, 32, 1, 0, 0},      // batch-1 plan: four 32-wide n-tiles
         {"3x3 128->128 pool nt32 24x40", 1, 24, 40, 3, 1, 128, 128, 128, 32, 1, 1, 0},
         {"7x7 head 128->38|19 K=6272", 2, 46, 46, 7, 2, 128, 128, 48, 48, 0, 0, 1},          // fp32 outputs after a long K loop
     };
-    // use_base_offset=0 is the product setting: the UMMA shared-memory descriptor swizzles on absolute smem address
-    // bits, so shifted (non-1024B-aligned) window starts need no phase field.  `probe` also runs the =1 variant
-    // (expected to MISMATCH; kept as the record of how that was established, profiles/r01_conv_tc_first_light.log).
-    const bool probe = argc > 1 && !strcmp(argv[1], "probe");
     int fails = 0;
-    for (int bo = probe ? 1 : 0; bo >= 0; --bo) {
-        for (const Case& c : cases) {
-            for (int pair = 0; pair <= ((c.n_tile % 32 == 0) ? 1 : 0); ++pair) {     // CTA-pair mode where it is eligible
-                for (int chunk = 0; chunk <= (c.n_tile <= 64 ? 1 : 0); ++chunk) {    // K-chunked accumulation (N <= 64)
-                    for (int narrow = 0; narrow <= 1; ++narrow) {                     // 8 x 16 pixel tiles (small batches)
-                        int r = run_case(c, bo, sms, pair, chunk, narrow);
-                        if (r >= 100) {   // sticky CUDA error: the context is gone
-                            printf("aborting after kernel failure\n");
-                            return 3;
-                        }
-                        if (bo == 0) fails += r;
-                    }
-                }
+    for (const Case& c : cases) {
+        for (int chunk = 0; chunk <= (c.n_tile <= 64 ? 1 : 0); ++chunk) {    // K-chunked accumulation (N <= 64)
+            int r = run_case(c, sms, chunk);
+            if (r >= 100) {   // sticky CUDA error: the context is gone
+                printf("aborting after kernel failure\n");
+                return 3;
             }
+            fails += r;
         }
     }
     printf("conv_tc: %s\n", fails == 0 ? "ALL OK" : "FAILURES");
-    if (do_perf) { perf(sms, 0, 0); perf(sms, 0, 1); }
+    if (do_perf) perf(sms);
     return fails == 0 ? 0 : 1;
 }

@@ -14,7 +14,7 @@ import os
 import sys
 import types
 
-ARGS = sys.argv[1:]     # optional: "crop" / "eval" / "pre" regenerate only those small fixtures
+ARGS = sys.argv[1:]     # optional: "crop" / "eval" / "pre" / "fuzz" regenerate only those small fixtures
 
 import numpy as np
 
@@ -146,16 +146,76 @@ def make_preprocess():
     print("preprocess fixture written")
 
 
+def fuzz_scenario(t):
+    """Scenario t of the pafprocess fuzz (tests/test_host.py, tests/test_gpu_tta.py): joint list [P, 5] and PAF [h, w, 38]."""
+    rs = np.random.RandomState(1000 + t)
+    h, w = int(rs.choice([12, 23, 46])), int(rs.choice([23, 46, 53]))
+    if t % 2:
+        h = max(h, 23)
+        jl, paf = synth.fuzz_persons(rs, h, w)
+    else:
+        jl, paf = synth.fuzz_field(rs, h, w, ("uniform", "cluster", "ties")[(t // 2) % 3])
+    return jl, paf, h, w
+
+
+FUZZ_SCENARIOS = 300
+CROWDS = ((30, 31), (50, 5), (80, 7))
+
+
+def make_pafprocess_fuzz():
+    """The reference's own pafprocess.cpp (oracle/_ref) on the fuzz scenarios and on three crowded stick-figure scenes.
+    Fuzz: per scenario the human count, per human a row [score, 18 x (cid | -1, x, y, part score)] (float32, exact);
+    crowds: paf_to_pose rows [score, 18 x (x / W, y / H, part score) | -1] (float64, exact)."""
+    from oracle import glue_port
+    ref = pafprocess_oracle.load_ref()
+    nh, rows, ins = [], [], []
+    for t in range(FUZZ_SCENARIOS):
+        jl, paf, h, w = fuzz_scenario(t)
+        ins += [jl, paf]
+        if len(jl) == 0:
+            nh.append(0)
+            continue
+        paf_up = np.ascontiguousarray(np.repeat(np.repeat(paf, 8, axis=0), 8, axis=1))
+        ref.process_paf(jl[None], np.zeros((h * 8, w * 8, 19), np.float32), paf_up)
+        nh.append(ref.get_num_humans())
+        for hid in range(ref.get_num_humans()):
+            r = np.full(1 + 18 * 4, -1.0, np.float32)
+            r[0] = ref.get_score(hid)
+            for p in range(18):
+                c = int(ref.get_part_cid(hid, p))
+                if c >= 0:
+                    r[1 + 4 * p: 5 + 4 * p] = (c, ref.get_part_x(c), ref.get_part_y(c), ref.get_part_score(c))
+            rows.append(r)
+    crowd = {}
+    for persons, seed in CROWDS:
+        heat, paf, _ = synth.stick_figures(persons, seed)
+        humans = glue_port.paf_to_pose(heat, paf, ref)[1]
+        c = np.full((len(humans), 1 + 18 * 3), -1.0, np.float64)
+        for i, (score, parts) in enumerate(humans):
+            c[i, 0] = score
+            for p, v in parts.items():
+                c[i, 1 + 3 * p: 4 + 3 * p] = v
+        crowd["crowd_%d_%d" % (persons, seed)] = c
+    np.savez_compressed(os.path.join(OUT, "pafprocess_fuzz.npz"), fuzz_digest=digest(*ins), humans_per_scenario=np.array(nh),
+                        humans=np.array(rows, np.float32).reshape(-1, 1 + 18 * 4), **crowd)
+    print("pafprocess fuzz fixture written: %d humans" % len(rows))
+
+
 def main():
+    if ARGS and set(ARGS) <= {"fuzz"}:
+        make_pafprocess_fuzz()
+        return
     import torch
     get_model, ref_p2p, ref_eval, cfg = import_reference()
+    if not ARGS or "fuzz" in ARGS:
+        make_pafprocess_fuzz()
     if not ARGS or "pre" in ARGS:
         make_preprocess()
     if not ARGS or "crop" in ARGS:
         make_crop()
     if not ARGS or "eval" in ARGS:
         make_eval(ref_eval)
-    if ARGS and set(ARGS) <= {"crop", "eval", "pre"}:
+    if ARGS and set(ARGS) <= {"crop", "eval", "pre", "fuzz"}:
         return
     torch.manual_seed(0)
 

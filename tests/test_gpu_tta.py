@@ -90,10 +90,11 @@ def test_fused_flip_inference_matches_reference_shaped_composition(built, he_sd)
 def test_pafprocess_kernels_fuzz_against_the_compiled_reference(built):
     """The limbs / assembly kernels (through the legacy lib.pafprocess surface: joint list + x8 maps, exactly what the
     SWIG module gets) on 80 random inputs the fixtures do not reach - duplicated peaks on one pixel, exact score ties,
-    cross links between persons, masked fields - against the reference's own pafprocess.cpp (oracle/_ref; the C port
-    when it is absent).  Same scenario generator as the host-side fuzz in tests/test_host.py."""
+    cross links between persons, masked fields - against what the reference's own pafprocess.cpp made of them (golden,
+    tests/golden/make_golden.py).  Same scenarios as the host-side fuzz in tests/test_host.py."""
     from lib.pafprocess import pafprocess
-    ref = pafprocess_oracle.load_ref() if pafprocess_oracle.have_ref() else pafprocess_oracle.load_port()
+    g = golden("pafprocess_fuzz")
+    start = np.concatenate([[0], np.cumsum(g["humans_per_scenario"])])
     humans = 0
     for t in range(80):
         rs = np.random.RandomState(1000 + t)
@@ -108,13 +109,13 @@ def test_pafprocess_kernels_fuzz_against_the_compiled_reference(built):
         paf_up = np.ascontiguousarray(np.repeat(np.repeat(paf, 8, 0), 8, 1))
         heat_up = np.zeros((h * 8, w * 8, 19), np.float32)
         assert pafprocess.process_paf(jl[None], heat_up, paf_up) == 0
-        ref.process_paf(jl[None], heat_up, paf_up)
-        assert pafprocess.get_num_humans() == ref.get_num_humans(), "scenario seed %d" % (1000 + t)
-        for hid in range(ref.get_num_humans()):
-            assert pafprocess.get_score(hid) == ref.get_score(hid), "scenario seed %d" % (1000 + t)
+        want = g["humans"][start[t]:start[t + 1]]
+        assert pafprocess.get_num_humans() == len(want), "scenario seed %d" % (1000 + t)
+        for hid, r in enumerate(want):
+            assert pafprocess.get_score(hid) == float(r[0]), "scenario seed %d" % (1000 + t)
             for p in range(18):
-                assert pafprocess.get_part_cid(hid, p) == ref.get_part_cid(hid, p), "scenario seed %d" % (1000 + t)
-        humans += ref.get_num_humans()
+                assert pafprocess.get_part_cid(hid, p) == int(r[1 + 4 * p]), "scenario seed %d" % (1000 + t)
+        humans += len(want)
     assert humans > 80
 
 

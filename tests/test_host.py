@@ -386,31 +386,28 @@ def test_device_cores_on_host_match_oracle(name, built):
 
 def test_device_cores_on_host_fuzz_against_the_compiled_reference(built):
     """300 random pafprocess inputs (peak sets with clusters / duplicated pixels, direction fields with exact ties, person
-    shapes with cross links) through csrc/post_core.h on the host and through the reference's own pafprocess.cpp
-    (oracle/_ref; the C port when the reference sources are absent): identical persons, scores and part assignments."""
+    shapes with cross links) through csrc/post_core.h on the host against what the reference's own pafprocess.cpp made of
+    them (golden, tests/golden/make_golden.py): identical persons, scores and part assignments."""
+    import hashlib
     lib = ctypes.CDLL(os.path.join(ROOT, "build", "libpostcore_host.so"))
     FP = ctypes.POINTER(ctypes.c_float)
     lib.core_process.argtypes = [ctypes.c_int, FP, ctypes.c_int, FP, ctypes.c_long, ctypes.c_long, ctypes.c_long,
                                  ctypes.c_int, ctypes.c_int]
     lib.core_result.restype = FP
-    ref = pafprocess_oracle.load_ref() if pafprocess_oracle.have_ref() else pafprocess_oracle.load_port()
+    g = golden("pafprocess_fuzz")
+    start = np.concatenate([[0], np.cumsum(g["humans_per_scenario"])])
     to_dicts = pkg_module("engine").humans_to_dicts
 
-    def ref_humans(jl, paf, h, w):
-        paf_up = np.ascontiguousarray(np.repeat(np.repeat(paf, 8, axis=0), 8, axis=1))
-        ref.process_paf(jl[None], np.zeros((h * 8, w * 8, 19), np.float32), paf_up)
+    def ref_humans(t, h, w):
         out = []
-        for hid in range(ref.get_num_humans()):
-            parts = {}
-            for p in range(18):
-                c = int(ref.get_part_cid(hid, p))
-                if c >= 0:
-                    parts[p] = (float(ref.get_part_x(c)) / (w * 8), float(ref.get_part_y(c)) / (h * 8),
-                                float(ref.get_part_score(c)))
+        for r in g["humans"][start[t]:start[t + 1]]:
+            parts = {p: (float(r[2 + 4 * p]) / (w * 8), float(r[3 + 4 * p]) / (h * 8), float(r[4 + 4 * p]))
+                     for p in range(18) if r[1 + 4 * p] >= 0}
             if parts:
-                out.append((float(ref.get_score(hid)), parts))
+                out.append((float(r[0]), parts))
         return out
     humans = 0
+    digest = hashlib.sha256()
     for t in range(300):
         rs = np.random.RandomState(1000 + t)
         h, w = int(rs.choice([12, 23, 46])), int(rs.choice([23, 46, 53]))
@@ -419,15 +416,18 @@ def test_device_cores_on_host_fuzz_against_the_compiled_reference(built):
             jl, paf = synth.fuzz_persons(rs, h, w)
         else:
             jl, paf = synth.fuzz_field(rs, h, w, ("uniform", "cluster", "ties")[(t // 2) % 3])
+        for a in (jl, paf):
+            digest.update(np.ascontiguousarray(a).tobytes())
         if len(jl) == 0:
             continue
-        want = ref_humans(jl, paf, h, w)
+        want = ref_humans(t, h, w)
         nh = lib.core_process(len(jl), jl.ctypes.data_as(FP), h * 8, paf.ctypes.data_as(FP), 1, w * 38, 38, 3, 0)
         rows = (np.ctypeslib.as_array(lib.core_result(), shape=(nh * 73,)).reshape(nh, 73).copy() if nh else
                 np.zeros((0, 73), np.float32))
         assert to_dicts(rows, w * 8, h * 8) == want, "scenario seed %d" % (1000 + t)
         assert lib.core_sort_mismatch() == 0
         humans += len(want)
+    assert digest.hexdigest()[:16] == str(g["fuzz_digest"]), "fuzz scenarios drifted from the golden ones"
     assert humans > 300
 
 

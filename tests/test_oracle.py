@@ -129,14 +129,13 @@ def test_pafprocess_port_matches_reference(name, built):
 
 
 def test_pafprocess_port_ties_and_scale(built):
-    """Large crowded scenes produce exactly-equal candidate scores; std::sort's order is reproduced."""
-    if not pafprocess_oracle.have_ref():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
-    port, ref = pafprocess_oracle.load_port(), pafprocess_oracle.load_ref()
+    """Large crowded scenes produce exactly-equal candidate scores; std::sort's order is reproduced (against what the
+    reference's own pafprocess.cpp made of the same scenes, tests/golden/make_golden.py)."""
+    port, g = pafprocess_oracle.load_port(), golden("pafprocess_fuzz")
     for persons, seed in [(30, 31), (50, 5), (80, 7)]:
         heat, paf, _ = synth.stick_figures(persons, seed)
         a = glue_port.paf_to_pose(heat, paf, port)[1]
-        b = glue_port.paf_to_pose(heat, paf, ref)[1]
+        b = humans_rows_to_dicts(g["crowd_%d_%d" % (persons, seed)])
         assert a == b and len(a) > persons // 2
 
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-launch device time and algorithmic TFLOP/s of one bf16 forward (CUDA events around every launch through
-b200pose_net_profile).  Usage on the GPU box: python tools/profile_layers.py [batch] > profiles/rNN_layers.txt"""
+b200pose_net_profile).  Usage on an H100: python tools/profile_layers.py [batch]"""
 import ctypes
 import importlib
 import os

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Video-file front-end on the B200 path: the flow and command line of the reference's video_demo.py (:47-125) - `--cfg`,
+"""Video-file front-end on the H100 path: the flow and command line of the reference's video_demo.py (:47-125) - `--cfg`,
 `--weight`, trailing config overrides, the video path asked on stdin, every frame drawn into output.avi - with the frames
 batched and pipelined through the fused engine (streaming.PoseStream) instead of one get_outputs + paf_to_pose_cpp per
 frame.  Extras: `--video` (skip the prompt), `--out`, `--batch`, `--synthetic-weights`, `--max-frames`.
