@@ -32,7 +32,7 @@ long b200pose_launch_count(void);
 typedef struct b200pose_net b200pose_net;
 
 #define B200POSE_NUM_TENSORS 184   /* state_dict entries, reference order (model0, model{1..6}_1, model{1..6}_2) */
-#define B200POSE_MODE_BF16 0       /* tcgen05 tensor cores, bf16 operands, fp32 accumulate                       */
+#define B200POSE_MODE_BF16 0       /* wgmma tensor cores, bf16 operands, fp32 accumulate                         */
 #define B200POSE_MODE_FP32 1       /* fp32-parity mode: fp32 FMA everywhere (1e-3 bar of BASELINE.json)          */
 #define B200POSE_MODE_BF16X3 2     /* high-precision tensor-core mode: value + residual bf16 planes for activations and
                                       weights, 3 MMA terms per K block (A_hi*W_hi + A_hi*W_lo + A_lo*W_hi); measured
@@ -75,6 +75,23 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess);
  * event pair around every launch; fills per-launch milliseconds and ALGORITHMIC FLOPs (2 x MACs of the unpadded
  * convolution).  Returns the number of launches, < 0 on error. */
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream);
+/* Test hooks of the last bf16 / bf16x3 forward's launch list (launch 0 = conv1_1, 1 .. 51 = the tensor-core launches);
+ * they let a test check one launch against a reference computed from that launch's real inputs.
+ *   b200pose_net_debug_run    : re-runs the first `launches` launches on the last forward's input (plain launches with
+ *                               the plan's own arguments, PDL included, no graph), then synchronises the stream.
+ *   b200pose_net_debug_launch : describes launch i in fields[0 .. B200POSE_DEBUG_LAUNCH_FIELDS - 1]:
+ *       0 input buffer id (-1 = the network input)  1 in_cstride  2 in_ch_base  3 in_ch_group_stride
+ *       4 output buffer id  5 out_cstride  6, 7 out_ch_off[2]  8, 9 store_ch[2]  10 H  11 W  12 ksize  13 cin_blocks
+ *       14 groups  15 n_tile  16 n_tiles  17 relu  18 pool  19 split  20 chunk  21 pdl  22 tps
+ *       23, 24 fp32 stage map written per group (-1 = none)  25 images  26 uint8 input normalisation (launch 0; 0 = fp32)
+ *     Returns the number of fields.
+ *   b200pose_net_debug_read   : copies images [img0, img0 + count) of one buffer to host memory: ids 0 .. 13 are the
+ *     bf16 NHWC activation buffers t1, t2, t3, t4, t5a, t5b, t6, t7, t8, t9, cat, bra, brb, br512 (lo_plane = 1: their
+ *     residual planes, bf16x3 only), 14 .. 25 the fp32 NCHW stage maps in saved_for_loss order. */
+#define B200POSE_DEBUG_LAUNCH_FIELDS 27
+int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream);
+int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap);
+int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes);
 /* Device pointers of the last forward's stage-6 maps (NCHW fp32), valid until the next forward. */
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w);
 

@@ -42,6 +42,9 @@ def lib():
         "b200pose_net_forward_u8": ([vp, vp, ci, ci, ci, ci, ci, ctypes.POINTER(vp), ci, vp], ci),
         "b200pose_net_set_preprocess": ([vp, ci], ci),
         "b200pose_net_profile": ([vp, vp, vp, ci, vp], ci),
+        "b200pose_net_debug_run": ([vp, ci, vp], ci),
+        "b200pose_net_debug_launch": ([vp, ci, vp, ci], ci),
+        "b200pose_net_debug_read": ([vp, ci, ci, ci, ci, vp, cl], ci),
         "b200pose_net_last_maps": ([vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(ci), ctypes.POINTER(ci),
                                     ctypes.POINTER(ci)], ci),
         "b200pose_post_create": ([ctypes.POINTER(vp), ci, ci, ci, ci], ci),
@@ -85,7 +88,8 @@ def lib():
 
 EXPORTED = ["b200pose_last_error", "b200pose_version", "b200pose_launch_count", "b200pose_net_create",
             "b200pose_net_destroy", "b200pose_net_tensor_shape", "b200pose_net_set_tensor", "b200pose_net_finalize",
-            "b200pose_net_forward", "b200pose_net_forward_u8", "b200pose_net_set_preprocess", "b200pose_net_profile", "b200pose_net_last_maps", "b200pose_post_create", "b200pose_post_destroy",
+            "b200pose_net_forward", "b200pose_net_forward_u8", "b200pose_net_set_preprocess", "b200pose_net_profile", "b200pose_net_debug_run", "b200pose_net_debug_launch",
+            "b200pose_net_debug_read", "b200pose_net_last_maps", "b200pose_post_create", "b200pose_post_destroy",
             "b200pose_post_run", "b200pose_post_sync", "b200pose_post_last_ticket", "b200pose_post_select", "b200pose_post_debug", "b200pose_post_debug_sort", "b200pose_post_status_accum", "b200pose_post_num_humans", "b200pose_post_status",
             "b200pose_post_get_humans", "b200pose_post_get_peaks", "b200pose_infer", "b200pose_infer_u8", "b200pose_flip_merge", "b200pose_infer_flip",
             "b200pose_infer_u8_flip", "b200pose_crop_geometry", "b200pose_net_crop_with_factor",

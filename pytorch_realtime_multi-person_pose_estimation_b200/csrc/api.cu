@@ -124,6 +124,18 @@ struct TcLayer {            // one grouped tensor-core launch
     float* bias = nullptr;        // [groups*n_tiles*n_tile]
 };
 
+// What ConvTcArgs does not keep about a launch (its tensor maps hold the input address, not the buffer): recorded per
+// launch by add_plan for the test hooks (b200pose_net_debug_launch).
+struct LaunchInfo {
+    int in_buf, in_cstride, out_buf;   // activation buffer ids (0 .. 13 = t1 .. br512, see kActC), -1 = none
+    int f32[2];                        // index of the fp32 stage map written per group, -1 = none
+};
+
+// Activation buffers t1 .. br512 (buffer ids 0 .. 13 of the test hooks): channels per pixel and spatial divisor.
+constexpr int kNumAct = 14;
+const int kActC[kNumAct] = {64, 64, 128, 128, 256, 256, 256, 512, 512, 256, 192, 256, 256, 1024};
+const int kActDiv[kNumAct] = {1, 2, 2, 4, 4, 4, 8, 8, 8, 8, 8, 8, 8, 8};
+
 }  // namespace
 
 struct b200pose_net {
@@ -139,6 +151,7 @@ struct b200pose_net {
     int pn = 0, pH = 0, pW = 0, pmode = -1;
     std::vector<ConvTcArgs> plan;
     std::vector<double> plan_flops;   // algorithmic FLOPs per launch of `plan`
+    std::vector<LaunchInfo> plan_info;   // buffers of each launch of `plan` (test hooks)
     bool plan_split = false;          // the plan was built for the split-precision (bf16x3) mode
     // Plans of other (n, H, W, mode) keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not
     // re-encode 51 tensor maps and synchronise the stream.  An entry is valid while the activation buffers it points
@@ -148,6 +161,7 @@ struct b200pose_net {
         bool split;
         std::vector<ConvTcArgs> plan;
         std::vector<double> flops;
+        std::vector<LaunchInfo> info;
         std::vector<const void*> buffers;
     };
     bool plan_cache_on = true;
@@ -218,6 +232,27 @@ struct b200pose_post {
 };
 
 namespace {
+
+// activation buffer `id` (0 .. 13 = t1 .. br512) or its residual plane
+DevBuf<__nv_bfloat16>* act_buffer(b200pose_net* net, int id, bool lo) {
+    DevBuf<__nv_bfloat16>* hi[kNumAct] = {&net->t1, &net->t2, &net->t3, &net->t4, &net->t5a, &net->t5b, &net->t6,
+                                          &net->t7, &net->t8, &net->t9, &net->cat, &net->bra, &net->brb, &net->br512};
+    DevBuf<__nv_bfloat16>* lp[kNumAct] = {&net->l1, &net->l2, &net->l3, &net->l4, &net->l5a, &net->l5b, &net->l6,
+                                          &net->l7, &net->l8, &net->l9, &net->lcat, &net->lbra, &net->lbrb, &net->lbr512};
+    return (id < 0 || id >= kNumAct) ? nullptr : (lo ? lp[id] : hi[id]);
+}
+
+int act_buffer_id(b200pose_net* net, const void* p) {
+    for (int i = 0; i < kNumAct; ++i)
+        if (act_buffer(net, i, false)->p == p) return i;
+    return -1;
+}
+
+int f32_map_id(const b200pose_net* net, const float* p) {
+    for (int i = 0; i < 12; ++i)
+        if (p != nullptr && net->out_f32[i].p == p) return i;
+    return -1;
+}
 
 int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_ids /*per group*/, int n_tile,
                   bool cat_input, int ks, int relu, int pool) {
@@ -300,6 +335,8 @@ int add_plan(b200pose_net* net, const TcLayer& L, int n, int H, int W, const __n
     if (e != cudaSuccess) return fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
     net->plan.push_back(a);
     net->plan_flops.push_back(2.0 * n * H * W * L.macs_per_pixel);
+    net->plan_info.push_back({act_buffer_id(net, in), in_cstride, act_buffer_id(net, out),
+                              {f32_map_id(net, f32_0), f32_map_id(net, f32_1)}});
     return 0;
 }
 
@@ -332,6 +369,7 @@ int build_plan_bf16(b200pose_net* net, int n, int H, int W, bool split, cudaStre
     for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px8 * (i % 2 == 0 ? kPaf : kHeat)));
     net->plan.clear();
     net->plan_flops.clear();
+    net->plan_info.clear();
     const std::vector<TcLayer>& T = net->tc;
 #define PLAN(...) do { if (add_plan(net, __VA_ARGS__)) return 1; } while (0)
     // trunk (conv1_1 runs on CUDA cores before the plan)
@@ -391,14 +429,16 @@ bool plan_cache_swap(b200pose_net* net, int n, int H, int W, int want) {
         slot->n = net->kn; slot->H = net->kH; slot->W = net->kW; slot->mode = net->kmode; slot->split = net->plan_split;
         slot->plan.swap(net->plan);
         slot->flops.swap(net->plan_flops);
+        slot->info.swap(net->plan_info);
         slot->buffers = plan_buffers(net);
-        net->plan.clear(); net->plan_flops.clear();
+        net->plan.clear(); net->plan_flops.clear(); net->plan_info.clear();
         net->kmode = -1;
     }
     for (auto& e : net->plan_cache)
         if (e.n == n && e.H == H && e.W == W && e.mode == want && !e.plan.empty() && e.buffers == plan_buffers(net)) {
             net->plan.swap(e.plan);
             net->plan_flops.swap(e.flops);
+            net->plan_info.swap(e.info);
             net->plan_split = e.split;
             net->kn = n; net->kH = H; net->kW = W; net->kmode = want;
             return true;
@@ -647,7 +687,7 @@ int b200pose_net_finalize(b200pose_net* net) {
     net->pmode = -1;
     drop_graphs(net);
     net->plan_cache.clear();      // cached plans point at the previous packed weights
-    net->plan.clear(); net->plan_flops.clear();
+    net->plan.clear(); net->plan_flops.clear(); net->plan_info.clear();
     net->kmode = -1;
     net->finalized = true;
     return 0;
@@ -742,6 +782,73 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
     for (auto& e : ev) cudaEventDestroy(e);
     tmp.release();
     return total;
+}
+
+static bool debug_plan_ready(const b200pose_net* net) {
+    return net && !net->plan.empty() && net->plan_info.size() == net->plan.size() &&
+           (net->pmode == B200POSE_MODE_BF16 || net->pmode == B200POSE_MODE_BF16X3);
+}
+
+int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream) {
+    if (!debug_plan_ready(net) || !net->last_in) return fail("debug_run: no bf16 / bf16x3 forward has run");
+    if (launches < 0 || launches > 1 + (int)net->plan.size()) return fail("debug_run: %d launches out of range", launches);
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (launches >= 1)
+        CU(conv_first_launch(net->last_in, net->last_in_u8, net->d_w[0], net->d_b[0], net->t1.p,
+                             net->plan_split ? net->l1.p : nullptr, net->pn, net->pH, net->pW, st));
+    for (int i = 0; i + 1 < launches; ++i) CU(conv_tc_launch(net->plan[i], net->num_sms, st));
+    g_launches += launches;
+    CU(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
+    if (!debug_plan_ready(net)) return fail("debug_launch: no bf16 / bf16x3 forward has run");
+    if (i < 0 || i > (int)net->plan.size() || cap < B200POSE_DEBUG_LAUNCH_FIELDS || !fields)
+        return fail("debug_launch: launch %d / capacity %d out of range", i, cap);
+    int* f = fields;
+    for (int k = 0; k < B200POSE_DEBUG_LAUNCH_FIELDS; ++k) f[k] = 0;
+    if (i == 0) {     // conv1_1 (CUDA cores / mma.sync): the network input -> t1
+        f[0] = -1; f[1] = 3; f[4] = 0; f[5] = 64; f[8] = 64;
+        f[10] = net->pH; f[11] = net->pW; f[12] = 3; f[14] = 1; f[15] = 64; f[16] = 1; f[17] = 1;
+        f[19] = net->plan_split ? 1 : 0; f[23] = f[24] = -1;
+        f[26] = net->last_in_u8;
+    } else {
+        const ConvTcArgs& a = net->plan[i - 1];
+        const LaunchInfo& li = net->plan_info[i - 1];
+        f[0] = li.in_buf; f[1] = li.in_cstride; f[2] = a.in_ch_base; f[3] = a.in_ch_group_stride;
+        f[4] = li.out_buf; f[5] = a.out_cstride; f[6] = a.out_ch_off[0]; f[7] = a.out_ch_off[1];
+        f[8] = a.store_ch[0]; f[9] = a.store_ch[1];
+        f[10] = a.H; f[11] = a.W; f[12] = a.ksize; f[13] = a.cin_blocks; f[14] = a.groups; f[15] = a.n_tile;
+        f[16] = a.n_tiles; f[17] = a.relu; f[18] = a.pool; f[19] = a.split; f[20] = a.chunk; f[21] = a.pdl; f[22] = a.tps;
+        f[23] = li.f32[0]; f[24] = li.f32[1];
+    }
+    f[25] = net->pn;
+    return B200POSE_DEBUG_LAUNCH_FIELDS;
+}
+
+int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes) {
+    if (!debug_plan_ready(net)) return fail("debug_read: no bf16 / bf16x3 forward has run");
+    const int n = net->pn, H = net->pH, W = net->pW;
+    if (img0 < 0 || count < 1 || img0 + count > n || !host) return fail("debug_read: images [%d, %d) out of range", img0, img0 + count);
+    const char* src = nullptr;
+    size_t per = 0;
+    if (buf >= 0 && buf < kNumAct) {
+        if (lo_plane && !net->plan_split) return fail("debug_read: residual planes exist in bf16x3 mode only");
+        per = (size_t)(H / kActDiv[buf]) * (W / kActDiv[buf]) * kActC[buf] * 2;
+        src = reinterpret_cast<const char*>(act_buffer(net, buf, lo_plane != 0)->p);
+    } else if (buf >= kNumAct && buf < kNumAct + 12 && !lo_plane) {
+        const int m = buf - kNumAct;
+        per = (size_t)(H / 8) * (W / 8) * (m % 2 == 0 ? kPaf : kHeat) * 4;
+        src = reinterpret_cast<const char*>(net->out_f32[m].p);
+    } else {
+        return fail("debug_read: no buffer %d (plane %d)", buf, lo_plane);
+    }
+    if (bytes < (long)(per * count)) return fail("debug_read: %ld bytes given, %zu needed", bytes, per * count);
+    CU(cudaSetDevice(net->device));
+    CU(cudaMemcpy(host, src + per * img0, per * count, cudaMemcpyDeviceToHost));
+    return 0;
 }
 
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w) {

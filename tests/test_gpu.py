@@ -38,9 +38,11 @@ def _forward(net, x, mode):
     return [o.cpu() for o in outs]
 
 
-def test_tcgen05_conv_kernel_cases(built):
-    """Standalone harness: 7 conv configurations (1x1/3x3/7x7, groups, fused pool, padded heads, 4 n-tiles) against
-    a plain CPU loop."""
+def test_wgmma_conv_kernel_cases(built):
+    """Standalone harness (tests/cuda/test_conv_tc.cu): 18 conv configurations (1x1/3x3/7x7, groups, fused pool, padded
+    heads, n-tiles of 32/48/64/128, more work items than SMs, bf16x3 in both chunk styles, channel slices of wider
+    buffers, a PDL-chained launch), each N <= 64 one also K-chunked, against a plain CPU loop with the interval rule of
+    oracle/conv_check.py."""
     r = subprocess.run([os.path.join(ROOT, "build", "test_conv_tc")], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
                        text=True, timeout=600)
     print(r.stdout)

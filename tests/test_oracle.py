@@ -170,3 +170,138 @@ def test_cubic_resize_restatement_vs_opencv():
     ah, ap = glue_port.multi_scale_maps([(h1, p1)] * 4, (12, 16))
     np.testing.assert_array_equal(ah, h1)          # (4 x) / 4 is exact
     np.testing.assert_array_equal(ap, p1)
+
+
+def _emulate_tc(x, w, b, ks, relu, pool, x_lo=None, w_lo=None, chunk=False, skip=None, shift=None, bias_roll=0):
+    """The tensor-core kernel's fp32 arithmetic restated in numpy: per 64-channel block, tap-major, each k16 step adds
+    its exact 16-product partial to the fp32 accumulator with one rounding; bf16x3 runs the terms A_hi W_hi, A_hi W_lo,
+    A_lo W_hi per block, K-chunked (7x7: one chunk per filter row; otherwise one per block and term), chunks summed in
+    fp32.  x: NHWC float32 bf16 values, w: OIHW float64 bf16 values.  Returns v = fp32(acc + bias), NCHW float64.
+    Mutations: skip = (block, tap, k16) left out; shift = tap whose window is read one pixel to the right;
+    bias_roll = bias of a neighbouring channel."""
+    n, H, W, C = x.shape
+    p = ks // 2
+    planes = [np.pad(x.astype(np.float64), ((0, 0), (p, p), (p, p + 1), (0, 0)))]
+    if x_lo is not None:
+        planes.append(np.pad(x_lo.astype(np.float64), ((0, 0), (p, p), (p, p + 1), (0, 0))))
+    terms = [(0, w)] if x_lo is None else [(0, w), (0, w_lo), (1, w)]
+    O = w.shape[0]
+    acc = np.zeros((n * H * W, O), np.float32)
+    total = np.zeros_like(acc)
+    for cb in range(C // 64):
+        for pl, wt in terms:
+            for tap in range(ks * ks):
+                dy, dx = divmod(tap, ks)
+                if chunk and ((ks == 7 and dx == 0) or (ks != 7 and tap == 0)):
+                    acc[:] = 0
+                ox = dx + (1 if shift == tap else 0)
+                a = planes[pl][:, dy:dy + H, ox:ox + W, :].reshape(-1, C)
+                for k in range(4):
+                    if skip == (cb, tap, k):
+                        continue
+                    c0 = cb * 64 + 16 * k
+                    part = a[:, c0:c0 + 16] @ wt[:, c0:c0 + 16, dy, dx].T
+                    acc = (acc.astype(np.float64) + part).astype(np.float32)
+                if chunk and ((ks == 7 and dx == ks - 1) or (ks != 7 and tap == ks * ks - 1)):
+                    total = total + acc          # float32 + float32: round to nearest
+    if not chunk:
+        total = acc
+    v = total + np.roll(b, -bias_roll).astype(np.float32)[None, :]
+    return torch.from_numpy(v.reshape(n, H, W, O).transpose(0, 3, 1, 2).astype(np.float64))
+
+
+def _layer(kind, seed):
+    """A realistic layer: (x NHWC float32 bf16 values, x_lo, w OIHW fp32, b, ks, relu, pool, logical input channels).
+    mconv1: a stage >= 2 Mconv1 of two groups reading the 192-channel concat buffer [PAF 0..37 | 0 0 | heat 40..58 |
+    0 x 5 | features 64..191]; trunk: a 3x3 256 -> 256 layer with the fused 2x2 pool at width 92 (a partial last tile)."""
+    from oracle import conv_check
+    rs = np.random.RandomState(seed)
+    if kind == "mconv1":
+        n, H, W, C, cin, cout, ks, pool = 1, 16, 20, 192, 185, 256, 7, 0
+        phys = np.r_[0:38, 40:59, 64:192]
+    else:
+        n, H, W, C, cin, cout, ks, pool = 1, 16, 92, 256, 256, 256, 3, 1
+        phys = np.arange(256)
+    full = np.zeros((n, H, W, C), np.float32)
+    full[..., phys] = np.maximum(rs.randn(n, H, W, len(phys)), 0).astype(np.float32) * 1.5
+    x = conv_check.bf16_round(torch.from_numpy(full.astype(np.float64))).numpy().astype(np.float32)
+    x_lo = conv_check.bf16_round(torch.from_numpy(full.astype(np.float64) - x)).numpy().astype(np.float32)
+    w = (rs.randn(cout, cin, ks, ks) * np.sqrt(2.0 / (cin * ks * ks))).astype(np.float32)
+    b = (rs.rand(cout) * 0.2 - 0.1).astype(np.float32)
+    return x, x_lo, w, b, ks, 1, pool, phys
+
+
+def _check(x, x_lo, w, b, ks, relu, pool, phys, got_hi, got_lo=None):
+    """The oracle's verdict for a layer (groups sharing the input are one conv here): Verdict of every output."""
+    from oracle import conv_check
+    C = x.shape[3]
+    w_hi, w_lo = conv_check.split_weights(w)
+    wp_hi = torch.zeros((w.shape[0], C, ks, ks), dtype=torch.float64)     # weights on the physical input channels
+    wp_lo = torch.zeros_like(wp_hi)
+    wp_hi[:, torch.from_numpy(phys)] = w_hi
+    wp_lo[:, torch.from_numpy(phys)] = w_lo
+    xt = torch.from_numpy(x.astype(np.float64)).permute(0, 3, 1, 2)
+    bt = torch.from_numpy(b.astype(np.float64))
+    split = got_lo is not None
+    if split:
+        r, S = conv_check.reference(xt, wp_hi, bt, ks, torch.from_numpy(x_lo.astype(np.float64)).permute(0, 3, 1, 2), wp_lo)
+    else:
+        r, S = conv_check.reference(xt, wp_hi, bt, ks)
+    e = conv_check.U * conv_check.bound_coef(ks, C, split=split, chunk=split) * S
+    if split:
+        return conv_check.check_split(got_hi, got_lo, r, e, relu, pool)
+    return conv_check.check_bf16(got_hi, r, e, relu, pool)
+
+
+@pytest.mark.parametrize("kind", ["mconv1", "trunk"])
+def test_conv_checker_accepts_the_kernel_arithmetic_and_rejects_each_mutation(kind):
+    """oracle/conv_check.py is what the GPU layer test trusts, so it must be able to fail.  The kernel's own fp32
+    accumulation order, emulated here, must pass; each of the faults a wgmma conv is prone to, applied to that emulation,
+    must be caught by the 2^-22 bound at the real K (mconv1: K = 49 x 192 = 9 408; trunk: 9 x 256 = 2 304)."""
+    from oracle import conv_check
+    x, x_lo, w, b, ks, relu, pool, phys = _layer(kind, 7)
+    w_hi, w_lo = conv_check.split_weights(w)
+    wp_hi = np.zeros((w.shape[0], x.shape[3], ks, ks))
+    wp_lo = np.zeros_like(wp_hi)
+    wp_hi[:, phys], wp_lo[:, phys] = w_hi.numpy(), w_lo.numpy()
+
+    def out_bf16(v):
+        return conv_check.bf16_round(conf(v))
+
+    def conf(v):
+        return conv_check.f_act(v, relu, pool)
+
+    v = _emulate_tc(x, wp_hi, b, ks, relu, pool)
+    ok = _check(x, x_lo, w, b, ks, relu, pool, phys, out_bf16(v))
+    print("%s bf16: emulated kernel accepted, max |v - r| / e = %.3f" % (kind, ok.ratio))
+    assert bool(ok.ok.all()), conv_check.describe(ok, out_bf16(v), kind, pool)
+
+    mutants = {
+        "k16 slice of one tap dropped": _emulate_tc(x, wp_hi, b, ks, relu, pool, skip=(1, ks * ks // 2 + 1, 2)),
+        "one tap read one pixel off": _emulate_tc(x, wp_hi, b, ks, relu, pool, shift=ks * ks - 1),
+        "neighbour's bias": _emulate_tc(x, wp_hi, b, ks, relu, pool, bias_roll=1),
+    }
+    last = v.clone()
+    last[..., -1] = v[..., -2]                     # the partial last tile's last column stored from its neighbour
+    mutants["last partial tile column wrong"] = last
+    swapped = v.clone()
+    swapped[:, [5, 6]] = v[:, [6, 5]]              # two channels of an n-tile swapped
+    mutants["two channels of an n-tile swapped"] = swapped
+    for name, mv in mutants.items():
+        verdict = _check(x, x_lo, w, b, ks, relu, pool, phys, out_bf16(mv))
+        assert not bool(verdict.ok.all()), "%s: mutation '%s' passed the checker" % (kind, name)
+        print("%s bf16: '%s' rejected (%d bad elements)" % (kind, name, int((~verdict.ok).sum())))
+    if pool:                                       # the 2x2 max taken over the wrong column pair
+        verdict = _check(x, x_lo, w, b, ks, relu, pool, phys, out_bf16(torch.roll(v, -1, 3)))
+        assert not bool(verdict.ok.all()), "%s: wrong pool neighbour passed the checker" % kind
+
+    # bf16x3: the three-term, K-chunked emulation passes; without the A_lo W_hi term it must not
+    for drop_lo, should_pass in ((False, True), (True, False)):
+        xl = np.zeros_like(x_lo) if drop_lo else x_lo      # without: A_hi W_hi + A_hi W_lo only
+        fv = conf(_emulate_tc(x, wp_hi, b, ks, relu, pool, x_lo=xl, w_lo=wp_lo, chunk=True))
+        hi = conv_check.bf16_round(fv)
+        lo = conv_check.bf16_round(fv - hi)
+        verdict = _check(x, x_lo, w, b, ks, relu, pool, phys, hi, lo)
+        assert bool(verdict.ok.all()) == should_pass, (kind, drop_lo, conv_check.describe(verdict, hi + lo, kind, pool))
+        print("%s bf16x3%s: %s, max |v - r| / e = %.3f" % (kind, " without A_lo W_hi" if drop_lo else "",
+                                                           "accepted" if should_pass else "rejected", verdict.ratio))
