@@ -71,6 +71,13 @@ int b200pose_net_forward_u8(b200pose_net* net, const unsigned char* images, int 
 #define B200POSE_PRE_INCEPTION 3   /* BGR -> RGB, x/128 - 1                         */
 #define B200POSE_PRE_SSD 4         /* x - (123, 117, 104) on (B, G, R)              */
 int b200pose_net_set_preprocess(b200pose_net* net, int preprocess);
+/* Ragged batch (DESIGN.md 1): n already cropped uint8 HWC BGR frames of different sizes, packed back to back (frame i is
+ * hw[2i] x hw[2i+1] x 3 bytes, both multiples of 8; n <= 1024).  The batch runs on the canvas Hc x Wc = (max H_i, max W_i):
+ * outputs[12] as b200pose_net_forward's at canvas size [n, C, Hc/8, Wc/8]; inside its own (H_i/8) x (W_i/8) each frame's
+ * maps are bit for bit those of b200pose_net_forward_u8 on that frame alone, outside they are +0.  Plans (and the CUDA
+ * graphs of small batches) are keyed on (n, Hc, Wc, mode): a new mix of frames on the same canvas rebuilds nothing. */
+int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frames, int on_device, int n, const int* hw,
+                                   int mode, float* const* outputs, int outputs_on_device, void* cuda_stream);
 /* Measurement hook: re-runs the launch list of the last bf16 forward (conv1_1 + 51 tensor-core launches) with a CUDA
  * event pair around every launch; fills per-launch milliseconds and ALGORITHMIC FLOPs (2 x MACs of the unpadded
  * convolution).  Returns the number of launches, < 0 on error. */
@@ -194,6 +201,13 @@ int b200pose_net_crop_with_factor(b200pose_net* net, const unsigned char* images
 int b200pose_infer_raw_u8(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device, int n,
                           int src_h, int src_w, int dest_size, int factor, int mode, float thresh, int flip,
                           void* cuda_stream);
+/* b200pose_infer_raw_u8 for n raw frames of DIFFERENT sizes, packed back to back (frame i: src_hw[2i] x src_hw[2i+1] x 3
+ * bytes), as one ragged batch (DESIGN.md 1): every frame is cropped to its own padded size and the batch runs on the
+ * canvas of the largest; with flip the network runs 2n images.  Per frame, person rows and peaks are those
+ * b200pose_infer_raw_u8 gives for that frame alone, in pixels of its own padded frame.  Fetched like b200pose_infer's. */
+int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device,
+                                 int n, const int* src_hw, int dest_size, int factor, int mode, float thresh, int flip,
+                                 void* cuda_stream);
 
 /* Multi-scale (+ flip) test-time averaging, BASELINE.json configs[4].  The reference at this commit has no multi-scale
  * loop (get_outputs is single-scale, evaluate/coco_eval.py:87-91); the protocol is composed from its own functions:

@@ -41,6 +41,7 @@ def lib():
         "b200pose_net_forward": ([vp, vp, ci, ci, ci, ci, ci, ctypes.POINTER(vp), ci, vp], ci),
         "b200pose_net_forward_u8": ([vp, vp, ci, ci, ci, ci, ci, ctypes.POINTER(vp), ci, vp], ci),
         "b200pose_net_set_preprocess": ([vp, ci], ci),
+        "b200pose_net_forward_ragged_u8": ([vp, vp, ci, ci, vp, ci, ctypes.POINTER(vp), ci, vp], ci),
         "b200pose_net_profile": ([vp, vp, vp, ci, vp], ci),
         "b200pose_net_debug_run": ([vp, ci, vp], ci),
         "b200pose_net_debug_launch": ([vp, ci, vp, ci], ci),
@@ -70,6 +71,7 @@ def lib():
         "b200pose_infer_raw_u8": ([vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, cf, ci, vp], ci),
         "b200pose_infer_raw_u8_multiscale": ([vp, vp, vp, ci, ci, ci, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf,
                                               ci, vp], ci),
+        "b200pose_infer_raw_u8_ragged": ([vp, vp, vp, ci, ci, vp, ci, ci, ci, cf, ci, vp], ci),
         "process_paf": ([ci, ci, ci, vp, ci, ci, ci, vp, ci, ci, ci, vp], ci),
         "get_num_humans": ([], ci),
         "get_part_cid": ([ci, ci], ci),
@@ -88,12 +90,12 @@ def lib():
 
 EXPORTED = ["b200pose_last_error", "b200pose_version", "b200pose_launch_count", "b200pose_net_create",
             "b200pose_net_destroy", "b200pose_net_tensor_shape", "b200pose_net_set_tensor", "b200pose_net_finalize",
-            "b200pose_net_forward", "b200pose_net_forward_u8", "b200pose_net_set_preprocess", "b200pose_net_profile", "b200pose_net_debug_run", "b200pose_net_debug_launch",
+            "b200pose_net_forward", "b200pose_net_forward_u8", "b200pose_net_forward_ragged_u8", "b200pose_net_set_preprocess", "b200pose_net_profile", "b200pose_net_debug_run", "b200pose_net_debug_launch",
             "b200pose_net_debug_read", "b200pose_net_last_maps", "b200pose_post_create", "b200pose_post_destroy",
             "b200pose_post_run", "b200pose_post_sync", "b200pose_post_last_ticket", "b200pose_post_select", "b200pose_post_debug", "b200pose_post_debug_sort", "b200pose_post_status_accum", "b200pose_post_num_humans", "b200pose_post_status",
             "b200pose_post_get_humans", "b200pose_post_get_peaks", "b200pose_infer", "b200pose_infer_u8", "b200pose_flip_merge", "b200pose_infer_flip",
             "b200pose_infer_u8_flip", "b200pose_crop_geometry", "b200pose_net_crop_with_factor",
-            "b200pose_infer_raw_u8", "b200pose_infer_raw_u8_multiscale", "process_paf", "get_num_humans",
+            "b200pose_infer_raw_u8", "b200pose_infer_raw_u8_ragged", "b200pose_infer_raw_u8_multiscale", "process_paf", "get_num_humans",
             "get_part_cid", "get_score", "get_part_x", "get_part_y", "get_part_score"]
 
 

@@ -133,6 +133,7 @@ struct LaunchInfo {
 
 // Activation buffers t1 .. br512 (buffer ids 0 .. 13 of the test hooks): channels per pixel and spatial divisor.
 constexpr int kNumAct = 14;
+constexpr int kMaxRagged = 1024;      // images of one ragged forward (flip: 2 per frame)
 const int kActC[kNumAct] = {64, 64, 128, 128, 256, 256, 256, 512, 512, 256, 192, 256, 256, 1024};
 const int kActDiv[kNumAct] = {1, 2, 2, 4, 4, 4, 8, 8, 8, 8, 8, 8, 8, 8};
 
@@ -170,7 +171,7 @@ struct b200pose_net {
     // (B200POSE_GRAPH=0: plain launches).  Graphs embed the tensor maps, i.e. buffer addresses: every plan build drops them.
     // Capture needs a real stream: calls on the legacy default stream (0) launch directly.
     struct GraphKey {
-        int n, H, W, mode, in_u8;
+        int n, H, W, mode, in_u8, ragged;
         const void* in;
         bool operator<(const GraphKey& o) const {
             if (n != o.n) return n < o.n;
@@ -178,6 +179,7 @@ struct b200pose_net {
             if (W != o.W) return W < o.W;
             if (mode != o.mode) return mode < o.mode;
             if (in_u8 != o.in_u8) return in_u8 < o.in_u8;
+            if (ragged != o.ragged) return ragged < o.ragged;
             return in < o.in;
         }
     };
@@ -199,6 +201,12 @@ struct b200pose_net {
     DevBuf<unsigned char> in_stage_u8;
     int preprocess = 1;                // normalisation fused into the uint8 entry points (preprocess_core.h; 1 = rtpose)
     DevBuf<unsigned char> raw_stage;   // raw (un-resized) frames of b200pose_*crop* / b200pose_infer_raw_u8
+    // Ragged batches (DESIGN.md §1): the extents table [H_0, W_0, H_1, W_1, ...] every kernel of a ragged forward reads.
+    // Allocated once for kMaxRagged images and never moved, so that plans and captured graphs stay valid across mixes;
+    // rewritten on the stream before each ragged forward.
+    int* d_ext = nullptr;
+    const int* last_ext = nullptr;     // extents of the last forward (null: uniform), for the test hooks
+    DevBuf<RaggedFrame> d_frames;      // per-frame source geometry of the last ragged crop
 };
 
 struct b200pose_post {
@@ -229,6 +237,9 @@ struct b200pose_post {
     DevBuf<float> ov_maps[2];                       // [heat | paf] copies, slot = run parity
     cudaEvent_t ev_maps = nullptr, ev_ld[2] = {nullptr, nullptr};   // maps copied (st) / limbs done with a slot (s2)
     bool have_ld[2] = {false, false};
+    // extents of a ragged run, slot = run parity: the peaks / limbs of run i on the second stream still read them while
+    // run i+1 rewrites the net's table
+    int* d_ext[2] = {nullptr, nullptr};
 };
 
 namespace {
@@ -403,6 +414,11 @@ int build_plan_bf16(b200pose_net* net, int n, int H, int W, bool split, cudaStre
              net->out_f32[2 * (s - 1)].p, net->out_f32[2 * (s - 1) + 1].p, kPaf, kHeat);
     }
 #undef PLAN
+    for (ConvTcArgs& a : net->plan) {      // ragged batches: the launch's output resolution relative to the input
+        int s = 0;
+        while ((a.H << s) < H) ++s;
+        a.ext_shift = s + a.pool;
+    }
     return 0;
 }
 
@@ -452,13 +468,23 @@ void drop_graphs(b200pose_net* net) {
     net->graph_seen.clear();
 }
 
-int launch_forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, cudaStream_t st, bool split) {
-    CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->t1.p, split ? net->l1.p : nullptr, n, H, W, st));
-    for (const ConvTcArgs& a : net->plan) CU(conv_tc_launch(a, net->num_sms, st));
+// plan launch i; a ragged forward passes its extents table (the plans are shared with uniform batches of the canvas size)
+cudaError_t launch_plan_entry(const b200pose_net* net, size_t i, const int* ext, cudaStream_t st) {
+    if (ext == nullptr) return conv_tc_launch(net->plan[i], net->num_sms, st);
+    ConvTcArgs a = net->plan[i];
+    a.ext = ext;
+    return conv_tc_launch(a, net->num_sms, st);
+}
+
+int launch_forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, cudaStream_t st, bool split,
+                        const int* ext) {
+    CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->t1.p, split ? net->l1.p : nullptr, n, H, W, ext, st));
+    for (size_t i = 0; i < net->plan.size(); ++i) CU(launch_plan_entry(net, i, ext, st));
     return 0;
 }
 
-int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, cudaStream_t st, bool split) {
+int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, cudaStream_t st, bool split,
+                 const int* ext) {
     const int want = split ? B200POSE_MODE_BF16X3 : B200POSE_MODE_BF16;
     if (net->pn != n || net->pH != H || net->pW != W || net->pmode != want) {
         if (!(net->plan_cache_on && plan_cache_swap(net, n, H, W, want))) {
@@ -473,11 +499,11 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     if (net->use_graph && small_plan(net, n, H, W) && st != nullptr && cudaStreamIsCapturing(st, &cap) == cudaSuccess &&
         cap == cudaStreamCaptureStatusNone) {
-        const b200pose_net::GraphKey key{n, H, W, want, in_u8, d_in};
+        const b200pose_net::GraphKey key{n, H, W, want, in_u8, ext != nullptr, d_in};
         auto it = net->graphs.find(key);
         if (it == net->graphs.end() && net->graph_seen.insert(key).second) {      // first sight: plain launches
             if (net->graph_seen.size() > 4096) net->graph_seen.clear();
-            if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split)) return 1;
+            if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext)) return 1;
             g_launches += launches;
             return 0;
         }
@@ -486,7 +512,7 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
             cudaGraph_t graph = nullptr;
             cudaGraphExec_t exec = nullptr;
             CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-            const int rc = launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split);
+            const int rc = launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext);
             cudaError_t e = cudaStreamEndCapture(st, &graph);
             if (rc == 0 && e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
             if (graph) cudaGraphDestroy(graph);
@@ -495,7 +521,7 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
                 fprintf(stderr, "[b200pose] CUDA graph capture of the forward pass failed (%s): launching directly\n",
                         rc ? b200pose_last_error() : cudaGetErrorString(e));
                 net->use_graph = false;
-                if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split)) return 1;
+                if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext)) return 1;
                 g_launches += launches;
                 return 0;
             }
@@ -505,12 +531,12 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
         g_launches += launches;
         return 0;
     }
-    if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split)) return 1;
+    if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext)) return 1;
     g_launches += launches;
     return 0;
 }
 
-int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, cudaStream_t st) {
+int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, cudaStream_t st, const int* ext) {
     const size_t px1 = (size_t)n * H * W;
     const int h = H / 8, w = W / 8;
     const size_t px8 = (size_t)n * h * w;
@@ -532,6 +558,9 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, cuda
         a.in = in; a.in_cstride = in_cs; a.in_ch_off = in_off; a.w = net->d_w[ci]; a.bias = net->d_b[ci];
         a.out = out; a.out_cstride = out_cs; a.out_ch_off = out_off; a.out_nchw = nchw;
         a.n_img = n; a.H = hh; a.W = ww; a.cin = s.cin; a.cout = s.cout; a.ks = s.ks; a.relu = relu;
+        a.ext = ext;
+        a.ext_shift = 0;
+        while ((hh << a.ext_shift) < H) ++a.ext_shift;
         CU(conv_f32_launch(a, st));
         ++g_launches;
         return 0;
@@ -631,6 +660,8 @@ void b200pose_net_destroy(b200pose_net* net) {
     DevBuf<float>* fb[] = {&net->in_stage, &net->f_a, &net->f_b, &net->f_cat, &net->f_x, &net->f_y, &net->f_in, &net->f_u8};
     net->in_stage_u8.release();
     net->raw_stage.release();
+    net->d_frames.release();
+    if (net->d_ext) cudaFree(net->d_ext);
     for (auto* b : fb) b->release();
     for (auto& b : net->out_f32) b.release();
     delete net;
@@ -693,8 +724,10 @@ int b200pose_net_finalize(b200pose_net* net) {
     return 0;
 }
 
+// ext: device extents table of a ragged batch (DESIGN.md §1), or null
 static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int input_on_device, int n, int H, int W,
-                            int mode, float* const* outputs, int outputs_on_device, cudaStream_t st, bool sync_host) {
+                            int mode, float* const* outputs, int outputs_on_device, cudaStream_t st, bool sync_host,
+                            const int* ext = nullptr) {
     if (!net || !net->finalized) return fail("net not finalized");
     if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
     CU(cudaSetDevice(net->device));
@@ -715,13 +748,14 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
     if (mode == B200POSE_MODE_FP32) {
         if (in_u8) {   // parity mode: materialise rtpose_preprocess, then the fp32 path
             CU(net->f_u8.ensure(elems));
-            CU(u8hwc_to_f32nchw_launch(static_cast<const unsigned char*>(d_in), net->f_u8.p, n, H, W, net->preprocess, st));
+            CU(u8hwc_to_f32nchw_launch(static_cast<const unsigned char*>(d_in), net->f_u8.p, n, H, W, net->preprocess, ext, st));
             ++g_launches;
-            rc = forward_fp32(net, net->f_u8.p, n, H, W, st);
-        } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, st);
-    } else rc = forward_bf16(net, d_in, in_u8 ? net->preprocess : 0, n, H, W, st, mode == B200POSE_MODE_BF16X3);
+            rc = forward_fp32(net, net->f_u8.p, n, H, W, st, ext);
+        } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, st, ext);
+    } else rc = forward_bf16(net, d_in, in_u8 ? net->preprocess : 0, n, H, W, st, mode == B200POSE_MODE_BF16X3, ext);
     if (rc) return rc;
     net->last_in = d_in;
+    net->last_ext = ext;
     net->last_in_u8 = (mode == B200POSE_MODE_FP32) ? 0 : (in_u8 ? net->preprocess : 0);
     net->pn = n; net->pH = H; net->pW = W;
     if (outputs) {
@@ -747,6 +781,76 @@ int b200pose_net_forward_u8(b200pose_net* net, const unsigned char* images, int 
                             reinterpret_cast<cudaStream_t>(cuda_stream), true);
 }
 
+// ------------------------------------------------------------------------------------------------ ragged batches
+// Validates the padded sizes of a ragged batch (DESIGN.md §1) and returns its canvas.
+static int ragged_canvas(int n, const int* hw, int* Hc, int* Wc) {
+    if (n < 1 || n > kMaxRagged) return fail("ragged batch: %d images (1 .. %d)", n, kMaxRagged);
+    if (!hw) return fail("ragged batch: null size table");
+    *Hc = *Wc = 0;
+    for (int i = 0; i < n; ++i) {
+        const int H = hw[2 * i], W = hw[2 * i + 1];
+        if (H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("ragged batch: image %d is %d x %d (multiples of 8 needed)", i, H, W);
+        if (H > *Hc) *Hc = H;
+        if (W > *Wc) *Wc = W;
+    }
+    return 0;
+}
+
+// Writes the extents of the next ragged forward into the net's fixed table (stream-ordered after the previous forward).
+static int upload_ext(b200pose_net* net, const std::vector<int>& ext, cudaStream_t st) {
+    if (!net->d_ext) CU(cudaMalloc(&net->d_ext, (size_t)kMaxRagged * 2 * sizeof(int)));
+    CU(cudaMemcpyAsync(net->d_ext, ext.data(), ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
+static int upload_frames(b200pose_net* net, const std::vector<RaggedFrame>& frames, cudaStream_t st) {
+    CU(net->d_frames.ensure(frames.size()));
+    CU(cudaMemcpyAsync(net->d_frames.p, frames.data(), frames.size() * sizeof(RaggedFrame), cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
+// the n frames of net->d_frames (sources at d_src) -> net->in_stage_u8 [n, Hc, Wc, 3]
+static int place_ragged_frames(b200pose_net* net, const unsigned char* d_src, int n, int Hc, int Wc, cudaStream_t st) {
+    CU(net->in_stage_u8.ensure((size_t)n * Hc * Wc * 3));
+    cudaError_t e = ragged_frames_launch(d_src, net->d_frames.p, n, net->in_stage_u8.p, Hc, Wc, st);
+    if (e != cudaSuccess) return fail("ragged_frames_launch: %s", cudaGetErrorString(e));
+    ++g_launches;
+    return 0;
+}
+
+int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frames, int on_device, int n, const int* hw,
+                                   int mode, float* const* outputs, int outputs_on_device, void* cuda_stream) {
+    if (!net || !net->finalized) return fail("net not finalized");
+    if (!frames) return fail("forward_ragged: null pointer");
+    int Hc, Wc;
+    if (int rc = ragged_canvas(n, hw, &Hc, &Wc)) return rc;
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    std::vector<RaggedFrame> tab(n);
+    long long bytes = 0;
+    for (int i = 0; i < n; ++i) {
+        tab[i] = RaggedFrame{};
+        tab[i].off = bytes;
+        tab[i].src_h = hw[2 * i];
+        tab[i].src_w = hw[2 * i + 1];      // g.pad_h == 0: copied as it is
+        bytes += (long long)hw[2 * i] * hw[2 * i + 1] * 3;
+    }
+    const unsigned char* d_src = frames;
+    if (!on_device) {
+        CU(net->raw_stage.ensure((size_t)bytes));
+        CU(cudaMemcpyAsync(net->raw_stage.p, frames, (size_t)bytes, cudaMemcpyHostToDevice, st));
+        d_src = net->raw_stage.p;
+    }
+    if (int rc = upload_frames(net, tab, st)) return rc;
+    if (int rc = place_ragged_frames(net, d_src, n, Hc, Wc, st)) return rc;
+    if (int rc = upload_ext(net, std::vector<int>(hw, hw + 2 * n), st)) return rc;
+    if (int rc = net_forward_impl(net, net->in_stage_u8.p, 1, 1, n, Hc, Wc, mode, outputs, outputs_on_device, st, true,
+                                  net->d_ext))
+        return rc;
+    if (!on_device) CU(cudaStreamSynchronize(st));
+    return 0;
+}
+
 int b200pose_net_set_preprocess(b200pose_net* net, int preprocess) {
     if (!net) return fail("null net");
     if (preprocess < 1 || preprocess > 4) return fail("preprocess must be 1 (rtpose), 2 (vgg), 3 (inception) or 4 (ssd)");
@@ -768,7 +872,7 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
     if (!d_in) { if (tmp.ensure((size_t)n * 3 * H * W) != cudaSuccess) return -1; cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st); d_in = tmp.p; net->last_in_u8 = 0; }
     cudaEventRecord(ev[0], st);
     conv_first_launch(d_in, net->last_in_u8, net->d_w[0], net->d_b[0], net->t1.p, net->plan_split ? net->l1.p : nullptr, n, H, W,
-                      st);
+                      nullptr, st);
     cudaEventRecord(ev[1], st);
     for (size_t i = 0; i < net->plan.size(); ++i) {
         conv_tc_launch(net->plan[i], net->num_sms, st);
@@ -796,8 +900,8 @@ int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (launches >= 1)
         CU(conv_first_launch(net->last_in, net->last_in_u8, net->d_w[0], net->d_b[0], net->t1.p,
-                             net->plan_split ? net->l1.p : nullptr, net->pn, net->pH, net->pW, st));
-    for (int i = 0; i + 1 < launches; ++i) CU(conv_tc_launch(net->plan[i], net->num_sms, st));
+                             net->plan_split ? net->l1.p : nullptr, net->pn, net->pH, net->pW, net->last_ext, st));
+    for (int i = 0; i + 1 < launches; ++i) CU(launch_plan_entry(net, (size_t)i, net->last_ext, st));
     g_launches += launches;
     CU(cudaStreamSynchronize(st));
     return 0;
@@ -883,6 +987,7 @@ int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, in
         CU(cudaHostAlloc(&p->hp_counts[b], (size_t)batch_cap * 18 * sizeof(int), cudaHostAllocDefault));
         CU(cudaHostAlloc(&p->hp_humans[b], (size_t)batch_cap * human_cap * kHumanFloats * sizeof(float), cudaHostAllocMapped | cudaHostAllocPortable));   // written by assemble_kernel (same pointer on the device: unified addressing)
         CU(cudaEventCreateWithFlags(&p->ev_ld[b], cudaEventDisableTiming));
+        CU(cudaMalloc(&p->d_ext[b], (size_t)batch_cap * 2 * sizeof(int)));
     }
     CU(cudaEventCreateWithFlags(&p->ev_maps, cudaEventDisableTiming));
     const char* ov = getenv("B200POSE_POST_OVERLAP");
@@ -907,6 +1012,7 @@ void b200pose_post_destroy(b200pose_post* p) {
         if (p->hp_status[b]) cudaFreeHost(p->hp_status[b]);
         if (p->hp_counts[b]) cudaFreeHost(p->hp_counts[b]);
         if (p->hp_humans[b]) cudaFreeHost(p->hp_humans[b]);
+        if (p->d_ext[b]) cudaFree(p->d_ext[b]);
     }
     if (p->ev_limbs) cudaEventDestroy(p->ev_limbs);
     if (p->ev_asm) cudaEventDestroy(p->ev_asm);
@@ -937,17 +1043,22 @@ static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st) 
     return 0;
 }
 
+// ext: device extents table of a ragged batch (h x w is then its canvas at the maps' resolution), or null
 static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_paf, int layout, int n, int h, int w,
-                        float thresh, cudaStream_t st) {
+                        float thresh, cudaStream_t st, const int* ext = nullptr) {
     if (n > p->pb.batch_cap) return fail("batch %d exceeds post batch_cap %d", n, p->pb.batch_cap);
     cudaStream_t ps = st;       // the stream peaks / limbs run on
     const int slot = (int)(p->runs & 1);
+    if (p->overlap && p->have_ld[slot]) CU(cudaStreamWaitEvent(st, p->ev_ld[slot], 0));   // run i-2 is done with this slot
+    if (ext) {
+        CU(cudaMemcpyAsync(p->d_ext[slot], ext, (size_t)n * 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        ext = p->d_ext[slot];
+    }
     if (p->overlap) {
         // private copy of the maps (15 MB at batch 32) so that the next forward may overwrite the network's output
         // buffers while this run's post-processing is still reading; everything after the copy runs on s2
         const size_t eh = (size_t)n * 19 * h * w, ep = (size_t)n * 38 * h * w;
         CU(p->ov_maps[slot].ensure(eh + ep));
-        if (p->have_ld[slot]) CU(cudaStreamWaitEvent(st, p->ev_ld[slot], 0));   // run i-2 is done with this slot
         CU(cudaMemcpyAsync(p->ov_maps[slot].p, d_heat, eh * 4, cudaMemcpyDeviceToDevice, st));
         CU(cudaMemcpyAsync(p->ov_maps[slot].p + eh, d_paf, ep * 4, cudaMemcpyDeviceToDevice, st));
         CU(cudaEventRecord(p->ev_maps, st));
@@ -962,10 +1073,11 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
     if (p->runs > 0) CU(cudaStreamWaitEvent(ps, p->ev_fetch[(p->runs - 1) & 1], 0));
     cudaError_t e;
     if (layout == 0) {
-        e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, (long)h * w, w, 1, h, w, thresh, ps);
+        e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, (long)h * w, w, 1, h, w, thresh, ps, ext);
         if (e != cudaSuccess) return fail("post_peaks: %s", cudaGetErrorString(e));
-        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps);
+        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps, ext);
     } else {
+        if (ext) return fail("post_run: ragged batches need the planar (layout 0) maps");
         e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, 1, (long)w * 19, 19, h, w, thresh, ps);
         if (e != cudaSuccess) return fail("post_peaks: %s", cudaGetErrorString(e));
         e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * 8, w, h, ps);
@@ -1112,14 +1224,14 @@ int b200pose_infer_u8(b200pose_net* net, b200pose_post* post, const unsigned cha
 
 // ------------------------------------------------------------------------------------------------ flip TTA
 static int flip_merge_dev(const float* nh, const float* fh, const float* np_, const float* fp, int layout, int n, int h,
-                          int w, float* oh, float* op, cudaStream_t st) {
+                          int w, float* oh, float* op, cudaStream_t st, const int* ext = nullptr) {
     cudaError_t e;
     if (layout == 0) {
-        e = tta_flip_merge(nh, fh, oh, n, kHeat, h, w, (long)h * w, w, 1, st);
-        if (e == cudaSuccess) e = tta_flip_merge(np_, fp, op, n, kPaf, h, w, (long)h * w, w, 1, st);
+        e = tta_flip_merge(nh, fh, oh, n, kHeat, h, w, (long)h * w, w, 1, ext, st);
+        if (e == cudaSuccess) e = tta_flip_merge(np_, fp, op, n, kPaf, h, w, (long)h * w, w, 1, ext, st);
     } else {
-        e = tta_flip_merge(nh, fh, oh, n, kHeat, h, w, 1, (long)w * kHeat, kHeat, st);
-        if (e == cudaSuccess) e = tta_flip_merge(np_, fp, op, n, kPaf, h, w, 1, (long)w * kPaf, kPaf, st);
+        e = tta_flip_merge(nh, fh, oh, n, kHeat, h, w, 1, (long)w * kHeat, kHeat, ext, st);
+        if (e == cudaSuccess) e = tta_flip_merge(np_, fp, op, n, kPaf, h, w, 1, (long)w * kPaf, kPaf, ext, st);
     }
     if (e != cudaSuccess) return fail("tta_flip_merge: %s", cudaGetErrorString(e));
     g_launches += 2;
@@ -1293,6 +1405,71 @@ int b200pose_infer_raw_u8(b200pose_net* net, b200pose_post* post, const unsigned
                         w, post->d_heat.p, post->d_paf.p, st);
     if (rc) return rc;
     return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h, w, thresh, st);
+}
+
+int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device,
+                                  int n, const int* src_hw, int dest_size, int factor, int mode, float thresh, int flip,
+                                  void* cuda_stream) {
+    if (!net || !post) return fail("null handle");
+    if (!net->finalized) return fail("net not finalized");
+    if (net->device != post->device) return fail("net and post live on different devices");
+    if (!images || !src_hw) return fail("infer_raw_ragged: null pointer");
+    if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
+    const int nimg = flip ? 2 * n : n;
+    if (nimg > kMaxRagged) return fail("ragged batch: %d images (at most %d)", nimg, kMaxRagged);
+    std::vector<RaggedFrame> tab(nimg);
+    std::vector<int> ext(2 * nimg);
+    long long raw = 0, max_bytes = 0;
+    int Hc = 0, Wc = 0;
+    for (int i = 0; i < n; ++i) {
+        RaggedFrame& f = tab[i];
+        f.src_h = src_hw[2 * i];
+        f.src_w = src_hw[2 * i + 1];
+        if (int rc = crop_check(1, f.src_h, f.src_w, dest_size, factor, &f.g)) return rc;
+        f.off = raw;
+        const long long b = (long long)f.src_h * f.src_w * 3;
+        raw += b;
+        if (b > max_bytes) max_bytes = b;
+        ext[2 * i] = f.g.pad_h;
+        ext[2 * i + 1] = f.g.pad_w;
+        if (f.g.pad_h > Hc) Hc = f.g.pad_h;
+        if (f.g.pad_w > Wc) Wc = f.g.pad_w;
+    }
+    for (int i = 0; i < n && flip; ++i) {      // mirrored raw frames follow the originals in the staging buffer
+        tab[n + i] = tab[i];
+        tab[n + i].off += raw;
+        ext[2 * (n + i)] = ext[2 * i];
+        ext[2 * (n + i) + 1] = ext[2 * i + 1];
+    }
+    if ((long)Hc * Wc > (1L << 28)) return fail("infer_raw_ragged: canvas too large");
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
+    const unsigned char* d_raw = images;
+    if (!input_on_device || flip) {
+        CU(net->raw_stage.ensure((size_t)raw * (flip ? 2 : 1)));
+        CU(cudaMemcpyAsync(net->raw_stage.p, images, (size_t)raw, input_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+        d_raw = net->raw_stage.p;
+    }
+    if (int rc = upload_frames(net, tab, st)) return rc;
+    if (flip) {       // the mirror reads the first n entries of the table (the originals)
+        cudaError_t e = tta_mirror_u8hwc_ragged(net->raw_stage.p, net->raw_stage.p + raw, net->d_frames.p, n, (long)max_bytes, st);
+        if (e != cudaSuccess) return fail("tta_mirror_u8hwc_ragged: %s", cudaGetErrorString(e));
+        ++g_launches;
+    }
+    if (int rc = place_ragged_frames(net, d_raw, nimg, Hc, Wc, st)) return rc;
+    if (int rc = upload_ext(net, ext, st)) return rc;
+    if (int rc = net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, Hc, Wc, mode, nullptr, 1, st, false, net->d_ext))
+        return rc;
+    const int h = Hc / 8, w = Wc / 8;
+    if (!flip) return post_run_dev(post, net->out_f32[11].p, net->out_f32[10].p, 0, n, h, w, thresh, st, net->d_ext);
+    const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
+    CU(post->d_heat.ensure(eh));
+    CU(post->d_paf.ensure(ep));
+    if (int rc = flip_merge_dev(net->out_f32[11].p, net->out_f32[11].p + eh, net->out_f32[10].p, net->out_f32[10].p + ep, 0, n,
+                                h, w, post->d_heat.p, post->d_paf.p, st, net->d_ext))
+        return rc;
+    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h, w, thresh, st, net->d_ext);
 }
 
 int b200pose_infer_raw_u8_multiscale(b200pose_net* net, b200pose_post* post, const unsigned char* images,

@@ -14,14 +14,18 @@ struct ConvF32Args {
     int out_cstride, out_ch_off;
     float* out_nchw;      // optional NCHW copy [n][cout][H][W]
     int n_img, H, W, cin, cout, ks, relu;
+    const int* ext;       // ragged batch (DESIGN.md §1): padded H, W per image at the network input, or null
+    int ext_shift;        // log2 of the network input size over H, W
 };
 
 // in: fp32 NCHW [N,3,H,W] (in_is_u8_hwc = 0), or uint8 HWC BGR [N,H,W,3] with the normalisation `in_is_u8_hwc`
 // (preprocess_core.h: 1 rtpose, 2 vgg, 3 inception, 4 ssd) fused into the load
 cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias,
                               __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo /*residual plane or null*/, int N, int H,
-                              int W, cudaStream_t s);
-cudaError_t u8hwc_to_f32nchw_launch(const unsigned char* in, float* out, int N, int H, int W, int mode, cudaStream_t s);
+                              int W, const int* ext /*ragged batch: padded H, W per image, or null*/, cudaStream_t s);
+// ext (ragged batch) or null: pixels outside image i's padded extent ext[2 i], ext[2 i + 1] become 0 (zero padding)
+cudaError_t u8hwc_to_f32nchw_launch(const unsigned char* in, float* out, int N, int H, int W, int mode, const int* ext,
+                                    cudaStream_t s);
 cudaError_t conv_f32_launch(const ConvF32Args& a, cudaStream_t s);
 cudaError_t maxpool_f32_launch(const float* in, float* out, int N, int H, int W, int C, cudaStream_t s);
 cudaError_t nchw_to_nhwc_f32_launch(const float* in, float* out, int N, int C, int H, int W, int out_cstride,

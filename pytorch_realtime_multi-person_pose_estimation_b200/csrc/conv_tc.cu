@@ -77,7 +77,8 @@ template <> struct Mma<32> {
 
 constexpr int kConsumerWarps = 8;
 
-template <int N, bool kChunk>
+// kRagged: a.ext is set (ragged batch); a separate instantiation so that uniform batches run the unmasked epilogue
+template <int N, bool kChunk, bool kRagged>
 __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B operands need 1024 B alignment.
@@ -264,13 +265,19 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             const int x = tc.x0 + wA;
             __nv_bfloat16* out_px[2] = {nullptr, nullptr};     // first channel of this n-tile at the lane's output pixel(s)
             int yo_px[2] = {0, 0}, xo = a.pool ? x >> 1 : x;
-            bool wr[2];
+            bool wr[2], inside[2];
+            int eh = Ho, ew = Wo;                              // the image's extent at the output resolution
+            if (kRagged) {
+                eh = __ldg(a.ext + 2 * tc.n) >> a.ext_shift;
+                ew = __ldg(a.ext + 2 * tc.n + 1) >> a.ext_shift;
+            }
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
                 const int y = tc.y0 + hA + hh;
                 // pooled: the lane with even w holds the 2x2 window (both rows) after the shuffle
                 wr[hh] = (y < a.H) && (x < a.W) && (a.pool ? (hh == 0 && !(lane & 4)) : true);
                 yo_px[hh] = a.pool ? y >> 1 : y;
+                inside[hh] = !kRagged || (yo_px[hh] < eh && xo < ew);
                 if (a.out != nullptr)
                     out_px[hh] = a.out + (static_cast<size_t>(tc.n * Ho + yo_px[hh]) * Wo + xo) * a.out_cstride +
                                  a.out_ch_off[tc.g] + ch_tile + cq;
@@ -293,7 +300,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
                     if (!wr[hh]) continue;
-                    const float lo = v[2 * hh], hi = v[2 * hh + 1];
+                    const float lo = inside[hh] ? v[2 * hh] : 0.f, hi = inside[hh] ? v[2 * hh + 1] : 0.f;
                     if (out_px[hh] != nullptr && 8 * j < store_ch) {
                         *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pack_bf16x2(lo, hi);
                         if (a.out_lo != nullptr) {      // split mode: residual plane v - bf16(v)
@@ -315,9 +322,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     if (threadIdx.x == 0) B2P_TL(9);
 }
 
-template <int N, bool kChunk>
+template <int N, bool kChunk, bool kRagged>
 __global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_kernel(const __grid_constant__ ConvTcArgs a) {
-    conv_tc_body<N, kChunk>(a);
+    conv_tc_body<N, kChunk, kRagged>(a);
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -392,10 +399,10 @@ namespace {
 // Programmatic dependent launch (a.pdl): the next layer's CTAs may start - barrier init, descriptor prefetch, weight loads -
 // while this layer's last CTAs drain; they wait (griddepcontrol.wait) before touching activations.  Used by the SMALL-batch
 // plans only, where the fixed cost per launch is most of a layer.
-template <int N, bool kChunk>
-cudaError_t launch(int grid, cudaStream_t stream, const ConvTcArgs& a) {
+template <int N, bool kChunk, bool kRagged>
+cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
     static DynSmemOptIn optin;   // per device: a second net on another GPU of the same process needs its own opt-in
-    cudaError_t e = optin.ensure(conv_tc_kernel<N, kChunk>, kConvTcSmemBytes);
+    cudaError_t e = optin.ensure(conv_tc_kernel<N, kChunk, kRagged>, kConvTcSmemBytes);
     if (e != cudaSuccess) return e;
     if (a.pdl) {
         cudaLaunchConfig_t cfg = {};
@@ -408,10 +415,15 @@ cudaError_t launch(int grid, cudaStream_t stream, const ConvTcArgs& a) {
         attr[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        return cudaLaunchKernelEx(&cfg, conv_tc_kernel<N, kChunk>, a);
+        return cudaLaunchKernelEx(&cfg, conv_tc_kernel<N, kChunk, kRagged>, a);
     }
-    conv_tc_kernel<N, kChunk><<<grid, kConvTcThreads, kConvTcSmemBytes, stream>>>(a);
+    conv_tc_kernel<N, kChunk, kRagged><<<grid, kConvTcThreads, kConvTcSmemBytes, stream>>>(a);
     return cudaGetLastError();
+}
+
+template <int N, bool kChunk>
+cudaError_t launch(int grid, cudaStream_t stream, const ConvTcArgs& a) {
+    return a.ext != nullptr ? launch_k<N, kChunk, true>(grid, stream, a) : launch_k<N, kChunk, false>(grid, stream, a);
 }
 }  // namespace
 

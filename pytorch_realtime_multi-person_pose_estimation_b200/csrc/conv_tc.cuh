@@ -62,6 +62,10 @@ struct ConvTcArgs {
     CUtensorMap tm_in;        // 4D (C, W, H, N) bf16, box (64, 16, 16+ks-1, 1), SWIZZLE_128B
     CUtensorMap tm_w;         // 3D (cin_pad, groups*n_tiles*n_tile, 2*taps) bf16 [hi taps | lo taps], box (64, n_tile, tps)
     CUtensorMap tm_in_lo;     // residual plane of the input (split mode)
+    // ---- ragged batches (DESIGN.md §1): ext[2 i], ext[2 i + 1] = padded H, W of image i at the network input; every
+    // output element of image i outside (ext >> ext_shift) is stored as +0.  null: every image fills the canvas.
+    const int* ext;
+    int ext_shift;            // log2 of the network input size over this launch's OUTPUT size (pooling included)
 };
 
 // Builds the tensor maps. `in` (and `in_lo` in split mode): NHWC buffers with `in_cstride` channels per pixel.

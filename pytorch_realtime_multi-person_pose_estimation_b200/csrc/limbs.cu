@@ -164,8 +164,9 @@ struct PlanePaf {          // the limb's two PAF planes in shared memory: channe
     __device__ __forceinline__ float at(int c, int y, int x) const { return pl[c * hw + (y >> 3) * lw + (x >> 3)]; }
 };
 
-__global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers pb, PafView paf0, long p_img, int h_up,
-                                                                   int lw, int lh, int paf_in_smem, int n_limbs) {
+__global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers pb, PafView paf0, long p_img, int h_up0,
+                                                                   int lw, int lh, int paf_in_smem, int n_limbs,
+                                                                   const int* __restrict__ ext) {
     extern __shared__ float s_planes[];
     __shared__ int s_item;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -198,6 +199,7 @@ __global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers p
         const int chunk = item - pl.work0;
         const int pa = c_lparts[limb][0], pbp = c_lparts[limb][1];
         const int c1 = c_lpaf[limb][0], c2 = c_lpaf[limb][1];
+        const int h_up = ext ? __ldg(ext + 2 * img) : h_up0;     // ragged batch: the image's own padded height
         PafView paf = paf0;
         paf.base += img * p_img;
         if (paf_in_smem && staged != li) {
@@ -808,7 +810,7 @@ __global__ void __launch_bounds__(kGreedyThreads) limb_greedy_kernel(PostBuffers
     } while (0)
 
 cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long p_img, long p_ch, long p_y, long p_x,
-                       int shift, int h_up, int lw, int lh, cudaStream_t s) {
+                       int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext) {
     if (batch > pb.batch_cap) return cudaErrorInvalidValue;
     if (pb.cand_smem_cap != kS) return cudaErrorInvalidValue;
     PafView pv{paf, p_ch, p_y, p_x, shift};
@@ -825,7 +827,7 @@ cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long 
     int dev = 0, sms = 132;
     B2P_TRY(cudaGetDevice(&dev));
     B2P_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb);
+    limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb, ext);
     B2P_TRY(cudaGetLastError());
     limb_gather_kernel<<<dim3(batch, kNumLimb), kGatherThreads, 0, s>>>(pb);
     B2P_TRY(cudaGetLastError());

@@ -100,14 +100,17 @@ __device__ __forceinline__ void refine_interior_slots(const float* plane, int w,
 }
 
 __global__ void __launch_bounds__(kPeakThreads, 512 / kPeakThreads) peaks_kernel(PostBuffers pb, const float* __restrict__ heat, long h_img,
-                                                             long h_ch, long h_y, long h_x, int h, int w, float thresh) {
+                                                             long h_ch, long h_y, long h_x, int h_max, int w_max, float thresh,
+                                                             const int* __restrict__ ext) {
     extern __shared__ float sm_f[];
     float* plane = sm_f;                       // [h*w]
-    float* hor_all = sm_f + h * w;             // [8 warps][5][40]
+    float* hor_all = sm_f + h_max * w_max;     // [8 warps][5][40]
     __shared__ int warp_cnt[kPeakThreads / 32];
     __shared__ int s_base, s_ni, s_nb;
     __shared__ uint16_t s_list[2048];          // peak indices: interior ones from the front, border ones from the back
     const int part = blockIdx.x, img = blockIdx.y;
+    // ragged batch: the image's own h x w (its NMS borders are its own edges), read at the canvas strides
+    const int h = ext ? __ldg(ext + 2 * img) >> 3 : h_max, w = ext ? __ldg(ext + 2 * img + 1) >> 3 : w_max;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int hw = h * w;
     const float* src = heat + img * h_img + part * h_ch;
@@ -449,14 +452,14 @@ void post_free(PostBuffers& pb) {
 }
 
 cudaError_t post_peaks(const PostBuffers& pb, int batch, const float* heat, long h_img, long h_ch, long h_y, long h_x,
-                       int h, int w, float thresh, cudaStream_t s) {
+                       int h, int w, float thresh, cudaStream_t s, const int* ext) {
     if (batch > pb.batch_cap) return cudaErrorInvalidValue;
     const size_t smem = ((size_t)h * w + (kPeakThreads / 32) * 5 * kHorStride) * sizeof(float);
     if (smem > 200 * 1024) return cudaErrorInvalidValue;
     static DynSmemOptIn optin;
     B2P_TRY(optin.ensure(peaks_kernel, smem));
     B2P_TRY(cudaMemsetAsync(pb.status, 0, batch * sizeof(int), s));
-    peaks_kernel<<<dim3(kNumPart, batch), kPeakThreads, smem, s>>>(pb, heat, h_img, h_ch, h_y, h_x, h, w, thresh);
+    peaks_kernel<<<dim3(kNumPart, batch), kPeakThreads, smem, s>>>(pb, heat, h_img, h_ch, h_y, h_x, h, w, thresh, ext);
     return cudaGetLastError();
 }
 

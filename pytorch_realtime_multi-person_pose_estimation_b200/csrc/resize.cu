@@ -9,6 +9,28 @@ namespace {
 
 constexpr int kThreads = 256;
 
+// The three bytes of destination pixel (y, x); zero outside the resized area (bottom / right padding).
+__device__ __forceinline__ void crop_pixel(const unsigned char* src, int src_h, int src_w, const CropGeom& g, int y, int x,
+                                           unsigned char* dst) {
+    unsigned char v0 = 0, v1 = 0, v2 = 0;
+    if (y < g.res_h && x < g.res_w) {
+        const long stride = (long)src_w * 3;
+        if (g.area2) {
+            v0 = rs_area2_px(src, src_h, src_w, stride, 3, 0, x, y);
+            v1 = rs_area2_px(src, src_h, src_w, stride, 3, 1, x, y);
+            v2 = rs_area2_px(src, src_h, src_w, stride, 3, 2, x, y);
+        } else {
+            const LinCoef cx = rs_coef_x(x, src_w, g.step), cy = rs_coef_y(y, src_h, g.step);
+            v0 = rs_linear_px(src, stride, 3, 0, cx, cy);
+            v1 = rs_linear_px(src, stride, 3, 1, cx, cy);
+            v2 = rs_linear_px(src, stride, 3, 2, cx, cy);
+        }
+    }
+    dst[0] = v0;
+    dst[1] = v1;
+    dst[2] = v2;
+}
+
 __global__ void __launch_bounds__(kThreads) crop_with_factor_kernel(const unsigned char* __restrict__ in,
                                                                     unsigned char* __restrict__ out, int src_h, int src_w,
                                                                     CropGeom g) {
@@ -18,23 +40,34 @@ __global__ void __launch_bounds__(kThreads) crop_with_factor_kernel(const unsign
     unsigned char* dst = out + img * dst_px * 3;
     for (long p = blockIdx.x * (long)kThreads + threadIdx.x; p < dst_px; p += (long)gridDim.x * kThreads) {
         const int y = (int)(p / g.pad_w), x = (int)(p - (long)y * g.pad_w);
-        unsigned char v0 = 0, v1 = 0, v2 = 0;
-        if (y < g.res_h && x < g.res_w) {
-            const long stride = (long)src_w * 3;
-            if (g.area2) {
-                v0 = rs_area2_px(src, src_h, src_w, stride, 3, 0, x, y);
-                v1 = rs_area2_px(src, src_h, src_w, stride, 3, 1, x, y);
-                v2 = rs_area2_px(src, src_h, src_w, stride, 3, 2, x, y);
-            } else {
-                const LinCoef cx = rs_coef_x(x, src_w, g.step), cy = rs_coef_y(y, src_h, g.step);
-                v0 = rs_linear_px(src, stride, 3, 0, cx, cy);
-                v1 = rs_linear_px(src, stride, 3, 1, cx, cy);
-                v2 = rs_linear_px(src, stride, 3, 2, cx, cy);
-            }
+        crop_pixel(src, src_h, src_w, g, y, x, dst + 3 * p);
+    }
+}
+
+// Ragged batch: frame `img` (source f.src_h x f.src_w at in + f.off) is cropped to its own f.g.pad_h x f.g.pad_w in the
+// top-left corner of its Hc x Wc canvas slot; the rest of the slot is zero.  f.g.pad_h == 0: the frame is already
+// cropped (f.src_h x f.src_w) and is copied as it is.
+__global__ void __launch_bounds__(kThreads) ragged_frames_kernel(const unsigned char* __restrict__ in,
+                                                                 const RaggedFrame* __restrict__ frames,
+                                                                 unsigned char* __restrict__ out, int Hc, int Wc) {
+    const int img = blockIdx.y;
+    const RaggedFrame f = frames[img];
+    const long dst_px = (long)Hc * Wc;
+    const unsigned char* src = in + f.off;
+    unsigned char* dst = out + img * dst_px * 3;
+    for (long p = blockIdx.x * (long)kThreads + threadIdx.x; p < dst_px; p += (long)gridDim.x * kThreads) {
+        const int y = (int)(p / Wc), x = (int)(p - (long)y * Wc);
+        if (f.g.pad_h == 0) {
+            const bool in_frame = y < f.src_h && x < f.src_w;
+            const unsigned char* s = src + ((long)y * f.src_w + x) * 3;
+            dst[3 * p + 0] = in_frame ? s[0] : 0;
+            dst[3 * p + 1] = in_frame ? s[1] : 0;
+            dst[3 * p + 2] = in_frame ? s[2] : 0;
+        } else if (y < f.g.pad_h && x < f.g.pad_w) {
+            crop_pixel(src, f.src_h, f.src_w, f.g, y, x, dst + 3 * p);
+        } else {
+            dst[3 * p + 0] = dst[3 * p + 1] = dst[3 * p + 2] = 0;
         }
-        dst[3 * p + 0] = v0;
-        dst[3 * p + 1] = v1;
-        dst[3 * p + 2] = v2;
     }
 }
 
@@ -77,6 +110,18 @@ cudaError_t crop_with_factor_launch(const unsigned char* in, unsigned char* out,
     if (bx > cap) bx = cap;
     if (bx < 1) bx = 1;
     crop_with_factor_kernel<<<dim3((unsigned)bx, (unsigned)n), kThreads, 0, s>>>(in, out, src_h, src_w, g);
+    return cudaGetLastError();
+}
+
+cudaError_t ragged_frames_launch(const unsigned char* in, const RaggedFrame* frames, int n, unsigned char* out, int Hc,
+                                 int Wc, cudaStream_t s) {
+    if (n < 1 || n > 65535 || Hc < 1 || Wc < 1) return cudaErrorInvalidValue;
+    const long px = (long)Hc * Wc;
+    long bx = (px + kThreads - 1) / kThreads;
+    const long cap = (132L * 8 + n - 1) / n;
+    if (bx > cap) bx = cap;
+    if (bx < 1) bx = 1;
+    ragged_frames_kernel<<<dim3((unsigned)bx, (unsigned)n), kThreads, 0, s>>>(in, frames, out, Hc, Wc);
     return cudaGetLastError();
 }
 

@@ -17,4 +17,16 @@ cudaError_t crop_with_factor_launch(const unsigned char* in, unsigned char* out,
 cudaError_t resize_cubic_accum_launch(const float* src, float* dst, long planes, int src_h, int src_w, int dst_h,
                                       int dst_w, int first, float divide_by, cudaStream_t s);
 
+// One frame of a ragged batch (DESIGN.md §1): uint8 HWC source at byte offset `off`, and its crop_with_factor geometry
+// (g.pad_h == 0: the source is an already cropped network input, copied unchanged).
+struct RaggedFrame {
+    long long off;
+    int src_h, src_w;
+    CropGeom g;
+};
+
+// frames [n] (device) -> out [n, Hc, Wc, 3]: frame i cropped (or copied) into the top-left corner of slot i, zeros elsewhere
+cudaError_t ragged_frames_launch(const unsigned char* in, const RaggedFrame* frames, int n, unsigned char* out, int Hc,
+                                 int Wc, cudaStream_t s);
+
 }  // namespace b2p

@@ -9,6 +9,35 @@ import numpy as np
 
 from . import _native as nat
 
+# A ragged batch runs on the canvas of its largest frame, and every layer pays for the whole canvas (DESIGN.md 2.8):
+# n * Hc * Wc may exceed the sum of the frames' own H_i * W_i by at most this factor.
+RAGGED_WASTE = 1.125
+
+
+def plan_ragged_batches(shapes, batch_cap, waste=RAGGED_WASTE):
+    """Groups frames of padded sizes shapes[i] = (H_i, W_i) into ragged batches of at most batch_cap frames.
+    Frames are ordered by orientation (landscape and square first, then portrait) and by size; a batch is closed when the
+    next frame would make n * Hc * Wc exceed `waste` times the sum of H_i * W_i, or the orientation changes.  Returns
+    lists of frame indices."""
+    order = sorted(range(len(shapes)), key=lambda i: (shapes[i][0] > shapes[i][1], shapes[i][0], shapes[i][1], i))
+    batches, cur, hc, wc, area = [], [], 0, 0, 0
+    for i in order:
+        h, w = shapes[i]
+        nh, nw, na = max(hc, h), max(wc, w), area + h * w
+        if cur and (len(cur) == batch_cap or (shapes[cur[0]][0] > shapes[cur[0]][1]) != (h > w)
+                    or (len(cur) + 1) * nh * nw > waste * na):
+            batches.append(cur)
+            cur, nh, nw, na = [], h, w, h * w
+        cur.append(i)
+        hc, wc, area = nh, nw, na
+    if cur:
+        batches.append(cur)
+    return batches
+
+
+def _at(v, i):
+    return v[i] if isinstance(v, (list, tuple)) else v
+
 
 class NativeNet:
     """Owns a b200pose_net handle on one CUDA device."""
@@ -46,6 +75,15 @@ class NativeNet:
         nat.check(nat.lib().b200pose_net_forward_u8(self._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H, W, mode,
                                                     arr, int(out_on_device), ctypes.c_void_p(stream)),
                   "b200pose_net_forward_u8")
+
+    def forward_ragged_u8_ptr(self, in_ptr, in_on_device, shapes, mode, out_ptrs, out_on_device, stream):
+        """Ragged batch: uint8 HWC BGR frames of the padded sizes shapes[i] = (H_i, W_i), packed back to back; the
+        12 maps come out at the canvas size [n, C, max H_i / 8, max W_i / 8], +0 outside each frame."""
+        hw = (ctypes.c_int * (2 * len(shapes)))(*[int(v) for s in shapes for v in s])
+        arr = (ctypes.c_void_p * 12)(*[ctypes.c_void_p(p) if p else None for p in out_ptrs])
+        nat.check(nat.lib().b200pose_net_forward_ragged_u8(self._h, ctypes.c_void_p(in_ptr), int(in_on_device), len(shapes),
+                                                           hw, mode, arr, int(out_on_device), ctypes.c_void_p(stream)),
+                  "b200pose_net_forward_ragged_u8")
 
     def crop_with_factor(self, images, dest_size=368, factor=8):
         """Device-side crop_with_factor (im_transform.py:119-134) of uint8 BGR frames of one size: [n,h,w,3] or [h,w,3]
@@ -203,7 +241,8 @@ class PoseEngine:
 
     def _remember(self, n, H, W):
         """Shape of the run just submitted, kept per ticket (two runs may be in flight with different batch sizes or
-        frame shapes: fetch(ticket=i) must read run i with run i's n and normalise by run i's W / H)."""
+        frame shapes: fetch(ticket=i) must read run i with run i's n and normalise by run i's W / H).  H, W: one size,
+        or per frame lists for a ragged batch."""
         t = self.post.last_ticket()
         if self.__dict__.get("_shapes") is None:
             self._shapes = {}
@@ -279,6 +318,19 @@ class PoseEngine:
         _, _, (ph, pw) = nat.crop_geometry(src_h, src_w, dest_size, factor)
         return self._remember(n, ph, pw)
 
+    def infer_raw_ragged_async_u8(self, in_ptr, in_on_device, src_shapes, dest_size=368, factor=8, thresh=0.1, flip=False,
+                                  stream=0):
+        """Raw uint8 BGR frames of different sizes src_shapes[i] = (h_i, w_i), packed back to back, as one ragged batch:
+        each frame is cropped to its own padded size and person coordinates refer to that padded frame."""
+        n = len(src_shapes)
+        hw = (ctypes.c_int * (2 * n))(*[int(v) for s in src_shapes for v in s])
+        nat.check(nat.lib().b200pose_infer_raw_u8_ragged(self.net._h, self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device),
+                                                         n, hw, int(dest_size), int(factor), self.mode,
+                                                         ctypes.c_float(thresh), int(bool(flip)), ctypes.c_void_p(stream)),
+                  "b200pose_infer_raw_u8_ragged")
+        pads = [nat.crop_geometry(h, w, dest_size, factor)[2] for h, w in src_shapes]
+        return self._remember(n, [p[0] for p in pads], [p[1] for p in pads])
+
     def infer_raw_multiscale_async_u8(self, in_ptr, in_on_device, n, src_h, src_w, scales, base_size=368, factor=8,
                                       thresh=0.1, flip=False, stream=0):
         """Multi-scale (+ flip) test-time averaging of raw uint8 BGR frames of one size (BASELINE.json configs[4]):
@@ -299,28 +351,41 @@ class PoseEngine:
         return self.infer_images(images, dest_size, factor, thresh, flip, scales, _arrays=True)
 
     def infer_images(self, images, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, _arrays=False):
-        """images: a list of raw uint8 BGR frames of arbitrary (mixed) sizes, as cv2.imread returns them.  Frames are
-        bucketed by shape (one launch sequence per bucket, at most batch_cap frames each); returns per-image human lists
-        in input order, coordinates normalised to the padded frame like paf_to_pose_cpp's.
-        scales: e.g. (0.5, 1.0, 1.5, 2.0) for multi-scale test-time averaging around dest_size."""
-        buckets = {}
-        for i, im in enumerate(images):
+        """images: a list of raw uint8 BGR frames of arbitrary (mixed) sizes, as cv2.imread returns them.  Returns per-image
+        human lists in input order, coordinates normalised to the padded frame like paf_to_pose_cpp's.
+        Single scale: the frames run as ragged batches of at most batch_cap frames of different sizes (plan_ragged_batches;
+        a batch of one source size takes the uniform entry point).  scales: e.g. (0.5, 1.0, 1.5, 2.0) for multi-scale
+        test-time averaging around dest_size, one launch sequence per source shape."""
+        for im in images:
             if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
                 raise nat.B200PoseError("infer_images: expected uint8 [h,w,3] frames")
-            buckets.setdefault(im.shape[:2], []).append(i)
+        if scales is None:
+            pads = [nat.crop_geometry(im.shape[0], im.shape[1], dest_size, factor)[2] for im in images]
+            groups = plan_ragged_batches(pads, self.post.batch_cap)
+        else:
+            buckets = {}
+            for i, im in enumerate(images):
+                buckets.setdefault(im.shape[:2], []).append(i)
+            groups = [idx[k:k + self.post.batch_cap] for idx in buckets.values()
+                      for k in range(0, len(idx), self.post.batch_cap)]
         out = [None] * len(images)
-        for (sh, sw), idx in buckets.items():
-            for k in range(0, len(idx), self.post.batch_cap):
-                part = idx[k:k + self.post.batch_cap]
+        for part in groups:
+            shapes = [images[i].shape[:2] for i in part]
+            if scales is not None or len(set(shapes)) == 1:
                 batch = np.ascontiguousarray(np.stack([images[i] for i in part]))
                 self._keep = batch
+                sh, sw = shapes[0]
                 if scales is None:
                     self.infer_raw_async_u8(batch.ctypes.data, False, len(part), sh, sw, dest_size, factor, thresh, flip)
                 else:
                     self.infer_raw_multiscale_async_u8(batch.ctypes.data, False, len(part), sh, sw, scales, dest_size,
                                                        factor, thresh, flip)
-                for i, humans in zip(part, self.fetch_arrays() if _arrays else self.fetch()):
-                    out[i] = humans.copy() if _arrays else humans
+            else:
+                batch = np.concatenate([np.ascontiguousarray(images[i]).ravel() for i in part])
+                self._keep = batch
+                self.infer_raw_ragged_async_u8(batch.ctypes.data, False, shapes, dest_size, factor, thresh, flip)
+            for i, humans in zip(part, self.fetch_arrays() if _arrays else self.fetch()):
+                out[i] = humans.copy() if _arrays else humans
         return out
 
     def fetch(self, check=True, ticket=None):
@@ -332,7 +397,7 @@ class PoseEngine:
             self.post.select(ticket)
         if check:
             self.post.check_status(n)
-        return [humans_to_dicts(self.post.humans(i), W, H) for i in range(n)]
+        return [humans_to_dicts(self.post.humans(i), _at(W, i), _at(H, i)) for i in range(n)]
 
     def fetch_arrays(self, check=True, ticket=None):
         """Like fetch() but without building Python objects: per image a float32 array [k, 73] with rows

@@ -109,8 +109,8 @@ EVAL_BATCH = 32      # images per device batch of the batched evaluation loop
 
 
 def _humans_batched(core, images, preprocess):
-    """images (raw BGR frames of mixed sizes) -> per image (humans, heat-map shape): one fused device pass per shape
-    bucket (crop_with_factor, normalisation, network, NMS, PAF matching, assembly - nothing but the person rows comes back)
+    """images (raw BGR frames of mixed sizes) -> per image (humans, heat-map shape): one fused device pass per ragged
+    batch of frames of different sizes (crop_with_factor, normalisation, network, NMS, PAF matching, assembly - nothing but the person rows comes back)
     instead of get_outputs + paf_to_pose_cpp per image.  Same kernels, same arithmetic: identical persons."""
     from .. import _native as nat
     from ..lib.utils.paf_to_pose import humans_from_rows
