@@ -1,15 +1,18 @@
 // C-ABI of libb200pose.so (include/b200pose.h): network object, post-processing object, fused inference and the
 // legacy pafprocess surface.  Host-side runtime only; the kernels live in conv_tc.cu, conv_misc.cu, postprocess.cu.
+#include <array>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <list>
 #include <map>
 #include <set>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/b200pose.h"
@@ -40,6 +43,13 @@ int fail(const char* fmt, ...) {
         cudaError_t e_ = (x);                                                                       \
         if (e_ != cudaSuccess) return fail("%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
     } while (0)
+
+// Counts the launches of a kernel wrapper that returned e.
+int launched(cudaError_t e, const char* what, int launches = 1) {
+    if (e != cudaSuccess) return fail("%s: %s", what, cudaGetErrorString(e));
+    g_launches += launches;
+    return 0;
+}
 
 // ---------------------------------------------------------------- layer table (rtpose_vgg.py:69-127)
 struct ConvSpec { int cin, cout, ks; };
@@ -124,18 +134,78 @@ struct TcLayer {            // one grouped tensor-core launch
     float* bias = nullptr;        // [groups*n_tiles*n_tile]
 };
 
-// What ConvTcArgs does not keep about a launch (its tensor maps hold the input address, not the buffer): recorded per
-// launch by add_plan for the test hooks (b200pose_net_debug_launch).
-struct LaunchInfo {
-    int in_buf, in_cstride, out_buf;   // activation buffer ids (0 .. 13 = t1 .. br512, see kActC), -1 = none
-    int f32[2];                        // index of the fp32 stage map written per group, -1 = none
-};
-
-// Activation buffers t1 .. br512 (buffer ids 0 .. 13 of the test hooks): channels per pixel and spatial divisor.
-constexpr int kNumAct = 14;
+// Activation buffers (the buffer ids of the test hooks): channels per pixel and spatial divisor.
+enum Act { T1, T2, T3, T4, T5A, T5B, T6, T7, T8, T9, CAT, BRA, BRB, BR512, kNumAct };
 constexpr int kMaxRagged = 1024;      // images of one ragged forward (flip: 2 per frame)
 const int kActC[kNumAct] = {64, 64, 128, 128, 256, 256, 256, 512, 512, 256, 192, 256, 256, 1024};
 const int kActDiv[kNumAct] = {1, 2, 2, 4, 4, 4, 8, 8, 8, 8, 8, 8, 8, 8};
+
+// One tensor-core launch of a bf16 plan: the buffers it reads and writes and its channel slices of them.  A launch
+// runs at the resolution of its input buffer.
+struct Wiring {
+    int in, in_base, in_group_stride;   // input buffer, first channel of group 0, channel offset of group 1
+    int out, out_off[2], store[2];      // output buffer; per group: first channel, channels stored per n-tile
+    bool maps;                          // stage head: also writes the stage's fp32 PAF (group 0) and heatmap (group 1)
+};
+// trunk (conv1_1 runs on CUDA cores before the plan)
+const Wiring kTrunkWiring[11] = {
+    // in  base stride out   out_off   store
+    {T1,   0, 0,      T2,   {0, 0},   {64, 0}},      // conv1_2 + pool
+    {T2,   0, 0,      T3,   {0, 0},   {128, 0}},     // conv2_1
+    {T3,   0, 0,      T4,   {0, 0},   {128, 0}},     // conv2_2 + pool
+    {T4,   0, 0,      T5A,  {0, 0},   {128, 0}},     // conv3_1
+    {T5A,  0, 0,      T5B,  {0, 0},   {128, 0}},     // conv3_2
+    {T5B,  0, 0,      T5A,  {0, 0},   {128, 0}},     // conv3_3
+    {T5A,  0, 0,      T6,   {0, 0},   {128, 0}},     // conv3_4 + pool
+    {T6,   0, 0,      T7,   {0, 0},   {128, 0}},     // conv4_1
+    {T7,   0, 0,      T8,   {0, 0},   {128, 0}},     // conv4_2
+    {T8,   0, 0,      T9,   {0, 0},   {128, 0}},     // conv4_3_CPM
+    {T9,   0, 0,      CAT,  {64, 0},  {128, 0}},     // conv4_4_CPM -> feature slice of the concat buffer
+};
+// Stages: both branches run as one two-group launch (group 0 = PAF, group 1 = heatmap); each group reads and writes
+// its own half of bra / brb / br512, and the head writes the PAF and heatmap slices of the concat buffer (DESIGN §1).
+const Wiring kStage1Wiring[5] = {
+    {CAT,   64, 0,    BRA,   {0, 128}, {128, 128}},       // the features only
+    {BRA,   0,  128,  BRB,   {0, 128}, {128, 128}},
+    {BRB,   0,  128,  BRA,   {0, 128}, {128, 128}},
+    {BRA,   0,  128,  BR512, {0, 512}, {128, 128}},
+    {BR512, 0,  512,  CAT,   {0, 40},  {40, 24}, true},
+};
+const Wiring kStageWiring[7] = {     // stages 2 .. 6
+    {CAT,   0,  0,    BRA,   {0, 128}, {128, 128}},       // all 192 channels
+    {BRA,   0,  128,  BRB,   {0, 128}, {128, 128}},
+    {BRB,   0,  128,  BRA,   {0, 128}, {128, 128}},
+    {BRA,   0,  128,  BRB,   {0, 128}, {128, 128}},
+    {BRB,   0,  128,  BRA,   {0, 128}, {128, 128}},
+    {BRA,   0,  128,  BRB,   {0, 128}, {128, 128}},
+    {BRB,   0,  128,  CAT,   {0, 40},  {40, 24}, true},
+};
+
+struct PlanLaunch {
+    ConvTcArgs a;
+    double flops;          // algorithmic (unpadded) FLOPs
+    int in, out;           // activation buffers (Act); ConvTcArgs keeps only tensor maps of the input
+    int f32[2];            // fp32 stage map written per group, -1 = none
+};
+
+// Device addresses a plan's tensor maps and arguments point into: activation buffers, residual planes, stage maps.
+using PlanBuffers = std::array<const void*, 2 * kNumAct + 12>;
+
+// The launch list of one (n, H, W, mode) key, valid while `buffers` are still the net's.
+struct Plan {
+    int n, H, W, mode;
+    bool split;            // bf16x3
+    std::vector<PlanLaunch> launches;
+    PlanBuffers buffers;
+};
+
+// What the last successful forward ran; b200pose_net_last_maps, _profile and the _debug_* hooks read it.
+struct LastForward {
+    int n = 0, H = 0, W = 0, mode = -1;
+    const void* in = nullptr;    // device input
+    int in_u8 = 0;               // normalisation of a uint8 input fused into conv1_1 (0: fp32 input)
+    const int* ext = nullptr;    // extents table of a ragged forward, null: uniform
+};
 
 }  // namespace
 
@@ -148,56 +218,23 @@ struct b200pose_net {
     float* d_b[kNumConvs] = {};
     // tensor-core layers: trunk 1..11 -> tc[0..10]; stage 1: tc[11..15]; stage t>=2: tc[16 + (t-2)*7 + li]
     std::vector<TcLayer> tc;
-    // ---- plan (depends on n, H, W)
-    int pn = 0, pH = 0, pW = 0, pmode = -1;
-    std::vector<ConvTcArgs> plan;
-    std::vector<double> plan_flops;   // algorithmic FLOPs per launch of `plan`
-    std::vector<LaunchInfo> plan_info;   // buffers of each launch of `plan` (test hooks)
-    bool plan_split = false;          // the plan was built for the split-precision (bf16x3) mode
-    // Plans of other (n, H, W, mode) keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not
-    // re-encode 51 tensor maps and synchronise the stream.  An entry is valid while the activation buffers it points
-    // into have not been reallocated.  B200POSE_PLAN_CACHE=0 (read when the net is created) turns it off.
-    struct PlanEntry {
-        int n, H, W, mode;
-        bool split;
-        std::vector<ConvTcArgs> plan;
-        std::vector<double> flops;
-        std::vector<LaunchInfo> info;
-        std::vector<const void*> buffers;
-    };
-    bool plan_cache_on = true;
-    bool conv_pdl = true;             // programmatic dependent launch between the layers of small-batch plans (B200POSE_CONV_PDL=0: never)
+    // Plans of the last 32 keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not re-encode
+    // 51 tensor maps and synchronise the stream.  `plan` is the one the last bf16 / bf16x3 forward selected.
+    std::list<Plan> plans;
+    const Plan* plan = nullptr;
     // The 52 launches of a forward pass are captured at the second use of a (shape, mode, input pointer) into a CUDA graph and replayed
     // (B200POSE_GRAPH=0: plain launches).  Graphs embed the tensor maps, i.e. buffer addresses: every plan build drops them.
     // Capture needs a real stream: calls on the legacy default stream (0) launch directly.
-    struct GraphKey {
-        int n, H, W, mode, in_u8, ragged;
-        const void* in;
-        bool operator<(const GraphKey& o) const {
-            if (n != o.n) return n < o.n;
-            if (H != o.H) return H < o.H;
-            if (W != o.W) return W < o.W;
-            if (mode != o.mode) return mode < o.mode;
-            if (in_u8 != o.in_u8) return in_u8 < o.in_u8;
-            if (ragged != o.ragged) return ragged < o.ragged;
-            return in < o.in;
-        }
-    };
+    using GraphKey = std::tuple<int, int, int, int, int, bool, const void*>;   // n, H, W, mode, in_u8, ragged, input
     bool use_graph = true;
     std::map<GraphKey, cudaGraphExec_t> graphs;
     std::set<GraphKey> graph_seen;    // a key is captured at its SECOND use: callers that pass a fresh pointer every time never pay a capture
-    int kn = 0, kH = 0, kW = 0, kmode = -1;      // key of the plan currently held in `plan`
-    std::vector<PlanEntry> plan_cache;
-    DevBuf<__nv_bfloat16> t1, t2, t3, t4, t5a, t5b, t6, t7, t8, t9, cat, bra, brb, br512;
-    // residual ("lo") planes of the same buffers, split-precision mode only
-    DevBuf<__nv_bfloat16> l1, l2, l3, l4, l5a, l5b, l6, l7, l8, l9, lcat, lbra, lbrb, lbr512;
-    std::map<const void*, __nv_bfloat16*> lo_of;
+    // bf16 activation buffers by Act id, and their residual ("lo") planes (split-precision mode only)
+    DevBuf<__nv_bfloat16> act[kNumAct], act_lo[kNumAct];
     DevBuf<float> in_stage, out_f32[12];
     // fp32 parity buffers
     DevBuf<float> f_a, f_b, f_cat, f_x, f_y, f_in, f_u8;
-    cudaStream_t own_stream = nullptr;
-    const void* last_in = nullptr;    // device pointer of the last forward's input (profiling hook)
-    int last_in_u8 = 0;
+    LastForward last;
     DevBuf<unsigned char> in_stage_u8;
     int preprocess = 1;                // normalisation fused into the uint8 entry points (preprocess_core.h; 1 = rtpose)
     DevBuf<unsigned char> raw_stage;   // raw (un-resized) frames of b200pose_*crop* / b200pose_infer_raw_u8
@@ -205,7 +242,6 @@ struct b200pose_net {
     // Allocated once for kMaxRagged images and never moved, so that plans and captured graphs stay valid across mixes;
     // rewritten on the stream before each ragged forward.
     int* d_ext = nullptr;
-    const int* last_ext = nullptr;     // extents of the last forward (null: uniform), for the test hooks
     DevBuf<RaggedFrame> d_frames;      // per-frame source geometry of the last ragged crop
 };
 
@@ -232,9 +268,7 @@ struct b200pose_post {
     // Peaks / limbs / assembly of run i all run on the second stream from a private copy of the maps (15 MB at batch 32),
     // so that the caller's stream is free for the convolutions of run i+1: the small kernels (peaks, assembly) co-reside
     // with the conv CTAs and the limbs blocks fill the SMs the conv launches leave idle in their last wave.
-    // B200POSE_POST_OVERLAP=0 keeps everything on the caller's stream.
-    bool overlap = true;
-    DevBuf<float> ov_maps[2];                       // [heat | paf] copies, slot = run parity
+    DevBuf<float> ov_maps[2];                      // [heat | paf] copies, slot = run parity
     cudaEvent_t ev_maps = nullptr, ev_ld[2] = {nullptr, nullptr};   // maps copied (st) / limbs done with a slot (s2)
     bool have_ld[2] = {false, false};
     // extents of a ragged run, slot = run parity: the peaks / limbs of run i on the second stream still read them while
@@ -243,27 +277,6 @@ struct b200pose_post {
 };
 
 namespace {
-
-// activation buffer `id` (0 .. 13 = t1 .. br512) or its residual plane
-DevBuf<__nv_bfloat16>* act_buffer(b200pose_net* net, int id, bool lo) {
-    DevBuf<__nv_bfloat16>* hi[kNumAct] = {&net->t1, &net->t2, &net->t3, &net->t4, &net->t5a, &net->t5b, &net->t6,
-                                          &net->t7, &net->t8, &net->t9, &net->cat, &net->bra, &net->brb, &net->br512};
-    DevBuf<__nv_bfloat16>* lp[kNumAct] = {&net->l1, &net->l2, &net->l3, &net->l4, &net->l5a, &net->l5b, &net->l6,
-                                          &net->l7, &net->l8, &net->l9, &net->lcat, &net->lbra, &net->lbrb, &net->lbr512};
-    return (id < 0 || id >= kNumAct) ? nullptr : (lo ? lp[id] : hi[id]);
-}
-
-int act_buffer_id(b200pose_net* net, const void* p) {
-    for (int i = 0; i < kNumAct; ++i)
-        if (act_buffer(net, i, false)->p == p) return i;
-    return -1;
-}
-
-int f32_map_id(const b200pose_net* net, const float* p) {
-    for (int i = 0; i < 12; ++i)
-        if (p != nullptr && net->out_f32[i].p == p) return i;
-    return -1;
-}
 
 int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_ids /*per group*/, int n_tile,
                   bool cat_input, int ks, int relu, int pool) {
@@ -310,13 +323,13 @@ bool small_plan(const b200pose_net* net, int n, int H, int W) {
     return 2 * n * ((H / 8 + kTileH - 1) / kTileH) * ((W / 8 + kTileW - 1) / kTileW) * 2 <= net->num_sms;
 }
 
-int add_plan(b200pose_net* net, const TcLayer& L, int n, int H, int W, const __nv_bfloat16* in, int in_cstride,
-             int in_ch_base, int in_group_stride, __nv_bfloat16* out, int out_cstride, int off0, int off1, int store0,
-             int store1, float* f32_0, float* f32_1, int f32c0, int f32c1) {
+// Appends tensor-core layer L, wired as `wr`, to plan p; a stage head writes the fp32 maps 2 * stage, 2 * stage + 1.
+int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& wr, int stage) {
+    const int n = p.n, H = p.H / kActDiv[wr.in], W = p.W / kActDiv[wr.in];
     ConvTcArgs a;
     memset(&a, 0, sizeof(a));
     a.n_img = n; a.H = H; a.W = W; a.ksize = L.ks; a.cin_blocks = L.cin_blocks;
-    a.in_ch_base = in_ch_base; a.in_ch_group_stride = in_group_stride; a.groups = L.groups;
+    a.in_ch_base = wr.in_base; a.in_ch_group_stride = wr.in_group_stride; a.groups = L.groups;
     a.n_tile = L.n_tile; a.n_tiles = L.n_tiles; a.bias = L.bias; a.relu = L.relu; a.pool = L.pool;
     {   // small batches: while the layer's CTAs fill at most half of the SMs, halve the work per CTA - 128-wide n-tiles become
         // 64-wide, then 32-wide (the weight layout does not depend on the n-tile)
@@ -324,142 +337,65 @@ int add_plan(b200pose_net* net, const TcLayer& L, int n, int H, int W, const __n
         if (L.n_tile == 128 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 64; a.n_tiles = L.n_tiles * 2; }
         if (a.n_tile == 64 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 32; a.n_tiles *= 2; }
     }
-    if (net->plan_split) {     // bf16x3: K-chunked accumulation in a second register set, so N <= 64
+    if (p.split) {     // bf16x3: K-chunked accumulation in a second register set, so N <= 64
         a.chunk = 1;
         if (a.n_tile > 64) { a.n_tile = 64; a.n_tiles = L.n_tiles * (L.n_tile / 64); }
     }
-    a.out = out; a.out_cstride = out_cstride;
-    a.out_ch_off[0] = off0; a.out_ch_off[1] = off1;
-    a.store_ch[0] = store0; a.store_ch[1] = store1;
-    a.out_f32[0] = f32_0; a.out_f32[1] = f32_1;
-    a.f32_ch[0] = f32c0; a.f32_ch[1] = f32c1;
+    a.out = net->act[wr.out].p; a.out_cstride = kActC[wr.out];
+    a.out_ch_off[0] = wr.out_off[0]; a.out_ch_off[1] = wr.out_off[1];
+    a.store_ch[0] = wr.store[0]; a.store_ch[1] = wr.store[1];
+    const int f32[2] = {wr.maps ? 2 * stage : -1, wr.maps ? 2 * stage + 1 : -1};
+    if (wr.maps) {
+        a.out_f32[0] = net->out_f32[f32[0]].p; a.out_f32[1] = net->out_f32[f32[1]].p;
+        a.f32_ch[0] = kPaf; a.f32_ch[1] = kHeat;
+    }
     // small batches (the 46 x 46 layers fill less than half of the SMs with 16 x 16 tiles): chain the layers with programmatic
-    // dependent launches; the first tensor-core layer follows conv1_1, which does not signal
-    a.pdl = (net->conv_pdl && !net->plan.empty() && small_plan(net, n, H, W)) ? 1 : 0;
+    // dependent launches; the first tensor-core layer follows conv1_1, which does not signal.  small_plan gets this
+    // layer's H, W and divides them by 8 again (DESIGN §2.1).
+    a.pdl = (!p.launches.empty() && small_plan(net, n, H, W)) ? 1 : 0;
+    while ((a.H << a.ext_shift) < p.H) ++a.ext_shift;      // ragged batches: the launch's output resolution relative to the input
+    a.ext_shift += a.pool;
     const __nv_bfloat16* in_lo = nullptr;
-    if (net->plan_split) {
+    if (p.split) {
         a.split = 1;
-        in_lo = net->lo_of.at(in);
-        a.out_lo = net->lo_of.at(out);
+        in_lo = net->act_lo[wr.in].p;
+        a.out_lo = net->act_lo[wr.out].p;
     }
-    cudaError_t e = conv_tc_make_maps(a, in, in_cstride, L.w, in_lo);
+    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], L.w, in_lo);
     if (e != cudaSuccess) return fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
-    net->plan.push_back(a);
-    net->plan_flops.push_back(2.0 * n * H * W * L.macs_per_pixel);
-    net->plan_info.push_back({act_buffer_id(net, in), in_cstride, act_buffer_id(net, out),
-                              {f32_map_id(net, f32_0), f32_map_id(net, f32_1)}});
+    p.launches.push_back({a, 2.0 * n * H * W * L.macs_per_pixel, wr.in, wr.out, {f32[0], f32[1]}});
     return 0;
 }
 
-int build_plan_bf16(b200pose_net* net, int n, int H, int W, bool split, cudaStream_t st) {
-    const size_t px1 = (size_t)n * H * W, px2 = px1 / 4, px4 = px1 / 16, px8 = px1 / 64;
-    const int h = H / 8, w = W / 8;
-    CU(net->t1.ensure(px1 * 64)); CU(net->t2.ensure(px2 * 64)); CU(net->t3.ensure(px2 * 128));
-    CU(net->t4.ensure(px4 * 128)); CU(net->t5a.ensure(px4 * 256)); CU(net->t5b.ensure(px4 * 256));
-    CU(net->t6.ensure(px8 * 256)); CU(net->t7.ensure(px8 * 512)); CU(net->t8.ensure(px8 * 512));
-    CU(net->t9.ensure(px8 * 256)); CU(net->cat.ensure(px8 * 192)); CU(net->bra.ensure(px8 * 256));
-    CU(net->brb.ensure(px8 * 256)); CU(net->br512.ensure(px8 * 1024));
-    // pad lanes of the concat buffer must read as zero; on the caller's stream (a non-blocking stream is not ordered
-    // against the legacy default stream a plain cudaMemset would use)
-    CU(cudaMemsetAsync(net->cat.p, 0, px8 * 192 * 2, st));
-    net->plan_split = split;
-    net->lo_of.clear();
-    if (split) {
-        CU(net->l1.ensure(px1 * 64)); CU(net->l2.ensure(px2 * 64)); CU(net->l3.ensure(px2 * 128));
-        CU(net->l4.ensure(px4 * 128)); CU(net->l5a.ensure(px4 * 256)); CU(net->l5b.ensure(px4 * 256));
-        CU(net->l6.ensure(px8 * 256)); CU(net->l7.ensure(px8 * 512)); CU(net->l8.ensure(px8 * 512));
-        CU(net->l9.ensure(px8 * 256)); CU(net->lcat.ensure(px8 * 192)); CU(net->lbra.ensure(px8 * 256));
-        CU(net->lbrb.ensure(px8 * 256)); CU(net->lbr512.ensure(px8 * 1024));
-        CU(cudaMemsetAsync(net->lcat.p, 0, px8 * 192 * 2, st));
-        DevBuf<__nv_bfloat16>* hi[] = {&net->t1, &net->t2, &net->t3, &net->t4, &net->t5a, &net->t5b, &net->t6, &net->t7,
-                                       &net->t8, &net->t9, &net->cat, &net->bra, &net->brb, &net->br512};
-        DevBuf<__nv_bfloat16>* lo[] = {&net->l1, &net->l2, &net->l3, &net->l4, &net->l5a, &net->l5b, &net->l6, &net->l7,
-                                       &net->l8, &net->l9, &net->lcat, &net->lbra, &net->lbrb, &net->lbr512};
-        for (int i = 0; i < 14; ++i) net->lo_of[hi[i]->p] = lo[i]->p;
+PlanBuffers plan_buffers(const b200pose_net* net) {
+    PlanBuffers b;
+    for (int i = 0; i < kNumAct; ++i) {
+        b[i] = net->act[i].p;
+        b[kNumAct + i] = net->act_lo[i].p;
     }
-    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px8 * (i % 2 == 0 ? kPaf : kHeat)));
-    net->plan.clear();
-    net->plan_flops.clear();
-    net->plan_info.clear();
-    const std::vector<TcLayer>& T = net->tc;
-#define PLAN(...) do { if (add_plan(net, __VA_ARGS__)) return 1; } while (0)
-    // trunk (conv1_1 runs on CUDA cores before the plan)
-    PLAN(T[0], n, H, W, net->t1.p, 64, 0, 0, net->t2.p, 64, 0, 0, 64, 0, nullptr, nullptr, 0, 0);              // conv1_2+pool
-    PLAN(T[1], n, H / 2, W / 2, net->t2.p, 64, 0, 0, net->t3.p, 128, 0, 0, 128, 0, nullptr, nullptr, 0, 0);    // conv2_1
-    PLAN(T[2], n, H / 2, W / 2, net->t3.p, 128, 0, 0, net->t4.p, 128, 0, 0, 128, 0, nullptr, nullptr, 0, 0);   // conv2_2+pool
-    PLAN(T[3], n, H / 4, W / 4, net->t4.p, 128, 0, 0, net->t5a.p, 256, 0, 0, 128, 0, nullptr, nullptr, 0, 0);  // conv3_1
-    PLAN(T[4], n, H / 4, W / 4, net->t5a.p, 256, 0, 0, net->t5b.p, 256, 0, 0, 128, 0, nullptr, nullptr, 0, 0); // conv3_2
-    PLAN(T[5], n, H / 4, W / 4, net->t5b.p, 256, 0, 0, net->t5a.p, 256, 0, 0, 128, 0, nullptr, nullptr, 0, 0); // conv3_3
-    PLAN(T[6], n, H / 4, W / 4, net->t5a.p, 256, 0, 0, net->t6.p, 256, 0, 0, 128, 0, nullptr, nullptr, 0, 0);  // conv3_4+pool
-    PLAN(T[7], n, h, w, net->t6.p, 256, 0, 0, net->t7.p, 512, 0, 0, 128, 0, nullptr, nullptr, 0, 0);            // conv4_1
-    PLAN(T[8], n, h, w, net->t7.p, 512, 0, 0, net->t8.p, 512, 0, 0, 128, 0, nullptr, nullptr, 0, 0);            // conv4_2
-    PLAN(T[9], n, h, w, net->t8.p, 512, 0, 0, net->t9.p, 256, 0, 0, 128, 0, nullptr, nullptr, 0, 0);            // conv4_3_CPM
-    PLAN(T[10], n, h, w, net->t9.p, 256, 0, 0, net->cat.p, 192, 64, 0, 128, 0, nullptr, nullptr, 0, 0);         // conv4_4_CPM -> feat slice
-    // stage 1 (both branches grouped)
-    PLAN(T[11], n, h, w, net->cat.p, 192, 64, 0, net->bra.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-    PLAN(T[12], n, h, w, net->bra.p, 256, 0, 128, net->brb.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-    PLAN(T[13], n, h, w, net->brb.p, 256, 0, 128, net->bra.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-    PLAN(T[14], n, h, w, net->bra.p, 256, 0, 128, net->br512.p, 1024, 0, 512, 128, 128, nullptr, nullptr, 0, 0);
-    PLAN(T[15], n, h, w, net->br512.p, 1024, 0, 512, net->cat.p, 192, 0, 40, 40, 24, net->out_f32[0].p,
-         net->out_f32[1].p, kPaf, kHeat);
-    for (int s = 2; s <= 6; ++s) {
-        const int b0 = 16 + (s - 2) * 7;
-        PLAN(T[b0 + 0], n, h, w, net->cat.p, 192, 0, 0, net->bra.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-        PLAN(T[b0 + 1], n, h, w, net->bra.p, 256, 0, 128, net->brb.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-        PLAN(T[b0 + 2], n, h, w, net->brb.p, 256, 0, 128, net->bra.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-        PLAN(T[b0 + 3], n, h, w, net->bra.p, 256, 0, 128, net->brb.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-        PLAN(T[b0 + 4], n, h, w, net->brb.p, 256, 0, 128, net->bra.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-        PLAN(T[b0 + 5], n, h, w, net->bra.p, 256, 0, 128, net->brb.p, 256, 0, 128, 128, 128, nullptr, nullptr, 0, 0);
-        PLAN(T[b0 + 6], n, h, w, net->brb.p, 256, 0, 128, net->cat.p, 192, 0, 40, 40, 24,
-             net->out_f32[2 * (s - 1)].p, net->out_f32[2 * (s - 1) + 1].p, kPaf, kHeat);
+    for (int i = 0; i < 12; ++i) b[2 * kNumAct + i] = net->out_f32[i].p;
+    return b;
+}
+
+// Fills p.launches, (re)allocating the buffers of p's key.
+int build_plan_bf16(b200pose_net* net, Plan& p, cudaStream_t st) {
+    const size_t px = (size_t)p.n * p.H * p.W;
+    for (int plane = 0; plane < (p.split ? 2 : 1); ++plane) {
+        DevBuf<__nv_bfloat16>* bufs = plane ? net->act_lo : net->act;
+        for (int i = 0; i < kNumAct; ++i) CU(bufs[i].ensure(px / (kActDiv[i] * kActDiv[i]) * kActC[i]));
+        // pad lanes of the concat buffer must read as zero; on the caller's stream (a non-blocking stream is not ordered
+        // against the legacy default stream a plain cudaMemset would use)
+        CU(cudaMemsetAsync(bufs[CAT].p, 0, px / 64 * kActC[CAT] * 2, st));
     }
-#undef PLAN
-    for (ConvTcArgs& a : net->plan) {      // ragged batches: the launch's output resolution relative to the input
-        int s = 0;
-        while ((a.H << s) < H) ++s;
-        a.ext_shift = s + a.pool;
-    }
+    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * (i % 2 == 0 ? kPaf : kHeat)));
+    int k = 0;
+    for (const Wiring& wr : kTrunkWiring)
+        if (add_plan(net, p, net->tc[k++], wr, 0)) return 1;
+    for (int s = 1; s <= 6; ++s)
+        for (int li = 0; li < stage_num_layers(s); ++li)
+            if (add_plan(net, p, net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], s - 1)) return 1;
+    p.buffers = plan_buffers(net);
     return 0;
-}
-
-std::vector<const void*> plan_buffers(const b200pose_net* net) {
-    std::vector<const void*> v = {net->t1.p, net->t2.p, net->t3.p, net->t4.p, net->t5a.p, net->t5b.p, net->t6.p, net->t7.p,
-                                  net->t8.p, net->t9.p, net->cat.p, net->bra.p, net->brb.p, net->br512.p,
-                                  net->l1.p, net->l2.p, net->l3.p, net->l4.p, net->l5a.p, net->l5b.p, net->l6.p, net->l7.p,
-                                  net->l8.p, net->l9.p, net->lcat.p, net->lbra.p, net->lbrb.p, net->lbr512.p};
-    for (const auto& b : net->out_f32) v.push_back(b.p);
-    return v;
-}
-
-// plan cache (experiment): returns true when a valid plan for the key was swapped into net->plan
-bool plan_cache_swap(b200pose_net* net, int n, int H, int W, int want) {
-    if (net->kmode >= 0 && !net->plan.empty()) {      // stash the plan we hold
-        b200pose_net::PlanEntry* slot = nullptr;
-        for (auto& e : net->plan_cache)
-            if (e.n == net->kn && e.H == net->kH && e.W == net->kW && e.mode == net->kmode) slot = &e;
-        if (!slot) {
-            if (net->plan_cache.size() >= 32) net->plan_cache.erase(net->plan_cache.begin());
-            net->plan_cache.emplace_back();
-            slot = &net->plan_cache.back();
-        }
-        slot->n = net->kn; slot->H = net->kH; slot->W = net->kW; slot->mode = net->kmode; slot->split = net->plan_split;
-        slot->plan.swap(net->plan);
-        slot->flops.swap(net->plan_flops);
-        slot->info.swap(net->plan_info);
-        slot->buffers = plan_buffers(net);
-        net->plan.clear(); net->plan_flops.clear(); net->plan_info.clear();
-        net->kmode = -1;
-    }
-    for (auto& e : net->plan_cache)
-        if (e.n == n && e.H == H && e.W == W && e.mode == want && !e.plan.empty() && e.buffers == plan_buffers(net)) {
-            net->plan.swap(e.plan);
-            net->plan_flops.swap(e.flops);
-            net->plan_info.swap(e.info);
-            net->plan_split = e.split;
-            net->kn = n; net->kH = H; net->kW = W; net->kmode = want;
-            return true;
-        }
-    return false;
 }
 
 void drop_graphs(b200pose_net* net) {
@@ -468,70 +404,80 @@ void drop_graphs(b200pose_net* net) {
     net->graph_seen.clear();
 }
 
-// plan launch i; a ragged forward passes its extents table (the plans are shared with uniform batches of the canvas size)
-cudaError_t launch_plan_entry(const b200pose_net* net, size_t i, const int* ext, cudaStream_t st) {
-    if (ext == nullptr) return conv_tc_launch(net->plan[i], net->num_sms, st);
-    ConvTcArgs a = net->plan[i];
-    a.ext = ext;
-    return conv_tc_launch(a, net->num_sms, st);
-}
-
-int launch_forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, cudaStream_t st, bool split,
-                        const int* ext) {
-    CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->t1.p, split ? net->l1.p : nullptr, n, H, W, ext, st));
-    for (size_t i = 0; i < net->plan.size(); ++i) CU(launch_plan_entry(net, i, ext, st));
+// Points net->plan at the plan of (n, H, W, mode): a kept one whose buffers are still the net's, or a new one (the
+// oldest of 32 is dropped).  A build may move the buffers the captured graphs point into: it synchronises the stream
+// and drops the graphs first.
+int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t st) {
+    const PlanBuffers bufs = plan_buffers(net);
+    for (const Plan& p : net->plans)
+        if (p.n == n && p.H == H && p.W == W && p.mode == mode && p.buffers == bufs) {
+            net->plan = &p;
+            return 0;
+        }
+    CU(cudaStreamSynchronize(st));
+    drop_graphs(net);
+    net->plan = nullptr;
+    net->plans.remove_if([&](const Plan& p) { return p.n == n && p.H == H && p.W == W && p.mode == mode; });
+    if (net->plans.size() >= 32) net->plans.pop_front();
+    net->plans.push_back(Plan{n, H, W, mode, mode == B200POSE_MODE_BF16X3, {}, {}});
+    if (build_plan_bf16(net, net->plans.back(), st)) {
+        net->plans.pop_back();
+        return 1;
+    }
+    net->plan = &net->plans.back();
     return 0;
 }
 
-int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, cudaStream_t st, bool split,
-                 const int* ext) {
-    const int want = split ? B200POSE_MODE_BF16X3 : B200POSE_MODE_BF16;
-    if (net->pn != n || net->pH != H || net->pW != W || net->pmode != want) {
-        if (!(net->plan_cache_on && plan_cache_swap(net, n, H, W, want))) {
-            CU(cudaStreamSynchronize(st));
-            drop_graphs(net);                   // the buffers the captured tensor maps point into may move
-            if (build_plan_bf16(net, n, H, W, split, st)) return 1;
-            net->kn = n; net->kH = H; net->kW = W; net->kmode = want;
-        }
-        net->pn = n; net->pH = H; net->pW = W; net->pmode = want;
+// The first k launches of a forward with net->plan: conv1_1, then the plan's.  A ragged forward passes its extents
+// table (the plans are shared with uniform batches of the canvas size).
+int launch_forward_bf16(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st) {
+    const Plan& p = *net->plan;
+    if (k >= 1)
+        CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr,
+                             p.n, p.H, p.W, ext, st));
+    for (int i = 0; i + 1 < k; ++i) {
+        ConvTcArgs a = p.launches[i].a;
+        a.ext = ext;
+        CU(conv_tc_launch(a, net->num_sms, st));
     }
-    const long launches = 1 + (long)net->plan.size();
+    return 0;
+}
+
+int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, int mode, cudaStream_t st,
+                 const int* ext) {
+    if (select_plan(net, n, H, W, mode, st)) return 1;
+    const int launches = 1 + (int)net->plan->launches.size();
+    cudaGraphExec_t exec = nullptr;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     if (net->use_graph && small_plan(net, n, H, W) && st != nullptr && cudaStreamIsCapturing(st, &cap) == cudaSuccess &&
         cap == cudaStreamCaptureStatusNone) {
-        const b200pose_net::GraphKey key{n, H, W, want, in_u8, ext != nullptr, d_in};
+        const b200pose_net::GraphKey key{n, H, W, mode, in_u8, ext != nullptr, d_in};
         auto it = net->graphs.find(key);
-        if (it == net->graphs.end() && net->graph_seen.insert(key).second) {      // first sight: plain launches
+        if (it != net->graphs.end()) {
+            exec = it->second;
+        } else if (net->graph_seen.insert(key).second) {      // first sight: plain launches
             if (net->graph_seen.size() > 4096) net->graph_seen.clear();
-            if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext)) return 1;
-            g_launches += launches;
-            return 0;
-        }
-        if (it == net->graphs.end()) {
+        } else {
             if (net->graphs.size() >= 64) drop_graphs(net);
             cudaGraph_t graph = nullptr;
-            cudaGraphExec_t exec = nullptr;
             CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-            const int rc = launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext);
+            const int rc = launch_forward_bf16(net, d_in, in_u8, ext, launches, st);
             cudaError_t e = cudaStreamEndCapture(st, &graph);
             if (rc == 0 && e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
             if (graph) cudaGraphDestroy(graph);
-            if (rc != 0 || e != cudaSuccess) {      // no graph (e.g. a launch attribute the capture refuses): plain launches from now on
+            if (rc == 0 && e == cudaSuccess) {
+                net->graphs.emplace(key, exec);
+            } else {      // no graph (e.g. a launch attribute the capture refuses): plain launches from now on
                 cudaGetLastError();
                 fprintf(stderr, "[b200pose] CUDA graph capture of the forward pass failed (%s): launching directly\n",
                         rc ? b200pose_last_error() : cudaGetErrorString(e));
                 net->use_graph = false;
-                if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext)) return 1;
-                g_launches += launches;
-                return 0;
+                exec = nullptr;
             }
-            it = net->graphs.emplace(key, exec).first;
         }
-        CU(cudaGraphLaunch(it->second, st));
-        g_launches += launches;
-        return 0;
     }
-    if (launch_forward_bf16(net, d_in, in_u8, n, H, W, st, split, ext)) return 1;
+    if (exec) CU(cudaGraphLaunch(exec, st));
+    else if (launch_forward_bf16(net, d_in, in_u8, ext, launches, st)) return 1;
     g_launches += launches;
     return 0;
 }
@@ -544,7 +490,6 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, cuda
     CU(net->f_a.ensure(px1 * 64)); CU(net->f_b.ensure(px1 * 64));
     CU(net->f_cat.ensure(px8 * kCat)); CU(net->f_x.ensure(px8 * 512)); CU(net->f_y.ensure(px8 * 512));
     for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px8 * (i % 2 == 0 ? kPaf : kHeat)));
-    net->pmode = B200POSE_MODE_FP32;   // invalidates the bf16 plan's claim on out_f32 (same buffers, same sizes)
     CU(nchw_to_nhwc_f32_launch(d_in, net->f_in.p, n, 3, H, W, 3, 0, st));
     ++g_launches;
     const float* cur = net->f_in.p;
@@ -635,10 +580,6 @@ int b200pose_net_create(b200pose_net** out, int cuda_device) {
     net->host_w.resize(kNumConvs);
     net->host_b.resize(kNumConvs);
     net->have.assign(B200POSE_NUM_TENSORS, false);
-    const char* pc = getenv("B200POSE_PLAN_CACHE");
-    net->plan_cache_on = !(pc && pc[0] == '0');
-    const char* pd = getenv("B200POSE_CONV_PDL");
-    net->conv_pdl = !(pd && pd[0] == '0');
     const char* gr = getenv("B200POSE_GRAPH");
     net->use_graph = !(gr && gr[0] == '0');
     *out = net;
@@ -651,12 +592,7 @@ void b200pose_net_destroy(b200pose_net* net) {
     drop_graphs(net);
     for (int i = 0; i < kNumConvs; ++i) { if (net->d_w[i]) cudaFree(net->d_w[i]); if (net->d_b[i]) cudaFree(net->d_b[i]); }
     for (TcLayer& L : net->tc) { if (L.w) cudaFree(L.w); if (L.bias) cudaFree(L.bias); }
-    DevBuf<__nv_bfloat16>* bb[] = {&net->t1, &net->t2, &net->t3, &net->t4, &net->t5a, &net->t5b, &net->t6,
-                                   &net->t7, &net->t8, &net->t9, &net->cat, &net->bra, &net->brb, &net->br512};
-    for (auto* b : bb) b->release();
-    DevBuf<__nv_bfloat16>* lb[] = {&net->l1, &net->l2, &net->l3, &net->l4, &net->l5a, &net->l5b, &net->l6,
-                                   &net->l7, &net->l8, &net->l9, &net->lcat, &net->lbra, &net->lbrb, &net->lbr512};
-    for (auto* b : lb) b->release();
+    for (int i = 0; i < kNumAct; ++i) { net->act[i].release(); net->act_lo[i].release(); }
     DevBuf<float>* fb[] = {&net->in_stage, &net->f_a, &net->f_b, &net->f_cat, &net->f_x, &net->f_y, &net->f_in, &net->f_u8};
     net->in_stage_u8.release();
     net->raw_stage.release();
@@ -714,12 +650,10 @@ int b200pose_net_finalize(b200pose_net* net) {
                               li == 6 ? 48 : 128, li == 0, s.ks, li != 6, 0))
                 return 1;
         }
-    net->pn = net->pH = net->pW = 0;
-    net->pmode = -1;
+    net->last = LastForward();
     drop_graphs(net);
-    net->plan_cache.clear();      // cached plans point at the previous packed weights
-    net->plan.clear(); net->plan_flops.clear(); net->plan_info.clear();
-    net->kmode = -1;
+    net->plan = nullptr;
+    net->plans.clear();      // the plans point at the previous packed weights
     net->finalized = true;
     return 0;
 }
@@ -744,7 +678,7 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
             d_in = net->in_stage.p;
         }
     }
-    int rc;
+    int rc, first_u8 = 0;     // the uint8 normalisation conv1_1 fuses (bf16 modes)
     if (mode == B200POSE_MODE_FP32) {
         if (in_u8) {   // parity mode: materialise rtpose_preprocess, then the fp32 path
             CU(net->f_u8.ensure(elems));
@@ -752,12 +686,13 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
             ++g_launches;
             rc = forward_fp32(net, net->f_u8.p, n, H, W, st, ext);
         } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, st, ext);
-    } else rc = forward_bf16(net, d_in, in_u8 ? net->preprocess : 0, n, H, W, st, mode == B200POSE_MODE_BF16X3, ext);
+    } else {
+        if (mode != B200POSE_MODE_BF16X3) mode = B200POSE_MODE_BF16;     // every other mode runs bf16
+        first_u8 = in_u8 ? net->preprocess : 0;
+        rc = forward_bf16(net, d_in, first_u8, n, H, W, mode, st, ext);
+    }
     if (rc) return rc;
-    net->last_in = d_in;
-    net->last_ext = ext;
-    net->last_in_u8 = (mode == B200POSE_MODE_FP32) ? 0 : (in_u8 ? net->preprocess : 0);
-    net->pn = n; net->pH = H; net->pW = W;
+    net->last = LastForward{n, H, W, mode, d_in, first_u8, ext};
     if (outputs) {
         const size_t px8 = (size_t)n * (H / 8) * (W / 8);
         for (int i = 0; i < 12; ++i)
@@ -809,12 +744,27 @@ static int upload_frames(b200pose_net* net, const std::vector<RaggedFrame>& fram
     return 0;
 }
 
-// the n frames of net->d_frames (sources at d_src) -> net->in_stage_u8 [n, Hc, Wc, 3]
-static int place_ragged_frames(b200pose_net* net, const unsigned char* d_src, int n, int Hc, int Wc, cudaStream_t st) {
+// Places the n frames of net->d_frames (sources at d_src) on an Hc x Wc canvas in net->in_stage_u8 and runs the
+// forward pass on them with extents `ext`.
+static int ragged_forward(b200pose_net* net, const unsigned char* d_src, int n, int Hc, int Wc, const std::vector<int>& ext,
+                          int mode, float* const* outputs, int outputs_on_device, cudaStream_t st, bool sync_host) {
     CU(net->in_stage_u8.ensure((size_t)n * Hc * Wc * 3));
-    cudaError_t e = ragged_frames_launch(d_src, net->d_frames.p, n, net->in_stage_u8.p, Hc, Wc, st);
-    if (e != cudaSuccess) return fail("ragged_frames_launch: %s", cudaGetErrorString(e));
-    ++g_launches;
+    if (launched(ragged_frames_launch(d_src, net->d_frames.p, n, net->in_stage_u8.p, Hc, Wc, st), "ragged_frames_launch"))
+        return 1;
+    if (int rc = upload_ext(net, ext, st)) return rc;
+    return net_forward_impl(net, net->in_stage_u8.p, 1, 1, n, Hc, Wc, mode, outputs, outputs_on_device, st, sync_host,
+                            net->d_ext);
+}
+
+// Raw uint8 frames of `bytes` on the device: a device input in place, else a copy in net->raw_stage.  flip: always
+// copied, with room for the mirror images behind the frames.
+static int stage_raw(b200pose_net* net, const unsigned char* images, int on_device, size_t bytes, int flip,
+                     cudaStream_t st, const unsigned char** d_raw) {
+    *d_raw = images;
+    if (on_device && !flip) return 0;
+    CU(net->raw_stage.ensure(bytes * (flip ? 2 : 1)));
+    CU(cudaMemcpyAsync(net->raw_stage.p, images, bytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    *d_raw = net->raw_stage.p;
     return 0;
 }
 
@@ -835,17 +785,11 @@ int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frame
         tab[i].src_w = hw[2 * i + 1];      // g.pad_h == 0: copied as it is
         bytes += (long long)hw[2 * i] * hw[2 * i + 1] * 3;
     }
-    const unsigned char* d_src = frames;
-    if (!on_device) {
-        CU(net->raw_stage.ensure((size_t)bytes));
-        CU(cudaMemcpyAsync(net->raw_stage.p, frames, (size_t)bytes, cudaMemcpyHostToDevice, st));
-        d_src = net->raw_stage.p;
-    }
+    const unsigned char* d_src;
+    if (int rc = stage_raw(net, frames, on_device, (size_t)bytes, 0, st, &d_src)) return rc;
     if (int rc = upload_frames(net, tab, st)) return rc;
-    if (int rc = place_ragged_frames(net, d_src, n, Hc, Wc, st)) return rc;
-    if (int rc = upload_ext(net, std::vector<int>(hw, hw + 2 * n), st)) return rc;
-    if (int rc = net_forward_impl(net, net->in_stage_u8.p, 1, 1, n, Hc, Wc, mode, outputs, outputs_on_device, st, true,
-                                  net->d_ext))
+    if (int rc = ragged_forward(net, d_src, n, Hc, Wc, std::vector<int>(hw, hw + 2 * n), mode, outputs, outputs_on_device,
+                                st, true))
         return rc;
     if (!on_device) CU(cudaStreamSynchronize(st));
     return 0;
@@ -858,90 +802,93 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess) {
     return 0;
 }
 
+// The last forward ran net->plan: a bf16 / bf16x3 forward has run since the last finalize.
+static bool last_ran_plan(const b200pose_net* net) {
+    const LastForward& l = net->last;
+    const Plan* p = net->plan;
+    return p && p->n == l.n && p->H == l.H && p->W == l.W && p->mode == l.mode;
+}
+
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream) {
-    if (!net || net->plan.empty() || (net->pmode != B200POSE_MODE_BF16 && net->pmode != B200POSE_MODE_BF16X3)) return -1;
+    if (!net || !last_ran_plan(net)) return -1;
     if (cudaSetDevice(net->device) != cudaSuccess) return -1;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    const int n = net->pn, H = net->pH, W = net->pW;
-    const int total = (int)net->plan.size() + 1;
+    const Plan& p = *net->plan;
+    const int n = p.n, H = p.H, W = p.W;
+    const int total = (int)p.launches.size() + 1;
     if (cap < total) return -1;
     std::vector<cudaEvent_t> ev(total + 1);
     for (auto& e : ev) cudaEventCreate(&e);
-    const void* d_in = net->last_in;
+    const void* d_in = net->last.in;
+    int in_u8 = net->last.in_u8;
     DevBuf<float> tmp;
-    if (!d_in) { if (tmp.ensure((size_t)n * 3 * H * W) != cudaSuccess) return -1; cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st); d_in = tmp.p; net->last_in_u8 = 0; }
+    if (!d_in) { if (tmp.ensure((size_t)n * 3 * H * W) != cudaSuccess) return -1; cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st); d_in = tmp.p; in_u8 = 0; }
     cudaEventRecord(ev[0], st);
-    conv_first_launch(d_in, net->last_in_u8, net->d_w[0], net->d_b[0], net->t1.p, net->plan_split ? net->l1.p : nullptr, n, H, W,
+    conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr, n, H, W,
                       nullptr, st);
     cudaEventRecord(ev[1], st);
-    for (size_t i = 0; i < net->plan.size(); ++i) {
-        conv_tc_launch(net->plan[i], net->num_sms, st);
+    for (size_t i = 0; i < p.launches.size(); ++i) {
+        conv_tc_launch(p.launches[i].a, net->num_sms, st);
         cudaEventRecord(ev[i + 2], st);
     }
     g_launches += total;
     if (cudaStreamSynchronize(st) != cudaSuccess) { fail("profile run failed: %s", cudaGetErrorString(cudaGetLastError())); return -1; }
     for (int i = 0; i < total; ++i) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
     flops[0] = 2.0 * n * H * W * 27.0 * 64.0;
-    for (size_t i = 0; i < net->plan.size(); ++i) flops[i + 1] = net->plan_flops[i];
+    for (size_t i = 0; i < p.launches.size(); ++i) flops[i + 1] = p.launches[i].flops;
     for (auto& e : ev) cudaEventDestroy(e);
     tmp.release();
     return total;
 }
 
-static bool debug_plan_ready(const b200pose_net* net) {
-    return net && !net->plan.empty() && net->plan_info.size() == net->plan.size() &&
-           (net->pmode == B200POSE_MODE_BF16 || net->pmode == B200POSE_MODE_BF16X3);
-}
-
 int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream) {
-    if (!debug_plan_ready(net) || !net->last_in) return fail("debug_run: no bf16 / bf16x3 forward has run");
-    if (launches < 0 || launches > 1 + (int)net->plan.size()) return fail("debug_run: %d launches out of range", launches);
+    if (!net || !last_ran_plan(net) || !net->last.in) return fail("debug_run: no bf16 / bf16x3 forward has run");
+    if (launches < 0 || launches > 1 + (int)net->plan->launches.size())
+        return fail("debug_run: %d launches out of range", launches);
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (launches >= 1)
-        CU(conv_first_launch(net->last_in, net->last_in_u8, net->d_w[0], net->d_b[0], net->t1.p,
-                             net->plan_split ? net->l1.p : nullptr, net->pn, net->pH, net->pW, net->last_ext, st));
-    for (int i = 0; i + 1 < launches; ++i) CU(launch_plan_entry(net, (size_t)i, net->last_ext, st));
+    if (launch_forward_bf16(net, net->last.in, net->last.in_u8, net->last.ext, launches, st)) return 1;
     g_launches += launches;
     CU(cudaStreamSynchronize(st));
     return 0;
 }
 
 int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
-    if (!debug_plan_ready(net)) return fail("debug_launch: no bf16 / bf16x3 forward has run");
-    if (i < 0 || i > (int)net->plan.size() || cap < B200POSE_DEBUG_LAUNCH_FIELDS || !fields)
+    if (!net || !last_ran_plan(net)) return fail("debug_launch: no bf16 / bf16x3 forward has run");
+    const Plan& p = *net->plan;
+    if (i < 0 || i > (int)p.launches.size() || cap < B200POSE_DEBUG_LAUNCH_FIELDS || !fields)
         return fail("debug_launch: launch %d / capacity %d out of range", i, cap);
     int* f = fields;
     for (int k = 0; k < B200POSE_DEBUG_LAUNCH_FIELDS; ++k) f[k] = 0;
     if (i == 0) {     // conv1_1 (CUDA cores / mma.sync): the network input -> t1
-        f[0] = -1; f[1] = 3; f[4] = 0; f[5] = 64; f[8] = 64;
-        f[10] = net->pH; f[11] = net->pW; f[12] = 3; f[14] = 1; f[15] = 64; f[16] = 1; f[17] = 1;
-        f[19] = net->plan_split ? 1 : 0; f[23] = f[24] = -1;
-        f[26] = net->last_in_u8;
+        f[0] = -1; f[1] = 3; f[4] = T1; f[5] = kActC[T1]; f[8] = 64;
+        f[10] = p.H; f[11] = p.W; f[12] = 3; f[14] = 1; f[15] = 64; f[16] = 1; f[17] = 1;
+        f[19] = p.split ? 1 : 0; f[23] = f[24] = -1;
+        f[26] = net->last.in_u8;
     } else {
-        const ConvTcArgs& a = net->plan[i - 1];
-        const LaunchInfo& li = net->plan_info[i - 1];
-        f[0] = li.in_buf; f[1] = li.in_cstride; f[2] = a.in_ch_base; f[3] = a.in_ch_group_stride;
-        f[4] = li.out_buf; f[5] = a.out_cstride; f[6] = a.out_ch_off[0]; f[7] = a.out_ch_off[1];
+        const PlanLaunch& l = p.launches[i - 1];
+        const ConvTcArgs& a = l.a;
+        f[0] = l.in; f[1] = kActC[l.in]; f[2] = a.in_ch_base; f[3] = a.in_ch_group_stride;
+        f[4] = l.out; f[5] = a.out_cstride; f[6] = a.out_ch_off[0]; f[7] = a.out_ch_off[1];
         f[8] = a.store_ch[0]; f[9] = a.store_ch[1];
         f[10] = a.H; f[11] = a.W; f[12] = a.ksize; f[13] = a.cin_blocks; f[14] = a.groups; f[15] = a.n_tile;
         f[16] = a.n_tiles; f[17] = a.relu; f[18] = a.pool; f[19] = a.split; f[20] = a.chunk; f[21] = a.pdl; f[22] = a.tps;
-        f[23] = li.f32[0]; f[24] = li.f32[1];
+        f[23] = l.f32[0]; f[24] = l.f32[1];
     }
-    f[25] = net->pn;
+    f[25] = p.n;
     return B200POSE_DEBUG_LAUNCH_FIELDS;
 }
 
 int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes) {
-    if (!debug_plan_ready(net)) return fail("debug_read: no bf16 / bf16x3 forward has run");
-    const int n = net->pn, H = net->pH, W = net->pW;
+    if (!net || !last_ran_plan(net)) return fail("debug_read: no bf16 / bf16x3 forward has run");
+    const int n = net->plan->n, H = net->plan->H, W = net->plan->W;
     if (img0 < 0 || count < 1 || img0 + count > n || !host) return fail("debug_read: images [%d, %d) out of range", img0, img0 + count);
     const char* src = nullptr;
     size_t per = 0;
     if (buf >= 0 && buf < kNumAct) {
-        if (lo_plane && !net->plan_split) return fail("debug_read: residual planes exist in bf16x3 mode only");
+        if (lo_plane && !net->plan->split) return fail("debug_read: residual planes exist in bf16x3 mode only");
         per = (size_t)(H / kActDiv[buf]) * (W / kActDiv[buf]) * kActC[buf] * 2;
-        src = reinterpret_cast<const char*>(act_buffer(net, buf, lo_plane != 0)->p);
+        src = reinterpret_cast<const char*>((lo_plane ? net->act_lo : net->act)[buf].p);
     } else if (buf >= kNumAct && buf < kNumAct + 12 && !lo_plane) {
         const int m = buf - kNumAct;
         per = (size_t)(H / 8) * (W / 8) * (m % 2 == 0 ? kPaf : kHeat) * 4;
@@ -956,9 +903,9 @@ int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, 
 }
 
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w) {
-    if (!net || net->pn == 0) return fail("no forward has run");
+    if (!net || net->last.n == 0) return fail("no forward has run");
     *paf = net->out_f32[10].p; *heat = net->out_f32[11].p;
-    *n = net->pn; *h = net->pH / 8; *w = net->pW / 8;
+    *n = net->last.n; *h = net->last.H / 8; *w = net->last.W / 8;
     return 0;
 }
 
@@ -970,10 +917,8 @@ int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, in
     CU(cudaSetDevice(cuda_device));
     b200pose_post* p = new b200pose_post();
     p->device = cuda_device;
-    // candidate-key pool: 6 Mi entries (48 MB) per image of the batch (capped at 2 GiB) - key slots for every (a, b) pair of the limbs that do not
-    // fit shared memory plus partition scratch, i.e. ~2 M pairs per image - capped at 1 GiB; exhausting it sets a status bit (loud error in the Python layer)
-    // two halves (warp slots + partition scratch / contiguous sorted lists), each with one slot per (a, b) PAIR of every
-    // limb: 8 Mi pairs per image of the batch (random-weight 368x368 maps produce ~1 M), capped at 8 GiB in total
+    // candidate-key pool (DESIGN §1): min(batch_cap x 16 Mi, 1 Gi) 8-byte entries, i.e. 128 MB per image of the batch and
+    // at most 8 GiB; exhausting it sets a status bit (a loud error in the Python layer)
     const long pool = (long)batch_cap * (16L << 20) < (1L << 30) ? (long)batch_cap * (16L << 20) : (1L << 30);
     cudaError_t e = post_alloc(p->pb, batch_cap, peak_cap, human_cap, pool);
     if (e != cudaSuccess) { delete p; return fail("post_alloc failed: %s", cudaGetErrorString(e)); }
@@ -990,8 +935,6 @@ int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, in
         CU(cudaMalloc(&p->d_ext[b], (size_t)batch_cap * 2 * sizeof(int)));
     }
     CU(cudaEventCreateWithFlags(&p->ev_maps, cudaEventDisableTiming));
-    const char* ov = getenv("B200POSE_POST_OVERLAP");
-    p->overlap = !(ov && ov[0] == '0');
     *out = p;
     return 0;
 }
@@ -1043,30 +986,32 @@ static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st) 
     return 0;
 }
 
+static int check_batch(const b200pose_post* p, int n) {
+    if (n > p->pb.batch_cap) return fail("batch %d exceeds post batch_cap %d", n, p->pb.batch_cap);
+    return 0;
+}
+
 // ext: device extents table of a ragged batch (h x w is then its canvas at the maps' resolution), or null
 static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_paf, int layout, int n, int h, int w,
                         float thresh, cudaStream_t st, const int* ext = nullptr) {
-    if (n > p->pb.batch_cap) return fail("batch %d exceeds post batch_cap %d", n, p->pb.batch_cap);
-    cudaStream_t ps = st;       // the stream peaks / limbs run on
+    if (int rc = check_batch(p, n)) return rc;
     const int slot = (int)(p->runs & 1);
-    if (p->overlap && p->have_ld[slot]) CU(cudaStreamWaitEvent(st, p->ev_ld[slot], 0));   // run i-2 is done with this slot
+    if (p->have_ld[slot]) CU(cudaStreamWaitEvent(st, p->ev_ld[slot], 0));   // run i-2 is done with this slot
     if (ext) {
         CU(cudaMemcpyAsync(p->d_ext[slot], ext, (size_t)n * 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
         ext = p->d_ext[slot];
     }
-    if (p->overlap) {
-        // private copy of the maps (15 MB at batch 32) so that the next forward may overwrite the network's output
-        // buffers while this run's post-processing is still reading; everything after the copy runs on s2
-        const size_t eh = (size_t)n * 19 * h * w, ep = (size_t)n * 38 * h * w;
-        CU(p->ov_maps[slot].ensure(eh + ep));
-        CU(cudaMemcpyAsync(p->ov_maps[slot].p, d_heat, eh * 4, cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemcpyAsync(p->ov_maps[slot].p + eh, d_paf, ep * 4, cudaMemcpyDeviceToDevice, st));
-        CU(cudaEventRecord(p->ev_maps, st));
-        CU(cudaStreamWaitEvent(p->s2, p->ev_maps, 0));
-        d_heat = p->ov_maps[slot].p;
-        d_paf = p->ov_maps[slot].p + eh;
-        ps = p->s2;
-    }
+    // private copy of the maps (15 MB at batch 32) so that the next forward may overwrite the network's output
+    // buffers while this run's post-processing is still reading; everything after the copy runs on s2
+    const size_t eh = (size_t)n * 19 * h * w, ep = (size_t)n * 38 * h * w;
+    CU(p->ov_maps[slot].ensure(eh + ep));
+    CU(cudaMemcpyAsync(p->ov_maps[slot].p, d_heat, eh * 4, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(p->ov_maps[slot].p + eh, d_paf, ep * 4, cudaMemcpyDeviceToDevice, st));
+    CU(cudaEventRecord(p->ev_maps, st));
+    CU(cudaStreamWaitEvent(p->s2, p->ev_maps, 0));
+    d_heat = p->ov_maps[slot].p;
+    d_paf = p->ov_maps[slot].p + eh;
+    cudaStream_t ps = p->s2;       // the stream peaks / limbs run on
     // the previous run's assembly (second stream) still reads the peak / connection buffers this run overwrites, and
     // its D2H copies of status / counts (enqueued after the assembly) must not race with this run's memset + peaks:
     // wait for the event recorded after those copies
@@ -1084,10 +1029,8 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
     }
     if (e != cudaSuccess) return fail("post_limbs: %s", cudaGetErrorString(e));
     g_launches += 2;
-    if (p->overlap) {
-        CU(cudaEventRecord(p->ev_ld[slot], ps));
-        p->have_ld[slot] = true;
-    }
+    CU(cudaEventRecord(p->ev_ld[slot], ps));
+    p->have_ld[slot] = true;
     p->hw_h = h; p->hw_w = w;
     return enqueue_assemble_and_fetch(p, n, ps);
 }
@@ -1201,27 +1144,6 @@ int b200pose_post_get_peaks(b200pose_post* p, int img, float* out, int max_peaks
     return k;
 }
 
-static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input, int in_u8, int input_on_device, int n,
-                      int H, int W, int mode, float thresh, void* cuda_stream) {
-    if (!net || !post) return fail("null handle");
-    if (net->device != post->device) return fail("net and post live on different devices");
-    // host input is staged asynchronously: the caller keeps it alive until b200pose_post_sync()
-    int rc = net_forward_impl(net, input, in_u8, input_on_device, n, H, W, mode, nullptr, 1,
-                              reinterpret_cast<cudaStream_t>(cuda_stream), false);
-    if (rc) return rc;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    return post_run_dev(post, net->out_f32[11].p, net->out_f32[10].p, 0, n, H / 8, W / 8, thresh, st);
-}
-
-int b200pose_infer(b200pose_net* net, b200pose_post* post, const float* input, int input_on_device, int n, int H, int W,
-                   int mode, float thresh, void* cuda_stream) {
-    return infer_impl(net, post, input, 0, input_on_device, n, H, W, mode, thresh, cuda_stream);
-}
-int b200pose_infer_u8(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device, int n,
-                      int H, int W, int mode, float thresh, void* cuda_stream) {
-    return infer_impl(net, post, images, 1, input_on_device, n, H, W, mode, thresh, cuda_stream);
-}
-
 // ------------------------------------------------------------------------------------------------ flip TTA
 static int flip_merge_dev(const float* nh, const float* fh, const float* np_, const float* fp, int layout, int n, int h,
                           int w, float* oh, float* op, cudaStream_t st, const int* ext = nullptr) {
@@ -1233,9 +1155,7 @@ static int flip_merge_dev(const float* nh, const float* fh, const float* np_, co
         e = tta_flip_merge(nh, fh, oh, n, kHeat, h, w, 1, (long)w * kHeat, kHeat, ext, st);
         if (e == cudaSuccess) e = tta_flip_merge(np_, fp, op, n, kPaf, h, w, 1, (long)w * kPaf, kPaf, ext, st);
     }
-    if (e != cudaSuccess) return fail("tta_flip_merge: %s", cudaGetErrorString(e));
-    g_launches += 2;
-    return 0;
+    return launched(e, "tta_flip_merge", 2);
 }
 
 int b200pose_flip_merge(b200pose_post* p, const float* normal_heat, const float* flipped_heat, const float* normal_paf,
@@ -1264,52 +1184,85 @@ int b200pose_flip_merge(b200pose_post* p, const float* normal_heat, const float*
     return 0;
 }
 
-static int infer_flip_impl(b200pose_net* net, b200pose_post* post, const void* input, int in_u8, int input_on_device,
-                           int n, int H, int W, int mode, float thresh, void* cuda_stream) {
+// ------------------------------------------------------------------------------------------------ fused inference
+// Every fused entry point checks its handles, stages its frames (with their mirror images when flip), runs the
+// forward pass and finishes with finish_infer.
+
+static int check_infer(const b200pose_net* net, const b200pose_post* post) {
     if (!net || !post) return fail("null handle");
     if (!net->finalized) return fail("net not finalized");
     if (net->device != post->device) return fail("net and post live on different devices");
-    if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
-    if (n > post->pb.batch_cap) return fail("batch %d exceeds post batch_cap %d", n, post->pb.batch_cap);
-    CU(cudaSetDevice(net->device));
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    // the 2n batch [frames | mirrored frames] is assembled in the net's staging buffer
-    const size_t elems = (size_t)n * 3 * H * W;
-    const cudaMemcpyKind kind = input_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const void* d_batch;
-    cudaError_t e;
-    if (in_u8) {
-        CU(net->in_stage_u8.ensure(2 * elems));
-        CU(cudaMemcpyAsync(net->in_stage_u8.p, input, elems, kind, st));
-        e = tta_mirror_u8hwc(net->in_stage_u8.p, net->in_stage_u8.p + elems, n, H, W, st);
-        d_batch = net->in_stage_u8.p;
-    } else {
-        CU(net->in_stage.ensure(2 * elems));
-        CU(cudaMemcpyAsync(net->in_stage.p, input, elems * 4, kind, st));
-        e = tta_mirror_f32(net->in_stage.p, net->in_stage.p + elems, (long)n * 3, H, W, st);
-        d_batch = net->in_stage.p;
-    }
-    if (e != cudaSuccess) return fail("tta_mirror: %s", cudaGetErrorString(e));
-    ++g_launches;
-    int rc = net_forward_impl(net, d_batch, in_u8, 1, 2 * n, H, W, mode, nullptr, 1, st, false);
-    if (rc) return rc;
-    const int h = H / 8, w = W / 8;
-    const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
-    CU(post->d_heat.ensure(eh));
-    CU(post->d_paf.ensure(ep));
-    rc = flip_merge_dev(net->out_f32[11].p, net->out_f32[11].p + eh, net->out_f32[10].p, net->out_f32[10].p + ep, 0, n, h,
-                        w, post->d_heat.p, post->d_paf.p, st);
-    if (rc) return rc;
-    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h, w, thresh, st);
+    return 0;
 }
 
+// Flip TTA: merges the last forward's 2n images [frames | mirrors] of stage-6 maps into n maps at oh / op.
+static int merge_last_flip(const b200pose_net* net, int n, float* oh, float* op, cudaStream_t st) {
+    const int h = net->last.H / 8, w = net->last.W / 8;
+    const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
+    const float *heat = net->out_f32[11].p, *paf = net->out_f32[10].p;
+    return flip_merge_dev(heat, heat + eh, paf, paf + ep, 0, n, h, w, oh, op, st, net->last.ext);
+}
+
+// Post-processing of the n frames of the last forward (flip: merged from its 2n images into post->d_heat / d_paf).
+static int finish_infer(const b200pose_net* net, b200pose_post* post, int n, int flip, float thresh, cudaStream_t st) {
+    const int h = net->last.H / 8, w = net->last.W / 8;
+    const float *heat = net->out_f32[11].p, *paf = net->out_f32[10].p;
+    if (flip) {
+        CU(post->d_heat.ensure((size_t)n * kHeat * h * w));
+        CU(post->d_paf.ensure((size_t)n * kPaf * h * w));
+        if (int rc = merge_last_flip(net, n, post->d_heat.p, post->d_paf.p, st)) return rc;
+        heat = post->d_heat.p;
+        paf = post->d_paf.p;
+    }
+    return post_run_dev(post, heat, paf, 0, n, h, w, thresh, st, net->last.ext);
+}
+
+static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input, int in_u8, int input_on_device, int n,
+                      int H, int W, int mode, float thresh, int flip, void* cuda_stream) {
+    if (int rc = check_infer(net, post)) return rc;
+    if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
+    if (int rc = check_batch(post, n)) return rc;
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (flip) {   // the 2n batch [frames | mirrored frames] is assembled in the net's staging buffer
+        const size_t elems = (size_t)n * 3 * H * W;
+        const cudaMemcpyKind kind = input_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+        cudaError_t e;
+        if (in_u8) {
+            CU(net->in_stage_u8.ensure(2 * elems));
+            CU(cudaMemcpyAsync(net->in_stage_u8.p, input, elems, kind, st));
+            e = tta_mirror_u8hwc(net->in_stage_u8.p, net->in_stage_u8.p + elems, n, H, W, st);
+            input = net->in_stage_u8.p;
+        } else {
+            CU(net->in_stage.ensure(2 * elems));
+            CU(cudaMemcpyAsync(net->in_stage.p, input, elems * 4, kind, st));
+            e = tta_mirror_f32(net->in_stage.p, net->in_stage.p + elems, (long)n * 3, H, W, st);
+            input = net->in_stage.p;
+        }
+        if (launched(e, "tta_mirror")) return 1;
+        input_on_device = 1;
+    }
+    // host input is staged asynchronously: the caller keeps it alive until b200pose_post_sync()
+    if (int rc = net_forward_impl(net, input, in_u8, input_on_device, flip ? 2 * n : n, H, W, mode, nullptr, 1, st, false))
+        return rc;
+    return finish_infer(net, post, n, flip, thresh, st);
+}
+
+int b200pose_infer(b200pose_net* net, b200pose_post* post, const float* input, int input_on_device, int n, int H, int W,
+                   int mode, float thresh, void* cuda_stream) {
+    return infer_impl(net, post, input, 0, input_on_device, n, H, W, mode, thresh, 0, cuda_stream);
+}
+int b200pose_infer_u8(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device, int n,
+                      int H, int W, int mode, float thresh, void* cuda_stream) {
+    return infer_impl(net, post, images, 1, input_on_device, n, H, W, mode, thresh, 0, cuda_stream);
+}
 int b200pose_infer_flip(b200pose_net* net, b200pose_post* post, const float* input, int input_on_device, int n, int H,
                         int W, int mode, float thresh, void* cuda_stream) {
-    return infer_flip_impl(net, post, input, 0, input_on_device, n, H, W, mode, thresh, cuda_stream);
+    return infer_impl(net, post, input, 0, input_on_device, n, H, W, mode, thresh, 1, cuda_stream);
 }
 int b200pose_infer_u8_flip(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device,
                            int n, int H, int W, int mode, float thresh, void* cuda_stream) {
-    return infer_flip_impl(net, post, images, 1, input_on_device, n, H, W, mode, thresh, cuda_stream);
+    return infer_impl(net, post, images, 1, input_on_device, n, H, W, mode, thresh, 1, cuda_stream);
 }
 
 // ------------------------------------------------------------------------------------------------ crop_with_factor
@@ -1344,75 +1297,60 @@ int b200pose_net_crop_with_factor(b200pose_net* net, const unsigned char* images
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     const size_t raw = (size_t)n * src_h * src_w * 3, outb = (size_t)n * g.pad_h * g.pad_w * 3;
-    const unsigned char* d_in = images;
-    if (!images_on_device) {
-        CU(net->raw_stage.ensure(raw));
-        CU(cudaMemcpyAsync(net->raw_stage.p, images, raw, cudaMemcpyHostToDevice, st));
-        d_in = net->raw_stage.p;
-    }
+    const unsigned char* d_in;
+    if (int rc = stage_raw(net, images, images_on_device, raw, 0, st, &d_in)) return rc;
     unsigned char* d_out = out;
     if (!out_on_device) {
         CU(net->in_stage_u8.ensure(outb));
         d_out = net->in_stage_u8.p;
     }
-    cudaError_t e = crop_with_factor_launch(d_in, d_out, n, src_h, src_w, g, st);
-    if (e != cudaSuccess) return fail("crop_with_factor_launch: %s", cudaGetErrorString(e));
-    ++g_launches;
+    if (launched(crop_with_factor_launch(d_in, d_out, n, src_h, src_w, g, st), "crop_with_factor_launch")) return 1;
     if (!out_on_device) CU(cudaMemcpyAsync(out, d_out, outb, cudaMemcpyDeviceToHost, st));
     if (!images_on_device || !out_on_device) CU(cudaStreamSynchronize(st));
     return 0;
 }
 
+// Raw frames of one size on the device (uniform fused entry points), their mirror images behind them when flip: mirrored
+// RAW frames, so that the padding of both orientations ends up on the right, as for the reference.
+static int stage_raw_uniform(b200pose_net* net, const unsigned char* images, int on_device, int n, int src_h, int src_w,
+                             int flip, cudaStream_t st, const unsigned char** d_raw) {
+    const size_t raw = (size_t)n * src_h * src_w * 3;
+    if (int rc = stage_raw(net, images, on_device, raw, flip, st, d_raw)) return rc;
+    if (flip && launched(tta_mirror_u8hwc(net->raw_stage.p, net->raw_stage.p + raw, n, src_h, src_w, st), "tta_mirror"))
+        return 1;
+    return 0;
+}
+
+// crop_with_factor of nimg raw frames into net->in_stage_u8, then the forward pass on them
+static int crop_and_forward(b200pose_net* net, const unsigned char* d_raw, int nimg, int src_h, int src_w,
+                            const CropGeom& g, int mode, cudaStream_t st) {
+    CU(net->in_stage_u8.ensure((size_t)nimg * g.pad_h * g.pad_w * 3));
+    if (launched(crop_with_factor_launch(d_raw, net->in_stage_u8.p, nimg, src_h, src_w, g, st), "crop_with_factor_launch"))
+        return 1;
+    return net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, g.pad_h, g.pad_w, mode, nullptr, 1, st, false);
+}
+
 int b200pose_infer_raw_u8(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device, int n,
                           int src_h, int src_w, int dest_size, int factor, int mode, float thresh, int flip,
                           void* cuda_stream) {
-    if (!net || !post) return fail("null handle");
-    if (!net->finalized) return fail("net not finalized");
-    if (net->device != post->device) return fail("net and post live on different devices");
+    if (int rc = check_infer(net, post)) return rc;
     if (!images) return fail("infer_raw: null pointer");
-    if (n > post->pb.batch_cap) return fail("batch %d exceeds post batch_cap %d", n, post->pb.batch_cap);
+    if (int rc = check_batch(post, n)) return rc;
     CropGeom g;
     if (int rc = crop_check(n, src_h, src_w, dest_size, factor, &g)) return rc;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    const int nimg = flip ? 2 * n : n, H = g.pad_h, W = g.pad_w;
-    const size_t raw = (size_t)n * src_h * src_w * 3;
     // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
-    const unsigned char* d_raw = images;
-    if (!input_on_device || flip) {
-        CU(net->raw_stage.ensure(raw * (flip ? 2 : 1)));
-        CU(cudaMemcpyAsync(net->raw_stage.p, images, raw, input_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-        d_raw = net->raw_stage.p;
-    }
-    cudaError_t e;
-    if (flip) {   // mirrored RAW frames: the padding of both orientations ends up on the right, as for the reference
-        e = tta_mirror_u8hwc(net->raw_stage.p, net->raw_stage.p + raw, n, src_h, src_w, st);
-        if (e != cudaSuccess) return fail("tta_mirror: %s", cudaGetErrorString(e));
-        ++g_launches;
-    }
-    CU(net->in_stage_u8.ensure((size_t)nimg * H * W * 3));
-    e = crop_with_factor_launch(d_raw, net->in_stage_u8.p, nimg, src_h, src_w, g, st);
-    if (e != cudaSuccess) return fail("crop_with_factor_launch: %s", cudaGetErrorString(e));
-    ++g_launches;
-    int rc = net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, H, W, mode, nullptr, 1, st, false);
-    if (rc) return rc;
-    const int h = H / 8, w = W / 8;
-    if (!flip) return post_run_dev(post, net->out_f32[11].p, net->out_f32[10].p, 0, n, h, w, thresh, st);
-    const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
-    CU(post->d_heat.ensure(eh));
-    CU(post->d_paf.ensure(ep));
-    rc = flip_merge_dev(net->out_f32[11].p, net->out_f32[11].p + eh, net->out_f32[10].p, net->out_f32[10].p + ep, 0, n, h,
-                        w, post->d_heat.p, post->d_paf.p, st);
-    if (rc) return rc;
-    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h, w, thresh, st);
+    const unsigned char* d_raw;
+    if (int rc = stage_raw_uniform(net, images, input_on_device, n, src_h, src_w, flip, st, &d_raw)) return rc;
+    if (int rc = crop_and_forward(net, d_raw, flip ? 2 * n : n, src_h, src_w, g, mode, st)) return rc;
+    return finish_infer(net, post, n, flip, thresh, st);
 }
 
 int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device,
                                   int n, const int* src_hw, int dest_size, int factor, int mode, float thresh, int flip,
                                   void* cuda_stream) {
-    if (!net || !post) return fail("null handle");
-    if (!net->finalized) return fail("net not finalized");
-    if (net->device != post->device) return fail("net and post live on different devices");
+    if (int rc = check_infer(net, post)) return rc;
     if (!images || !src_hw) return fail("infer_raw_ragged: null pointer");
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
     const int nimg = flip ? 2 * n : n;
@@ -1445,60 +1383,30 @@ int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const u
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
-    const unsigned char* d_raw = images;
-    if (!input_on_device || flip) {
-        CU(net->raw_stage.ensure((size_t)raw * (flip ? 2 : 1)));
-        CU(cudaMemcpyAsync(net->raw_stage.p, images, (size_t)raw, input_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-        d_raw = net->raw_stage.p;
-    }
+    const unsigned char* d_raw;
+    if (int rc = stage_raw(net, images, input_on_device, (size_t)raw, flip, st, &d_raw)) return rc;
     if (int rc = upload_frames(net, tab, st)) return rc;
-    if (flip) {       // the mirror reads the first n entries of the table (the originals)
-        cudaError_t e = tta_mirror_u8hwc_ragged(net->raw_stage.p, net->raw_stage.p + raw, net->d_frames.p, n, (long)max_bytes, st);
-        if (e != cudaSuccess) return fail("tta_mirror_u8hwc_ragged: %s", cudaGetErrorString(e));
-        ++g_launches;
-    }
-    if (int rc = place_ragged_frames(net, d_raw, nimg, Hc, Wc, st)) return rc;
-    if (int rc = upload_ext(net, ext, st)) return rc;
-    if (int rc = net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, Hc, Wc, mode, nullptr, 1, st, false, net->d_ext))
-        return rc;
-    const int h = Hc / 8, w = Wc / 8;
-    if (!flip) return post_run_dev(post, net->out_f32[11].p, net->out_f32[10].p, 0, n, h, w, thresh, st, net->d_ext);
-    const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
-    CU(post->d_heat.ensure(eh));
-    CU(post->d_paf.ensure(ep));
-    if (int rc = flip_merge_dev(net->out_f32[11].p, net->out_f32[11].p + eh, net->out_f32[10].p, net->out_f32[10].p + ep, 0, n,
-                                h, w, post->d_heat.p, post->d_paf.p, st, net->d_ext))
-        return rc;
-    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h, w, thresh, st, net->d_ext);
+    // the mirror reads the first n entries of the table (the originals)
+    if (flip && launched(tta_mirror_u8hwc_ragged(net->raw_stage.p, net->raw_stage.p + raw, net->d_frames.p, n, (long)max_bytes, st),
+                         "tta_mirror_u8hwc_ragged"))
+        return 1;
+    if (int rc = ragged_forward(net, d_raw, nimg, Hc, Wc, ext, mode, nullptr, 1, st, false)) return rc;
+    return finish_infer(net, post, n, flip, thresh, st);
 }
 
 int b200pose_infer_raw_u8_multiscale(b200pose_net* net, b200pose_post* post, const unsigned char* images,
                                      int input_on_device, int n, int src_h, int src_w, int base_size, int factor,
                                      const double* scales, int n_scales, int mode, float thresh, int flip,
                                      void* cuda_stream) {
-    if (!net || !post) return fail("null handle");
-    if (!net->finalized) return fail("net not finalized");
-    if (net->device != post->device) return fail("net and post live on different devices");
+    if (int rc = check_infer(net, post)) return rc;
     if (!images || !scales || n_scales < 1 || n_scales > 16) return fail("infer_multiscale: bad arguments");
-    if (n > post->pb.batch_cap) return fail("batch %d exceeds post batch_cap %d", n, post->pb.batch_cap);
+    if (int rc = check_batch(post, n)) return rc;
     CropGeom base;
     if (int rc = crop_check(n, src_h, src_w, base_size, factor, &base)) return rc;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    const int nimg = flip ? 2 * n : n;
-    const size_t raw = (size_t)n * src_h * src_w * 3;
-    const unsigned char* d_raw = images;
-    if (!input_on_device || flip) {
-        CU(net->raw_stage.ensure(raw * (flip ? 2 : 1)));
-        CU(cudaMemcpyAsync(net->raw_stage.p, images, raw, input_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-        d_raw = net->raw_stage.p;
-    }
-    cudaError_t e;
-    if (flip) {
-        e = tta_mirror_u8hwc(net->raw_stage.p, net->raw_stage.p + raw, n, src_h, src_w, st);
-        if (e != cudaSuccess) return fail("tta_mirror: %s", cudaGetErrorString(e));
-        ++g_launches;
-    }
+    const unsigned char* d_raw;
+    if (int rc = stage_raw_uniform(net, images, input_on_device, n, src_h, src_w, flip, st, &d_raw)) return rc;
     const int h1 = base.pad_h / 8, w1 = base.pad_w / 8;
     CU(post->d_heat.ensure((size_t)n * kHeat * h1 * w1));
     CU(post->d_paf.ensure((size_t)n * kPaf * h1 * w1));
@@ -1506,28 +1414,21 @@ int b200pose_infer_raw_u8_multiscale(b200pose_net* net, b200pose_post* post, con
         const int dest = (int)((double)base_size * scales[k]);       // Python: int(base_size * s)
         CropGeom g;
         if (int rc = crop_check(n, src_h, src_w, dest, factor, &g)) return rc;
-        const int H = g.pad_h, W = g.pad_w, h = H / 8, w = W / 8;
-        CU(net->in_stage_u8.ensure((size_t)nimg * H * W * 3));
-        e = crop_with_factor_launch(d_raw, net->in_stage_u8.p, nimg, src_h, src_w, g, st);
-        if (e != cudaSuccess) return fail("crop_with_factor_launch: %s", cudaGetErrorString(e));
-        ++g_launches;
-        if (int rc = net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, H, W, mode, nullptr, 1, st, false)) return rc;
+        if (int rc = crop_and_forward(net, d_raw, flip ? 2 * n : n, src_h, src_w, g, mode, st)) return rc;
+        const int h = g.pad_h / 8, w = g.pad_w / 8;
         const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
         const float *s_heat = net->out_f32[11].p, *s_paf = net->out_f32[10].p;
         if (flip) {
             CU(post->tta_out.ensure(eh + ep));
-            if (int rc = flip_merge_dev(s_heat, s_heat + eh, s_paf, s_paf + ep, 0, n, h, w, post->tta_out.p,
-                                        post->tta_out.p + eh, st))
-                return rc;
+            if (int rc = merge_last_flip(net, n, post->tta_out.p, post->tta_out.p + eh, st)) return rc;
             s_heat = post->tta_out.p;
             s_paf = post->tta_out.p + eh;
         }
         const float div = (k == n_scales - 1) ? (float)n_scales : 0.f;
-        e = resize_cubic_accum_launch(s_heat, post->d_heat.p, (long)n * kHeat, h, w, h1, w1, k == 0, div, st);
+        cudaError_t e = resize_cubic_accum_launch(s_heat, post->d_heat.p, (long)n * kHeat, h, w, h1, w1, k == 0, div, st);
         if (e == cudaSuccess)
             e = resize_cubic_accum_launch(s_paf, post->d_paf.p, (long)n * kPaf, h, w, h1, w1, k == 0, div, st);
-        if (e != cudaSuccess) return fail("resize_cubic_accum_launch: %s", cudaGetErrorString(e));
-        g_launches += 2;
+        if (launched(e, "resize_cubic_accum_launch", 2)) return 1;
     }
     return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h1, w1, thresh, st);
 }
