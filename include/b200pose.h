@@ -137,6 +137,9 @@ int b200pose_post_debug(b200pose_post* post, unsigned long long* out, int n, int
 /* Test hook: sorts n 64-bit candidate keys (high word = ~score bits, low word = pair index) on the device with the
  * product's sorting kernels - libstdc++'s std::sort order (pafprocess.cpp:97), ties included.  Host pointers. */
 int b200pose_post_debug_sort(b200pose_post* post, const unsigned long long* keys, int n, unsigned long long* out);
+/* Test hook: waits for the device, then copies the first heat_floats / paf_floats floats of the maps the last flip or
+ * multi-scale run averaged and post-processed (NCHW fp32; a ragged run's at its canvas pitch) to host memory. */
+int b200pose_post_debug_maps(b200pose_post* post, float* heat, long heat_floats, float* paf, long paf_floats);
 /* OR of the status words of every image of every run since the last reset (sticky accumulator kept on the device):
  * with runs in flight a caller reads only some results back; this proves that no run at all overflowed a capacity
  * (the reference's std::vectors grow without bound, pafprocess.cpp:24-44, so an overflow is a divergence).  < 0 on error. */
@@ -219,6 +222,17 @@ int b200pose_infer_raw_u8_multiscale(b200pose_net* net, b200pose_post* post, con
                                      int input_on_device, int n, int src_h, int src_w, int base_size, int factor,
                                      const double* scales, int n_scales, int mode, float thresh, int flip,
                                      void* cuda_stream);
+/* b200pose_infer_raw_u8_multiscale for n raw frames of DIFFERENT sizes, packed back to back as for
+ * b200pose_infer_raw_u8_ragged (frame i: src_hw[2i] x src_hw[2i+1] x 3 bytes).  Every scale runs as one ragged batch
+ * on the canvas of that scale's largest padded frame; each frame's maps are resized from its own extent at that scale
+ * to its own base grid and averaged on the canvas of the base padded sizes (+0 outside each frame).  Per frame, person
+ * rows and peaks are those b200pose_infer_raw_u8_multiscale gives for that frame alone, in pixels of its own padded
+ * base frame.  1 <= n_scales <= 16, n <= the post object's batch_cap, and with flip 2n <= 1024.  Fetched like
+ * b200pose_infer's. */
+int b200pose_infer_raw_u8_multiscale_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images,
+                                            int input_on_device, int n, const int* src_hw, int base_size, int factor,
+                                            const double* scales, int n_scales, int mode, float thresh, int flip,
+                                            void* cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument

@@ -45,6 +45,7 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_post_debug": ([vp, vp, ci, ci], ci),
     "b200pose_post_status_accum": ([vp, ci], ci),
     "b200pose_post_debug_sort": ([vp, vp, ci, vp], ci),
+    "b200pose_post_debug_maps": ([vp, vp, cl, vp, cl], ci),
     "b200pose_post_num_humans": ([vp, ci], ci),
     "b200pose_post_status": ([vp, ci], ci),
     "b200pose_post_get_humans": ([vp, ci, vp, ci], ci),
@@ -60,6 +61,8 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_infer_raw_u8_multiscale": ([vp, vp, vp, ci, ci, ci, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf,
                                           ci, vp], ci),
     "b200pose_infer_raw_u8_ragged": ([vp, vp, vp, ci, ci, vp, ci, ci, ci, cf, ci, vp], ci),
+    "b200pose_infer_raw_u8_multiscale_ragged": ([vp, vp, vp, ci, ci, vp, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci,
+                                                 cf, ci, vp], ci),
     "process_paf": ([ci, ci, ci, vp, ci, ci, ci, vp, ci, ci, ci, vp], ci),
     "get_num_humans": ([], ci),
     "get_part_cid": ([ci, ci], ci),

@@ -274,6 +274,10 @@ struct b200pose_post {
     // extents of a ragged run, slot = run parity: the peaks / limbs of run i on the second stream still read them while
     // run i+1 rewrites the net's table
     int* d_ext[2] = {nullptr, nullptr};
+    // ragged multi-scale averaging: the frames' base extents (the net's table holds the last scale's) and the resize
+    // geometry of every (scale, frame)
+    DevBuf<int> ms_ext;
+    DevBuf<RaggedResize> ms_resize;
 };
 
 namespace {
@@ -947,6 +951,7 @@ void b200pose_post_destroy(b200pose_post* p) {
     p->d_heat.release(); p->d_paf.release();
     p->tta_in.release(); p->tta_out.release();
     p->ov_maps[0].release(); p->ov_maps[1].release();
+    p->ms_ext.release(); p->ms_resize.release();
     if (p->ev_maps) cudaEventDestroy(p->ev_maps);
     for (int b = 0; b < 2; ++b) if (p->ev_ld[b]) cudaEventDestroy(p->ev_ld[b]);
     for (int b = 0; b < 2; ++b) {
@@ -1097,6 +1102,17 @@ int b200pose_post_debug(b200pose_post* p, unsigned long long* out, int n, int re
     if (!p || n > 16) return -1;
     if (cudaMemcpy(out, p->pb.dbg, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
     if (reset) cudaMemset(p->pb.dbg, 0, 16 * sizeof(unsigned long long));
+    return 0;
+}
+
+int b200pose_post_debug_maps(b200pose_post* p, float* heat, long heat_floats, float* paf, long paf_floats) {
+    if (!p || !heat || !paf) return fail("debug_maps: null pointer");
+    if (heat_floats < 0 || paf_floats < 0 || (size_t)heat_floats > p->d_heat.n || (size_t)paf_floats > p->d_paf.n)
+        return fail("debug_maps: %ld / %ld floats asked, %zu / %zu held", heat_floats, paf_floats, p->d_heat.n, p->d_paf.n);
+    CU(cudaSetDevice(p->device));
+    CU(cudaDeviceSynchronize());
+    CU(cudaMemcpy(heat, p->d_heat.p, (size_t)heat_floats * 4, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(paf, p->d_paf.p, (size_t)paf_floats * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
 static int post_ready(b200pose_post* p, int img) {
@@ -1347,6 +1363,52 @@ int b200pose_infer_raw_u8(b200pose_net* net, b200pose_post* post, const unsigned
     return finish_infer(net, post, n, flip, thresh, st);
 }
 
+// The ragged crop of n raw frames packed back to back (src_hw: their sizes) for dest_size: frame table, padded extents
+// and canvas, the frames' total and largest size in bytes.  flip: the mirrored frames follow the originals, in the
+// staging buffer and in both tables.
+struct RaggedCrop {
+    std::vector<RaggedFrame> tab;
+    std::vector<int> ext;
+    int Hc = 0, Wc = 0;
+    long long raw = 0, max_bytes = 0;
+};
+
+static int ragged_crop(int n, const int* src_hw, int dest_size, int factor, int flip, RaggedCrop* c) {
+    const int nimg = flip ? 2 * n : n;
+    if (nimg > kMaxRagged) return fail("ragged batch: %d images (at most %d)", nimg, kMaxRagged);
+    c->tab.assign(nimg, RaggedFrame{});
+    c->ext.assign(2 * nimg, 0);
+    for (int i = 0; i < n; ++i) {
+        RaggedFrame& f = c->tab[i];
+        f.src_h = src_hw[2 * i];
+        f.src_w = src_hw[2 * i + 1];
+        if (int rc = crop_check(1, f.src_h, f.src_w, dest_size, factor, &f.g)) return rc;
+        f.off = c->raw;
+        const long long b = (long long)f.src_h * f.src_w * 3;
+        c->raw += b;
+        if (b > c->max_bytes) c->max_bytes = b;
+        c->ext[2 * i] = f.g.pad_h;
+        c->ext[2 * i + 1] = f.g.pad_w;
+        if (f.g.pad_h > c->Hc) c->Hc = f.g.pad_h;
+        if (f.g.pad_w > c->Wc) c->Wc = f.g.pad_w;
+    }
+    for (int i = 0; i < n && flip; ++i) {      // mirrored raw frames follow the originals in the staging buffer
+        c->tab[n + i] = c->tab[i];
+        c->tab[n + i].off += c->raw;
+        c->ext[2 * (n + i)] = c->ext[2 * i];
+        c->ext[2 * (n + i) + 1] = c->ext[2 * i + 1];
+    }
+    if ((long)c->Hc * c->Wc > (1L << 28)) return fail("infer_raw_ragged: canvas too large");
+    return 0;
+}
+
+// With flip: mirrors the n raw frames of the staging buffer behind them.  Reads the first n entries of net->d_frames.
+static int mirror_raw_ragged(b200pose_net* net, int n, const RaggedCrop& c, cudaStream_t st) {
+    return launched(tta_mirror_u8hwc_ragged(net->raw_stage.p, net->raw_stage.p + c.raw, net->d_frames.p, n,
+                                            (long)c.max_bytes, st),
+                    "tta_mirror_u8hwc_ragged");
+}
+
 int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device,
                                   int n, const int* src_hw, int dest_size, int factor, int mode, float thresh, int flip,
                                   void* cuda_stream) {
@@ -1354,43 +1416,16 @@ int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const u
     if (!images || !src_hw) return fail("infer_raw_ragged: null pointer");
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
     const int nimg = flip ? 2 * n : n;
-    if (nimg > kMaxRagged) return fail("ragged batch: %d images (at most %d)", nimg, kMaxRagged);
-    std::vector<RaggedFrame> tab(nimg);
-    std::vector<int> ext(2 * nimg);
-    long long raw = 0, max_bytes = 0;
-    int Hc = 0, Wc = 0;
-    for (int i = 0; i < n; ++i) {
-        RaggedFrame& f = tab[i];
-        f.src_h = src_hw[2 * i];
-        f.src_w = src_hw[2 * i + 1];
-        if (int rc = crop_check(1, f.src_h, f.src_w, dest_size, factor, &f.g)) return rc;
-        f.off = raw;
-        const long long b = (long long)f.src_h * f.src_w * 3;
-        raw += b;
-        if (b > max_bytes) max_bytes = b;
-        ext[2 * i] = f.g.pad_h;
-        ext[2 * i + 1] = f.g.pad_w;
-        if (f.g.pad_h > Hc) Hc = f.g.pad_h;
-        if (f.g.pad_w > Wc) Wc = f.g.pad_w;
-    }
-    for (int i = 0; i < n && flip; ++i) {      // mirrored raw frames follow the originals in the staging buffer
-        tab[n + i] = tab[i];
-        tab[n + i].off += raw;
-        ext[2 * (n + i)] = ext[2 * i];
-        ext[2 * (n + i) + 1] = ext[2 * i + 1];
-    }
-    if ((long)Hc * Wc > (1L << 28)) return fail("infer_raw_ragged: canvas too large");
+    RaggedCrop c;
+    if (int rc = ragged_crop(n, src_hw, dest_size, factor, flip, &c)) return rc;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
     const unsigned char* d_raw;
-    if (int rc = stage_raw(net, images, input_on_device, (size_t)raw, flip, st, &d_raw)) return rc;
-    if (int rc = upload_frames(net, tab, st)) return rc;
-    // the mirror reads the first n entries of the table (the originals)
-    if (flip && launched(tta_mirror_u8hwc_ragged(net->raw_stage.p, net->raw_stage.p + raw, net->d_frames.p, n, (long)max_bytes, st),
-                         "tta_mirror_u8hwc_ragged"))
-        return 1;
-    if (int rc = ragged_forward(net, d_raw, nimg, Hc, Wc, ext, mode, nullptr, 1, st, false)) return rc;
+    if (int rc = stage_raw(net, images, input_on_device, (size_t)c.raw, flip, st, &d_raw)) return rc;
+    if (int rc = upload_frames(net, c.tab, st)) return rc;
+    if (flip && mirror_raw_ragged(net, n, c, st)) return 1;
+    if (int rc = ragged_forward(net, d_raw, nimg, c.Hc, c.Wc, c.ext, mode, nullptr, 1, st, false)) return rc;
     return finish_infer(net, post, n, flip, thresh, st);
 }
 
@@ -1431,6 +1466,65 @@ int b200pose_infer_raw_u8_multiscale(b200pose_net* net, b200pose_post* post, con
         if (launched(e, "resize_cubic_accum_launch", 2)) return 1;
     }
     return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h1, w1, thresh, st);
+}
+
+int b200pose_infer_raw_u8_multiscale_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images,
+                                            int input_on_device, int n, const int* src_hw, int base_size, int factor,
+                                            const double* scales, int n_scales, int mode, float thresh, int flip,
+                                            void* cuda_stream) {
+    if (int rc = check_infer(net, post)) return rc;
+    if (!images || !src_hw || !scales || n_scales < 1 || n_scales > 16) return fail("infer_multiscale_ragged: bad arguments");
+    if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
+    // every scale's geometry first: an invalid frame size fails before anything is enqueued
+    RaggedCrop base;
+    if (int rc = ragged_crop(n, src_hw, base_size, factor, 0, &base)) return rc;
+    std::vector<RaggedCrop> sc(n_scales);
+    std::vector<RaggedResize> rz((size_t)n_scales * n);
+    for (int k = 0; k < n_scales; ++k) {
+        const int dest = (int)((double)base_size * scales[k]);       // Python: int(base_size * s)
+        if (int rc = ragged_crop(n, src_hw, dest, factor, flip, &sc[k])) return rc;
+        for (int i = 0; i < n; ++i)
+            rz[(size_t)k * n + i] = ragged_resize(sc[k].ext[2 * i] / 8, sc[k].ext[2 * i + 1] / 8, base.ext[2 * i] / 8,
+                                                  base.ext[2 * i + 1] / 8);
+    }
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
+    const unsigned char* d_raw;
+    if (int rc = stage_raw(net, images, input_on_device, (size_t)base.raw, flip, st, &d_raw)) return rc;
+    if (flip) {      // the sources and offsets of the frame table are those of every scale
+        if (int rc = upload_frames(net, base.tab, st)) return rc;
+        if (mirror_raw_ragged(net, n, base, st)) return 1;
+    }
+    CU(post->ms_ext.ensure(base.ext.size()));
+    CU(cudaMemcpyAsync(post->ms_ext.p, base.ext.data(), base.ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CU(post->ms_resize.ensure(rz.size()));
+    CU(cudaMemcpyAsync(post->ms_resize.p, rz.data(), rz.size() * sizeof(RaggedResize), cudaMemcpyHostToDevice, st));
+    const int h1 = base.Hc / 8, w1 = base.Wc / 8;
+    CU(post->d_heat.ensure((size_t)n * kHeat * h1 * w1));
+    CU(post->d_paf.ensure((size_t)n * kPaf * h1 * w1));
+    for (int k = 0; k < n_scales; ++k) {
+        const RaggedCrop& c = sc[k];
+        if (int rc = upload_frames(net, c.tab, st)) return rc;
+        if (int rc = ragged_forward(net, d_raw, flip ? 2 * n : n, c.Hc, c.Wc, c.ext, mode, nullptr, 1, st, false)) return rc;
+        const int h = c.Hc / 8, w = c.Wc / 8;
+        const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
+        const float *s_heat = net->out_f32[11].p, *s_paf = net->out_f32[10].p;
+        if (flip) {
+            CU(post->tta_out.ensure(eh + ep));
+            if (int rc = merge_last_flip(net, n, post->tta_out.p, post->tta_out.p + eh, st)) return rc;
+            s_heat = post->tta_out.p;
+            s_paf = post->tta_out.p + eh;
+        }
+        const float div = (k == n_scales - 1) ? (float)n_scales : 0.f;
+        const RaggedResize* f = post->ms_resize.p + (size_t)k * n;
+        cudaError_t e = resize_cubic_accum_ragged_launch(s_heat, post->d_heat.p, f, n, kHeat, h, w, h1, w1, k == 0, div, st);
+        if (e == cudaSuccess)
+            e = resize_cubic_accum_ragged_launch(s_paf, post->d_paf.p, f, n, kPaf, h, w, h1, w1, k == 0, div, st);
+        if (launched(e, "resize_cubic_accum_ragged_launch", 2)) return 1;
+    }
+    // the net's extents table now holds the last scale's: post-processing reads the base extents
+    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h1, w1, thresh, st, post->ms_ext.p);
 }
 
 // ------------------------------------------------------------------------------------------------ legacy pafprocess

@@ -88,6 +88,28 @@ __global__ void __launch_bounds__(kThreads) resize_cubic_accum_kernel(const floa
     }
 }
 
+// Ragged batch: one thread per destination element of the base canvas; frame (plane / channels)'s own extents and steps.
+__global__ void __launch_bounds__(kThreads) resize_cubic_accum_ragged_kernel(const float* __restrict__ src,
+                                                                             float* __restrict__ dst,
+                                                                             const RaggedResize* __restrict__ frames,
+                                                                             long planes, int channels, int shc, int swc,
+                                                                             int dhc, int dwc, int first, float divide_by) {
+    const long per = (long)dhc * dwc, total = planes * per;
+    for (long i = blockIdx.x * (long)kThreads + threadIdx.x; i < total; i += (long)gridDim.x * kThreads) {
+        const long plane = i / per;
+        const int q = (int)(i - plane * per);
+        const int y = q / dwc, x = q - y * dwc;
+        const RaggedResize f = frames[plane / channels];
+        float v = 0.f;
+        if (y < f.dh && x < f.dw) {
+            v = rs_cubic_ragged_at(src + plane * (long)shc * swc, swc, f, y, x);
+            if (!first) v = __fadd_rn(dst[i], v);
+            if (divide_by > 0.f) v = __fdiv_rn(v, divide_by);
+        }
+        dst[i] = v;
+    }
+}
+
 }  // namespace
 
 cudaError_t resize_cubic_accum_launch(const float* src, float* dst, long planes, int src_h, int src_w, int dst_h,
@@ -98,6 +120,18 @@ cudaError_t resize_cubic_accum_launch(const float* src, float* dst, long planes,
     if (b > 132L * 8) b = 132L * 8;
     resize_cubic_accum_kernel<<<(unsigned)b, kThreads, 0, s>>>(src, dst, planes, src_h, src_w, dst_h, dst_w,
                                                              rs_step(dst_h, src_h), rs_step(dst_w, src_w), first, divide_by);
+    return cudaGetLastError();
+}
+
+cudaError_t resize_cubic_accum_ragged_launch(const float* src, float* dst, const RaggedResize* frames, int n, int channels,
+                                             int src_hc, int src_wc, int dst_hc, int dst_wc, int first, float divide_by,
+                                             cudaStream_t s) {
+    if (n < 1 || channels < 1 || src_hc < 1 || src_wc < 1 || dst_hc < 1 || dst_wc < 1) return cudaErrorInvalidValue;
+    const long planes = (long)n * channels, total = planes * dst_hc * dst_wc;
+    long b = (total + kThreads - 1) / kThreads;
+    if (b > 132L * 8) b = 132L * 8;
+    resize_cubic_accum_ragged_kernel<<<(unsigned)b, kThreads, 0, s>>>(src, dst, frames, planes, channels, src_hc, src_wc,
+                                                                    dst_hc, dst_wc, first, divide_by);
     return cudaGetLastError();
 }
 

@@ -17,6 +17,13 @@ cudaError_t crop_with_factor_launch(const unsigned char* in, unsigned char* out,
 cudaError_t resize_cubic_accum_launch(const float* src, float* dst, long planes, int src_h, int src_w, int dst_h,
                                       int dst_w, int first, float divide_by, cudaStream_t s);
 
+// Ragged batch of n frames: src [n, channels, src_hc, src_wc] -> dst [n, channels, dst_hc, dst_wc] (canvas pitches);
+// frames[i] (device) gives frame i's extent at both resolutions.  Inside frame i's destination extent the running sum as
+// above, every other element of the destination canvas is written +0.
+cudaError_t resize_cubic_accum_ragged_launch(const float* src, float* dst, const RaggedResize* frames, int n, int channels,
+                                             int src_hc, int src_wc, int dst_hc, int dst_wc, int first, float divide_by,
+                                             cudaStream_t s);
+
 // One frame of a ragged batch (DESIGN.md §1): uint8 HWC source at byte offset `off`, and its crop_with_factor geometry
 // (g.pad_h == 0: the source is an already cropped network input, copied unchanged).
 struct RaggedFrame {

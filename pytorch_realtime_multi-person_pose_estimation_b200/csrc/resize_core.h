@@ -188,6 +188,24 @@ B2P_RS_HD float rs_cubic_at(const float* plane, long sy, long sx, const CubCoef&
     return o;
 }
 
+// One frame of a ragged multi-scale average (DESIGN.md 2.7): its sh x sw maps, read at the pitch of a larger source
+// canvas, resized to its own dh x dw base grid.  The taps clamp at the frame's extent, not the canvas's, so every value
+// is the one the frame resized alone gives.
+struct RaggedResize {
+    int sh, sw, dh, dw;
+    double step_y, step_x;     // rs_step(dh, sh), rs_step(dw, sw)
+};
+
+// host only
+inline RaggedResize ragged_resize(int sh, int sw, int dh, int dw) {
+    return RaggedResize{sh, sw, dh, dw, rs_step(dh, sh), rs_step(dw, sw)};
+}
+
+// Destination element (y, x) of frame f, y < f.dh and x < f.dw; `plane` is the frame's source plane, `pitch` floats per row.
+B2P_RS_HD float rs_cubic_ragged_at(const float* plane, long pitch, const RaggedResize& f, int y, int x) {
+    return rs_cubic_at(plane, pitch, 1, rs_cubic_coef(x, f.sw, f.step_x), rs_cubic_coef(y, f.sh, f.step_y));
+}
+
 struct CropGeom {
     double im_scale;       // dest_size / min(h, w)                       (im_transform.py:125)
     double step;           // 1 / im_scale: source pixels per destination pixel

@@ -346,6 +346,22 @@ class PoseEngine:
         _, _, (ph, pw) = nat.crop_geometry(src_h, src_w, base_size, factor)
         return self._remember(n, ph, pw)
 
+    def infer_raw_multiscale_ragged_async_u8(self, in_ptr, in_on_device, src_shapes, scales, base_size=368, factor=8,
+                                             thresh=0.1, flip=False, stream=0):
+        """Multi-scale (+ flip) test-time averaging of raw uint8 BGR frames of different sizes src_shapes[i] = (h_i, w_i),
+        packed back to back: every scale runs as one ragged batch, and person coordinates refer to each frame's own
+        padded base frame."""
+        n = len(src_shapes)
+        hw = (ctypes.c_int * (2 * n))(*[int(v) for s in src_shapes for v in s])
+        arr = (ctypes.c_double * len(scales))(*[float(s) for s in scales])
+        nat.check(nat.lib().b200pose_infer_raw_u8_multiscale_ragged(self.net._h, self.post._h, ctypes.c_void_p(in_ptr),
+                                                                    int(in_on_device), n, hw, int(base_size), int(factor),
+                                                                    arr, len(scales), self.mode, ctypes.c_float(thresh),
+                                                                    int(bool(flip)), ctypes.c_void_p(stream)),
+                  "b200pose_infer_raw_u8_multiscale_ragged")
+        pads = [nat.crop_geometry(h, w, base_size, factor)[2] for h, w in src_shapes]
+        return self._remember(n, [p[0] for p in pads], [p[1] for p in pads])
+
     def infer_images_arrays(self, images, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None):
         """infer_images, but per image the raw person rows (float32 [k, 73], pixel coordinates of the padded frame)."""
         return self.infer_images(images, dest_size, factor, thresh, flip, scales, _arrays=True)
@@ -353,25 +369,19 @@ class PoseEngine:
     def infer_images(self, images, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, _arrays=False):
         """images: a list of raw uint8 BGR frames of arbitrary (mixed) sizes, as cv2.imread returns them.  Returns per-image
         human lists in input order, coordinates normalised to the padded frame like paf_to_pose_cpp's.
-        Single scale: the frames run as ragged batches of at most batch_cap frames of different sizes (plan_ragged_batches;
-        a batch of one source size takes the uniform entry point).  scales: e.g. (0.5, 1.0, 1.5, 2.0) for multi-scale
-        test-time averaging around dest_size, one launch sequence per source shape."""
+        The frames run as ragged batches of at most batch_cap frames of different sizes (plan_ragged_batches on the
+        padded sizes at dest_size; a batch of one source size takes the uniform entry point).  scales: e.g.
+        (0.5, 1.0, 1.5, 2.0) for multi-scale test-time averaging around dest_size; every scale of a batch runs as one
+        device batch."""
         for im in images:
             if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
                 raise nat.B200PoseError("infer_images: expected uint8 [h,w,3] frames")
-        if scales is None:
-            pads = [nat.crop_geometry(im.shape[0], im.shape[1], dest_size, factor)[2] for im in images]
-            groups = plan_ragged_batches(pads, self.post.batch_cap)
-        else:
-            buckets = {}
-            for i, im in enumerate(images):
-                buckets.setdefault(im.shape[:2], []).append(i)
-            groups = [idx[k:k + self.post.batch_cap] for idx in buckets.values()
-                      for k in range(0, len(idx), self.post.batch_cap)]
+        pads = [nat.crop_geometry(im.shape[0], im.shape[1], dest_size, factor)[2] for im in images]
+        groups = plan_ragged_batches(pads, self.post.batch_cap)
         out = [None] * len(images)
         for part in groups:
             shapes = [images[i].shape[:2] for i in part]
-            if scales is not None or len(set(shapes)) == 1:
+            if len(set(shapes)) == 1:
                 batch = np.ascontiguousarray(np.stack([images[i] for i in part]))
                 self._keep = batch
                 sh, sw = shapes[0]
@@ -383,7 +393,11 @@ class PoseEngine:
             else:
                 batch = np.concatenate([np.ascontiguousarray(images[i]).ravel() for i in part])
                 self._keep = batch
-                self.infer_raw_ragged_async_u8(batch.ctypes.data, False, shapes, dest_size, factor, thresh, flip)
+                if scales is None:
+                    self.infer_raw_ragged_async_u8(batch.ctypes.data, False, shapes, dest_size, factor, thresh, flip)
+                else:
+                    self.infer_raw_multiscale_ragged_async_u8(batch.ctypes.data, False, shapes, scales, dest_size, factor,
+                                                              thresh, flip)
             for i, humans in zip(part, self.fetch_arrays() if _arrays else self.fetch()):
                 out[i] = humans.copy() if _arrays else humans
         return out

@@ -3,8 +3,10 @@
 orientations, five aspect ratios, many distinct padded shapes) with batch_cap 32; one step = one pass over the list.
 Prints ONE JSON line: frames/s (wall clock, host frames in, person rows out) and kernel launches per frame.
 
-  python tools/bench_mixed.py --steps K --warmup W [--mode bf16|bf16x3|fp32] [--flip] [--dump-outputs DIR]
+  python tools/bench_mixed.py --steps K --warmup W [--mode bf16|bf16x3|fp32] [--flip] [--scales S [S ...]]
+                              [--dump-outputs DIR]
 
+--scales 0.5 1.0 1.5 2.0 runs multi-scale test-time averaging around the 368 base size (passed to infer_images).
 --dump-outputs DIR writes the last step's person rows (float32 [k, 73], all images in list order) and the per-image
 counts as DIR/humans.npy and DIR/humans_per_image.npy, so that two builds can be compared row for row.  The script
 only calls PoseEngine.infer_images_arrays, so it also runs against builds that predate ragged batches."""
@@ -45,6 +47,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--mode", default="bf16", choices=["bf16", "bf16x3", "fp32"])
     ap.add_argument("--flip", action="store_true")
+    ap.add_argument("--scales", type=float, nargs="+", default=None, metavar="S")
     ap.add_argument("--dump-outputs", default="", metavar="DIR")
     args = ap.parse_args()
     import torch
@@ -57,12 +60,12 @@ def main():
     frames = mixed_frames()
     pads = {nat.crop_geometry(f.shape[0], f.shape[1], DEST, 8)[2] for f in frames}
     for _ in range(max(args.warmup, 1)):
-        eng.infer_images_arrays(frames, dest_size=DEST, flip=args.flip)
+        eng.infer_images_arrays(frames, dest_size=DEST, flip=args.flip, scales=args.scales)
     torch.cuda.synchronize()
     l0 = nat.launch_count()
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        out = eng.infer_images_arrays(frames, dest_size=DEST, flip=args.flip)
+        out = eng.infer_images_arrays(frames, dest_size=DEST, flip=args.flip, scales=args.scales)
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
     n = len(frames) * args.steps
@@ -78,7 +81,7 @@ def main():
         "higher_is_better": True, "launches_per_frame": round(launches / n, 2), "gpu_launches": int(launches),
         "gpu": torch.cuda.get_device_properties(0).name,
         "config": {"frames": len(frames), "distinct_padded_shapes": len(pads), "dest_size": DEST, "batch_cap": 32,
-                   "mode": args.mode, "flip": bool(args.flip),
+                   "mode": args.mode, "flip": bool(args.flip), "scales": args.scales,
                    "input": "host uint8 BGR frames; crop_with_factor, network and post-processing on the device; "
                             "results read back per batch (wall clock)"}}))
 
