@@ -38,6 +38,11 @@ typedef struct b200pose_net b200pose_net;
                                       weights, 3 MMA terms per K block (A_hi*W_hi + A_hi*W_lo + A_lo*W_hi); measured
                                       1.4e-3 max-abs @368x368 (bf16: 7e-2, fp32 mode: 3e-5) - the tensor core's own fp32
                                       accumulation is the floor, see DESIGN.md 2.3                                   */
+#define B200POSE_MODE_FP8 3        /* fp8 tensor-core mode: the 51 wgmma convolutions run on e4m3 operands, activations
+                                      scaled by 2^ea per (launch, image) from the max |bf16| their writers stored, weights
+                                      by 2^ew per output channel; activations stay bf16 in memory and conv1_1 runs as in
+                                      bf16 mode (DESIGN.md 2.3).  Before this mode existed, 3 ran as bf16; every other
+                                      value outside 0 .. 3 still does.                                                 */
 
 int b200pose_net_create(b200pose_net** out, int cuda_device);
 void b200pose_net_destroy(b200pose_net* net);
@@ -82,7 +87,7 @@ int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frame
  * event pair around every launch; fills per-launch milliseconds and ALGORITHMIC FLOPs (2 x MACs of the unpadded
  * convolution).  Returns the number of launches, < 0 on error. */
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream);
-/* Test hooks of the last bf16 / bf16x3 forward's launch list (launch 0 = conv1_1, 1 .. 51 = the tensor-core launches);
+/* Test hooks of the last bf16 / bf16x3 / fp8 forward's launch list (launch 0 = conv1_1, 1 .. 51 = the tensor-core launches);
  * they let a test check one launch against a reference computed from that launch's real inputs.
  *   b200pose_net_debug_run    : re-runs the first `launches` launches on the last forward's input (plain launches with
  *                               the plan's own arguments, PDL included, no graph), then synchronises the stream.
@@ -99,6 +104,11 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
 int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream);
 int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap);
 int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes);
+/* fp8 test hook: for tensor-core launch `launch` (1 .. 51) of the last fp8 forward, the activation scale exponent ea each
+ * of its n_img images used, as the kernel recorded it (act_exp[n_img], n_img = the forward's batch), and the weight
+ * exponent ew of each packed output row (w_exp[cap], rows = groups * n_tiles * n_tile; pad rows 0).  Returns the number
+ * of rows, < 0 on error. */
+int b200pose_net_debug_fp8(b200pose_net* net, int launch, int* act_exp, int n_img, int* w_exp, int cap);
 /* Device pointers of the last forward's stage-6 maps (NCHW fp32), valid until the next forward. */
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w);
 

@@ -11,8 +11,8 @@ _lib = None
 c_float_p = ctypes.POINTER(ctypes.c_float)
 NUM_TENSORS = 184
 HUMAN_FLOATS = 73
-MODE_BF16, MODE_FP32, MODE_BF16X3 = 0, 1, 2
-MODES = {"bf16": MODE_BF16, "fp32": MODE_FP32, "bf16x3": MODE_BF16X3}
+MODE_BF16, MODE_FP32, MODE_BF16X3, MODE_FP8 = 0, 1, 2, 3
+MODES = {"bf16": MODE_BF16, "fp32": MODE_FP32, "bf16x3": MODE_BF16X3, "fp8": MODE_FP8}
 PREPROCESS = {"rtpose": 1, "vgg": 2, "inception": 3, "ssd": 4}      # get_outputs' `preprocess` names
 
 
@@ -34,6 +34,7 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_net_debug_run": ([vp, ci, vp], ci),
     "b200pose_net_debug_launch": ([vp, ci, vp, ci], ci),
     "b200pose_net_debug_read": ([vp, ci, ci, ci, ci, vp, cl], ci),
+    "b200pose_net_debug_fp8": ([vp, ci, vp, ci, vp, ci], ci),
     "b200pose_net_last_maps": ([vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(ci), ctypes.POINTER(ci),
                                 ctypes.POINTER(ci)], ci),
     "b200pose_post_create": ([ctypes.POINTER(vp), ci, ci, ci, ci], ci),

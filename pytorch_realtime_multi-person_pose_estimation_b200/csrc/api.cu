@@ -18,6 +18,7 @@
 #include "../../include/b200pose.h"
 #include "conv_misc.cuh"
 #include "conv_tc.cuh"
+#include "fp8_core.h"
 #include "postprocess.cuh"
 #include "resize.cuh"
 #include "tta.cuh"
@@ -132,6 +133,12 @@ struct TcLayer {            // one grouped tensor-core launch
     double macs_per_pixel = 0;    // algorithmic (unpadded) MACs per output pixel, all groups
     __nv_bfloat16* w = nullptr;   // [taps][groups*n_tiles*n_tile][cin_blocks*64]
     float* bias = nullptr;        // [groups*n_tiles*n_tile]
+    std::vector<int> convs;       // state-dict conv per group
+    bool cat_input = false;       // reads the concat buffer (input channels permuted, cat_phys)
+    // fp8 mode, packed at the first fp8 plan build (pack_fp8_layer):
+    uint8_t* w8 = nullptr;        // [taps][rows][cin_blocks*64] e4m3(w * 2^ew[row]), K order fp8_k_to_channel
+    int* w_exp = nullptr;         // ew per row (device)
+    std::vector<int> h_w_exp;     // ... and its host copy (b200pose_net_debug_fp8)
 };
 
 // Activation buffers (the buffer ids of the test hooks): channels per pixel and spatial divisor.
@@ -189,12 +196,13 @@ struct PlanLaunch {
 };
 
 // Device addresses a plan's tensor maps and arguments point into: activation buffers, residual planes, stage maps.
-using PlanBuffers = std::array<const void*, 2 * kNumAct + 12>;
+using PlanBuffers = std::array<const void*, 2 * kNumAct + 12 + 2>;    // + the fp8 amax and exponent tables
 
 // The launch list of one (n, H, W, mode) key, valid while `buffers` are still the net's.
 struct Plan {
     int n, H, W, mode;
     bool split;            // bf16x3
+    bool fp8;
     std::vector<PlanLaunch> launches;
     PlanBuffers buffers;
 };
@@ -243,6 +251,10 @@ struct b200pose_net {
     // rewritten on the stream before each ragged forward.
     int* d_ext = nullptr;
     DevBuf<RaggedFrame> d_frames;      // per-frame source geometry of the last ragged crop
+    // fp8 mode (DESIGN.md §2.3): amax[launch * n + image] = max |bf16| (fp32 bits) launch (0 = conv1_1) stored for the
+    // image; zeroed at the start of every fp8 forward
+    DevBuf<unsigned> amax;
+    DevBuf<int> ea;                    // ea[launch * n + image]: the activation exponent the fp8 kernel used
 };
 
 struct b200pose_post {
@@ -289,7 +301,7 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_id
     const int cin_pad = cat_input ? 192 : sp.cin;
     const int cout_pad = ((sp.cout + n_tile - 1) / n_tile) * n_tile;
     L.ks = ks; L.cin_blocks = cin_pad / 64; L.groups = groups; L.n_tile = n_tile; L.n_tiles = cout_pad / n_tile;
-    L.relu = relu; L.pool = pool;
+    L.relu = relu; L.pool = pool; L.convs = conv_ids; L.cat_input = cat_input;
     const int taps = ks * ks, rows = groups * cout_pad;
     L.macs_per_pixel = 0;
     for (int g = 0; g < groups; ++g) L.macs_per_pixel += (double)conv_spec(conv_ids[g]).cin * conv_spec(conv_ids[g]).cout * taps;
@@ -320,6 +332,44 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_id
     return 0;
 }
 
+// fp8 weights of layer L, packed when the first fp8 plan is built (half the bytes of L.w; nets that never run fp8 do not
+// pay for them): per output row ew = floor(log2(448 / max|w_row|)) and e4m3(w * 2^ew), one rounding from the fp32
+// weight; each 32-channel slice in the K order the kernel's A fragments have (fp8_k_to_channel).
+int pack_fp8_layer(const b200pose_net* net, TcLayer& L) {
+    const int groups = L.groups, taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, cout_pad = L.n_tiles * L.n_tile;
+    const int rows = groups * cout_pad;
+    const bool cat_input = L.cat_input;
+    const std::vector<int>& conv_ids = L.convs;
+    L.h_w_exp.assign(rows, 0);
+    std::vector<uint8_t> w8((size_t)taps * rows * cin_pad, 0);
+    std::vector<float> phys(cin_pad);
+    for (int g = 0; g < groups; ++g) {
+        const ConvSpec s = conv_spec(conv_ids[g]);
+        const std::vector<float>& hw = net->host_w[conv_ids[g]];
+        for (int o = 0; o < s.cout; ++o) {
+            float m = 0.f;
+            for (size_t i = (size_t)o * s.cin * taps; i < (size_t)(o + 1) * s.cin * taps; ++i) m = std::max(m, std::fabs(hw[i]));
+            uint32_t mb;
+            memcpy(&mb, &m, 4);
+            const int ew = fp8_exp_from_amax(mb);
+            const int row = g * cout_pad + o;
+            L.h_w_exp[row] = ew;
+            for (int t = 0; t < taps; ++t) {
+                std::fill(phys.begin(), phys.end(), 0.f);
+                for (int c = 0; c < s.cin; ++c) phys[cat_input ? cat_phys(c) : c] = hw[((size_t)o * s.cin + c) * taps + t];
+                uint8_t* dst = &w8[((size_t)t * rows + row) * cin_pad];
+                for (int k = 0; k < cin_pad; ++k)
+                    dst[k] = e4m3_rn_bits(phys[(k & ~31) + fp8_k_to_channel(k & 31)] * exp2_int(ew));
+            }
+        }
+    }
+    CU(cudaMalloc(&L.w8, w8.size()));
+    CU(cudaMalloc(&L.w_exp, rows * sizeof(int)));
+    CU(cudaMemcpy(L.w8, w8.data(), w8.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(L.w_exp, L.h_w_exp.data(), rows * sizeof(int), cudaMemcpyHostToDevice));
+    return 0;
+}
+
 // Small-batch plans: the 46 x 46 stage layers (two groups) would fill at most half of the SMs with one n-tile per group.
 // Their launches are the launch-bound part of the product: they are chained by PDL and replayed as a CUDA graph; the large
 // plans are GPU-bound and get neither (a capture only adds a CPU hiccup).
@@ -328,7 +378,8 @@ bool small_plan(const b200pose_net* net, int n, int H, int W) {
 }
 
 // Appends tensor-core layer L, wired as `wr`, to plan p; a stage head writes the fp32 maps 2 * stage, 2 * stage + 1.
-int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& wr, int stage) {
+// fp8: writers[] are the launches (amax table rows) that wrote the channels it reads; writers[1] may be -1.
+int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& wr, int stage, const int writers[2]) {
     const int n = p.n, H = p.H / kActDiv[wr.in], W = p.W / kActDiv[wr.in];
     ConvTcArgs a;
     memset(&a, 0, sizeof(a));
@@ -341,9 +392,18 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         if (L.n_tile == 128 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 64; a.n_tiles = L.n_tiles * 2; }
         if (a.n_tile == 64 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 32; a.n_tiles *= 2; }
     }
-    if (p.split) {     // bf16x3: K-chunked accumulation in a second register set, so N <= 64
+    if (p.split || p.fp8) {     // bf16x3, fp8: K-chunked accumulation in a second register set, so N <= 64
         a.chunk = 1;
         if (a.n_tile > 64) { a.n_tile = 64; a.n_tiles = L.n_tiles * (L.n_tile / 64); }
+    }
+    if (p.fp8) {
+        a.fp8 = 1;
+        const int slot = 1 + (int)p.launches.size();      // amax table row of this launch (0 = conv1_1)
+        a.amax_out = net->amax.p + (size_t)slot * n;
+        a.amax_in[0] = net->amax.p + (size_t)writers[0] * n;
+        a.amax_in[1] = writers[1] >= 0 ? net->amax.p + (size_t)writers[1] * n : nullptr;
+        a.w_exp = L.w_exp;
+        a.ea_out = net->ea.p + (size_t)slot * n;
     }
     a.out = net->act[wr.out].p; a.out_cstride = kActC[wr.out];
     a.out_ch_off[0] = wr.out_off[0]; a.out_ch_off[1] = wr.out_off[1];
@@ -365,19 +425,22 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         in_lo = net->act_lo[wr.in].p;
         a.out_lo = net->act_lo[wr.out].p;
     }
-    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], L.w, in_lo);
+    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], p.fp8 ? (const void*)L.w8 : L.w, in_lo);
     if (e != cudaSuccess) return fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
     p.launches.push_back({a, 2.0 * n * H * W * L.macs_per_pixel, wr.in, wr.out, {f32[0], f32[1]}});
     return 0;
 }
 
-PlanBuffers plan_buffers(const b200pose_net* net) {
+// fp8: the plan also points into the amax and exponent tables (only fp8 plans do, so only they depend on them)
+PlanBuffers plan_buffers(const b200pose_net* net, bool fp8) {
     PlanBuffers b;
     for (int i = 0; i < kNumAct; ++i) {
         b[i] = net->act[i].p;
         b[kNumAct + i] = net->act_lo[i].p;
     }
     for (int i = 0; i < 12; ++i) b[2 * kNumAct + i] = net->out_f32[i].p;
+    b[2 * kNumAct + 12] = fp8 ? net->amax.p : nullptr;
+    b[2 * kNumAct + 13] = fp8 ? net->ea.p : nullptr;
     return b;
 }
 
@@ -392,13 +455,31 @@ int build_plan_bf16(b200pose_net* net, Plan& p, cudaStream_t st) {
         CU(cudaMemsetAsync(bufs[CAT].p, 0, px / 64 * kActC[CAT] * 2, st));
     }
     for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * (i % 2 == 0 ? kPaf : kHeat)));
+    if (p.fp8) {
+        CU(net->amax.ensure((size_t)(1 + 51) * p.n));
+        CU(net->ea.ensure((size_t)(1 + 51) * p.n));
+        for (TcLayer& L : net->tc)
+            if (L.w8 == nullptr && pack_fp8_layer(net, L)) return 1;
+    }
+    // fp8: the launch that last wrote each buffer (amax table row); the concat buffer has two writers, conv4_4_CPM
+    // (features) and the latest stage head (PAF + heatmap)
+    int writer[kNumAct], cat_head = -1;
+    for (int& w : writer) w = -1;
+    writer[T1] = 0;
+    auto add = [&](const TcLayer& L, const Wiring& wr, int stage) {
+        const int ws[2] = {writer[wr.in], wr.in == CAT && wr.in_base == 0 ? cat_head : -1};
+        if (add_plan(net, p, L, wr, stage, ws)) return 1;
+        if (wr.out == CAT && wr.maps) cat_head = (int)p.launches.size();
+        else writer[wr.out] = (int)p.launches.size();
+        return 0;
+    };
     int k = 0;
     for (const Wiring& wr : kTrunkWiring)
-        if (add_plan(net, p, net->tc[k++], wr, 0)) return 1;
+        if (add(net->tc[k++], wr, 0)) return 1;
     for (int s = 1; s <= 6; ++s)
         for (int li = 0; li < stage_num_layers(s); ++li)
-            if (add_plan(net, p, net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], s - 1)) return 1;
-    p.buffers = plan_buffers(net);
+            if (add(net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], s - 1)) return 1;
+    p.buffers = plan_buffers(net, p.fp8);
     return 0;
 }
 
@@ -412,7 +493,7 @@ void drop_graphs(b200pose_net* net) {
 // oldest of 32 is dropped).  A build may move the buffers the captured graphs point into: it synchronises the stream
 // and drops the graphs first.
 int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t st) {
-    const PlanBuffers bufs = plan_buffers(net);
+    const PlanBuffers bufs = plan_buffers(net, mode == B200POSE_MODE_FP8);
     for (const Plan& p : net->plans)
         if (p.n == n && p.H == H && p.W == W && p.mode == mode && p.buffers == bufs) {
             net->plan = &p;
@@ -423,7 +504,7 @@ int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t s
     net->plan = nullptr;
     net->plans.remove_if([&](const Plan& p) { return p.n == n && p.H == H && p.W == W && p.mode == mode; });
     if (net->plans.size() >= 32) net->plans.pop_front();
-    net->plans.push_back(Plan{n, H, W, mode, mode == B200POSE_MODE_BF16X3, {}, {}});
+    net->plans.push_back(Plan{n, H, W, mode, mode == B200POSE_MODE_BF16X3, mode == B200POSE_MODE_FP8, {}, {}});
     if (build_plan_bf16(net, net->plans.back(), st)) {
         net->plans.pop_back();
         return 1;
@@ -433,12 +514,15 @@ int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t s
 }
 
 // The first k launches of a forward with net->plan: conv1_1, then the plan's.  A ragged forward passes its extents
-// table (the plans are shared with uniform batches of the canvas size).
-int launch_forward_bf16(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st) {
+// table (the plans are shared with uniform batches of the canvas size).  fp8: zero_amax clears the amax table first (a
+// memset, not a launch); re-runs of launches (debug_run) leave it as it is - they record the same maxima again.
+int launch_forward_bf16(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st,
+                        bool zero_amax = false) {
     const Plan& p = *net->plan;
+    if (p.fp8 && zero_amax) CU(cudaMemsetAsync(net->amax.p, 0, (size_t)(1 + p.launches.size()) * p.n * sizeof(unsigned), st));
     if (k >= 1)
         CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr,
-                             p.n, p.H, p.W, ext, st));
+                             p.n, p.H, p.W, ext, st, p.fp8 ? net->amax.p : nullptr));
     for (int i = 0; i + 1 < k; ++i) {
         ConvTcArgs a = p.launches[i].a;
         a.ext = ext;
@@ -465,7 +549,7 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
             if (net->graphs.size() >= 64) drop_graphs(net);
             cudaGraph_t graph = nullptr;
             CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-            const int rc = launch_forward_bf16(net, d_in, in_u8, ext, launches, st);
+            const int rc = launch_forward_bf16(net, d_in, in_u8, ext, launches, st, true);
             cudaError_t e = cudaStreamEndCapture(st, &graph);
             if (rc == 0 && e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
             if (graph) cudaGraphDestroy(graph);
@@ -481,7 +565,7 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
         }
     }
     if (exec) CU(cudaGraphLaunch(exec, st));
-    else if (launch_forward_bf16(net, d_in, in_u8, ext, launches, st)) return 1;
+    else if (launch_forward_bf16(net, d_in, in_u8, ext, launches, st, true)) return 1;
     g_launches += launches;
     return 0;
 }
@@ -595,8 +679,10 @@ void b200pose_net_destroy(b200pose_net* net) {
     cudaSetDevice(net->device);
     drop_graphs(net);
     for (int i = 0; i < kNumConvs; ++i) { if (net->d_w[i]) cudaFree(net->d_w[i]); if (net->d_b[i]) cudaFree(net->d_b[i]); }
-    for (TcLayer& L : net->tc) { if (L.w) cudaFree(L.w); if (L.bias) cudaFree(L.bias); }
+    for (TcLayer& L : net->tc) { if (L.w) cudaFree(L.w); if (L.bias) cudaFree(L.bias); if (L.w8) cudaFree(L.w8); if (L.w_exp) cudaFree(L.w_exp); }
     for (int i = 0; i < kNumAct; ++i) { net->act[i].release(); net->act_lo[i].release(); }
+    net->amax.release();
+    net->ea.release();
     DevBuf<float>* fb[] = {&net->in_stage, &net->f_a, &net->f_b, &net->f_cat, &net->f_x, &net->f_y, &net->f_in, &net->f_u8};
     net->in_stage_u8.release();
     net->raw_stage.release();
@@ -635,7 +721,7 @@ int b200pose_net_finalize(b200pose_net* net) {
         CU(cudaMemcpy(net->d_w[i], net->host_w[i].data(), net->host_w[i].size() * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(net->d_b[i], net->host_b[i].data(), net->host_b[i].size() * 4, cudaMemcpyHostToDevice));
     }
-    for (TcLayer& L : net->tc) { if (L.w) cudaFree(L.w); if (L.bias) cudaFree(L.bias); }
+    for (TcLayer& L : net->tc) { if (L.w) cudaFree(L.w); if (L.bias) cudaFree(L.bias); if (L.w8) cudaFree(L.w8); if (L.w_exp) cudaFree(L.w_exp); }
     net->tc.assign(16 + 5 * 7, TcLayer());
     for (int i = 1; i < 12; ++i) {
         const ConvSpec s = kTrunk[i];
@@ -691,7 +777,7 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
             rc = forward_fp32(net, net->f_u8.p, n, H, W, st, ext);
         } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, st, ext);
     } else {
-        if (mode != B200POSE_MODE_BF16X3) mode = B200POSE_MODE_BF16;     // every other mode runs bf16
+        if (mode != B200POSE_MODE_BF16X3 && mode != B200POSE_MODE_FP8) mode = B200POSE_MODE_BF16;     // every other mode runs bf16
         first_u8 = in_u8 ? net->preprocess : 0;
         rc = forward_bf16(net, d_in, first_u8, n, H, W, mode, st, ext);
     }
@@ -829,7 +915,7 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
     if (!d_in) { if (tmp.ensure((size_t)n * 3 * H * W) != cudaSuccess) return -1; cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st); d_in = tmp.p; in_u8 = 0; }
     cudaEventRecord(ev[0], st);
     conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr, n, H, W,
-                      nullptr, st);
+                      nullptr, st, p.fp8 ? net->amax.p : nullptr);
     cudaEventRecord(ev[1], st);
     for (size_t i = 0; i < p.launches.size(); ++i) {
         conv_tc_launch(p.launches[i].a, net->num_sms, st);
@@ -904,6 +990,26 @@ int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, 
     CU(cudaSetDevice(net->device));
     CU(cudaMemcpy(host, src + per * img0, per * count, cudaMemcpyDeviceToHost));
     return 0;
+}
+
+int b200pose_net_debug_fp8(b200pose_net* net, int launch, int* act_exp, int n_img, int* w_exp, int cap) {
+    if (!net || !last_ran_plan(net) || !net->plan->fp8) { fail("debug_fp8: no fp8 forward has run"); return -1; }
+    const Plan& p = *net->plan;
+    if (launch < 1 || launch > (int)p.launches.size() || n_img != p.n || !act_exp || !w_exp) {
+        fail("debug_fp8: launch %d / images %d out of range", launch, n_img);
+        return -1;
+    }
+    const ConvTcArgs& a = p.launches[launch - 1].a;
+    const int rows = a.groups * a.n_tiles * a.n_tile;
+    if (cap < rows) { fail("debug_fp8: %d rows, capacity %d", rows, cap); return -1; }
+    if (cudaSetDevice(net->device) != cudaSuccess) { fail("debug_fp8: cudaSetDevice failed"); return -1; }
+    if (cudaMemcpy(act_exp, a.ea_out, p.n * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) {
+        fail("debug_fp8: reading the exponent table failed");
+        return -1;
+    }
+    const TcLayer& L = net->tc[launch - 1];
+    for (int r = 0; r < rows; ++r) w_exp[r] = L.h_w_exp[r];
+    return rows;
 }
 
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w) {

@@ -22,7 +22,8 @@ struct ConvF32Args {
 // (preprocess_core.h: 1 rtpose, 2 vgg, 3 inception, 4 ssd) fused into the load
 cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias,
                               __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo /*residual plane or null*/, int N, int H,
-                              int W, const int* ext /*ragged batch: padded H, W per image, or null*/, cudaStream_t s);
+                              int W, const int* ext /*ragged batch: padded H, W per image, or null*/, cudaStream_t s,
+                              unsigned* amax = nullptr /*fp8 mode: per-image max |stored bf16| (fp32 bits), atomic max*/);
 // ext (ragged batch) or null: pixels outside image i's padded extent ext[2 i], ext[2 i + 1] become 0 (zero padding)
 cudaError_t u8hwc_to_f32nchw_launch(const unsigned char* in, float* out, int N, int H, int W, int mode, const int* ext,
                                     cudaStream_t s);

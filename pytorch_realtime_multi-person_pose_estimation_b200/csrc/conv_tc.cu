@@ -23,6 +23,7 @@
 #include <cstdio>
 
 #include "conv_tc.cuh"
+#include "fp8_core.h"
 #include "host_util.h"
 #include "ptx.cuh"
 
@@ -74,11 +75,24 @@ template <> struct Mma<48> {
 template <> struct Mma<32> {
     static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n32k16_rs(d, a, b, s); }
 };
+template <int N> struct Mma8;      // e4m3, k32
+template <> struct Mma8<64> {
+    static __device__ __forceinline__ void run(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n64k32_e4m3_rs(d, a, b, s); }
+};
+template <> struct Mma8<48> {
+    static __device__ __forceinline__ void run(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n48k32_e4m3_rs(d, a, b, s); }
+};
+template <> struct Mma8<32> {
+    static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n32k32_e4m3_rs(d, a, b, s); }
+};
 
 constexpr int kConsumerWarps = 8;
 
-// kRagged: a.ext is set (ragged batch); a separate instantiation so that uniform batches run the unmasked epilogue
-template <int N, bool kChunk, bool kRagged>
+// kRagged: a.ext is set (ragged batch); a separate instantiation so that uniform batches run the unmasked epilogue.
+// kFp8 (with kChunk): the fp8 mode (DESIGN.md §2.3) - each tap's A fragments are converted from the bf16 patch to e4m3 in
+// registers, the weights are e4m3 slices of 64-byte rows, every tap's two k32 MMAs start a fresh accumulator that is
+// then added to the fp32 sum, and the epilogue records the per-image max |stored bf16|.
+template <int N, bool kChunk, bool kRagged, bool kFp8>
 __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B operands need 1024 B alignment.
@@ -101,7 +115,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     const int taps = a.ksize * a.ksize;
     const int pad = a.ksize >> 1;
     const uint32_t patch_tx = kPatchPitch * (kTileH + a.ksize - 1) * 128;
-    constexpr uint32_t b_tx = N * 128;                       // one tap's weight slice
+    constexpr uint32_t b_tx = kFp8 ? N * 64 : N * 128;       // one tap's weight slice
     // The weight ring is cut into stages of `tps` consecutive taps (a.tps, chosen with the tensor map's box): fewer, larger
     // stages mean fewer barrier round trips per tile.
     const int tps = a.tps;
@@ -184,10 +198,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
         const int wA = lane >> 2;
         const int cq = 2 * (lane & 3);
         const uint32_t patch0 = smem_u32(patch_smem);
-        const uint64_t bdesc_hi = make_sdesc_sw128(0, 1024);
+        const uint64_t bdesc_hi = kFp8 ? make_sdesc_sw64(0, 512) : make_sdesc_sw128(0, 1024);
         const uint32_t b_lo0 = (smem_u32(b_smem) & 0x3FFFFu) >> 4;
-        const bool row_chunks = kChunk && a.ksize == 7;    // K-chunked mode: one chunk per filter row (7x7; tps == 1) ...
-        const bool blk_chunks = kChunk && !row_chunks;     // ... or per (channel block, term)
+        const bool row_chunks = kChunk && !kFp8 && a.ksize == 7;    // K-chunked mode: one chunk per filter row (7x7; tps == 1) ...
+        const bool blk_chunks = kChunk && !kFp8 && !row_chunks;     // ... or per (channel block, term); fp8: per tap
         const int Ho = a.pool ? a.H >> 1 : a.H;
         const int Wo = a.pool ? a.W >> 1 : a.W;
         float acc[N / 2];
@@ -200,6 +214,15 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             if (kChunk) {
 #pragma unroll
                 for (int i = 0; i < N / 2; ++i) sum[i] = 0.f;
+            }
+            int ea = 0;           // fp8: the activation scale exponent of this tile's image
+            float sa = 1.f;
+            if constexpr (kFp8) {
+                uint32_t m = __ldcg(a.amax_in[0] + tc.n);
+                if (a.amax_in[1] != nullptr) m = max(m, __ldcg(a.amax_in[1] + tc.n));
+                ea = fp8_exp_from_amax(m);
+                sa = exp2_int(ea);
+                if (a.ea_out != nullptr && warp == 4 && lane == 0) a.ea_out[tc.n] = ea;
             }
             uint32_t scale = 0;       // 0: the next MMA overwrites the accumulators
             for (int cb = 0; cb < a.cin_blocks; ++cb) {
@@ -223,6 +246,27 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                             uint32_t af[4][4];
 #pragma unroll
                             for (int k = 0; k < 4; ++k) ldmatrix_x4(row_addr + (((2 * k + kc) ^ sw) << 4), af[k]);
+                            if constexpr (kFp8) {
+                                // k32 step s takes bf16 k16 steps 2s, 2s + 1 (K order: fp8_k_to_channel)
+                                uint32_t a8[2][4];
+#pragma unroll
+                                for (int s = 0; s < 2; ++s) {
+                                    a8[s][0] = bf16x4_to_e4m3x4(af[2 * s][0], af[2 * s][2], sa);
+                                    a8[s][1] = bf16x4_to_e4m3x4(af[2 * s][1], af[2 * s][3], sa);
+                                    a8[s][2] = bf16x4_to_e4m3x4(af[2 * s + 1][0], af[2 * s + 1][2], sa);
+                                    a8[s][3] = bf16x4_to_e4m3x4(af[2 * s + 1][1], af[2 * s + 1][3], sa);
+                                }
+                                fence_regs(acc);
+                                wgmma_fence();
+#pragma unroll
+                                for (int s = 0; s < 2; ++s)
+                                    Mma8<N>::run(acc, a8[s], bdesc_hi | (b_lo + j * (b_tx >> 4) + s * 2), s);
+                                wgmma_commit();
+                                wgmma_wait_all();
+                                fence_regs(acc);
+#pragma unroll
+                                for (int i = 0; i < N / 2; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
+                            } else {
                             fence_regs(acc);
                             wgmma_fence();
 #pragma unroll
@@ -233,6 +277,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                             wgmma_commit();
                             wgmma_wait_all();      // the next tap's ldmatrix reuses the A registers
                             fence_regs(acc);
+                            }
                             if (++dx == a.ksize) { dx = 0; ++dy; }
                         }
                         __syncwarp();
@@ -259,6 +304,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             // ---- epilogue
             const int ch_tile = tc.nt * N;                     // first channel of this n-tile within the group
             const float* bias = a.bias + (tc.g * a.n_tiles + tc.nt) * N;
+            const int* w_exp = a.w_exp + (tc.g * a.n_tiles + tc.nt) * N;
+            uint32_t amax = 0;    // fp8: max |stored bf16| bits of this lane
             const int store_ch = a.store_ch[tc.g];
             float* of32 = a.out_f32[tc.g];
             const int f32_ch = a.f32_ch[tc.g];
@@ -286,10 +333,20 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             for (int j = 0; j < N / 8; ++j) {
                 const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + cq));
                 float v[4];
+                if constexpr (kFp8) {     // acc * 2^-(ea + ew) is exact: one rounding, at the bias add
+                    const int2 w2 = __ldg(reinterpret_cast<const int2*>(w_exp + 8 * j + cq));
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        v[e] = __fadd_rn(__fmul_rn(sum[4 * j + e], exp2_int(-(ea + ((e & 1) ? w2.y : w2.x)))),
+                                         (e & 1) ? b2.y : b2.x);
+                        if (a.relu) v[e] = fmaxf(v[e], 0.f);
+                    }
+                } else {
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     v[e] = (kChunk ? sum[4 * j + e] : acc[4 * j + e]) + ((e & 1) ? b2.y : b2.x);
                     if (a.relu) v[e] = fmaxf(v[e], 0.f);
+                }
                 }
                 if (a.pool) {
                     v[0] = fmaxf(v[0], v[2]);
@@ -302,7 +359,13 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                     if (!wr[hh]) continue;
                     const float lo = inside[hh] ? v[2 * hh] : 0.f, hi = inside[hh] ? v[2 * hh + 1] : 0.f;
                     if (out_px[hh] != nullptr && 8 * j < store_ch) {
-                        *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pack_bf16x2(lo, hi);
+                        if constexpr (kFp8) {
+                            const uint32_t pk = pack_bf16x2(lo, hi);
+                            *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pk;
+                            amax = max(amax, max(pk & 0x7fffu, (pk >> 16) & 0x7fffu));
+                        } else {
+                            *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pack_bf16x2(lo, hi);
+                        }
                         if (a.out_lo != nullptr) {      // split mode: residual plane v - bf16(v)
                             __nv_bfloat16* dlo = a.out_lo + (out_px[hh] - a.out) + 8 * j;
                             *reinterpret_cast<uint32_t*>(dlo) =
@@ -316,6 +379,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                     }
                 }
             }
+            if constexpr (kFp8) {     // max of non-negative float bits: order-independent, so runs stay deterministic
+                amax = __reduce_max_sync(0xffffffffu, amax);
+                if (lane == 0 && amax != 0) atomicMax(a.amax_out + tc.n, amax << 16);
+            }
             if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(7);
         }
     }
@@ -324,7 +391,12 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
 
 template <int N, bool kChunk, bool kRagged>
 __global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_kernel(const __grid_constant__ ConvTcArgs a) {
-    conv_tc_body<N, kChunk, kRagged>(a);
+    conv_tc_body<N, kChunk, kRagged, false>(a);
+}
+
+template <int N, bool kRagged>
+__global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_fp8_kernel(const __grid_constant__ ConvTcArgs a) {
+    conv_tc_body<N, true, kRagged, true>(a);
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -346,7 +418,7 @@ PFN_encodeTiled get_encode_fn() {
 
 }  // namespace
 
-cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cstride, const __nv_bfloat16* w,
+cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cstride, const void* w,
                               const __nv_bfloat16* in_lo) {
     PFN_encodeTiled enc = get_encode_fn();
     if (enc == nullptr) return cudaErrorNotSupported;
@@ -354,6 +426,7 @@ cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cst
     if (a.n_tile != 32 && a.n_tile != 48 && a.n_tile != 64 && a.n_tile != 128) return cudaErrorInvalidValue;
     if (a.groups < 1 || a.groups > 2 || in_cstride % 8 != 0) return cudaErrorInvalidValue;
     if (a.split && in_lo == nullptr) return cudaErrorInvalidValue;
+    if (a.fp8 && (a.split || !a.chunk || a.n_tile > 64)) return cudaErrorInvalidValue;
     for (int plane = 0; plane <= (a.split ? 1 : 0); ++plane) {
         cuuint64_t dims[4] = {(cuuint64_t)in_cstride, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.n_img};
         cuuint64_t strides[3] = {(cuuint64_t)in_cstride * 2, (cuuint64_t)a.W * in_cstride * 2,
@@ -375,17 +448,20 @@ cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cst
         const int taps = a.ksize * a.ksize;
         // taps per weight stage: as many as leave kMinBStages stages in the ring (N = 128: 2 taps of 16 KB, N = 32: 8 taps of
         // 4 KB).  The K-chunked 7x7 mode closes a chunk at every filter-row end, which a stage must not straddle.
-        const int tap_bytes = a.n_tile * 128;
+        // fp8: one byte per weight, 64-byte rows (SWIZZLE_64B), chunks per tap, no residual slices
+        const int esz = a.fp8 ? 1 : 2;
+        const int tap_bytes = a.n_tile * 64 * esz;
         int tps = (kNumBStages * kBStageBytes) / (kMinBStages * tap_bytes);
-        if (tps < 1 || (a.chunk && a.ksize == 7)) tps = 1;
+        if (tps < 1 || (a.chunk && !a.fp8 && a.ksize == 7)) tps = 1;
         if (tps > taps) tps = taps;
         a.tps = tps;
-        cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)rows, (cuuint64_t)(2 * taps)};
-        cuuint64_t strides[2] = {(cuuint64_t)cin_pad * 2, (cuuint64_t)rows * cin_pad * 2};
+        cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)rows, (cuuint64_t)(a.fp8 ? taps : 2 * taps)};
+        cuuint64_t strides[2] = {(cuuint64_t)cin_pad * esz, (cuuint64_t)rows * cin_pad * esz};
         cuuint32_t box[3] = {64, (cuuint32_t)a.n_tile, (cuuint32_t)tps};
         cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&a.tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<__nv_bfloat16*>(w), dims, strides,
-                         box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+        CUresult r = enc(&a.tm_w, a.fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3,
+                         const_cast<void*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         a.fp8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
             fprintf(stderr, "[b200pose] cuTensorMapEncodeTiled(w) failed: %d\n", (int)r);
@@ -399,10 +475,13 @@ namespace {
 // Programmatic dependent launch (a.pdl): the next layer's CTAs may start - barrier init, descriptor prefetch, weight loads -
 // while this layer's last CTAs drain; they wait (griddepcontrol.wait) before touching activations.  Used by the SMALL-batch
 // plans only, where the fixed cost per launch is most of a layer.
-template <int N, bool kChunk, bool kRagged>
+template <int N, bool kChunk, bool kRagged, bool kFp8 = false>
 cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
     static DynSmemOptIn optin;   // per device: a second net on another GPU of the same process needs its own opt-in
-    cudaError_t e = optin.ensure(conv_tc_kernel<N, kChunk, kRagged>, kConvTcSmemBytes);
+    void (*kernel)(ConvTcArgs);
+    if constexpr (kFp8) kernel = conv_tc_fp8_kernel<N, kRagged>;
+    else kernel = conv_tc_kernel<N, kChunk, kRagged>;
+    cudaError_t e = optin.ensure(kernel, kConvTcSmemBytes);
     if (e != cudaSuccess) return e;
     if (a.pdl) {
         cudaLaunchConfig_t cfg = {};
@@ -415,15 +494,15 @@ cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
         attr[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        return cudaLaunchKernelEx(&cfg, conv_tc_kernel<N, kChunk, kRagged>, a);
+        return cudaLaunchKernelEx(&cfg, kernel, a);
     }
-    conv_tc_kernel<N, kChunk, kRagged><<<grid, kConvTcThreads, kConvTcSmemBytes, stream>>>(a);
+    kernel<<<grid, kConvTcThreads, kConvTcSmemBytes, stream>>>(a);
     return cudaGetLastError();
 }
 
-template <int N, bool kChunk>
+template <int N, bool kChunk, bool kFp8 = false>
 cudaError_t launch(int grid, cudaStream_t stream, const ConvTcArgs& a) {
-    return a.ext != nullptr ? launch_k<N, kChunk, true>(grid, stream, a) : launch_k<N, kChunk, false>(grid, stream, a);
+    return a.ext != nullptr ? launch_k<N, kChunk, true, kFp8>(grid, stream, a) : launch_k<N, kChunk, false, kFp8>(grid, stream, a);
 }
 }  // namespace
 
@@ -435,6 +514,15 @@ cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream
     const int tiles_y = (a.H + kTileH - 1) / kTileH;
     const int total = a.n_img * tiles_y * tiles_x * a.groups * a.n_tiles;
     const int grid = total < num_sms ? total : num_sms;
+    if (a.fp8) {
+        if (!a.chunk || a.amax_out == nullptr || a.amax_in[0] == nullptr || a.w_exp == nullptr) return cudaErrorInvalidValue;
+        switch (a.n_tile) {
+            case 64: return launch<64, true, true>(grid, stream, a);
+            case 48: return launch<48, true, true>(grid, stream, a);
+            case 32: return launch<32, true, true>(grid, stream, a);
+            default: return cudaErrorInvalidValue;
+        }
+    }
     switch (a.n_tile) {
         case 128: return launch<128, false>(grid, stream, a);
         case 64: return a.chunk ? launch<64, true>(grid, stream, a) : launch<64, false>(grid, stream, a);

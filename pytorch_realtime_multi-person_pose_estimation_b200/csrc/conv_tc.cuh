@@ -66,12 +66,19 @@ struct ConvTcArgs {
     // output element of image i outside (ext >> ext_shift) is stored as +0.  null: every image fills the canvas.
     const int* ext;
     int ext_shift;            // log2 of the network input size over this launch's OUTPUT size (pooling included)
+    // ---- fp8 mode (DESIGN.md §2.3): e4m3 operands, per-(launch, image) activation and per-row weight scales; n_tile <= 64
+    int fp8;
+    const unsigned* amax_in[2];   // per-image max |bf16| (fp32 bits) of the launches that wrote the input; [1] may be null
+    unsigned* amax_out;           // this launch's per-image max |stored bf16|, atomic max
+    const int* w_exp;             // [groups * n_tiles * n_tile]: weight row r holds e4m3(w * 2^w_exp[r])
+    int* ea_out;                  // the activation exponent each image used (may be null)
 };
 
 // Builds the tensor maps. `in` (and `in_lo` in split mode): NHWC buffers with `in_cstride` channels per pixel.
 // `w`: packed weights [2*taps][groups*n_tiles*n_tile][cin_blocks*64]: bf16(w) for the first `taps` slices, the
-// residual bf16(w - hi) for the second.
-cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cstride, const __nv_bfloat16* w,
+// residual bf16(w - hi) for the second.  fp8 mode (a.fp8): [taps][rows][cin_blocks*64] e4m3 bytes, each 32-channel
+// slice in the K order of fp8_k_to_channel (fp8_core.h).
+cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cstride, const void* w,
                               const __nv_bfloat16* in_lo = nullptr);
 cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream);
 

@@ -158,4 +158,67 @@ __device__ __forceinline__ void wgmma_m64n32k16_rs(float (&d)[16], const uint32_
         : "memory");
 }
 
+// ---------------------------------------------------------------- fp8 (e4m3) wgmma, k32
+// As make_sdesc_sw128 for 64-byte rows (64 e4m3) with the 64-byte swizzle: layout type 2.
+__device__ __forceinline__ uint64_t make_sdesc_sw64(uint32_t saddr, uint32_t sbo_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
+    d |= 1ull << 16;
+    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
+    d |= 2ull << 62;
+    return d;
+}
+
+// e4m3x4 from two bf16x2 registers u (bytes 0, 1) and v (bytes 2, 3), each value multiplied by the power of two s first
+// (exact), then rounded to nearest even on the e4m3 grid.
+__device__ __forceinline__ uint32_t bf16x4_to_e4m3x4(uint32_t u, uint32_t v, float s) {
+    const float u0 = __uint_as_float(u << 16) * s, u1 = __uint_as_float(u & 0xffff0000u) * s;
+    const float v0 = __uint_as_float(v << 16) * s, v1 = __uint_as_float(v & 0xffff0000u) * s;
+    uint16_t lo, hi;     // cvt puts its first source in the upper byte
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(u1), "f"(u0));
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(v1), "f"(v0));
+    uint32_t r;
+    asm("mov.b32 %0, {%1, %2};" : "=r"(r) : "h"(lo), "h"(hi));
+    return r;
+}
+
+// D[64 x 64] (+)= A[64 x 32, registers] * B[32 x 64, shared memory descriptor], e4m3 -> fp32.
+__device__ __forceinline__ void wgmma_m64n64k32_e4m3_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
+        : "memory");
+}
+
+// D[64 x 48] (+)= A[64 x 32, registers] * B[32 x 48, shared memory descriptor], e4m3 -> fp32.
+__device__ __forceinline__ void wgmma_m64n48k32_e4m3_rs(float (&d)[24], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %29, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
+        "{%24, %25, %26, %27}, %28, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
+        : "memory");
+}
+
+// D[64 x 32] (+)= A[64 x 32, registers] * B[32 x 32, shared memory descriptor], e4m3 -> fp32.
+__device__ __forceinline__ void wgmma_m64n32k32_e4m3_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
+        : "memory");
+}
+
 }  // namespace b2p

@@ -9,8 +9,9 @@ the input's device pointer to libb200pose.so, which runs the hand-written sm_90a
 
 Precision: `model.precision = 'bf16x3'` (default: split-precision operands on the wgmma tensor cores with K-chunked
 fp32 accumulation - maps within 1.4e-4 of the reference's fp32 network at 368x368, inside its 1e-3 tolerance), `'bf16'`
-(the fast mode of the batched engine and the benchmark: ~4.5x faster, maps within ~8e-2) or `'fp32'` (CUDA cores,
-bit-identical to the oracle's fp32 network); the environment variable B200POSE_MODE sets the default.
+(the fast mode of the batched engine and the benchmark: ~4.5x faster, maps within ~8e-2), `'fp8'` (e4m3 operands with
+per-image activation and per-channel weight scales; DESIGN.md 2.3) or `'fp32'` (CUDA cores, bit-identical to the
+oracle's fp32 network); the environment variable B200POSE_MODE sets the default.
 """
 import os
 import threading

@@ -3,7 +3,7 @@
 orientations, five aspect ratios, many distinct padded shapes) with batch_cap 32; one step = one pass over the list.
 Prints ONE JSON line: frames/s (wall clock, host frames in, person rows out) and kernel launches per frame.
 
-  python tools/bench_mixed.py --steps K --warmup W [--mode bf16|bf16x3|fp32] [--flip] [--scales S [S ...]]
+  python tools/bench_mixed.py --steps K --warmup W [--mode bf16|bf16x3|fp32|fp8] [--flip] [--scales S [S ...]]
                               [--dump-outputs DIR]
 
 --scales 0.5 1.0 1.5 2.0 runs multi-scale test-time averaging around the 368 base size (passed to infer_images).
@@ -45,7 +45,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--mode", default="bf16", choices=["bf16", "bf16x3", "fp32"])
+    ap.add_argument("--mode", default="bf16", choices=["bf16", "bf16x3", "fp32", "fp8"])
     ap.add_argument("--flip", action="store_true")
     ap.add_argument("--scales", type=float, nargs="+", default=None, metavar="S")
     ap.add_argument("--dump-outputs", default="", metavar="DIR")
