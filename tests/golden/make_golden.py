@@ -14,7 +14,7 @@ import os
 import sys
 import types
 
-ARGS = sys.argv[1:]     # optional: "crop" / "eval" / "pre" / "fuzz" regenerate only those small fixtures
+ARGS = sys.argv[1:]     # optional: "crop" / "eval" / "pre" / "fuzz" / "edges" regenerate only those small fixtures
 
 import numpy as np
 
@@ -201,12 +201,48 @@ def make_pafprocess_fuzz():
     print("pafprocess fuzz fixture written: %d humans" % len(rows))
 
 
+def make_edges(ref_p2p, cfg):
+    """The reference's NMS + paf_to_pose_cpp (compiled pafprocess.cpp) on the adversarial heat maps of
+    oracle/synth.EDGE_CASES (plateaus, k/16 values, checkerboards, maxima at the threshold, edge spikes, twin maxima),
+    with OpenCV's IPP path off: the product restates OpenCV's own cubic resize, not IPP's.  Per case the joint list
+    (float32 [P, 5]) and the human rows [k, 1 + 18 x 3] like the post_*.npz fixtures; one digest over all inputs."""
+    import cv2
+    use_ipp = cv2.ipp.useIPP()
+    cv2.ipp.setUseIPP(False)      # process-wide: restored below, so the other fixtures keep this build's default
+    try:
+        _write_edges(ref_p2p, cfg)
+    finally:
+        cv2.ipp.setUseIPP(use_ipp)
+
+
+def _write_edges(ref_p2p, cfg):
+    out, ins = {}, []
+    for case in synth.EDGE_CASES:
+        name = synth.edge_case_name(*case)
+        heat, paf = synth.edge_maps(*case)
+        ins += [heat, paf]
+        per_joint = ref_p2p.NMS(heat, upsampFactor=cfg.MODEL.DOWNSAMPLE, config=cfg)
+        jl = np.array([tuple(p) + (j,) for j, peaks in enumerate(per_joint) for p in peaks]).astype(np.float32).reshape(-1, 5)
+        humans = ref_p2p.paf_to_pose_cpp(heat, paf, cfg)
+        rows = np.full((len(humans), 1 + 18 * 3), -1.0, np.float64)
+        for i, hm in enumerate(humans):
+            rows[i, 0] = hm.score
+            for p, bp in hm.body_parts.items():
+                rows[i, 1 + 3 * p: 4 + 3 * p] = (bp.x, bp.y, bp.score)
+        out[name + "_joint_list"] = jl
+        out[name + "_humans"] = rows
+        print("edges", name, "peaks", len(jl), "humans", len(humans))
+    np.savez_compressed(os.path.join(OUT, "post_edges.npz"), in_digest=digest(*ins), **out)
+
+
 def main():
     if ARGS and set(ARGS) <= {"fuzz"}:
         make_pafprocess_fuzz()
         return
     import torch
     get_model, ref_p2p, ref_eval, cfg = import_reference()
+    if "edges" in ARGS:
+        make_edges(ref_p2p, cfg)
     if not ARGS or "fuzz" in ARGS:
         make_pafprocess_fuzz()
     if not ARGS or "pre" in ARGS:
@@ -215,7 +251,9 @@ def main():
         make_crop()
     if not ARGS or "eval" in ARGS:
         make_eval(ref_eval)
-    if ARGS and set(ARGS) <= {"crop", "eval", "pre", "fuzz"}:
+    if not ARGS:
+        make_edges(ref_p2p, cfg)
+    if ARGS and set(ARGS) <= {"crop", "eval", "pre", "fuzz", "edges"}:
         return
     torch.manual_seed(0)
 
