@@ -294,6 +294,25 @@ struct b200pose_post {
 
 namespace {
 
+// Calls row(g, o, r, w) for output channel o of every group g of layer L (packed row r = g * cout_pad + o), w its fp32
+// weights in packed order [tap][cin_pad]: input channels at their physical channel of the buffer the layer reads (cat_phys
+// for the concat buffer), zero in the pad channels.
+template <class F> void for_each_weight_row(const b200pose_net* net, const TcLayer& L, F&& row) {
+    const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, cout_pad = L.n_tiles * L.n_tile;
+    std::vector<float> w((size_t)taps * cin_pad);
+    for (int g = 0; g < L.groups; ++g) {
+        const ConvSpec s = conv_spec(L.convs[g]);
+        const std::vector<float>& hw = net->host_w[L.convs[g]];
+        for (int o = 0; o < s.cout; ++o) {
+            std::fill(w.begin(), w.end(), 0.f);
+            for (int c = 0; c < s.cin; ++c)
+                for (int t = 0; t < taps; ++t)
+                    w[(size_t)t * cin_pad + (L.cat_input ? cat_phys(c) : c)] = hw[((size_t)o * s.cin + c) * taps + t];
+            row(g, o, g * cout_pad + o, w.data());
+        }
+    }
+}
+
 int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_ids /*per group*/, int n_tile,
                   bool cat_input, int ks, int relu, int pool) {
     const int groups = (int)conv_ids.size();
@@ -308,23 +327,16 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_id
     // [hi taps | lo taps]: bf16(w) and the residual bf16(w - hi) (used by the split-precision mode only)
     std::vector<uint16_t> w((size_t)2 * taps * rows * cin_pad, 0);
     std::vector<float> b((size_t)rows, 0.f);
-    for (int g = 0; g < groups; ++g) {
-        const ConvSpec s = conv_spec(conv_ids[g]);
-        const std::vector<float>& hw = net->host_w[conv_ids[g]];
-        const std::vector<float>& hb = net->host_b[conv_ids[g]];
-        for (int o = 0; o < s.cout; ++o) {
-            b[g * cout_pad + o] = hb[o];
-            for (int c = 0; c < s.cin; ++c) {
-                const int pc = cat_input ? cat_phys(c) : c;
-                for (int t = 0; t < taps; ++t) {
-                    const float wf = hw[((size_t)o * s.cin + c) * taps + t];
-                    const uint16_t hi = f2bf(wf);
-                    w[((size_t)t * rows + g * cout_pad + o) * cin_pad + pc] = hi;
-                    w[((size_t)(taps + t) * rows + g * cout_pad + o) * cin_pad + pc] = f2bf(wf - bf2f(hi));
-                }
+    for_each_weight_row(net, L, [&](int g, int o, int r, const float* wr) {
+        b[r] = net->host_b[conv_ids[g]][o];
+        for (int t = 0; t < taps; ++t)
+            for (int k = 0; k < cin_pad; ++k) {
+                const float wf = wr[(size_t)t * cin_pad + k];
+                const uint16_t hi = f2bf(wf);
+                w[((size_t)t * rows + r) * cin_pad + k] = hi;
+                w[((size_t)(taps + t) * rows + r) * cin_pad + k] = f2bf(wf - bf2f(hi));
             }
-        }
-    }
+    });
     CU(cudaMalloc(&L.w, w.size() * 2));
     CU(cudaMalloc(&L.bias, b.size() * 4));
     CU(cudaMemcpy(L.w, w.data(), w.size() * 2, cudaMemcpyHostToDevice));
@@ -336,33 +348,22 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_id
 // pay for them): per output row ew = floor(log2(448 / max|w_row|)) and e4m3(w * 2^ew), one rounding from the fp32
 // weight; each 32-channel slice in the K order the kernel's A fragments have (fp8_k_to_channel).
 int pack_fp8_layer(const b200pose_net* net, TcLayer& L) {
-    const int groups = L.groups, taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, cout_pad = L.n_tiles * L.n_tile;
-    const int rows = groups * cout_pad;
-    const bool cat_input = L.cat_input;
-    const std::vector<int>& conv_ids = L.convs;
+    const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, rows = L.groups * L.n_tiles * L.n_tile;
     L.h_w_exp.assign(rows, 0);
     std::vector<uint8_t> w8((size_t)taps * rows * cin_pad, 0);
-    std::vector<float> phys(cin_pad);
-    for (int g = 0; g < groups; ++g) {
-        const ConvSpec s = conv_spec(conv_ids[g]);
-        const std::vector<float>& hw = net->host_w[conv_ids[g]];
-        for (int o = 0; o < s.cout; ++o) {
-            float m = 0.f;
-            for (size_t i = (size_t)o * s.cin * taps; i < (size_t)(o + 1) * s.cin * taps; ++i) m = std::max(m, std::fabs(hw[i]));
-            uint32_t mb;
-            memcpy(&mb, &m, 4);
-            const int ew = fp8_exp_from_amax(mb);
-            const int row = g * cout_pad + o;
-            L.h_w_exp[row] = ew;
-            for (int t = 0; t < taps; ++t) {
-                std::fill(phys.begin(), phys.end(), 0.f);
-                for (int c = 0; c < s.cin; ++c) phys[cat_input ? cat_phys(c) : c] = hw[((size_t)o * s.cin + c) * taps + t];
-                uint8_t* dst = &w8[((size_t)t * rows + row) * cin_pad];
-                for (int k = 0; k < cin_pad; ++k)
-                    dst[k] = e4m3_rn_bits(phys[(k & ~31) + fp8_k_to_channel(k & 31)] * exp2_int(ew));
-            }
+    for_each_weight_row(net, L, [&](int, int, int r, const float* wr) {
+        float m = 0.f;
+        for (size_t i = 0; i < (size_t)taps * cin_pad; ++i) m = std::max(m, std::fabs(wr[i]));
+        uint32_t mb;
+        memcpy(&mb, &m, 4);
+        const int ew = fp8_exp_from_amax(mb);
+        L.h_w_exp[r] = ew;
+        for (int t = 0; t < taps; ++t) {
+            const float* src = wr + (size_t)t * cin_pad;
+            uint8_t* dst = &w8[((size_t)t * rows + r) * cin_pad];
+            for (int k = 0; k < cin_pad; ++k) dst[k] = e4m3_rn_bits(src[(k & ~31) + fp8_k_to_channel(k & 31)] * exp2_int(ew));
         }
-    }
+    });
     CU(cudaMalloc(&L.w8, w8.size()));
     CU(cudaMalloc(&L.w_exp, rows * sizeof(int)));
     CU(cudaMemcpy(L.w8, w8.data(), w8.size(), cudaMemcpyHostToDevice));
@@ -515,18 +516,22 @@ int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t s
 
 // The first k launches of a forward with net->plan: conv1_1, then the plan's.  A ragged forward passes its extents
 // table (the plans are shared with uniform batches of the canvas size).  fp8: zero_amax clears the amax table first (a
-// memset, not a launch); re-runs of launches (debug_run) leave it as it is - they record the same maxima again.
+// memset, not a launch); re-runs of launches (debug_run, profile) leave it as it is - they record the same maxima again.
+// after (b200pose_net_profile): after[i] is recorded behind launch i.
 int launch_forward_bf16(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st,
-                        bool zero_amax = false) {
+                        bool zero_amax = false, const cudaEvent_t* after = nullptr) {
     const Plan& p = *net->plan;
     if (p.fp8 && zero_amax) CU(cudaMemsetAsync(net->amax.p, 0, (size_t)(1 + p.launches.size()) * p.n * sizeof(unsigned), st));
-    if (k >= 1)
+    if (k >= 1) {
         CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr,
                              p.n, p.H, p.W, ext, st, p.fp8 ? net->amax.p : nullptr));
+        if (after) CU(cudaEventRecord(after[0], st));
+    }
     for (int i = 0; i + 1 < k; ++i) {
         ConvTcArgs a = p.launches[i].a;
         a.ext = ext;
         CU(conv_tc_launch(a, net->num_sms, st));
+        if (after) CU(cudaEventRecord(after[i + 1], st));
     }
     return 0;
 }
@@ -834,16 +839,30 @@ static int upload_frames(b200pose_net* net, const std::vector<RaggedFrame>& fram
     return 0;
 }
 
-// Places the n frames of net->d_frames (sources at d_src) on an Hc x Wc canvas in net->in_stage_u8 and runs the
-// forward pass on them with extents `ext`.
-static int ragged_forward(b200pose_net* net, const unsigned char* d_src, int n, int Hc, int Wc, const std::vector<int>& ext,
-                          int mode, float* const* outputs, int outputs_on_device, cudaStream_t st, bool sync_host) {
-    CU(net->in_stage_u8.ensure((size_t)n * Hc * Wc * 3));
-    if (launched(ragged_frames_launch(d_src, net->d_frames.p, n, net->in_stage_u8.p, Hc, Wc, st), "ragged_frames_launch"))
-        return 1;
-    if (int rc = upload_ext(net, ext, st)) return rc;
-    return net_forward_impl(net, net->in_stage_u8.p, 1, 1, n, Hc, Wc, mode, outputs, outputs_on_device, st, sync_host,
-                            net->d_ext);
+// A batch of raw uint8 frames packed back to back, cropped for one destination size: frame table (flip: the mirrored
+// frames follow the originals, in the staging buffer and in both tables), padded extents and canvas, the frames' total
+// and largest size in bytes.  A uniform batch (frames of one size) keeps `ext` empty: its kernels get no extents table.
+struct RawBatch {
+    std::vector<RaggedFrame> tab;
+    std::vector<int> ext;
+    int Hc = 0, Wc = 0;
+    long long raw = 0, max_bytes = 0;
+    bool ragged() const { return !ext.empty(); }
+};
+
+// Crops the nimg frames of c (sources at d_raw; ragged: frame table already in net->d_frames) into net->in_stage_u8
+// and runs the forward pass on them.
+static int crop_and_forward(b200pose_net* net, const unsigned char* d_raw, int nimg, const RawBatch& c, int mode,
+                            cudaStream_t st, float* const* outputs = nullptr, int outputs_on_device = 1,
+                            bool sync_host = false) {
+    CU(net->in_stage_u8.ensure((size_t)nimg * c.Hc * c.Wc * 3));
+    const RaggedFrame& f = c.tab[0];
+    cudaError_t e = c.ragged() ? ragged_frames_launch(d_raw, net->d_frames.p, nimg, net->in_stage_u8.p, c.Hc, c.Wc, st)
+                               : crop_with_factor_launch(d_raw, net->in_stage_u8.p, nimg, f.src_h, f.src_w, f.g, st);
+    if (launched(e, c.ragged() ? "ragged_frames_launch" : "crop_with_factor_launch")) return 1;
+    if (c.ragged() && upload_ext(net, c.ext, st)) return 1;
+    return net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, c.Hc, c.Wc, mode, outputs, outputs_on_device, st,
+                            sync_host, c.ragged() ? net->d_ext : nullptr);
 }
 
 // Raw uint8 frames of `bytes` on the device: a device input in place, else a copy in net->raw_stage.  flip: always
@@ -866,21 +885,21 @@ int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frame
     if (int rc = ragged_canvas(n, hw, &Hc, &Wc)) return rc;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    std::vector<RaggedFrame> tab(n);
-    long long bytes = 0;
+    RawBatch c;
+    c.tab.assign(n, RaggedFrame{});
+    c.ext.assign(hw, hw + 2 * n);
+    c.Hc = Hc;
+    c.Wc = Wc;
     for (int i = 0; i < n; ++i) {
-        tab[i] = RaggedFrame{};
-        tab[i].off = bytes;
-        tab[i].src_h = hw[2 * i];
-        tab[i].src_w = hw[2 * i + 1];      // g.pad_h == 0: copied as it is
-        bytes += (long long)hw[2 * i] * hw[2 * i + 1] * 3;
+        c.tab[i].off = c.raw;
+        c.tab[i].src_h = hw[2 * i];
+        c.tab[i].src_w = hw[2 * i + 1];      // g.pad_h == 0: copied as it is
+        c.raw += (long long)hw[2 * i] * hw[2 * i + 1] * 3;
     }
     const unsigned char* d_src;
-    if (int rc = stage_raw(net, frames, on_device, (size_t)bytes, 0, st, &d_src)) return rc;
-    if (int rc = upload_frames(net, tab, st)) return rc;
-    if (int rc = ragged_forward(net, d_src, n, Hc, Wc, std::vector<int>(hw, hw + 2 * n), mode, outputs, outputs_on_device,
-                                st, true))
-        return rc;
+    if (int rc = stage_raw(net, frames, on_device, (size_t)c.raw, 0, st, &d_src)) return rc;
+    if (int rc = upload_frames(net, c.tab, st)) return rc;
+    if (int rc = crop_and_forward(net, d_src, n, c, mode, st, outputs, outputs_on_device, true)) return rc;
     if (!on_device) CU(cudaStreamSynchronize(st));
     return 0;
 }
@@ -914,21 +933,18 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
     DevBuf<float> tmp;
     if (!d_in) { if (tmp.ensure((size_t)n * 3 * H * W) != cudaSuccess) return -1; cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st); d_in = tmp.p; in_u8 = 0; }
     cudaEventRecord(ev[0], st);
-    conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr, n, H, W,
-                      nullptr, st, p.fp8 ? net->amax.p : nullptr);
-    cudaEventRecord(ev[1], st);
-    for (size_t i = 0; i < p.launches.size(); ++i) {
-        conv_tc_launch(p.launches[i].a, net->num_sms, st);
-        cudaEventRecord(ev[i + 2], st);
-    }
+    int rc = launch_forward_bf16(net, d_in, in_u8, nullptr, total, st, false, ev.data() + 1);
     g_launches += total;
-    if (cudaStreamSynchronize(st) != cudaSuccess) { fail("profile run failed: %s", cudaGetErrorString(cudaGetLastError())); return -1; }
-    for (int i = 0; i < total; ++i) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
-    flops[0] = 2.0 * n * H * W * 27.0 * 64.0;
-    for (size_t i = 0; i < p.launches.size(); ++i) flops[i + 1] = p.launches[i].flops;
+    if (rc == 0 && cudaStreamSynchronize(st) != cudaSuccess)
+        rc = fail("profile run failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (rc == 0) {
+        for (int i = 0; i < total; ++i) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
+        flops[0] = 2.0 * n * H * W * 27.0 * 64.0;
+        for (size_t i = 0; i < p.launches.size(); ++i) flops[i + 1] = p.launches[i].flops;
+    }
     for (auto& e : ev) cudaEventDestroy(e);
     tmp.release();
-    return total;
+    return rc ? -1 : total;
 }
 
 int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream) {
@@ -1432,187 +1448,92 @@ int b200pose_net_crop_with_factor(b200pose_net* net, const unsigned char* images
     return 0;
 }
 
-// Raw frames of one size on the device (uniform fused entry points), their mirror images behind them when flip: mirrored
-// RAW frames, so that the padding of both orientations ends up on the right, as for the reference.
-static int stage_raw_uniform(b200pose_net* net, const unsigned char* images, int on_device, int n, int src_h, int src_w,
-                             int flip, cudaStream_t st, const unsigned char** d_raw) {
-    const size_t raw = (size_t)n * src_h * src_w * 3;
-    if (int rc = stage_raw(net, images, on_device, raw, flip, st, d_raw)) return rc;
-    if (flip && launched(tta_mirror_u8hwc(net->raw_stage.p, net->raw_stage.p + raw, n, src_h, src_w, st), "tta_mirror"))
-        return 1;
-    return 0;
-}
-
-// crop_with_factor of nimg raw frames into net->in_stage_u8, then the forward pass on them
-static int crop_and_forward(b200pose_net* net, const unsigned char* d_raw, int nimg, int src_h, int src_w,
-                            const CropGeom& g, int mode, cudaStream_t st) {
-    CU(net->in_stage_u8.ensure((size_t)nimg * g.pad_h * g.pad_w * 3));
-    if (launched(crop_with_factor_launch(d_raw, net->in_stage_u8.p, nimg, src_h, src_w, g, st), "crop_with_factor_launch"))
-        return 1;
-    return net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, g.pad_h, g.pad_w, mode, nullptr, 1, st, false);
-}
-
-int b200pose_infer_raw_u8(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device, int n,
-                          int src_h, int src_w, int dest_size, int factor, int mode, float thresh, int flip,
-                          void* cuda_stream) {
-    if (int rc = check_infer(net, post)) return rc;
-    if (!images) return fail("infer_raw: null pointer");
-    if (int rc = check_batch(post, n)) return rc;
-    CropGeom g;
-    if (int rc = crop_check(n, src_h, src_w, dest_size, factor, &g)) return rc;
-    CU(cudaSetDevice(net->device));
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
-    const unsigned char* d_raw;
-    if (int rc = stage_raw_uniform(net, images, input_on_device, n, src_h, src_w, flip, st, &d_raw)) return rc;
-    if (int rc = crop_and_forward(net, d_raw, flip ? 2 * n : n, src_h, src_w, g, mode, st)) return rc;
-    return finish_infer(net, post, n, flip, thresh, st);
-}
-
-// The ragged crop of n raw frames packed back to back (src_hw: their sizes) for dest_size: frame table, padded extents
-// and canvas, the frames' total and largest size in bytes.  flip: the mirrored frames follow the originals, in the
-// staging buffer and in both tables.
-struct RaggedCrop {
-    std::vector<RaggedFrame> tab;
-    std::vector<int> ext;
-    int Hc = 0, Wc = 0;
-    long long raw = 0, max_bytes = 0;
-};
-
-static int ragged_crop(int n, const int* src_hw, int dest_size, int factor, int flip, RaggedCrop* c) {
+// n raw frames of one size src_h x src_w (src_hw null) or of the sizes src_hw[2 i], src_hw[2 i + 1] (a ragged batch),
+// cropped for dest_size.
+static int raw_batch(int n, int src_h, int src_w, const int* src_hw, int dest_size, int factor, int flip, RawBatch* c) {
     const int nimg = flip ? 2 * n : n;
-    if (nimg > kMaxRagged) return fail("ragged batch: %d images (at most %d)", nimg, kMaxRagged);
+    if (src_hw && nimg > kMaxRagged) return fail("ragged batch: %d images (at most %d)", nimg, kMaxRagged);
+    *c = RawBatch{};
     c->tab.assign(nimg, RaggedFrame{});
-    c->ext.assign(2 * nimg, 0);
     for (int i = 0; i < n; ++i) {
         RaggedFrame& f = c->tab[i];
-        f.src_h = src_hw[2 * i];
-        f.src_w = src_hw[2 * i + 1];
+        f.src_h = src_hw ? src_hw[2 * i] : src_h;
+        f.src_w = src_hw ? src_hw[2 * i + 1] : src_w;
         if (int rc = crop_check(1, f.src_h, f.src_w, dest_size, factor, &f.g)) return rc;
         f.off = c->raw;
         const long long b = (long long)f.src_h * f.src_w * 3;
         c->raw += b;
         if (b > c->max_bytes) c->max_bytes = b;
-        c->ext[2 * i] = f.g.pad_h;
-        c->ext[2 * i + 1] = f.g.pad_w;
         if (f.g.pad_h > c->Hc) c->Hc = f.g.pad_h;
         if (f.g.pad_w > c->Wc) c->Wc = f.g.pad_w;
     }
     for (int i = 0; i < n && flip; ++i) {      // mirrored raw frames follow the originals in the staging buffer
         c->tab[n + i] = c->tab[i];
         c->tab[n + i].off += c->raw;
-        c->ext[2 * (n + i)] = c->ext[2 * i];
-        c->ext[2 * (n + i) + 1] = c->ext[2 * i + 1];
     }
-    if ((long)c->Hc * c->Wc > (1L << 28)) return fail("infer_raw_ragged: canvas too large");
+    for (int i = 0; i < nimg && src_hw; ++i) {
+        c->ext.push_back(c->tab[i].g.pad_h);
+        c->ext.push_back(c->tab[i].g.pad_w);
+    }
+    if ((long)c->Hc * c->Wc > (1L << 28)) return fail("infer_raw: canvas too large");
     return 0;
 }
 
-// With flip: mirrors the n raw frames of the staging buffer behind them.  Reads the first n entries of net->d_frames.
-static int mirror_raw_ragged(b200pose_net* net, int n, const RaggedCrop& c, cudaStream_t st) {
-    return launched(tta_mirror_u8hwc_ragged(net->raw_stage.p, net->raw_stage.p + c.raw, net->d_frames.p, n,
-                                            (long)c.max_bytes, st),
-                    "tta_mirror_u8hwc_ragged");
-}
-
-int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device,
-                                  int n, const int* src_hw, int dest_size, int factor, int mode, float thresh, int flip,
-                                  void* cuda_stream) {
+// The fused inference of raw uint8 frames (b200pose_infer_raw_u8*): n frames of one size src_h x src_w, or of the
+// sizes src_hw (a ragged batch), are staged with their mirror images when flip, cropped for every scale and run
+// through the network.  scales null: one scale, base_size, post-processed as it is.  Else every scale s runs at
+// int(base_size * s) and its maps are resized (bicubic) to the grid of base_size, averaged and post-processed.
+static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char* images, int on_device, int n,
+                     int src_h, int src_w, const int* src_hw, int base_size, int factor, const double* scales,
+                     int n_scales, int mode, float thresh, int flip, void* cuda_stream) {
     if (int rc = check_infer(net, post)) return rc;
-    if (!images || !src_hw) return fail("infer_raw_ragged: null pointer");
+    if (!images) return fail("infer_raw: null pointer");
+    if (scales && (n_scales < 1 || n_scales > 16)) return fail("infer_raw: %d scales (1 .. 16)", n_scales);
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
-    const int nimg = flip ? 2 * n : n;
-    RaggedCrop c;
-    if (int rc = ragged_crop(n, src_hw, dest_size, factor, flip, &c)) return rc;
-    CU(cudaSetDevice(net->device));
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
-    const unsigned char* d_raw;
-    if (int rc = stage_raw(net, images, input_on_device, (size_t)c.raw, flip, st, &d_raw)) return rc;
-    if (int rc = upload_frames(net, c.tab, st)) return rc;
-    if (flip && mirror_raw_ragged(net, n, c, st)) return 1;
-    if (int rc = ragged_forward(net, d_raw, nimg, c.Hc, c.Wc, c.ext, mode, nullptr, 1, st, false)) return rc;
-    return finish_infer(net, post, n, flip, thresh, st);
-}
-
-int b200pose_infer_raw_u8_multiscale(b200pose_net* net, b200pose_post* post, const unsigned char* images,
-                                     int input_on_device, int n, int src_h, int src_w, int base_size, int factor,
-                                     const double* scales, int n_scales, int mode, float thresh, int flip,
-                                     void* cuda_stream) {
-    if (int rc = check_infer(net, post)) return rc;
-    if (!images || !scales || n_scales < 1 || n_scales > 16) return fail("infer_multiscale: bad arguments");
-    if (int rc = check_batch(post, n)) return rc;
-    CropGeom base;
-    if (int rc = crop_check(n, src_h, src_w, base_size, factor, &base)) return rc;
-    CU(cudaSetDevice(net->device));
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    const unsigned char* d_raw;
-    if (int rc = stage_raw_uniform(net, images, input_on_device, n, src_h, src_w, flip, st, &d_raw)) return rc;
-    const int h1 = base.pad_h / 8, w1 = base.pad_w / 8;
-    CU(post->d_heat.ensure((size_t)n * kHeat * h1 * w1));
-    CU(post->d_paf.ensure((size_t)n * kPaf * h1 * w1));
-    for (int k = 0; k < n_scales; ++k) {
-        const int dest = (int)((double)base_size * scales[k]);       // Python: int(base_size * s)
-        CropGeom g;
-        if (int rc = crop_check(n, src_h, src_w, dest, factor, &g)) return rc;
-        if (int rc = crop_and_forward(net, d_raw, flip ? 2 * n : n, src_h, src_w, g, mode, st)) return rc;
-        const int h = g.pad_h / 8, w = g.pad_w / 8;
-        const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
-        const float *s_heat = net->out_f32[11].p, *s_paf = net->out_f32[10].p;
-        if (flip) {
-            CU(post->tta_out.ensure(eh + ep));
-            if (int rc = merge_last_flip(net, n, post->tta_out.p, post->tta_out.p + eh, st)) return rc;
-            s_heat = post->tta_out.p;
-            s_paf = post->tta_out.p + eh;
-        }
-        const float div = (k == n_scales - 1) ? (float)n_scales : 0.f;
-        cudaError_t e = resize_cubic_accum_launch(s_heat, post->d_heat.p, (long)n * kHeat, h, w, h1, w1, k == 0, div, st);
-        if (e == cudaSuccess)
-            e = resize_cubic_accum_launch(s_paf, post->d_paf.p, (long)n * kPaf, h, w, h1, w1, k == 0, div, st);
-        if (launched(e, "resize_cubic_accum_launch", 2)) return 1;
-    }
-    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h1, w1, thresh, st);
-}
-
-int b200pose_infer_raw_u8_multiscale_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images,
-                                            int input_on_device, int n, const int* src_hw, int base_size, int factor,
-                                            const double* scales, int n_scales, int mode, float thresh, int flip,
-                                            void* cuda_stream) {
-    if (int rc = check_infer(net, post)) return rc;
-    if (!images || !src_hw || !scales || n_scales < 1 || n_scales > 16) return fail("infer_multiscale_ragged: bad arguments");
-    if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
+    const bool ragged = src_hw != nullptr;
     // every scale's geometry first: an invalid frame size fails before anything is enqueued
-    RaggedCrop base;
-    if (int rc = ragged_crop(n, src_hw, base_size, factor, 0, &base)) return rc;
-    std::vector<RaggedCrop> sc(n_scales);
-    std::vector<RaggedResize> rz((size_t)n_scales * n);
-    for (int k = 0; k < n_scales; ++k) {
-        const int dest = (int)((double)base_size * scales[k]);       // Python: int(base_size * s)
-        if (int rc = ragged_crop(n, src_hw, dest, factor, flip, &sc[k])) return rc;
-        for (int i = 0; i < n; ++i)
-            rz[(size_t)k * n + i] = ragged_resize(sc[k].ext[2 * i] / 8, sc[k].ext[2 * i + 1] / 8, base.ext[2 * i] / 8,
-                                                  base.ext[2 * i + 1] / 8);
+    RawBatch base;
+    if (scales && raw_batch(n, src_h, src_w, src_hw, base_size, factor, 0, &base)) return 1;
+    std::vector<RawBatch> sc(scales ? n_scales : 1);
+    std::vector<RaggedResize> rz;
+    for (int k = 0; k < (int)sc.size(); ++k) {
+        const int dest = scales ? (int)((double)base_size * scales[k]) : base_size;       // Python: int(base_size * s)
+        if (int rc = raw_batch(n, src_h, src_w, src_hw, dest, factor, flip, &sc[k])) return rc;
+        for (int i = 0; i < n && scales && ragged; ++i)
+            rz.push_back(ragged_resize(sc[k].ext[2 * i] / 8, sc[k].ext[2 * i + 1] / 8, base.ext[2 * i] / 8,
+                                       base.ext[2 * i + 1] / 8));
     }
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
     const unsigned char* d_raw;
-    if (int rc = stage_raw(net, images, input_on_device, (size_t)base.raw, flip, st, &d_raw)) return rc;
-    if (flip) {      // the sources and offsets of the frame table are those of every scale
-        if (int rc = upload_frames(net, base.tab, st)) return rc;
-        if (mirror_raw_ragged(net, n, base, st)) return 1;
+    if (int rc = stage_raw(net, images, on_device, (size_t)sc[0].raw, flip, st, &d_raw)) return rc;
+    // the sources and offsets of the frame table are those of every scale
+    if (ragged && upload_frames(net, sc[0].tab, st)) return 1;
+    if (flip) {      // mirrored RAW frames, so that the padding of both orientations ends up on the right, as for the reference
+        unsigned char* mirror = net->raw_stage.p + sc[0].raw;
+        cudaError_t e = ragged ? tta_mirror_u8hwc_ragged(net->raw_stage.p, mirror, net->d_frames.p, n, (long)sc[0].max_bytes, st)
+                               : tta_mirror_u8hwc(net->raw_stage.p, mirror, n, src_h, src_w, st);
+        if (launched(e, "tta_mirror")) return 1;
     }
-    CU(post->ms_ext.ensure(base.ext.size()));
-    CU(cudaMemcpyAsync(post->ms_ext.p, base.ext.data(), base.ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    CU(post->ms_resize.ensure(rz.size()));
-    CU(cudaMemcpyAsync(post->ms_resize.p, rz.data(), rz.size() * sizeof(RaggedResize), cudaMemcpyHostToDevice, st));
+    const int nimg = flip ? 2 * n : n;
+    if (!scales) {
+        if (int rc = crop_and_forward(net, d_raw, nimg, sc[0], mode, st)) return rc;
+        return finish_infer(net, post, n, flip, thresh, st);
+    }
+    if (ragged) {
+        CU(post->ms_ext.ensure(base.ext.size()));
+        CU(cudaMemcpyAsync(post->ms_ext.p, base.ext.data(), base.ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+        CU(post->ms_resize.ensure(rz.size()));
+        CU(cudaMemcpyAsync(post->ms_resize.p, rz.data(), rz.size() * sizeof(RaggedResize), cudaMemcpyHostToDevice, st));
+    }
     const int h1 = base.Hc / 8, w1 = base.Wc / 8;
     CU(post->d_heat.ensure((size_t)n * kHeat * h1 * w1));
     CU(post->d_paf.ensure((size_t)n * kPaf * h1 * w1));
     for (int k = 0; k < n_scales; ++k) {
-        const RaggedCrop& c = sc[k];
-        if (int rc = upload_frames(net, c.tab, st)) return rc;
-        if (int rc = ragged_forward(net, d_raw, flip ? 2 * n : n, c.Hc, c.Wc, c.ext, mode, nullptr, 1, st, false)) return rc;
+        const RawBatch& c = sc[k];
+        if (ragged && k > 0 && upload_frames(net, c.tab, st)) return 1;
+        if (int rc = crop_and_forward(net, d_raw, nimg, c, mode, st)) return rc;
         const int h = c.Hc / 8, w = c.Wc / 8;
         const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
         const float *s_heat = net->out_f32[11].p, *s_paf = net->out_f32[10].p;
@@ -1623,14 +1544,54 @@ int b200pose_infer_raw_u8_multiscale_ragged(b200pose_net* net, b200pose_post* po
             s_paf = post->tta_out.p + eh;
         }
         const float div = (k == n_scales - 1) ? (float)n_scales : 0.f;
-        const RaggedResize* f = post->ms_resize.p + (size_t)k * n;
-        cudaError_t e = resize_cubic_accum_ragged_launch(s_heat, post->d_heat.p, f, n, kHeat, h, w, h1, w1, k == 0, div, st);
-        if (e == cudaSuccess)
-            e = resize_cubic_accum_ragged_launch(s_paf, post->d_paf.p, f, n, kPaf, h, w, h1, w1, k == 0, div, st);
-        if (launched(e, "resize_cubic_accum_ragged_launch", 2)) return 1;
+        cudaError_t e;
+        if (ragged) {
+            const RaggedResize* f = post->ms_resize.p + (size_t)k * n;
+            e = resize_cubic_accum_ragged_launch(s_heat, post->d_heat.p, f, n, kHeat, h, w, h1, w1, k == 0, div, st);
+            if (e == cudaSuccess)
+                e = resize_cubic_accum_ragged_launch(s_paf, post->d_paf.p, f, n, kPaf, h, w, h1, w1, k == 0, div, st);
+        } else {
+            e = resize_cubic_accum_launch(s_heat, post->d_heat.p, (long)n * kHeat, h, w, h1, w1, k == 0, div, st);
+            if (e == cudaSuccess)
+                e = resize_cubic_accum_launch(s_paf, post->d_paf.p, (long)n * kPaf, h, w, h1, w1, k == 0, div, st);
+        }
+        if (launched(e, "resize_cubic_accum", 2)) return 1;
     }
     // the net's extents table now holds the last scale's: post-processing reads the base extents
-    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h1, w1, thresh, st, post->ms_ext.p);
+    return post_run_dev(post, post->d_heat.p, post->d_paf.p, 0, n, h1, w1, thresh, st, ragged ? post->ms_ext.p : nullptr);
+}
+
+int b200pose_infer_raw_u8(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device, int n,
+                          int src_h, int src_w, int dest_size, int factor, int mode, float thresh, int flip,
+                          void* cuda_stream) {
+    return infer_raw(net, post, images, input_on_device, n, src_h, src_w, nullptr, dest_size, factor, nullptr, 0, mode,
+                     thresh, flip, cuda_stream);
+}
+
+int b200pose_infer_raw_u8_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images, int input_on_device,
+                                  int n, const int* src_hw, int dest_size, int factor, int mode, float thresh, int flip,
+                                  void* cuda_stream) {
+    return src_hw ? infer_raw(net, post, images, input_on_device, n, 0, 0, src_hw, dest_size, factor, nullptr, 0, mode,
+                              thresh, flip, cuda_stream)
+                  : fail("infer_raw_ragged: null size table");
+}
+
+int b200pose_infer_raw_u8_multiscale(b200pose_net* net, b200pose_post* post, const unsigned char* images,
+                                     int input_on_device, int n, int src_h, int src_w, int base_size, int factor,
+                                     const double* scales, int n_scales, int mode, float thresh, int flip,
+                                     void* cuda_stream) {
+    return scales ? infer_raw(net, post, images, input_on_device, n, src_h, src_w, nullptr, base_size, factor, scales,
+                              n_scales, mode, thresh, flip, cuda_stream)
+                  : fail("infer_multiscale: null scales");
+}
+
+int b200pose_infer_raw_u8_multiscale_ragged(b200pose_net* net, b200pose_post* post, const unsigned char* images,
+                                            int input_on_device, int n, const int* src_hw, int base_size, int factor,
+                                            const double* scales, int n_scales, int mode, float thresh, int flip,
+                                            void* cuda_stream) {
+    return scales && src_hw ? infer_raw(net, post, images, input_on_device, n, 0, 0, src_hw, base_size, factor, scales,
+                                        n_scales, mode, thresh, flip, cuda_stream)
+                            : fail("infer_multiscale_ragged: null pointer");
 }
 
 // ------------------------------------------------------------------------------------------------ legacy pafprocess

@@ -8,6 +8,7 @@
 //   maxpool_f32_kernel: MaxPool2d(2,2) NHWC fp32 (parity mode only; the bf16 path fuses pooling in the conv epilogue)
 //   nchw_to_nhwc / nhwc_slice_to_nchw : layout glue for the parity path.
 #include <cstdint>
+#include <type_traits>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
@@ -139,8 +140,7 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_kernel(const void* __re
     }
 }
 
-
-// ------------------------------------------------------------------ conv1_1 on the tensor cores (bf16 mode)
+// ------------------------------------------------------------------ conv1_1 on the tensor cores (bf16 and fp8 modes)
 // conv1_1 is a GEMM with K = 27: far too thin for a wgmma tile pipeline (one 64 x 64 x 32 MMA per 64 pixels), and its
 // roofline is HBM (0.4 MB in, 17.7 MB out per frame: 0.09 ms per batch of 32 at the measured copy bandwidth) - the fp32
 // CUDA-core kernel above needs 0.50 ms for its 7.5 G fused multiply-adds.  Here every warp runs warp-level
@@ -159,11 +159,13 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int kIn>
+// fp8 mode (DESIGN.md §2.3): kAmax also records each image's max |stored bf16| (fp32 bits, atomic max) in amax[n] for
+// the next launch's activation scale.
+template <int kIn, bool kAmax>
 __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* __restrict__ in_v, const float* __restrict__ wgt,
                                                                     const float* __restrict__ bias,
                                                                     __nv_bfloat16* __restrict__ out, int H, int W,
-                                                                    const int* __restrict__ ext) {
+                                                                    const int* __restrict__ ext, unsigned* amax) {
     constexpr bool kU8 = kIn != 0;
     constexpr int kRowF = kF_TW + 2, kPlaneF = (kF_TH + 2) * kRowF;
     __shared__ float s_in[3 * kPlaneF];
@@ -225,116 +227,7 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
 #pragma unroll
     for (int j = 0; j < 8; ++j) { bs[j][0] = __ldg(bias + 8 * j + 2 * q); bs[j][1] = __ldg(bias + 8 * j + 2 * q + 1); }
     __syncthreads();
-    const float* srow = s_in + warp * kRowF;             // this warp's output row of the tile (ty = warp)
-#pragma unroll 1
-    for (int mt = 0; mt < kF_TW / 16; ++mt) {
-        uint32_t afrag[2][4];
-#pragma unroll
-        for (int s2 = 0; s2 < 2; ++s2) {
-            float v[4][2];                               // [a-register][col 0 / col 1]: rows r0 (a0, a2) and r0 + 8 (a1, a3)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int off = aoff[s2][j];
-                v[j][0] = off >= 0 ? srow[off + 16 * mt + r0] : 0.f;
-                v[j][1] = off >= 0 ? srow[off + 16 * mt + r0 + 8] : 0.f;
-            }
-            afrag[s2][0] = pack_bf16(v[0][0], v[1][0]);  // row r0,     k = 2q, 2q+1
-            afrag[s2][1] = pack_bf16(v[0][1], v[1][1]);  // row r0 + 8, k = 2q, 2q+1
-            afrag[s2][2] = pack_bf16(v[2][0], v[3][0]);  // row r0,     k = 2q+8, 2q+9
-            afrag[s2][3] = pack_bf16(v[2][1], v[3][1]);  // row r0 + 8, k = 2q+8, 2q+9
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            float d[4] = {bs[j][0], bs[j][1], bs[j][0], bs[j][1]};
-            mma_bf16_16816(d, afrag[0], bfrag[j][0][0], bfrag[j][0][1]);
-            mma_bf16_16816(d, afrag[1], bfrag[j][1][0], bfrag[j][1][1]);
-            // d0, d1: pixel row r0, channels 8j + 2q, +1;  d2, d3: pixel row r0 + 8
-            const int p0 = warp * kF_TW + 16 * mt + r0, p1 = p0 + 8;
-            s_out[p0 * 32 + ((j ^ (p0 & 7)) << 2) + q] = pack_bf16(fmaxf(d[0], 0.f), fmaxf(d[1], 0.f));
-            s_out[p1 * 32 + ((j ^ (p1 & 7)) << 2) + q] = pack_bf16(fmaxf(d[2], 0.f), fmaxf(d[3], 0.f));
-        }
-    }
-    __syncthreads();
-    for (int i = tid; i < kF_TH * kF_TW * 8; i += kF_Threads) {
-        const int p = i >> 3, ch = i & 7;
-        const int y = y0 + p / kF_TW, x = x0 + p % kF_TW;
-        if (y < H && x < W)
-            reinterpret_cast<uint4*>(out + (((size_t)n * H + y) * W + x) * 64)[ch] =
-                (y < eh && x < ew) ? reinterpret_cast<const uint4*>(s_out + p * 32)[ch ^ (p & 7)] : make_uint4(0, 0, 0, 0);
-    }
-}
-
-// fp8 mode (DESIGN.md §2.3): conv_first_mma_kernel that also records each image's max |stored bf16| (fp32 bits, atomic
-// max) in amax[n] for the next launch's activation scale.  A copy rather than a shared body, so that the bf16 kernel's
-// machine code stays exactly what was validated.
-template <int kIn>
-__global__ void __launch_bounds__(kF_Threads) conv_first_mma_amax_kernel(const void* __restrict__ in_v,
-                                                                         const float* __restrict__ wgt,
-                                                                         const float* __restrict__ bias,
-                                                                         __nv_bfloat16* __restrict__ out, int H, int W,
-                                                                         const int* __restrict__ ext, unsigned* amax) {
-    constexpr bool kU8 = kIn != 0;
-    constexpr int kRowF = kF_TW + 2, kPlaneF = (kF_TH + 2) * kRowF;
-    __shared__ float s_in[3 * kPlaneF];
-    __shared__ __align__(16) uint32_t s_out[kF_TH * kF_TW * 32];      // [pixel][8 chunks of 16 B], chunk index ^ (pixel & 7)
-    const int n = blockIdx.z, y0 = blockIdx.y * kF_TH, x0 = blockIdx.x * kF_TW;
-    // ragged batch: canvas pixels outside the image are the convolution's zero padding (not a uint8 0, which the
-    // normalisation would map to a non-zero value) and its outputs there are +0
-    const int eh = ext ? __ldg(ext + 2 * n) : H, ew = ext ? __ldg(ext + 2 * n + 1) : W;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    for (int i = tid; i < 3 * kPlaneF; i += kF_Threads) {
-        int c, yy, xx;
-        if (kU8) {   // channel fastest: consecutive threads read consecutive bytes
-            c = i % 3;
-            const int r = i / 3;
-            yy = r / kRowF;
-            xx = r - yy * kRowF;
-        } else {
-            c = i / kPlaneF;
-            const int r = i - c * kPlaneF;
-            yy = r / kRowF;
-            xx = r - yy * kRowF;
-        }
-        const int gy = y0 + yy - 1, gx = x0 + xx - 1;
-        float v = 0.f;
-        if (gy >= 0 && gy < eh && gx >= 0 && gx < ew) {
-            if (kU8) {
-                const unsigned char u =
-                    static_cast<const unsigned char*>(in_v)[(((size_t)n * H + gy) * W + gx) * 3 + pre_src_channel(kIn, c)];
-                v = pre_value(kIn, u, c);
-            } else {
-                v = static_cast<const float*>(in_v)[(((size_t)n * 3 + c) * H + gy) * W + gx];
-            }
-        }
-        s_in[c * kPlaneF + yy * kRowF + xx] = v;
-    }
-    // this thread's K indices of the A / B fragments: k-step s, register pair i: kk = 16 s + 8 (i >> 1)... see PTX m16n8k16
-    const int q = lane & 3, r0 = lane >> 2;
-    int aoff[2][4];                  // [k-step][a-register half: cols 2q, 2q+1, 2q+8, 2q+9] -> s_in offset, or -1 (K padding)
-#pragma unroll
-    for (int s2 = 0; s2 < 2; ++s2)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int kk = 16 * s2 + 2 * q + (j & 1) + 8 * (j >> 1);
-            aoff[s2][j] = kk < 27 ? (kk / 9) * kPlaneF + ((kk % 9) / 3) * kRowF + (kk % 3) : -1;
-        }
-    uint32_t bfrag[8][2][2];         // [n-tile][k-step][b0, b1]: B[k][n] = w[n][k], n = 8 j + r0, k = 16 s + 2 q (+1) (+8)
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int s2 = 0; s2 < 2; ++s2)
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                const int k0 = 16 * s2 + 2 * q + 8 * hh;
-                const float w0 = k0 < 27 ? __ldg(wgt + (8 * j + r0) * 27 + k0) : 0.f;
-                const float w1 = k0 + 1 < 27 ? __ldg(wgt + (8 * j + r0) * 27 + k0 + 1) : 0.f;
-                bfrag[j][s2][hh] = pack_bf16(w0, w1);
-            }
-    float bs[8][2];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { bs[j][0] = __ldg(bias + 8 * j + 2 * q); bs[j][1] = __ldg(bias + 8 * j + 2 * q + 1); }
-    __syncthreads();
-    const float* srow = s_in + warp * kRowF;             // this warp's output row of the tile (ty = warp)
+    const float* srow = s_in + warp * kRowF;            // this warp's output row of the tile (ty = warp)
 #pragma unroll 1
     for (int mt = 0; mt < kF_TW / 16; ++mt) {
         uint32_t afrag[2][4];
@@ -371,13 +264,17 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_amax_kernel(const v
         if (y < H && x < W) {
             const uint4 v = (y < eh && x < ew) ? reinterpret_cast<const uint4*>(s_out + p * 32)[ch ^ (p & 7)] : make_uint4(0, 0, 0, 0);
             reinterpret_cast<uint4*>(out + (((size_t)n * H + y) * W + x) * 64)[ch] = v;
-            const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+            if constexpr (kAmax) {
+                const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-            for (int k = 0; k < 4; ++k) mx = max(mx, max(w4[k] & 0x7fffu, (w4[k] >> 16) & 0x7fffu));
+                for (int k = 0; k < 4; ++k) mx = max(mx, max(w4[k] & 0x7fffu, (w4[k] >> 16) & 0x7fffu));
+            }
         }
     }
-    mx = __reduce_max_sync(0xffffffffu, mx);     // max of non-negative float bits: order-independent
-    if (lane == 0 && mx != 0) atomicMax(amax + n, mx << 16);
+    if constexpr (kAmax) {
+        mx = __reduce_max_sync(0xffffffffu, mx);     // max of non-negative float bits: order-independent
+        if (lane == 0 && mx != 0) atomicMax(amax + n, mx << 16);
+    }
 }
 
 // ------------------------------------------------------------------ fp32 parity conv
@@ -492,35 +389,22 @@ cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_o
                               __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo, int N, int H, int W, const int* ext,
                               cudaStream_t s, unsigned* amax) {
     dim3 grid((W + kF_TW - 1) / kF_TW, (H + kF_TH - 1) / kF_TH, N);
-    if (amax != nullptr) {          // fp8 mode: the bf16 tensor-core kernel, recording amax
-        if (out_lo != nullptr) return cudaErrorInvalidValue;
-        switch (in_is_u8_hwc) {
-            case kPreNone: conv_first_mma_amax_kernel<kPreNone><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax); break;
-            case kPreRtpose: conv_first_mma_amax_kernel<kPreRtpose><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax); break;
-            case kPreVgg: conv_first_mma_amax_kernel<kPreVgg><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax); break;
-            case kPreInception: conv_first_mma_amax_kernel<kPreInception><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax); break;
-            case kPreSsd: conv_first_mma_amax_kernel<kPreSsd><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax); break;
-            default: return cudaErrorInvalidValue;
-        }
-        return cudaGetLastError();
-    }
-    if (out_lo == nullptr) {        // bf16 mode: tensor cores
-        switch (in_is_u8_hwc) {
-            case kPreNone: conv_first_mma_kernel<kPreNone><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext); break;
-            case kPreRtpose: conv_first_mma_kernel<kPreRtpose><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext); break;
-            case kPreVgg: conv_first_mma_kernel<kPreVgg><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext); break;
-            case kPreInception: conv_first_mma_kernel<kPreInception><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext); break;
-            case kPreSsd: conv_first_mma_kernel<kPreSsd><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext); break;
-            default: return cudaErrorInvalidValue;
-        }
-        return cudaGetLastError();
-    }
+    if (amax != nullptr && out_lo != nullptr) return cudaErrorInvalidValue;
+    auto launch = [&](auto pre) {
+        constexpr int kIn = decltype(pre)::value;
+        if (amax != nullptr)            // fp8 mode: the bf16 tensor-core kernel, recording amax
+            conv_first_mma_kernel<kIn, true><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax);
+        else if (out_lo == nullptr)     // bf16 mode: tensor cores
+            conv_first_mma_kernel<kIn, false><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, nullptr);
+        else                            // bf16x3 mode: fp32 CUDA cores, residual plane
+            conv_first_kernel<kIn><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext);
+    };
     switch (in_is_u8_hwc) {
-        case kPreNone: conv_first_kernel<kPreNone><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext); break;
-        case kPreRtpose: conv_first_kernel<kPreRtpose><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext); break;
-        case kPreVgg: conv_first_kernel<kPreVgg><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext); break;
-        case kPreInception: conv_first_kernel<kPreInception><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext); break;
-        case kPreSsd: conv_first_kernel<kPreSsd><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext); break;
+        case kPreNone: launch(std::integral_constant<int, kPreNone>()); break;
+        case kPreRtpose: launch(std::integral_constant<int, kPreRtpose>()); break;
+        case kPreVgg: launch(std::integral_constant<int, kPreVgg>()); break;
+        case kPreInception: launch(std::integral_constant<int, kPreInception>()); break;
+        case kPreSsd: launch(std::integral_constant<int, kPreSsd>()); break;
         default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();

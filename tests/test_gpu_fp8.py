@@ -294,6 +294,23 @@ def test_fp8_launch_count_of_every_entry_point_equals_bf16(layer_net):
                 packed.ctypes.data, False, [f.shape[:2] for f in raw], (0.5, 1.0), 96, 8, 0.1, True), pe.fetch_arrays()),
         }
 
+    # launches per call: conv1_1 + 51 tensor-core layers per forward, 1 crop (crop_with_factor or the ragged frame copy)
+    # and 1 mirror of the raw frames, 2 flip merges and 2 resize-accumulates (heat, PAF) per scale, 3 of post-processing
+    # (peaks, limbs, assembly); the raw entry points all run with flip, the multi-scale ones at 2 scales
+    fwd, crop, mirror, merge, resize, post = 52, 1, 1, 2, 2, 3
+    want = {
+        "net_forward": fwd,
+        "net_forward_u8": fwd,
+        "net_forward_ragged_u8": crop + fwd,
+        "infer": fwd + post,
+        "infer_u8": fwd + post,
+        "infer_flip": mirror + fwd + merge + post,
+        "infer_u8_flip": mirror + fwd + merge + post,
+        "infer_raw_u8": mirror + crop + fwd + merge + post,
+        "infer_raw_u8_ragged": mirror + crop + fwd + merge + post,
+        "infer_raw_u8_multiscale": mirror + 2 * (crop + fwd + merge + resize) + post,
+        "infer_raw_u8_multiscale_ragged": mirror + 2 * (crop + fwd + merge + resize) + post,
+    }
     deltas = {}
     for mode in ("bf16", "fp8"):
         pe = pkg_module("engine").PoseEngine.from_net(layer_net, mode=mode, batch_cap=8, peak_cap=1024, human_cap=2048)
@@ -304,8 +321,10 @@ def test_fp8_launch_count_of_every_entry_point_equals_bf16(layer_net):
             fn()
             torch.cuda.synchronize()
             deltas[(mode, name)] = nat.launch_count() - c0
-    for name in calls(None, "bf16"):
-        assert deltas[("fp8", name)] == deltas[("bf16", name)] > 0, (name, deltas[("fp8", name)], deltas[("bf16", name)])
+    assert set(want) == set(calls(None, "bf16"))
+    for name in want:
+        assert deltas[("fp8", name)] == deltas[("bf16", name)] == want[name], \
+            (name, deltas[("fp8", name)], deltas[("bf16", name)], want[name])
 
 
 def test_fp8_harness_exact_integer_cases_and_accumulator_characterisation(built):
