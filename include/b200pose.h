@@ -41,8 +41,13 @@ typedef struct b200pose_net b200pose_net;
 #define B200POSE_MODE_FP8 3        /* fp8 tensor-core mode: the 51 wgmma convolutions run on e4m3 operands, activations
                                       scaled by 2^ea per (launch, image) from the max |bf16| their writers stored, weights
                                       by 2^ew per output channel; activations stay bf16 in memory and conv1_1 runs as in
-                                      bf16 mode (DESIGN.md 2.3).  Before this mode existed, 3 ran as bf16; every other
-                                      value outside 0 .. 3 still does.                                                 */
+                                      bf16 mode (DESIGN.md 2.3).  Before this mode existed, 3 ran as bf16.             */
+#define B200POSE_MODE_FP16 4       /* fp16 tensor-core mode: the bf16 plan with IEEE binary16 activations and weights
+                                      (10 mantissa bits against bf16's 7), fp32 full-K accumulation; fp32 stage maps.
+                                      binary16 overflows above 65504: every forward flags each image whose input or a
+                                      stored value is +-inf or NaN in binary16, and weights beyond it are refused (b200pose_net_overflow, b200pose_post_overflow), the maps
+                                      of a flagged image are not to be trusted (DESIGN.md 2.3).  Before this mode existed,
+                                      4 ran as bf16; every value outside 0 .. 4 still does.                            */
 
 int b200pose_net_create(b200pose_net** out, int cuda_device);
 void b200pose_net_destroy(b200pose_net* net);
@@ -87,7 +92,7 @@ int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frame
  * event pair around every launch; fills per-launch milliseconds and ALGORITHMIC FLOPs (2 x MACs of the unpadded
  * convolution).  Returns the number of launches, < 0 on error. */
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream);
-/* Test hooks of the last bf16 / bf16x3 / fp8 forward's launch list (launch 0 = conv1_1, 1 .. 51 = the tensor-core launches);
+/* Test hooks of the last bf16 / bf16x3 / fp8 / fp16 forward's launch list (launch 0 = conv1_1, 1 .. 51 = the tensor-core launches);
  * they let a test check one launch against a reference computed from that launch's real inputs.
  *   b200pose_net_debug_run    : re-runs the first `launches` launches on the last forward's input (plain launches with
  *                               the plan's own arguments, PDL included, no graph), then synchronises the stream.
@@ -96,11 +101,15 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
  *       4 output buffer id  5 out_cstride  6, 7 out_ch_off[2]  8, 9 store_ch[2]  10 H  11 W  12 ksize  13 cin_blocks
  *       14 groups  15 n_tile  16 n_tiles  17 relu  18 pool  19 split  20 chunk  21 pdl  22 tps
  *       23, 24 fp32 stage map written per group (-1 = none)  25 images  26 uint8 input normalisation (launch 0; 0 = fp32)
- *     Returns the number of fields.
+ *     cap >= B200POSE_DEBUG_LAUNCH_FIELDS.  With cap >= 28 it also writes
+ *       27 (B200POSE_DEBUG_LAUNCH_FORMAT) format of the 16-bit activation planes: 0 bfloat16, 1 IEEE binary16 (fp16 mode)
+ *     Returns the number of fields written.
  *   b200pose_net_debug_read   : copies images [img0, img0 + count) of one buffer to host memory: ids 0 .. 13 are the
  *     bf16 NHWC activation buffers t1, t2, t3, t4, t5a, t5b, t6, t7, t8, t9, cat, bra, brb, br512 (lo_plane = 1: their
- *     residual planes, bf16x3 only), 14 .. 25 the fp32 NCHW stage maps in saved_for_loss order. */
+ *     residual planes, bf16x3 only), 14 .. 25 the fp32 NCHW stage maps in saved_for_loss order.  The activation
+ *     buffers hold bfloat16 bits, or binary16 bits after an fp16 forward (debug_launch field 27). */
 #define B200POSE_DEBUG_LAUNCH_FIELDS 27
+#define B200POSE_DEBUG_LAUNCH_FORMAT 27
 int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream);
 int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap);
 int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes);
@@ -109,6 +118,10 @@ int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, 
  * exponent ew of each packed output row (w_exp[cap], rows = groups * n_tiles * n_tile; pad rows 0).  Returns the number
  * of rows, < 0 on error. */
 int b200pose_net_debug_fp8(b200pose_net* net, int launch, int* act_exp, int n_img, int* w_exp, int cap);
+/* fp16 overflow report of the last forward (any entry point): waits for cuda_stream, then flags[i] = 1 if image i
+ * (n = the forward's batch; flip: frames, then mirrors) stored a value beyond binary16's range (+-inf or NaN) in any
+ * layer, else 0.  Forwards of the other modes flag nothing.  Returns the number of flagged images, < 0 on error. */
+int b200pose_net_overflow(b200pose_net* net, int* flags, int n, void* cuda_stream);
 /* Device pointers of the last forward's stage-6 maps (NCHW fp32), valid until the next forward. */
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w);
 
@@ -156,6 +169,9 @@ int b200pose_post_debug_maps(b200pose_post* post, float* heat, long heat_floats,
 int b200pose_post_status_accum(b200pose_post* post, int reset);
 int b200pose_post_num_humans(b200pose_post* post, int img);             /* < 0 on error */
 int b200pose_post_status(b200pose_post* post, int img);                 /* status bits of the last run */
+/* fp16 mode: 1 if the network overflowed binary16 for frame img of the selected fused run (in any forward of it: either
+ * orientation with flip, any scale), else 0 (always 0 for other modes and for b200pose_post_run).  < 0 on error. */
+int b200pose_post_overflow(b200pose_post* post, int img);
 int b200pose_post_get_humans(b200pose_post* post, int img, float* out, int max_humans);   /* returns count */
 /* joint list rows (x, y, score, id, part), the array paf_to_pose.py:376-378 builds; returns count */
 int b200pose_post_get_peaks(b200pose_post* post, int img, float* out, int max_peaks);

@@ -11,8 +11,8 @@ _lib = None
 c_float_p = ctypes.POINTER(ctypes.c_float)
 NUM_TENSORS = 184
 HUMAN_FLOATS = 73
-MODE_BF16, MODE_FP32, MODE_BF16X3, MODE_FP8 = 0, 1, 2, 3
-MODES = {"bf16": MODE_BF16, "fp32": MODE_FP32, "bf16x3": MODE_BF16X3, "fp8": MODE_FP8}
+MODE_BF16, MODE_FP32, MODE_BF16X3, MODE_FP8, MODE_FP16 = 0, 1, 2, 3, 4
+MODES = {"bf16": MODE_BF16, "fp32": MODE_FP32, "bf16x3": MODE_BF16X3, "fp8": MODE_FP8, "fp16": MODE_FP16}
 PREPROCESS = {"rtpose": 1, "vgg": 2, "inception": 3, "ssd": 4}      # get_outputs' `preprocess` names
 
 
@@ -35,6 +35,7 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_net_debug_launch": ([vp, ci, vp, ci], ci),
     "b200pose_net_debug_read": ([vp, ci, ci, ci, ci, vp, cl], ci),
     "b200pose_net_debug_fp8": ([vp, ci, vp, ci, vp, ci], ci),
+    "b200pose_net_overflow": ([vp, vp, ci, vp], ci),
     "b200pose_net_last_maps": ([vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(ci), ctypes.POINTER(ci),
                                 ctypes.POINTER(ci)], ci),
     "b200pose_post_create": ([ctypes.POINTER(vp), ci, ci, ci, ci], ci),
@@ -49,6 +50,7 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_post_debug_maps": ([vp, vp, cl, vp, cl], ci),
     "b200pose_post_num_humans": ([vp, ci], ci),
     "b200pose_post_status": ([vp, ci], ci),
+    "b200pose_post_overflow": ([vp, ci], ci),
     "b200pose_post_get_humans": ([vp, ci, vp, ci], ci),
     "b200pose_post_get_peaks": ([vp, ci, vp, ci], ci),
     "b200pose_infer": ([vp, vp, vp, ci, ci, ci, ci, ci, cf, vp], ci),

@@ -18,6 +18,7 @@
 #include "../../include/b200pose.h"
 #include "conv_misc.cuh"
 #include "conv_tc.cuh"
+#include "f16_core.h"
 #include "fp8_core.h"
 #include "postprocess.cuh"
 #include "resize.cuh"
@@ -139,6 +140,8 @@ struct TcLayer {            // one grouped tensor-core launch
     uint8_t* w8 = nullptr;        // [taps][rows][cin_blocks*64] e4m3(w * 2^ew[row]), K order fp8_k_to_channel
     int* w_exp = nullptr;         // ew per row (device)
     std::vector<int> h_w_exp;     // ... and its host copy (b200pose_net_debug_fp8)
+    // fp16 mode, packed at the first fp16 plan build (pack_f16_layer):
+    uint16_t* w16 = nullptr;      // [taps][rows][cin_blocks*64] binary16(w)
 };
 
 // Activation buffers (the buffer ids of the test hooks): channels per pixel and spatial divisor.
@@ -196,13 +199,14 @@ struct PlanLaunch {
 };
 
 // Device addresses a plan's tensor maps and arguments point into: activation buffers, residual planes, stage maps.
-using PlanBuffers = std::array<const void*, 2 * kNumAct + 12 + 2>;    // + the fp8 amax and exponent tables
+using PlanBuffers = std::array<const void*, 2 * kNumAct + 12 + 3>;    // + the fp8 amax and exponent tables, fp16 flags
 
 // The launch list of one (n, H, W, mode) key, valid while `buffers` are still the net's.
 struct Plan {
     int n, H, W, mode;
     bool split;            // bf16x3
     bool fp8;
+    bool f16;              // fp16: binary16 activation planes and weights
     std::vector<PlanLaunch> launches;
     PlanBuffers buffers;
 };
@@ -255,6 +259,9 @@ struct b200pose_net {
     // image; zeroed at the start of every fp8 forward
     DevBuf<unsigned> amax;
     DevBuf<int> ea;                    // ea[launch * n + image]: the activation exponent the fp8 kernel used
+    // fp16 mode: ovf[image] = 1 when a launch stored a value beyond binary16's range for the image; zeroed at the start
+    // of every fp16 forward
+    DevBuf<unsigned> ovf;
 };
 
 struct b200pose_post {
@@ -290,6 +297,11 @@ struct b200pose_post {
     // geometry of every (scale, frame)
     DevBuf<int> ms_ext;
     DevBuf<RaggedResize> ms_resize;
+    // fp16 overflow flags of the fused runs, slot = run parity: one row of 2 * batch_cap images per forward of the run (a
+    // multi-scale run makes one forward per scale), copied from the net's flags behind each forward
+    unsigned* hp_ovf[2] = {nullptr, nullptr};
+    int ovf_rows[2] = {0, 0}, ovf_imgs[2] = {0, 0};    // forwards copied, images per forward (2n with flip)
+    int ovf_pending = 0, ovf_pending_imgs = 0;          // ... of the run being enqueued
 };
 
 namespace {
@@ -371,6 +383,34 @@ int pack_fp8_layer(const b200pose_net* net, TcLayer& L) {
     return 0;
 }
 
+// fp16 mode: a weight beyond binary16's range would be +-inf, and inf * 0 = NaN sums can be turned into a finite 0 by
+// the ReLU, i.e. not reported by the overflow flags; such weights are refused instead.
+int check_f16_weight(float w, int conv) {
+    const uint16_t h = f16_rn_bits(w);
+    if ((h & 0x7c00u) == 0x7c00u) return fail("fp16 mode: conv %d has weight %g, beyond binary16's range (65504)", conv, w);
+    return 0;
+}
+
+// fp16 weights of layer L, packed when the first fp16 plan is built: binary16(w), one rounding from the fp32 weight, in
+// the layout of the bf16 value slices (pad rows and channels 0).
+int pack_f16_layer(const b200pose_net* net, TcLayer& L) {
+    const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, rows = L.groups * L.n_tiles * L.n_tile;
+    std::vector<uint16_t> w16((size_t)taps * rows * cin_pad, 0);
+    int rc = 0;
+    for_each_weight_row(net, L, [&](int g, int, int r, const float* wr) {
+        for (int t = 0; t < taps; ++t)
+            for (int k = 0; k < cin_pad; ++k) {
+                const float w = wr[(size_t)t * cin_pad + k];
+                if (rc == 0) rc = check_f16_weight(w, L.convs[g]);
+                w16[((size_t)t * rows + r) * cin_pad + k] = f16_rn_bits(w);
+            }
+    });
+    if (rc) return rc;
+    CU(cudaMalloc(&L.w16, w16.size() * 2));
+    CU(cudaMemcpy(L.w16, w16.data(), w16.size() * 2, cudaMemcpyHostToDevice));
+    return 0;
+}
+
 // Small-batch plans: the 46 x 46 stage layers (two groups) would fill at most half of the SMs with one n-tile per group.
 // Their launches are the launch-bound part of the product: they are chained by PDL and replayed as a CUDA graph; the large
 // plans are GPU-bound and get neither (a capture only adds a CPU hiccup).
@@ -406,6 +446,10 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         a.w_exp = L.w_exp;
         a.ea_out = net->ea.p + (size_t)slot * n;
     }
+    if (p.f16) {
+        a.f16 = 1;
+        a.ovf_out = net->ovf.p;
+    }
     a.out = net->act[wr.out].p; a.out_cstride = kActC[wr.out];
     a.out_ch_off[0] = wr.out_off[0]; a.out_ch_off[1] = wr.out_off[1];
     a.store_ch[0] = wr.store[0]; a.store_ch[1] = wr.store[1];
@@ -426,14 +470,16 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         in_lo = net->act_lo[wr.in].p;
         a.out_lo = net->act_lo[wr.out].p;
     }
-    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], p.fp8 ? (const void*)L.w8 : L.w, in_lo);
+    const void* w = p.fp8 ? (const void*)L.w8 : (p.f16 ? (const void*)L.w16 : L.w);
+    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], w, in_lo);
     if (e != cudaSuccess) return fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
     p.launches.push_back({a, 2.0 * n * H * W * L.macs_per_pixel, wr.in, wr.out, {f32[0], f32[1]}});
     return 0;
 }
 
-// fp8: the plan also points into the amax and exponent tables (only fp8 plans do, so only they depend on them)
-PlanBuffers plan_buffers(const b200pose_net* net, bool fp8) {
+// fp8: the plan also points into the amax and exponent tables, fp16 into the overflow flags (only plans of that mode
+// do, so only they depend on them)
+PlanBuffers plan_buffers(const b200pose_net* net, bool fp8, bool f16) {
     PlanBuffers b;
     for (int i = 0; i < kNumAct; ++i) {
         b[i] = net->act[i].p;
@@ -442,6 +488,7 @@ PlanBuffers plan_buffers(const b200pose_net* net, bool fp8) {
     for (int i = 0; i < 12; ++i) b[2 * kNumAct + i] = net->out_f32[i].p;
     b[2 * kNumAct + 12] = fp8 ? net->amax.p : nullptr;
     b[2 * kNumAct + 13] = fp8 ? net->ea.p : nullptr;
+    b[2 * kNumAct + 14] = f16 ? net->ovf.p : nullptr;
     return b;
 }
 
@@ -462,6 +509,13 @@ int build_plan_bf16(b200pose_net* net, Plan& p, cudaStream_t st) {
         for (TcLayer& L : net->tc)
             if (L.w8 == nullptr && pack_fp8_layer(net, L)) return 1;
     }
+    if (p.f16) {
+        CU(net->ovf.ensure((size_t)p.n));
+        for (float w : net->host_w[0])      // conv1_1 converts its fp32 weights in the kernel
+            if (check_f16_weight(w, 0)) return 1;
+        for (TcLayer& L : net->tc)
+            if (L.w16 == nullptr && pack_f16_layer(net, L)) return 1;
+    }
     // fp8: the launch that last wrote each buffer (amax table row); the concat buffer has two writers, conv4_4_CPM
     // (features) and the latest stage head (PAF + heatmap)
     int writer[kNumAct], cat_head = -1;
@@ -480,7 +534,7 @@ int build_plan_bf16(b200pose_net* net, Plan& p, cudaStream_t st) {
     for (int s = 1; s <= 6; ++s)
         for (int li = 0; li < stage_num_layers(s); ++li)
             if (add(net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], s - 1)) return 1;
-    p.buffers = plan_buffers(net, p.fp8);
+    p.buffers = plan_buffers(net, p.fp8, p.f16);
     return 0;
 }
 
@@ -494,7 +548,7 @@ void drop_graphs(b200pose_net* net) {
 // oldest of 32 is dropped).  A build may move the buffers the captured graphs point into: it synchronises the stream
 // and drops the graphs first.
 int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t st) {
-    const PlanBuffers bufs = plan_buffers(net, mode == B200POSE_MODE_FP8);
+    const PlanBuffers bufs = plan_buffers(net, mode == B200POSE_MODE_FP8, mode == B200POSE_MODE_FP16);
     for (const Plan& p : net->plans)
         if (p.n == n && p.H == H && p.W == W && p.mode == mode && p.buffers == bufs) {
             net->plan = &p;
@@ -505,7 +559,8 @@ int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t s
     net->plan = nullptr;
     net->plans.remove_if([&](const Plan& p) { return p.n == n && p.H == H && p.W == W && p.mode == mode; });
     if (net->plans.size() >= 32) net->plans.pop_front();
-    net->plans.push_back(Plan{n, H, W, mode, mode == B200POSE_MODE_BF16X3, mode == B200POSE_MODE_FP8, {}, {}});
+    net->plans.push_back(Plan{n, H, W, mode, mode == B200POSE_MODE_BF16X3, mode == B200POSE_MODE_FP8,
+                              mode == B200POSE_MODE_FP16, {}, {}});
     if (build_plan_bf16(net, net->plans.back(), st)) {
         net->plans.pop_back();
         return 1;
@@ -515,16 +570,18 @@ int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t s
 }
 
 // The first k launches of a forward with net->plan: conv1_1, then the plan's.  A ragged forward passes its extents
-// table (the plans are shared with uniform batches of the canvas size).  fp8: zero_amax clears the amax table first (a
-// memset, not a launch); re-runs of launches (debug_run, profile) leave it as it is - they record the same maxima again.
+// table (the plans are shared with uniform batches of the canvas size).  fp8 / fp16: zero_amax clears the amax table /
+// the overflow flags first (a memset, not a launch); re-runs of launches (debug_run, profile) leave them as they are -
+// they record the same maxima and flags again.
 // after (b200pose_net_profile): after[i] is recorded behind launch i.
 int launch_forward_bf16(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st,
                         bool zero_amax = false, const cudaEvent_t* after = nullptr) {
     const Plan& p = *net->plan;
     if (p.fp8 && zero_amax) CU(cudaMemsetAsync(net->amax.p, 0, (size_t)(1 + p.launches.size()) * p.n * sizeof(unsigned), st));
+    if (p.f16 && zero_amax) CU(cudaMemsetAsync(net->ovf.p, 0, (size_t)p.n * sizeof(unsigned), st));
     if (k >= 1) {
         CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr,
-                             p.n, p.H, p.W, ext, st, p.fp8 ? net->amax.p : nullptr));
+                             p.n, p.H, p.W, ext, st, p.fp8 ? net->amax.p : nullptr, p.f16 ? net->ovf.p : nullptr));
         if (after) CU(cudaEventRecord(after[0], st));
     }
     for (int i = 0; i + 1 < k; ++i) {
@@ -684,10 +741,17 @@ void b200pose_net_destroy(b200pose_net* net) {
     cudaSetDevice(net->device);
     drop_graphs(net);
     for (int i = 0; i < kNumConvs; ++i) { if (net->d_w[i]) cudaFree(net->d_w[i]); if (net->d_b[i]) cudaFree(net->d_b[i]); }
-    for (TcLayer& L : net->tc) { if (L.w) cudaFree(L.w); if (L.bias) cudaFree(L.bias); if (L.w8) cudaFree(L.w8); if (L.w_exp) cudaFree(L.w_exp); }
+    for (TcLayer& L : net->tc) {
+        if (L.w) cudaFree(L.w);
+        if (L.bias) cudaFree(L.bias);
+        if (L.w8) cudaFree(L.w8);
+        if (L.w_exp) cudaFree(L.w_exp);
+        if (L.w16) cudaFree(L.w16);
+    }
     for (int i = 0; i < kNumAct; ++i) { net->act[i].release(); net->act_lo[i].release(); }
     net->amax.release();
     net->ea.release();
+    net->ovf.release();
     DevBuf<float>* fb[] = {&net->in_stage, &net->f_a, &net->f_b, &net->f_cat, &net->f_x, &net->f_y, &net->f_in, &net->f_u8};
     net->in_stage_u8.release();
     net->raw_stage.release();
@@ -726,7 +790,13 @@ int b200pose_net_finalize(b200pose_net* net) {
         CU(cudaMemcpy(net->d_w[i], net->host_w[i].data(), net->host_w[i].size() * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(net->d_b[i], net->host_b[i].data(), net->host_b[i].size() * 4, cudaMemcpyHostToDevice));
     }
-    for (TcLayer& L : net->tc) { if (L.w) cudaFree(L.w); if (L.bias) cudaFree(L.bias); if (L.w8) cudaFree(L.w8); if (L.w_exp) cudaFree(L.w_exp); }
+    for (TcLayer& L : net->tc) {
+        if (L.w) cudaFree(L.w);
+        if (L.bias) cudaFree(L.bias);
+        if (L.w8) cudaFree(L.w8);
+        if (L.w_exp) cudaFree(L.w_exp);
+        if (L.w16) cudaFree(L.w16);
+    }
     net->tc.assign(16 + 5 * 7, TcLayer());
     for (int i = 1; i < 12; ++i) {
         const ConvSpec s = kTrunk[i];
@@ -782,7 +852,8 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
             rc = forward_fp32(net, net->f_u8.p, n, H, W, st, ext);
         } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, st, ext);
     } else {
-        if (mode != B200POSE_MODE_BF16X3 && mode != B200POSE_MODE_FP8) mode = B200POSE_MODE_BF16;     // every other mode runs bf16
+        if (mode != B200POSE_MODE_BF16X3 && mode != B200POSE_MODE_FP8 && mode != B200POSE_MODE_FP16)
+            mode = B200POSE_MODE_BF16;     // every other mode runs bf16
         first_u8 = in_u8 ? net->preprocess : 0;
         rc = forward_bf16(net, d_in, first_u8, n, H, W, mode, st, ext);
     }
@@ -838,6 +909,9 @@ static int upload_frames(b200pose_net* net, const std::vector<RaggedFrame>& fram
     CU(cudaMemcpyAsync(net->d_frames.p, frames.data(), frames.size() * sizeof(RaggedFrame), cudaMemcpyHostToDevice, st));
     return 0;
 }
+
+// fp16 overflow rows a fused run keeps: one per forward, at most 16 scales
+constexpr int kMaxOvfRows = 16;
 
 // A batch of raw uint8 frames packed back to back, cropped for one destination size: frame table (flip: the mirrored
 // frames follow the originals, in the staging buffer and in both tables), padded extents and canvas, the frames' total
@@ -962,10 +1036,12 @@ int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream) {
 int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
     if (!net || !last_ran_plan(net)) return fail("debug_launch: no bf16 / bf16x3 forward has run");
     const Plan& p = *net->plan;
-    if (i < 0 || i > (int)p.launches.size() || cap < B200POSE_DEBUG_LAUNCH_FIELDS || !fields)
+    // fields 0 .. 26 are required; the format field is written when there is room for it
+    constexpr int kAll = B200POSE_DEBUG_LAUNCH_FORMAT + 1;
+    const int nf = cap < kAll ? cap : kAll;
+    if (i < 0 || i > (int)p.launches.size() || nf < B200POSE_DEBUG_LAUNCH_FIELDS || !fields)
         return fail("debug_launch: launch %d / capacity %d out of range", i, cap);
-    int* f = fields;
-    for (int k = 0; k < B200POSE_DEBUG_LAUNCH_FIELDS; ++k) f[k] = 0;
+    int f[kAll] = {};
     if (i == 0) {     // conv1_1 (CUDA cores / mma.sync): the network input -> t1
         f[0] = -1; f[1] = 3; f[4] = T1; f[5] = kActC[T1]; f[8] = 64;
         f[10] = p.H; f[11] = p.W; f[12] = 3; f[14] = 1; f[15] = 64; f[16] = 1; f[17] = 1;
@@ -982,7 +1058,9 @@ int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
         f[23] = l.f32[0]; f[24] = l.f32[1];
     }
     f[25] = p.n;
-    return B200POSE_DEBUG_LAUNCH_FIELDS;
+    f[B200POSE_DEBUG_LAUNCH_FORMAT] = p.f16 ? 1 : 0;
+    for (int k = 0; k < nf; ++k) fields[k] = f[k];
+    return nf;
 }
 
 int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes) {
@@ -1028,6 +1106,23 @@ int b200pose_net_debug_fp8(b200pose_net* net, int launch, int* act_exp, int n_im
     return rows;
 }
 
+int b200pose_net_overflow(b200pose_net* net, int* flags, int n, void* cuda_stream) {
+    if (!net || !flags) { fail("overflow: null pointer"); return -1; }
+    if (net->last.n == 0) { fail("overflow: no forward has run"); return -1; }
+    if (n != net->last.n) { fail("overflow: %d images asked, the last forward ran %d", n, net->last.n); return -1; }
+    std::vector<unsigned> h(n, 0u);
+    if (cudaSetDevice(net->device) != cudaSuccess ||
+        cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(cuda_stream)) != cudaSuccess ||
+        (net->last.mode == B200POSE_MODE_FP16 &&
+         cudaMemcpy(h.data(), net->ovf.p, n * sizeof(unsigned), cudaMemcpyDeviceToHost) != cudaSuccess)) {
+        fail("overflow: %s", cudaGetErrorString(cudaGetLastError()));
+        return -1;
+    }
+    int flagged = 0;
+    for (int i = 0; i < n; ++i) flagged += (flags[i] = h[i] != 0);
+    return flagged;
+}
+
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w) {
     if (!net || net->last.n == 0) return fail("no forward has run");
     *paf = net->out_f32[10].p; *heat = net->out_f32[11].p;
@@ -1059,6 +1154,7 @@ int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, in
         CU(cudaHostAlloc(&p->hp_humans[b], (size_t)batch_cap * human_cap * kHumanFloats * sizeof(float), cudaHostAllocMapped | cudaHostAllocPortable));   // written by assemble_kernel (same pointer on the device: unified addressing)
         CU(cudaEventCreateWithFlags(&p->ev_ld[b], cudaEventDisableTiming));
         CU(cudaMalloc(&p->d_ext[b], (size_t)batch_cap * 2 * sizeof(int)));
+        CU(cudaHostAlloc(&p->hp_ovf[b], (size_t)kMaxOvfRows * 2 * batch_cap * sizeof(unsigned), cudaHostAllocDefault));
     }
     CU(cudaEventCreateWithFlags(&p->ev_maps, cudaEventDisableTiming));
     *out = p;
@@ -1083,6 +1179,7 @@ void b200pose_post_destroy(b200pose_post* p) {
         if (p->hp_counts[b]) cudaFreeHost(p->hp_counts[b]);
         if (p->hp_humans[b]) cudaFreeHost(p->hp_humans[b]);
         if (p->d_ext[b]) cudaFree(p->d_ext[b]);
+        if (p->hp_ovf[b]) cudaFreeHost(p->hp_ovf[b]);
     }
     if (p->ev_limbs) cudaEventDestroy(p->ev_limbs);
     if (p->ev_asm) cudaEventDestroy(p->ev_asm);
@@ -1108,6 +1205,9 @@ static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st) 
     CU(cudaMemcpyAsync(p->hp_counts[b], pb.counts, (size_t)n * 18 * sizeof(int), cudaMemcpyDeviceToHost, p->s2));
     CU(cudaEventRecord(p->ev_fetch[b], p->s2));
     p->slot_n[b] = n;
+    p->ovf_rows[b] = p->ovf_pending;
+    p->ovf_imgs[b] = p->ovf_pending_imgs;
+    p->ovf_pending = 0;
     p->runs += 1;
     p->h_px.clear();
     return 0;
@@ -1167,6 +1267,7 @@ int b200pose_post_run(b200pose_post* p, const float* heat, const float* paf, int
     if (!p) return fail("null post");
     CU(cudaSetDevice(p->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    p->ovf_pending = 0;      // maps from the caller: no network ran in this run
     const float *dh = heat, *dp = paf;
     if (!on_device) {
         CU(p->d_heat.ensure((size_t)n * 19 * h * w));
@@ -1244,6 +1345,14 @@ static int post_ready(b200pose_post* p, int img) {
 }
 int b200pose_post_num_humans(b200pose_post* p, int img) { return post_ready(p, img) ? p->hp_nh[p->cur][img] : -1; }
 int b200pose_post_status(b200pose_post* p, int img) { return post_ready(p, img) ? p->hp_status[p->cur][img] : -1; }
+int b200pose_post_overflow(b200pose_post* p, int img) {
+    if (!post_ready(p, img)) return -1;
+    const int b = p->cur, n = p->slot_n[b];
+    const unsigned* h = p->hp_ovf[b];
+    for (int k = 0; k < p->ovf_rows[b]; ++k, h += 2 * (size_t)p->pb.batch_cap)
+        if (h[img] || (p->ovf_imgs[b] == 2 * n && h[n + img])) return 1;
+    return 0;
+}
 int b200pose_post_get_humans(b200pose_post* p, int img, float* out, int max_humans) {
     if (!post_ready(p, img)) return -1;
     const int n = p->hp_nh[p->cur][img] < max_humans ? p->hp_nh[p->cur][img] : max_humans;
@@ -1333,6 +1442,19 @@ static int check_infer(const b200pose_net* net, const b200pose_post* post) {
     return 0;
 }
 
+// fp16: behind a fused run's forward of nimg images, copies the net's overflow flags into the next row of the run's slot
+// (b200pose_post_overflow reads them once the run is fetched).  Stream-ordered before the run's post-processing, whose
+// completion the fetch waits for.
+static int stash_overflow(const b200pose_net* net, b200pose_post* post, int nimg, cudaStream_t st) {
+    if (net->last.mode != B200POSE_MODE_FP16) return 0;
+    if (post->ovf_pending >= kMaxOvfRows || nimg > 2 * post->pb.batch_cap) return fail("overflow rows exhausted");
+    unsigned* dst = post->hp_ovf[post->runs & 1] + (size_t)post->ovf_pending * 2 * post->pb.batch_cap;
+    CU(cudaMemcpyAsync(dst, net->ovf.p, nimg * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    post->ovf_pending += 1;
+    post->ovf_pending_imgs = nimg;
+    return 0;
+}
+
 // Flip TTA: merges the last forward's 2n images [frames | mirrors] of stage-6 maps into n maps at oh / op.
 static int merge_last_flip(const b200pose_net* net, int n, float* oh, float* op, cudaStream_t st) {
     const int h = net->last.H / 8, w = net->last.W / 8;
@@ -1360,6 +1482,7 @@ static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input,
     if (int rc = check_infer(net, post)) return rc;
     if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
     if (int rc = check_batch(post, n)) return rc;
+    post->ovf_pending = 0;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (flip) {   // the 2n batch [frames | mirrored frames] is assembled in the net's staging buffer
@@ -1383,6 +1506,7 @@ static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input,
     // host input is staged asynchronously: the caller keeps it alive until b200pose_post_sync()
     if (int rc = net_forward_impl(net, input, in_u8, input_on_device, flip ? 2 * n : n, H, W, mode, nullptr, 1, st, false))
         return rc;
+    if (int rc = stash_overflow(net, post, flip ? 2 * n : n, st)) return rc;
     return finish_infer(net, post, n, flip, thresh, st);
 }
 
@@ -1491,6 +1615,7 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
     if (scales && (n_scales < 1 || n_scales > 16)) return fail("infer_raw: %d scales (1 .. 16)", n_scales);
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
     const bool ragged = src_hw != nullptr;
+    post->ovf_pending = 0;
     // every scale's geometry first: an invalid frame size fails before anything is enqueued
     RawBatch base;
     if (scales && raw_batch(n, src_h, src_w, src_hw, base_size, factor, 0, &base)) return 1;
@@ -1519,6 +1644,7 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
     const int nimg = flip ? 2 * n : n;
     if (!scales) {
         if (int rc = crop_and_forward(net, d_raw, nimg, sc[0], mode, st)) return rc;
+        if (int rc = stash_overflow(net, post, nimg, st)) return rc;
         return finish_infer(net, post, n, flip, thresh, st);
     }
     if (ragged) {
@@ -1534,6 +1660,7 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
         const RawBatch& c = sc[k];
         if (ragged && k > 0 && upload_frames(net, c.tab, st)) return 1;
         if (int rc = crop_and_forward(net, d_raw, nimg, c, mode, st)) return rc;
+        if (int rc = stash_overflow(net, post, nimg, st)) return rc;
         const int h = c.Hc / 8, w = c.Wc / 8;
         const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
         const float *s_heat = net->out_f32[11].p, *s_paf = net->out_f32[10].p;

@@ -14,6 +14,7 @@
 
 #include "conv_misc.cuh"
 #include "preprocess_core.h"
+#include "ptx.cuh"
 
 namespace b2p {
 
@@ -158,10 +159,23 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&v);
 }
+// fp16 mode: the same fragments in binary16
+__device__ __forceinline__ void mma_f16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+template <bool kF16> __device__ __forceinline__ uint32_t pack16(float lo, float hi) {
+    if constexpr (kF16) return pack_f16x2(lo, hi);
+    else return pack_bf16(lo, hi);
+}
 
 // fp8 mode (DESIGN.md §2.3): kAmax also records each image's max |stored bf16| (fp32 bits, atomic max) in amax[n] for
-// the next launch's activation scale.
-template <int kIn, bool kAmax>
+// the next launch's activation scale.  fp16 mode (kF16): inputs, weights and outputs are binary16, and amax[n] is the
+// image's overflow flag, set to 1 when an input value (an fp32 input beyond 65504, or NaN) or a stored value is not
+// finite in binary16 - an infinite input can give NaN sums, which the ReLU would turn into a finite 0.
+template <int kIn, bool kAmax, bool kF16>
 __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* __restrict__ in_v, const float* __restrict__ wgt,
                                                                     const float* __restrict__ bias,
                                                                     __nv_bfloat16* __restrict__ out, int H, int W,
@@ -221,13 +235,14 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
                 const int k0 = 16 * s2 + 2 * q + 8 * hh;
                 const float w0 = k0 < 27 ? __ldg(wgt + (8 * j + r0) * 27 + k0) : 0.f;
                 const float w1 = k0 + 1 < 27 ? __ldg(wgt + (8 * j + r0) * 27 + k0 + 1) : 0.f;
-                bfrag[j][s2][hh] = pack_bf16(w0, w1);
+                bfrag[j][s2][hh] = pack16<kF16>(w0, w1);
             }
     float bs[8][2];
 #pragma unroll
     for (int j = 0; j < 8; ++j) { bs[j][0] = __ldg(bias + 8 * j + 2 * q); bs[j][1] = __ldg(bias + 8 * j + 2 * q + 1); }
     __syncthreads();
     const float* srow = s_in + warp * kRowF;            // this warp's output row of the tile (ty = warp)
+    uint32_t bad_in = 0;                                 // fp16: a non-finite binary16 input fragment
 #pragma unroll 1
     for (int mt = 0; mt < kF_TW / 16; ++mt) {
         uint32_t afrag[2][4];
@@ -240,20 +255,28 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
                 v[j][0] = off >= 0 ? srow[off + 16 * mt + r0] : 0.f;
                 v[j][1] = off >= 0 ? srow[off + 16 * mt + r0 + 8] : 0.f;
             }
-            afrag[s2][0] = pack_bf16(v[0][0], v[1][0]);  // row r0,     k = 2q, 2q+1
-            afrag[s2][1] = pack_bf16(v[0][1], v[1][1]);  // row r0 + 8, k = 2q, 2q+1
-            afrag[s2][2] = pack_bf16(v[2][0], v[3][0]);  // row r0,     k = 2q+8, 2q+9
-            afrag[s2][3] = pack_bf16(v[2][1], v[3][1]);  // row r0 + 8, k = 2q+8, 2q+9
+            afrag[s2][0] = pack16<kF16>(v[0][0], v[1][0]);  // row r0,     k = 2q, 2q+1
+            afrag[s2][1] = pack16<kF16>(v[0][1], v[1][1]);  // row r0 + 8, k = 2q, 2q+1
+            afrag[s2][2] = pack16<kF16>(v[2][0], v[3][0]);  // row r0,     k = 2q+8, 2q+9
+            afrag[s2][3] = pack16<kF16>(v[2][1], v[3][1]);  // row r0 + 8, k = 2q+8, 2q+9
+            if constexpr (kF16)
+                bad_in |= f16x2_nonfinite(afrag[s2][0]) | f16x2_nonfinite(afrag[s2][1]) | f16x2_nonfinite(afrag[s2][2]) |
+                          f16x2_nonfinite(afrag[s2][3]);
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             float d[4] = {bs[j][0], bs[j][1], bs[j][0], bs[j][1]};
-            mma_bf16_16816(d, afrag[0], bfrag[j][0][0], bfrag[j][0][1]);
-            mma_bf16_16816(d, afrag[1], bfrag[j][1][0], bfrag[j][1][1]);
+            if constexpr (kF16) {
+                mma_f16_16816(d, afrag[0], bfrag[j][0][0], bfrag[j][0][1]);
+                mma_f16_16816(d, afrag[1], bfrag[j][1][0], bfrag[j][1][1]);
+            } else {
+                mma_bf16_16816(d, afrag[0], bfrag[j][0][0], bfrag[j][0][1]);
+                mma_bf16_16816(d, afrag[1], bfrag[j][1][0], bfrag[j][1][1]);
+            }
             // d0, d1: pixel row r0, channels 8j + 2q, +1;  d2, d3: pixel row r0 + 8
             const int p0 = warp * kF_TW + 16 * mt + r0, p1 = p0 + 8;
-            s_out[p0 * 32 + ((j ^ (p0 & 7)) << 2) + q] = pack_bf16(fmaxf(d[0], 0.f), fmaxf(d[1], 0.f));
-            s_out[p1 * 32 + ((j ^ (p1 & 7)) << 2) + q] = pack_bf16(fmaxf(d[2], 0.f), fmaxf(d[3], 0.f));
+            s_out[p0 * 32 + ((j ^ (p0 & 7)) << 2) + q] = pack16<kF16>(fmaxf(d[0], 0.f), fmaxf(d[1], 0.f));
+            s_out[p1 * 32 + ((j ^ (p1 & 7)) << 2) + q] = pack16<kF16>(fmaxf(d[2], 0.f), fmaxf(d[3], 0.f));
         }
     }
     __syncthreads();
@@ -269,11 +292,15 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
 #pragma unroll
                 for (int k = 0; k < 4; ++k) mx = max(mx, max(w4[k] & 0x7fffu, (w4[k] >> 16) & 0x7fffu));
             }
+            if constexpr (kF16) mx |= f16x2_nonfinite(v.x) | f16x2_nonfinite(v.y) | f16x2_nonfinite(v.z) | f16x2_nonfinite(v.w);
         }
     }
     if constexpr (kAmax) {
         mx = __reduce_max_sync(0xffffffffu, mx);     // max of non-negative float bits: order-independent
         if (lane == 0 && mx != 0) atomicMax(amax + n, mx << 16);
+    }
+    if constexpr (kF16) {
+        if (__any_sync(0xffffffffu, mx | bad_in) && lane == 0) atomicOr(amax + n, 1u);
     }
 }
 
@@ -387,15 +414,18 @@ __global__ void nchw_to_nhwc_f32_kernel(const float* __restrict__ in, float* __r
 
 cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias,
                               __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo, int N, int H, int W, const int* ext,
-                              cudaStream_t s, unsigned* amax) {
+                              cudaStream_t s, unsigned* amax, unsigned* ovf) {
     dim3 grid((W + kF_TW - 1) / kF_TW, (H + kF_TH - 1) / kF_TH, N);
-    if (amax != nullptr && out_lo != nullptr) return cudaErrorInvalidValue;
+    if ((amax != nullptr || ovf != nullptr) && out_lo != nullptr) return cudaErrorInvalidValue;
+    if (amax != nullptr && ovf != nullptr) return cudaErrorInvalidValue;
     auto launch = [&](auto pre) {
         constexpr int kIn = decltype(pre)::value;
         if (amax != nullptr)            // fp8 mode: the bf16 tensor-core kernel, recording amax
-            conv_first_mma_kernel<kIn, true><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax);
+            conv_first_mma_kernel<kIn, true, false><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax);
+        else if (ovf != nullptr)        // fp16 mode: binary16 operands and output, overflow flags
+            conv_first_mma_kernel<kIn, false, true><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, ovf);
         else if (out_lo == nullptr)     // bf16 mode: tensor cores
-            conv_first_mma_kernel<kIn, false><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, nullptr);
+            conv_first_mma_kernel<kIn, false, false><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, nullptr);
         else                            // bf16x3 mode: fp32 CUDA cores, residual plane
             conv_first_kernel<kIn><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext);
     };

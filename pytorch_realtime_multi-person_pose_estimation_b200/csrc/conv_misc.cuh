@@ -23,7 +23,8 @@ struct ConvF32Args {
 cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias,
                               __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo /*residual plane or null*/, int N, int H,
                               int W, const int* ext /*ragged batch: padded H, W per image, or null*/, cudaStream_t s,
-                              unsigned* amax = nullptr /*fp8 mode: per-image max |stored bf16| (fp32 bits), atomic max*/);
+                              unsigned* amax = nullptr /*fp8 mode: per-image max |stored bf16| (fp32 bits), atomic max*/,
+                              unsigned* ovf = nullptr /*fp16 mode: binary16 output; per-image flag, 1 = a value overflowed*/);
 // ext (ragged batch) or null: pixels outside image i's padded extent ext[2 i], ext[2 i + 1] become 0 (zero padding)
 cudaError_t u8hwc_to_f32nchw_launch(const unsigned char* in, float* out, int N, int H, int W, int mode, const int* ext,
                                     cudaStream_t s);

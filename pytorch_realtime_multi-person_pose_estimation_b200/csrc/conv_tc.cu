@@ -62,7 +62,8 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int N> struct Mma;
+// 16-bit operands, k16: bfloat16 (kF16 = false) or IEEE binary16
+template <int N, bool kF16 = false> struct Mma;
 template <> struct Mma<128> {
     static __device__ __forceinline__ void run(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n128k16_rs(d, a, b, s); }
 };
@@ -74,6 +75,18 @@ template <> struct Mma<48> {
 };
 template <> struct Mma<32> {
     static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n32k16_rs(d, a, b, s); }
+};
+template <> struct Mma<128, true> {
+    static __device__ __forceinline__ void run(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n128k16_f16_rs(d, a, b, s); }
+};
+template <> struct Mma<64, true> {
+    static __device__ __forceinline__ void run(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n64k16_f16_rs(d, a, b, s); }
+};
+template <> struct Mma<48, true> {
+    static __device__ __forceinline__ void run(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n48k16_f16_rs(d, a, b, s); }
+};
+template <> struct Mma<32, true> {
+    static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n32k16_f16_rs(d, a, b, s); }
 };
 template <int N> struct Mma8;      // e4m3, k32
 template <> struct Mma8<64> {
@@ -92,7 +105,9 @@ constexpr int kConsumerWarps = 8;
 // kFp8 (with kChunk): the fp8 mode (DESIGN.md §2.3) - each tap's A fragments are converted from the bf16 patch to e4m3 in
 // registers, the weights are e4m3 slices of 64-byte rows, every tap's two k32 MMAs start a fresh accumulator that is
 // then added to the fp32 sum, and the epilogue records the per-image max |stored bf16|.
-template <int N, bool kChunk, bool kRagged, bool kFp8>
+// kF16: the fp16 mode - the bf16 plan with binary16 activations and weights (same fragments, same full-K fp32
+// accumulation); the epilogue stores binary16 and flags every image for which a stored value is +-inf or NaN.
+template <int N, bool kChunk, bool kRagged, bool kFp8, bool kF16 = false>
 __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B operands need 1024 B alignment.
@@ -271,7 +286,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                             wgmma_fence();
 #pragma unroll
                             for (int k = 0; k < 4; ++k) {
-                                Mma<N>::run(acc, af[k], bdesc_hi | (b_lo + j * (b_tx >> 4) + k * 2), scale);
+                                Mma<N, kF16>::run(acc, af[k], bdesc_hi | (b_lo + j * (b_tx >> 4) + k * 2), scale);
                                 scale = 1;
                             }
                             wgmma_commit();
@@ -306,6 +321,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             const float* bias = a.bias + (tc.g * a.n_tiles + tc.nt) * N;
             const int* w_exp = a.w_exp + (tc.g * a.n_tiles + tc.nt) * N;
             uint32_t amax = 0;    // fp8: max |stored bf16| bits of this lane
+            uint32_t ovf = 0;     // fp16: non-zero once a value this lane stored is not finite
             const int store_ch = a.store_ch[tc.g];
             float* of32 = a.out_f32[tc.g];
             const int f32_ch = a.f32_ch[tc.g];
@@ -363,6 +379,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                             const uint32_t pk = pack_bf16x2(lo, hi);
                             *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pk;
                             amax = max(amax, max(pk & 0x7fffu, (pk >> 16) & 0x7fffu));
+                        } else if constexpr (kF16) {
+                            const uint32_t pk = pack_f16x2(lo, hi);
+                            *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pk;
+                            ovf |= f16x2_nonfinite(pk);
                         } else {
                             *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pack_bf16x2(lo, hi);
                         }
@@ -383,6 +403,12 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                 amax = __reduce_max_sync(0xffffffffu, amax);
                 if (lane == 0 && amax != 0) atomicMax(a.amax_out + tc.n, amax << 16);
             }
+            // fp16: only lanes that stored a non-finite value take part; ptxas aggregates them into one reduction per warp.
+            // No vote and no lane-0 branch here: either makes the whole tile loop divergent for the compiler, which then
+            // builds the wgmma descriptors in vector registers instead of on the uniform datapath (5 % slower).
+            if constexpr (kF16) {
+                if (ovf) atomicOr(a.ovf_out + tc.n, 1u);
+            }
             if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(7);
         }
     }
@@ -397,6 +423,11 @@ __global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_kernel(const __grid
 template <int N, bool kRagged>
 __global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_fp8_kernel(const __grid_constant__ ConvTcArgs a) {
     conv_tc_body<N, true, kRagged, true>(a);
+}
+
+template <int N, bool kRagged>
+__global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_f16_kernel(const __grid_constant__ ConvTcArgs a) {
+    conv_tc_body<N, false, kRagged, false, true>(a);
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -427,13 +458,15 @@ cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cst
     if (a.groups < 1 || a.groups > 2 || in_cstride % 8 != 0) return cudaErrorInvalidValue;
     if (a.split && in_lo == nullptr) return cudaErrorInvalidValue;
     if (a.fp8 && (a.split || !a.chunk || a.n_tile > 64)) return cudaErrorInvalidValue;
+    if (a.f16 && (a.split || a.chunk || a.fp8)) return cudaErrorInvalidValue;
+    const CUtensorMapDataType t16 = a.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     for (int plane = 0; plane <= (a.split ? 1 : 0); ++plane) {
         cuuint64_t dims[4] = {(cuuint64_t)in_cstride, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.n_img};
         cuuint64_t strides[3] = {(cuuint64_t)in_cstride * 2, (cuuint64_t)a.W * in_cstride * 2,
                                  (cuuint64_t)a.H * a.W * in_cstride * 2};
         cuuint32_t box[4] = {64, (cuuint32_t)kPatchPitch, (cuuint32_t)(kTileH + a.ksize - 1), 1};
         cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(plane ? &a.tm_in_lo : &a.tm_in, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
+        CUresult r = enc(plane ? &a.tm_in_lo : &a.tm_in, t16, 4,
                          const_cast<__nv_bfloat16*>(plane ? in_lo : in), dims, strides,
                          box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -455,11 +488,11 @@ cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cst
         if (tps < 1 || (a.chunk && !a.fp8 && a.ksize == 7)) tps = 1;
         if (tps > taps) tps = taps;
         a.tps = tps;
-        cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)rows, (cuuint64_t)(a.fp8 ? taps : 2 * taps)};
+        cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)rows, (cuuint64_t)(a.fp8 || a.f16 ? taps : 2 * taps)};
         cuuint64_t strides[2] = {(cuuint64_t)cin_pad * esz, (cuuint64_t)rows * cin_pad * esz};
         cuuint32_t box[3] = {64, (cuuint32_t)a.n_tile, (cuuint32_t)tps};
         cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&a.tm_w, a.fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3,
+        CUresult r = enc(&a.tm_w, a.fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : t16, 3,
                          const_cast<void*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          a.fp8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -475,11 +508,12 @@ namespace {
 // Programmatic dependent launch (a.pdl): the next layer's CTAs may start - barrier init, descriptor prefetch, weight loads -
 // while this layer's last CTAs drain; they wait (griddepcontrol.wait) before touching activations.  Used by the SMALL-batch
 // plans only, where the fixed cost per launch is most of a layer.
-template <int N, bool kChunk, bool kRagged, bool kFp8 = false>
+template <int N, bool kChunk, bool kRagged, bool kFp8 = false, bool kF16 = false>
 cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
     static DynSmemOptIn optin;   // per device: a second net on another GPU of the same process needs its own opt-in
     void (*kernel)(ConvTcArgs);
     if constexpr (kFp8) kernel = conv_tc_fp8_kernel<N, kRagged>;
+    else if constexpr (kF16) kernel = conv_tc_f16_kernel<N, kRagged>;
     else kernel = conv_tc_kernel<N, kChunk, kRagged>;
     cudaError_t e = optin.ensure(kernel, kConvTcSmemBytes);
     if (e != cudaSuccess) return e;
@@ -500,9 +534,10 @@ cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
     return cudaGetLastError();
 }
 
-template <int N, bool kChunk, bool kFp8 = false>
+template <int N, bool kChunk, bool kFp8 = false, bool kF16 = false>
 cudaError_t launch(int grid, cudaStream_t stream, const ConvTcArgs& a) {
-    return a.ext != nullptr ? launch_k<N, kChunk, true, kFp8>(grid, stream, a) : launch_k<N, kChunk, false, kFp8>(grid, stream, a);
+    return a.ext != nullptr ? launch_k<N, kChunk, true, kFp8, kF16>(grid, stream, a)
+                            : launch_k<N, kChunk, false, kFp8, kF16>(grid, stream, a);
 }
 }  // namespace
 
@@ -520,6 +555,16 @@ cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream
             case 64: return launch<64, true, true>(grid, stream, a);
             case 48: return launch<48, true, true>(grid, stream, a);
             case 32: return launch<32, true, true>(grid, stream, a);
+            default: return cudaErrorInvalidValue;
+        }
+    }
+    if (a.f16) {
+        if (a.chunk || a.split || a.ovf_out == nullptr) return cudaErrorInvalidValue;
+        switch (a.n_tile) {
+            case 128: return launch<128, false, false, true>(grid, stream, a);
+            case 64: return launch<64, false, false, true>(grid, stream, a);
+            case 48: return launch<48, false, false, true>(grid, stream, a);
+            case 32: return launch<32, false, false, true>(grid, stream, a);
             default: return cudaErrorInvalidValue;
         }
     }

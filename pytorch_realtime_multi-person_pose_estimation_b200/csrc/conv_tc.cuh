@@ -72,12 +72,16 @@ struct ConvTcArgs {
     unsigned* amax_out;           // this launch's per-image max |stored bf16|, atomic max
     const int* w_exp;             // [groups * n_tiles * n_tile]: weight row r holds e4m3(w * 2^w_exp[r])
     int* ea_out;                  // the activation exponent each image used (may be null)
+    // ---- fp16 mode (DESIGN.md §2.3): binary16 activations (`in`, `out`) and weights, full-K fp32 accumulation
+    int f16;
+    unsigned* ovf_out;            // per image: set to 1 when a value the launch stores is +-inf or NaN in binary16
 };
 
 // Builds the tensor maps. `in` (and `in_lo` in split mode): NHWC buffers with `in_cstride` channels per pixel.
 // `w`: packed weights [2*taps][groups*n_tiles*n_tile][cin_blocks*64]: bf16(w) for the first `taps` slices, the
 // residual bf16(w - hi) for the second.  fp8 mode (a.fp8): [taps][rows][cin_blocks*64] e4m3 bytes, each 32-channel
-// slice in the K order of fp8_k_to_channel (fp8_core.h).
+// slice in the K order of fp8_k_to_channel (fp8_core.h).  fp16 mode (a.f16): `in` holds binary16 bits and `w` is
+// [taps][rows][cin_blocks*64] binary16 (no residual slices).
 cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cstride, const void* w,
                               const __nv_bfloat16* in_lo = nullptr);
 cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream);

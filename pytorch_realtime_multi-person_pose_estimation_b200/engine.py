@@ -39,6 +39,14 @@ def _at(v, i):
     return v[i] if isinstance(v, (list, tuple)) else v
 
 
+def check_overflow_flags(flags):
+    """fp16 mode: binary16 tops out at 65504; an image whose activations went beyond it has inf / NaN maps."""
+    bad = [int(i) for i in np.nonzero(np.asarray(flags))[0]]
+    if bad:
+        raise nat.B200PoseError("fp16 overflow: activations of image(s) %s exceeded the binary16 range (65504); their maps "
+                                "are not valid - run them in bf16, bf16x3 or fp32 mode" % bad)
+
+
 class NativeNet:
     """Owns a b200pose_net handle on one CUDA device."""
 
@@ -84,6 +92,18 @@ class NativeNet:
         nat.check(nat.lib().b200pose_net_forward_ragged_u8(self._h, ctypes.c_void_p(in_ptr), int(in_on_device), len(shapes),
                                                            hw, mode, arr, int(out_on_device), ctypes.c_void_p(stream)),
                   "b200pose_net_forward_ragged_u8")
+
+    def overflow(self, n, stream=0):
+        """Per image of the last forward (n = its batch): True if the fp16 mode overflowed binary16 for it.  Waits for
+        `stream`.  Always False for the other modes."""
+        flags = np.zeros(n, np.int32)
+        if nat.lib().b200pose_net_overflow(self._h, flags.ctypes.data, int(n), ctypes.c_void_p(stream)) < 0:
+            nat.check(1, "b200pose_net_overflow")
+        return flags.astype(bool)
+
+    def check_overflow(self, n, stream=0):
+        """Raises B200PoseError naming the images of the last forward whose fp16 values overflowed."""
+        check_overflow_flags(self.overflow(n, stream))
 
     def crop_with_factor(self, images, dest_size=368, factor=8):
         """Device-side crop_with_factor (im_transform.py:119-134) of uint8 BGR frames of one size: [n,h,w,3] or [h,w,3]
@@ -174,6 +194,13 @@ class NativePost:
                 raise nat.B200PoseError("post-processing capacity exceeded on image %d (status bits %d: 1=peaks>%d per "
                                         "part, 2=candidate pool, 4=rows, 8=humans>%d); raise the caps"
                                         % (i, st & 0xF, self.peak_cap, self.human_cap))
+
+    def overflow(self, img):
+        """True if the network overflowed binary16 for frame img of the selected fused fp16 run."""
+        v = int(nat.lib().b200pose_post_overflow(self._h, img))
+        if v < 0:
+            nat.check(1, "b200pose_post_overflow")
+        return v == 1
 
     def humans(self, img):
         """float32 [k, 73]: score, 18 x (x, y, peak score, peak id | -1)."""
@@ -409,9 +436,14 @@ class PoseEngine:
             self.post.sync()
         else:
             self.post.select(ticket)
+        self._check_overflow(n)
         if check:
             self.post.check_status(n)
         return [humans_to_dicts(self.post.humans(i), _at(W, i), _at(H, i)) for i in range(n)]
+
+    def _check_overflow(self, n):
+        if self.mode == nat.MODE_FP16:      # whatever `check` says: overflowed maps are never handed back in silence
+            check_overflow_flags([self.post.overflow(i) for i in range(n)])
 
     def fetch_arrays(self, check=True, ticket=None):
         """Like fetch() but without building Python objects: per image a float32 array [k, 73] with rows
@@ -421,6 +453,7 @@ class PoseEngine:
             self.post.sync()
         else:
             self.post.select(ticket)
+        self._check_overflow(n)
         if check:
             self.post.check_status(n)
         return [self.post.humans(i) for i in range(n)]

@@ -10,8 +10,13 @@ the input's device pointer to libb200pose.so, which runs the hand-written sm_90a
 Precision: `model.precision = 'bf16x3'` (default: split-precision operands on the wgmma tensor cores with K-chunked
 fp32 accumulation - maps within 1.4e-4 of the reference's fp32 network at 368x368, inside its 1e-3 tolerance), `'bf16'`
 (the fast mode of the batched engine and the benchmark: ~4.5x faster, maps within ~8e-2), `'fp8'` (e4m3 operands with
-per-image activation and per-channel weight scales; DESIGN.md 2.3) or `'fp32'` (CUDA cores, bit-identical to the
-oracle's fp32 network); the environment variable B200POSE_MODE sets the default.
+per-image activation and per-channel weight scales; DESIGN.md 2.3), `'fp16'` (IEEE binary16 operands on the bf16 plan:
+about 8x finer rounding than bf16; kernels at bf16's speed, frames/s 2 - 4 % lower in DESIGN.md 6; an image whose input or activations
+leave binary16's range raises B200PoseError) or `'fp32'` (CUDA cores, bit-identical to the oracle's fp32 network); the
+environment variable B200POSE_MODE sets the default.
+
+In fp16 mode `forward` and `get_outputs` check for overflow before they return: that waits for the forward on the current
+stream (one stream synchronisation per call, which `get_outputs` pays anyway when it copies the maps to the host).
 """
 import os
 import threading
@@ -149,6 +154,8 @@ class rtpose_model(nn.Module):
             heat = torch.empty((1, 19, ph // 8, pw // 8), dtype=torch.float32, device=device)
             net.forward_u8_ptr(frame.data_ptr(), True, 1, ph, pw, nat.MODES[self.precision],
                                [0] * 10 + [paf.data_ptr(), heat.data_ptr()], True, stream)
+            if nat.MODES[self.precision] == nat.MODE_FP16:
+                net.check_overflow(1, stream)
         return paf, heat, scale
 
     def pose_engine(self, batch_cap=32, peak_cap=2048, human_cap=2048):
@@ -186,6 +193,8 @@ class rtpose_model(nn.Module):
             stream = torch.cuda.current_stream().cuda_stream
             net.forward_ptr(x.data_ptr(), True, n, H, W, nat.MODES[self.precision], [t.data_ptr() for t in saved], True,
                             stream)
+            if nat.MODES[self.precision] == nat.MODE_FP16:
+                net.check_overflow(n, stream)
         return (saved[-2], saved[-1]), saved
 
 

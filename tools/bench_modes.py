@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bf16 against fp8 on the network forward of bench.py's workload (seeded weights, batch 32 of seeded 368 x 368 uint8
-frames), alternating the two modes in one process: frames/s per run of each mode, then per-launch milliseconds and
-TFLOP/s of both plans from b200pose_net_profile (algorithmic FLOPs), with the card's name and power limit read in the
-same call.  Prints a table and ONE JSON line.
+"""Two arithmetic modes (default bf16 against fp8) on the network forward of bench.py's workload (seeded weights, batch 32
+of seeded 368 x 368 uint8 frames), alternating the modes in one process: frames/s per run of each mode, then per-launch
+milliseconds and TFLOP/s of both plans from b200pose_net_profile (algorithmic FLOPs), with the card's name and power
+limit read in the same call.  Prints a table and ONE JSON line.
 
-  python tools/bench_modes.py [--runs R] [--steps K] [--warmup W] [--batch N]
+  python tools/bench_modes.py [--modes bf16 fp16] [--runs R] [--steps K] [--warmup W] [--batch N]
 """
 import argparse
 import importlib
@@ -20,7 +20,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import _b200_alias  # noqa: E402
 
-MODES = ("bf16", "fp8")
 
 
 def card():
@@ -35,7 +34,11 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--modes", nargs=2, default=["bf16", "fp8"], metavar=("BASE", "OTHER"),
+                    help="the two modes to alternate; times are reported as OTHER / BASE")
     args = ap.parse_args()
+    MODES = tuple(args.modes)
+    base, other = MODES
     import torch
     _b200_alias.load_package()
     engine = importlib.import_module(_b200_alias.PKG + ".engine")
@@ -80,16 +83,16 @@ def main():
     print("%s; batch %d x %dx%d; %d runs x %d steps per mode, alternating" % (name, n, H, W, args.runs, args.steps))
     for m in MODES:
         print("  %-5s frames/s: %s" % (m, " ".join("%.1f" % v for v in fps[m])))
-    print("launch  GFLOP    bf16 ms  TFLOP/s   fp8 ms  TFLOP/s  fp8/bf16 time")
-    for i in range(len(prof["bf16"][0])):
-        (mb, fb), (m8, _) = (prof["bf16"][0][i], prof["bf16"][1][i]), (prof["fp8"][0][i], None)
-        print("%6d  %6.1f  %8.3f  %7.1f  %7.3f  %7.1f  %6.2f" % (i, fb / 1e9, mb, fb / mb / 1e9, m8, fb / m8 / 1e9, m8 / mb))
+    print("launch  GFLOP  %6s ms  TFLOP/s  %6s ms  TFLOP/s  %s/%s time" % (base, other, other, base))
+    for i in range(len(prof[base][0])):
+        (mb, fb), m8 = (prof[base][0][i], prof[base][1][i]), prof[other][0][i]
+        print("%6d  %6.1f  %9.3f  %7.1f  %9.3f  %7.1f  %6.3f" % (i, fb / 1e9, mb, fb / mb / 1e9, m8, fb / m8 / 1e9, m8 / mb))
     tot = {m: (float(prof[m][0].sum()), float(prof[m][1].sum())) for m in MODES}
     for m in MODES:
         print("  %-5s all launches: %.3f ms, %.1f TFLOP/s" % (m, tot[m][0], tot[m][1] / tot[m][0] / 1e9))
     print(json.dumps({"card": name, "batch": n, "fps": fps,
                       "profile_ms": {m: [round(float(v), 4) for v in prof[m][0]] for m in MODES},
-                      "gflop": [round(float(v) / 1e9, 3) for v in prof["bf16"][1]]}))
+                      "gflop": [round(float(v) / 1e9, 3) for v in prof[base][1]]}))
 
 
 if __name__ == "__main__":
