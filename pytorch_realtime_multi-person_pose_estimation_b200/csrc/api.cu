@@ -132,17 +132,22 @@ template <class T> struct DevBuf {
 struct TcLayer {            // one grouped tensor-core launch
     int ks, cin_blocks, groups, n_tile, n_tiles, relu, pool;
     double macs_per_pixel = 0;    // algorithmic (unpadded) MACs per output pixel, all groups
-    __nv_bfloat16* w = nullptr;   // [taps][groups*n_tiles*n_tile][cin_blocks*64]
     float* bias = nullptr;        // [groups*n_tiles*n_tile]
     std::vector<int> convs;       // state-dict conv per group
     bool cat_input = false;       // reads the concat buffer (input channels permuted, cat_phys)
-    // fp8 mode, packed at the first fp8 plan build (pack_fp8_layer):
-    uint8_t* w8 = nullptr;        // [taps][rows][cin_blocks*64] e4m3(w * 2^ew[row]), K order fp8_k_to_channel
-    int* w_exp = nullptr;         // ew per row (device)
+    // packed weights per encoding (TcWeights, tc_format.h), rows groups*n_tiles*n_tile of cin_blocks*64 channels; see
+    // ensure_packed for when each is packed
+    void* w[kNumTcWeights] = {};
+    int* w_exp = nullptr;         // e4m3: ew per row (device)
     std::vector<int> h_w_exp;     // ... and its host copy (b200pose_net_debug_fp8)
-    // fp16 mode, packed at the first fp16 plan build (pack_f16_layer):
-    uint16_t* w16 = nullptr;      // [taps][rows][cin_blocks*64] binary16(w)
 };
+
+void free_tc_layer(TcLayer& L) {
+    for (void* w : L.w)
+        if (w) cudaFree(w);
+    if (L.bias) cudaFree(L.bias);
+    if (L.w_exp) cudaFree(L.w_exp);
+}
 
 // Activation buffers (the buffer ids of the test hooks): channels per pixel and spatial divisor.
 enum Act { T1, T2, T3, T4, T5A, T5B, T6, T7, T8, T9, CAT, BRA, BRB, BR512, kNumAct };
@@ -150,7 +155,7 @@ constexpr int kMaxRagged = 1024;      // images of one ragged forward (flip: 2 p
 const int kActC[kNumAct] = {64, 64, 128, 128, 256, 256, 256, 512, 512, 256, 192, 256, 256, 1024};
 const int kActDiv[kNumAct] = {1, 2, 2, 4, 4, 4, 8, 8, 8, 8, 8, 8, 8, 8};
 
-// One tensor-core launch of a bf16 plan: the buffers it reads and writes and its channel slices of them.  A launch
+// One launch of a tensor-core plan: the buffers it reads and writes and its channel slices of them.  A launch
 // runs at the resolution of its input buffer.
 struct Wiring {
     int in, in_base, in_group_stride;   // input buffer, first channel of group 0, channel offset of group 1
@@ -199,21 +204,21 @@ struct PlanLaunch {
 };
 
 // Device addresses a plan's tensor maps and arguments point into: activation buffers, residual planes, stage maps.
-using PlanBuffers = std::array<const void*, 2 * kNumAct + 12 + 3>;    // + the fp8 amax and exponent tables, fp16 flags
+using PlanBuffers = std::array<const void*, 2 * kNumAct + 12 + 2>;    // + the format's aux table, the fp8 exponent table
 
-// The launch list of one (n, H, W, mode) key, valid while `buffers` are still the net's.
+// The launch list of one (n, H, W, format) key, valid while `buffers` are still the net's.
 struct Plan {
-    int n, H, W, mode;
-    bool split;            // bf16x3
-    bool fp8;
-    bool f16;              // fp16: binary16 activation planes and weights
+    int n, H, W;
+    TcFormat fmt;
     std::vector<PlanLaunch> launches;
     PlanBuffers buffers;
 };
 
 // What the last successful forward ran; b200pose_net_last_maps, _profile and the _debug_* hooks read it.
 struct LastForward {
-    int n = 0, H = 0, W = 0, mode = -1;
+    int n = 0, H = 0, W = 0;
+    bool fp32 = false;           // the fp32 path ran, else the tensor-core path in format fmt
+    TcFormat fmt = TcFormat::kBf16;
     const void* in = nullptr;    // device input
     int in_u8 = 0;               // normalisation of a uint8 input fused into conv1_1 (0: fp32 input)
     const int* ext = nullptr;    // extents table of a ragged forward, null: uniform
@@ -231,17 +236,17 @@ struct b200pose_net {
     // tensor-core layers: trunk 1..11 -> tc[0..10]; stage 1: tc[11..15]; stage t>=2: tc[16 + (t-2)*7 + li]
     std::vector<TcLayer> tc;
     // Plans of the last 32 keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not re-encode
-    // 51 tensor maps and synchronise the stream.  `plan` is the one the last bf16 / bf16x3 forward selected.
+    // 51 tensor maps and synchronise the stream.  `plan` is the one the last tensor-core forward selected.
     std::list<Plan> plans;
     const Plan* plan = nullptr;
-    // The 52 launches of a forward pass are captured at the second use of a (shape, mode, input pointer) into a CUDA graph and replayed
+    // The 52 launches of a forward pass are captured at the second use of a (shape, format, input pointer) into a CUDA graph and replayed
     // (B200POSE_GRAPH=0: plain launches).  Graphs embed the tensor maps, i.e. buffer addresses: every plan build drops them.
     // Capture needs a real stream: calls on the legacy default stream (0) launch directly.
-    using GraphKey = std::tuple<int, int, int, int, int, bool, const void*>;   // n, H, W, mode, in_u8, ragged, input
+    using GraphKey = std::tuple<int, int, int, TcFormat, int, bool, const void*>;   // n, H, W, format, in_u8, ragged, input
     bool use_graph = true;
     std::map<GraphKey, cudaGraphExec_t> graphs;
     std::set<GraphKey> graph_seen;    // a key is captured at its SECOND use: callers that pass a fresh pointer every time never pay a capture
-    // bf16 activation buffers by Act id, and their residual ("lo") planes (split-precision mode only)
+    // bf16 (fp16: binary16) activation buffers by Act id, and their residual ("lo") planes (bf16x3 only)
     DevBuf<__nv_bfloat16> act[kNumAct], act_lo[kNumAct];
     DevBuf<float> in_stage, out_f32[12];
     // fp32 parity buffers
@@ -325,22 +330,26 @@ template <class F> void for_each_weight_row(const b200pose_net* net, const TcLay
     }
 }
 
-int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_ids /*per group*/, int n_tile,
-                  bool cat_input, int ks, int relu, int pool) {
-    const int groups = (int)conv_ids.size();
+// The layer of the convs conv_ids (one per group), before any weights are packed.
+TcLayer make_tc_layer(const std::vector<int>& conv_ids, int n_tile, bool cat_input, int ks, int relu, int pool) {
     const ConvSpec sp = conv_spec(conv_ids[0]);
     const int cin_pad = cat_input ? 192 : sp.cin;
     const int cout_pad = ((sp.cout + n_tile - 1) / n_tile) * n_tile;
-    L.ks = ks; L.cin_blocks = cin_pad / 64; L.groups = groups; L.n_tile = n_tile; L.n_tiles = cout_pad / n_tile;
+    TcLayer L;
+    L.ks = ks; L.cin_blocks = cin_pad / 64; L.groups = (int)conv_ids.size(); L.n_tile = n_tile; L.n_tiles = cout_pad / n_tile;
     L.relu = relu; L.pool = pool; L.convs = conv_ids; L.cat_input = cat_input;
-    const int taps = ks * ks, rows = groups * cout_pad;
-    L.macs_per_pixel = 0;
-    for (int g = 0; g < groups; ++g) L.macs_per_pixel += (double)conv_spec(conv_ids[g]).cin * conv_spec(conv_ids[g]).cout * taps;
-    // [hi taps | lo taps]: bf16(w) and the residual bf16(w - hi) (used by the split-precision mode only)
+    for (int c : conv_ids) L.macs_per_pixel += (double)conv_spec(c).cin * conv_spec(c).cout * ks * ks;
+    return L;
+}
+
+// bf16 weights of layer L and its bias (every format's): [hi taps | lo taps], bf16(w) and the residual bf16(w - hi) (read
+// by bf16x3 only)
+int pack_tc_layer(b200pose_net* net, TcLayer& L) {
+    const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, rows = L.groups * L.n_tiles * L.n_tile;
     std::vector<uint16_t> w((size_t)2 * taps * rows * cin_pad, 0);
     std::vector<float> b((size_t)rows, 0.f);
     for_each_weight_row(net, L, [&](int g, int o, int r, const float* wr) {
-        b[r] = net->host_b[conv_ids[g]][o];
+        b[r] = net->host_b[L.convs[g]][o];
         for (int t = 0; t < taps; ++t)
             for (int k = 0; k < cin_pad; ++k) {
                 const float wf = wr[(size_t)t * cin_pad + k];
@@ -349,16 +358,17 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L, const std::vector<int>& conv_id
                 w[((size_t)(taps + t) * rows + r) * cin_pad + k] = f2bf(wf - bf2f(hi));
             }
     });
-    CU(cudaMalloc(&L.w, w.size() * 2));
+    void*& dw = L.w[(int)TcWeights::kBf16HiLo];
+    CU(cudaMalloc(&dw, w.size() * 2));
     CU(cudaMalloc(&L.bias, b.size() * 4));
-    CU(cudaMemcpy(L.w, w.data(), w.size() * 2, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(dw, w.data(), w.size() * 2, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(L.bias, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
     return 0;
 }
 
-// fp8 weights of layer L, packed when the first fp8 plan is built (half the bytes of L.w; nets that never run fp8 do not
-// pay for them): per output row ew = floor(log2(448 / max|w_row|)) and e4m3(w * 2^ew), one rounding from the fp32
-// weight; each 32-channel slice in the K order the kernel's A fragments have (fp8_k_to_channel).
+// fp8 weights of layer L (half the bytes of the bf16 ones): per output row ew = floor(log2(448 / max|w_row|)) and
+// e4m3(w * 2^ew), one rounding from the fp32 weight; each 32-channel slice in the K order the kernel's A fragments have
+// (fp8_k_to_channel).
 int pack_fp8_layer(const b200pose_net* net, TcLayer& L) {
     const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, rows = L.groups * L.n_tiles * L.n_tile;
     L.h_w_exp.assign(rows, 0);
@@ -376,9 +386,10 @@ int pack_fp8_layer(const b200pose_net* net, TcLayer& L) {
             for (int k = 0; k < cin_pad; ++k) dst[k] = e4m3_rn_bits(src[(k & ~31) + fp8_k_to_channel(k & 31)] * exp2_int(ew));
         }
     });
-    CU(cudaMalloc(&L.w8, w8.size()));
+    void*& dw = L.w[(int)TcWeights::kE4m3];
+    CU(cudaMalloc(&dw, w8.size()));
     CU(cudaMalloc(&L.w_exp, rows * sizeof(int)));
-    CU(cudaMemcpy(L.w8, w8.data(), w8.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(dw, w8.data(), w8.size(), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(L.w_exp, L.h_w_exp.data(), rows * sizeof(int), cudaMemcpyHostToDevice));
     return 0;
 }
@@ -391,8 +402,8 @@ int check_f16_weight(float w, int conv) {
     return 0;
 }
 
-// fp16 weights of layer L, packed when the first fp16 plan is built: binary16(w), one rounding from the fp32 weight, in
-// the layout of the bf16 value slices (pad rows and channels 0).
+// fp16 weights of layer L: binary16(w), one rounding from the fp32 weight, in the layout of the bf16 value slices (pad
+// rows and channels 0).
 int pack_f16_layer(const b200pose_net* net, TcLayer& L) {
     const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, rows = L.groups * L.n_tiles * L.n_tile;
     std::vector<uint16_t> w16((size_t)taps * rows * cin_pad, 0);
@@ -406,9 +417,34 @@ int pack_f16_layer(const b200pose_net* net, TcLayer& L) {
             }
     });
     if (rc) return rc;
-    CU(cudaMalloc(&L.w16, w16.size() * 2));
-    CU(cudaMemcpy(L.w16, w16.data(), w16.size() * 2, cudaMemcpyHostToDevice));
+    void*& dw = L.w[(int)TcWeights::kBinary16];
+    CU(cudaMalloc(&dw, w16.size() * 2));
+    CU(cudaMemcpy(dw, w16.data(), w16.size() * 2, cudaMemcpyHostToDevice));
     return 0;
+}
+
+// Packs the weights of layer L that format fmt reads, unless they are packed already.  The bf16 ones (with the bias) are
+// packed at finalize, the e4m3 and binary16 ones when the first plan of their format is built: nets that never run those
+// formats do not pay for them.
+int ensure_packed(b200pose_net* net, TcLayer& L, TcFormat fmt) {
+    const TcWeights enc = tc_weights(fmt);
+    if (L.w[(int)enc] != nullptr) return 0;
+    switch (enc) {
+        case TcWeights::kBf16HiLo: return pack_tc_layer(net, L);
+        case TcWeights::kE4m3: return pack_fp8_layer(net, L);
+        case TcWeights::kBinary16: return pack_f16_layer(net, L);
+    }
+    return fail("unknown weight encoding %d", (int)enc);
+}
+
+// The per-image table of format f (tc_aux): fp8 amax rows (conv1_1, then each launch), fp16 overflow flags; null otherwise.
+unsigned* aux_table(const b200pose_net* net, TcFormat f) {
+    switch (tc_aux(f)) {
+        case TcAux::kAmax: return net->amax.p;
+        case TcAux::kOverflow: return net->ovf.p;
+        case TcAux::kNone: break;
+    }
+    return nullptr;
 }
 
 // Small-batch plans: the 46 x 46 stage layers (two groups) would fill at most half of the SMs with one n-tile per group.
@@ -424,6 +460,7 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
     const int n = p.n, H = p.H / kActDiv[wr.in], W = p.W / kActDiv[wr.in];
     ConvTcArgs a;
     memset(&a, 0, sizeof(a));
+    a.fmt = p.fmt;
     a.n_img = n; a.H = H; a.W = W; a.ksize = L.ks; a.cin_blocks = L.cin_blocks;
     a.in_ch_base = wr.in_base; a.in_ch_group_stride = wr.in_group_stride; a.groups = L.groups;
     a.n_tile = L.n_tile; a.n_tiles = L.n_tiles; a.bias = L.bias; a.relu = L.relu; a.pool = L.pool;
@@ -433,12 +470,9 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         if (L.n_tile == 128 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 64; a.n_tiles = L.n_tiles * 2; }
         if (a.n_tile == 64 && 2 * pix * L.groups * a.n_tiles <= net->num_sms) { a.n_tile = 32; a.n_tiles *= 2; }
     }
-    if (p.split || p.fp8) {     // bf16x3, fp8: K-chunked accumulation in a second register set, so N <= 64
-        a.chunk = 1;
-        if (a.n_tile > 64) { a.n_tile = 64; a.n_tiles = L.n_tiles * (L.n_tile / 64); }
-    }
-    if (p.fp8) {
-        a.fp8 = 1;
+    const int max_n = tc_max_n_tile(p.fmt);
+    if (a.n_tile > max_n) { a.n_tile = max_n; a.n_tiles = L.n_tiles * (L.n_tile / max_n); }
+    if (tc_aux(p.fmt) == TcAux::kAmax) {
         const int slot = 1 + (int)p.launches.size();      // amax table row of this launch (0 = conv1_1)
         a.amax_out = net->amax.p + (size_t)slot * n;
         a.amax_in[0] = net->amax.p + (size_t)writers[0] * n;
@@ -446,10 +480,7 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         a.w_exp = L.w_exp;
         a.ea_out = net->ea.p + (size_t)slot * n;
     }
-    if (p.f16) {
-        a.f16 = 1;
-        a.ovf_out = net->ovf.p;
-    }
+    if (tc_aux(p.fmt) == TcAux::kOverflow) a.ovf_out = net->ovf.p;
     a.out = net->act[wr.out].p; a.out_cstride = kActC[wr.out];
     a.out_ch_off[0] = wr.out_off[0]; a.out_ch_off[1] = wr.out_off[1];
     a.store_ch[0] = wr.store[0]; a.store_ch[1] = wr.store[1];
@@ -465,37 +496,34 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
     while ((a.H << a.ext_shift) < p.H) ++a.ext_shift;      // ragged batches: the launch's output resolution relative to the input
     a.ext_shift += a.pool;
     const __nv_bfloat16* in_lo = nullptr;
-    if (p.split) {
-        a.split = 1;
+    if (tc_planes(p.fmt) == 2) {
         in_lo = net->act_lo[wr.in].p;
         a.out_lo = net->act_lo[wr.out].p;
     }
-    const void* w = p.fp8 ? (const void*)L.w8 : (p.f16 ? (const void*)L.w16 : L.w);
-    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], w, in_lo);
+    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], L.w[(int)tc_weights(p.fmt)], in_lo);
     if (e != cudaSuccess) return fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
     p.launches.push_back({a, 2.0 * n * H * W * L.macs_per_pixel, wr.in, wr.out, {f32[0], f32[1]}});
     return 0;
 }
 
-// fp8: the plan also points into the amax and exponent tables, fp16 into the overflow flags (only plans of that mode
+// fp8 plans also point into the amax and exponent tables, fp16 plans into the overflow flags (only plans of that format
 // do, so only they depend on them)
-PlanBuffers plan_buffers(const b200pose_net* net, bool fp8, bool f16) {
+PlanBuffers plan_buffers(const b200pose_net* net, TcFormat fmt) {
     PlanBuffers b;
     for (int i = 0; i < kNumAct; ++i) {
         b[i] = net->act[i].p;
         b[kNumAct + i] = net->act_lo[i].p;
     }
     for (int i = 0; i < 12; ++i) b[2 * kNumAct + i] = net->out_f32[i].p;
-    b[2 * kNumAct + 12] = fp8 ? net->amax.p : nullptr;
-    b[2 * kNumAct + 13] = fp8 ? net->ea.p : nullptr;
-    b[2 * kNumAct + 14] = f16 ? net->ovf.p : nullptr;
+    b[2 * kNumAct + 12] = aux_table(net, fmt);
+    b[2 * kNumAct + 13] = tc_aux(fmt) == TcAux::kAmax ? net->ea.p : nullptr;
     return b;
 }
 
 // Fills p.launches, (re)allocating the buffers of p's key.
-int build_plan_bf16(b200pose_net* net, Plan& p, cudaStream_t st) {
+int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
     const size_t px = (size_t)p.n * p.H * p.W;
-    for (int plane = 0; plane < (p.split ? 2 : 1); ++plane) {
+    for (int plane = 0; plane < tc_planes(p.fmt); ++plane) {
         DevBuf<__nv_bfloat16>* bufs = plane ? net->act_lo : net->act;
         for (int i = 0; i < kNumAct; ++i) CU(bufs[i].ensure(px / (kActDiv[i] * kActDiv[i]) * kActC[i]));
         // pad lanes of the concat buffer must read as zero; on the caller's stream (a non-blocking stream is not ordered
@@ -503,19 +531,16 @@ int build_plan_bf16(b200pose_net* net, Plan& p, cudaStream_t st) {
         CU(cudaMemsetAsync(bufs[CAT].p, 0, px / 64 * kActC[CAT] * 2, st));
     }
     for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * (i % 2 == 0 ? kPaf : kHeat)));
-    if (p.fp8) {
+    if (tc_aux(p.fmt) == TcAux::kAmax) {
         CU(net->amax.ensure((size_t)(1 + 51) * p.n));
         CU(net->ea.ensure((size_t)(1 + 51) * p.n));
-        for (TcLayer& L : net->tc)
-            if (L.w8 == nullptr && pack_fp8_layer(net, L)) return 1;
     }
-    if (p.f16) {
-        CU(net->ovf.ensure((size_t)p.n));
+    if (tc_aux(p.fmt) == TcAux::kOverflow) CU(net->ovf.ensure((size_t)p.n));
+    if (tc_binary16(p.fmt))
         for (float w : net->host_w[0])      // conv1_1 converts its fp32 weights in the kernel
             if (check_f16_weight(w, 0)) return 1;
-        for (TcLayer& L : net->tc)
-            if (L.w16 == nullptr && pack_f16_layer(net, L)) return 1;
-    }
+    for (TcLayer& L : net->tc)
+        if (ensure_packed(net, L, p.fmt)) return 1;
     // fp8: the launch that last wrote each buffer (amax table row); the concat buffer has two writers, conv4_4_CPM
     // (features) and the latest stage head (PAF + heatmap)
     int writer[kNumAct], cat_head = -1;
@@ -534,7 +559,7 @@ int build_plan_bf16(b200pose_net* net, Plan& p, cudaStream_t st) {
     for (int s = 1; s <= 6; ++s)
         for (int li = 0; li < stage_num_layers(s); ++li)
             if (add(net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], s - 1)) return 1;
-    p.buffers = plan_buffers(net, p.fp8, p.f16);
+    p.buffers = plan_buffers(net, p.fmt);
     return 0;
 }
 
@@ -544,24 +569,23 @@ void drop_graphs(b200pose_net* net) {
     net->graph_seen.clear();
 }
 
-// Points net->plan at the plan of (n, H, W, mode): a kept one whose buffers are still the net's, or a new one (the
+// Points net->plan at the plan of (n, H, W, fmt): a kept one whose buffers are still the net's, or a new one (the
 // oldest of 32 is dropped).  A build may move the buffers the captured graphs point into: it synchronises the stream
 // and drops the graphs first.
-int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t st) {
-    const PlanBuffers bufs = plan_buffers(net, mode == B200POSE_MODE_FP8, mode == B200POSE_MODE_FP16);
+int select_plan(b200pose_net* net, int n, int H, int W, TcFormat fmt, cudaStream_t st) {
+    const PlanBuffers bufs = plan_buffers(net, fmt);
     for (const Plan& p : net->plans)
-        if (p.n == n && p.H == H && p.W == W && p.mode == mode && p.buffers == bufs) {
+        if (p.n == n && p.H == H && p.W == W && p.fmt == fmt && p.buffers == bufs) {
             net->plan = &p;
             return 0;
         }
     CU(cudaStreamSynchronize(st));
     drop_graphs(net);
     net->plan = nullptr;
-    net->plans.remove_if([&](const Plan& p) { return p.n == n && p.H == H && p.W == W && p.mode == mode; });
+    net->plans.remove_if([&](const Plan& p) { return p.n == n && p.H == H && p.W == W && p.fmt == fmt; });
     if (net->plans.size() >= 32) net->plans.pop_front();
-    net->plans.push_back(Plan{n, H, W, mode, mode == B200POSE_MODE_BF16X3, mode == B200POSE_MODE_FP8,
-                              mode == B200POSE_MODE_FP16, {}, {}});
-    if (build_plan_bf16(net, net->plans.back(), st)) {
+    net->plans.push_back(Plan{n, H, W, fmt, {}, {}});
+    if (build_plan_tc(net, net->plans.back(), st)) {
         net->plans.pop_back();
         return 1;
     }
@@ -570,18 +594,21 @@ int select_plan(b200pose_net* net, int n, int H, int W, int mode, cudaStream_t s
 }
 
 // The first k launches of a forward with net->plan: conv1_1, then the plan's.  A ragged forward passes its extents
-// table (the plans are shared with uniform batches of the canvas size).  fp8 / fp16: zero_amax clears the amax table /
-// the overflow flags first (a memset, not a launch); re-runs of launches (debug_run, profile) leave them as they are -
-// they record the same maxima and flags again.
+// table (the plans are shared with uniform batches of the canvas size).  fp8 / fp16: zero_aux clears the format's aux
+// table - the amax rows / the overflow flags - first (a memset, not a launch); re-runs of launches (debug_run, profile)
+// leave it as it is - they record the same maxima and flags again.
 // after (b200pose_net_profile): after[i] is recorded behind launch i.
-int launch_forward_bf16(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st,
-                        bool zero_amax = false, const cudaEvent_t* after = nullptr) {
+int launch_forward_tc(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st,
+                      bool zero_aux = false, const cudaEvent_t* after = nullptr) {
     const Plan& p = *net->plan;
-    if (p.fp8 && zero_amax) CU(cudaMemsetAsync(net->amax.p, 0, (size_t)(1 + p.launches.size()) * p.n * sizeof(unsigned), st));
-    if (p.f16 && zero_amax) CU(cudaMemsetAsync(net->ovf.p, 0, (size_t)p.n * sizeof(unsigned), st));
+    unsigned* aux = aux_table(net, p.fmt);
+    if (aux != nullptr && zero_aux) {
+        const size_t rows = tc_aux(p.fmt) == TcAux::kAmax ? 1 + p.launches.size() : 1;
+        CU(cudaMemsetAsync(aux, 0, rows * p.n * sizeof(unsigned), st));
+    }
     if (k >= 1) {
-        CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], net->act[T1].p, p.split ? net->act_lo[T1].p : nullptr,
-                             p.n, p.H, p.W, ext, st, p.fp8 ? net->amax.p : nullptr, p.f16 ? net->ovf.p : nullptr));
+        CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], p.fmt, net->act[T1].p,
+                             tc_planes(p.fmt) == 2 ? net->act_lo[T1].p : nullptr, aux, p.n, p.H, p.W, ext, st));
         if (after) CU(cudaEventRecord(after[0], st));
     }
     for (int i = 0; i + 1 < k; ++i) {
@@ -593,15 +620,15 @@ int launch_forward_bf16(const b200pose_net* net, const void* d_in, int in_u8, co
     return 0;
 }
 
-int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, int mode, cudaStream_t st,
-                 const int* ext) {
-    if (select_plan(net, n, H, W, mode, st)) return 1;
+int forward_tc(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, TcFormat fmt, cudaStream_t st,
+               const int* ext) {
+    if (select_plan(net, n, H, W, fmt, st)) return 1;
     const int launches = 1 + (int)net->plan->launches.size();
     cudaGraphExec_t exec = nullptr;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     if (net->use_graph && small_plan(net, n, H, W) && st != nullptr && cudaStreamIsCapturing(st, &cap) == cudaSuccess &&
         cap == cudaStreamCaptureStatusNone) {
-        const b200pose_net::GraphKey key{n, H, W, mode, in_u8, ext != nullptr, d_in};
+        const b200pose_net::GraphKey key{n, H, W, fmt, in_u8, ext != nullptr, d_in};
         auto it = net->graphs.find(key);
         if (it != net->graphs.end()) {
             exec = it->second;
@@ -611,7 +638,7 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
             if (net->graphs.size() >= 64) drop_graphs(net);
             cudaGraph_t graph = nullptr;
             CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-            const int rc = launch_forward_bf16(net, d_in, in_u8, ext, launches, st, true);
+            const int rc = launch_forward_tc(net, d_in, in_u8, ext, launches, st, true);
             cudaError_t e = cudaStreamEndCapture(st, &graph);
             if (rc == 0 && e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
             if (graph) cudaGraphDestroy(graph);
@@ -627,7 +654,7 @@ int forward_bf16(b200pose_net* net, const void* d_in, int in_u8, int n, int H, i
         }
     }
     if (exec) CU(cudaGraphLaunch(exec, st));
-    else if (launch_forward_bf16(net, d_in, in_u8, ext, launches, st, true)) return 1;
+    else if (launch_forward_tc(net, d_in, in_u8, ext, launches, st, true)) return 1;
     g_launches += launches;
     return 0;
 }
@@ -741,13 +768,7 @@ void b200pose_net_destroy(b200pose_net* net) {
     cudaSetDevice(net->device);
     drop_graphs(net);
     for (int i = 0; i < kNumConvs; ++i) { if (net->d_w[i]) cudaFree(net->d_w[i]); if (net->d_b[i]) cudaFree(net->d_b[i]); }
-    for (TcLayer& L : net->tc) {
-        if (L.w) cudaFree(L.w);
-        if (L.bias) cudaFree(L.bias);
-        if (L.w8) cudaFree(L.w8);
-        if (L.w_exp) cudaFree(L.w_exp);
-        if (L.w16) cudaFree(L.w16);
-    }
+    for (TcLayer& L : net->tc) free_tc_layer(L);
     for (int i = 0; i < kNumAct; ++i) { net->act[i].release(); net->act_lo[i].release(); }
     net->amax.release();
     net->ea.release();
@@ -790,31 +811,21 @@ int b200pose_net_finalize(b200pose_net* net) {
         CU(cudaMemcpy(net->d_w[i], net->host_w[i].data(), net->host_w[i].size() * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(net->d_b[i], net->host_b[i].data(), net->host_b[i].size() * 4, cudaMemcpyHostToDevice));
     }
-    for (TcLayer& L : net->tc) {
-        if (L.w) cudaFree(L.w);
-        if (L.bias) cudaFree(L.bias);
-        if (L.w8) cudaFree(L.w8);
-        if (L.w_exp) cudaFree(L.w_exp);
-        if (L.w16) cudaFree(L.w16);
-    }
-    net->tc.assign(16 + 5 * 7, TcLayer());
+    for (TcLayer& L : net->tc) free_tc_layer(L);
+    net->tc.clear();
     for (int i = 1; i < 12; ++i) {
         const ConvSpec s = kTrunk[i];
-        if (pack_tc_layer(net, net->tc[i - 1], {i}, s.cout < 128 ? s.cout : 128, false, 3, 1, kPoolAfter[i])) return 1;
+        net->tc.push_back(make_tc_layer({i}, s.cout < 128 ? s.cout : 128, false, 3, 1, kPoolAfter[i]));
     }
-    for (int li = 0; li < 5; ++li) {
-        const ConvSpec s = stage_layer(1, 0, li);
-        if (pack_tc_layer(net, net->tc[11 + li], {conv_index(1, 0, li), conv_index(1, 1, li)}, li == 4 ? 48 : 128, false,
-                          s.ks, li != 4, 0))
-            return 1;
-    }
+    for (int li = 0; li < 5; ++li)
+        net->tc.push_back(make_tc_layer({conv_index(1, 0, li), conv_index(1, 1, li)}, li == 4 ? 48 : 128, false,
+                                        stage_layer(1, 0, li).ks, li != 4, 0));
     for (int st = 2; st <= 6; ++st)
-        for (int li = 0; li < 7; ++li) {
-            const ConvSpec s = stage_layer(st, 0, li);
-            if (pack_tc_layer(net, net->tc[16 + (st - 2) * 7 + li], {conv_index(st, 0, li), conv_index(st, 1, li)},
-                              li == 6 ? 48 : 128, li == 0, s.ks, li != 6, 0))
-                return 1;
-        }
+        for (int li = 0; li < 7; ++li)
+            net->tc.push_back(make_tc_layer({conv_index(st, 0, li), conv_index(st, 1, li)}, li == 6 ? 48 : 128, li == 0,
+                                            stage_layer(st, 0, li).ks, li != 6, 0));
+    for (TcLayer& L : net->tc)
+        if (ensure_packed(net, L, TcFormat::kBf16)) return 1;
     net->last = LastForward();
     drop_graphs(net);
     net->plan = nullptr;
@@ -843,7 +854,8 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
             d_in = net->in_stage.p;
         }
     }
-    int rc, first_u8 = 0;     // the uint8 normalisation conv1_1 fuses (bf16 modes)
+    int rc, first_u8 = 0;     // the uint8 normalisation conv1_1 fuses (tensor-core formats)
+    TcFormat fmt = TcFormat::kBf16;
     if (mode == B200POSE_MODE_FP32) {
         if (in_u8) {   // parity mode: materialise rtpose_preprocess, then the fp32 path
             CU(net->f_u8.ensure(elems));
@@ -852,13 +864,14 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
             rc = forward_fp32(net, net->f_u8.p, n, H, W, st, ext);
         } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, st, ext);
     } else {
-        if (mode != B200POSE_MODE_BF16X3 && mode != B200POSE_MODE_FP8 && mode != B200POSE_MODE_FP16)
-            mode = B200POSE_MODE_BF16;     // every other mode runs bf16
+        if (mode == B200POSE_MODE_BF16X3) fmt = TcFormat::kBf16x3;
+        else if (mode == B200POSE_MODE_FP8) fmt = TcFormat::kFp8;
+        else if (mode == B200POSE_MODE_FP16) fmt = TcFormat::kFp16;     // every other mode runs bf16
         first_u8 = in_u8 ? net->preprocess : 0;
-        rc = forward_bf16(net, d_in, first_u8, n, H, W, mode, st, ext);
+        rc = forward_tc(net, d_in, first_u8, n, H, W, fmt, st, ext);
     }
     if (rc) return rc;
-    net->last = LastForward{n, H, W, mode, d_in, first_u8, ext};
+    net->last = LastForward{n, H, W, mode == B200POSE_MODE_FP32, fmt, d_in, first_u8, ext};
     if (outputs) {
         const size_t px8 = (size_t)n * (H / 8) * (W / 8);
         for (int i = 0; i < 12; ++i)
@@ -985,11 +998,11 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess) {
     return 0;
 }
 
-// The last forward ran net->plan: a bf16 / bf16x3 forward has run since the last finalize.
+// The last forward ran net->plan: a tensor-core forward has run since the last finalize.
 static bool last_ran_plan(const b200pose_net* net) {
     const LastForward& l = net->last;
     const Plan* p = net->plan;
-    return p && p->n == l.n && p->H == l.H && p->W == l.W && p->mode == l.mode;
+    return p && !l.fp32 && p->n == l.n && p->H == l.H && p->W == l.W && p->fmt == l.fmt;
 }
 
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream) {
@@ -1007,7 +1020,7 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
     DevBuf<float> tmp;
     if (!d_in) { if (tmp.ensure((size_t)n * 3 * H * W) != cudaSuccess) return -1; cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st); d_in = tmp.p; in_u8 = 0; }
     cudaEventRecord(ev[0], st);
-    int rc = launch_forward_bf16(net, d_in, in_u8, nullptr, total, st, false, ev.data() + 1);
+    int rc = launch_forward_tc(net, d_in, in_u8, nullptr, total, st, false, ev.data() + 1);
     g_launches += total;
     if (rc == 0 && cudaStreamSynchronize(st) != cudaSuccess)
         rc = fail("profile run failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -1022,19 +1035,19 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
 }
 
 int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream) {
-    if (!net || !last_ran_plan(net) || !net->last.in) return fail("debug_run: no bf16 / bf16x3 forward has run");
+    if (!net || !last_ran_plan(net) || !net->last.in) return fail("debug_run: no tensor-core forward has run");
     if (launches < 0 || launches > 1 + (int)net->plan->launches.size())
         return fail("debug_run: %d launches out of range", launches);
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (launch_forward_bf16(net, net->last.in, net->last.in_u8, net->last.ext, launches, st)) return 1;
+    if (launch_forward_tc(net, net->last.in, net->last.in_u8, net->last.ext, launches, st)) return 1;
     g_launches += launches;
     CU(cudaStreamSynchronize(st));
     return 0;
 }
 
 int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
-    if (!net || !last_ran_plan(net)) return fail("debug_launch: no bf16 / bf16x3 forward has run");
+    if (!net || !last_ran_plan(net)) return fail("debug_launch: no tensor-core forward has run");
     const Plan& p = *net->plan;
     // fields 0 .. 26 are required; the format field is written when there is room for it
     constexpr int kAll = B200POSE_DEBUG_LAUNCH_FORMAT + 1;
@@ -1045,7 +1058,7 @@ int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
     if (i == 0) {     // conv1_1 (CUDA cores / mma.sync): the network input -> t1
         f[0] = -1; f[1] = 3; f[4] = T1; f[5] = kActC[T1]; f[8] = 64;
         f[10] = p.H; f[11] = p.W; f[12] = 3; f[14] = 1; f[15] = 64; f[16] = 1; f[17] = 1;
-        f[19] = p.split ? 1 : 0; f[23] = f[24] = -1;
+        f[19] = tc_planes(p.fmt) - 1; f[23] = f[24] = -1;
         f[26] = net->last.in_u8;
     } else {
         const PlanLaunch& l = p.launches[i - 1];
@@ -1054,23 +1067,23 @@ int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
         f[4] = l.out; f[5] = a.out_cstride; f[6] = a.out_ch_off[0]; f[7] = a.out_ch_off[1];
         f[8] = a.store_ch[0]; f[9] = a.store_ch[1];
         f[10] = a.H; f[11] = a.W; f[12] = a.ksize; f[13] = a.cin_blocks; f[14] = a.groups; f[15] = a.n_tile;
-        f[16] = a.n_tiles; f[17] = a.relu; f[18] = a.pool; f[19] = a.split; f[20] = a.chunk; f[21] = a.pdl; f[22] = a.tps;
+        f[16] = a.n_tiles; f[17] = a.relu; f[18] = a.pool; f[19] = a.split; f[20] = tc_chunked(a.fmt) ? 1 : 0; f[21] = a.pdl; f[22] = a.tps;
         f[23] = l.f32[0]; f[24] = l.f32[1];
     }
     f[25] = p.n;
-    f[B200POSE_DEBUG_LAUNCH_FORMAT] = p.f16 ? 1 : 0;
+    f[B200POSE_DEBUG_LAUNCH_FORMAT] = tc_binary16(p.fmt) ? 1 : 0;
     for (int k = 0; k < nf; ++k) fields[k] = f[k];
     return nf;
 }
 
 int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes) {
-    if (!net || !last_ran_plan(net)) return fail("debug_read: no bf16 / bf16x3 forward has run");
+    if (!net || !last_ran_plan(net)) return fail("debug_read: no tensor-core forward has run");
     const int n = net->plan->n, H = net->plan->H, W = net->plan->W;
     if (img0 < 0 || count < 1 || img0 + count > n || !host) return fail("debug_read: images [%d, %d) out of range", img0, img0 + count);
     const char* src = nullptr;
     size_t per = 0;
     if (buf >= 0 && buf < kNumAct) {
-        if (lo_plane && !net->plan->split) return fail("debug_read: residual planes exist in bf16x3 mode only");
+        if (lo_plane && tc_planes(net->plan->fmt) < 2) return fail("debug_read: residual planes exist in bf16x3 mode only");
         per = (size_t)(H / kActDiv[buf]) * (W / kActDiv[buf]) * kActC[buf] * 2;
         src = reinterpret_cast<const char*>((lo_plane ? net->act_lo : net->act)[buf].p);
     } else if (buf >= kNumAct && buf < kNumAct + 12 && !lo_plane) {
@@ -1087,7 +1100,7 @@ int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, 
 }
 
 int b200pose_net_debug_fp8(b200pose_net* net, int launch, int* act_exp, int n_img, int* w_exp, int cap) {
-    if (!net || !last_ran_plan(net) || !net->plan->fp8) { fail("debug_fp8: no fp8 forward has run"); return -1; }
+    if (!net || !last_ran_plan(net) || net->plan->fmt != TcFormat::kFp8) { fail("debug_fp8: no fp8 forward has run"); return -1; }
     const Plan& p = *net->plan;
     if (launch < 1 || launch > (int)p.launches.size() || n_img != p.n || !act_exp || !w_exp) {
         fail("debug_fp8: launch %d / images %d out of range", launch, n_img);
@@ -1113,7 +1126,7 @@ int b200pose_net_overflow(b200pose_net* net, int* flags, int n, void* cuda_strea
     std::vector<unsigned> h(n, 0u);
     if (cudaSetDevice(net->device) != cudaSuccess ||
         cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(cuda_stream)) != cudaSuccess ||
-        (net->last.mode == B200POSE_MODE_FP16 &&
+        (!net->last.fp32 && tc_aux(net->last.fmt) == TcAux::kOverflow &&
          cudaMemcpy(h.data(), net->ovf.p, n * sizeof(unsigned), cudaMemcpyDeviceToHost) != cudaSuccess)) {
         fail("overflow: %s", cudaGetErrorString(cudaGetLastError()));
         return -1;
@@ -1446,7 +1459,7 @@ static int check_infer(const b200pose_net* net, const b200pose_post* post) {
 // (b200pose_post_overflow reads them once the run is fetched).  Stream-ordered before the run's post-processing, whose
 // completion the fetch waits for.
 static int stash_overflow(const b200pose_net* net, b200pose_post* post, int nimg, cudaStream_t st) {
-    if (net->last.mode != B200POSE_MODE_FP16) return 0;
+    if (net->last.fp32 || tc_aux(net->last.fmt) != TcAux::kOverflow) return 0;
     if (post->ovf_pending >= kMaxOvfRows || nimg > 2 * post->pb.batch_cap) return fail("overflow rows exhausted");
     unsigned* dst = post->hp_ovf[post->runs & 1] + (size_t)post->ovf_pending * 2 * post->pb.batch_cap;
     CU(cudaMemcpyAsync(dst, net->ovf.p, nimg * sizeof(unsigned), cudaMemcpyDeviceToHost, st));

@@ -166,21 +166,24 @@ __device__ __forceinline__ void mma_f16_16816(float (&d)[4], const uint32_t (&a)
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-template <bool kF16> __device__ __forceinline__ uint32_t pack16(float lo, float hi) {
-    if constexpr (kF16) return pack_f16x2(lo, hi);
+template <bool kBinary16> __device__ __forceinline__ uint32_t pack16(float lo, float hi) {
+    if constexpr (kBinary16) return pack_f16x2(lo, hi);
     else return pack_bf16(lo, hi);
 }
 
-// fp8 mode (DESIGN.md §2.3): kAmax also records each image's max |stored bf16| (fp32 bits, atomic max) in amax[n] for
-// the next launch's activation scale.  fp16 mode (kF16): inputs, weights and outputs are binary16, and amax[n] is the
-// image's overflow flag, set to 1 when an input value (an fp32 input beyond 65504, or NaN) or a stored value is not
-// finite in binary16 - an infinite input can give NaN sums, which the ReLU would turn into a finite 0.
-template <int kIn, bool kAmax, bool kF16>
+// F: bf16, fp8 or fp16 (tc_format.h).  fp8 (DESIGN.md §2.3) also records each image's max |stored bf16| (fp32 bits,
+// atomic max) in aux[n] for the next launch's activation scale.  fp16: inputs, weights and outputs are binary16, and
+// aux[n] is the image's overflow flag, set to 1 when an input value (an fp32 input beyond 65504, or NaN) or a stored
+// value is not finite in binary16 - an infinite input can give NaN sums, which the ReLU would turn into a finite 0.
+template <int kIn, TcFormat F>
 __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* __restrict__ in_v, const float* __restrict__ wgt,
                                                                     const float* __restrict__ bias,
                                                                     __nv_bfloat16* __restrict__ out, int H, int W,
-                                                                    const int* __restrict__ ext, unsigned* amax) {
+                                                                    const int* __restrict__ ext, unsigned* aux) {
     constexpr bool kU8 = kIn != 0;
+    constexpr bool kAmax = tc_aux(F) == TcAux::kAmax;
+    constexpr bool kOverflow = tc_aux(F) == TcAux::kOverflow;
+    constexpr bool kBinary16 = tc_binary16(F);
     constexpr int kRowF = kF_TW + 2, kPlaneF = (kF_TH + 2) * kRowF;
     __shared__ float s_in[3 * kPlaneF];
     __shared__ __align__(16) uint32_t s_out[kF_TH * kF_TW * 32];      // [pixel][8 chunks of 16 B], chunk index ^ (pixel & 7)
@@ -235,7 +238,7 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
                 const int k0 = 16 * s2 + 2 * q + 8 * hh;
                 const float w0 = k0 < 27 ? __ldg(wgt + (8 * j + r0) * 27 + k0) : 0.f;
                 const float w1 = k0 + 1 < 27 ? __ldg(wgt + (8 * j + r0) * 27 + k0 + 1) : 0.f;
-                bfrag[j][s2][hh] = pack16<kF16>(w0, w1);
+                bfrag[j][s2][hh] = pack16<kBinary16>(w0, w1);
             }
     float bs[8][2];
 #pragma unroll
@@ -255,18 +258,18 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
                 v[j][0] = off >= 0 ? srow[off + 16 * mt + r0] : 0.f;
                 v[j][1] = off >= 0 ? srow[off + 16 * mt + r0 + 8] : 0.f;
             }
-            afrag[s2][0] = pack16<kF16>(v[0][0], v[1][0]);  // row r0,     k = 2q, 2q+1
-            afrag[s2][1] = pack16<kF16>(v[0][1], v[1][1]);  // row r0 + 8, k = 2q, 2q+1
-            afrag[s2][2] = pack16<kF16>(v[2][0], v[3][0]);  // row r0,     k = 2q+8, 2q+9
-            afrag[s2][3] = pack16<kF16>(v[2][1], v[3][1]);  // row r0 + 8, k = 2q+8, 2q+9
-            if constexpr (kF16)
+            afrag[s2][0] = pack16<kBinary16>(v[0][0], v[1][0]);  // row r0,     k = 2q, 2q+1
+            afrag[s2][1] = pack16<kBinary16>(v[0][1], v[1][1]);  // row r0 + 8, k = 2q, 2q+1
+            afrag[s2][2] = pack16<kBinary16>(v[2][0], v[3][0]);  // row r0,     k = 2q+8, 2q+9
+            afrag[s2][3] = pack16<kBinary16>(v[2][1], v[3][1]);  // row r0 + 8, k = 2q+8, 2q+9
+            if constexpr (kOverflow)
                 bad_in |= f16x2_nonfinite(afrag[s2][0]) | f16x2_nonfinite(afrag[s2][1]) | f16x2_nonfinite(afrag[s2][2]) |
                           f16x2_nonfinite(afrag[s2][3]);
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             float d[4] = {bs[j][0], bs[j][1], bs[j][0], bs[j][1]};
-            if constexpr (kF16) {
+            if constexpr (kBinary16) {
                 mma_f16_16816(d, afrag[0], bfrag[j][0][0], bfrag[j][0][1]);
                 mma_f16_16816(d, afrag[1], bfrag[j][1][0], bfrag[j][1][1]);
             } else {
@@ -275,8 +278,8 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
             }
             // d0, d1: pixel row r0, channels 8j + 2q, +1;  d2, d3: pixel row r0 + 8
             const int p0 = warp * kF_TW + 16 * mt + r0, p1 = p0 + 8;
-            s_out[p0 * 32 + ((j ^ (p0 & 7)) << 2) + q] = pack16<kF16>(fmaxf(d[0], 0.f), fmaxf(d[1], 0.f));
-            s_out[p1 * 32 + ((j ^ (p1 & 7)) << 2) + q] = pack16<kF16>(fmaxf(d[2], 0.f), fmaxf(d[3], 0.f));
+            s_out[p0 * 32 + ((j ^ (p0 & 7)) << 2) + q] = pack16<kBinary16>(fmaxf(d[0], 0.f), fmaxf(d[1], 0.f));
+            s_out[p1 * 32 + ((j ^ (p1 & 7)) << 2) + q] = pack16<kBinary16>(fmaxf(d[2], 0.f), fmaxf(d[3], 0.f));
         }
     }
     __syncthreads();
@@ -292,15 +295,15 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
 #pragma unroll
                 for (int k = 0; k < 4; ++k) mx = max(mx, max(w4[k] & 0x7fffu, (w4[k] >> 16) & 0x7fffu));
             }
-            if constexpr (kF16) mx |= f16x2_nonfinite(v.x) | f16x2_nonfinite(v.y) | f16x2_nonfinite(v.z) | f16x2_nonfinite(v.w);
+            if constexpr (kOverflow) mx |= f16x2_nonfinite(v.x) | f16x2_nonfinite(v.y) | f16x2_nonfinite(v.z) | f16x2_nonfinite(v.w);
         }
     }
     if constexpr (kAmax) {
         mx = __reduce_max_sync(0xffffffffu, mx);     // max of non-negative float bits: order-independent
-        if (lane == 0 && mx != 0) atomicMax(amax + n, mx << 16);
+        if (lane == 0 && mx != 0) atomicMax(aux + n, mx << 16);
     }
-    if constexpr (kF16) {
-        if (__any_sync(0xffffffffu, mx | bad_in) && lane == 0) atomicOr(amax + n, 1u);
+    if constexpr (kOverflow) {
+        if (__any_sync(0xffffffffu, mx | bad_in) && lane == 0) atomicOr(aux + n, 1u);
     }
 }
 
@@ -412,22 +415,28 @@ __global__ void nchw_to_nhwc_f32_kernel(const float* __restrict__ in, float* __r
 
 }  // namespace
 
-cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias,
-                              __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo, int N, int H, int W, const int* ext,
-                              cudaStream_t s, unsigned* amax, unsigned* ovf) {
+cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias, TcFormat fmt,
+                              __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo, unsigned* aux, int N, int H, int W,
+                              const int* ext, cudaStream_t s) {
     dim3 grid((W + kF_TW - 1) / kF_TW, (H + kF_TH - 1) / kF_TH, N);
-    if ((amax != nullptr || ovf != nullptr) && out_lo != nullptr) return cudaErrorInvalidValue;
-    if (amax != nullptr && ovf != nullptr) return cudaErrorInvalidValue;
+    if ((tc_planes(fmt) == 2 && out_lo == nullptr) || (tc_aux(fmt) != TcAux::kNone && aux == nullptr))
+        return cudaErrorInvalidValue;
     auto launch = [&](auto pre) {
         constexpr int kIn = decltype(pre)::value;
-        if (amax != nullptr)            // fp8 mode: the bf16 tensor-core kernel, recording amax
-            conv_first_mma_kernel<kIn, true, false><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, amax);
-        else if (ovf != nullptr)        // fp16 mode: binary16 operands and output, overflow flags
-            conv_first_mma_kernel<kIn, false, true><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, ovf);
-        else if (out_lo == nullptr)     // bf16 mode: tensor cores
-            conv_first_mma_kernel<kIn, false, false><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, nullptr);
-        else                            // bf16x3 mode: fp32 CUDA cores, residual plane
-            conv_first_kernel<kIn><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext);
+        switch (fmt) {
+            case TcFormat::kBf16:       // tensor cores
+                conv_first_mma_kernel<kIn, TcFormat::kBf16><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, nullptr);
+                break;
+            case TcFormat::kBf16x3:     // fp32 CUDA cores, residual plane
+                conv_first_kernel<kIn><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, out_lo, H, W, ext);
+                break;
+            case TcFormat::kFp8:        // the bf16 tensor-core kernel, recording amax
+                conv_first_mma_kernel<kIn, TcFormat::kFp8><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, aux);
+                break;
+            case TcFormat::kFp16:       // binary16 operands and output, overflow flags
+                conv_first_mma_kernel<kIn, TcFormat::kFp16><<<grid, kF_Threads, 0, s>>>(in, w_oihw, bias, out_nhwc, H, W, ext, aux);
+                break;
+        }
     };
     switch (in_is_u8_hwc) {
         case kPreNone: launch(std::integral_constant<int, kPreNone>()); break;

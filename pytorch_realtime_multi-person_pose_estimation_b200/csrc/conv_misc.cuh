@@ -3,6 +3,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include "tc_format.h"
+
 namespace b2p {
 
 struct ConvF32Args {
@@ -18,13 +20,14 @@ struct ConvF32Args {
     int ext_shift;        // log2 of the network input size over H, W
 };
 
-// in: fp32 NCHW [N,3,H,W] (in_is_u8_hwc = 0), or uint8 HWC BGR [N,H,W,3] with the normalisation `in_is_u8_hwc`
-// (preprocess_core.h: 1 rtpose, 2 vgg, 3 inception, 4 ssd) fused into the load
-cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias,
-                              __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo /*residual plane or null*/, int N, int H,
-                              int W, const int* ext /*ragged batch: padded H, W per image, or null*/, cudaStream_t s,
-                              unsigned* amax = nullptr /*fp8 mode: per-image max |stored bf16| (fp32 bits), atomic max*/,
-                              unsigned* ovf = nullptr /*fp16 mode: binary16 output; per-image flag, 1 = a value overflowed*/);
+// conv1_1 in format fmt.  in: fp32 NCHW [N,3,H,W] (in_is_u8_hwc = 0), or uint8 HWC BGR [N,H,W,3] with the
+// normalisation `in_is_u8_hwc` (preprocess_core.h: 1 rtpose, 2 vgg, 3 inception, 4 ssd) fused into the load.
+// out_lo: the residual plane (bf16x3).  aux: the format's per-image table (tc_aux): fp8 max |stored bf16| (fp32 bits,
+// atomic max), fp16 overflow flags (1 = a value overflowed).  cudaErrorInvalidValue when the format's pointer is null.
+// ext: ragged batch, padded H, W per image, or null.
+cudaError_t conv_first_launch(const void* in, int in_is_u8_hwc, const float* w_oihw, const float* bias, TcFormat fmt,
+                              __nv_bfloat16* out_nhwc, __nv_bfloat16* out_lo, unsigned* aux, int N, int H, int W,
+                              const int* ext, cudaStream_t s);
 // ext (ragged batch) or null: pixels outside image i's padded extent ext[2 i], ext[2 i + 1] become 0 (zero padding)
 cudaError_t u8hwc_to_f32nchw_launch(const unsigned char* in, float* out, int N, int H, int W, int mode, const int* ext,
                                     cudaStream_t s);

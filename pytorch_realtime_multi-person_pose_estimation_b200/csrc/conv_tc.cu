@@ -62,53 +62,34 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// 16-bit operands, k16: bfloat16 (kF16 = false) or IEEE binary16
-template <int N, bool kF16 = false> struct Mma;
-template <> struct Mma<128> {
-    static __device__ __forceinline__ void run(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n128k16_rs(d, a, b, s); }
-};
-template <> struct Mma<64> {
-    static __device__ __forceinline__ void run(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n64k16_rs(d, a, b, s); }
-};
-template <> struct Mma<48> {
-    static __device__ __forceinline__ void run(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n48k16_rs(d, a, b, s); }
-};
-template <> struct Mma<32> {
-    static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n32k16_rs(d, a, b, s); }
-};
-template <> struct Mma<128, true> {
-    static __device__ __forceinline__ void run(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n128k16_f16_rs(d, a, b, s); }
-};
-template <> struct Mma<64, true> {
-    static __device__ __forceinline__ void run(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n64k16_f16_rs(d, a, b, s); }
-};
-template <> struct Mma<48, true> {
-    static __device__ __forceinline__ void run(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n48k16_f16_rs(d, a, b, s); }
-};
-template <> struct Mma<32, true> {
-    static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n32k16_f16_rs(d, a, b, s); }
-};
-template <int N> struct Mma8;      // e4m3, k32
-template <> struct Mma8<64> {
-    static __device__ __forceinline__ void run(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n64k32_e4m3_rs(d, a, b, s); }
-};
-template <> struct Mma8<48> {
-    static __device__ __forceinline__ void run(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n48k32_e4m3_rs(d, a, b, s); }
-};
-template <> struct Mma8<32> {
-    static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t s) { wgmma_m64n32k32_e4m3_rs(d, a, b, s); }
-};
+// wgmma of format F with A in registers: k16 on bf16 (bf16, bf16x3) or binary16 (fp16) operands, k32 on e4m3 (fp8)
+#define B2P_MMA(SHAPE)                                                        \
+    if constexpr (tc_weights(F) == TcWeights::kE4m3) SHAPE("e4m3", "32", ""); \
+    else if constexpr (tc_binary16(F)) SHAPE("f16", "16", ", 0");             \
+    else SHAPE("bf16", "16", ", 0")
+template <TcFormat F, int N>
+__device__ __forceinline__ void mma(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+    if constexpr (N == 128) { B2P_MMA(B2P_WGMMA_M64N128_RS); }
+    else if constexpr (N == 64) { B2P_MMA(B2P_WGMMA_M64N64_RS); }
+    else if constexpr (N == 48) { B2P_MMA(B2P_WGMMA_M64N48_RS); }
+    else { static_assert(N == 32, "n-tile"); B2P_MMA(B2P_WGMMA_M64N32_RS); }
+}
+#undef B2P_MMA
 
 constexpr int kConsumerWarps = 8;
 
-// kRagged: a.ext is set (ragged batch); a separate instantiation so that uniform batches run the unmasked epilogue.
-// kFp8 (with kChunk): the fp8 mode (DESIGN.md §2.3) - each tap's A fragments are converted from the bf16 patch to e4m3 in
-// registers, the weights are e4m3 slices of 64-byte rows, every tap's two k32 MMAs start a fresh accumulator that is
-// then added to the fp32 sum, and the epilogue records the per-image max |stored bf16|.
-// kF16: the fp16 mode - the bf16 plan with binary16 activations and weights (same fragments, same full-K fp32
-// accumulation); the epilogue stores binary16 and flags every image for which a stored value is +-inf or NaN.
-template <int N, bool kChunk, bool kRagged, bool kFp8, bool kF16 = false>
+// F: the arithmetic format (tc_format.h).  kRagged: a.ext is set (ragged batch); a separate instantiation so that uniform
+// batches run the unmasked epilogue.
+// fp8 (DESIGN.md §2.3): each tap's A fragments are converted from the bf16 patch to e4m3 in registers, the weights are
+// e4m3 slices of 64-byte rows, every tap's two k32 MMAs start a fresh accumulator that is then added to the fp32 sum,
+// and the epilogue records the per-image max |stored bf16|.
+// fp16: the bf16 plan with binary16 activations and weights (same fragments, same full-K fp32 accumulation); the
+// epilogue stores binary16 and flags every image for which a stored value is +-inf or NaN.
+template <TcFormat F, int N, bool kRagged>
 __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
+    constexpr bool kChunk = tc_chunked(F);
+    constexpr bool kE4m3 = tc_weights(F) == TcWeights::kE4m3;
+    constexpr TcAux kAux = tc_aux(F);
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B operands need 1024 B alignment.
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -130,7 +111,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     const int taps = a.ksize * a.ksize;
     const int pad = a.ksize >> 1;
     const uint32_t patch_tx = kPatchPitch * (kTileH + a.ksize - 1) * 128;
-    constexpr uint32_t b_tx = kFp8 ? N * 64 : N * 128;       // one tap's weight slice
+    constexpr uint32_t b_tx = N * tc_w_row_bytes(F);         // one tap's weight slice
     // The weight ring is cut into stages of `tps` consecutive taps (a.tps, chosen with the tensor map's box): fewer, larger
     // stages mean fewer barrier round trips per tile.
     const int tps = a.tps;
@@ -213,10 +194,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
         const int wA = lane >> 2;
         const int cq = 2 * (lane & 3);
         const uint32_t patch0 = smem_u32(patch_smem);
-        const uint64_t bdesc_hi = kFp8 ? make_sdesc_sw64(0, 512) : make_sdesc_sw128(0, 1024);
+        const uint64_t bdesc_hi = kE4m3 ? make_sdesc_sw64(0, 512) : make_sdesc_sw128(0, 1024);
         const uint32_t b_lo0 = (smem_u32(b_smem) & 0x3FFFFu) >> 4;
-        const bool row_chunks = kChunk && !kFp8 && a.ksize == 7;    // K-chunked mode: one chunk per filter row (7x7; tps == 1) ...
-        const bool blk_chunks = kChunk && !kFp8 && !row_chunks;     // ... or per (channel block, term); fp8: per tap
+        const bool row_chunks = kChunk && !kE4m3 && a.ksize == 7;   // bf16x3: one chunk per filter row (7x7; tps == 1) ...
+        const bool blk_chunks = kChunk && !kE4m3 && !row_chunks;    // ... or per (channel block, term); fp8: per tap
         const int Ho = a.pool ? a.H >> 1 : a.H;
         const int Wo = a.pool ? a.W >> 1 : a.W;
         float acc[N / 2];
@@ -232,7 +213,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             }
             int ea = 0;           // fp8: the activation scale exponent of this tile's image
             float sa = 1.f;
-            if constexpr (kFp8) {
+            if constexpr (kE4m3) {
                 uint32_t m = __ldcg(a.amax_in[0] + tc.n);
                 if (a.amax_in[1] != nullptr) m = max(m, __ldcg(a.amax_in[1] + tc.n));
                 ea = fp8_exp_from_amax(m);
@@ -261,7 +242,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                             uint32_t af[4][4];
 #pragma unroll
                             for (int k = 0; k < 4; ++k) ldmatrix_x4(row_addr + (((2 * k + kc) ^ sw) << 4), af[k]);
-                            if constexpr (kFp8) {
+                            if constexpr (kE4m3) {
                                 // k32 step s takes bf16 k16 steps 2s, 2s + 1 (K order: fp8_k_to_channel)
                                 uint32_t a8[2][4];
 #pragma unroll
@@ -275,7 +256,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                                 wgmma_fence();
 #pragma unroll
                                 for (int s = 0; s < 2; ++s)
-                                    Mma8<N>::run(acc, a8[s], bdesc_hi | (b_lo + j * (b_tx >> 4) + s * 2), s);
+                                    mma<F, N>(acc, a8[s], bdesc_hi | (b_lo + j * (b_tx >> 4) + s * 2), s);
                                 wgmma_commit();
                                 wgmma_wait_all();
                                 fence_regs(acc);
@@ -286,7 +267,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                             wgmma_fence();
 #pragma unroll
                             for (int k = 0; k < 4; ++k) {
-                                Mma<N, kF16>::run(acc, af[k], bdesc_hi | (b_lo + j * (b_tx >> 4) + k * 2), scale);
+                                mma<F, N>(acc, af[k], bdesc_hi | (b_lo + j * (b_tx >> 4) + k * 2), scale);
                                 scale = 1;
                             }
                             wgmma_commit();
@@ -349,7 +330,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             for (int j = 0; j < N / 8; ++j) {
                 const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + cq));
                 float v[4];
-                if constexpr (kFp8) {     // acc * 2^-(ea + ew) is exact: one rounding, at the bias add
+                if constexpr (kE4m3) {    // acc * 2^-(ea + ew) is exact: one rounding, at the bias add
                     const int2 w2 = __ldg(reinterpret_cast<const int2*>(w_exp + 8 * j + cq));
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
@@ -375,18 +356,18 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                     if (!wr[hh]) continue;
                     const float lo = inside[hh] ? v[2 * hh] : 0.f, hi = inside[hh] ? v[2 * hh + 1] : 0.f;
                     if (out_px[hh] != nullptr && 8 * j < store_ch) {
-                        if constexpr (kFp8) {
+                        if constexpr (kAux == TcAux::kAmax) {
                             const uint32_t pk = pack_bf16x2(lo, hi);
                             *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pk;
                             amax = max(amax, max(pk & 0x7fffu, (pk >> 16) & 0x7fffu));
-                        } else if constexpr (kF16) {
+                        } else if constexpr (kAux == TcAux::kOverflow) {
                             const uint32_t pk = pack_f16x2(lo, hi);
                             *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pk;
                             ovf |= f16x2_nonfinite(pk);
                         } else {
                             *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pack_bf16x2(lo, hi);
                         }
-                        if (a.out_lo != nullptr) {      // split mode: residual plane v - bf16(v)
+                        if (a.out_lo != nullptr) {      // bf16x3: residual plane v - bf16(v)
                             __nv_bfloat16* dlo = a.out_lo + (out_px[hh] - a.out) + 8 * j;
                             *reinterpret_cast<uint32_t*>(dlo) =
                                 pack_bf16x2(lo - __bfloat162float(__float2bfloat16_rn(lo)), hi - __bfloat162float(__float2bfloat16_rn(hi)));
@@ -399,14 +380,14 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                     }
                 }
             }
-            if constexpr (kFp8) {     // max of non-negative float bits: order-independent, so runs stay deterministic
+            if constexpr (kAux == TcAux::kAmax) {     // max of non-negative float bits: order-independent, so runs stay deterministic
                 amax = __reduce_max_sync(0xffffffffu, amax);
                 if (lane == 0 && amax != 0) atomicMax(a.amax_out + tc.n, amax << 16);
             }
             // fp16: only lanes that stored a non-finite value take part; ptxas aggregates them into one reduction per warp.
             // No vote and no lane-0 branch here: either makes the whole tile loop divergent for the compiler, which then
             // builds the wgmma descriptors in vector registers instead of on the uniform datapath (5 % slower).
-            if constexpr (kF16) {
+            if constexpr (kAux == TcAux::kOverflow) {
                 if (ovf) atomicOr(a.ovf_out + tc.n, 1u);
             }
             if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(7);
@@ -415,19 +396,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     if (threadIdx.x == 0) B2P_TL(9);
 }
 
-template <int N, bool kChunk, bool kRagged>
+template <TcFormat F, int N, bool kRagged>
 __global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_kernel(const __grid_constant__ ConvTcArgs a) {
-    conv_tc_body<N, kChunk, kRagged, false>(a);
-}
-
-template <int N, bool kRagged>
-__global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_fp8_kernel(const __grid_constant__ ConvTcArgs a) {
-    conv_tc_body<N, true, kRagged, true>(a);
-}
-
-template <int N, bool kRagged>
-__global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_f16_kernel(const __grid_constant__ ConvTcArgs a) {
-    conv_tc_body<N, false, kRagged, false, true>(a);
+    conv_tc_body<F, N, kRagged>(a);
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -456,17 +427,16 @@ cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cst
     if (a.ksize != 1 && a.ksize != 3 && a.ksize != 7) return cudaErrorInvalidValue;
     if (a.n_tile != 32 && a.n_tile != 48 && a.n_tile != 64 && a.n_tile != 128) return cudaErrorInvalidValue;
     if (a.groups < 1 || a.groups > 2 || in_cstride % 8 != 0) return cudaErrorInvalidValue;
-    if (a.split && in_lo == nullptr) return cudaErrorInvalidValue;
-    if (a.fp8 && (a.split || !a.chunk || a.n_tile > 64)) return cudaErrorInvalidValue;
-    if (a.f16 && (a.split || a.chunk || a.fp8)) return cudaErrorInvalidValue;
-    const CUtensorMapDataType t16 = a.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    for (int plane = 0; plane <= (a.split ? 1 : 0); ++plane) {
+    if (a.n_tile > tc_max_n_tile(a.fmt)) return cudaErrorInvalidValue;
+    if (tc_planes(a.fmt) == 2 && in_lo == nullptr) return cudaErrorInvalidValue;
+    a.split = tc_planes(a.fmt) - 1;
+    for (int plane = 0; plane < tc_planes(a.fmt); ++plane) {
         cuuint64_t dims[4] = {(cuuint64_t)in_cstride, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.n_img};
         cuuint64_t strides[3] = {(cuuint64_t)in_cstride * 2, (cuuint64_t)a.W * in_cstride * 2,
                                  (cuuint64_t)a.H * a.W * in_cstride * 2};
         cuuint32_t box[4] = {64, (cuuint32_t)kPatchPitch, (cuuint32_t)(kTileH + a.ksize - 1), 1};
         cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(plane ? &a.tm_in_lo : &a.tm_in, t16, 4,
+        CUresult r = enc(plane ? &a.tm_in_lo : &a.tm_in, tc_act_type(a.fmt), 4,
                          const_cast<__nv_bfloat16*>(plane ? in_lo : in), dims, strides,
                          box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -480,21 +450,19 @@ cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cst
         const int rows = a.groups * a.n_tiles * a.n_tile;
         const int taps = a.ksize * a.ksize;
         // taps per weight stage: as many as leave kMinBStages stages in the ring (N = 128: 2 taps of 16 KB, N = 32: 8 taps of
-        // 4 KB).  The K-chunked 7x7 mode closes a chunk at every filter-row end, which a stage must not straddle.
-        // fp8: one byte per weight, 64-byte rows (SWIZZLE_64B), chunks per tap, no residual slices
-        const int esz = a.fp8 ? 1 : 2;
+        // 4 KB).  bf16x3 closes a 7x7 chunk at every filter-row end, which a stage must not straddle (fp8 chunks per tap).
+        const int esz = tc_w_row_bytes(a.fmt) / 64;      // bytes per weight
         const int tap_bytes = a.n_tile * 64 * esz;
         int tps = (kNumBStages * kBStageBytes) / (kMinBStages * tap_bytes);
-        if (tps < 1 || (a.chunk && !a.fp8 && a.ksize == 7)) tps = 1;
+        if (tps < 1 || (tc_chunked(a.fmt) && tc_weights(a.fmt) != TcWeights::kE4m3 && a.ksize == 7)) tps = 1;
         if (tps > taps) tps = taps;
         a.tps = tps;
-        cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)rows, (cuuint64_t)(a.fp8 || a.f16 ? taps : 2 * taps)};
+        cuuint64_t dims[3] = {(cuuint64_t)cin_pad, (cuuint64_t)rows, (cuuint64_t)tc_w_slices(a.fmt, taps)};
         cuuint64_t strides[2] = {(cuuint64_t)cin_pad * esz, (cuuint64_t)rows * cin_pad * esz};
         cuuint32_t box[3] = {64, (cuuint32_t)a.n_tile, (cuuint32_t)tps};
         cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&a.tm_w, a.fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : t16, 3,
-                         const_cast<void*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         a.fp8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+        CUresult r = enc(&a.tm_w, tc_w_type(a.fmt), 3, const_cast<void*>(w), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, tc_w_swizzle(a.fmt),
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
             fprintf(stderr, "[b200pose] cuTensorMapEncodeTiled(w) failed: %d\n", (int)r);
@@ -508,14 +476,13 @@ namespace {
 // Programmatic dependent launch (a.pdl): the next layer's CTAs may start - barrier init, descriptor prefetch, weight loads -
 // while this layer's last CTAs drain; they wait (griddepcontrol.wait) before touching activations.  Used by the SMALL-batch
 // plans only, where the fixed cost per launch is most of a layer.
-template <int N, bool kChunk, bool kRagged, bool kFp8 = false, bool kF16 = false>
+template <TcFormat F, int N>
 cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
-    static DynSmemOptIn optin;   // per device: a second net on another GPU of the same process needs its own opt-in
-    void (*kernel)(ConvTcArgs);
-    if constexpr (kFp8) kernel = conv_tc_fp8_kernel<N, kRagged>;
-    else if constexpr (kF16) kernel = conv_tc_f16_kernel<N, kRagged>;
-    else kernel = conv_tc_kernel<N, kChunk, kRagged>;
-    cudaError_t e = optin.ensure(kernel, kConvTcSmemBytes);
+    // per kernel (uniform, ragged) and device: a second net on another GPU of the same process needs its own opt-in
+    static DynSmemOptIn optin[2];
+    const bool ragged = a.ext != nullptr;
+    void (*kernel)(ConvTcArgs) = ragged ? conv_tc_kernel<F, N, true> : conv_tc_kernel<F, N, false>;
+    cudaError_t e = optin[ragged].ensure(kernel, kConvTcSmemBytes);
     if (e != cudaSuccess) return e;
     if (a.pdl) {
         cudaLaunchConfig_t cfg = {};
@@ -534,47 +501,38 @@ cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
     return cudaGetLastError();
 }
 
-template <int N, bool kChunk, bool kFp8 = false, bool kF16 = false>
+// n-tiles 128 (not in the chunked formats), 64, 48 and 32
+template <TcFormat F>
 cudaError_t launch(int grid, cudaStream_t stream, const ConvTcArgs& a) {
-    return a.ext != nullptr ? launch_k<N, kChunk, true, kFp8, kF16>(grid, stream, a)
-                            : launch_k<N, kChunk, false, kFp8, kF16>(grid, stream, a);
+    switch (a.n_tile) {
+        case 128:
+            if constexpr (tc_max_n_tile(F) >= 128) return launch_k<F, 128>(grid, stream, a);
+            break;
+        case 64: return launch_k<F, 64>(grid, stream, a);
+        case 48: return launch_k<F, 48>(grid, stream, a);
+        case 32: return launch_k<F, 32>(grid, stream, a);
+    }
+    return cudaErrorInvalidValue;
 }
 }  // namespace
 
 cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream) {
     if (a.pool && ((a.H | a.W) & 1)) return cudaErrorInvalidValue;
-    if (a.chunk && a.n_tile > 64) return cudaErrorInvalidValue;      // K-chunked mode keeps a second accumulator set
     if (a.tps < 1) return cudaErrorInvalidValue;                     // conv_tc_make_maps has not run
+    if (tc_aux(a.fmt) == TcAux::kAmax && (a.amax_out == nullptr || a.amax_in[0] == nullptr || a.w_exp == nullptr))
+        return cudaErrorInvalidValue;
+    if (tc_aux(a.fmt) == TcAux::kOverflow && a.ovf_out == nullptr) return cudaErrorInvalidValue;
     const int tiles_x = (a.W + kTileW - 1) / kTileW;
     const int tiles_y = (a.H + kTileH - 1) / kTileH;
     const int total = a.n_img * tiles_y * tiles_x * a.groups * a.n_tiles;
     const int grid = total < num_sms ? total : num_sms;
-    if (a.fp8) {
-        if (!a.chunk || a.amax_out == nullptr || a.amax_in[0] == nullptr || a.w_exp == nullptr) return cudaErrorInvalidValue;
-        switch (a.n_tile) {
-            case 64: return launch<64, true, true>(grid, stream, a);
-            case 48: return launch<48, true, true>(grid, stream, a);
-            case 32: return launch<32, true, true>(grid, stream, a);
-            default: return cudaErrorInvalidValue;
-        }
+    switch (a.fmt) {
+        case TcFormat::kBf16: return launch<TcFormat::kBf16>(grid, stream, a);
+        case TcFormat::kBf16x3: return launch<TcFormat::kBf16x3>(grid, stream, a);
+        case TcFormat::kFp8: return launch<TcFormat::kFp8>(grid, stream, a);
+        case TcFormat::kFp16: return launch<TcFormat::kFp16>(grid, stream, a);
     }
-    if (a.f16) {
-        if (a.chunk || a.split || a.ovf_out == nullptr) return cudaErrorInvalidValue;
-        switch (a.n_tile) {
-            case 128: return launch<128, false, false, true>(grid, stream, a);
-            case 64: return launch<64, false, false, true>(grid, stream, a);
-            case 48: return launch<48, false, false, true>(grid, stream, a);
-            case 32: return launch<32, false, false, true>(grid, stream, a);
-            default: return cudaErrorInvalidValue;
-        }
-    }
-    switch (a.n_tile) {
-        case 128: return launch<128, false>(grid, stream, a);
-        case 64: return a.chunk ? launch<64, true>(grid, stream, a) : launch<64, false>(grid, stream, a);
-        case 48: return a.chunk ? launch<48, true>(grid, stream, a) : launch<48, false>(grid, stream, a);
-        case 32: return a.chunk ? launch<32, true>(grid, stream, a) : launch<32, false>(grid, stream, a);
-        default: return cudaErrorInvalidValue;
-    }
+    return cudaErrorInvalidValue;
 }
 
 #ifdef B2P_CONV_TIMELINE

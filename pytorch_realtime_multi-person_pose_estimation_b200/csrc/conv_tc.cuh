@@ -7,6 +7,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include "tc_format.h"
+
 namespace b2p {
 
 constexpr int kTileW = 8;         // CTA tile: 8 (w) x 16 (h) output pixels = two wgmma M=64 halves of 8 x 8 (one per consumer warpgroup)
@@ -49,39 +51,35 @@ struct ConvTcArgs {
     int store_ch[2];          // channels (multiple of 8) stored per group *per n-tile*
     float* out_f32[2];        // optional NCHW fp32 copy per group (heads), may be null
     int f32_ch[2];            // valid channels of the fp32 copy
-    // ---- split-precision ("bf16x3") mode: operands are hi + lo bf16 planes, three MMA terms per K block
-    int split;                // 0: plain bf16; 1: A_hi*W_hi + A_hi*W_lo + A_lo*W_hi
-    __nv_bfloat16* out_lo;    // residual plane of the output (same geometry as `out`), split mode only
-    // ---- K-chunked accumulation (n_tile <= 64): see conv_tc_chunk_kernel
-    int chunk;
+    // ---- bf16x3: operands are hi + lo bf16 planes, three MMA terms per K block
+    int split;                // set by conv_tc_make_maps: 1 in bf16x3 (A_hi*W_hi + A_hi*W_lo + A_lo*W_hi), else 0
+    __nv_bfloat16* out_lo;    // residual plane of the output (same geometry as `out`), bf16x3 only
+    // ---- arithmetic format (tc_format.h): selects the kernel
+    TcFormat fmt;
     // ---- taps per weight stage (set by conv_tc_make_maps together with the weight map's box)
     int tps;
     // ---- programmatic dependent launch of this layer behind the previous one (small-batch plans)
     int pdl;
     // ---- tensor maps
     CUtensorMap tm_in;        // 4D (C, W, H, N) bf16, box (64, 16, 16+ks-1, 1), SWIZZLE_128B
-    CUtensorMap tm_w;         // 3D (cin_pad, groups*n_tiles*n_tile, 2*taps) bf16 [hi taps | lo taps], box (64, n_tile, tps)
-    CUtensorMap tm_in_lo;     // residual plane of the input (split mode)
+    CUtensorMap tm_w;         // 3D (cin_pad, groups*n_tiles*n_tile, tc_w_slices), box (64, n_tile, tps)
+    CUtensorMap tm_in_lo;     // residual plane of the input (bf16x3)
     // ---- ragged batches (DESIGN.md §1): ext[2 i], ext[2 i + 1] = padded H, W of image i at the network input; every
     // output element of image i outside (ext >> ext_shift) is stored as +0.  null: every image fills the canvas.
     const int* ext;
     int ext_shift;            // log2 of the network input size over this launch's OUTPUT size (pooling included)
-    // ---- fp8 mode (DESIGN.md §2.3): e4m3 operands, per-(launch, image) activation and per-row weight scales; n_tile <= 64
-    int fp8;
+    // ---- fp8 (DESIGN.md §2.3): e4m3 operands, per-(launch, image) activation and per-row weight scales
     const unsigned* amax_in[2];   // per-image max |bf16| (fp32 bits) of the launches that wrote the input; [1] may be null
     unsigned* amax_out;           // this launch's per-image max |stored bf16|, atomic max
     const int* w_exp;             // [groups * n_tiles * n_tile]: weight row r holds e4m3(w * 2^w_exp[r])
     int* ea_out;                  // the activation exponent each image used (may be null)
-    // ---- fp16 mode (DESIGN.md §2.3): binary16 activations (`in`, `out`) and weights, full-K fp32 accumulation
-    int f16;
+    // ---- fp16 (DESIGN.md §2.3): binary16 activations (`in`, `out`) and weights, full-K fp32 accumulation
     unsigned* ovf_out;            // per image: set to 1 when a value the launch stores is +-inf or NaN in binary16
 };
 
-// Builds the tensor maps. `in` (and `in_lo` in split mode): NHWC buffers with `in_cstride` channels per pixel.
-// `w`: packed weights [2*taps][groups*n_tiles*n_tile][cin_blocks*64]: bf16(w) for the first `taps` slices, the
-// residual bf16(w - hi) for the second.  fp8 mode (a.fp8): [taps][rows][cin_blocks*64] e4m3 bytes, each 32-channel
-// slice in the K order of fp8_k_to_channel (fp8_core.h).  fp16 mode (a.f16): `in` holds binary16 bits and `w` is
-// [taps][rows][cin_blocks*64] binary16 (no residual slices).
+// Builds the tensor maps and sets a.tps and a.split from a.fmt. `in` (and `in_lo` in bf16x3): NHWC buffers with
+// `in_cstride` channels per pixel (fp16: binary16 bits).  `w`: the packed weights of tc_weights(a.fmt) (tc_format.h)
+// with rows = groups*n_tiles*n_tile and cin_pad = cin_blocks*64.
 cudaError_t conv_tc_make_maps(ConvTcArgs& a, const __nv_bfloat16* in, int in_cstride, const void* w,
                               const __nv_bfloat16* in_lo = nullptr);
 cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream);

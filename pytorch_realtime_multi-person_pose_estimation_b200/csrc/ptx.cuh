@@ -106,75 +106,53 @@ __device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t saddr, uint32_t sb
     return d;
 }
 
-// D[64 x N] (+)= A[64 x 16, registers] * B[16 x N, shared memory descriptor], 16-bit operands (TYPE: "bf16" or
-// "f16"; A fragments and the K-major B layout are the same for both) -> fp32.  scale_d = 0: D = A * B.
-#define B2P_WGMMA_M64N128K16_RS(TYPE) \
+// D[64 x N] (+)= A[64 x K, registers] * B[K x N, shared memory descriptor] -> fp32, the statement for one N, used
+// inside a function with the operands d (float[N / 2]), a (uint32_t[4]), desc_b and scale_d (0: D = A * B).
+// TYPE, K: "bf16" or "f16" with K = "16" (the same A fragments and K-major B layout for both), or "e4m3" with
+// K = "32".  TAIL: ", 0" (B not transposed) for the 16-bit types, "" for e4m3, which has no transpose operand.
+#define B2P_WGMMA_M64N128_RS(TYPE, K, TAIL) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\t" \
         "setp.ne.b32 p, %69, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPE "." TYPE " " \
+        "wgmma.mma_async.sync.aligned.m64n128k" K ".f32." TYPE "." TYPE " " \
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, " \
-        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}\n" \
+        "{%64, %65, %66, %67}, %68, p, 1, 1" TAIL ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d) \
         : "memory")
-__device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N128K16_RS("bf16");
-}
-__device__ __forceinline__ void wgmma_m64n128k16_f16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N128K16_RS("f16");
-}
 
-#define B2P_WGMMA_M64N64K16_RS(TYPE) \
+#define B2P_WGMMA_M64N64_RS(TYPE, K, TAIL) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\t" \
         "setp.ne.b32 p, %37, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32." TYPE "." TYPE " " \
+        "wgmma.mma_async.sync.aligned.m64n64k" K ".f32." TYPE "." TYPE " " \
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, " \
-        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n" \
+        "{%32, %33, %34, %35}, %36, p, 1, 1" TAIL ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d) \
         : "memory")
-__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N64K16_RS("bf16");
-}
-__device__ __forceinline__ void wgmma_m64n64k16_f16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N64K16_RS("f16");
-}
 
-#define B2P_WGMMA_M64N48K16_RS(TYPE) \
+#define B2P_WGMMA_M64N48_RS(TYPE, K, TAIL) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\t" \
         "setp.ne.b32 p, %29, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n48k16.f32." TYPE "." TYPE " " \
+        "wgmma.mma_async.sync.aligned.m64n48k" K ".f32." TYPE "." TYPE " " \
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, " \
-        "{%24, %25, %26, %27}, %28, p, 1, 1, 0;\n\t}\n" \
+        "{%24, %25, %26, %27}, %28, p, 1, 1" TAIL ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]) \
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d) \
         : "memory")
-__device__ __forceinline__ void wgmma_m64n48k16_rs(float (&d)[24], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N48K16_RS("bf16");
-}
-__device__ __forceinline__ void wgmma_m64n48k16_f16_rs(float (&d)[24], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N48K16_RS("f16");
-}
 
-#define B2P_WGMMA_M64N32K16_RS(TYPE) \
+#define B2P_WGMMA_M64N32_RS(TYPE, K, TAIL) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\t" \
         "setp.ne.b32 p, %21, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32." TYPE "." TYPE " " \
+        "wgmma.mma_async.sync.aligned.m64n32k" K ".f32." TYPE "." TYPE " " \
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, " \
-        "{%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}\n" \
+        "{%16, %17, %18, %19}, %20, p, 1, 1" TAIL ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d) \
         : "memory")
-__device__ __forceinline__ void wgmma_m64n32k16_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N32K16_RS("bf16");
-}
-__device__ __forceinline__ void wgmma_m64n32k16_f16_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    B2P_WGMMA_M64N32K16_RS("f16");
-}
 
 // ---------------------------------------------------------------- binary16 (fp16 mode)
 // Two floats rounded to nearest even on the binary16 grid (subnormals kept, beyond 65504 + half an ulp: +-inf); lo in
@@ -190,7 +168,7 @@ __device__ __forceinline__ uint32_t f16x2_nonfinite(uint32_t v) {
     return ((v & 0x7c007c00u) + 0x04000400u) & 0x80008000u;
 }
 
-// ---------------------------------------------------------------- fp8 (e4m3) wgmma, k32
+// ---------------------------------------------------------------- fp8 (e4m3)
 // As make_sdesc_sw128 for 64-byte rows (64 e4m3) with the 64-byte swizzle: layout type 2.
 __device__ __forceinline__ uint64_t make_sdesc_sw64(uint32_t saddr, uint32_t sbo_bytes) {
     uint64_t d = 0;
@@ -212,45 +190,6 @@ __device__ __forceinline__ uint32_t bf16x4_to_e4m3x4(uint32_t u, uint32_t v, flo
     uint32_t r;
     asm("mov.b32 %0, {%1, %2};" : "=r"(r) : "h"(lo), "h"(hi));
     return r;
-}
-
-// D[64 x 64] (+)= A[64 x 32, registers] * B[32 x 64, shared memory descriptor], e4m3 -> fp32.
-__device__ __forceinline__ void wgmma_m64n64k32_e4m3_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %37, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
-        : "memory");
-}
-
-// D[64 x 48] (+)= A[64 x 32, registers] * B[32 x 48, shared memory descriptor], e4m3 -> fp32.
-__device__ __forceinline__ void wgmma_m64n48k32_e4m3_rs(float (&d)[24], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %29, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n48k32.f32.e4m3.e4m3 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
-        "{%24, %25, %26, %27}, %28, p, 1, 1;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
-        : "memory");
-}
-
-// D[64 x 32] (+)= A[64 x 32, registers] * B[32 x 32, shared memory descriptor], e4m3 -> fp32.
-__device__ __forceinline__ void wgmma_m64n32k32_e4m3_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %21, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-        "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
-        : "memory");
 }
 
 }  // namespace b2p

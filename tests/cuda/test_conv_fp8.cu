@@ -96,7 +96,7 @@ static void launch(const Fp8Conv& c, const __nv_bfloat16* d_in, __nv_bfloat16* d
         a.out_f32[g] = d_f32 ? d_f32[g] : nullptr;
         a.f32_ch[g] = d_f32 ? f32_ch[g] : 0;
     }
-    a.chunk = 1; a.fp8 = 1; a.pdl = c.pdl;
+    a.fmt = TcFormat::kFp8; a.pdl = c.pdl;
     a.amax_in[0] = d_amax_in; a.amax_out = d_amax_out; a.w_exp = d_wexp; a.ea_out = d_ea;
     a.ext = c.ext;
     while ((a.H << a.ext_shift) < c.H) ++a.ext_shift;

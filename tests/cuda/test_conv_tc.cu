@@ -45,7 +45,7 @@ static double bf16_ulp(double v) {
 struct Case {
     const char* name;
     int n, H, W, ks, groups, cin_g, in_stride_g, cout_g, n_tile, relu, pool, head;
-    int split;          // bf16x3: hi + lo planes, three MMA terms (run K-chunked)
+    int split;          // 1: run in bf16x3 only (hi + lo planes, three MMA terms, K-chunked); 0: see main
     int in_base, in_c;  // first input channel of group 0 / channels per input pixel (0: cin_g or cin_g * groups)
     int out_off, out_c; // first output channel of group 0 / channels per output pixel (0: groups * cout_g)
     int pdl;            // the input is written by a preceding launch (identity 1x1 conv) and this one is PDL-chained to it
@@ -55,7 +55,9 @@ struct Case {
 // r = sum(a * w) + b and S = sum|a * w| + |b| in double, e = 2^-22 * c * S with c from the kernel's accumulation
 // structure, accept R(f(r - e)) <= got <= R(f(r + e)) (f = ReLU then 2x2 max, R = bf16 round-to-nearest-even).
 // head: out_ch_off {0,40}, store {40,24}, f32 {38,19}; cout_g is the padded per-group Cout (n_tile).
-static int run_case(const Case& c, int num_sms, int chunk = 0) {
+static int run_case(const Case& c, int num_sms, TcFormat fmt) {
+    const bool split = tc_planes(fmt) == 2;
+    const char* fmt_name = split ? "bf16x3" : "bf16";
     const int taps = c.ks * c.ks, pad = c.ks / 2;
     const int cin_blocks = c.cin_g / 64;
     const int in_c = c.in_c ? c.in_c : ((c.in_stride_g == 0) ? c.cin_g : c.cin_g * c.groups);
@@ -63,7 +65,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
     const int rows = c.groups * c.cout_g;
     const int Ho = c.pool ? c.H / 2 : c.H, Wo = c.pool ? c.W / 2 : c.W;
     const int out_c = c.head ? 64 : (c.out_c ? c.out_c : rows);
-    const int nterms = c.split ? 3 : 1;
+    const int nterms = split ? 3 : 1;
 
     // activations: hi = bf16(x) (lo = bf16(x - hi) in split mode); weights likewise
     std::vector<float> in((size_t)c.n * c.H * c.W * in_c), in_lo(in.size(), 0.f), w((size_t)taps * rows * c.cin_g),
@@ -71,13 +73,13 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
     for (size_t i = 0; i < in.size(); ++i) {
         const float x = frand();
         in[i] = bf16r(x);
-        if (c.split) in_lo[i] = bf16r(x - in[i]);
+        if (split) in_lo[i] = bf16r(x - in[i]);
     }
     const float ws = 1.0f / std::sqrt((float)(taps * c.cin_g));
     for (size_t i = 0; i < w.size(); ++i) {
         const float x = frand() * 2.f * ws * 1.7f;
         w[i] = bf16r(x);
-        if (c.split) w_lo[i] = bf16r(x - w[i]);
+        if (split) w_lo[i] = bf16r(x - w[i]);
     }
     for (auto& v : bias) v = frand() * 0.2f;
     const int valid[2] = {c.head ? 38 : c.cout_g, c.head ? 19 : c.cout_g};
@@ -110,7 +112,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
     } else {
         CK(cudaMemcpy(d_in, in_h.data(), in_h.size() * 2, cudaMemcpyHostToDevice));
     }
-    if (c.split) {
+    if (split) {
         CK(cudaMalloc(&d_in_lo, in_h.size() * 2));
         CK(cudaMalloc(&d_out_lo, out_elems * 2));
         CK(cudaMemcpy(d_in_lo, in_lo_h.data(), in_h.size() * 2, cudaMemcpyHostToDevice));
@@ -133,8 +135,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
         a.out_f32[g] = d_f32[g];
         a.f32_ch[g] = c.head ? valid[g] : 0;
     }
-    a.chunk = chunk;
-    a.split = c.split;
+    a.fmt = fmt;
     a.out_lo = d_out_lo;
     a.pdl = c.pdl;
     CK(conv_tc_make_maps(a, d_in, in_c, d_w, d_in_lo));
@@ -155,7 +156,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
     CK(conv_tc_launch(a, num_sms, 0));
     cudaError_t e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
-        printf("case %-34s chunk=%d : KERNEL FAILED: %s\n", c.name, chunk, cudaGetErrorString(e));
+        printf("case %-34s %-6s : KERNEL FAILED: %s\n", c.name, fmt_name, cudaGetErrorString(e));
         return 100;
     }
 #ifdef B2P_CONV_TIMELINE
@@ -165,7 +166,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
         const char* names[10] = {"entry", "prologue done", "patch cb0", "patch cb1", "first weights", "MMAs issued", "acc complete",
                                  "tile stored", "before final sync", "exit"};
         for (int cta = 0; cta < 4; ++cta) {
-            printf("  timeline %s chunk=%d CTA %d (clk since entry):", c.name, chunk, cta);
+            printf("  timeline %s %s CTA %d (clk since entry):", c.name, fmt_name, cta);
             for (int sl = 1; sl < 10; ++sl) {
                 const unsigned long long v = tl[cta * kTlSlots + sl], v0 = tl[cta * kTlSlots];
                 printf(" %s=%lld", names[sl], v ? (long long)(v - v0) : -1LL);
@@ -174,9 +175,9 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
         }
     }
 #endif
-    std::vector<__nv_bfloat16> out_h(out_elems), out_lo_h(c.split ? out_elems : 0);
+    std::vector<__nv_bfloat16> out_h(out_elems), out_lo_h(split ? out_elems : 0);
     CK(cudaMemcpy(out_h.data(), d_out, out_elems * 2, cudaMemcpyDeviceToHost));
-    if (c.split) CK(cudaMemcpy(out_lo_h.data(), d_out_lo, out_elems * 2, cudaMemcpyDeviceToHost));
+    if (split) CK(cudaMemcpy(out_lo_h.data(), d_out_lo, out_elems * 2, cudaMemcpyDeviceToHost));
     std::vector<float> f32_h[2];
     if (c.head)
         for (int g = 0; g < 2; ++g) {
@@ -204,7 +205,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
                                     const double ah = in[ib + k], al = in_lo[ib + k], wh = w[wb + k], wl = w_lo[wb + k];
                                     acc += ah * wh;
                                     sa += std::fabs(ah * wh);
-                                    if (c.split) {      // A_hi W_lo + A_lo W_hi
+                                    if (split) {      // A_hi W_lo + A_lo W_hi
                                         acc += ah * wl + al * wh;
                                         sa += std::fabs(ah * wl) + std::fabs(al * wh);
                                     }
@@ -216,7 +217,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
                     }
     // e = 2^-22 * coef * S (oracle/conv_check.py bound_coef)
     double coef;
-    if (chunk) coef = c.ks == 7 ? 28 + 16 + nterms * cin_blocks * 7 : taps * 4 + 16 + nterms * cin_blocks;
+    if (tc_chunked(fmt)) coef = c.ks == 7 ? 28 + 16 + nterms * cin_blocks * 7 : taps * 4 + 16 + nterms * cin_blocks;
     else coef = std::ceil(nterms * taps * c.cin_g / 16.0) + 16;
     const double U = std::ldexp(1.0, -22);
     auto fpos = [&](double v) { return c.relu && v < 0 ? 0.0 : v; };
@@ -247,7 +248,7 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
                         const double got = __bfloat162float(out_h[oi]);
                         bool ok;
                         double dist;
-                        if (c.split) {
+                        if (split) {
                             const double lo = __bfloat162float(out_lo_h[oi]), wsl = std::ldexp(std::fabs(fr), -16);
                             ok = got + lo >= flo - wsl && got + lo <= fhi + wsl && std::fabs(lo) <= bf16_ulp(got) / 2;
                             dist = std::max(0.0, std::fabs(got + lo - fr) - wsl);
@@ -255,13 +256,13 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
                             ok = got >= bf16_rne(flo) && got <= bf16_rne(fhi);
                             dist = std::max(0.0, std::fabs(got - fr) - bf16_ulp(got) / 2);
                         }
-                        if (c.head && co >= valid[g]) ok = got == 0 && (!c.split || __bfloat162float(out_lo_h[oi]) == 0);
+                        if (c.head && co >= valid[g]) ok = got == 0 && (!split || __bfloat162float(out_lo_h[oi]) == 0);
                         ++checked;
                         if (ef > 0) max_ratio = std::max(max_ratio, dist / ef);
                         if (!ok) {
                             if (printed++ < 5)
                                 printf("  bad: n=%d y=%d x=%d ch=%d got %.9g interval [%.9g, %.9g]\n", n, yo, xo, oc, got,
-                                       c.split ? flo : bf16_rne(flo), c.split ? fhi : bf16_rne(fhi));
+                                       split ? flo : bf16_rne(flo), split ? fhi : bf16_rne(fhi));
                             ++bad;
                         }
                         if (c.head && co < valid[g]) {
@@ -280,11 +281,11 @@ static int run_case(const Case& c, int num_sms, int chunk = 0) {
                     const size_t oi = ((size_t)(n * Ho + yo) * Wo + xo) * out_c + oc;
                     uint16_t bits, lbits = 0xFFFF;
                     memcpy(&bits, &out_h[oi], 2);
-                    if (c.split) memcpy(&lbits, &out_lo_h[oi], 2);
+                    if (split) memcpy(&lbits, &out_lo_h[oi], 2);
                     if (bits != 0xFFFF || lbits != 0xFFFF) ++bad;
                 }
             }
-    printf("case %-34s chunk=%d : %ld outputs, max|v-r|/e bf16 %.3f f32 %.3f  bad=%ld  %s\n", c.name, chunk, checked,
+    printf("case %-34s %-6s : %ld outputs, max|v-r|/e bf16 %.3f f32 %.3f  bad=%ld  %s\n", c.name, fmt_name, checked,
            max_ratio, max_ratio32, bad, bad == 0 ? "OK" : "MISMATCH");
     cudaFree(d_in); cudaFree(d_w); cudaFree(d_bias); cudaFree(d_out);
     if (d_in_lo) cudaFree(d_in_lo);
@@ -381,8 +382,10 @@ int main(int argc, char** argv) {
     };
     int fails = 0;
     for (const Case& c : cases) {
-        for (int chunk = c.split; chunk <= (c.n_tile <= 64 ? 1 : 0); ++chunk) {    // K-chunked accumulation (N <= 64)
-            int r = run_case(c, sms, chunk);
+        // bf16, and for N <= 64 (the n-tiles of the K-chunked kernel) bf16x3 as well; split cases in bf16x3 only
+        const TcFormat fmts[2] = {TcFormat::kBf16, TcFormat::kBf16x3};
+        for (int f = c.split; f <= (c.n_tile <= 64 ? 1 : 0); ++f) {
+            int r = run_case(c, sms, fmts[f]);
             if (r >= 100) {   // sticky CUDA error: the context is gone
                 printf("aborting after kernel failure\n");
                 return 3;

@@ -1,5 +1,5 @@
 """Reference rules of the fp8 (e4m3) mode (DESIGN.md §2.3), written independently of csrc/fp8_core.h: the scale exponent
-rule, e4m3 quantisation (torch.float8_e4m3fn) and the per-launch error bound of conv_tc_fp8_kernel.
+rule, e4m3 quantisation (torch.float8_e4m3fn) and the per-launch error bound of conv_tc_kernel in fp8.
 
 A launch's e4m3 operands qa = e4m3(a * 2^ea), qw = e4m3(w * 2^ew) have exact products in fp32.  Each tap runs two k32
 wgmmas into a fresh accumulator (the second adds to the first) and the tap's partial is added to an fp32 sum (RN).
@@ -69,7 +69,7 @@ def e4m3_all_bf16_in_range():
 
 
 def emulate(x64, ea, qw, ew, b, ks, acc_bits=None, mutate=None):
-    """Host emulation of conv_tc_fp8_kernel for one image (x64: float64 [1, C, H, W] bf16 values; qw: e4m3 values of
+    """Host emulation of conv_tc_kernel in fp8 for one image (x64: float64 [1, C, H, W] bf16 values; qw: e4m3 values of
     w * 2^ew [O, C, ks, ks]): exact e4m3 products; per (channel block, tap) two k32 steps into a fresh accumulator that
     keeps `acc_bits` bits (ACC_BITS) relative to the largest of its terms and the incoming value, truncating each term
     toward zero (the characterised behaviour, DESIGN.md §3); the tap partials summed in fp32 (RN) in the kernel's

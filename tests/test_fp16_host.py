@@ -188,8 +188,8 @@ def _ptxas(src):
     return re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'(.*?)(?=Compiling entry|\Z)", r.stdout, re.S)
 
 
-@pytest.mark.parametrize("src,name,count", [("conv_tc.cu", "conv_tc_f16_kernel", 8),
-                                            ("conv_misc.cu", "conv_first_mma_kernelILi.ELb0ELb1E", 5)])   # kF16 = true
+@pytest.mark.parametrize("src,name,count", [("conv_tc.cu", "conv_tc_kernelILNS_8TcFormatE3E", 8),      # TcFormat::kFp16
+                                            ("conv_misc.cu", "conv_first_mma_kernelILi.ELNS_8TcFormatE3E", 5)])
 def test_fp16_kernels_do_not_spill(built, src, name, count):
     bodies = [(fn, body) for fn, body in _ptxas(src) if re.search(name, fn)]
     assert len(bodies) == count

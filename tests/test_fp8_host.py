@@ -98,8 +98,8 @@ def _ptxas(src):
     return re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'(.*?)(?=Compiling entry|\Z)", r.stdout, re.S)
 
 
-@pytest.mark.parametrize("src,name,count", [("conv_tc.cu", "conv_tc_fp8_kernel", 6),
-                                            ("conv_misc.cu", "conv_first_mma_kernelILi.ELb1E", 5)])   # kAmax = true
+@pytest.mark.parametrize("src,name,count", [("conv_tc.cu", "conv_tc_kernelILNS_8TcFormatE2E", 6),      # TcFormat::kFp8
+                                            ("conv_misc.cu", "conv_first_mma_kernelILi.ELNS_8TcFormatE2E", 5)])
 def test_fp8_kernels_do_not_spill(built, src, name, count):
     bodies = [(fn, body) for fn, body in _ptxas(src) if re.search(name, fn)]
     assert len(bodies) == count
@@ -134,7 +134,7 @@ def _ratio(got, r, e):
 
 @pytest.mark.parametrize("ks,cin", [(1, 64), (3, 128), (7, 128), (7, 192)])
 def test_checker_accepts_the_emulated_kernel_and_rejects_mutations(ks, cin):
-    """The float64 interval of tests/fp8_check.py accepts the host emulation of conv_tc_fp8_kernel at the characterised
+    """The float64 interval of tests/fp8_check.py accepts the host emulation of the fp8 conv_tc_kernel at the characterised
     accumulator precision (ACC_BITS, measured by build/test_conv_fp8 acc) and rejects a descale by ea + 1, one
     channel's ew off by one, a dropped k32 slice, a tap read one pixel off and a scaled bias at every shape here.  One
     mutation stays below the bound and the test states it: weights quantised with one scale per tensor.  It changes only

@@ -41,8 +41,8 @@ def _forward(net, x, mode):
 def test_wgmma_conv_kernel_cases(built):
     """Standalone harness (tests/cuda/test_conv_tc.cu): 18 conv configurations (1x1/3x3/7x7, groups, fused pool, padded
     heads, n-tiles of 32/48/64/128, more work items than SMs, bf16x3 in both chunk styles, channel slices of wider
-    buffers, a PDL-chained launch), each N <= 64 one also K-chunked, against a plain CPU loop with the interval rule of
-    oracle/conv_check.py."""
+    buffers, a PDL-chained launch), each N <= 64 one also in bf16x3 (both planes, K-chunked), against a plain CPU loop
+    with the interval rule of oracle/conv_check.py."""
     r = subprocess.run([os.path.join(ROOT, "build", "test_conv_tc")], stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
                        text=True, timeout=600)
     print(r.stdout)
