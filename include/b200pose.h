@@ -38,7 +38,7 @@ typedef struct b200pose_net b200pose_net;
                                       weights, 3 MMA terms per K block (A_hi*W_hi + A_hi*W_lo + A_lo*W_hi); measured
                                       1.4e-3 max-abs @368x368 (bf16: 7e-2, fp32 mode: 3e-5) - the tensor core's own fp32
                                       accumulation is the floor, see DESIGN.md 2.3                                   */
-#define B200POSE_MODE_FP8 3        /* fp8 tensor-core mode: the 51 wgmma convolutions run on e4m3 operands, activations
+#define B200POSE_MODE_FP8 3        /* fp8 tensor-core mode: the wgmma convolutions run on e4m3 operands, activations
                                       scaled by 2^ea per (launch, image) from the max |bf16| their writers stored, weights
                                       by 2^ew per output channel; activations stay bf16 in memory and conv1_1 runs as in
                                       bf16 mode (DESIGN.md 2.3).  Before this mode existed, 3 ran as bf16.             */
@@ -59,10 +59,13 @@ int b200pose_net_set_tensor(b200pose_net* net, int index, const float* host_data
 int b200pose_net_finalize(b200pose_net* net);
 /* forward: input fp32 NCHW [n,3,H,W] (H, W multiples of 8); outputs[12] fp32 NCHW in saved_for_loss order
  * [paf1, heat1, ..., paf6, heat6] (paf [n,38,H/8,W/8], heat [n,19,H/8,W/8]); entries may be NULL to skip the
- * copy-out.  *_on_device: 0 = host pointers (copies are issued on `cuda_stream` and synchronised before return),
- * 1 = device pointers (asynchronous on `cuda_stream`).  cuda_stream: a cudaStream_t cast to void* (NULL = default).
- * On a real stream (not the legacy default stream, not one that is being captured) the 52 launches of a SMALL-batch
- * (launch-bound: up to 4 frames of 368x368) bf16 / bf16x3 forward pass are captured at the SECOND use of a (shape, mode, input pointer) into a CUDA graph and replayed afterwards
+ * copy-out.  With k stages (b200pose_net_set_stages) only entries 0 .. 2k-1 are written; the others must be NULL (a
+ * non-NULL one is an error naming it).  *_on_device: 0 = host pointers (copies are issued on `cuda_stream` and
+ * synchronised before return), 1 = device pointers (asynchronous on `cuda_stream`).  cuda_stream: a cudaStream_t cast
+ * to void* (NULL = default).
+ * On a real stream (not the legacy default stream, not one that is being captured) the launches (52 with six stages)
+ * of a SMALL-batch (launch-bound: up to 4 frames of 368x368) tensor-core forward pass are captured at the SECOND use of
+ * a (shape, mode, stages, input pointer) into a CUDA graph and replayed afterwards
  * (a caller that passes a fresh pointer every time never pays a capture); the input buffer's
  * CONTENTS may change between calls, results are those of plain launches (tests/test_gpu.py:
  * test_graph_replay_equals_plain_launches).  B200POSE_GRAPH=0 disables the capture. */
@@ -81,6 +84,12 @@ int b200pose_net_forward_u8(b200pose_net* net, const unsigned char* images, int 
 #define B200POSE_PRE_INCEPTION 3   /* BGR -> RGB, x/128 - 1                         */
 #define B200POSE_PRE_SSD 4         /* x - (123, 117, 104) on (B, G, R)              */
 int b200pose_net_set_preprocess(b200pose_net* net, int preprocess);
+/* Refinement stages every later forward of the net runs (every b200pose_net_forward*, b200pose_infer* and the flip,
+ * raw, ragged and multi-scale variants): the trunk, stage 1 and stages 2 .. `stages`, 1 <= stages <= 6, default 6.  The
+ * stage count is part of the plan and CUDA-graph keys; the fused entry points post-process (flip-merge, resize and
+ * average) stage `stages`'s maps, and b200pose_net_last_maps returns them.  Each stage's maps are those a six-stage
+ * forward gives for that stage, bit for bit.  Any other value is an error and leaves the setting as it was. */
+int b200pose_net_set_stages(b200pose_net* net, int stages);
 /* Ragged batch (DESIGN.md 1): n already cropped uint8 HWC BGR frames of different sizes, packed back to back (frame i is
  * hw[2i] x hw[2i+1] x 3 bytes, both multiples of 8; n <= 1024).  The batch runs on the canvas Hc x Wc = (max H_i, max W_i):
  * outputs[12] as b200pose_net_forward's at canvas size [n, C, Hc/8, Wc/8]; inside its own (H_i/8) x (W_i/8) each frame's
@@ -88,11 +97,12 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess);
  * graphs of small batches) are keyed on (n, Hc, Wc, mode): a new mix of frames on the same canvas rebuilds nothing. */
 int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frames, int on_device, int n, const int* hw,
                                    int mode, float* const* outputs, int outputs_on_device, void* cuda_stream);
-/* Measurement hook: re-runs the launch list of the last bf16 forward (conv1_1 + 51 tensor-core launches) with a CUDA
- * event pair around every launch; fills per-launch milliseconds and ALGORITHMIC FLOPs (2 x MACs of the unpadded
- * convolution).  Returns the number of launches, < 0 on error. */
+/* Measurement hook: re-runs the launch list of the last tensor-core forward (conv1_1 + 16 + 7 (k - 1) tensor-core
+ * launches for k stages: 51 with six) with a CUDA event pair around every launch; fills per-launch milliseconds and
+ * ALGORITHMIC FLOPs (2 x MACs of the unpadded convolution).  Returns the number of launches, < 0 on error. */
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream);
-/* Test hooks of the last bf16 / bf16x3 / fp8 / fp16 forward's launch list (launch 0 = conv1_1, 1 .. 51 = the tensor-core launches);
+/* Test hooks of the last bf16 / bf16x3 / fp8 / fp16 forward's launch list (launch 0 = conv1_1, 1 .. 16 + 7 (k - 1) = the
+ * tensor-core launches of its k stages, 1 .. 51 with six);
  * they let a test check one launch against a reference computed from that launch's real inputs.
  *   b200pose_net_debug_run    : re-runs the first `launches` launches on the last forward's input (plain launches with
  *                               the plan's own arguments, PDL included, no graph), then synchronises the stream.
@@ -106,14 +116,15 @@ int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, v
  *     Returns the number of fields written.
  *   b200pose_net_debug_read   : copies images [img0, img0 + count) of one buffer to host memory: ids 0 .. 13 are the
  *     bf16 NHWC activation buffers t1, t2, t3, t4, t5a, t5b, t6, t7, t8, t9, cat, bra, brb, br512 (lo_plane = 1: their
- *     residual planes, bf16x3 only), 14 .. 25 the fp32 NCHW stage maps in saved_for_loss order.  The activation
+ *     residual planes, bf16x3 only), 14 .. 25 the fp32 NCHW stage maps in saved_for_loss order (those of the stages the
+ *     forward ran).  The activation
  *     buffers hold bfloat16 bits, or binary16 bits after an fp16 forward (debug_launch field 27). */
 #define B200POSE_DEBUG_LAUNCH_FIELDS 27
 #define B200POSE_DEBUG_LAUNCH_FORMAT 27
 int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream);
 int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap);
 int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, int count, void* host, long bytes);
-/* fp8 test hook: for tensor-core launch `launch` (1 .. 51) of the last fp8 forward, the activation scale exponent ea each
+/* fp8 test hook: for tensor-core launch `launch` (1 .. 51 with six stages) of the last fp8 forward, the activation scale exponent ea each
  * of its n_img images used, as the kernel recorded it (act_exp[n_img], n_img = the forward's batch), and the weight
  * exponent ew of each packed output row (w_exp[cap], rows = groups * n_tiles * n_tile; pad rows 0).  Returns the number
  * of rows, < 0 on error. */
@@ -122,7 +133,8 @@ int b200pose_net_debug_fp8(b200pose_net* net, int launch, int* act_exp, int n_im
  * (n = the forward's batch; flip: frames, then mirrors) stored a value beyond binary16's range (+-inf or NaN) in any
  * layer, else 0.  Forwards of the other modes flag nothing.  Returns the number of flagged images, < 0 on error. */
 int b200pose_net_overflow(b200pose_net* net, int* flags, int n, void* cuda_stream);
-/* Device pointers of the last forward's stage-6 maps (NCHW fp32), valid until the next forward. */
+/* Device pointers of the last forward's final maps (NCHW fp32): those of its last stage (stage 6 by default), valid
+ * until the next forward. */
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w);
 
 /* ------------------------------------------------------------------------------------------------------------

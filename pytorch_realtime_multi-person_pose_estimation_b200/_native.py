@@ -29,6 +29,7 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_net_forward": ([vp, vp, ci, ci, ci, ci, ci, ctypes.POINTER(vp), ci, vp], ci),
     "b200pose_net_forward_u8": ([vp, vp, ci, ci, ci, ci, ci, ctypes.POINTER(vp), ci, vp], ci),
     "b200pose_net_set_preprocess": ([vp, ci], ci),
+    "b200pose_net_set_stages": ([vp, ci], ci),
     "b200pose_net_forward_ragged_u8": ([vp, vp, ci, ci, vp, ci, ctypes.POINTER(vp), ci, vp], ci),
     "b200pose_net_profile": ([vp, vp, vp, ci, vp], ci),
     "b200pose_net_debug_run": ([vp, ci, vp], ci),

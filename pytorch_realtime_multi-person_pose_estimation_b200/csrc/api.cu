@@ -60,6 +60,7 @@ const ConvSpec kTrunk[12] = {{3, 64, 3},    {64, 64, 3},   {64, 128, 3},  {128, 
 const bool kPoolAfter[12] = {false, true, false, true, false, false, false, true, false, false, false, false};
 constexpr int kPaf = 38, kHeat = 19, kFeat = 128, kCat = kPaf + kHeat + kFeat;
 
+constexpr int kStages = 6;     // refinement stages of the network; a forward may stop after any of them
 int stage_num_layers(int stage) { return stage == 1 ? 5 : 7; }
 ConvSpec stage_layer(int stage, int branch, int li) {
     const int outc = branch == 0 ? kPaf : kHeat;
@@ -206,10 +207,12 @@ struct PlanLaunch {
 // Device addresses a plan's tensor maps and arguments point into: activation buffers, residual planes, stage maps.
 using PlanBuffers = std::array<const void*, 2 * kNumAct + 12 + 2>;    // + the format's aux table, the fp8 exponent table
 
-// The launch list of one (n, H, W, format) key, valid while `buffers` are still the net's.
+// The launch list of one (n, H, W, format, stages) key, valid while `buffers` are still the net's: the trunk and the
+// launches of stages 1 .. stages.
 struct Plan {
     int n, H, W;
     TcFormat fmt;
+    int stages;
     std::vector<PlanLaunch> launches;
     PlanBuffers buffers;
 };
@@ -219,6 +222,7 @@ struct LastForward {
     int n = 0, H = 0, W = 0;
     bool fp32 = false;           // the fp32 path ran, else the tensor-core path in format fmt
     TcFormat fmt = TcFormat::kBf16;
+    int stages = kStages;        // stages run; the final maps are stage `stages`'s (out_f32[2 stages - 2], [2 stages - 1])
     const void* in = nullptr;    // device input
     int in_u8 = 0;               // normalisation of a uint8 input fused into conv1_1 (0: fp32 input)
     const int* ext = nullptr;    // extents table of a ragged forward, null: uniform
@@ -236,13 +240,14 @@ struct b200pose_net {
     // tensor-core layers: trunk 1..11 -> tc[0..10]; stage 1: tc[11..15]; stage t>=2: tc[16 + (t-2)*7 + li]
     std::vector<TcLayer> tc;
     // Plans of the last 32 keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not re-encode
-    // 51 tensor maps and synchronise the stream.  `plan` is the one the last tensor-core forward selected.
+    // up to 51 tensor maps and synchronise the stream.  `plan` is the one the last tensor-core forward selected.
     std::list<Plan> plans;
     const Plan* plan = nullptr;
-    // The 52 launches of a forward pass are captured at the second use of a (shape, format, input pointer) into a CUDA graph and replayed
-    // (B200POSE_GRAPH=0: plain launches).  Graphs embed the tensor maps, i.e. buffer addresses: every plan build drops them.
-    // Capture needs a real stream: calls on the legacy default stream (0) launch directly.
-    using GraphKey = std::tuple<int, int, int, TcFormat, int, bool, const void*>;   // n, H, W, format, in_u8, ragged, input
+    // The launches of a forward pass (52 with six stages) are captured at the second use of a (shape, format, stages,
+    // input pointer) into a CUDA graph and replayed (B200POSE_GRAPH=0: plain launches).  Graphs embed the tensor maps,
+    // i.e. buffer addresses: every plan build drops them.  Capture needs a real stream: calls on the legacy default stream
+    // (0) launch directly.
+    using GraphKey = std::tuple<int, int, int, TcFormat, int, int, bool, const void*>;   // n, H, W, format, stages, in_u8, ragged, input
     bool use_graph = true;
     std::map<GraphKey, cudaGraphExec_t> graphs;
     std::set<GraphKey> graph_seen;    // a key is captured at its SECOND use: callers that pass a fresh pointer every time never pay a capture
@@ -254,6 +259,7 @@ struct b200pose_net {
     LastForward last;
     DevBuf<unsigned char> in_stage_u8;
     int preprocess = 1;                // normalisation fused into the uint8 entry points (preprocess_core.h; 1 = rtpose)
+    int stages = kStages;              // refinement stages every later forward runs (b200pose_net_set_stages)
     DevBuf<unsigned char> raw_stage;   // raw (un-resized) frames of b200pose_*crop* / b200pose_infer_raw_u8
     // Ragged batches (DESIGN.md §1): the extents table [H_0, W_0, H_1, W_1, ...] every kernel of a ragged forward reads.
     // Allocated once for kMaxRagged images and never moved, so that plans and captured graphs stay valid across mixes;
@@ -310,6 +316,10 @@ struct b200pose_post {
 };
 
 namespace {
+
+// The final maps of the last forward: the PAF and heatmap of its last stage.
+const float* last_paf(const b200pose_net* net) { return net->out_f32[2 * net->last.stages - 2].p; }
+const float* last_heat(const b200pose_net* net) { return net->out_f32[2 * net->last.stages - 1].p; }
 
 // Calls row(g, o, r, w) for output channel o of every group g of layer L (packed row r = g * cout_pad + o), w its fp32
 // weights in packed order [tap][cin_pad]: input channels at their physical channel of the buffer the layer reads (cat_phys
@@ -531,7 +541,7 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
         CU(cudaMemsetAsync(bufs[CAT].p, 0, px / 64 * kActC[CAT] * 2, st));
     }
     for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * (i % 2 == 0 ? kPaf : kHeat)));
-    if (tc_aux(p.fmt) == TcAux::kAmax) {
+    if (tc_aux(p.fmt) == TcAux::kAmax) {     // rows for six stages whatever p.stages: plans of every stage count share them
         CU(net->amax.ensure((size_t)(1 + 51) * p.n));
         CU(net->ea.ensure((size_t)(1 + 51) * p.n));
     }
@@ -556,7 +566,7 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
     int k = 0;
     for (const Wiring& wr : kTrunkWiring)
         if (add(net->tc[k++], wr, 0)) return 1;
-    for (int s = 1; s <= 6; ++s)
+    for (int s = 1; s <= p.stages; ++s)
         for (int li = 0; li < stage_num_layers(s); ++li)
             if (add(net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], s - 1)) return 1;
     p.buffers = plan_buffers(net, p.fmt);
@@ -569,22 +579,23 @@ void drop_graphs(b200pose_net* net) {
     net->graph_seen.clear();
 }
 
-// Points net->plan at the plan of (n, H, W, fmt): a kept one whose buffers are still the net's, or a new one (the
-// oldest of 32 is dropped).  A build may move the buffers the captured graphs point into: it synchronises the stream
-// and drops the graphs first.
-int select_plan(b200pose_net* net, int n, int H, int W, TcFormat fmt, cudaStream_t st) {
+// Points net->plan at the plan of (n, H, W, fmt, stages): a kept one whose buffers are still the net's, or a new one
+// (the oldest of 32 is dropped).  A build may move the buffers the captured graphs point into: it synchronises the
+// stream and drops the graphs first.
+int select_plan(b200pose_net* net, int n, int H, int W, TcFormat fmt, int stages, cudaStream_t st) {
     const PlanBuffers bufs = plan_buffers(net, fmt);
+    auto same_key = [&](const Plan& p) { return p.n == n && p.H == H && p.W == W && p.fmt == fmt && p.stages == stages; };
     for (const Plan& p : net->plans)
-        if (p.n == n && p.H == H && p.W == W && p.fmt == fmt && p.buffers == bufs) {
+        if (same_key(p) && p.buffers == bufs) {
             net->plan = &p;
             return 0;
         }
     CU(cudaStreamSynchronize(st));
     drop_graphs(net);
     net->plan = nullptr;
-    net->plans.remove_if([&](const Plan& p) { return p.n == n && p.H == H && p.W == W && p.fmt == fmt; });
+    net->plans.remove_if(same_key);
     if (net->plans.size() >= 32) net->plans.pop_front();
-    net->plans.push_back(Plan{n, H, W, fmt, {}, {}});
+    net->plans.push_back(Plan{n, H, W, fmt, stages, {}, {}});
     if (build_plan_tc(net, net->plans.back(), st)) {
         net->plans.pop_back();
         return 1;
@@ -620,15 +631,15 @@ int launch_forward_tc(const b200pose_net* net, const void* d_in, int in_u8, cons
     return 0;
 }
 
-int forward_tc(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, TcFormat fmt, cudaStream_t st,
-               const int* ext) {
-    if (select_plan(net, n, H, W, fmt, st)) return 1;
+int forward_tc(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int W, TcFormat fmt, int stages,
+               cudaStream_t st, const int* ext) {
+    if (select_plan(net, n, H, W, fmt, stages, st)) return 1;
     const int launches = 1 + (int)net->plan->launches.size();
     cudaGraphExec_t exec = nullptr;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     if (net->use_graph && small_plan(net, n, H, W) && st != nullptr && cudaStreamIsCapturing(st, &cap) == cudaSuccess &&
         cap == cudaStreamCaptureStatusNone) {
-        const b200pose_net::GraphKey key{n, H, W, fmt, in_u8, ext != nullptr, d_in};
+        const b200pose_net::GraphKey key{n, H, W, fmt, stages, in_u8, ext != nullptr, d_in};
         auto it = net->graphs.find(key);
         if (it != net->graphs.end()) {
             exec = it->second;
@@ -659,7 +670,8 @@ int forward_tc(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int
     return 0;
 }
 
-int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, cudaStream_t st, const int* ext) {
+int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int stages, cudaStream_t st,
+                 const int* ext) {
     const size_t px1 = (size_t)n * H * W;
     const int h = H / 8, w = W / 8;
     const size_t px8 = (size_t)n * h * w;
@@ -701,7 +713,7 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, cuda
             std::swap(ping, pong);
         }
     }
-    for (int s = 1; s <= 6; ++s)
+    for (int s = 1; s <= stages; ++s)
         for (int b = 0; b < 2; ++b) {
             const int nl = stage_num_layers(s);
             const float* in = net->f_cat.p;
@@ -717,7 +729,7 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, cuda
                 if (conv(conv_index(s, b, li), in, in_cs, in_off, dst, sp.cout, 0, h, w, lastl ? 0 : 1, nchw)) return 1;
                 in = dst; in_cs = sp.cout; in_off = 0;
             }
-            if (b == 1 && s < 6) {
+            if (b == 1 && s < stages) {
                 CU(nchw_to_nhwc_f32_launch(net->out_f32[2 * (s - 1)].p, net->f_cat.p, n, kPaf, h, w, kCat, 0, st));
                 CU(nchw_to_nhwc_f32_launch(net->out_f32[2 * (s - 1) + 1].p, net->f_cat.p, n, kHeat, h, w, kCat, kPaf, st));
                 g_launches += 2;
@@ -834,12 +846,23 @@ int b200pose_net_finalize(b200pose_net* net) {
     return 0;
 }
 
+// Entries of outputs[12] for stages the net does not run must be NULL: a caller must not read a map no stage wrote as if
+// it were fresh.
+static int check_outputs(const b200pose_net* net, float* const* outputs) {
+    for (int i = 2 * net->stages; outputs && i < 12; ++i)
+        if (outputs[i])
+            return fail("outputs[%d] must be NULL: the net runs %d stage(s), stage %d does not run", i, net->stages, i / 2 + 1);
+    return 0;
+}
+
 // ext: device extents table of a ragged batch (DESIGN.md §1), or null
 static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int input_on_device, int n, int H, int W,
                             int mode, float* const* outputs, int outputs_on_device, cudaStream_t st, bool sync_host,
                             const int* ext = nullptr) {
     if (!net || !net->finalized) return fail("net not finalized");
     if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
+    if (int rc = check_outputs(net, outputs)) return rc;
+    const int stages = net->stages;
     CU(cudaSetDevice(net->device));
     const void* d_in = input;
     const size_t elems = (size_t)n * 3 * H * W;
@@ -861,20 +884,20 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
             CU(net->f_u8.ensure(elems));
             CU(u8hwc_to_f32nchw_launch(static_cast<const unsigned char*>(d_in), net->f_u8.p, n, H, W, net->preprocess, ext, st));
             ++g_launches;
-            rc = forward_fp32(net, net->f_u8.p, n, H, W, st, ext);
-        } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, st, ext);
+            rc = forward_fp32(net, net->f_u8.p, n, H, W, stages, st, ext);
+        } else rc = forward_fp32(net, static_cast<const float*>(d_in), n, H, W, stages, st, ext);
     } else {
         if (mode == B200POSE_MODE_BF16X3) fmt = TcFormat::kBf16x3;
         else if (mode == B200POSE_MODE_FP8) fmt = TcFormat::kFp8;
         else if (mode == B200POSE_MODE_FP16) fmt = TcFormat::kFp16;     // every other mode runs bf16
         first_u8 = in_u8 ? net->preprocess : 0;
-        rc = forward_tc(net, d_in, first_u8, n, H, W, fmt, st, ext);
+        rc = forward_tc(net, d_in, first_u8, n, H, W, fmt, stages, st, ext);
     }
     if (rc) return rc;
-    net->last = LastForward{n, H, W, mode == B200POSE_MODE_FP32, fmt, d_in, first_u8, ext};
+    net->last = LastForward{n, H, W, mode == B200POSE_MODE_FP32, fmt, stages, d_in, first_u8, ext};
     if (outputs) {
         const size_t px8 = (size_t)n * (H / 8) * (W / 8);
-        for (int i = 0; i < 12; ++i)
+        for (int i = 0; i < 2 * stages; ++i)
             if (outputs[i])
                 CU(cudaMemcpyAsync(outputs[i], net->out_f32[i].p, px8 * (i % 2 == 0 ? kPaf : kHeat) * 4,
                                    outputs_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
@@ -968,6 +991,7 @@ int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frame
                                    int mode, float* const* outputs, int outputs_on_device, void* cuda_stream) {
     if (!net || !net->finalized) return fail("net not finalized");
     if (!frames) return fail("forward_ragged: null pointer");
+    if (int rc = check_outputs(net, outputs)) return rc;
     int Hc, Wc;
     if (int rc = ragged_canvas(n, hw, &Hc, &Wc)) return rc;
     CU(cudaSetDevice(net->device));
@@ -998,11 +1022,18 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess) {
     return 0;
 }
 
+int b200pose_net_set_stages(b200pose_net* net, int stages) {
+    if (!net) return fail("null net");
+    if (stages < 1 || stages > kStages) return fail("stages must be 1 .. %d, got %d", kStages, stages);
+    net->stages = stages;
+    return 0;
+}
+
 // The last forward ran net->plan: a tensor-core forward has run since the last finalize.
 static bool last_ran_plan(const b200pose_net* net) {
     const LastForward& l = net->last;
     const Plan* p = net->plan;
-    return p && !l.fp32 && p->n == l.n && p->H == l.H && p->W == l.W && p->fmt == l.fmt;
+    return p && !l.fp32 && p->n == l.n && p->H == l.H && p->W == l.W && p->fmt == l.fmt && p->stages == l.stages;
 }
 
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream) {
@@ -1088,7 +1119,9 @@ int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, 
         src = reinterpret_cast<const char*>((lo_plane ? net->act_lo : net->act)[buf].p);
     } else if (buf >= kNumAct && buf < kNumAct + 12 && !lo_plane) {
         const int m = buf - kNumAct;
-        per = (size_t)(H / 8) * (W / 8) * (m % 2 == 0 ? kPaf : kHeat) * 4;
+        if (m >= 2 * net->last.stages)
+            return fail("debug_read: stage map %d was not written by the last forward (%d stages)", m, net->last.stages);
+        per =(size_t)(H / 8) * (W / 8) * (m % 2 == 0 ? kPaf : kHeat) * 4;
         src = reinterpret_cast<const char*>(net->out_f32[m].p);
     } else {
         return fail("debug_read: no buffer %d (plane %d)", buf, lo_plane);
@@ -1138,7 +1171,7 @@ int b200pose_net_overflow(b200pose_net* net, int* flags, int n, void* cuda_strea
 
 int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** heat, int* n, int* h, int* w) {
     if (!net || net->last.n == 0) return fail("no forward has run");
-    *paf = net->out_f32[10].p; *heat = net->out_f32[11].p;
+    *paf = last_paf(net); *heat = last_heat(net);
     *n = net->last.n; *h = net->last.H / 8; *w = net->last.W / 8;
     return 0;
 }
@@ -1468,18 +1501,18 @@ static int stash_overflow(const b200pose_net* net, b200pose_post* post, int nimg
     return 0;
 }
 
-// Flip TTA: merges the last forward's 2n images [frames | mirrors] of stage-6 maps into n maps at oh / op.
+// Flip TTA: merges the last forward's 2n images [frames | mirrors] of final maps into n maps at oh / op.
 static int merge_last_flip(const b200pose_net* net, int n, float* oh, float* op, cudaStream_t st) {
     const int h = net->last.H / 8, w = net->last.W / 8;
     const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
-    const float *heat = net->out_f32[11].p, *paf = net->out_f32[10].p;
+    const float *heat = last_heat(net), *paf = last_paf(net);
     return flip_merge_dev(heat, heat + eh, paf, paf + ep, 0, n, h, w, oh, op, st, net->last.ext);
 }
 
 // Post-processing of the n frames of the last forward (flip: merged from its 2n images into post->d_heat / d_paf).
 static int finish_infer(const b200pose_net* net, b200pose_post* post, int n, int flip, float thresh, cudaStream_t st) {
     const int h = net->last.H / 8, w = net->last.W / 8;
-    const float *heat = net->out_f32[11].p, *paf = net->out_f32[10].p;
+    const float *heat = last_heat(net), *paf = last_paf(net);
     if (flip) {
         CU(post->d_heat.ensure((size_t)n * kHeat * h * w));
         CU(post->d_paf.ensure((size_t)n * kPaf * h * w));
@@ -1676,7 +1709,7 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
         if (int rc = stash_overflow(net, post, nimg, st)) return rc;
         const int h = c.Hc / 8, w = c.Wc / 8;
         const size_t eh = (size_t)n * kHeat * h * w, ep = (size_t)n * kPaf * h * w;
-        const float *s_heat = net->out_f32[11].p, *s_paf = net->out_f32[10].p;
+        const float *s_heat = last_heat(net), *s_paf = last_paf(net);
         if (flip) {
             CU(post->tta_out.ensure(eh + ep));
             if (int rc = merge_last_flip(net, n, post->tta_out.p, post->tta_out.p + eh, st)) return rc;

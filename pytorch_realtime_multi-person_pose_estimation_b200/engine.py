@@ -72,6 +72,14 @@ class NativeNet:
             raise nat.B200PoseError("unknown preprocess %r (expected one of %s)" % (name, sorted(nat.PREPROCESS)))
         nat.check(nat.lib().b200pose_net_set_preprocess(self._h, nat.PREPROCESS[name]), "b200pose_net_set_preprocess")
 
+    def set_stages(self, k):
+        """Refinement stages every later forward runs: the trunk, stage 1 and stages 2 .. k (1 <= k <= 6, default 6).
+        Forwards fill the first 2k of the 12 stage maps; the fused entry points post-process stage k's maps."""
+        k = int(k)
+        if k != self.__dict__.get("_stages", 6):      # the net's count: every change of it goes through here
+            nat.check(nat.lib().b200pose_net_set_stages(self._h, k), "b200pose_net_set_stages")
+            self._stages = k
+
     def forward_ptr(self, in_ptr, in_on_device, n, H, W, mode, out_ptrs, out_on_device, stream):
         arr = (ctypes.c_void_p * 12)(*[ctypes.c_void_p(p) if p else None for p in out_ptrs])
         nat.check(nat.lib().b200pose_net_forward(self._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H, W, mode,
@@ -253,18 +261,30 @@ def humans_to_dicts(rows, width, height):
 
 
 class PoseEngine:
-    """Fused batched inference on one GPU: images -> humans, maps never leave the device."""
+    """Fused batched inference on one GPU: images -> humans, maps never leave the device.  `stages`: the refinement
+    stages each submission runs (1 .. 6); the fused entry points post-process the last one's maps."""
 
-    def __init__(self, state_arrays, device_index=0, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, net=None):
+    stages = 6
+
+    def __init__(self, state_arrays, device_index=0, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, net=None,
+                 stages=6):
         if net is None:
             net = NativeNet(device_index)
             net.load_state_dict_arrays(state_arrays)
         self.net = net
+        self.stages = int(stages)
+        self.net.set_stages(self.stages)      # an invalid count fails here, before any submission
         self.post = NativePost(device_index, batch_cap, peak_cap, human_cap)
         self.mode = nat.MODES[mode]
         self.device_index = device_index
         self._shapes = {}
         self._last = None
+
+    def _net_h(self):
+        """The net's handle, set to this engine's stage count: engines may share a net with each other and with the
+        module (rtpose_model.pose_engine), so the count is set before every submission."""
+        self.net.set_stages(self.stages)
+        return self.net._h
 
     def _remember(self, n, H, W):
         """Shape of the run just submitted, kept per ticket (two runs may be in flight with different batch sizes or
@@ -287,9 +307,9 @@ class PoseEngine:
         return self._shapes[ticket]
 
     @classmethod
-    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024):
+    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=6):
         """An engine around an existing NativeNet (e.g. the one a get_model() module already packed its weights into)."""
-        return cls(None, net.device_index, mode, batch_cap, peak_cap, human_cap, net=net)
+        return cls(None, net.device_index, mode, batch_cap, peak_cap, human_cap, net=net, stages=stages)
 
     def submit_images(self, images, dest_size=368, factor=8, thresh=0.1, flip=False):
         """Asynchronous half of infer_images for frames of ONE shape (a video stream): returns a ticket; the frames must
@@ -309,13 +329,13 @@ class PoseEngine:
         return t
 
     def infer_async(self, in_ptr, in_on_device, n, H, W, thresh=0.1, stream=0):
-        nat.check(nat.lib().b200pose_infer(self.net._h, self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H, W,
+        nat.check(nat.lib().b200pose_infer(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H, W,
                                            self.mode, ctypes.c_float(thresh), ctypes.c_void_p(stream)), "b200pose_infer")
         return self._remember(n, H, W)
 
     def infer_async_u8(self, in_ptr, in_on_device, n, H, W, thresh=0.1, stream=0):
         """uint8 HWC BGR frames [n,H,W,3] (host pinned or device); preprocessing runs on the device."""
-        nat.check(nat.lib().b200pose_infer_u8(self.net._h, self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H,
+        nat.check(nat.lib().b200pose_infer_u8(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H,
                                               W, self.mode, ctypes.c_float(thresh), ctypes.c_void_p(stream)),
                   "b200pose_infer_u8")
         return self._remember(n, H, W)
@@ -323,13 +343,13 @@ class PoseEngine:
     def infer_flip_async(self, in_ptr, in_on_device, n, H, W, thresh=0.1, stream=0):
         """Flip test-time averaging (fp32 NCHW input): frames + device-made mirrored copies as one 2n batch, maps merged
         as handle_paf_and_heat does, post-processing on the averaged maps."""
-        nat.check(nat.lib().b200pose_infer_flip(self.net._h, self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n,
+        nat.check(nat.lib().b200pose_infer_flip(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n,
                                                 H, W, self.mode, ctypes.c_float(thresh), ctypes.c_void_p(stream)),
                   "b200pose_infer_flip")
         return self._remember(n, H, W)
 
     def infer_flip_async_u8(self, in_ptr, in_on_device, n, H, W, thresh=0.1, stream=0):
-        nat.check(nat.lib().b200pose_infer_u8_flip(self.net._h, self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device),
+        nat.check(nat.lib().b200pose_infer_u8_flip(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device),
                                                    n, H, W, self.mode, ctypes.c_float(thresh), ctypes.c_void_p(stream)),
                   "b200pose_infer_u8_flip")
         return self._remember(n, H, W)
@@ -338,7 +358,7 @@ class PoseEngine:
                            stream=0):
         """Raw uint8 BGR frames of one size [n,src_h,src_w,3]: crop_with_factor (resize + pad), the network and the
         post-processing all run on the device.  Person coordinates refer to the padded frame."""
-        nat.check(nat.lib().b200pose_infer_raw_u8(self.net._h, self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n,
+        nat.check(nat.lib().b200pose_infer_raw_u8(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n,
                                                   src_h, src_w, int(dest_size), int(factor), self.mode,
                                                   ctypes.c_float(thresh), int(bool(flip)), ctypes.c_void_p(stream)),
                   "b200pose_infer_raw_u8")
@@ -351,7 +371,7 @@ class PoseEngine:
         each frame is cropped to its own padded size and person coordinates refer to that padded frame."""
         n = len(src_shapes)
         hw = (ctypes.c_int * (2 * n))(*[int(v) for s in src_shapes for v in s])
-        nat.check(nat.lib().b200pose_infer_raw_u8_ragged(self.net._h, self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device),
+        nat.check(nat.lib().b200pose_infer_raw_u8_ragged(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device),
                                                          n, hw, int(dest_size), int(factor), self.mode,
                                                          ctypes.c_float(thresh), int(bool(flip)), ctypes.c_void_p(stream)),
                   "b200pose_infer_raw_u8_ragged")
@@ -364,7 +384,7 @@ class PoseEngine:
         every scale s runs crop_with_factor(int(base_size * s)) + the network on the device, the maps are resized
         (bicubic) to the grid of base_size, averaged, and post-processed.  Coordinates refer to the padded base frame."""
         arr = (ctypes.c_double * len(scales))(*[float(s) for s in scales])
-        nat.check(nat.lib().b200pose_infer_raw_u8_multiscale(self.net._h, self.post._h, ctypes.c_void_p(in_ptr),
+        nat.check(nat.lib().b200pose_infer_raw_u8_multiscale(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr),
                                                              int(in_on_device), n, src_h, src_w, int(base_size),
                                                              int(factor), arr, len(scales), self.mode,
                                                              ctypes.c_float(thresh), int(bool(flip)),
@@ -381,7 +401,7 @@ class PoseEngine:
         n = len(src_shapes)
         hw = (ctypes.c_int * (2 * n))(*[int(v) for s in src_shapes for v in s])
         arr = (ctypes.c_double * len(scales))(*[float(s) for s in scales])
-        nat.check(nat.lib().b200pose_infer_raw_u8_multiscale_ragged(self.net._h, self.post._h, ctypes.c_void_p(in_ptr),
+        nat.check(nat.lib().b200pose_infer_raw_u8_multiscale_ragged(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr),
                                                                     int(in_on_device), n, hw, int(base_size), int(factor),
                                                                     arr, len(scales), self.mode, ctypes.c_float(thresh),
                                                                     int(bool(flip)), ctypes.c_void_p(stream)),

@@ -15,9 +15,15 @@ about 8x finer rounding than bf16; kernels at bf16's speed, frames/s 2 - 4 % low
 leave binary16's range raises B200PoseError) or `'fp32'` (CUDA cores, bit-identical to the oracle's fp32 network); the
 environment variable B200POSE_MODE sets the default.
 
+Refinement stages: `model.stages = k` (1 .. 6; default 6, or the environment variable B200POSE_STAGES) runs the trunk
+and stages 1 .. k only.  `forward` then returns `((paf_k, heat_k), saved_for_loss[:2k])`, and `get_outputs`, the
+batched `run_eval` and `PoseStream` use stage k's maps: a faster, coarser prediction of the same kind (every stage's
+maps are trained against the same targets).  Stage k's maps are those of a six-stage forward, bit for bit.
+
 In fp16 mode `forward` and `get_outputs` check for overflow before they return: that waits for the forward on the current
 stream (one stream synchronisation per call, which `get_outputs` pays anyway when it copies the maps to the host).
 """
+import numbers
 import os
 import threading
 
@@ -27,6 +33,7 @@ import torch.nn as nn
 from ... import _native as nat
 from ...engine import NativeNet
 
+STAGES = 6      # refinement stages of the network; `rtpose_model.stages` may stop after any of them
 _TRUNK = [(3, 64), (64, 64), "P", (64, 128), (128, 128), "P", (128, 256), (256, 256), (256, 256), (256, 256), "P",
           (256, 512), (512, 512), (512, 256), (256, 128)]
 
@@ -67,6 +74,7 @@ class rtpose_model(nn.Module):
         for s in range(1, 7):
             setattr(self, "model%d_2" % s, _make_branch(_stage_spec(s, 19)))
         self.precision = os.environ.get("B200POSE_MODE", "bf16x3")
+        self.stages = int(os.environ.get("B200POSE_STAGES", STAGES))
         self._engines = {}     # device index -> (signature, NativeNet); shared by DataParallel replicas
         self._lock = threading.Lock()
         # DataParallel replicas are shallow copies with EMPTY `_parameters` (torch/nn/parallel/replicate.py): plain
@@ -126,13 +134,21 @@ class rtpose_model(nn.Module):
         self._lock = threading.Lock()
         self._master = [self]
 
+    def _stage_count(self):
+        """`stages` as an int in 1 .. 6; ValueError otherwise, raised before any device work."""
+        k = self.stages
+        if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= k <= STAGES:
+            raise ValueError("stages must be an integer in 1 .. %d, got %r" % (STAGES, k))
+        return int(k)
+
     def maps_from_frame(self, img, preprocess, dest_size, factor):
         """The device-side body of get_outputs (evaluate/coco_eval.py:80-114) for one raw uint8 BGR frame: the frame
         goes to the GPU as bytes, crop_with_factor (bilinear resize + zero padding, bit-identical to cv2's) and the
         `preprocess` normalisation run there, fused into the first convolution's load, and only the two final maps come
-        back.  Returns (paf [1,38,h,w], heat [1,19,h,w]) CUDA tensors and im_scale."""
+        back: those of stage `stages`.  Returns (paf [1,38,h,w], heat [1,19,h,w]) CUDA tensors and im_scale."""
         import ctypes
         import numpy as np
+        k = self._stage_count()
         master = self._master[0]
         device = next(master.parameters()).device
         if device.type != "cuda":
@@ -141,6 +157,7 @@ class rtpose_model(nn.Module):
             raise ValueError("precision must be one of %s" % list(nat.MODES))
         net = self._engine(device)
         net.set_preprocess(preprocess)
+        net.set_stages(k)
         img = np.ascontiguousarray(img)
         sh, sw = img.shape[:2]
         scale, _, (ph, pw) = nat.crop_geometry(sh, sw, dest_size, factor)
@@ -152,31 +169,34 @@ class rtpose_model(nn.Module):
                                                               1, ctypes.c_void_p(stream)), "b200pose_net_crop_with_factor")
             paf = torch.empty((1, 38, ph // 8, pw // 8), dtype=torch.float32, device=device)
             heat = torch.empty((1, 19, ph // 8, pw // 8), dtype=torch.float32, device=device)
-            net.forward_u8_ptr(frame.data_ptr(), True, 1, ph, pw, nat.MODES[self.precision],
-                               [0] * 10 + [paf.data_ptr(), heat.data_ptr()], True, stream)
+            outs = [0] * 12
+            outs[2 * k - 2:2 * k] = [paf.data_ptr(), heat.data_ptr()]
+            net.forward_u8_ptr(frame.data_ptr(), True, 1, ph, pw, nat.MODES[self.precision], outs, True, stream)
             if nat.MODES[self.precision] == nat.MODE_FP16:
                 net.check_overflow(1, stream)
         return paf, heat, scale
 
     def pose_engine(self, batch_cap=32, peak_cap=2048, human_cap=2048):
         """The batched fused engine (network + post-processing, maps never leave the device) around this module's native
-        net and weights; cached per (device, precision, capacities).  evaluate.coco_eval.run_eval and the streaming
-        front-ends use it."""
+        net and weights, running `stages` stages; cached per (device, precision, stages, capacities).
+        evaluate.coco_eval.run_eval and the streaming front-ends use it."""
         from ...engine import PoseEngine
+        k = self._stage_count()
         master = self._master[0]
         device = next(master.parameters()).device
         if device.type != "cuda":
             raise nat.B200PoseError("the model must be on a CUDA device (model.cuda()): this build has no CPU fallback")
         net = self._engine(device)
         idx = device.index if device.index is not None else torch.cuda.current_device()
-        key = (idx, self.precision, batch_cap, peak_cap, human_cap)
+        key = (idx, self.precision, k, batch_cap, peak_cap, human_cap)
         with master._lock:
             cache = master.__dict__.setdefault("_pose_engines", {})
             if key not in cache:
-                cache[key] = PoseEngine.from_net(net, self.precision, batch_cap, peak_cap, human_cap)
+                cache[key] = PoseEngine.from_net(net, self.precision, batch_cap, peak_cap, human_cap, stages=k)
             return cache[key]
 
     def forward(self, x):
+        k = self._stage_count()
         if not x.is_cuda:
             raise nat.B200PoseError("rtpose_model.forward needs a CUDA tensor: this build has no CPU fallback")
         if self.precision not in nat.MODES:
@@ -188,11 +208,12 @@ class rtpose_model(nn.Module):
         net = self._engine(x.device)
         h, w = H // 8, W // 8
         saved = [torch.empty((n, 38 if i % 2 == 0 else 19, h, w), dtype=torch.float32, device=x.device)
-                 for i in range(12)]
+                 for i in range(2 * k)]
+        net.set_stages(k)
         with torch.cuda.device(x.device):
             stream = torch.cuda.current_stream().cuda_stream
-            net.forward_ptr(x.data_ptr(), True, n, H, W, nat.MODES[self.precision], [t.data_ptr() for t in saved], True,
-                            stream)
+            net.forward_ptr(x.data_ptr(), True, n, H, W, nat.MODES[self.precision],
+                            [t.data_ptr() for t in saved] + [0] * (12 - 2 * k), True, stream)
             if nat.MODES[self.precision] == nat.MODE_FP16:
                 net.check_overflow(n, stream)
         return (saved[-2], saved[-1]), saved
