@@ -19,8 +19,8 @@ from test_gpu_layers import BUF_C, Hooks, _nchw, _forward, launch_table, layer_n
 
 pytestmark = pytest.mark.gpu
 REF = "cuda"
-SHAPES = [((1, 8, 8), (0,)), ((2, 64, 72), (0, 1)), ((1, 368, 368), (0,)), ((8, 368, 368), (0, 7)),
-          ((32, 368, 368), (0, 31))]
+SHAPES = [((1, 8, 8), (0,)), ((2, 64, 72), (0, 1)), ((1, 184, 248), (0,)), ((1, 368, 368), (0,)),
+          ((2, 368, 496), (0, 1)), ((8, 368, 368), (0, 7)), ((32, 368, 368), (0, 31))]
 
 
 def _debug_fp8(hooks, i, n):
