@@ -234,6 +234,7 @@ int b200pose_infer_u8_flip(b200pose_net* net, b200pose_post* post, const unsigne
  *                                    it, then the maps are merged as handle_paf_and_heat does.
  *     Person coordinates are in pixels of the padded frame (pad_h x pad_w), like the reference's.
  * ---------------------------------------------------------------------------------------------------------- */
+/* (Video frames in NV12 / I420 or rotated: b200pose_infer_frames, section 3d.) */
 int b200pose_crop_geometry(int src_h, int src_w, int dest_size, int factor, double* im_scale, int* res_h, int* res_w,
                            int* pad_h, int* pad_w);
 int b200pose_net_crop_with_factor(b200pose_net* net, const unsigned char* images, int images_on_device, int n, int src_h,
@@ -271,6 +272,41 @@ int b200pose_infer_raw_u8_multiscale_ragged(b200pose_net* net, b200pose_post* po
                                             int input_on_device, int n, const int* src_hw, int base_size, int factor,
                                             const double* scales, int n_scales, int mode, float thresh, int flip,
                                             void* cuda_stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * 3d. Video frames: replaces the host-side cv2.cvtColor + cv2.rotate ahead of get_outputs   video_demo.py:29-46
+ *     (DESIGN.md 2.10).  Frames as decoders and capture devices hand them out - NV12 (Y plane + interleaved UV plane
+ *     of h/2 rows), planar I420 (Y, U, V; U and V h/2 x w/2) or pitched BGR HWC - every plane with its own pitch, in
+ *     host or device memory.  They are converted on the device to uint8 HWC BGR, rotated by `rotate` degrees clockwise
+ *     (0, 90 = cv2.ROTATE_90_CLOCKWISE, 180, 270 = cv2.ROTATE_90_COUNTERCLOCKWISE), bit for bit what
+ *     cv2.rotate(cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420), code) gives (OpenCV 4.13; csrc/frame_core.h).
+ *     4:2:0 frames need even sizes; every pitch must cover a row (BGR 3w, Y w, NV12 UV w, I420 U / V w/2 bytes).
+ *     on_device = 0: host planes, copied into device staging with cudaMemcpy2DAsync (NV12 / I420 cross PCIe at half
+ *     the bytes of BGR); 1: device planes, read in place.  Every frame is checked before anything is enqueued; an
+ *     invalid one fails naming the frame and the field.
+ * ---------------------------------------------------------------------------------------------------------- */
+#define B200POSE_FRAME_BGR 0
+#define B200POSE_FRAME_NV12 1
+#define B200POSE_FRAME_I420 2
+typedef struct b200pose_frame {
+    const unsigned char* plane[3];   /* BGR: [0]; NV12: Y, UV; I420: Y, U, V */
+    int pitch[3];                    /* bytes per row of each plane */
+    int h, w;                        /* stored size in pixels */
+} b200pose_frame;
+/* n <= 1024 frames -> out: their rotated BGR HWC frames packed back to back (frame i: oh_i x ow_i x 3 bytes, (oh, ow) =
+ * (h, w) or (w, h) when rotated by 90 / 270).  out_on_device: 0 = host memory (the call synchronises the stream),
+ * 1 = device memory (asynchronous on cuda_stream). */
+int b200pose_net_convert_frames(b200pose_net* net, const b200pose_frame* frames, int n, int format, int on_device,
+                                int rotate, unsigned char* out, int out_on_device, void* cuda_stream);
+/* frames -> conversion -> the b200pose_infer_raw_u8* pipeline at the rotated sizes: scales NULL runs one scale
+ * (dest_size), else multi-scale averaging around dest_size; frames of one rotated size run as a uniform batch, mixed
+ * sizes as a ragged one.  n <= the post object's batch_cap, and with flip 2n <= 1024.  Per frame, person rows and peaks
+ * are those the b200pose_infer_raw_u8* entry point gives for the converted, rotated frame, in pixels of its padded
+ * frame.  Packed BGR frames (pitch 3w, each frame right behind the previous one) with rotate 0 take that entry point
+ * as they are, without a conversion launch.  Host frames stay alive until the fetch; fetched like b200pose_infer's. */
+int b200pose_infer_frames(b200pose_net* net, b200pose_post* post, const b200pose_frame* frames, int n, int format,
+                          int on_device, int rotate, int dest_size, int factor, const double* scales, int n_scales,
+                          int mode, float thresh, int flip, void* cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument

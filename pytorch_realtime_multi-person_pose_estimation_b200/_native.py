@@ -67,6 +67,9 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_infer_raw_u8_ragged": ([vp, vp, vp, ci, ci, vp, ci, ci, ci, cf, ci, vp], ci),
     "b200pose_infer_raw_u8_multiscale_ragged": ([vp, vp, vp, ci, ci, vp, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci,
                                                  cf, ci, vp], ci),
+    "b200pose_net_convert_frames": ([vp, vp, ci, ci, ci, ci, vp, ci, vp], ci),
+    "b200pose_infer_frames": ([vp, vp, vp, ci, ci, ci, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf, ci, vp],
+                              ci),
     "process_paf": ([ci, ci, ci, vp, ci, ci, ci, vp, ci, ci, ci, vp], ci),
     "get_num_humans": ([], ci),
     "get_part_cid": ([ci, ci], ci),
@@ -75,6 +78,25 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "get_part_y": ([ci], ci),
     "get_part_score": ([ci], cf),
 }
+
+# b200pose_frame (include/b200pose.h 3d): pixel formats and the per-frame descriptor
+FRAME_FORMATS = {"bgr": 0, "nv12": 1, "i420": 2}
+# cv2.ROTATE_90_CLOCKWISE, cv2.ROTATE_180, cv2.ROTATE_90_COUNTERCLOCKWISE -> degrees clockwise
+_CV2_ROTATIONS = {0: 90, 1: 180, 2: 270}
+
+
+class Frame(ctypes.Structure):
+    _fields_ = [("plane", ctypes.c_void_p * 3), ("pitch", ctypes.c_int * 3), ("h", ctypes.c_int), ("w", ctypes.c_int)]
+
+
+def rotation_of(rotate_code):
+    """Degrees clockwise of a cv2.ROTATE_* code (None: 0) - the `rotate` argument of the frame entry points."""
+    if rotate_code is None:
+        return 0
+    if rotate_code not in _CV2_ROTATIONS:
+        raise B200PoseError("unknown cv2 rotate code %r (cv2.ROTATE_90_CLOCKWISE, _180 or _90_COUNTERCLOCKWISE)"
+                            % (rotate_code,))
+    return _CV2_ROTATIONS[rotate_code]
 
 
 class B200PoseError(RuntimeError):

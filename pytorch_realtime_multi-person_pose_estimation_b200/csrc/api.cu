@@ -19,6 +19,7 @@
 #include "conv_misc.cuh"
 #include "conv_tc.cuh"
 #include "f16_core.h"
+#include "frames.cuh"
 #include "fp8_core.h"
 #include "postprocess.cuh"
 #include "resize.cuh"
@@ -266,6 +267,10 @@ struct b200pose_net {
     // rewritten on the stream before each ragged forward.
     int* d_ext = nullptr;
     DevBuf<RaggedFrame> d_frames;      // per-frame source geometry of the last ragged crop
+    // video frames (b200pose_net_convert_frames, b200pose_infer_frames): the planes of host frames, packed, and the
+    // source table of the last conversion
+    DevBuf<unsigned char> frame_stage;
+    DevBuf<FrameSrc> d_frame_src;
     // fp8 mode (DESIGN.md §2.3): amax[launch * n + image] = max |bf16| (fp32 bits) launch (0 = conv1_1) stored for the
     // image; zeroed at the start of every fp8 forward
     DevBuf<unsigned> amax;
@@ -789,6 +794,8 @@ void b200pose_net_destroy(b200pose_net* net) {
     net->in_stage_u8.release();
     net->raw_stage.release();
     net->d_frames.release();
+    net->frame_stage.release();
+    net->d_frame_src.release();
     if (net->d_ext) cudaFree(net->d_ext);
     for (auto* b : fb) b->release();
     for (auto& b : net->out_f32) b.release();
@@ -1649,15 +1656,136 @@ static int raw_batch(int n, int src_h, int src_w, const int* src_hw, int dest_si
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ video frames
+// The frames of one b200pose_net_convert_frames / b200pose_infer_frames call, checked: the source table
+// convert_frames_kernel reads (host planes until they are staged), the rotated sizes [oh_0, ow_0, oh_1, ...], the packed
+// BGR output's size and the largest rotated frame's pixel count.
+struct FrameBatch {
+    std::vector<FrameSrc> tab;
+    std::vector<int> hw;
+    int format = 0, rotate = 0;
+    long long bytes = 0, max_px = 0;
+    bool uniform() const {
+        for (size_t i = 2; i < hw.size(); i += 2)
+            if (hw[i] != hw[0] || hw[i + 1] != hw[1]) return false;
+        return true;
+    }
+};
+
+constexpr const char* kFrameFormatName[3] = {"BGR", "NV12", "I420"};
+
+// Plane k of a stored h x w frame of `format`: bytes per row and rows.
+static void frame_plane_shape(int format, int k, int h, int w, long* row, int* rows) {
+    *row = format == kFrameBGR ? 3L * w : (k == 0 || format == kFrameNV12 ? (long)w : (long)w / 2);
+    *rows = k == 0 ? h : h / 2;
+}
+
+static int frame_planes(int format) { return format == kFrameBGR ? 1 : (format == kFrameNV12 ? 2 : 3); }
+
+// Checks every frame of a call before anything is enqueued.
+static int check_frames(const b200pose_frame* frames, int n, int max_n, int format, int rotate, FrameBatch* b) {
+    if (format < kFrameBGR || format > kFrameI420)
+        return fail("frames: format %d is unknown (B200POSE_FRAME_BGR 0, _NV12 1, _I420 2)", format);
+    if (rotate != 0 && rotate != 90 && rotate != 180 && rotate != 270)
+        return fail("frames: rotate %d (0, 90, 180 or 270 degrees clockwise)", rotate);
+    if (!frames) return fail("frames: null frame table");
+    if (n < 1 || n > max_n) return fail("frames: %d frames (1 .. %d)", n, max_n);
+    *b = FrameBatch{};
+    b->format = format;
+    b->rotate = rotate;
+    for (int i = 0; i < n; ++i) {
+        const b200pose_frame& f = frames[i];
+        if (f.h < 1 || f.w < 1 || (long)f.h * f.w > (1L << 28))
+            return fail("frame %d: size h = %d, w = %d (1 .. 2^28 pixels)", i, f.h, f.w);
+        if (format != kFrameBGR && (f.h % 2 || f.w % 2))
+            return fail("frame %d: %s needs even sizes, h = %d, w = %d", i, kFrameFormatName[format], f.h, f.w);
+        FrameSrc s{};
+        for (int k = 0; k < frame_planes(format); ++k) {
+            long row;
+            int rows;
+            frame_plane_shape(format, k, f.h, f.w, &row, &rows);
+            if (!f.plane[k]) return fail("frame %d: plane[%d] is null", i, k);
+            if (f.pitch[k] < row)
+                return fail("frame %d: pitch[%d] = %d is shorter than a %s row of %ld bytes", i, k, f.pitch[k],
+                            kFrameFormatName[format], row);
+            s.plane[k] = f.plane[k];
+            s.pitch[k] = f.pitch[k];
+        }
+        s.h = f.h;
+        s.w = f.w;
+        s.off = b->bytes;
+        int oh, ow;
+        fr_rotated_size(f.h, f.w, rotate, &oh, &ow);
+        b->hw.push_back(oh);
+        b->hw.push_back(ow);
+        b->bytes += (long long)oh * ow * 3;
+        if ((long long)oh * ow > b->max_px) b->max_px = (long long)oh * ow;
+        b->tab.push_back(s);
+    }
+    return 0;
+}
+
+// Packed BGR frames (pitch 3w, frame i + 1 right behind frame i) that need no rotation: the raw-frame path reads them
+// as they are.
+static bool frames_are_packed_bgr(const FrameBatch& b) {
+    if (b.format != kFrameBGR || b.rotate != 0) return false;
+    for (const FrameSrc& s : b.tab)
+        if (s.pitch[0] != 3 * s.w || s.plane[0] != b.tab[0].plane[0] + s.off) return false;
+    return true;
+}
+
+// Converts the frames of b into `out` (device, b.bytes): host planes are first copied, packed, into net->frame_stage.
+static int convert_frames_dev(b200pose_net* net, const FrameBatch& b, int on_device, unsigned char* out, cudaStream_t st) {
+    std::vector<FrameSrc> tab = b.tab;
+    const int planes = frame_planes(b.format);
+    if (!on_device) {
+        size_t total = 0;
+        for (const FrameSrc& s : tab)
+            for (int k = 0; k < planes; ++k) {
+                long row;
+                int rows;
+                frame_plane_shape(b.format, k, s.h, s.w, &row, &rows);
+                total += (size_t)row * rows;
+            }
+        CU(net->frame_stage.ensure(total));
+        size_t at = 0;
+        for (FrameSrc& s : tab)
+            for (int k = 0; k < planes; ++k) {
+                long row;
+                int rows;
+                frame_plane_shape(b.format, k, s.h, s.w, &row, &rows);
+                CU(cudaMemcpy2DAsync(net->frame_stage.p + at, row, s.plane[k], s.pitch[k], row, rows,
+                                     cudaMemcpyHostToDevice, st));
+                s.plane[k] = net->frame_stage.p + at;
+                s.pitch[k] = (int)row;
+                at += (size_t)row * rows;
+            }
+    }
+    CU(net->d_frame_src.ensure(tab.size()));
+    CU(cudaMemcpyAsync(net->d_frame_src.p, tab.data(), tab.size() * sizeof(FrameSrc), cudaMemcpyHostToDevice, st));
+    return launched(convert_frames_launch(net->d_frame_src.p, (int)tab.size(), b.format, b.rotate, (long)b.max_px, out, st),
+                    "convert_frames_launch");
+}
+
+// The frames of b converted into net->raw_stage, with room for their mirror images behind them when flip: what
+// stage_raw makes of packed BGR frames.
+static int stage_frames(b200pose_net* net, const FrameBatch& b, int on_device, int flip, cudaStream_t st,
+                        const unsigned char** d_raw) {
+    CU(net->raw_stage.ensure((size_t)b.bytes * (flip ? 2 : 1)));
+    *d_raw = net->raw_stage.p;
+    return convert_frames_dev(net, b, on_device, net->raw_stage.p, st);
+}
+
 // The fused inference of raw uint8 frames (b200pose_infer_raw_u8*): n frames of one size src_h x src_w, or of the
 // sizes src_hw (a ragged batch), are staged with their mirror images when flip, cropped for every scale and run
 // through the network.  scales null: one scale, base_size, post-processed as it is.  Else every scale s runs at
 // int(base_size * s) and its maps are resized (bicubic) to the grid of base_size, averaged and post-processed.
+// fb (b200pose_infer_frames): the frames are those of fb, converted into the staging buffer, instead of `images`.
 static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char* images, int on_device, int n,
                      int src_h, int src_w, const int* src_hw, int base_size, int factor, const double* scales,
-                     int n_scales, int mode, float thresh, int flip, void* cuda_stream) {
+                     int n_scales, int mode, float thresh, int flip, void* cuda_stream, const FrameBatch* fb = nullptr) {
     if (int rc = check_infer(net, post)) return rc;
-    if (!images) return fail("infer_raw: null pointer");
+    if (!images && !fb) return fail("infer_raw: null pointer");
     if (scales && (n_scales < 1 || n_scales > 16)) return fail("infer_raw: %d scales (1 .. 16)", n_scales);
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
     const bool ragged = src_hw != nullptr;
@@ -1678,7 +1806,9 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
     const unsigned char* d_raw;
-    if (int rc = stage_raw(net, images, on_device, (size_t)sc[0].raw, flip, st, &d_raw)) return rc;
+    if (int rc = fb ? stage_frames(net, *fb, on_device, flip, st, &d_raw)
+                    : stage_raw(net, images, on_device, (size_t)sc[0].raw, flip, st, &d_raw))
+        return rc;
     // the sources and offsets of the frame table are those of every scale
     if (ragged && upload_frames(net, sc[0].tab, st)) return 1;
     if (flip) {      // mirrored RAW frames, so that the padding of both orientations ends up on the right, as for the reference
@@ -1765,6 +1895,42 @@ int b200pose_infer_raw_u8_multiscale_ragged(b200pose_net* net, b200pose_post* po
     return scales && src_hw ? infer_raw(net, post, images, input_on_device, n, 0, 0, src_hw, base_size, factor, scales,
                                         n_scales, mode, thresh, flip, cuda_stream)
                             : fail("infer_multiscale_ragged: null pointer");
+}
+
+int b200pose_net_convert_frames(b200pose_net* net, const b200pose_frame* frames, int n, int format, int on_device,
+                                int rotate, unsigned char* out, int out_on_device, void* cuda_stream) {
+    if (!net) return fail("null net");
+    if (!out) return fail("convert_frames: null output");
+    FrameBatch b;
+    if (int rc = check_frames(frames, n, kMaxRagged, format, rotate, &b)) return rc;
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    unsigned char* d_out = out;
+    if (!out_on_device) {
+        CU(net->raw_stage.ensure((size_t)b.bytes));
+        d_out = net->raw_stage.p;
+    }
+    if (int rc = convert_frames_dev(net, b, on_device, d_out, st)) return rc;
+    if (!out_on_device) CU(cudaMemcpyAsync(out, d_out, (size_t)b.bytes, cudaMemcpyDeviceToHost, st));
+    if (!on_device || !out_on_device) CU(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int b200pose_infer_frames(b200pose_net* net, b200pose_post* post, const b200pose_frame* frames, int n, int format,
+                          int on_device, int rotate, int dest_size, int factor, const double* scales, int n_scales,
+                          int mode, float thresh, int flip, void* cuda_stream) {
+    if (int rc = check_infer(net, post)) return rc;
+    FrameBatch b;
+    if (int rc = check_frames(frames, n, post->pb.batch_cap, format, rotate, &b)) return rc;
+    if (flip && 2 * n > kMaxRagged) return fail("frames: %d frames with flip (2n <= %d)", n, kMaxRagged);
+    const bool uniform = b.uniform();
+    const int h = uniform ? b.hw[0] : 0, w = uniform ? b.hw[1] : 0;
+    const int* hw = uniform ? nullptr : b.hw.data();
+    if (frames_are_packed_bgr(b))
+        return infer_raw(net, post, b.tab[0].plane[0], on_device, n, h, w, hw, dest_size, factor, scales, n_scales, mode,
+                         thresh, flip, cuda_stream);
+    return infer_raw(net, post, nullptr, on_device, n, h, w, hw, dest_size, factor, scales, n_scales, mode, thresh, flip,
+                     cuda_stream, &b);
 }
 
 // ------------------------------------------------------------------------------------------------ legacy pafprocess

@@ -47,6 +47,90 @@ def check_overflow_flags(flags):
                                 "are not valid - run them in bf16, bf16x3 or fp32 mode" % bad)
 
 
+def _plane(a):
+    """(array kept alive, pointer, row pitch in bytes, shape, on_device) of one uint8 plane: a numpy array or a torch
+    tensor (CUDA: read in place).  Rows may be padded (the pitch is the row stride); within a row the bytes must be
+    contiguous, else the plane is copied."""
+    if isinstance(a, np.ndarray):
+        if a.dtype != np.uint8:
+            raise nat.B200PoseError("frames: expected uint8 planes, got %s" % a.dtype)
+        if a.ndim not in (2, 3):
+            raise nat.B200PoseError("frames: a plane has 2 or 3 dimensions, got shape %s" % (a.shape,))
+        if a.strides[-1] != 1 or (a.ndim == 3 and a.strides[1] != a.shape[2]) or a.strides[0] < a.shape[1] * a.strides[1]:
+            a = np.ascontiguousarray(a)
+        return a, a.ctypes.data, a.strides[0], a.shape, False
+    import torch
+    if not isinstance(a, torch.Tensor) or a.dtype != torch.uint8:
+        raise nat.B200PoseError("frames: expected uint8 numpy arrays or torch tensors, got %r" % (type(a),))
+    if not a.is_cuda:
+        return _plane(a.numpy())
+    if a.dim() not in (2, 3):
+        raise nat.B200PoseError("frames: a plane has 2 or 3 dimensions, got shape %s" % (tuple(a.shape),))
+    if a.stride(-1) != 1 or (a.dim() == 3 and a.stride(1) != a.shape[2]) or \
+            a.stride(0) < a.shape[1] * a.stride(1):
+        a = a.contiguous()
+    return a, a.data_ptr(), a.stride(0), tuple(a.shape), True
+
+
+def _frame_planes(frame, fmt):
+    """The planes of one frame: BGR (h, w, 3); NV12 / I420 as one packed 2-D (3h/2, w) array (cv2.cvtColor's layout)
+    or as a tuple (Y, UV) / (Y, U, V), UV given as (h/2, w) or (h/2, w/2, 2)."""
+    if fmt == "bgr":
+        return [frame]
+    if isinstance(frame, (tuple, list)):
+        return list(frame)
+    if len(frame.shape) != 2 or frame.shape[0] % 3:
+        raise nat.B200PoseError("frames: a packed %s frame is a 2-D (3h/2, w) array, got shape %s"
+                                % (fmt.upper(), tuple(frame.shape)))
+    h, w = frame.shape[0] * 2 // 3, frame.shape[1]
+    if fmt == "nv12":
+        return [frame[:h], frame[h:]]
+    if not isinstance(frame, np.ndarray):
+        frame = frame.contiguous()
+    else:
+        frame = np.ascontiguousarray(frame)
+    flat, q = frame.reshape(-1), (h // 2) * (w // 2)
+    return [frame[:h], flat[h * w:h * w + q].reshape(h // 2, w // 2), flat[h * w + q:h * w + 2 * q].reshape(h // 2, w // 2)]
+
+
+def frame_table(frames, format):
+    """frames -> (ctypes array of b200pose_frame, the arrays it points into, on_device, stored sizes [(h, w)]).
+    Plane shapes are checked here, so the library never reads past a plane; sizes and pitches are checked there."""
+    if format not in nat.FRAME_FORMATS:
+        raise nat.B200PoseError("frames: unknown format %r (expected one of %s)" % (format, sorted(nat.FRAME_FORMATS)))
+    table = (nat.Frame * max(1, len(frames)))()
+    keep, sides, sizes = [], set(), []
+    for i, frame in enumerate(frames):
+        planes = [_plane(a) for a in _frame_planes(frame, format)]
+        want = {"bgr": 1, "nv12": 2, "i420": 3}[format]
+        if len(planes) != want:
+            raise nat.B200PoseError("frame %d: %s has %d planes, got %d" % (i, format.upper(), want, len(planes)))
+        shp = [p[3] for p in planes]
+        h, w = shp[0][0], shp[0][1]
+        if format == "bgr":
+            ok = len(shp[0]) == 3 and shp[0][2] == 3
+        elif format == "nv12":
+            ok = len(shp[0]) == 2 and tuple(shp[1]) in ((h // 2, w), (h // 2, w // 2, 2))
+        else:
+            ok = len(shp[0]) == 2 and all(tuple(s) == (h // 2, w // 2) for s in shp[1:])
+        if not ok:
+            raise nat.B200PoseError("frame %d: plane shapes %s do not form a %s frame" % (i, shp, format.upper()))
+        for k, (arr, ptr, pitch, _, dev) in enumerate(planes):
+            table[i].plane[k] = ptr
+            table[i].pitch[k] = pitch
+            keep.append(arr)
+            sides.add(dev)
+        table[i].h, table[i].w = h, w
+        sizes.append((h, w))
+    if len(sides) > 1:
+        raise nat.B200PoseError("frames: all planes must be host arrays or all CUDA tensors")
+    return table, keep, sides == {True}, sizes
+
+
+def rotated_size(h, w, rotate):
+    return (w, h) if rotate in (90, 270) else (h, w)
+
+
 class NativeNet:
     """Owns a b200pose_net handle on one CUDA device."""
 
@@ -129,6 +213,21 @@ class NativeNet:
                                                           int(dest_size), int(factor), ctypes.c_void_p(out.ctypes.data), 0,
                                                           None), "b200pose_net_crop_with_factor")
         return (out[0] if single else out), scale, (rh, rw, 3)
+
+    def convert_frames(self, frames, format="nv12", rotate=0, stream=0):
+        """Device-side cv2.rotate(cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420)) of frames as PoseEngine.infer_frames
+        takes them: a list of uint8 BGR host arrays [oh, ow, 3], `rotate` degrees clockwise."""
+        table, keep, on_dev, sizes = frame_table(frames, format)
+        outs = [rotated_size(h, w, rotate) for h, w in sizes]
+        flat = np.empty(sum(h * w * 3 for h, w in outs), np.uint8)
+        nat.check(nat.lib().b200pose_net_convert_frames(self._h, table, len(frames), nat.FRAME_FORMATS[format],
+                                                        int(on_dev), int(rotate), ctypes.c_void_p(flat.ctypes.data), 0,
+                                                        ctypes.c_void_p(stream)), "b200pose_net_convert_frames")
+        res, at = [], 0
+        for h, w in outs:
+            res.append(flat[at:at + h * w * 3].reshape(h, w, 3))
+            at += h * w * 3
+        return res
 
     def __del__(self):
         try:
@@ -321,12 +420,59 @@ class PoseEngine:
             raise nat.B200PoseError("submit_images: %d frames exceed batch_cap %d" % (len(batch), self.post.batch_cap))
         t = self.infer_raw_async_u8(batch.ctypes.data, False, len(batch), batch.shape[1], batch.shape[2], dest_size, factor,
                                     thresh, flip)
+        return self._hold(t, batch)
+
+    def _hold(self, t, inputs):
+        """Keeps the host inputs of run t alive until its fetch: host staging is read asynchronously."""
         if self.__dict__.get("_alive") is None:
             self._alive = {}
-        self._alive[t] = batch                      # host staging is read asynchronously: keep it until the fetch
+        self._alive[t] = inputs
         for old in [k for k in self._alive if k < t - 1]:
             del self._alive[old]
         return t
+
+    def infer_frames_async(self, frames, format="nv12", rotate=0, dest_size=368, factor=8, thresh=0.1, flip=False,
+                           scales=None, stream=0):
+        """Video frames as decoders hand them out, converted and rotated on the device ahead of crop_with_factor
+        (b200pose_infer_frames): `format` 'nv12', 'i420' or 'bgr'; numpy arrays or CUDA uint8 tensors (read in place);
+        4:2:0 frames as one packed 2-D (3h/2, w) array (cv2.cvtColor's layout) or as planes (Y, UV) / (Y, U, V) whose
+        row strides are their pitches, so a padded decoder surface needs no copy; BGR as (h, w, 3).  `rotate`: degrees
+        clockwise (nat.rotation_of maps cv2.ROTATE_* codes).  Frames of one rotated size run as a uniform batch, mixed
+        sizes as a ragged one; scales as for infer_images.  Returns a ticket; host frames are kept alive until the
+        fetch.  Person coordinates refer to each rotated frame's padded frame."""
+        table, keep, on_dev, sizes = frame_table(frames, format)
+        rot = int(rotate)
+        arr = None if scales is None else (ctypes.c_double * len(scales))(*[float(s) for s in scales])
+        nat.check(nat.lib().b200pose_infer_frames(self._net_h(), self.post._h, table, len(frames),
+                                                  nat.FRAME_FORMATS[format], int(on_dev), rot, int(dest_size), int(factor),
+                                                  arr, 0 if scales is None else len(scales), self.mode,
+                                                  ctypes.c_float(thresh), int(bool(flip)), ctypes.c_void_p(stream)),
+                  "b200pose_infer_frames")
+        pads = [nat.crop_geometry(*rotated_size(h, w, rot), dest_size, factor)[2] for h, w in sizes]
+        if len(set(pads)) == 1:
+            t = self._remember(len(frames), pads[0][0], pads[0][1])
+        else:
+            t = self._remember(len(frames), [p[0] for p in pads], [p[1] for p in pads])
+        return self._hold(t, None if on_dev else keep)
+
+    def infer_frames_arrays(self, frames, format="nv12", rotate=0, dest_size=368, factor=8, thresh=0.1, flip=False,
+                            scales=None):
+        """infer_frames, but per frame the raw person rows (float32 [k, 73], pixel coordinates of the padded frame)."""
+        return self.infer_frames(frames, format, rotate, dest_size, factor, thresh, flip, scales, _arrays=True)
+
+    def infer_frames(self, frames, format="nv12", rotate=0, dest_size=368, factor=8, thresh=0.1, flip=False,
+                     scales=None, _arrays=False):
+        """Blocking infer_frames_async over any number of frames: per-frame human lists in input order.  Frames are
+        grouped into batches of at most batch_cap by plan_ragged_batches on their rotated padded sizes, as
+        infer_images groups BGR frames."""
+        _, _, _, sizes = frame_table(frames, format)
+        pads = [nat.crop_geometry(*rotated_size(h, w, int(rotate)), dest_size, factor)[2] for h, w in sizes]
+        out = [None] * len(frames)
+        for part in plan_ragged_batches(pads, self.post.batch_cap):
+            self.infer_frames_async([frames[i] for i in part], format, rotate, dest_size, factor, thresh, flip, scales)
+            for i, humans in zip(part, self.fetch_arrays() if _arrays else self.fetch()):
+                out[i] = humans.copy() if _arrays else humans
+        return out
 
     def infer_async(self, in_ptr, in_on_device, n, H, W, thresh=0.1, stream=0):
         nat.check(nat.lib().b200pose_infer(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H, W,

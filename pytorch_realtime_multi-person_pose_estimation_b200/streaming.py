@@ -8,6 +8,7 @@ fused engine), the host decodes the next frames and draws batch i.  The drawing 
 from .lib.utils.common import draw_humans
 from .lib.utils.paf_to_pose import humans_from_rows
 from . import _native as nat
+from . import engine
 
 
 def frames_of(capture, rotate_code=None, limit=None):
@@ -29,9 +30,14 @@ class PoseStream:
 
     model: a module from lib.network.rtpose_vgg.get_model() (bare or DataParallel-wrapped) on a CUDA device.
     frames: any iterator of uint8 BGR frames of ONE shape.  batch=1 minimises latency (camera), larger batches raise
-    throughput (files).  `draw=False` skips the rendering."""
+    throughput (files).  `draw=False` skips the rendering.
+    format 'nv12' / 'i420' (frames as PoseEngine.infer_frames_async takes them, e.g. decoder surfaces already on the GPU)
+    and rotate (degrees clockwise; nat.rotation_of maps cv2.ROTATE_* codes): the frames are converted and rotated on
+    the device; with draw=True each batch is also converted back to host BGR for the drawing, and the converted frame
+    is the one yielded."""
 
-    def __init__(self, model, frames, batch=8, preprocess='rtpose', dest_size=368, factor=8, thresh=0.1, draw=True):
+    def __init__(self, model, frames, batch=8, preprocess='rtpose', dest_size=368, factor=8, thresh=0.1, draw=True,
+                 format='bgr', rotate=None):
         core = getattr(model, "module", model)
         if not hasattr(core, "pose_engine"):
             raise nat.B200PoseError("PoseStream needs a model from lib.network.rtpose_vgg.get_model()")
@@ -39,6 +45,7 @@ class PoseStream:
         self.engine.net.set_preprocess(preprocess)
         self.frames, self.batch = iter(frames), max(1, int(batch))
         self.dest_size, self.factor, self.thresh, self.draw = dest_size, factor, thresh, draw
+        self.format, self.rotate = format, int(rotate or 0)
 
     def _next_batch(self):
         out = []
@@ -48,9 +55,9 @@ class PoseStream:
                 break
         return out
 
-    def _finish(self, ticket, batch):
+    def _finish(self, ticket, batch, size):
         rows = self.engine.fetch_arrays(ticket=ticket)
-        _, _, (ph, pw) = nat.crop_geometry(batch[0].shape[0], batch[0].shape[1], self.dest_size, self.factor)
+        _, _, (ph, pw) = nat.crop_geometry(size[0], size[1], self.dest_size, self.factor)
         for frame, r in zip(batch, rows):
             humans = humans_from_rows(r, pw, ph)
             # draw_humans scales by the ORIGINAL frame size, like the reference front-ends (coordinates are normalised by
@@ -61,12 +68,24 @@ class PoseStream:
         pending = None
         while True:
             batch = self._next_batch()
-            if batch:
+            if batch and self.format == 'bgr' and not self.rotate:
                 if any(f.shape != batch[0].shape for f in batch):
                     raise nat.B200PoseError("PoseStream: the frames of a stream must share one shape")
                 ticket = self.engine.submit_images(batch, self.dest_size, self.factor, self.thresh)
+                size = batch[0].shape[:2]
+            elif batch:
+                sizes = {engine.rotated_size(h, w, self.rotate) for h, w in engine.frame_table(batch, self.format)[3]}
+                if len(sizes) != 1:
+                    raise nat.B200PoseError("PoseStream: the frames of a stream must share one shape")
+                size = sizes.pop()
+                # host BGR frames to draw on: one more conversion launch and its download, before the submission so
+                # that its synchronisation waits only for the batch already in flight
+                shown = self.engine.net.convert_frames(batch, self.format, self.rotate) if self.draw else batch
+                ticket = self.engine.infer_frames_async(batch, self.format, self.rotate, self.dest_size, self.factor,
+                                                        self.thresh)
+                batch = shown
             if pending is not None:
                 yield from self._finish(*pending)
             if not batch:
                 return
-            pending = (ticket, batch)
+            pending = (ticket, batch, size)
