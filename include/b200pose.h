@@ -157,6 +157,29 @@ void b200pose_post_destroy(b200pose_post* post);
  * thresh = cfg.TEST.THRESH_HEATMAP.  Results stay on the device until fetched. */
 int b200pose_post_run(b200pose_post* post, const float* heat, const float* paf, int on_device, int layout, int n, int h,
                       int w, float thresh, void* cuda_stream);
+/* Post-processing settings (lib/pafprocess/pafprocess.h:7-13, compile-time constants in the reference).  They apply
+ * to the runs submitted after the call: b200pose_post_run and every fused b200pose_infer* entry point of this post
+ * object.  Each run keeps the settings it was submitted with, also while another run is in flight.  Comparisons keep
+ * the reference's form (pafprocess.cpp:73-90, 187-191): a sample counts iff vec . paf > paf_thresh, a pair is kept iff
+ * more than paf_min_above samples count, a person is dropped iff parts < min_parts or score / parts < min_person_score.
+ * The defaults run exactly the kernels of the reference's constants.  A looser prune may keep more persons than
+ * human_cap; that sets B200POSE_ST_HUMAN_OVERFLOW as usual.  The legacy process_paf surface (section 4) always uses
+ * the reference's constants.
+ *   b200pose_post_default_params : the defaults below
+ *   b200pose_post_set_params     : p = NULL restores the defaults; a value outside its range is refused with an error
+ *                                  naming the field, and the settings stay as they were
+ *   b200pose_post_get_params     : the settings the next run will use */
+typedef struct b200pose_post_params {
+    float paf_thresh;        /* THRESH_VECTOR_SCORE, pafprocess.h:7  = cfg.TEST.THRESH_PAF; finite                   0.05 */
+    int paf_samples;         /* STEP_PAF, pafprocess.h:13            = cfg.TEST.NUM_INTERMED_PTS_BETWEEN_KEYPOINTS;
+                                1 .. 64                                                                               10 */
+    int paf_min_above;       /* THRESH_VECTOR_CNT1, pafprocess.h:8; -1 .. paf_samples                                  6 */
+    int min_parts;           /* THRESH_PART_CNT, pafprocess.h:9; 0 .. 18                                               4 */
+    float min_person_score;  /* THRESH_HUMAN_SCORE, pafprocess.h:10; finite                                          0.3 */
+} b200pose_post_params;
+int b200pose_post_default_params(b200pose_post_params* out);
+int b200pose_post_set_params(b200pose_post* post, const b200pose_post_params* p);
+int b200pose_post_get_params(b200pose_post* post, b200pose_post_params* out);
 /* Every run copies its results (person rows, counts, status) to pinned host memory by itself, on a second stream right
  * after the person assembly, into one of two slots (run parity) - so a caller may submit run i+1 before reading run i
  * (at most two runs in flight).  The getters below read the selected slot.

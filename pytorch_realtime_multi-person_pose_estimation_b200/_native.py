@@ -43,6 +43,9 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_post_destroy": ([vp], None),
     "b200pose_post_run": ([vp, vp, vp, ci, ci, ci, ci, ci, cf, vp], ci),
     "b200pose_post_sync": ([vp], ci),
+    "b200pose_post_default_params": ([vp], ci),
+    "b200pose_post_set_params": ([vp, vp], ci),
+    "b200pose_post_get_params": ([vp, vp], ci),
     "b200pose_post_last_ticket": ([vp], cl),
     "b200pose_post_select": ([vp, cl], ci),
     "b200pose_post_debug": ([vp, vp, ci, ci], ci),
@@ -83,6 +86,15 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
 FRAME_FORMATS = {"bgr": 0, "nv12": 1, "i420": 2}
 # cv2.ROTATE_90_CLOCKWISE, cv2.ROTATE_180, cv2.ROTATE_90_COUNTERCLOCKWISE -> degrees clockwise
 _CV2_ROTATIONS = {0: 90, 1: 180, 2: 270}
+
+
+class PostParams(ctypes.Structure):
+    """b200pose_post_params (include/b200pose.h section 2): the settings of PAF scoring and the person prune."""
+    _fields_ = [("paf_thresh", ctypes.c_float), ("paf_samples", ctypes.c_int), ("paf_min_above", ctypes.c_int),
+                ("min_parts", ctypes.c_int), ("min_person_score", ctypes.c_float)]
+
+    def as_dict(self):
+        return {name: getattr(self, name) for name, _ in self._fields_}
 
 
 class Frame(ctypes.Structure):

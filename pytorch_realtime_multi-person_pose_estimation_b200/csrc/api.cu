@@ -318,6 +318,10 @@ struct b200pose_post {
     unsigned* hp_ovf[2] = {nullptr, nullptr};
     int ovf_rows[2] = {0, 0}, ovf_imgs[2] = {0, 0};    // forwards copied, images per forward (2n with flip)
     int ovf_pending = 0, ovf_pending_imgs = 0;          // ... of the run being enqueued
+    // scoring / prune settings of the runs submitted from now on (b200pose_post_set_params); they travel to the kernels
+    // by value, so a run in flight keeps its own
+    PostParams params{DefaultPostParams::paf_thresh, DefaultPostParams::paf_samples, DefaultPostParams::paf_min_above,
+                      DefaultPostParams::min_parts, DefaultPostParams::min_person_score};
 };
 
 namespace {
@@ -1240,15 +1244,25 @@ void b200pose_post_destroy(b200pose_post* p) {
     delete p;
 }
 
-// After the limbs kernel was enqueued on `st`: assembly + result copies on the second stream.
-static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st) {
+// The settings a run launches with: null (the kernels compiled with the reference's constants) when they are the
+// defaults, so default runs execute exactly the kernels they always did.
+static const PostParams* run_params(const b200pose_post* p) {
+    const PostParams& q = p->params;
+    const bool dflt = q.paf_thresh == DefaultPostParams::paf_thresh && q.paf_samples == DefaultPostParams::paf_samples &&
+                      q.paf_min_above == DefaultPostParams::paf_min_above && q.min_parts == DefaultPostParams::min_parts &&
+                      q.min_person_score == DefaultPostParams::min_person_score;
+    return dflt ? nullptr : &q;
+}
+
+// After the limbs kernel was enqueued on `st`: assembly + result copies on the second stream.  prm: as for post_limbs.
+static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st, const PostParams* prm) {
     CU(cudaEventRecord(p->ev_limbs, st));
     CU(cudaStreamWaitEvent(p->s2, p->ev_limbs, 0));
     const int b = (int)(p->runs & 1);
     // the assembly kernel writes the person rows straight into this run's pinned host slot (unified addressing): only the
     // rows that exist cross PCIe, instead of a copy of the full-capacity buffer (4.8 MB per step at batch 32)
     p->pb.humans_out = p->hp_humans[b];
-    cudaError_t e = post_assemble(p->pb, n, p->s2);
+    cudaError_t e = post_assemble(p->pb, n, p->s2, prm);
     if (e != cudaSuccess) return fail("post_assemble: %s", cudaGetErrorString(e));
     ++g_launches;
     CU(cudaEventRecord(p->ev_asm, p->s2));
@@ -1297,22 +1311,23 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
     // wait for the event recorded after those copies
     if (p->runs > 0) CU(cudaStreamWaitEvent(ps, p->ev_fetch[(p->runs - 1) & 1], 0));
     cudaError_t e;
+    const PostParams* prm = run_params(p);
     if (layout == 0) {
         e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, (long)h * w, w, 1, h, w, thresh, ps, ext);
         if (e != cudaSuccess) return fail("post_peaks: %s", cudaGetErrorString(e));
-        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps, ext);
+        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps, ext, prm);
     } else {
         if (ext) return fail("post_run: ragged batches need the planar (layout 0) maps");
         e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, 1, (long)w * 19, 19, h, w, thresh, ps);
         if (e != cudaSuccess) return fail("post_peaks: %s", cudaGetErrorString(e));
-        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * 8, w, h, ps);
+        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * 8, w, h, ps, nullptr, prm);
     }
     if (e != cudaSuccess) return fail("post_limbs: %s", cudaGetErrorString(e));
     g_launches += 2;
     CU(cudaEventRecord(p->ev_ld[slot], ps));
     p->have_ld[slot] = true;
     p->hw_h = h; p->hw_w = w;
-    return enqueue_assemble_and_fetch(p, n, ps);
+    return enqueue_assemble_and_fetch(p, n, ps, prm);
 }
 
 int b200pose_post_run(b200pose_post* p, const float* heat, const float* paf, int on_device, int layout, int n, int h,
@@ -1330,6 +1345,33 @@ int b200pose_post_run(b200pose_post* p, const float* heat, const float* paf, int
         dh = p->d_heat.p; dp = p->d_paf.p;
     }
     return post_run_dev(p, dh, dp, layout, n, h, w, thresh, st);
+}
+
+int b200pose_post_default_params(b200pose_post_params* out) {
+    if (!out) return fail("post_default_params: null pointer");
+    *out = b200pose_post_params{DefaultPostParams::paf_thresh, DefaultPostParams::paf_samples,
+                                DefaultPostParams::paf_min_above, DefaultPostParams::min_parts,
+                                DefaultPostParams::min_person_score};
+    return 0;
+}
+
+int b200pose_post_set_params(b200pose_post* p, const b200pose_post_params* in) {
+    if (!p) return fail("null post");
+    b200pose_post_params q;
+    if (in) q = *in;
+    else b200pose_post_default_params(&q);
+    const PostParams v{q.paf_thresh, q.paf_samples, q.paf_min_above, q.min_parts, q.min_person_score};
+    char msg[160];
+    if (!post_params_check(v, msg, sizeof(msg))) return fail("post params: %s", msg);
+    p->params = v;
+    return 0;
+}
+
+int b200pose_post_get_params(b200pose_post* p, b200pose_post_params* out) {
+    if (!p || !out) return fail("post_get_params: null pointer");
+    const PostParams& q = p->params;
+    *out = b200pose_post_params{q.paf_thresh, q.paf_samples, q.paf_min_above, q.min_parts, q.min_person_score};
+    return 0;
 }
 
 long b200pose_post_last_ticket(b200pose_post* p) { return p ? p->runs - 1 : -1; }
@@ -1985,10 +2027,11 @@ int process_paf(int p1, int p2, int p3, float* peaks, int h1, int h2, int h3, fl
     CU(cudaMemcpyAsync(pb.peak_s, hs.data(), hs.size() * 4, cudaMemcpyHostToDevice, st));
     CU(p->d_paf.ensure((size_t)f1 * f2 * f3));
     CU(cudaMemcpyAsync(p->d_paf.p, pafmap, (size_t)f1 * f2 * f3 * 4, cudaMemcpyHostToDevice, st));
+    // the reference's drop-in keeps the reference's constants (g_legacy's settings are never changed either)
     cudaError_t e = post_limbs(pb, 1, p->d_paf.p, 0, 1, (long)f2 * f3, f3, 0, h1, f2, f1, st);
     if (e != cudaSuccess) return fail("post_limbs: %s", cudaGetErrorString(e));
     ++g_launches;
-    if (enqueue_assemble_and_fetch(p, 1, st)) return 3;
+    if (enqueue_assemble_and_fetch(p, 1, st, nullptr)) return 3;
     if (b200pose_post_sync(p)) return 3;
     if (p->hp_status[p->cur][0] & 0xff & ~16) return fail("process_paf: capacity exceeded (status %d)", p->hp_status[p->cur][0]);
     g_leg_nh = p->hp_nh[p->cur][0];

@@ -164,9 +164,11 @@ struct PlanePaf {          // the limb's two PAF planes in shared memory: channe
     __device__ __forceinline__ float at(int c, int y, int x) const { return pl[c * hw + (y >> 3) * lw + (x >> 3)]; }
 };
 
+// Prm: DefaultPostParams (the instantiation of default runs) or PostParams (run-time settings, post_limbs)
+template <class Prm>
 __global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers pb, PafView paf0, long p_img, int h_up0,
                                                                    int lw, int lh, int paf_in_smem, int n_limbs,
-                                                                   const int* __restrict__ ext) {
+                                                                   const int* __restrict__ ext, Prm prm) {
     extern __shared__ float s_planes[];
     __shared__ int s_item;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -236,8 +238,8 @@ __global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers p
                 bool pass = false;
                 if (p < npairs) {
                     const int ax = __ldg(axp + a), ay = __ldg(ayp + a), bx = __ldg(bxp + b), by = __ldg(byp + b);
-                    pass = paf_in_smem ? pair_score_t(pp, 0, 1, ax, ay, bx, by, h_up, &sc)
-                                       : pair_score_t(paf, c1, c2, ax, ay, bx, by, h_up, &sc);
+                    pass = paf_in_smem ? pair_score_t(pp, 0, 1, ax, ay, bx, by, h_up, prm, &sc)
+                                       : pair_score_t(paf, c1, c2, ax, ay, bx, by, h_up, prm, &sc);
                 }
                 const unsigned m = __ballot_sync(0xffffffffu, pass);
                 if (pass) dst[cnt + __popc(m & lt)] = cand_key(sc, (uint32_t)p);
@@ -810,7 +812,7 @@ __global__ void __launch_bounds__(kGreedyThreads) limb_greedy_kernel(PostBuffers
     } while (0)
 
 cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long p_img, long p_ch, long p_y, long p_x,
-                       int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext) {
+                       int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext, const PostParams* prm) {
     if (batch > pb.batch_cap) return cudaErrorInvalidValue;
     if (pb.cand_smem_cap != kS) return cudaErrorInvalidValue;
     PafView pv{paf, p_ch, p_y, p_x, shift};
@@ -822,12 +824,19 @@ cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long 
         in_smem = 1;
         smem = (size_t)2 * lw * lh * sizeof(float);
     }
-    static DynSmemOptIn optin_score, optin_sort;
-    B2P_TRY(optin_score.ensure(limb_score_kernel, smem));
+    static DynSmemOptIn optin_score, optin_score_p, optin_sort;
     int dev = 0, sms = 132;
     B2P_TRY(cudaGetDevice(&dev));
     B2P_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb, ext);
+    if (!prm) {
+        B2P_TRY(optin_score.ensure(limb_score_kernel<DefaultPostParams>, smem));
+        limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
+                                                               ext, DefaultPostParams{});
+    } else {
+        B2P_TRY(optin_score_p.ensure(limb_score_kernel<PostParams>, smem));
+        limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
+                                                               ext, *prm);
+    }
     B2P_TRY(cudaGetLastError());
     limb_gather_kernel<<<dim3(batch, kNumLimb), kGatherThreads, 0, s>>>(pb);
     B2P_TRY(cudaGetLastError());

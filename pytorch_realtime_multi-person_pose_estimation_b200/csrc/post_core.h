@@ -14,6 +14,7 @@
 #define B2P_HD inline
 #include <math.h>
 #endif
+#include <stdio.h>
 
 namespace b2p {
 
@@ -57,40 +58,84 @@ struct PafView {
 // the FP64 conversion pipe (20 conversions per candidate pair).
 B2P_HD int round_half_up(float v) { return v == 0x1.fffffep-2f ? 0 : (int)f_add(v, 0.5f); }
 
+// The five settings of pair scoring and the prune, pafprocess.h:7-13.  PostParams carries them at run time (kernel
+// arguments by value, so every run keeps the values it was submitted with); DefaultPostParams is the reference's
+// constants as compile-time values, the instantiation every default run executes, with the sample loop fully unrolled.
+struct PostParams {
+    float paf_thresh;        // THRESH_VECTOR_SCORE: a PAF sample counts if vec . paf > paf_thresh
+    int paf_samples;         // STEP_PAF: samples along a candidate limb, 1 .. kMaxPafSamples
+    int paf_min_above;       // THRESH_VECTOR_CNT1: keep a pair iff more than this many samples count
+    int min_parts;           // THRESH_PART_CNT: drop a person with fewer parts
+    float min_person_score;  // THRESH_HUMAN_SCORE: drop a person whose score / parts is lower
+};
+struct DefaultPostParams {
+    static constexpr float paf_thresh = 0.05f;
+    static constexpr int paf_samples = kStepPaf;
+    static constexpr int paf_min_above = 6;
+    static constexpr int min_parts = 4;
+    static constexpr float min_person_score = 0.3f;
+};
+constexpr int kMaxPafSamples = 64;
+
+// Range check of run-time settings (host): true if valid, else false with the first field out of range, its value and
+// its range in msg.
+inline bool post_params_check(const PostParams& q, char* msg, int cap) {
+    if (!isfinite(q.paf_thresh)) return snprintf(msg, cap, "paf_thresh must be finite, got %g", (double)q.paf_thresh), false;
+    if (q.paf_samples < 1 || q.paf_samples > kMaxPafSamples)
+        return snprintf(msg, cap, "paf_samples must be 1 .. %d, got %d", kMaxPafSamples, q.paf_samples), false;
+    if (q.paf_min_above < -1 || q.paf_min_above > q.paf_samples)
+        return snprintf(msg, cap, "paf_min_above must be -1 .. paf_samples (%d), got %d", q.paf_samples, q.paf_min_above),
+               false;
+    if (q.min_parts < 0 || q.min_parts > kNumPart)
+        return snprintf(msg, cap, "min_parts must be 0 .. %d, got %d", kNumPart, q.min_parts), false;
+    if (!isfinite(q.min_person_score))
+        return snprintf(msg, cap, "min_person_score must be finite, got %g", (double)q.min_person_score), false;
+    return true;
+}
+
 // Scores one (a, b) peak pair of a limb.  Returns true and the candidate score if it passes both criteria.
 // `Paf` is any accessor with `float at(int c, int y, int x) const` (PafView, or the shared-memory planes of the scoring
-// kernel).  Restated from pafprocess.cpp:57-94 operation for operation, with two EXACT simplifications of its double
-// precision parts (both proven below and pinned by the host tests against the compiled reference):
+// kernel); `Prm` is PostParams or DefaultPostParams.  Restated from pafprocess.cpp:57-94 operation for operation, with
+// two EXACT simplifications of its double precision parts (both proven below and pinned by the host tests against the
+// compiled reference):
 //   * `norm < 1e-12` (double):  norm = sqrt(dx^2 + dy^2) of integer dx, dy is 0 or >= 1, so the test is `norm == 0`.
-//   * the length penalty  pen = 0.5*h_up/norm - 1.0 (double), crit2 = (float)((double)(scores/10) + min(pen, 0)):
+//   * the length penalty  pen = 0.5*h_up/norm - 1.0 (double), crit2 = (float)((double)(scores/n) + min(pen, 0)):
 //     q = fl(0.5*h_up/norm) < 1  <=>  norm > 0.5*h_up, because 1 - 0.5*h_up/norm is either <= 0 or >= 2^-25 (norm is a
 //     float, 0.5*h_up a multiple of 0.5 below 2^24), far from the 2^-54 rounding boundary below 1; and q - 1.0 is exact
-//     (Sterbenz).  So without penalty crit2 is (float)(double)(scores/10) = scores/10 itself, and the double expression
+//     (Sterbenz).  So without penalty crit2 is (float)(double)(scores/n) = scores/n itself, and the double expression
 //     is evaluated only for pairs longer than half the image height.
-template <class Paf>
-B2P_HD bool pair_score_t(const Paf& paf, int c1, int c2, int ax, int ay, int bx, int by, int h_up, float* score_out) {
+// Neither argument depends on the settings.  The penalty argument involves only norm and h_up.  round_half_up is exact
+// for 0 <= v <= 16384, and v = fl(a + fl(i * fl(d / n))), 0 <= i < n, lies within a few ulps of the segment between the
+// two peaks' coordinates a and a + d for every sample count n: it is in that range whenever the peaks are, and every
+// sample lands on a pixel between the two peaks, inside the map.  The thresholds only enter the compares
+// `s > paf_thresh` (float) and `crit1 > paf_min_above` (int), which the reference makes in the same types.
+template <class Paf, class Prm>
+B2P_HD bool pair_score_t(const Paf& paf, int c1, int c2, int ax, int ay, int bx, int by, int h_up, const Prm& prm,
+                         float* score_out) {
     const int dxi = bx - ax, dyi = by - ay;
     float vx = (float)dxi, vy = (float)dyi;
     const float norm = f_sqrt(f_add(f_mul(vx, vx), f_mul(vy, vy)));
     if (!(norm > 0.f)) return false;
     vx = f_div(vx, norm);
     vy = f_div(vy, norm);
-    const float step_x = f_div((float)dxi, (float)kStepPaf);
-    const float step_y = f_div((float)dyi, (float)kStepPaf);
+    const int n = prm.paf_samples;
+    const float step_x = f_div((float)dxi, (float)n);
+    const float step_y = f_div((float)dyi, (float)n);
     float scores = 0.0f;
     int crit1 = 0;
+    // unrolled for the compile-time count; a run-time count (PostParams) keeps a rolled loop of at most kMaxPafSamples
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-    for (int i = 0; i < kStepPaf; ++i) {
+    for (int i = 0; i < n; ++i) {
         const int lx = round_half_up(f_add((float)ax, f_mul((float)i, step_x)));
         const int ly = round_half_up(f_add((float)ay, f_mul((float)i, step_y)));
         const float s = f_add(f_mul(vx, paf.at(c1, ly, lx)), f_mul(vy, paf.at(c2, ly, lx)));
         scores = f_add(scores, s);
-        if (s > 0.05f) crit1 += 1;
+        if (s > prm.paf_thresh) crit1 += 1;
     }
-    if (crit1 <= 6) return false;
-    float crit2 = f_div(scores, (float)kStepPaf);
+    if (crit1 <= prm.paf_min_above) return false;
+    float crit2 = f_div(scores, (float)n);
     if (norm > 0.5f * (float)h_up) {
         const double pen = 0.5 * h_up / (double)norm - 1.0;
         crit2 = (float)((double)crit2 + pen);
@@ -102,7 +147,7 @@ B2P_HD bool pair_score_t(const Paf& paf, int c1, int c2, int ax, int ay, int bx,
     return false;
 }
 B2P_HD bool pair_score(const PafView& paf, int c1, int c2, int ax, int ay, int bx, int by, int h_up, float* score_out) {
-    return pair_score_t(paf, c1, c2, ax, ay, bx, by, h_up, score_out);
+    return pair_score_t(paf, c1, c2, ax, ay, bx, by, h_up, DefaultPostParams{}, score_out);
 }
 
 // Candidate key: high 32 bits = ~bits(score) (score > 0, so ascending key == descending score), low 32 bits =
@@ -720,12 +765,15 @@ struct Assembler {
             ++nrows;
         }
     }
-    // prune (pafprocess.cpp:187-191): keep rows with count >= 4 and score/count >= 0.3
-    B2P_HD bool keep(int r) const {
+    // prune (pafprocess.cpp:187-191): keep rows with count >= min_parts and score/count >= min_person_score (the
+    // reference's float compares; its int THRESH_PART_CNT converts to float)
+    template <class Prm>
+    B2P_HD bool keep(int r, const Prm& prm) const {
         if (!alive[r]) return false;
         const float* row = rows + r * kRowFloats;
-        return !(row[19] < 4.f || f_div(row[18], row[19]) < 0.3f);
+        return !(row[19] < (float)prm.min_parts || f_div(row[18], row[19]) < prm.min_person_score);
     }
+    B2P_HD bool keep(int r) const { return keep(r, DefaultPostParams{}); }
 };
 
 }  // namespace b2p

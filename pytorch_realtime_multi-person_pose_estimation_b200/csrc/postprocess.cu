@@ -276,7 +276,9 @@ __global__ void __launch_bounds__(kPeakThreads, 512 / kPeakThreads) peaks_kernel
 }
 
 // ------------------------------------------------------------------ assembly
-__global__ void __launch_bounds__(kAsmThreads) assemble_kernel(PostBuffers pb) {
+// Prm: DefaultPostParams (the instantiation of default runs) or PostParams (run-time prune settings, post_assemble)
+template <class Prm>
+__global__ void __launch_bounds__(kAsmThreads) assemble_kernel(PostBuffers pb, Prm prm) {
     extern __shared__ int sm_kept[];     // [human_cap]
     __shared__ int part_base[kNumPart + 1];
     __shared__ int s_nh, s_nrows;
@@ -357,7 +359,7 @@ __global__ void __launch_bounds__(kAsmThreads) assemble_kernel(PostBuffers pb) {
         Assembler& as = s_as;
         int nh = 0, st = 0;
         for (int r = 0; r < as.nrows; ++r)
-            if (as.keep(r)) {
+            if (as.keep(r, prm)) {
                 if (nh < pb.human_cap) sm_kept[nh++] = r;
                 else st |= 8;
             }
@@ -463,9 +465,10 @@ cudaError_t post_peaks(const PostBuffers& pb, int batch, const float* heat, long
     return cudaGetLastError();
 }
 
-cudaError_t post_assemble(const PostBuffers& pb, int batch, cudaStream_t s) {
+cudaError_t post_assemble(const PostBuffers& pb, int batch, cudaStream_t s, const PostParams* prm) {
     if (batch > pb.batch_cap) return cudaErrorInvalidValue;
-    assemble_kernel<<<batch, kAsmThreads, pb.human_cap * sizeof(int), s>>>(pb);
+    if (!prm) assemble_kernel<<<batch, kAsmThreads, pb.human_cap * sizeof(int), s>>>(pb, DefaultPostParams{});
+    else assemble_kernel<<<batch, kAsmThreads, pb.human_cap * sizeof(int), s>>>(pb, *prm);
     return cudaGetLastError();
 }
 

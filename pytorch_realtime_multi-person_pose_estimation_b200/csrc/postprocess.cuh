@@ -84,14 +84,17 @@ cudaError_t post_peaks(const PostBuffers& pb, int batch, const float* heat, long
                        int h, int w, float thresh, cudaStream_t s, const int* ext = nullptr);
 // paf: fp32 view per image: base + img*p_img, strides (p_ch, p_y, p_x), shift (3: low-res, 0: already upsampled).
 // ext (ragged batch) or null: h_up of image i is its own padded height ext[2 i].
+// prm: the scoring settings, copied into the launch; null = the reference's constants (the DefaultPostParams kernel).
 cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long p_img, long p_ch, long p_y,
-                                    long p_x, int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext = nullptr);
+                                    long p_x, int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext = nullptr,
+                                    const PostParams* prm = nullptr);
 // Test hook (limbs.cu): exact std::sort of n host keys through the global-memory partition + shared-memory range kernels.
 cudaError_t post_debug_sort(const PostBuffers& pb, const unsigned long long* keys, int n, unsigned long long* out,
                             cudaStream_t s);
 // Person assembly of the connections post_limbs() left in `pb`.  Small footprint (128 threads, human_cap*4 B smem per
 // image): it can run on a second stream next to the convolutions of the following batch.
-cudaError_t post_assemble(const PostBuffers& pb, int batch, cudaStream_t s);
+// prm: the prune settings, as for post_limbs.
+cudaError_t post_assemble(const PostBuffers& pb, int batch, cudaStream_t s, const PostParams* prm = nullptr);
 // lw x lh: dimensions of the low-resolution PAF planes (used to stage them in shared memory when shift == 3)
 
 }  // namespace b2p

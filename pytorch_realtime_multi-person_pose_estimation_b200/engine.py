@@ -247,6 +247,28 @@ class NativePost:
                   "b200pose_post_create")
         self.batch_cap, self.peak_cap, self.human_cap = batch_cap, peak_cap, human_cap
 
+    def set_params(self, **fields):
+        """Settings of PAF scoring and the person prune for the runs submitted from now on (fused runs included):
+        paf_thresh, paf_samples, paf_min_above, min_parts, min_person_score (include/b200pose.h section 2).  Fields not
+        given take their defaults, so set_params() restores the reference's constants.  A value outside its range
+        raises B200PoseError naming the field and leaves the settings unchanged."""
+        q = nat.PostParams()
+        nat.check(nat.lib().b200pose_post_default_params(ctypes.byref(q)), "b200pose_post_default_params")
+        names = [name for name, _ in nat.PostParams._fields_]
+        for k, v in fields.items():
+            if k not in names:
+                raise nat.B200PoseError("set_params: unknown field %r (one of %s)" % (k, ", ".join(names)))
+            if isinstance(getattr(q, k), int) and (int(v) != v or not -2 ** 31 <= v < 2 ** 31):   # ctypes would wrap
+                raise nat.B200PoseError("set_params: %s must be a 32-bit integer, got %r" % (k, v))
+            setattr(q, k, v)
+        nat.check(nat.lib().b200pose_post_set_params(self._h, ctypes.byref(q)), "b200pose_post_set_params")
+
+    def params(self):
+        """The settings the next run uses, as a dict of set_params' fields."""
+        q = nat.PostParams()
+        nat.check(nat.lib().b200pose_post_get_params(self._h, ctypes.byref(q)), "b200pose_post_get_params")
+        return q.as_dict()
+
     def run(self, heat_ptr, paf_ptr, on_device, layout, n, h, w, thresh, stream=0):
         nat.check(nat.lib().b200pose_post_run(self._h, ctypes.c_void_p(heat_ptr), ctypes.c_void_p(paf_ptr), int(on_device),
                                               layout, n, h, w, ctypes.c_float(thresh), ctypes.c_void_p(stream)),
@@ -337,6 +359,19 @@ class NativePost:
             pass
 
 
+def post_params_from_cfg(cfg):
+    """The post-processing settings of a reference config: cfg.TEST.THRESH_PAF and
+    cfg.TEST.NUM_INTERMED_PTS_BETWEEN_KEYPOINTS on top of the defaults (the reference declares both keys but its
+    pafprocess ignores them).  paf_min_above keeps its default 6, so fewer than 7 samples need it set explicitly.
+    For NativePost.set_params(**d) or PoseEngine(post_params=d)."""
+    q = nat.PostParams()
+    nat.check(nat.lib().b200pose_post_default_params(ctypes.byref(q)), "b200pose_post_default_params")
+    d = q.as_dict()
+    d["paf_thresh"] = float(np.float32(cfg.TEST.THRESH_PAF))
+    d["paf_samples"] = int(cfg.TEST.NUM_INTERMED_PTS_BETWEEN_KEYPOINTS)
+    return d
+
+
 def humans_to_dicts(rows, width, height):
     """[(score, {part: (x/width, y/height, peak score)})] - the content paf_to_pose_cpp puts into Human objects.
     Conversions are done in bulk (float32 -> Python float, i.e. double, then the divisions in double exactly like the
@@ -361,12 +396,14 @@ def humans_to_dicts(rows, width, height):
 
 class PoseEngine:
     """Fused batched inference on one GPU: images -> humans, maps never leave the device.  `stages`: the refinement
-    stages each submission runs (1 .. 6); the fused entry points post-process the last one's maps."""
+    stages each submission runs (1 .. 6); the fused entry points post-process the last one's maps.  `post_params`: the
+    post-processing settings of the submissions (a dict of NativePost.set_params' fields; None: the reference's
+    constants), changed later with set_post_params."""
 
     stages = 6
 
     def __init__(self, state_arrays, device_index=0, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, net=None,
-                 stages=6):
+                 stages=6, post_params=None):
         if net is None:
             net = NativeNet(device_index)
             net.load_state_dict_arrays(state_arrays)
@@ -374,6 +411,8 @@ class PoseEngine:
         self.stages = int(stages)
         self.net.set_stages(self.stages)      # an invalid count fails here, before any submission
         self.post = NativePost(device_index, batch_cap, peak_cap, human_cap)
+        if post_params:
+            self.post.set_params(**post_params)
         self.mode = nat.MODES[mode]
         self.device_index = device_index
         self._shapes = {}
@@ -384,6 +423,11 @@ class PoseEngine:
         module (rtpose_model.pose_engine), so the count is set before every submission."""
         self.net.set_stages(self.stages)
         return self.net._h
+
+    def set_post_params(self, params=None, **fields):
+        """Post-processing settings of the following submissions (a dict such as post_params_from_cfg's, and / or
+        fields; see NativePost.set_params).  Runs already submitted keep theirs."""
+        self.post.set_params(**dict(params or {}, **fields))
 
     def _remember(self, n, H, W):
         """Shape of the run just submitted, kept per ticket (two runs may be in flight with different batch sizes or
@@ -406,9 +450,10 @@ class PoseEngine:
         return self._shapes[ticket]
 
     @classmethod
-    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=6):
+    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=6, post_params=None):
         """An engine around an existing NativeNet (e.g. the one a get_model() module already packed its weights into)."""
-        return cls(None, net.device_index, mode, batch_cap, peak_cap, human_cap, net=net, stages=stages)
+        return cls(None, net.device_index, mode, batch_cap, peak_cap, human_cap, net=net, stages=stages,
+                   post_params=post_params)
 
     def submit_images(self, images, dest_size=368, factor=8, thresh=0.1, flip=False):
         """Asynchronous half of infer_images for frames of ONE shape (a video stream): returns a ticket; the frames must
