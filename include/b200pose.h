@@ -1,7 +1,8 @@
 /* b200pose - C ABI of the H100-native OpenPose (rtpose VGG19) inference path.
  *
  * Plain pointers and sizes only; no torch / numpy types.  Every entry point returns 0 on success and a
- * non-zero code on failure (b200pose_last_error() gives the text) unless stated otherwise.
+ * non-zero code on failure (b200pose_last_error() gives the text) unless stated otherwise.  A failed call leaves no
+ * CUDA error pending for later calls, and the objects it was given stay usable.
  *
  * Threading: b200pose_last_error() is per thread; a net / post object and the legacy process_paf surface serialise
  * nothing themselves - use one object per host thread (or your own lock).  All work of a call is enqueued on the

@@ -9,10 +9,12 @@
 #include <cstring>
 #include <list>
 #include <map>
+#include <memory>
 #include <set>
 #include <mutex>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200pose.h"
@@ -41,15 +43,21 @@ int fail(const char* fmt, ...) {
     g_err = buf;
     return 1;
 }
+// fail() for a CUDA call that failed: also clears the thread's last CUDA error, which the launch wrappers report
+// (cudaGetLastError), so that the error does not fail a later call.  Sticky errors cannot be cleared.
+template <class... A> int cuda_fail(const char* fmt, A... args) {
+    cudaGetLastError();
+    return fail(fmt, args...);
+}
 #define CU(x)                                                                                       \
     do {                                                                                            \
         cudaError_t e_ = (x);                                                                       \
-        if (e_ != cudaSuccess) return fail("%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
+        if (e_ != cudaSuccess) return cuda_fail("%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
     } while (0)
 
 // Counts the launches of a kernel wrapper that returned e.
 int launched(cudaError_t e, const char* what, int launches = 1) {
-    if (e != cudaSuccess) return fail("%s: %s", what, cudaGetErrorString(e));
+    if (e != cudaSuccess) return cuda_fail("%s: %s", what, cudaGetErrorString(e));
     g_launches += launches;
     return 0;
 }
@@ -116,14 +124,17 @@ float bf2f(uint16_t b) {
     return f;
 }
 
-template <class T> struct DevBuf {
+// Owners of the CUDA resources of the net and post objects: each releases what it holds when it is destroyed, so that a
+// call that fails part-way leaks nothing.  Move-only.
+template <class T> struct DevBuf {      // device memory
     T* p = nullptr;
     size_t n = 0;
-    cudaError_t ensure(size_t count) {
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), n(std::exchange(o.n, 0)) {}
+    ~DevBuf() { release(); }
+    cudaError_t ensure(size_t count) {  // room for count elements: a larger request frees the old buffer first
         if (count <= n) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        n = 0;
+        release();
         cudaError_t e = cudaMalloc(&p, count * sizeof(T));
         if (e == cudaSuccess) n = count;
         return e;
@@ -131,25 +142,37 @@ template <class T> struct DevBuf {
     void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
 
+template <class T> struct HostBuf {     // pinned host memory
+    T* p = nullptr;
+    HostBuf() = default;
+    HostBuf(HostBuf&& o) noexcept : p(std::exchange(o.p, nullptr)) {}
+    ~HostBuf() { if (p) cudaFreeHost(p); }
+    cudaError_t alloc(size_t count, unsigned flags) { return cudaHostAlloc(&p, count * sizeof(T), flags); }   // once
+};
+
+template <class H, cudaError_t (*Destroy)(H)> struct Handle {     // created through &h; reads as the raw handle
+    H h = nullptr;
+    Handle() = default;
+    Handle(Handle&& o) noexcept : h(std::exchange(o.h, nullptr)) {}
+    ~Handle() { if (h) Destroy(h); }
+    operator H() const { return h; }
+};
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using GraphExec = Handle<cudaGraphExec_t, cudaGraphExecDestroy>;
+
 struct TcLayer {            // one grouped tensor-core launch
     int ks, cin_blocks, groups, n_tile, n_tiles, relu, pool;
     double macs_per_pixel = 0;    // algorithmic (unpadded) MACs per output pixel, all groups
-    float* bias = nullptr;        // [groups*n_tiles*n_tile]
+    DevBuf<float> bias;           // [groups*n_tiles*n_tile]
     std::vector<int> convs;       // state-dict conv per group
     bool cat_input = false;       // reads the concat buffer (input channels permuted, cat_phys)
     // packed weights per encoding (TcWeights, tc_format.h), rows groups*n_tiles*n_tile of cin_blocks*64 channels; see
     // ensure_packed for when each is packed
-    void* w[kNumTcWeights] = {};
-    int* w_exp = nullptr;         // e4m3: ew per row (device)
+    DevBuf<unsigned char> w[kNumTcWeights];
+    DevBuf<int> w_exp;            // e4m3: ew per row (device)
     std::vector<int> h_w_exp;     // ... and its host copy (b200pose_net_debug_fp8)
 };
-
-void free_tc_layer(TcLayer& L) {
-    for (void* w : L.w)
-        if (w) cudaFree(w);
-    if (L.bias) cudaFree(L.bias);
-    if (L.w_exp) cudaFree(L.w_exp);
-}
 
 // Activation buffers (the buffer ids of the test hooks): channels per pixel and spatial divisor.
 enum Act { T1, T2, T3, T4, T5A, T5B, T6, T7, T8, T9, CAT, BRA, BRB, BR512, kNumAct };
@@ -236,8 +259,7 @@ struct b200pose_net {
     bool finalized = false;
     std::vector<std::vector<float>> host_w, host_b;   // per conv
     std::vector<bool> have;                            // per tensor
-    float* d_w[kNumConvs] = {};                        // fp32 OIHW (parity mode, conv1_1)
-    float* d_b[kNumConvs] = {};
+    DevBuf<float> d_w[kNumConvs], d_b[kNumConvs];      // fp32 OIHW (parity mode, conv1_1)
     // tensor-core layers: trunk 1..11 -> tc[0..10]; stage 1: tc[11..15]; stage t>=2: tc[16 + (t-2)*7 + li]
     std::vector<TcLayer> tc;
     // Plans of the last 32 keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not re-encode
@@ -250,7 +272,7 @@ struct b200pose_net {
     // (0) launch directly.
     using GraphKey = std::tuple<int, int, int, TcFormat, int, int, bool, const void*>;   // n, H, W, format, stages, in_u8, ragged, input
     bool use_graph = true;
-    std::map<GraphKey, cudaGraphExec_t> graphs;
+    std::map<GraphKey, GraphExec> graphs;
     std::set<GraphKey> graph_seen;    // a key is captured at its SECOND use: callers that pass a fresh pointer every time never pay a capture
     // bf16 (fp16: binary16) activation buffers by Act id, and their residual ("lo") planes (bf16x3 only)
     DevBuf<__nv_bfloat16> act[kNumAct], act_lo[kNumAct];
@@ -265,7 +287,7 @@ struct b200pose_net {
     // Ragged batches (DESIGN.md §1): the extents table [H_0, W_0, H_1, W_1, ...] every kernel of a ragged forward reads.
     // Allocated once for kMaxRagged images and never moved, so that plans and captured graphs stay valid across mixes;
     // rewritten on the stream before each ragged forward.
-    int* d_ext = nullptr;
+    DevBuf<int> d_ext;
     DevBuf<RaggedFrame> d_frames;      // per-frame source geometry of the last ragged crop
     // video frames (b200pose_net_convert_frames, b200pose_infer_frames): the planes of host frames, packed, and the
     // source table of the last conversion
@@ -278,6 +300,7 @@ struct b200pose_net {
     // fp16 mode: ovf[image] = 1 when a launch stored a value beyond binary16's range for the image; zeroed at the start
     // of every fp16 forward
     DevBuf<unsigned> ovf;
+    ~b200pose_net() { graphs.clear(); }     // the graph execs go before the buffers they point into
 };
 
 struct b200pose_post {
@@ -287,14 +310,12 @@ struct b200pose_post {
     DevBuf<float> tta_in, tta_out;   // b200pose_flip_merge staging for host pointers
     // Results are copied to pinned host memory by the run itself (second stream, right after the assembly) into one
     // of two slots selected by the run's parity, so the host can fetch run i while run i+1 is in flight.
-    cudaStream_t s2 = nullptr;
-    cudaEvent_t ev_limbs = nullptr, ev_asm = nullptr, ev_fetch[2] = {nullptr, nullptr};
+    Stream s2;
+    Event ev_limbs, ev_asm, ev_fetch[2];
     long runs = 0;                  // runs submitted so far; ticket of the latest = runs - 1
     int slot_n[2] = {0, 0};
-    int* hp_nh[2] = {nullptr, nullptr};
-    int* hp_status[2] = {nullptr, nullptr};
-    int* hp_counts[2] = {nullptr, nullptr};
-    float* hp_humans[2] = {nullptr, nullptr};
+    HostBuf<int> hp_nh[2], hp_status[2], hp_counts[2];
+    HostBuf<float> hp_humans[2];
     int cur = 0;                    // slot the getters read
     long cur_ticket = -1;
     std::vector<float> h_px_s;
@@ -304,24 +325,26 @@ struct b200pose_post {
     // so that the caller's stream is free for the convolutions of run i+1: the small kernels (peaks, assembly) co-reside
     // with the conv CTAs and the limbs blocks fill the SMs the conv launches leave idle in their last wave.
     DevBuf<float> ov_maps[2];                      // [heat | paf] copies, slot = run parity
-    cudaEvent_t ev_maps = nullptr, ev_ld[2] = {nullptr, nullptr};   // maps copied (st) / limbs done with a slot (s2)
+    Event ev_maps, ev_ld[2];                       // maps copied (st) / limbs done with a slot (s2)
     bool have_ld[2] = {false, false};
     // extents of a ragged run, slot = run parity: the peaks / limbs of run i on the second stream still read them while
     // run i+1 rewrites the net's table
-    int* d_ext[2] = {nullptr, nullptr};
+    DevBuf<int> d_ext[2];
     // ragged multi-scale averaging: the frames' base extents (the net's table holds the last scale's) and the resize
     // geometry of every (scale, frame)
     DevBuf<int> ms_ext;
     DevBuf<RaggedResize> ms_resize;
     // fp16 overflow flags of the fused runs, slot = run parity: one row of 2 * batch_cap images per forward of the run (a
     // multi-scale run makes one forward per scale), copied from the net's flags behind each forward
-    unsigned* hp_ovf[2] = {nullptr, nullptr};
+    HostBuf<unsigned> hp_ovf[2];
     int ovf_rows[2] = {0, 0}, ovf_imgs[2] = {0, 0};    // forwards copied, images per forward (2n with flip)
     int ovf_pending = 0, ovf_pending_imgs = 0;          // ... of the run being enqueued
     // scoring / prune settings of the runs submitted from now on (b200pose_post_set_params); they travel to the kernels
     // by value, so a run in flight keeps its own
     PostParams params{DefaultPostParams::paf_thresh, DefaultPostParams::paf_samples, DefaultPostParams::paf_min_above,
                       DefaultPostParams::min_parts, DefaultPostParams::min_person_score};
+    // the second stream's work still reads the buffers; post_free is null-safe (post_alloc zeroes pb first)
+    ~b200pose_post() { if (s2) cudaStreamSynchronize(s2); post_free(pb); }
 };
 
 namespace {
@@ -377,11 +400,11 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L) {
                 w[((size_t)(taps + t) * rows + r) * cin_pad + k] = f2bf(wf - bf2f(hi));
             }
     });
-    void*& dw = L.w[(int)TcWeights::kBf16HiLo];
-    CU(cudaMalloc(&dw, w.size() * 2));
-    CU(cudaMalloc(&L.bias, b.size() * 4));
-    CU(cudaMemcpy(dw, w.data(), w.size() * 2, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(L.bias, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
+    DevBuf<unsigned char>& dw = L.w[(int)TcWeights::kBf16HiLo];
+    CU(dw.ensure(w.size() * 2));
+    CU(L.bias.ensure(b.size()));
+    CU(cudaMemcpy(dw.p, w.data(), w.size() * 2, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(L.bias.p, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -405,11 +428,11 @@ int pack_fp8_layer(const b200pose_net* net, TcLayer& L) {
             for (int k = 0; k < cin_pad; ++k) dst[k] = e4m3_rn_bits(src[(k & ~31) + fp8_k_to_channel(k & 31)] * exp2_int(ew));
         }
     });
-    void*& dw = L.w[(int)TcWeights::kE4m3];
-    CU(cudaMalloc(&dw, w8.size()));
-    CU(cudaMalloc(&L.w_exp, rows * sizeof(int)));
-    CU(cudaMemcpy(dw, w8.data(), w8.size(), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(L.w_exp, L.h_w_exp.data(), rows * sizeof(int), cudaMemcpyHostToDevice));
+    DevBuf<unsigned char>& dw = L.w[(int)TcWeights::kE4m3];
+    CU(dw.ensure(w8.size()));
+    CU(L.w_exp.ensure(rows));
+    CU(cudaMemcpy(dw.p, w8.data(), w8.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(L.w_exp.p, L.h_w_exp.data(), rows * sizeof(int), cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -436,9 +459,9 @@ int pack_f16_layer(const b200pose_net* net, TcLayer& L) {
             }
     });
     if (rc) return rc;
-    void*& dw = L.w[(int)TcWeights::kBinary16];
-    CU(cudaMalloc(&dw, w16.size() * 2));
-    CU(cudaMemcpy(dw, w16.data(), w16.size() * 2, cudaMemcpyHostToDevice));
+    DevBuf<unsigned char>& dw = L.w[(int)TcWeights::kBinary16];
+    CU(dw.ensure(w16.size() * 2));
+    CU(cudaMemcpy(dw.p, w16.data(), w16.size() * 2, cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -447,13 +470,16 @@ int pack_f16_layer(const b200pose_net* net, TcLayer& L) {
 // formats do not pay for them.
 int ensure_packed(b200pose_net* net, TcLayer& L, TcFormat fmt) {
     const TcWeights enc = tc_weights(fmt);
-    if (L.w[(int)enc] != nullptr) return 0;
+    if (L.w[(int)enc].p != nullptr) return 0;
+    int rc;
     switch (enc) {
-        case TcWeights::kBf16HiLo: return pack_tc_layer(net, L);
-        case TcWeights::kE4m3: return pack_fp8_layer(net, L);
-        case TcWeights::kBinary16: return pack_f16_layer(net, L);
+        case TcWeights::kBf16HiLo: rc = pack_tc_layer(net, L); break;
+        case TcWeights::kE4m3: rc = pack_fp8_layer(net, L); break;
+        case TcWeights::kBinary16: rc = pack_f16_layer(net, L); break;
+        default: return fail("unknown weight encoding %d", (int)enc);
     }
-    return fail("unknown weight encoding %d", (int)enc);
+    if (rc) L.w[(int)enc].release();      // a pack that failed part-way is redone by the next call
+    return rc;
 }
 
 // The per-image table of format f (tc_aux): fp8 amax rows (conv1_1, then each launch), fp16 overflow flags; null otherwise.
@@ -482,7 +508,7 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
     a.fmt = p.fmt;
     a.n_img = n; a.H = H; a.W = W; a.ksize = L.ks; a.cin_blocks = L.cin_blocks;
     a.in_ch_base = wr.in_base; a.in_ch_group_stride = wr.in_group_stride; a.groups = L.groups;
-    a.n_tile = L.n_tile; a.n_tiles = L.n_tiles; a.bias = L.bias; a.relu = L.relu; a.pool = L.pool;
+    a.n_tile = L.n_tile; a.n_tiles = L.n_tiles; a.bias = L.bias.p; a.relu = L.relu; a.pool = L.pool;
     {   // small batches: while the layer's CTAs fill at most half of the SMs, halve the work per CTA - 128-wide n-tiles become
         // 64-wide, then 32-wide (the weight layout does not depend on the n-tile)
         const int pix = n * ((H + kTileH - 1) / kTileH) * ((W + kTileW - 1) / kTileW);
@@ -496,7 +522,7 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         a.amax_out = net->amax.p + (size_t)slot * n;
         a.amax_in[0] = net->amax.p + (size_t)writers[0] * n;
         a.amax_in[1] = writers[1] >= 0 ? net->amax.p + (size_t)writers[1] * n : nullptr;
-        a.w_exp = L.w_exp;
+        a.w_exp = L.w_exp.p;
         a.ea_out = net->ea.p + (size_t)slot * n;
     }
     if (tc_aux(p.fmt) == TcAux::kOverflow) a.ovf_out = net->ovf.p;
@@ -519,8 +545,8 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         in_lo = net->act_lo[wr.in].p;
         a.out_lo = net->act_lo[wr.out].p;
     }
-    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], L.w[(int)tc_weights(p.fmt)], in_lo);
-    if (e != cudaSuccess) return fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
+    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], L.w[(int)tc_weights(p.fmt)].p, in_lo);
+    if (e != cudaSuccess) return cuda_fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
     p.launches.push_back({a, 2.0 * n * H * W * L.macs_per_pixel, wr.in, wr.out, {f32[0], f32[1]}});
     return 0;
 }
@@ -583,7 +609,6 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
 }
 
 void drop_graphs(b200pose_net* net) {
-    for (auto& kv : net->graphs) cudaGraphExecDestroy(kv.second);
     net->graphs.clear();
     net->graph_seen.clear();
 }
@@ -619,7 +644,7 @@ int select_plan(b200pose_net* net, int n, int H, int W, TcFormat fmt, int stages
 // leave it as it is - they record the same maxima and flags again.
 // after (b200pose_net_profile): after[i] is recorded behind launch i.
 int launch_forward_tc(const b200pose_net* net, const void* d_in, int in_u8, const int* ext, int k, cudaStream_t st,
-                      bool zero_aux = false, const cudaEvent_t* after = nullptr) {
+                      bool zero_aux = false, const Event* after = nullptr) {
     const Plan& p = *net->plan;
     unsigned* aux = aux_table(net, p.fmt);
     if (aux != nullptr && zero_aux) {
@@ -627,7 +652,7 @@ int launch_forward_tc(const b200pose_net* net, const void* d_in, int in_u8, cons
         CU(cudaMemsetAsync(aux, 0, rows * p.n * sizeof(unsigned), st));
     }
     if (k >= 1) {
-        CU(conv_first_launch(d_in, in_u8, net->d_w[0], net->d_b[0], p.fmt, net->act[T1].p,
+        CU(conv_first_launch(d_in, in_u8, net->d_w[0].p, net->d_b[0].p, p.fmt, net->act[T1].p,
                              tc_planes(p.fmt) == 2 ? net->act_lo[T1].p : nullptr, aux, p.n, p.H, p.W, ext, st));
         if (after) CU(cudaEventRecord(after[0], st));
     }
@@ -663,7 +688,7 @@ int forward_tc(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int
             if (rc == 0 && e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
             if (graph) cudaGraphDestroy(graph);
             if (rc == 0 && e == cudaSuccess) {
-                net->graphs.emplace(key, exec);
+                net->graphs[key].h = exec;
             } else {      // no graph (e.g. a launch attribute the capture refuses): plain launches from now on
                 cudaGetLastError();
                 fprintf(stderr, "[b200pose] CUDA graph capture of the forward pass failed (%s): launching directly\n",
@@ -698,7 +723,7 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
                     int relu, float* nchw) -> int {
         const ConvSpec s = conv_spec(ci);
         ConvF32Args a;
-        a.in = in; a.in_cstride = in_cs; a.in_ch_off = in_off; a.w = net->d_w[ci]; a.bias = net->d_b[ci];
+        a.in = in; a.in_cstride = in_cs; a.in_ch_off = in_off; a.w = net->d_w[ci].p; a.bias = net->d_b[ci].p;
         a.out = out; a.out_cstride = out_cs; a.out_ch_off = out_off; a.out_nchw = nchw;
         a.n_img = n; a.H = hh; a.W = ww; a.cin = s.cin; a.cout = s.cout; a.ks = s.ks; a.relu = relu;
         a.ext = ext;
@@ -766,7 +791,7 @@ int b200pose_net_tensor_shape(int index, long dims[4]) {
 int b200pose_net_create(b200pose_net** out, int cuda_device) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return fail("b200pose: no CUDA device available (this library has no CPU fallback)");
+        return cuda_fail("b200pose: no CUDA device available (this library has no CPU fallback)");
     CU(cudaSetDevice(cuda_device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, cuda_device));
@@ -787,22 +812,6 @@ int b200pose_net_create(b200pose_net** out, int cuda_device) {
 void b200pose_net_destroy(b200pose_net* net) {
     if (!net) return;
     cudaSetDevice(net->device);
-    drop_graphs(net);
-    for (int i = 0; i < kNumConvs; ++i) { if (net->d_w[i]) cudaFree(net->d_w[i]); if (net->d_b[i]) cudaFree(net->d_b[i]); }
-    for (TcLayer& L : net->tc) free_tc_layer(L);
-    for (int i = 0; i < kNumAct; ++i) { net->act[i].release(); net->act_lo[i].release(); }
-    net->amax.release();
-    net->ea.release();
-    net->ovf.release();
-    DevBuf<float>* fb[] = {&net->in_stage, &net->f_a, &net->f_b, &net->f_cat, &net->f_x, &net->f_y, &net->f_in, &net->f_u8};
-    net->in_stage_u8.release();
-    net->raw_stage.release();
-    net->d_frames.release();
-    net->frame_stage.release();
-    net->d_frame_src.release();
-    if (net->d_ext) cudaFree(net->d_ext);
-    for (auto* b : fb) b->release();
-    for (auto& b : net->out_f32) b.release();
     delete net;
 }
 
@@ -827,14 +836,15 @@ int b200pose_net_finalize(b200pose_net* net) {
     for (int i = 0; i < B200POSE_NUM_TENSORS; ++i)
         if (!net->have[i]) return fail("state_dict tensor %d was never set", i);
     for (int i = 0; i < kNumConvs; ++i) {
-        if (net->d_w[i]) cudaFree(net->d_w[i]);
-        if (net->d_b[i]) cudaFree(net->d_b[i]);
-        CU(cudaMalloc(&net->d_w[i], net->host_w[i].size() * 4));
-        CU(cudaMalloc(&net->d_b[i], net->host_b[i].size() * 4));
-        CU(cudaMemcpy(net->d_w[i], net->host_w[i].data(), net->host_w[i].size() * 4, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(net->d_b[i], net->host_b[i].data(), net->host_b[i].size() * 4, cudaMemcpyHostToDevice));
+        // freed first, not reused: cudaFree synchronises the device, so a forward in flight on another stream has
+        // stopped reading the weights before the synchronous copies below overwrite them
+        net->d_w[i].release();
+        net->d_b[i].release();
+        CU(net->d_w[i].ensure(net->host_w[i].size()));
+        CU(net->d_b[i].ensure(net->host_b[i].size()));
+        CU(cudaMemcpy(net->d_w[i].p, net->host_w[i].data(), net->host_w[i].size() * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(net->d_b[i].p, net->host_b[i].data(), net->host_b[i].size() * 4, cudaMemcpyHostToDevice));
     }
-    for (TcLayer& L : net->tc) free_tc_layer(L);
     net->tc.clear();
     for (int i = 1; i < 12; ++i) {
         const ConvSpec s = kTrunk[i];
@@ -946,8 +956,8 @@ static int ragged_canvas(int n, const int* hw, int* Hc, int* Wc) {
 
 // Writes the extents of the next ragged forward into the net's fixed table (stream-ordered after the previous forward).
 static int upload_ext(b200pose_net* net, const std::vector<int>& ext, cudaStream_t st) {
-    if (!net->d_ext) CU(cudaMalloc(&net->d_ext, (size_t)kMaxRagged * 2 * sizeof(int)));
-    CU(cudaMemcpyAsync(net->d_ext, ext.data(), ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CU(net->d_ext.ensure((size_t)kMaxRagged * 2));
+    CU(cudaMemcpyAsync(net->d_ext.p, ext.data(), ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     return 0;
 }
 
@@ -983,7 +993,7 @@ static int crop_and_forward(b200pose_net* net, const unsigned char* d_raw, int n
     if (launched(e, c.ragged() ? "ragged_frames_launch" : "crop_with_factor_launch")) return 1;
     if (c.ragged() && upload_ext(net, c.ext, st)) return 1;
     return net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, c.Hc, c.Wc, mode, outputs, outputs_on_device, st,
-                            sync_host, c.ragged() ? net->d_ext : nullptr);
+                            sync_host, c.ragged() ? net->d_ext.p : nullptr);
 }
 
 // Raw uint8 frames of `bytes` on the device: a device input in place, else a copy in net->raw_stage.  flip: always
@@ -1049,31 +1059,35 @@ static bool last_ran_plan(const b200pose_net* net) {
 
 int b200pose_net_profile(b200pose_net* net, float* ms, double* flops, int cap, void* cuda_stream) {
     if (!net || !last_ran_plan(net)) return -1;
-    if (cudaSetDevice(net->device) != cudaSuccess) return -1;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     const Plan& p = *net->plan;
     const int n = p.n, H = p.H, W = p.W;
     const int total = (int)p.launches.size() + 1;
     if (cap < total) return -1;
-    std::vector<cudaEvent_t> ev(total + 1);
-    for (auto& e : ev) cudaEventCreate(&e);
-    const void* d_in = net->last.in;
-    int in_u8 = net->last.in_u8;
+    std::vector<Event> ev(total + 1);
     DevBuf<float> tmp;
-    if (!d_in) { if (tmp.ensure((size_t)n * 3 * H * W) != cudaSuccess) return -1; cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st); d_in = tmp.p; in_u8 = 0; }
-    cudaEventRecord(ev[0], st);
-    int rc = launch_forward_tc(net, d_in, in_u8, nullptr, total, st, false, ev.data() + 1);
-    g_launches += total;
-    if (rc == 0 && cudaStreamSynchronize(st) != cudaSuccess)
-        rc = fail("profile run failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (rc == 0) {
-        for (int i = 0; i < total; ++i) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
+    auto run = [&]() -> int {
+        CU(cudaSetDevice(net->device));
+        for (Event& e : ev) CU(cudaEventCreate(&e.h));
+        const void* d_in = net->last.in;
+        int in_u8 = net->last.in_u8;
+        if (!d_in) {
+            CU(tmp.ensure((size_t)n * 3 * H * W));
+            CU(cudaMemsetAsync(tmp.p, 0, (size_t)n * 3 * H * W * 4, st));
+            d_in = tmp.p;
+            in_u8 = 0;
+        }
+        CU(cudaEventRecord(ev[0], st));
+        const int rc = launch_forward_tc(net, d_in, in_u8, nullptr, total, st, false, ev.data() + 1);
+        g_launches += total;
+        if (rc) return rc;
+        CU(cudaStreamSynchronize(st));
+        for (int i = 0; i < total; ++i) CU(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
         flops[0] = 2.0 * n * H * W * 27.0 * 64.0;
         for (size_t i = 0; i < p.launches.size(); ++i) flops[i + 1] = p.launches[i].flops;
-    }
-    for (auto& e : ev) cudaEventDestroy(e);
-    tmp.release();
-    return rc ? -1 : total;
+        return 0;
+    };
+    return run() ? -1 : total;
 }
 
 int b200pose_net_debug_run(b200pose_net* net, int launches, void* cuda_stream) {
@@ -1153,11 +1167,9 @@ int b200pose_net_debug_fp8(b200pose_net* net, int launch, int* act_exp, int n_im
     const ConvTcArgs& a = p.launches[launch - 1].a;
     const int rows = a.groups * a.n_tiles * a.n_tile;
     if (cap < rows) { fail("debug_fp8: %d rows, capacity %d", rows, cap); return -1; }
-    if (cudaSetDevice(net->device) != cudaSuccess) { fail("debug_fp8: cudaSetDevice failed"); return -1; }
-    if (cudaMemcpy(act_exp, a.ea_out, p.n * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) {
-        fail("debug_fp8: reading the exponent table failed");
-        return -1;
-    }
+    cudaError_t e = cudaSetDevice(net->device);
+    if (e == cudaSuccess) e = cudaMemcpy(act_exp, a.ea_out, p.n * sizeof(int), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { cuda_fail("debug_fp8: reading the exponent table: %s", cudaGetErrorString(e)); return -1; }
     const TcLayer& L = net->tc[launch - 1];
     for (int r = 0; r < rows; ++r) w_exp[r] = L.h_w_exp[r];
     return rows;
@@ -1168,13 +1180,11 @@ int b200pose_net_overflow(b200pose_net* net, int* flags, int n, void* cuda_strea
     if (net->last.n == 0) { fail("overflow: no forward has run"); return -1; }
     if (n != net->last.n) { fail("overflow: %d images asked, the last forward ran %d", n, net->last.n); return -1; }
     std::vector<unsigned> h(n, 0u);
-    if (cudaSetDevice(net->device) != cudaSuccess ||
-        cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(cuda_stream)) != cudaSuccess ||
-        (!net->last.fp32 && tc_aux(net->last.fmt) == TcAux::kOverflow &&
-         cudaMemcpy(h.data(), net->ovf.p, n * sizeof(unsigned), cudaMemcpyDeviceToHost) != cudaSuccess)) {
-        fail("overflow: %s", cudaGetErrorString(cudaGetLastError()));
-        return -1;
-    }
+    cudaError_t e = cudaSetDevice(net->device);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(cuda_stream));
+    if (e == cudaSuccess && !net->last.fp32 && tc_aux(net->last.fmt) == TcAux::kOverflow)
+        e = cudaMemcpy(h.data(), net->ovf.p, n * sizeof(unsigned), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { cuda_fail("overflow: %s", cudaGetErrorString(e)); return -1; }
     int flagged = 0;
     for (int i = 0; i < n; ++i) flagged += (flags[i] = h[i] != 0);
     return flagged;
@@ -1191,56 +1201,34 @@ int b200pose_net_last_maps(b200pose_net* net, const float** paf, const float** h
 int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, int peak_cap, int human_cap) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return fail("b200pose: no CUDA device available (this library has no CPU fallback)");
+        return cuda_fail("b200pose: no CUDA device available (this library has no CPU fallback)");
     CU(cudaSetDevice(cuda_device));
-    b200pose_post* p = new b200pose_post();
+    std::unique_ptr<b200pose_post> p(new b200pose_post());
     p->device = cuda_device;
     // candidate-key pool (DESIGN §1): min(batch_cap x 16 Mi, 1 Gi) 8-byte entries, i.e. 128 MB per image of the batch and
     // at most 8 GiB; exhausting it sets a status bit (a loud error in the Python layer)
     const long pool = (long)batch_cap * (16L << 20) < (1L << 30) ? (long)batch_cap * (16L << 20) : (1L << 30);
     cudaError_t e = post_alloc(p->pb, batch_cap, peak_cap, human_cap, pool);
-    if (e != cudaSuccess) { delete p; return fail("post_alloc failed: %s", cudaGetErrorString(e)); }
-    CU(cudaStreamCreateWithFlags(&p->s2, cudaStreamNonBlocking));
-    CU(cudaEventCreateWithFlags(&p->ev_limbs, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&p->ev_asm, cudaEventDisableTiming));
+    if (e != cudaSuccess) return cuda_fail("post_alloc failed: %s", cudaGetErrorString(e));
+    CU(cudaStreamCreateWithFlags(&p->s2.h, cudaStreamNonBlocking));
+    for (Event* ev : {&p->ev_limbs, &p->ev_asm, &p->ev_maps, &p->ev_fetch[0], &p->ev_fetch[1], &p->ev_ld[0], &p->ev_ld[1]})
+        CU(cudaEventCreateWithFlags(&ev->h, cudaEventDisableTiming));
     for (int b = 0; b < 2; ++b) {
-        CU(cudaEventCreateWithFlags(&p->ev_fetch[b], cudaEventDisableTiming));
-        CU(cudaHostAlloc(&p->hp_nh[b], (size_t)batch_cap * sizeof(int), cudaHostAllocDefault));
-        CU(cudaHostAlloc(&p->hp_status[b], (size_t)batch_cap * sizeof(int), cudaHostAllocDefault));
-        CU(cudaHostAlloc(&p->hp_counts[b], (size_t)batch_cap * 18 * sizeof(int), cudaHostAllocDefault));
-        CU(cudaHostAlloc(&p->hp_humans[b], (size_t)batch_cap * human_cap * kHumanFloats * sizeof(float), cudaHostAllocMapped | cudaHostAllocPortable));   // written by assemble_kernel (same pointer on the device: unified addressing)
-        CU(cudaEventCreateWithFlags(&p->ev_ld[b], cudaEventDisableTiming));
-        CU(cudaMalloc(&p->d_ext[b], (size_t)batch_cap * 2 * sizeof(int)));
-        CU(cudaHostAlloc(&p->hp_ovf[b], (size_t)kMaxOvfRows * 2 * batch_cap * sizeof(unsigned), cudaHostAllocDefault));
+        CU(p->hp_nh[b].alloc(batch_cap, cudaHostAllocDefault));
+        CU(p->hp_status[b].alloc(batch_cap, cudaHostAllocDefault));
+        CU(p->hp_counts[b].alloc((size_t)batch_cap * 18, cudaHostAllocDefault));
+        // written by assemble_kernel (same pointer on the device: unified addressing)
+        CU(p->hp_humans[b].alloc((size_t)batch_cap * human_cap * kHumanFloats, cudaHostAllocMapped | cudaHostAllocPortable));
+        CU(p->d_ext[b].ensure((size_t)batch_cap * 2));
+        CU(p->hp_ovf[b].alloc((size_t)kMaxOvfRows * 2 * batch_cap, cudaHostAllocDefault));
     }
-    CU(cudaEventCreateWithFlags(&p->ev_maps, cudaEventDisableTiming));
-    *out = p;
+    *out = p.release();
     return 0;
 }
 
 void b200pose_post_destroy(b200pose_post* p) {
     if (!p) return;
     cudaSetDevice(p->device);
-    if (p->s2) cudaStreamSynchronize(p->s2);
-    post_free(p->pb);
-    p->d_heat.release(); p->d_paf.release();
-    p->tta_in.release(); p->tta_out.release();
-    p->ov_maps[0].release(); p->ov_maps[1].release();
-    p->ms_ext.release(); p->ms_resize.release();
-    if (p->ev_maps) cudaEventDestroy(p->ev_maps);
-    for (int b = 0; b < 2; ++b) if (p->ev_ld[b]) cudaEventDestroy(p->ev_ld[b]);
-    for (int b = 0; b < 2; ++b) {
-        if (p->ev_fetch[b]) cudaEventDestroy(p->ev_fetch[b]);
-        if (p->hp_nh[b]) cudaFreeHost(p->hp_nh[b]);
-        if (p->hp_status[b]) cudaFreeHost(p->hp_status[b]);
-        if (p->hp_counts[b]) cudaFreeHost(p->hp_counts[b]);
-        if (p->hp_humans[b]) cudaFreeHost(p->hp_humans[b]);
-        if (p->d_ext[b]) cudaFree(p->d_ext[b]);
-        if (p->hp_ovf[b]) cudaFreeHost(p->hp_ovf[b]);
-    }
-    if (p->ev_limbs) cudaEventDestroy(p->ev_limbs);
-    if (p->ev_asm) cudaEventDestroy(p->ev_asm);
-    if (p->s2) cudaStreamDestroy(p->s2);
     delete p;
 }
 
@@ -1261,15 +1249,13 @@ static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st, 
     const int b = (int)(p->runs & 1);
     // the assembly kernel writes the person rows straight into this run's pinned host slot (unified addressing): only the
     // rows that exist cross PCIe, instead of a copy of the full-capacity buffer (4.8 MB per step at batch 32)
-    p->pb.humans_out = p->hp_humans[b];
-    cudaError_t e = post_assemble(p->pb, n, p->s2, prm);
-    if (e != cudaSuccess) return fail("post_assemble: %s", cudaGetErrorString(e));
-    ++g_launches;
+    p->pb.humans_out = p->hp_humans[b].p;
+    if (launched(post_assemble(p->pb, n, p->s2, prm), "post_assemble")) return 1;
     CU(cudaEventRecord(p->ev_asm, p->s2));
     const PostBuffers& pb = p->pb;
-    CU(cudaMemcpyAsync(p->hp_nh[b], pb.n_humans, n * sizeof(int), cudaMemcpyDeviceToHost, p->s2));
-    CU(cudaMemcpyAsync(p->hp_status[b], pb.status, n * sizeof(int), cudaMemcpyDeviceToHost, p->s2));
-    CU(cudaMemcpyAsync(p->hp_counts[b], pb.counts, (size_t)n * 18 * sizeof(int), cudaMemcpyDeviceToHost, p->s2));
+    CU(cudaMemcpyAsync(p->hp_nh[b].p, pb.n_humans, n * sizeof(int), cudaMemcpyDeviceToHost, p->s2));
+    CU(cudaMemcpyAsync(p->hp_status[b].p, pb.status, n * sizeof(int), cudaMemcpyDeviceToHost, p->s2));
+    CU(cudaMemcpyAsync(p->hp_counts[b].p, pb.counts, (size_t)n * 18 * sizeof(int), cudaMemcpyDeviceToHost, p->s2));
     CU(cudaEventRecord(p->ev_fetch[b], p->s2));
     p->slot_n[b] = n;
     p->ovf_rows[b] = p->ovf_pending;
@@ -1292,8 +1278,8 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
     const int slot = (int)(p->runs & 1);
     if (p->have_ld[slot]) CU(cudaStreamWaitEvent(st, p->ev_ld[slot], 0));   // run i-2 is done with this slot
     if (ext) {
-        CU(cudaMemcpyAsync(p->d_ext[slot], ext, (size_t)n * 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
-        ext = p->d_ext[slot];
+        CU(cudaMemcpyAsync(p->d_ext[slot].p, ext, (size_t)n * 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        ext = p->d_ext[slot].p;
     }
     // private copy of the maps (15 MB at batch 32) so that the next forward may overwrite the network's output
     // buffers while this run's post-processing is still reading; everything after the copy runs on s2
@@ -1314,16 +1300,15 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
     const PostParams* prm = run_params(p);
     if (layout == 0) {
         e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, (long)h * w, w, 1, h, w, thresh, ps, ext);
-        if (e != cudaSuccess) return fail("post_peaks: %s", cudaGetErrorString(e));
+        if (launched(e, "post_peaks")) return 1;
         e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps, ext, prm);
     } else {
         if (ext) return fail("post_run: ragged batches need the planar (layout 0) maps");
         e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, 1, (long)w * 19, 19, h, w, thresh, ps);
-        if (e != cudaSuccess) return fail("post_peaks: %s", cudaGetErrorString(e));
+        if (launched(e, "post_peaks")) return 1;
         e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * 8, w, h, ps, nullptr, prm);
     }
-    if (e != cudaSuccess) return fail("post_limbs: %s", cudaGetErrorString(e));
-    g_launches += 2;
+    if (launched(e, "post_limbs")) return 1;
     CU(cudaEventRecord(p->ev_ld[slot], ps));
     p->have_ld[slot] = true;
     p->hw_h = h; p->hw_w = w;
@@ -1396,11 +1381,12 @@ int b200pose_post_status_accum(b200pose_post* p, int reset) {
     // OR of the status words of every image of every run since the last reset: lets a caller that keeps runs in flight
     // (and only reads some of them back) prove that NO run overflowed a capacity
     if (!p) return -1;
-    if (cudaSetDevice(p->device) != cudaSuccess) return -1;
-    if (cudaStreamSynchronize(p->s2) != cudaSuccess) return -1;
     std::vector<int> h(p->pb.batch_cap);
-    if (cudaMemcpy(h.data(), p->pb.status_acc, h.size() * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    if (reset && cudaMemset(p->pb.status_acc, 0, h.size() * sizeof(int)) != cudaSuccess) return -1;
+    cudaError_t e = cudaSetDevice(p->device);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(p->s2);
+    if (e == cudaSuccess) e = cudaMemcpy(h.data(), p->pb.status_acc, h.size() * sizeof(int), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && reset) e = cudaMemset(p->pb.status_acc, 0, h.size() * sizeof(int));
+    if (e != cudaSuccess) { cuda_fail("status_accum: %s", cudaGetErrorString(e)); return -1; }
     int acc = 0;
     for (int v : h) acc |= v;
     return acc;
@@ -1410,16 +1396,14 @@ int b200pose_post_debug_sort(b200pose_post* p, const unsigned long long* keys, i
     if (!p || !keys || !out) return fail("debug_sort: null pointer");
     CU(cudaSetDevice(p->device));
     CU(cudaStreamSynchronize(p->s2));
-    cudaError_t e = post_debug_sort(p->pb, keys, n, out, nullptr);
-    if (e != cudaSuccess) return fail("post_debug_sort: %s", cudaGetErrorString(e));
-    g_launches += 2;
-    return 0;
+    return launched(post_debug_sort(p->pb, keys, n, out, nullptr), "post_debug_sort", 2);
 }
 
 int b200pose_post_debug(b200pose_post* p, unsigned long long* out, int n, int reset) {
     if (!p || n > 16) return -1;
-    if (cudaMemcpy(out, p->pb.dbg, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    if (reset) cudaMemset(p->pb.dbg, 0, 16 * sizeof(unsigned long long));
+    cudaError_t e = cudaMemcpy(out, p->pb.dbg, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && reset) e = cudaMemset(p->pb.dbg, 0, 16 * sizeof(unsigned long long));
+    if (e != cudaSuccess) { cuda_fail("post_debug: %s", cudaGetErrorString(e)); return -1; }
     return 0;
 }
 
@@ -1438,20 +1422,20 @@ static int post_ready(b200pose_post* p, int img) {
     if (p->cur_ticket < 0 && b200pose_post_sync(p)) return 0;
     return img >= 0 && img < p->slot_n[p->cur];
 }
-int b200pose_post_num_humans(b200pose_post* p, int img) { return post_ready(p, img) ? p->hp_nh[p->cur][img] : -1; }
-int b200pose_post_status(b200pose_post* p, int img) { return post_ready(p, img) ? p->hp_status[p->cur][img] : -1; }
+int b200pose_post_num_humans(b200pose_post* p, int img) { return post_ready(p, img) ? p->hp_nh[p->cur].p[img] : -1; }
+int b200pose_post_status(b200pose_post* p, int img) { return post_ready(p, img) ? p->hp_status[p->cur].p[img] : -1; }
 int b200pose_post_overflow(b200pose_post* p, int img) {
     if (!post_ready(p, img)) return -1;
     const int b = p->cur, n = p->slot_n[b];
-    const unsigned* h = p->hp_ovf[b];
+    const unsigned* h = p->hp_ovf[b].p;
     for (int k = 0; k < p->ovf_rows[b]; ++k, h += 2 * (size_t)p->pb.batch_cap)
         if (h[img] || (p->ovf_imgs[b] == 2 * n && h[n + img])) return 1;
     return 0;
 }
 int b200pose_post_get_humans(b200pose_post* p, int img, float* out, int max_humans) {
     if (!post_ready(p, img)) return -1;
-    const int n = p->hp_nh[p->cur][img] < max_humans ? p->hp_nh[p->cur][img] : max_humans;
-    memcpy(out, p->hp_humans[p->cur] + (size_t)img * p->pb.human_cap * kHumanFloats, (size_t)n * kHumanFloats * sizeof(float));
+    const int n = p->hp_nh[p->cur].p[img] < max_humans ? p->hp_nh[p->cur].p[img] : max_humans;
+    memcpy(out, p->hp_humans[p->cur].p + (size_t)img * p->pb.human_cap * kHumanFloats, (size_t)n * kHumanFloats * sizeof(float));
     return n;
 }
 int b200pose_post_get_peaks(b200pose_post* p, int img, float* out, int max_peaks) {
@@ -1464,16 +1448,14 @@ int b200pose_post_get_peaks(b200pose_post* p, int img, float* out, int max_peaks
     if (p->h_px.empty()) {
         const size_t tot = per * last_n;
         p->h_px.resize(tot); p->h_py.resize(tot); p->h_px_s.resize(tot);
-        if (cudaMemcpy(p->h_px.data(), pb.peak_x, tot * 4, cudaMemcpyDeviceToHost) != cudaSuccess ||
-            cudaMemcpy(p->h_py.data(), pb.peak_y, tot * 4, cudaMemcpyDeviceToHost) != cudaSuccess ||
-            cudaMemcpy(p->h_px_s.data(), pb.peak_s, tot * 4, cudaMemcpyDeviceToHost) != cudaSuccess) {
-            fail("peak copy failed");
-            return -1;
-        }
+        cudaError_t e = cudaMemcpy(p->h_px.data(), pb.peak_x, tot * 4, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(p->h_py.data(), pb.peak_y, tot * 4, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(p->h_px_s.data(), pb.peak_s, tot * 4, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) { cuda_fail("peak copy failed: %s", cudaGetErrorString(e)); return -1; }
     }
     int k = 0;
     for (int part = 0; part < 18; ++part) {
-        const int c = p->hp_counts[p->cur][(size_t)img * 18 + part];
+        const int c = p->hp_counts[p->cur].p[(size_t)img * 18 + part];
         for (int i = 0; i < c && k < max_peaks; ++i, ++k) {
             const size_t o = (size_t)img * per + (size_t)part * pb.peak_cap + i;
             out[5 * k + 0] = (float)p->h_px[o];
@@ -1543,7 +1525,7 @@ static int check_infer(const b200pose_net* net, const b200pose_post* post) {
 static int stash_overflow(const b200pose_net* net, b200pose_post* post, int nimg, cudaStream_t st) {
     if (net->last.fp32 || tc_aux(net->last.fmt) != TcAux::kOverflow) return 0;
     if (post->ovf_pending >= kMaxOvfRows || nimg > 2 * post->pb.batch_cap) return fail("overflow rows exhausted");
-    unsigned* dst = post->hp_ovf[post->runs & 1] + (size_t)post->ovf_pending * 2 * post->pb.batch_cap;
+    unsigned* dst = post->hp_ovf[post->runs & 1].p + (size_t)post->ovf_pending * 2 * post->pb.batch_cap;
     CU(cudaMemcpyAsync(dst, net->ovf.p, nimg * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     post->ovf_pending += 1;
     post->ovf_pending_imgs = nimg;
@@ -2028,14 +2010,14 @@ int process_paf(int p1, int p2, int p3, float* peaks, int h1, int h2, int h3, fl
     CU(p->d_paf.ensure((size_t)f1 * f2 * f3));
     CU(cudaMemcpyAsync(p->d_paf.p, pafmap, (size_t)f1 * f2 * f3 * 4, cudaMemcpyHostToDevice, st));
     // the reference's drop-in keeps the reference's constants (g_legacy's settings are never changed either)
-    cudaError_t e = post_limbs(pb, 1, p->d_paf.p, 0, 1, (long)f2 * f3, f3, 0, h1, f2, f1, st);
-    if (e != cudaSuccess) return fail("post_limbs: %s", cudaGetErrorString(e));
-    ++g_launches;
+    if (launched(post_limbs(pb, 1, p->d_paf.p, 0, 1, (long)f2 * f3, f3, 0, h1, f2, f1, st), "post_limbs")) return 1;
     if (enqueue_assemble_and_fetch(p, 1, st, nullptr)) return 3;
     if (b200pose_post_sync(p)) return 3;
-    if (p->hp_status[p->cur][0] & 0xff & ~16) return fail("process_paf: capacity exceeded (status %d)", p->hp_status[p->cur][0]);
-    g_leg_nh = p->hp_nh[p->cur][0];
-    g_leg_humans.assign(p->hp_humans[p->cur], p->hp_humans[p->cur] + (size_t)g_leg_nh * kHumanFloats);
+    const int status = p->hp_status[p->cur].p[0];
+    if (status & 0xff & ~16) return fail("process_paf: capacity exceeded (status %d)", status);
+    g_leg_nh = p->hp_nh[p->cur].p[0];
+    const float* humans = p->hp_humans[p->cur].p;
+    g_leg_humans.assign(humans, humans + (size_t)g_leg_nh * kHumanFloats);
     return 0;
 }
 // The reference's getters index its vectors unchecked (pafprocess.cpp:196-218); out-of-range arguments return -1 / 0 here.
