@@ -51,6 +51,20 @@ typedef struct b200pose_net b200pose_net;
                                       4 ran as bf16; every value outside 0 .. 4 still does.                            */
 
 int b200pose_net_create(b200pose_net** out, int cuda_device);
+/* A net of the reference's second network, OpenPose_Model(l2_stages, l1_stages, 38, 19)    lib/network/openpose.py:111-199
+ * (DESIGN.md 2.11): rtpose's trunk with PReLU after conv4_2, conv4_3_CPM and conv4_4_CPM, then l2 PAF stages and l1
+ * heat-map stages, one after the other, of dense 3x3 blocks with PReLU.  1 <= l2, 1 <= l1, l2 + l1 <= 12.  The net keeps
+ * its architecture: b200pose_net_set_tensor / _finalize validate against its own tensor table (the reference's
+ * state_dict order, b200pose_openpose_tensor_shape), outputs[12] of every forward hold its maps in saved_for_loss order
+ * [paf_1 .. paf_l2, heat_1 .. heat_l1] (the other entries must be NULL), and the final maps - what b200pose_net_last_maps
+ * returns and every fused entry point post-processes - are paf_l2 and heat_l1.  Modes bf16, bf16x3 and fp32; fp8 and
+ * fp16, and b200pose_net_set_stages, are refused with an error naming the architecture, leaving the net usable. */
+int b200pose_net_create_openpose(b200pose_net** out, int cuda_device, int l2_stages, int l1_stages);
+/* OpenPose_Model(l2_stages, l1_stages)'s state_dict, without a device: the number of tensors (< 0: no such architecture)
+ * and the shape of tensor `index` (weights: 4 dims OIHW; biases and PReLU slopes: 1 dim), returning its number of dims
+ * (< 0: out of range).  Each conv's tensors come in the order weight, bias, PReLU slope. */
+int b200pose_openpose_num_tensors(int l2_stages, int l1_stages);
+int b200pose_openpose_tensor_shape(int l2_stages, int l1_stages, int index, long dims[4]);
 void b200pose_net_destroy(b200pose_net* net);
 /* Shape of state_dict tensor `index` (weights: 4 dims OIHW, biases: 1 dim); returns number of dims. */
 int b200pose_net_tensor_shape(int index, long dims[4]);

@@ -22,6 +22,9 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_version": ([], ci),
     "b200pose_launch_count": ([], cl),
     "b200pose_net_create": ([ctypes.POINTER(vp), ci], ci),
+    "b200pose_net_create_openpose": ([ctypes.POINTER(vp), ci, ci, ci], ci),
+    "b200pose_openpose_num_tensors": ([ci, ci], ci),
+    "b200pose_openpose_tensor_shape": ([ci, ci, ci, ctypes.POINTER(cl)], ci),
     "b200pose_net_destroy": ([vp], None),
     "b200pose_net_tensor_shape": ([ci, ctypes.POINTER(cl)], ci),
     "b200pose_net_set_tensor": ([vp, ci, vp, cl], ci),
@@ -152,3 +155,18 @@ def crop_geometry(src_h, src_w, dest_size=368, factor=8):
 
 def launch_count():
     return int(lib().b200pose_launch_count())
+
+
+def openpose_shapes(l2_stages=4, l1_stages=2):
+    """The state_dict shapes of OpenPose_Model(l2_stages, l1_stages, 38, 19) in the reference's order, from the
+    library's own table (no device needed)."""
+    n = lib().b200pose_openpose_num_tensors(int(l2_stages), int(l1_stages))
+    if n < 0:
+        raise B200PoseError("OpenPose_Model(%r, %r): stages must be l2 >= 1, l1 >= 1, l2 + l1 <= 12"
+                            % (l2_stages, l1_stages))
+    dims = (ctypes.c_long * 4)()
+    out = []
+    for i in range(n):
+        nd = lib().b200pose_openpose_tensor_shape(int(l2_stages), int(l1_stages), i, dims)
+        out.append(tuple(int(d) for d in dims[:nd]))
+    return out

@@ -109,6 +109,83 @@ ConvSpec conv_spec(int ci) {
 // concat channel c of torch.cat([paf, heat, feat], 1) (rtpose_vgg.py:165)
 int cat_phys(int c) { return c < kPaf ? c : (c < kPaf + kHeat ? c + 2 : c + 7); }
 
+// ---------------------------------------------------------------- OpenPose_Model (lib/network/openpose.py), DESIGN §2.11
+// Trunk: rtpose's twelve convs, with a per-channel PReLU instead of the ReLU after conv4_2, conv4_3_CPM and conv4_4_CPM.
+// Then l2 PAF stages and l1 heat-map stages, one after the other (stage t of the net = L2 stage t + 1 for t < l2, else
+// L1 stage t - l2 + 1).  A stage is five dense blocks of three 3x3 convs Mconv{b}_{0,1,2} whose outputs are concatenated,
+// a 1x1 Mconv6 and the 1x1 head Mconv7; every conv but Mconv7 is followed by a PReLU.  Stage inputs: the features (L2
+// stage 1), cat[features, paf] (L2 stages >= 2, L1 stage 1), cat[features, heat, paf] (L1 stages >= 2).
+enum Nonlin { kNoAct, kRelu, kPrelu };
+constexpr int kOpMaxStages = 12, kOpStageConvs = 17;
+bool op_valid(int l2, int l1) { return l2 >= 1 && l1 >= 1 && l2 + l1 <= kOpMaxStages; }
+int op_num_convs(int l2, int l1) { return 12 + kOpStageConvs * (l2 + l1); }
+struct OpStage {
+    bool paf, first;                  // PAF (L2) stage; first stage of its branch (96 inner channels)
+    int in, inner, innerout, out;     // StageBlock's channels
+};
+OpStage op_stage(int l2, int t) {
+    const bool paf = t < l2, first = t == 0 || t == l2;
+    const int in = t == 0 ? kFeat : (paf || first ? kFeat + kPaf : kFeat + kHeat + kPaf);
+    return {paf, first, in, first ? 96 : 128, first ? 256 : 512, paf ? kPaf : kHeat};
+}
+// conv ci in state_dict order: trunk 0..11, then 17 per stage (Mconv1_0 .. Mconv5_2, Mconv6, Mconv7)
+struct OpConv { ConvSpec s; Nonlin act; };
+OpConv op_conv(int l2, int ci) {
+    if (ci < 12) return {kTrunk[ci], ci >= 9 ? kPrelu : kRelu};
+    const int t = (ci - 12) / kOpStageConvs, li = (ci - 12) % kOpStageConvs;
+    const OpStage g = op_stage(l2, t);
+    if (li == 16) return {{g.innerout, g.out, 1}, kNoAct};
+    if (li == 15) return {{3 * g.inner, g.innerout, 1}, kPrelu};
+    return {{li % 3 ? g.inner : (li == 0 ? g.in : 3 * g.inner), g.inner, 3}, kPrelu};
+}
+// state_dict tensor `index` of OpenPose_Model(l2, l1): conv *ci, *kind 0 = weight, 1 = bias, 2 = PReLU slope (each conv's
+// tensors in that order).  False when out of range.
+bool op_tensor(int l2, int l1, int index, int* ci, int* kind) {
+    for (int c = 0; c < op_num_convs(l2, l1); ++c) {
+        const int nt = op_conv(l2, c).act == kPrelu ? 3 : 2;
+        if (index < nt) {
+            *ci = c;
+            *kind = index;
+            return index >= 0;
+        }
+        index -= nt;
+    }
+    return false;
+}
+int op_num_tensors(int l2, int l1) {
+    int n = 0;
+    for (int c = 0; c < op_num_convs(l2, l1); ++c) n += op_conv(l2, c).act == kPrelu ? 3 : 2;
+    return n;
+}
+int op_tensor_shape(int l2, int l1, int index, long dims[4]) {
+    int ci, kind;
+    if (!op_valid(l2, l1) || !op_tensor(l2, l1, index, &ci, &kind)) return -1;
+    const ConvSpec s = op_conv(l2, ci).s;
+    dims[0] = s.cout;
+    if (kind != 0) return 1;
+    dims[1] = s.cin; dims[2] = s.ks; dims[3] = s.ks;
+    return 4;
+}
+
+// Input channel permutation of a tensor-core layer: reference channel c of its input -> channel of the buffer it reads.
+enum InPerm {
+    kPermNone,
+    kPermRtposeCat,      // torch.cat([paf, heat, feat]) in the concat buffer (cat_phys)
+    kPermFeatPaf,        // OpenPose_Model: torch.cat([features, paf]) in the concat buffer
+    kPermFeatHeatPaf,    // ... torch.cat([features, heat, paf])
+    kPermSlots,          // a dense block's cat of three outputs of `slot` channels, one 128-channel slot each
+};
+int perm_phys(InPerm perm, int slot, int c) {
+    switch (perm) {
+        case kPermNone: break;
+        case kPermRtposeCat: return cat_phys(c);
+        case kPermFeatPaf: return c < kFeat ? 64 + c : c - kFeat;
+        case kPermFeatHeatPaf: return c < kFeat ? 64 + c : (c < kFeat + kHeat ? 40 + c - kFeat : c - kFeat - kHeat);
+        case kPermSlots: return (c / slot) * 128 + c % slot;
+    }
+    return c;
+}
+
 uint16_t f2bf(float f) {
     uint32_t u;
     memcpy(&u, &f, 4);
@@ -163,10 +240,13 @@ using GraphExec = Handle<cudaGraphExec_t, cudaGraphExecDestroy>;
 
 struct TcLayer {            // one grouped tensor-core launch
     int ks, cin_blocks, groups, n_tile, n_tiles, relu, pool;
+    bool prelu = false;           // PReLU epilogue (OpenPose_Model) with `slope`, instead of `relu`
     double macs_per_pixel = 0;    // algorithmic (unpadded) MACs per output pixel, all groups
     DevBuf<float> bias;           // [groups*n_tiles*n_tile]
+    DevBuf<float> slope;          // PReLU slopes, laid out like the bias (pad rows 0)
     std::vector<int> convs;       // state-dict conv per group
-    bool cat_input = false;       // reads the concat buffer (input channels permuted, cat_phys)
+    InPerm perm = kPermNone;      // input channels permuted (perm_phys) ...
+    int slot = 0;                 // ... kPermSlots: channels per slot
     // packed weights per encoding (TcWeights, tc_format.h), rows groups*n_tiles*n_tile of cin_blocks*64 channels; see
     // ensure_packed for when each is packed
     DevBuf<unsigned char> w[kNumTcWeights];
@@ -220,6 +300,25 @@ const Wiring kStageWiring[7] = {     // stages 2 .. 6
     {BRA,   0,  128,  BRB,   {0, 128}, {128, 128}},
     {BRB,   0,  128,  CAT,   {0, 40},  {40, 24}, true},
 };
+// OpenPose_Model (DESIGN §2.11): bra and brb hold 768 channels, six 128-channel slots: a dense block's three outputs go to
+// slots 0, 1, 2 (stages of 128 inner channels) or 3, 4, 5 (the 96-channel first stage of each branch: lanes 96..127 of
+// those slots are never written and stay +0).  Blocks 1, 3, 5 write bra, blocks 2, 4 brb: Mconv{b}_0 reads all three
+// slots of the other buffer, _1 reads slot 0 and writes slot 1, _2 reads slot 1 and writes slot 2.  Mconv6 writes br512
+// (512 channels).  The PAF heads store 64 lanes at channel 0 of the concat buffer - PAF, then +0 from zero rows and bias
+// over the heat slot and the pad lanes, so that an L2 stage >= 2 or L1 stage 1, which reads the heat slot against zero
+// weights, never reads an earlier forward's values; the heat-map heads store the 24 lanes from channel 40.
+constexpr int kOpActBr = 768, kOpActBr512 = 512;
+Wiring op_wiring(int l2, int t, int li) {
+    const OpStage g = op_stage(l2, t);
+    const int base = g.first ? 384 : 0, store = g.inner == 96 ? 48 : 128;
+    if (li == 16) return g.paf ? Wiring{BR512, 0, 0, CAT, {0, 0}, {64, 0}, true} : Wiring{BR512, 0, 0, CAT, {40, 0}, {24, 0}, true};
+    if (li == 15) return {BRA, base, 0, BR512, {0, 0}, {128, 0}};
+    const int b = li / 3, j = li % 3;
+    const int cur = b % 2 ? BRB : BRA, prev = b % 2 ? BRA : BRB;
+    if (li == 0) return {CAT, t == 0 ? 64 : 0, 0, cur, {base, 0}, {store, 0}};
+    if (j == 0) return {prev, base, 0, cur, {base, 0}, {store, 0}};
+    return {cur, base + 128 * (j - 1), 0, cur, {base + 128 * j, 0}, {store, 0}};
+}
 
 struct PlanLaunch {
     ConvTcArgs a;
@@ -256,10 +355,12 @@ struct LastForward {
 
 struct b200pose_net {
     int device = 0, num_sms = 0;
+    // architecture, fixed at creation: OpenPose_Model(l2, l1) (b200pose_net_create_openpose), or rtpose when l2 == 0
+    int l2 = 0, l1 = 0;
     bool finalized = false;
-    std::vector<std::vector<float>> host_w, host_b;   // per conv
-    std::vector<bool> have;                            // per tensor
-    DevBuf<float> d_w[kNumConvs], d_b[kNumConvs];      // fp32 OIHW (parity mode, conv1_1)
+    std::vector<std::vector<float>> host_w, host_b, host_slope;   // per conv (slope: PReLU convs only)
+    std::vector<bool> have;                                        // per tensor
+    std::vector<DevBuf<float>> d_w, d_b, d_slope;      // per conv, fp32 OIHW (parity mode, conv1_1) and PReLU slopes
     // tensor-core layers: trunk 1..11 -> tc[0..10]; stage 1: tc[11..15]; stage t>=2: tc[16 + (t-2)*7 + li]
     std::vector<TcLayer> tc;
     // Plans of the last 32 keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not re-encode
@@ -279,6 +380,7 @@ struct b200pose_net {
     DevBuf<float> in_stage, out_f32[12];
     // fp32 parity buffers
     DevBuf<float> f_a, f_b, f_cat, f_x, f_y, f_in, f_u8;
+    DevBuf<float> f_cat3, f_z;         // OpenPose_Model: cat[features, heat, paf], Mconv6's output
     LastForward last;
     DevBuf<unsigned char> in_stage_u8;
     int preprocess = 1;                // normalisation fused into the uint8 entry points (preprocess_core.h; 1 = rtpose)
@@ -349,38 +451,69 @@ struct b200pose_post {
 
 namespace {
 
-// The final maps of the last forward: the PAF and heatmap of its last stage.
-const float* last_paf(const b200pose_net* net) { return net->out_f32[2 * net->last.stages - 2].p; }
-const float* last_heat(const b200pose_net* net) { return net->out_f32[2 * net->last.stages - 1].p; }
+bool is_openpose(const b200pose_net* net) { return net->l2 > 0; }
+ConvSpec net_conv(const b200pose_net* net, int ci) { return is_openpose(net) ? op_conv(net->l2, ci).s : conv_spec(ci); }
+int net_num_convs(const b200pose_net* net) { return is_openpose(net) ? op_num_convs(net->l2, net->l1) : kNumConvs; }
+int net_num_tensors(const b200pose_net* net) {
+    return is_openpose(net) ? op_num_tensors(net->l2, net->l1) : B200POSE_NUM_TENSORS;
+}
+// "OpenPose_Model(l2, l1)" or "rtpose": the refusals name the net's architecture
+std::string arch_name(const b200pose_net* net) {
+    return is_openpose(net) ? "OpenPose_Model(" + std::to_string(net->l2) + ", " + std::to_string(net->l1) + ")" : "rtpose";
+}
+// Stage maps a forward of the net writes (outputs[] entries, saved_for_loss order) and the channels of map i: rtpose
+// [paf_1, heat_1, ..., paf_k, heat_k]; OpenPose_Model [paf_1 .. paf_l2, heat_1 .. heat_l1].
+int net_num_maps(const b200pose_net* net, int stages) { return is_openpose(net) ? net->l2 + net->l1 : 2 * stages; }
+int map_ch(const b200pose_net* net, int i) {
+    return (is_openpose(net) ? i < net->l2 : i % 2 == 0) ? kPaf : kHeat;
+}
+// channels per pixel of activation buffer i
+int act_c(const b200pose_net* net, int i) {
+    if (is_openpose(net) && (i == BRA || i == BRB)) return kOpActBr;
+    if (is_openpose(net) && i == BR512) return kOpActBr512;
+    return kActC[i];
+}
+
+// The final maps of the last forward: the PAF and heatmap of its last stage (OpenPose_Model: of its last L2 and L1
+// stages).
+const float* last_paf(const b200pose_net* net) {
+    return net->out_f32[is_openpose(net) ? net->l2 - 1 : 2 * net->last.stages - 2].p;
+}
+const float* last_heat(const b200pose_net* net) {
+    return net->out_f32[is_openpose(net) ? net->l2 + net->l1 - 1 : 2 * net->last.stages - 1].p;
+}
 
 // Calls row(g, o, r, w) for output channel o of every group g of layer L (packed row r = g * cout_pad + o), w its fp32
-// weights in packed order [tap][cin_pad]: input channels at their physical channel of the buffer the layer reads (cat_phys
-// for the concat buffer), zero in the pad channels.
+// weights in packed order [tap][cin_pad]: input channels at their physical channel of the buffer the layer reads
+// (perm_phys), zero in the pad channels.
 template <class F> void for_each_weight_row(const b200pose_net* net, const TcLayer& L, F&& row) {
     const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, cout_pad = L.n_tiles * L.n_tile;
     std::vector<float> w((size_t)taps * cin_pad);
     for (int g = 0; g < L.groups; ++g) {
-        const ConvSpec s = conv_spec(L.convs[g]);
+        const ConvSpec s = net_conv(net, L.convs[g]);
         const std::vector<float>& hw = net->host_w[L.convs[g]];
         for (int o = 0; o < s.cout; ++o) {
             std::fill(w.begin(), w.end(), 0.f);
             for (int c = 0; c < s.cin; ++c)
                 for (int t = 0; t < taps; ++t)
-                    w[(size_t)t * cin_pad + (L.cat_input ? cat_phys(c) : c)] = hw[((size_t)o * s.cin + c) * taps + t];
+                    w[(size_t)t * cin_pad + perm_phys(L.perm, L.slot, c)] = hw[((size_t)o * s.cin + c) * taps + t];
             row(g, o, g * cout_pad + o, w.data());
         }
     }
 }
 
-// The layer of the convs conv_ids (one per group), before any weights are packed.
-TcLayer make_tc_layer(const std::vector<int>& conv_ids, int n_tile, bool cat_input, int ks, int relu, int pool) {
-    const ConvSpec sp = conv_spec(conv_ids[0]);
-    const int cin_pad = cat_input ? 192 : sp.cin;
+// The layer of the convs conv_ids (one per group), before any weights are packed.  Its input is 192 channels of the
+// concat buffer (the concat permutations), three 128-channel slots (kPermSlots) or the conv's input channels rounded up to
+// 64.  prelu: the convs' PReLU replaces `relu`.
+TcLayer make_tc_layer(const b200pose_net* net, const std::vector<int>& conv_ids, int n_tile, InPerm perm, int relu,
+                      int pool, bool prelu = false) {
+    const ConvSpec sp = net_conv(net, conv_ids[0]);
+    const int cin_pad = perm == kPermSlots ? 3 * 128 : (perm != kPermNone ? 192 : (sp.cin + 63) / 64 * 64);
     const int cout_pad = ((sp.cout + n_tile - 1) / n_tile) * n_tile;
     TcLayer L;
-    L.ks = ks; L.cin_blocks = cin_pad / 64; L.groups = (int)conv_ids.size(); L.n_tile = n_tile; L.n_tiles = cout_pad / n_tile;
-    L.relu = relu; L.pool = pool; L.convs = conv_ids; L.cat_input = cat_input;
-    for (int c : conv_ids) L.macs_per_pixel += (double)conv_spec(c).cin * conv_spec(c).cout * ks * ks;
+    L.ks = sp.ks; L.cin_blocks = cin_pad / 64; L.groups = (int)conv_ids.size(); L.n_tile = n_tile; L.n_tiles = cout_pad / n_tile;
+    L.relu = relu; L.pool = pool; L.prelu = prelu; L.convs = conv_ids; L.perm = perm; L.slot = sp.cin / 3;
+    for (int c : conv_ids) L.macs_per_pixel += (double)net_conv(net, c).cin * net_conv(net, c).cout * sp.ks * sp.ks;
     return L;
 }
 
@@ -389,9 +522,10 @@ TcLayer make_tc_layer(const std::vector<int>& conv_ids, int n_tile, bool cat_inp
 int pack_tc_layer(b200pose_net* net, TcLayer& L) {
     const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, rows = L.groups * L.n_tiles * L.n_tile;
     std::vector<uint16_t> w((size_t)2 * taps * rows * cin_pad, 0);
-    std::vector<float> b((size_t)rows, 0.f);
+    std::vector<float> b((size_t)rows, 0.f), s(L.prelu ? rows : 0, 0.f);
     for_each_weight_row(net, L, [&](int g, int o, int r, const float* wr) {
         b[r] = net->host_b[L.convs[g]][o];
+        if (L.prelu) s[r] = net->host_slope[L.convs[g]][o];
         for (int t = 0; t < taps; ++t)
             for (int k = 0; k < cin_pad; ++k) {
                 const float wf = wr[(size_t)t * cin_pad + k];
@@ -405,6 +539,10 @@ int pack_tc_layer(b200pose_net* net, TcLayer& L) {
     CU(L.bias.ensure(b.size()));
     CU(cudaMemcpy(dw.p, w.data(), w.size() * 2, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(L.bias.p, b.data(), b.size() * 4, cudaMemcpyHostToDevice));
+    if (L.prelu) {
+        CU(L.slope.ensure(s.size()));
+        CU(cudaMemcpy(L.slope.p, s.data(), s.size() * 4, cudaMemcpyHostToDevice));
+    }
     return 0;
 }
 
@@ -499,9 +637,9 @@ bool small_plan(const b200pose_net* net, int n, int H, int W) {
     return 2 * n * ((H / 8 + kTileH - 1) / kTileH) * ((W / 8 + kTileW - 1) / kTileW) * 2 <= net->num_sms;
 }
 
-// Appends tensor-core layer L, wired as `wr`, to plan p; a stage head writes the fp32 maps 2 * stage, 2 * stage + 1.
-// fp8: writers[] are the launches (amax table rows) that wrote the channels it reads; writers[1] may be -1.
-int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& wr, int stage, const int writers[2]) {
+// Appends tensor-core layer L, wired as `wr`, to plan p; a stage head writes the fp32 maps map0 (group 0) and map0 + 1
+// (group 1).  fp8: writers[] are the launches (amax table rows) that wrote the channels it reads; writers[1] may be -1.
+int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& wr, int map0, const int writers[2]) {
     const int n = p.n, H = p.H / kActDiv[wr.in], W = p.W / kActDiv[wr.in];
     ConvTcArgs a;
     memset(&a, 0, sizeof(a));
@@ -509,6 +647,7 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
     a.n_img = n; a.H = H; a.W = W; a.ksize = L.ks; a.cin_blocks = L.cin_blocks;
     a.in_ch_base = wr.in_base; a.in_ch_group_stride = wr.in_group_stride; a.groups = L.groups;
     a.n_tile = L.n_tile; a.n_tiles = L.n_tiles; a.bias = L.bias.p; a.relu = L.relu; a.pool = L.pool;
+    a.slope = L.prelu ? L.slope.p : nullptr;
     {   // small batches: while the layer's CTAs fill at most half of the SMs, halve the work per CTA - 128-wide n-tiles become
         // 64-wide, then 32-wide (the weight layout does not depend on the n-tile)
         const int pix = n * ((H + kTileH - 1) / kTileH) * ((W + kTileW - 1) / kTileW);
@@ -526,14 +665,15 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         a.ea_out = net->ea.p + (size_t)slot * n;
     }
     if (tc_aux(p.fmt) == TcAux::kOverflow) a.ovf_out = net->ovf.p;
-    a.out = net->act[wr.out].p; a.out_cstride = kActC[wr.out];
+    a.out = net->act[wr.out].p; a.out_cstride = act_c(net, wr.out);
     a.out_ch_off[0] = wr.out_off[0]; a.out_ch_off[1] = wr.out_off[1];
     a.store_ch[0] = wr.store[0]; a.store_ch[1] = wr.store[1];
-    const int f32[2] = {wr.maps ? 2 * stage : -1, wr.maps ? 2 * stage + 1 : -1};
-    if (wr.maps) {
-        a.out_f32[0] = net->out_f32[f32[0]].p; a.out_f32[1] = net->out_f32[f32[1]].p;
-        a.f32_ch[0] = kPaf; a.f32_ch[1] = kHeat;
-    }
+    const int f32[2] = {wr.maps ? map0 : -1, wr.maps && L.groups == 2 ? map0 + 1 : -1};
+    for (int g = 0; g < 2; ++g)
+        if (f32[g] >= 0) {
+            a.out_f32[g] = net->out_f32[f32[g]].p;
+            a.f32_ch[g] = map_ch(net, f32[g]);
+        }
     // small batches (the 46 x 46 layers fill less than half of the SMs with 16 x 16 tiles): chain the layers with programmatic
     // dependent launches; the first tensor-core layer follows conv1_1, which does not signal.  small_plan gets this
     // layer's H, W and divides them by 8 again (DESIGN §2.1).
@@ -545,7 +685,7 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         in_lo = net->act_lo[wr.in].p;
         a.out_lo = net->act_lo[wr.out].p;
     }
-    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, kActC[wr.in], L.w[(int)tc_weights(p.fmt)].p, in_lo);
+    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, act_c(net, wr.in), L.w[(int)tc_weights(p.fmt)].p, in_lo);
     if (e != cudaSuccess) return cuda_fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
     p.launches.push_back({a, 2.0 * n * H * W * L.macs_per_pixel, wr.in, wr.out, {f32[0], f32[1]}});
     return 0;
@@ -570,12 +710,14 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
     const size_t px = (size_t)p.n * p.H * p.W;
     for (int plane = 0; plane < tc_planes(p.fmt); ++plane) {
         DevBuf<__nv_bfloat16>* bufs = plane ? net->act_lo : net->act;
-        for (int i = 0; i < kNumAct; ++i) CU(bufs[i].ensure(px / (kActDiv[i] * kActDiv[i]) * kActC[i]));
+        for (int i = 0; i < kNumAct; ++i) CU(bufs[i].ensure(px / (kActDiv[i] * kActDiv[i]) * act_c(net, i)));
         // pad lanes of the concat buffer must read as zero; on the caller's stream (a non-blocking stream is not ordered
         // against the legacy default stream a plain cudaMemset would use)
         CU(cudaMemsetAsync(bufs[CAT].p, 0, px / 64 * kActC[CAT] * 2, st));
+        if (is_openpose(net))     // ... and those of the 96-channel dense-block slots
+            for (int i : {BRA, BRB}) CU(cudaMemsetAsync(bufs[i].p, 0, px / 64 * act_c(net, i) * 2, st));
     }
-    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * (i % 2 == 0 ? kPaf : kHeat)));
+    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * map_ch(net, i)));
     if (tc_aux(p.fmt) == TcAux::kAmax) {     // rows for six stages whatever p.stages: plans of every stage count share them
         CU(net->amax.ensure((size_t)(1 + 51) * p.n));
         CU(net->ea.ensure((size_t)(1 + 51) * p.n));
@@ -591,9 +733,9 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
     int writer[kNumAct], cat_head = -1;
     for (int& w : writer) w = -1;
     writer[T1] = 0;
-    auto add = [&](const TcLayer& L, const Wiring& wr, int stage) {
+    auto add = [&](const TcLayer& L, const Wiring& wr, int map0) {
         const int ws[2] = {writer[wr.in], wr.in == CAT && wr.in_base == 0 ? cat_head : -1};
-        if (add_plan(net, p, L, wr, stage, ws)) return 1;
+        if (add_plan(net, p, L, wr, map0, ws)) return 1;
         if (wr.out == CAT && wr.maps) cat_head = (int)p.launches.size();
         else writer[wr.out] = (int)p.launches.size();
         return 0;
@@ -601,9 +743,15 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
     int k = 0;
     for (const Wiring& wr : kTrunkWiring)
         if (add(net->tc[k++], wr, 0)) return 1;
-    for (int s = 1; s <= p.stages; ++s)
-        for (int li = 0; li < stage_num_layers(s); ++li)
-            if (add(net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], s - 1)) return 1;
+    if (is_openpose(net)) {      // every stage, one after the other; stage t writes map t
+        for (int t = 0; t < net->l2 + net->l1; ++t)
+            for (int li = 0; li < kOpStageConvs; ++li)
+                if (add(net->tc[k++], op_wiring(net->l2, t, li), t)) return 1;
+    } else {
+        for (int s = 1; s <= p.stages; ++s)
+            for (int li = 0; li < stage_num_layers(s); ++li)
+                if (add(net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], 2 * (s - 1))) return 1;
+    }
     p.buffers = plan_buffers(net, p.fmt);
     return 0;
 }
@@ -712,20 +860,24 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
     CU(net->f_in.ensure(px1 * 3));
     CU(net->f_a.ensure(px1 * 64)); CU(net->f_b.ensure(px1 * 64));
     CU(net->f_cat.ensure(px8 * kCat)); CU(net->f_x.ensure(px8 * 512)); CU(net->f_y.ensure(px8 * 512));
-    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px8 * (i % 2 == 0 ? kPaf : kHeat)));
+    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px8 * map_ch(net, i)));
+    const bool op = is_openpose(net);
+    if (op) { CU(net->f_cat3.ensure(px8 * kCat)); CU(net->f_z.ensure(px8 * 512)); }
     CU(nchw_to_nhwc_f32_launch(d_in, net->f_in.p, n, 3, H, W, 3, 0, st));
     ++g_launches;
     const float* cur = net->f_in.p;
     int cur_c = 3, ch = H, cw = W;
     float* ping = net->f_a.p;
     float* pong = net->f_b.p;
+    // relu: the conv's ReLU (rtpose); a conv with PReLU slopes applies those instead
     auto conv = [&](int ci, const float* in, int in_cs, int in_off, float* out, int out_cs, int out_off, int hh, int ww,
                     int relu, float* nchw) -> int {
-        const ConvSpec s = conv_spec(ci);
+        const ConvSpec s = net_conv(net, ci);
         ConvF32Args a;
         a.in = in; a.in_cstride = in_cs; a.in_ch_off = in_off; a.w = net->d_w[ci].p; a.bias = net->d_b[ci].p;
         a.out = out; a.out_cstride = out_cs; a.out_ch_off = out_off; a.out_nchw = nchw;
         a.n_img = n; a.H = hh; a.W = ww; a.cin = s.cin; a.cout = s.cout; a.ks = s.ks; a.relu = relu;
+        a.slope = net->d_slope[ci].p;
         a.ext = ext;
         a.ext_shift = 0;
         while ((hh << a.ext_shift) < H) ++a.ext_shift;
@@ -737,7 +889,11 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
         const ConvSpec s = kTrunk[i];
         const bool last = (i == 11);
         float* dst = last ? net->f_cat.p : ping;
-        if (conv(i, cur, cur_c, 0, dst, last ? kCat : s.cout, last ? kPaf + kHeat : 0, ch, cw, 1, nullptr)) return 1;
+        // OpenPose_Model: the features go to cat[features, paf] at channel 0, and through f_z (NCHW) into
+        // cat[features, heat, paf]
+        const int cat_cs = op ? kFeat + kPaf : kCat, cat_off = op ? 0 : kPaf + kHeat;
+        if (conv(i, cur, cur_c, 0, dst, last ? cat_cs : s.cout, last ? cat_off : 0, ch, cw, 1, last && op ? net->f_z.p : nullptr))
+            return 1;
         cur = dst; cur_c = s.cout;
         std::swap(ping, pong);
         if (kPoolAfter[i]) {
@@ -746,6 +902,47 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
             cur = ping; ch /= 2; cw /= 2;
             std::swap(ping, pong);
         }
+    }
+    if (op) {
+        // inputs in the reference's channel order: f_cat = cat[features, paf], f_cat3 = cat[features, heat, paf]; a
+        // dense block's three outputs side by side in f_x (blocks 1, 3, 5) or f_y (2, 4); Mconv6 -> f_z; the head's
+        // NHWC output is scratch (f_y), its NCHW copy the stage map
+        constexpr int kCat2 = kFeat + kPaf, kCat3 = kFeat + kHeat + kPaf;
+        CU(nchw_to_nhwc_f32_launch(net->f_z.p, net->f_cat3.p, n, kFeat, h, w, kCat3, 0, st));
+        ++g_launches;
+        for (int t = 0; t < net->l2 + net->l1; ++t) {
+            const OpStage g = op_stage(net->l2, t);
+            const int ci0 = 12 + kOpStageConvs * t, cs = 3 * g.inner;
+            float* blk[2] = {net->f_x.p, net->f_y.p};
+            for (int li = 0; li < 15; ++li) {
+                const int b = li / 3, j = li % 3;
+                float* dst = blk[b % 2];
+                int rc;
+                if (li == 0) {
+                    const bool three = !g.paf && !g.first;
+                    rc = conv(ci0, three ? net->f_cat3.p : net->f_cat.p, three ? kCat3 : kCat2, 0, dst, cs, 0, h, w, 0, nullptr);
+                } else if (j == 0) {
+                    rc = conv(ci0 + li, blk[(b + 1) % 2], cs, 0, dst, cs, 0, h, w, 0, nullptr);
+                } else {
+                    rc = conv(ci0 + li, dst, cs, (j - 1) * g.inner, dst, cs, j * g.inner, h, w, 0, nullptr);
+                }
+                if (rc) return 1;
+            }
+            if (conv(ci0 + 15, net->f_x.p, cs, 0, net->f_z.p, g.innerout, 0, h, w, 0, nullptr)) return 1;
+            if (conv(ci0 + 16, net->f_z.p, g.innerout, 0, net->f_y.p, g.out, 0, h, w, 0, net->out_f32[t].p)) return 1;
+            // the next stages' inputs: an L2 head's PAF into cat[features, paf] (and the last one into
+            // cat[features, heat, paf]), an L1 head's heat map into cat[features, heat, paf]
+            if (g.paf) {
+                CU(nchw_to_nhwc_f32_launch(net->out_f32[t].p, net->f_cat.p, n, kPaf, h, w, kCat2, kFeat, st));
+                ++g_launches;
+            }
+            if (t == net->l2 - 1 || !g.paf) {
+                CU(nchw_to_nhwc_f32_launch(net->out_f32[t].p, net->f_cat3.p, n, g.out, h, w, kCat3,
+                                           g.paf ? kFeat + kHeat : kFeat, st));
+                ++g_launches;
+            }
+        }
+        return 0;
     }
     for (int s = 1; s <= stages; ++s)
         for (int b = 0; b < 2; ++b) {
@@ -788,7 +985,16 @@ int b200pose_net_tensor_shape(int index, long dims[4]) {
     return 1;
 }
 
-int b200pose_net_create(b200pose_net** out, int cuda_device) {
+int b200pose_openpose_num_tensors(int l2_stages, int l1_stages) {
+    return op_valid(l2_stages, l1_stages) ? op_num_tensors(l2_stages, l1_stages) : -1;
+}
+
+int b200pose_openpose_tensor_shape(int l2_stages, int l1_stages, int index, long dims[4]) {
+    return op_tensor_shape(l2_stages, l1_stages, index, dims);
+}
+
+// A net of architecture OpenPose_Model(l2, l1), or rtpose when l2 == 0.
+static int net_create(b200pose_net** out, int cuda_device, int l2, int l1) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return cuda_fail("b200pose: no CUDA device available (this library has no CPU fallback)");
@@ -800,13 +1006,30 @@ int b200pose_net_create(b200pose_net** out, int cuda_device) {
     b200pose_net* net = new b200pose_net();
     net->device = cuda_device;
     net->num_sms = prop.multiProcessorCount;
-    net->host_w.resize(kNumConvs);
-    net->host_b.resize(kNumConvs);
-    net->have.assign(B200POSE_NUM_TENSORS, false);
+    net->l2 = l2;
+    net->l1 = l1;
+    if (l2 > 0) net->stages = l2 + l1;     // the plan and graph keys' stage count: all of them, always
+    const int nc = net_num_convs(net);
+    net->host_w.resize(nc);
+    net->host_b.resize(nc);
+    net->host_slope.resize(nc);
+    net->d_w.resize(nc);
+    net->d_b.resize(nc);
+    net->d_slope.resize(nc);
+    net->have.assign(net_num_tensors(net), false);
     const char* gr = getenv("B200POSE_GRAPH");
     net->use_graph = !(gr && gr[0] == '0');
     *out = net;
     return 0;
+}
+
+int b200pose_net_create(b200pose_net** out, int cuda_device) { return net_create(out, cuda_device, 0, 0); }
+
+int b200pose_net_create_openpose(b200pose_net** out, int cuda_device, int l2_stages, int l1_stages) {
+    if (!op_valid(l2_stages, l1_stages))
+        return fail("OpenPose_Model(%d, %d): stages must be l2 >= 1, l1 >= 1, l2 + l1 <= %d", l2_stages, l1_stages,
+                    kOpMaxStages);
+    return net_create(out, cuda_device, l2_stages, l1_stages);
 }
 
 void b200pose_net_destroy(b200pose_net* net) {
@@ -818,12 +1041,16 @@ void b200pose_net_destroy(b200pose_net* net) {
 int b200pose_net_set_tensor(b200pose_net* net, int index, const float* host_data, long count) {
     if (!net || !host_data) return fail("set_tensor: null pointer");
     long dims[4];
-    const int nd = b200pose_net_tensor_shape(index, dims);
-    if (nd < 0) return fail("tensor index %d out of range", index);
+    const bool op = is_openpose(net);
+    const int nd = op ? op_tensor_shape(net->l2, net->l1, index, dims) : b200pose_net_tensor_shape(index, dims);
+    const std::string who = op ? arch_name(net) + ": " : "";
+    if (nd < 0) return fail("%stensor index %d out of range", who.c_str(), index);
     long expect = 1;
     for (int i = 0; i < nd; ++i) expect *= dims[i];
-    if (count != expect) return fail("tensor %d: got %ld elements, expected %ld", index, count, expect);
-    std::vector<float>& dst = (index % 2 == 0) ? net->host_w[index / 2] : net->host_b[index / 2];
+    if (count != expect) return fail("%stensor %d: got %ld elements, expected %ld", who.c_str(), index, count, expect);
+    int ci = index / 2, kind = index % 2;
+    if (op) op_tensor(net->l2, net->l1, index, &ci, &kind);
+    std::vector<float>& dst = kind == 0 ? net->host_w[ci] : (kind == 1 ? net->host_b[ci] : net->host_slope[ci]);
     dst.assign(host_data, host_data + count);
     net->have[index] = true;
     net->finalized = false;
@@ -833,30 +1060,55 @@ int b200pose_net_set_tensor(b200pose_net* net, int index, const float* host_data
 int b200pose_net_finalize(b200pose_net* net) {
     if (!net) return fail("null net");
     CU(cudaSetDevice(net->device));
-    for (int i = 0; i < B200POSE_NUM_TENSORS; ++i)
+    for (int i = 0; i < net_num_tensors(net); ++i)
         if (!net->have[i]) return fail("state_dict tensor %d was never set", i);
-    for (int i = 0; i < kNumConvs; ++i) {
+    for (int i = 0; i < net_num_convs(net); ++i) {
         // freed first, not reused: cudaFree synchronises the device, so a forward in flight on another stream has
         // stopped reading the weights before the synchronous copies below overwrite them
         net->d_w[i].release();
         net->d_b[i].release();
+        net->d_slope[i].release();
         CU(net->d_w[i].ensure(net->host_w[i].size()));
         CU(net->d_b[i].ensure(net->host_b[i].size()));
+        CU(net->d_slope[i].ensure(net->host_slope[i].size()));
         CU(cudaMemcpy(net->d_w[i].p, net->host_w[i].data(), net->host_w[i].size() * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(net->d_b[i].p, net->host_b[i].data(), net->host_b[i].size() * 4, cudaMemcpyHostToDevice));
+        if (!net->host_slope[i].empty())
+            CU(cudaMemcpy(net->d_slope[i].p, net->host_slope[i].data(), net->host_slope[i].size() * 4, cudaMemcpyHostToDevice));
     }
     net->tc.clear();
-    for (int i = 1; i < 12; ++i) {
-        const ConvSpec s = kTrunk[i];
-        net->tc.push_back(make_tc_layer({i}, s.cout < 128 ? s.cout : 128, false, 3, 1, kPoolAfter[i]));
+    if (is_openpose(net)) {
+        for (int i = 1; i < 12; ++i) {
+            const ConvSpec s = kTrunk[i];
+            const bool prelu = op_conv(net->l2, i).act == kPrelu;
+            net->tc.push_back(make_tc_layer(net, {i}, s.cout < 128 ? s.cout : 128, kPermNone, !prelu, kPoolAfter[i], prelu));
+        }
+        // n-tiles: 48 for the 96-channel convs (two tiles, no pad lanes), 128 for the others; the heads 64 (PAF: zero rows
+        // 38..63 store +0 over the heat slot) and 32 (heat map)
+        for (int t = 0; t < net->l2 + net->l1; ++t) {
+            const OpStage g = op_stage(net->l2, t);
+            for (int li = 0; li < kOpStageConvs; ++li) {
+                const int ci = 12 + kOpStageConvs * t + li;
+                const int n_tile = li == 16 ? (g.paf ? 64 : 32) : (li < 15 && g.inner == 96 ? 48 : 128);
+                InPerm perm = kPermNone;
+                if (li == 0 && t > 0) perm = g.paf || g.first ? kPermFeatPaf : kPermFeatHeatPaf;
+                else if (li == 15 || (li > 0 && li % 3 == 0)) perm = kPermSlots;
+                net->tc.push_back(make_tc_layer(net, {ci}, n_tile, perm, 0, 0, op_conv(net->l2, ci).act == kPrelu));
+            }
+        }
+    } else {
+        for (int i = 1; i < 12; ++i) {
+            const ConvSpec s = kTrunk[i];
+            net->tc.push_back(make_tc_layer(net, {i}, s.cout < 128 ? s.cout : 128, kPermNone, 1, kPoolAfter[i]));
+        }
+        for (int li = 0; li < 5; ++li)
+            net->tc.push_back(make_tc_layer(net, {conv_index(1, 0, li), conv_index(1, 1, li)}, li == 4 ? 48 : 128, kPermNone,
+                                            li != 4, 0));
+        for (int st = 2; st <= 6; ++st)
+            for (int li = 0; li < 7; ++li)
+                net->tc.push_back(make_tc_layer(net, {conv_index(st, 0, li), conv_index(st, 1, li)}, li == 6 ? 48 : 128,
+                                                li == 0 ? kPermRtposeCat : kPermNone, li != 6, 0));
     }
-    for (int li = 0; li < 5; ++li)
-        net->tc.push_back(make_tc_layer({conv_index(1, 0, li), conv_index(1, 1, li)}, li == 4 ? 48 : 128, false,
-                                        stage_layer(1, 0, li).ks, li != 4, 0));
-    for (int st = 2; st <= 6; ++st)
-        for (int li = 0; li < 7; ++li)
-            net->tc.push_back(make_tc_layer({conv_index(st, 0, li), conv_index(st, 1, li)}, li == 6 ? 48 : 128, li == 0,
-                                            stage_layer(st, 0, li).ks, li != 6, 0));
     for (TcLayer& L : net->tc)
         if (ensure_packed(net, L, TcFormat::kBf16)) return 1;
     net->last = LastForward();
@@ -870,9 +1122,21 @@ int b200pose_net_finalize(b200pose_net* net) {
 // Entries of outputs[12] for stages the net does not run must be NULL: a caller must not read a map no stage wrote as if
 // it were fresh.
 static int check_outputs(const b200pose_net* net, float* const* outputs) {
-    for (int i = 2 * net->stages; outputs && i < 12; ++i)
-        if (outputs[i])
+    for (int i = net_num_maps(net, net->stages); outputs && i < 12; ++i)
+        if (outputs[i]) {
+            if (is_openpose(net))
+                return fail("outputs[%d] must be NULL: %s writes %d maps", i, arch_name(net).c_str(), net->l2 + net->l1);
             return fail("outputs[%d] must be NULL: the net runs %d stage(s), stage %d does not run", i, net->stages, i / 2 + 1);
+        }
+    return 0;
+}
+
+// OpenPose_Model nets run the bf16, bf16x3 and fp32 modes; the fp8 and fp16 modes (their per-launch tables follow
+// rtpose's launch list) are refused before anything is enqueued.
+static int check_mode(const b200pose_net* net, int mode) {
+    if (is_openpose(net) && (mode == B200POSE_MODE_FP8 || mode == B200POSE_MODE_FP16))
+        return fail("%s runs modes bf16, bf16x3 and fp32, not %s", arch_name(net).c_str(),
+                    mode == B200POSE_MODE_FP8 ? "fp8" : "fp16");
     return 0;
 }
 
@@ -883,6 +1147,7 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
     if (!net || !net->finalized) return fail("net not finalized");
     if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
     if (int rc = check_outputs(net, outputs)) return rc;
+    if (int rc = check_mode(net, mode)) return rc;
     const int stages = net->stages;
     CU(cudaSetDevice(net->device));
     const void* d_in = input;
@@ -918,9 +1183,9 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
     net->last = LastForward{n, H, W, mode == B200POSE_MODE_FP32, fmt, stages, d_in, first_u8, ext};
     if (outputs) {
         const size_t px8 = (size_t)n * (H / 8) * (W / 8);
-        for (int i = 0; i < 2 * stages; ++i)
+        for (int i = 0; i < net_num_maps(net, stages); ++i)
             if (outputs[i])
-                CU(cudaMemcpyAsync(outputs[i], net->out_f32[i].p, px8 * (i % 2 == 0 ? kPaf : kHeat) * 4,
+                CU(cudaMemcpyAsync(outputs[i], net->out_f32[i].p, px8 * map_ch(net, i) * 4,
                                    outputs_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
     }
     if (sync_host && (!input_on_device || (outputs && !outputs_on_device))) CU(cudaStreamSynchronize(st));
@@ -1013,6 +1278,7 @@ int b200pose_net_forward_ragged_u8(b200pose_net* net, const unsigned char* frame
     if (!net || !net->finalized) return fail("net not finalized");
     if (!frames) return fail("forward_ragged: null pointer");
     if (int rc = check_outputs(net, outputs)) return rc;
+    if (int rc = check_mode(net, mode)) return rc;
     int Hc, Wc;
     if (int rc = ragged_canvas(n, hw, &Hc, &Wc)) return rc;
     CU(cudaSetDevice(net->device));
@@ -1045,6 +1311,8 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess) {
 
 int b200pose_net_set_stages(b200pose_net* net, int stages) {
     if (!net) return fail("null net");
+    if (is_openpose(net))
+        return fail("%s: the stage count is the architecture's (set at b200pose_net_create_openpose)", arch_name(net).c_str());
     if (stages < 1 || stages > kStages) return fail("stages must be 1 .. %d, got %d", kStages, stages);
     net->stages = stages;
     return 0;
@@ -1119,7 +1387,7 @@ int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
     } else {
         const PlanLaunch& l = p.launches[i - 1];
         const ConvTcArgs& a = l.a;
-        f[0] = l.in; f[1] = kActC[l.in]; f[2] = a.in_ch_base; f[3] = a.in_ch_group_stride;
+        f[0] = l.in; f[1] = act_c(net, l.in); f[2] = a.in_ch_base; f[3] = a.in_ch_group_stride;
         f[4] = l.out; f[5] = a.out_cstride; f[6] = a.out_ch_off[0]; f[7] = a.out_ch_off[1];
         f[8] = a.store_ch[0]; f[9] = a.store_ch[1];
         f[10] = a.H; f[11] = a.W; f[12] = a.ksize; f[13] = a.cin_blocks; f[14] = a.groups; f[15] = a.n_tile;
@@ -1140,13 +1408,13 @@ int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, 
     size_t per = 0;
     if (buf >= 0 && buf < kNumAct) {
         if (lo_plane && tc_planes(net->plan->fmt) < 2) return fail("debug_read: residual planes exist in bf16x3 mode only");
-        per = (size_t)(H / kActDiv[buf]) * (W / kActDiv[buf]) * kActC[buf] * 2;
+        per = (size_t)(H / kActDiv[buf]) * (W / kActDiv[buf]) * act_c(net, buf) * 2;
         src = reinterpret_cast<const char*>((lo_plane ? net->act_lo : net->act)[buf].p);
     } else if (buf >= kNumAct && buf < kNumAct + 12 && !lo_plane) {
         const int m = buf - kNumAct;
-        if (m >= 2 * net->last.stages)
+        if (m >= net_num_maps(net, net->last.stages))
             return fail("debug_read: stage map %d was not written by the last forward (%d stages)", m, net->last.stages);
-        per =(size_t)(H / 8) * (W / 8) * (m % 2 == 0 ? kPaf : kHeat) * 4;
+        per =(size_t)(H / 8) * (W / 8) * map_ch(net, m) * 4;
         src = reinterpret_cast<const char*>(net->out_f32[m].p);
     } else {
         return fail("debug_read: no buffer %d (plane %d)", buf, lo_plane);
@@ -1512,11 +1780,11 @@ int b200pose_flip_merge(b200pose_post* p, const float* normal_heat, const float*
 // Every fused entry point checks its handles, stages its frames (with their mirror images when flip), runs the
 // forward pass and finishes with finish_infer.
 
-static int check_infer(const b200pose_net* net, const b200pose_post* post) {
+static int check_infer(const b200pose_net* net, const b200pose_post* post, int mode) {
     if (!net || !post) return fail("null handle");
     if (!net->finalized) return fail("net not finalized");
     if (net->device != post->device) return fail("net and post live on different devices");
-    return 0;
+    return check_mode(net, mode);
 }
 
 // fp16: behind a fused run's forward of nimg images, copies the net's overflow flags into the next row of the run's slot
@@ -1556,7 +1824,7 @@ static int finish_infer(const b200pose_net* net, b200pose_post* post, int n, int
 
 static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input, int in_u8, int input_on_device, int n,
                       int H, int W, int mode, float thresh, int flip, void* cuda_stream) {
-    if (int rc = check_infer(net, post)) return rc;
+    if (int rc = check_infer(net, post, mode)) return rc;
     if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
     if (int rc = check_batch(post, n)) return rc;
     post->ovf_pending = 0;
@@ -1808,7 +2076,7 @@ static int stage_frames(b200pose_net* net, const FrameBatch& b, int on_device, i
 static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char* images, int on_device, int n,
                      int src_h, int src_w, const int* src_hw, int base_size, int factor, const double* scales,
                      int n_scales, int mode, float thresh, int flip, void* cuda_stream, const FrameBatch* fb = nullptr) {
-    if (int rc = check_infer(net, post)) return rc;
+    if (int rc = check_infer(net, post, mode)) return rc;
     if (!images && !fb) return fail("infer_raw: null pointer");
     if (scales && (n_scales < 1 || n_scales > 16)) return fail("infer_raw: %d scales (1 .. 16)", n_scales);
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
@@ -1943,7 +2211,7 @@ int b200pose_net_convert_frames(b200pose_net* net, const b200pose_frame* frames,
 int b200pose_infer_frames(b200pose_net* net, b200pose_post* post, const b200pose_frame* frames, int n, int format,
                           int on_device, int rotate, int dest_size, int factor, const double* scales, int n_scales,
                           int mode, float thresh, int flip, void* cuda_stream) {
-    if (int rc = check_infer(net, post)) return rc;
+    if (int rc = check_infer(net, post, mode)) return rc;
     FrameBatch b;
     if (int rc = check_frames(frames, n, post->pb.batch_cap, format, rotate, &b)) return rc;
     if (flip && 2 * n > kMaxRagged) return fail("frames: %d frames with flip (2n <= %d)", n, kMaxRagged);

@@ -312,6 +312,8 @@ __global__ void __launch_bounds__(kF_Threads) conv_first_mma_kernel(const void* 
 constexpr int kR_Threads = 256;
 constexpr int kR_KC = 16;   // input channels per smem chunk
 
+// kPrelu: a.slope's PReLU instead of a.relu (its own instantiation: the ReLU kernel keeps its machine code)
+template <bool kPrelu>
 __global__ void __launch_bounds__(kR_Threads) conv_f32_kernel(ConvF32Args a) {
     __shared__ float s_a[kR_KC][64 + 4];     // [cin][pixel]
     __shared__ float s_b[kR_KC][64 + 4];     // [cin][cout]
@@ -376,7 +378,8 @@ __global__ void __launch_bounds__(kR_Threads) conv_f32_kernel(ConvF32Args a) {
             const int o = co0 + cg * 4 + j;
             if (o >= a.cout) continue;
             float v = acc[i][j] + a.bias[o];
-            if (a.relu) v = fmaxf(v, 0.f);
+            if constexpr (kPrelu) v = v > 0.f ? v : __fmul_rn(a.slope[o], v);
+            else if (a.relu) v = fmaxf(v, 0.f);
             if (!inside) v = 0.f;
             a.out[(((size_t)n * a.H + y) * a.W + x) * a.out_cstride + a.out_ch_off + o] = v;
             if (a.out_nchw) a.out_nchw[(((size_t)n * a.cout + o) * a.H + y) * a.W + x] = v;
@@ -478,7 +481,8 @@ cudaError_t u8hwc_to_f32nchw_launch(const unsigned char* in, float* out, int N, 
 cudaError_t conv_f32_launch(const ConvF32Args& a, cudaStream_t s) {
     const int tiles = ((a.W + 7) / 8) * ((a.H + 7) / 8);
     dim3 grid(tiles, (a.cout + 63) / 64, a.n_img);
-    conv_f32_kernel<<<grid, kR_Threads, 0, s>>>(a);
+    if (a.slope) conv_f32_kernel<true><<<grid, kR_Threads, 0, s>>>(a);
+    else conv_f32_kernel<false><<<grid, kR_Threads, 0, s>>>(a);
     return cudaGetLastError();
 }
 

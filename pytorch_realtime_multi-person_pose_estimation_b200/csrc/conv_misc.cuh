@@ -18,6 +18,8 @@ struct ConvF32Args {
     int n_img, H, W, cin, cout, ks, relu;
     const int* ext;       // ragged batch (DESIGN.md §1): padded H, W per image at the network input, or null
     int ext_shift;        // log2 of the network input size over H, W
+    const float* slope;   // PReLU slope per output channel (OpenPose_Model): v = v > 0 ? v : slope * v after the bias,
+                          // instead of `relu`; null: relu / none
 };
 
 // conv1_1 in format fmt.  in: fp32 NCHW [N,3,H,W] (in_is_u8_hwc = 0), or uint8 HWC BGR [N,H,W,3] with the

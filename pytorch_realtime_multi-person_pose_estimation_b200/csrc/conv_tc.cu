@@ -85,7 +85,9 @@ constexpr int kConsumerWarps = 8;
 // and the epilogue records the per-image max |stored bf16|.
 // fp16: the bf16 plan with binary16 activations and weights (same fragments, same full-K fp32 accumulation); the
 // epilogue stores binary16 and flags every image for which a stored value is +-inf or NaN.
-template <TcFormat F, int N, bool kRagged>
+// kPrelu: the epilogue applies the per-channel PReLU of a.slope instead of a.relu (a separate instantiation, so that the
+// kernels without it keep their machine code).
+template <TcFormat F, int N, bool kRagged, bool kPrelu>
 __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     constexpr bool kChunk = tc_chunked(F);
     constexpr bool kE4m3 = tc_weights(F) == TcWeights::kE4m3;
@@ -338,6 +340,13 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                                          (e & 1) ? b2.y : b2.x);
                         if (a.relu) v[e] = fmaxf(v[e], 0.f);
                     }
+                } else if constexpr (kPrelu) {    // torch's prelu: one multiply, after the bias
+                    const float2 s2 = __ldg(reinterpret_cast<const float2*>(a.slope + (tc.g * a.n_tiles + tc.nt) * N + 8 * j + cq));
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const float u = (kChunk ? sum[4 * j + e] : acc[4 * j + e]) + ((e & 1) ? b2.y : b2.x);
+                        v[e] = u > 0.f ? u : __fmul_rn((e & 1) ? s2.y : s2.x, u);
+                    }
                 } else {
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
@@ -396,9 +405,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
     if (threadIdx.x == 0) B2P_TL(9);
 }
 
-template <TcFormat F, int N, bool kRagged>
+template <TcFormat F, int N, bool kRagged, bool kPrelu>
 __global__ void __launch_bounds__(kConvTcThreads, 1) conv_tc_kernel(const __grid_constant__ ConvTcArgs a) {
-    conv_tc_body<F, N, kRagged>(a);
+    conv_tc_body<F, N, kRagged, kPrelu>(a);
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -478,11 +487,18 @@ namespace {
 // plans only, where the fixed cost per launch is most of a layer.
 template <TcFormat F, int N>
 cudaError_t launch_k(int grid, cudaStream_t stream, const ConvTcArgs& a) {
-    // per kernel (uniform, ragged) and device: a second net on another GPU of the same process needs its own opt-in
-    static DynSmemOptIn optin[2];
+    // per kernel (uniform, ragged; PReLU) and device: a second net on another GPU of the same process needs its own opt-in
+    static DynSmemOptIn optin[4];
     const bool ragged = a.ext != nullptr;
-    void (*kernel)(ConvTcArgs) = ragged ? conv_tc_kernel<F, N, true> : conv_tc_kernel<F, N, false>;
-    cudaError_t e = optin[ragged].ensure(kernel, kConvTcSmemBytes);
+    const bool prelu = a.slope != nullptr;
+    void (*kernel)(ConvTcArgs) = ragged ? conv_tc_kernel<F, N, true, false> : conv_tc_kernel<F, N, false, false>;
+    if (prelu) {      // PReLU (OpenPose_Model's plans) in the formats those plans run: bf16, bf16x3
+        if constexpr (tc_weights(F) == TcWeights::kBf16HiLo)
+            kernel = ragged ? conv_tc_kernel<F, N, true, true> : conv_tc_kernel<F, N, false, true>;
+        else
+            return cudaErrorInvalidValue;
+    }
+    cudaError_t e = optin[2 * prelu + ragged].ensure(kernel, kConvTcSmemBytes);
     if (e != cudaSuccess) return e;
     if (a.pdl) {
         cudaLaunchConfig_t cfg = {};

@@ -75,6 +75,9 @@ struct ConvTcArgs {
     int* ea_out;                  // the activation exponent each image used (may be null)
     // ---- fp16 (DESIGN.md §2.3): binary16 activations (`in`, `out`) and weights, full-K fp32 accumulation
     unsigned* ovf_out;            // per image: set to 1 when a value the launch stores is +-inf or NaN in binary16
+    // ---- PReLU (OpenPose_Model, DESIGN.md §2.11): per output channel slope, laid out like `bias`; null = relu / none.
+    // v = acc + bias; v = v > 0 ? v : slope * v.  Selects the PReLU kernel (bf16 and bf16x3 only).
+    const float* slope;
 };
 
 // Builds the tensor maps and sets a.tps and a.split from a.fmt. `in` (and `in_lo` in bf16x3): NHWC buffers with

@@ -132,18 +132,38 @@ def rotated_size(h, w, rotate):
 
 
 class NativeNet:
-    """Owns a b200pose_net handle on one CUDA device."""
+    """Owns a b200pose_net handle on one CUDA device: the rtpose VGG19 network, or OpenPose_Model(l2, l1) for a net
+    made by NativeNet.openpose."""
 
-    def __init__(self, device_index):
+    openpose_stages = None       # (l2_stages, l1_stages) of an OpenPose_Model net
+
+    def __init__(self, device_index, openpose=None):
         self._h = ctypes.c_void_p()
-        nat.check(nat.lib().b200pose_net_create(ctypes.byref(self._h), int(device_index)), "b200pose_net_create")
+        if openpose is None:
+            nat.check(nat.lib().b200pose_net_create(ctypes.byref(self._h), int(device_index)), "b200pose_net_create")
+        else:
+            l2, l1 = (int(v) for v in openpose)
+            nat.check(nat.lib().b200pose_net_create_openpose(ctypes.byref(self._h), int(device_index), l2, l1),
+                      "b200pose_net_create_openpose")
+            self.openpose_stages = (l2, l1)
         self.device_index = int(device_index)
 
+    @classmethod
+    def openpose(cls, device_index=0, l2_stages=4, l1_stages=2):
+        """A net of the reference's OpenPose_Model(l2_stages, l1_stages, 38, 19) (lib/network/openpose.py): load its
+        state dict with load_state_dict_arrays (or use openpose_engine, which checks the names too)."""
+        return cls(device_index, openpose=(l2_stages, l1_stages))
+
+    @property
+    def num_tensors(self):
+        return nat.NUM_TENSORS if self.openpose_stages is None else len(nat.openpose_shapes(*self.openpose_stages))
+
     def load_state_dict_arrays(self, arrays):
-        """arrays: 184 float32 numpy arrays in the reference state_dict order."""
+        """arrays: the net's state_dict tensors as float32 numpy arrays in the reference's order (rtpose: 184)."""
         L = nat.lib()
-        if len(arrays) != nat.NUM_TENSORS:
-            raise nat.B200PoseError("expected %d tensors, got %d" % (nat.NUM_TENSORS, len(arrays)))
+        if len(arrays) != self.num_tensors:
+            what = "rtpose" if self.openpose_stages is None else "OpenPose_Model(%d, %d)" % self.openpose_stages
+            raise nat.B200PoseError("%s: expected %d tensors, got %d" % (what, self.num_tensors, len(arrays)))
         for i, a in enumerate(arrays):
             a = np.ascontiguousarray(a, dtype=np.float32)
             nat.check(L.b200pose_net_set_tensor(self._h, i, a.ctypes.data, a.size), "set_tensor(%d)" % i)
@@ -396,20 +416,31 @@ def humans_to_dicts(rows, width, height):
 
 class PoseEngine:
     """Fused batched inference on one GPU: images -> humans, maps never leave the device.  `stages`: the refinement
-    stages each submission runs (1 .. 6); the fused entry points post-process the last one's maps.  `post_params`: the
+    stages each submission runs (1 .. 6, default 6); the fused entry points post-process the last one's maps.  On an
+    OpenPose_Model net (NativeNet.openpose) the count is the architecture's: `stages` must stay None, and modes fp8 /
+    fp16 are refused here.  `post_params`: the
     post-processing settings of the submissions (a dict of NativePost.set_params' fields; None: the reference's
     constants), changed later with set_post_params."""
 
     stages = 6
 
     def __init__(self, state_arrays, device_index=0, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, net=None,
-                 stages=6, post_params=None):
+                 stages=None, post_params=None):
         if net is None:
             net = NativeNet(device_index)
             net.load_state_dict_arrays(state_arrays)
         self.net = net
-        self.stages = int(stages)
-        self.net.set_stages(self.stages)      # an invalid count fails here, before any submission
+        if net.openpose_stages is not None:
+            # the stage count is the architecture's: the engine never sets one; fp8 / fp16 do not run on such a net
+            what = "OpenPose_Model(%d, %d)" % net.openpose_stages
+            if stages is not None:
+                raise nat.B200PoseError("%s runs all its stages; stages=%r cannot be set" % (what, stages))
+            if mode in ("fp8", "fp16"):
+                raise nat.B200PoseError("%s runs modes bf16, bf16x3 and fp32, not %s" % (what, mode))
+            self.stages = None
+        else:
+            self.stages = 6 if stages is None else int(stages)
+            self.net.set_stages(self.stages)      # an invalid count fails here, before any submission
         self.post = NativePost(device_index, batch_cap, peak_cap, human_cap)
         if post_params:
             self.post.set_params(**post_params)
@@ -420,8 +451,9 @@ class PoseEngine:
 
     def _net_h(self):
         """The net's handle, set to this engine's stage count: engines may share a net with each other and with the
-        module (rtpose_model.pose_engine), so the count is set before every submission."""
-        self.net.set_stages(self.stages)
+        module (rtpose_model.pose_engine), so the count is set before every submission (not on an OpenPose_Model net)."""
+        if self.net.openpose_stages is None:
+            self.net.set_stages(self.stages)
         return self.net._h
 
     def set_post_params(self, params=None, **fields):
@@ -450,7 +482,7 @@ class PoseEngine:
         return self._shapes[ticket]
 
     @classmethod
-    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=6, post_params=None):
+    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=None, post_params=None):
         """An engine around an existing NativeNet (e.g. the one a get_model() module already packed its weights into)."""
         return cls(None, net.device_index, mode, batch_cap, peak_cap, human_cap, net=net, stages=stages,
                    post_params=post_params)
@@ -694,3 +726,54 @@ class PoseEngine:
             self._keep = images
             run_f32(images.data_ptr(), True, n, H, W, thresh, torch.cuda.current_stream().cuda_stream)
         return self.fetch()
+
+
+def openpose_state_dict_keys(l2_stages=4, l1_stages=2):
+    """The state_dict keys of the reference's OpenPose_Model(l2_stages, l1_stages) (lib/network/openpose.py), in order:
+    feature_extractor (make_vgg19_block's Sequential: conv / ReLU / pool entries, PReLU after conv4_2, conv4_3_CPM and
+    conv4_4_CPM), then l2_stages.{i} and l1_stages.{i} (StageBlock: Mconv{b}_{j}.Mconv / .MPrelu, Mconv6, Mconv7)."""
+    keys, idx = [], 0
+    for name in ("1_1", "1_2", "P", "2_1", "2_2", "P", "3_1", "3_2", "3_3", "3_4", "P", "4_1", "4_2", "4_3", "4_4"):
+        if name == "P":
+            idx += 1
+            continue
+        keys += ["feature_extractor.%d.weight" % idx, "feature_extractor.%d.bias" % idx]
+        if name in ("4_2", "4_3", "4_4"):
+            keys.append("feature_extractor.%d.weight" % (idx + 1))
+        idx += 2
+    for branch, count in (("l2_stages", l2_stages), ("l1_stages", l1_stages)):
+        for i in range(count):
+            for blk in ["Mconv%d_%d" % (b, j) for b in range(1, 6) for j in range(3)] + ["Mconv6"]:
+                p = "%s.%d.%s." % (branch, i, blk)
+                keys += [p + "Mconv.weight", p + "Mconv.bias", p + "MPrelu.weight"]
+            keys += ["%s.%d.Mconv7.weight" % (branch, i), "%s.%d.Mconv7.bias" % (branch, i)]
+    return keys
+
+
+def openpose_engine(state_dict, l2_stages=4, l1_stages=2, device_index=0, mode="bf16", **engine_kwargs):
+    """A PoseEngine running the reference's OpenPose_Model(l2_stages, l1_stages, 38, 19) with `state_dict` (its
+    state_dict(), or any mapping of the same keys, in the same order, to tensors or arrays).  Every key and shape is
+    checked against the model's - names from openpose_state_dict_keys, shapes from the library's table - and the first
+    mismatch is named.  Modes bf16, bf16x3 and fp32; engine_kwargs as for PoseEngine (batch_cap, post_params, ...)."""
+    keys = openpose_state_dict_keys(l2_stages, l1_stages)
+    shapes = nat.openpose_shapes(l2_stages, l1_stages)
+    what = "OpenPose_Model(%d, %d)" % (l2_stages, l1_stages)
+    items = list(state_dict.items())
+    arrays = []
+    for i, want in enumerate(keys):
+        if i >= len(items):
+            raise nat.B200PoseError("%s state_dict: entry %d %r is missing (%d entries given, %d expected)"
+                                    % (what, i, want, len(items), len(keys)))
+        k, v = items[i]
+        if k != want:
+            raise nat.B200PoseError("%s state_dict: entry %d is %r, expected %r" % (what, i, k, want))
+        a = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
+        if tuple(a.shape) != shapes[i]:
+            raise nat.B200PoseError("%s state_dict: %r has shape %s, expected %s" % (what, k, tuple(a.shape), shapes[i]))
+        arrays.append(np.ascontiguousarray(a, dtype=np.float32))
+    if len(items) > len(keys):
+        raise nat.B200PoseError("%s state_dict: unexpected entry %d %r (%d expected)" % (what, len(keys), items[len(keys)][0],
+                                                                                      len(keys)))
+    net = NativeNet.openpose(device_index, l2_stages, l1_stages)
+    net.load_state_dict_arrays(arrays)
+    return PoseEngine.from_net(net, mode=mode, **engine_kwargs)

@@ -28,7 +28,9 @@ def frames_of(capture, rotate_code=None, limit=None):
 class PoseStream:
     """for frame, humans, drawn in PoseStream(model, frames, batch=8): ...
 
-    model: a module from lib.network.rtpose_vgg.get_model() (bare or DataParallel-wrapped) on a CUDA device.
+    model: a module from lib.network.rtpose_vgg.get_model() (bare or DataParallel-wrapped) on a CUDA device, or a
+    PoseEngine (e.g. engine.openpose_engine's, to run OpenPose_Model); the stream then runs on that engine's net and
+    post-processing, and submits batches of at most its batch_cap frames.
     frames: any iterator of uint8 BGR frames of ONE shape.  batch=1 minimises latency (camera), larger batches raise
     throughput (files).  `draw=False` skips the rendering.
     format 'nv12' / 'i420' (frames as PoseEngine.infer_frames_async takes them, e.g. decoder surfaces already on the GPU)
@@ -38,10 +40,14 @@ class PoseStream:
 
     def __init__(self, model, frames, batch=8, preprocess='rtpose', dest_size=368, factor=8, thresh=0.1, draw=True,
                  format='bgr', rotate=None):
-        core = getattr(model, "module", model)
-        if not hasattr(core, "pose_engine"):
-            raise nat.B200PoseError("PoseStream needs a model from lib.network.rtpose_vgg.get_model()")
-        self.engine = core.pose_engine(batch_cap=max(1, int(batch)))
+        if isinstance(model, engine.PoseEngine):
+            self.engine = model
+            batch = min(max(1, int(batch)), model.post.batch_cap)
+        else:
+            core = getattr(model, "module", model)
+            if not hasattr(core, "pose_engine"):
+                raise nat.B200PoseError("PoseStream needs a model from lib.network.rtpose_vgg.get_model() or a PoseEngine")
+            self.engine = core.pose_engine(batch_cap=max(1, int(batch)))
         self.engine.net.set_preprocess(preprocess)
         self.frames, self.batch = iter(frames), max(1, int(batch))
         self.dest_size, self.factor, self.thresh, self.draw = dest_size, factor, thresh, draw

@@ -19,6 +19,32 @@ def he_state_arrays(seed=1234):
     return out
 
 
+def openpose_state_dict(l2_stages=4, l1_stages=2, seed=2024):
+    """Seeded weights for OpenPose_Model(l2_stages, l1_stages, 38, 19), an OrderedDict in its state_dict order (keys:
+    engine.openpose_state_dict_keys, shapes: the library's table).  PReLU slopes ~ U(-0.5, 1.5) - negative and steeper
+    than 1, so that a PReLU mistake shows - biases U(-0.1, 0.1), weights N(0, g / fan_in) with the gain that keeps the
+    activations' variance through the conv's activation: 2 for ReLU and for none, 2 / (1 + 7/12) for PReLU (He's rule;
+    7/12 is the slopes' mean square), so that 90 layers neither explode nor vanish."""
+    from collections import OrderedDict
+    from . import _native as nat
+    from .engine import openpose_state_dict_keys
+    keys = openpose_state_dict_keys(l2_stages, l1_stages)
+    shapes = nat.openpose_shapes(l2_stages, l1_stages)
+    g = torch.Generator().manual_seed(seed)
+    sd = OrderedDict()
+    for i, (key, shape) in enumerate(zip(keys, shapes)):
+        if len(shape) == 4:
+            # a conv's tensors are weight, bias and, with a PReLU after it, the slope
+            prelu = i + 2 < len(keys) and len(shapes[i + 2]) == 1 and not keys[i + 2].endswith("bias")
+            gain = 2.0 / (1.0 + 7.0 / 12.0) if prelu else 2.0
+            sd[key] = torch.randn(shape, generator=g) * float(np.sqrt(gain / (shape[1] * shape[2] * shape[3])))
+        elif key.endswith("bias"):
+            sd[key] = torch.rand(shape, generator=g) * 0.2 - 0.1
+        else:
+            sd[key] = torch.rand(shape, generator=g) * 2.0 - 0.5
+    return sd
+
+
 # 18 COCO parts of a schematic standing person in a unit box, and the 19 limbs / their PAF channel pairs in the order of
 # pafprocess.h:16-24 (the layout SURVEY.md appendix B pins).
 _BODY = ((.50, .08), (.50, .22), (.36, .22), (.30, .40), (.27, .56), (.64, .22), (.70, .40), (.73, .56), (.42, .55),
