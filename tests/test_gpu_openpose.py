@@ -42,14 +42,15 @@ def net(pe):
 def _maps(net, mode, x=None, frames=None, shapes=None):
     """The l2 + l1 maps (device tensors) of a forward of fp32 NCHW x, uint8 frames [n,H,W,3] or a ragged batch."""
     nat = _nat()
+    l2, l1 = net.openpose_stages
     if x is not None:
         n, _, H, W = x.shape
     elif shapes is None:
         n, H, W = frames.shape[:3]
     else:
         n, H, W = len(shapes), max(s[0] for s in shapes), max(s[1] for s in shapes)
-    outs = [torch.empty((n, 38 if i < L2 else 19, H // 8, W // 8), device="cuda") for i in range(L2 + L1)]
-    ptrs = [o.data_ptr() for o in outs] + [0] * (12 - L2 - L1)
+    outs = [torch.empty((n, 38 if i < l2 else 19, H // 8, W // 8), device="cuda") for i in range(l2 + l1)]
+    ptrs = [o.data_ptr() for o in outs] + [0] * (12 - l2 - l1)
     st = torch.cuda.current_stream().cuda_stream
     if x is not None:
         net.forward_ptr(x.data_ptr(), True, n, H, W, nat.MODES[mode], ptrs, True, st)
@@ -166,7 +167,7 @@ def _assert_same(got, want, what):
 def _final(net, mode, crops):
     """(heat_l1, paf_l2) of padded uint8 frames [n,H,W,3], NCHW host float32."""
     outs = _maps(net, mode, frames=torch.from_numpy(np.ascontiguousarray(crops)).cuda())
-    return outs[-1].cpu().numpy(), outs[L2 - 1].cpu().numpy()
+    return outs[-1].cpu().numpy(), outs[net.openpose_stages[0] - 1].cpu().numpy()
 
 
 def _engine(net, mode):
@@ -178,6 +179,27 @@ def _crop(net, frames, dest):
     return net.crop_with_factor(np.ascontiguousarray(frames), dest, 8)[0]
 
 
+def _check_u8_flip_and_ragged(pe, ref, net, mode, frames, mixed):
+    """infer_u8, infer_u8_flip and infer_images on mixed sizes (one ragged batch) against the composed path: forward,
+    flip merge, post-processing; each ragged frame as it comes out alone.  Returns the peaks of infer_u8."""
+    label = "OpenPose_Model(%d, %d) %s" % (net.openpose_stages + (mode,))
+    n, H, W = frames.shape[:3]
+    pe.infer_async_u8(frames.ctypes.data, False, n, H, W)
+    want = _post(ref, *_final(net, mode, frames))
+    _assert_same(_fused(pe, n), want, "%s infer_u8" % label)
+    peaks = sum(len(p) for p in want[1])
+    pe.infer_flip_async_u8(frames.ctypes.data, False, n, H, W)
+    got = _fused(pe, n)
+    heat, paf = _final(net, mode, np.concatenate([frames, frames[:, :, ::-1]]))
+    mp, mh = ref.flip_merge(heat[:n], heat[n:], paf[:n], paf[n:], layout=0)
+    _assert_same(got, _post(ref, mh, mp), "%s infer_u8_flip" % label)
+    got = pe.infer_images_arrays(mixed, 96, 8)
+    for i, f in enumerate(mixed):
+        want = _post(ref, *_final(net, mode, _crop(net, f[None], 96)))
+        np.testing.assert_array_equal(got[i], want[0][0], err_msg="%s infer_images frame %d" % (label, i))
+    return peaks
+
+
 @pytest.mark.parametrize("mode", MODES)
 def test_fused_entry_points_equal_the_composed_path(net, mode):
     eng = pkg_module("engine")
@@ -187,23 +209,7 @@ def test_fused_entry_points_equal_the_composed_path(net, mode):
     frames = rs.randint(0, 256, (2, 96, 128, 3)).astype(np.uint8)
     raw = rs.randint(0, 256, (2, 90, 123, 3)).astype(np.uint8)
     mixed = [rs.randint(0, 256, s + (3,)).astype(np.uint8) for s in ((90, 123), (120, 100))]
-    peaks = 0
-    # infer_u8
-    pe.infer_async_u8(frames.ctypes.data, False, 2, 96, 128)
-    want = _post(ref, *_final(net, mode, frames))
-    _assert_same(_fused(pe, 2), want, "%s infer_u8" % mode)
-    peaks += sum(len(p) for p in want[1])
-    # infer_u8_flip
-    pe.infer_flip_async_u8(frames.ctypes.data, False, 2, 96, 128)
-    got = _fused(pe, 2)
-    heat, paf = _final(net, mode, np.concatenate([frames, frames[:, :, ::-1]]))
-    mp, mh = ref.flip_merge(heat[:2], heat[2:], paf[:2], paf[2:], layout=0)
-    _assert_same(got, _post(ref, mh, mp), "%s infer_u8_flip" % mode)
-    # infer_images on mixed sizes (one ragged batch): each frame as it comes out alone
-    got = pe.infer_images_arrays(mixed, 96, 8)
-    for i, f in enumerate(mixed):
-        want = _post(ref, *_final(net, mode, _crop(net, f[None], 96)))
-        np.testing.assert_array_equal(got[i], want[0][0], err_msg="%s infer_images frame %d" % (mode, i))
+    peaks = _check_u8_flip_and_ragged(pe, ref, net, mode, frames, mixed)
     # infer_frames, NV12: the same persons as BGR frames converted on the device and cropped
     nv12 = [rs.randint(0, 256, (144, 128)).astype(np.uint8) for _ in range(2)]
     bgr = net.convert_frames(nv12, "nv12")
@@ -291,3 +297,95 @@ def test_refusals_name_the_architecture_and_leave_the_net_usable(pe, net):
         eng.PoseEngine.from_net(net, stages=3)
     after = _maps(net, "bf16", frames=frames)
     assert all(torch.equal(x, y) for x, y in zip(before, after))
+
+
+# ------------------------------------------------------------------------------------------------ other layouts
+# (l2, l1) beyond (4, 2): a PAF stage that is first and last (l2 = 1), a one-stage L1 branch that never reads
+# cat[features, heat, paf] (l1 = 1), a heat map that feeds several L1 stages (l1 >= 3), all twelve outputs (l2 + l1 = 12)
+LAYOUTS = [(1, 1), (1, 11), (11, 1), (2, 3), (6, 6)]
+LAYOUT_IDS = ["%d-%d" % lay for lay in LAYOUTS]
+
+
+@pytest.fixture(scope="module")
+def layout_engines(built):
+    """openpose_engine(sd, l2, l1) per layout, made when a test first asks for it; one layout at a time."""
+    made = {}
+
+    def get(layout):
+        if layout not in made:
+            made.clear()
+            sd = openpose_port.he_state_dict(*layout)
+            made[layout] = sd, pkg_module("engine").openpose_engine(sd, *layout, batch_cap=8, peak_cap=1024,
+                                                                    human_cap=2048)
+        return made[layout]
+    return get
+
+
+@pytest.mark.parametrize("layout", LAYOUTS, ids=LAYOUT_IDS)
+def test_layout_fp32_is_bit_identical_to_the_exact_oracle_uniform_and_ragged(layout_engines, layout):
+    """Every map the layout returns (at (1, 11) and (11, 1) all twelve output pointers) equals forward_exact; in a ragged
+    batch, each frame's maps inside its extent equal the oracle's of that frame alone, and +0 beyond it."""
+    sd, pe = layout_engines(layout)
+    l2, l1 = layout
+    x = _input(2, (64, 64), 5)
+    got = _maps(pe.net, "fp32", x=x.cuda())
+    want = openpose_port.forward_exact(sd, x.numpy(), l2, l1)
+    assert len(got) == len(want) == l2 + l1
+    for i, (g, w) in enumerate(zip(got, want)):
+        np.testing.assert_array_equal(g.cpu().numpy(), w, err_msg="%s map %d" % (layout, i))
+    rs = np.random.RandomState(13)
+    shapes = [(64, 72), (48, 80), (72, 56)]
+    frames = [rs.randint(0, 256, s + (3,)).astype(np.uint8) for s in shapes]
+    packed = torch.from_numpy(np.concatenate([f.ravel() for f in frames])).cuda()
+    got = _maps(pe.net, "fp32", frames=packed, shapes=shapes)
+    for i, f in enumerate(frames):
+        want = openpose_port.forward_exact(sd, glue_port.rtpose_preprocess(f)[None].astype(np.float32), l2, l1)
+        h, w = f.shape[0] // 8, f.shape[1] // 8
+        for m, (g, wm) in enumerate(zip(got, want)):
+            g = g[i].cpu().numpy()
+            np.testing.assert_array_equal(g[:, :h, :w], wm[0], err_msg="%s frame %d map %d" % (layout, i, m))
+            assert not g[:, h:, :].any() and not g[:, :, w:].any(), (layout, i, m)
+
+
+@pytest.mark.parametrize("mode,tol", [("bf16x3", 1e-3), ("bf16", 0.25)])
+@pytest.mark.parametrize("layout", LAYOUTS, ids=LAYOUT_IDS)
+def test_layout_against_the_reference_golden(layout_engines, layout, mode, tol):
+    """Every saved map against the unmodified module's (tests/golden/openpose_<l2>_<l1>_64.npz), at the tolerances of
+    test_368_against_the_reference_golden."""
+    _, pe = layout_engines(layout)
+    g = golden("openpose_%d_%d_64" % layout)
+    x = torch.rand((1, 3, 64, 64), generator=torch.Generator().manual_seed(int(g["seed"]))) - 0.5
+    outs = _maps(pe.net, mode, x=x.cuda())
+    errs = [float(np.abs(o.cpu().numpy() - g["maps_%d" % i]).max()) for i, o in enumerate(outs)]
+    print("OpenPose_Model(%d, %d) %s @64: max|err| per map %s (maps up to %.1f)"
+          % (layout + (mode, " ".join("%.1e" % e for e in errs), float(np.max(g["stage_absmax"])))))
+    assert len(outs) == sum(layout) and max(errs) < tol, errs
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("layout", LAYOUTS, ids=LAYOUT_IDS)
+def test_layout_ragged_frames_equal_each_frame_alone(layout_engines, layout, mode):
+    _, pe = layout_engines(layout)
+    rs = np.random.RandomState(9)
+    shapes = [(64, 72), (48, 80), (72, 56)]
+    frames = [rs.randint(0, 256, s + (3,)).astype(np.uint8) for s in shapes]
+    packed = torch.from_numpy(np.concatenate([f.ravel() for f in frames])).cuda()
+    rag = _maps(pe.net, mode, frames=packed, shapes=shapes)
+    for i, f in enumerate(frames):
+        alone = _maps(pe.net, mode, frames=torch.from_numpy(f[None]).cuda())
+        h, w = f.shape[0] // 8, f.shape[1] // 8
+        for m, (a, b) in enumerate(zip(rag, alone)):
+            assert torch.equal(a[i, :, :h, :w], b[0]), (layout, mode, i, m)
+            assert not a[i, :, h:, :].any() and not a[i, :, :, w:].any(), (layout, mode, i, m)
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("layout", [(1, 1), (6, 6)], ids=["1-1", "6-6"])
+def test_layout_fused_entry_points_equal_the_composed_path(layout_engines, layout, mode):
+    _, pe0 = layout_engines(layout)
+    pe = _engine(pe0.net, mode)
+    ref = pkg_module("engine").NativePost(0, batch_cap=8, peak_cap=1024, human_cap=2048)
+    rs = np.random.RandomState(62)
+    frames = rs.randint(0, 256, (2, 96, 128, 3)).astype(np.uint8)
+    mixed = [rs.randint(0, 256, s + (3,)).astype(np.uint8) for s in ((90, 123), (120, 100))]
+    assert _check_u8_flip_and_ragged(pe, ref, pe.net, mode, frames, mixed) > 0

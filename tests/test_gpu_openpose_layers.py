@@ -1,5 +1,7 @@
-"""GPU (-m gpu): every launch of OpenPose_Model(4, 2)'s bf16 and bf16x3 plans against a float64 reference of its own
-inputs, as tests/test_gpu_layers.py does for rtpose.
+"""GPU (-m gpu): every launch of OpenPose_Model(l2, l1)'s bf16 and bf16x3 plans against a float64 reference of its own
+inputs, as tests/test_gpu_layers.py does for rtpose, at the default layout (4, 2) and at layouts that (4, 2) does not
+exercise: a PAF stage that is first and last (l2 = 1), a one-stage L1 branch (l1 = 1), a heat map feeding several later
+stages (l1 >= 3) and all twelve outputs (l2 + l1 = 12).
 
 The library's test hooks re-run the plan launch by launch and hand out each launch's real input and output planes and
 its geometry.  Every element a launch writes is checked against the interval a correctly accumulated fp32 sum could
@@ -29,14 +31,20 @@ FIELDS = ["in_buf", "in_cstride", "in_ch_base", "in_ch_group_stride", "out_buf",
           "store0", "store1", "H", "W", "ksize", "cin_blocks", "groups", "n_tile", "n_tiles", "relu", "pool", "split",
           "chunk", "pdl", "tps", "map0", "map1", "n", "in_u8"]
 REF = "cuda"
-SHAPES = [((1, 8, 8), (0,)), ((2, 64, 72), (0, 1)), ((1, 368, 368), (0,)), ((32, 368, 368), (0, 31))]
+SHAPES = [((1, 8, 8), (0,)), ((2, 64, 72), (0, 1)), ((1, 184, 248), (0,)), ((1, 368, 368), (0,)),
+          ((2, 368, 496), (0, 1)), ((8, 368, 368), (0, 7)), ((32, 368, 368), (0, 31))]
+# (l2, l1) -> the shapes it runs: (4, 2) every shape of the rtpose check; the other layouts two small plans, (6, 6) also
+# the one-frame plan at full resolution
+LAYOUTS = {(4, 2): SHAPES, (1, 1): SHAPES[:2], (1, 11): SHAPES[:2], (11, 1): SHAPES[:2], (2, 3): SHAPES[:2],
+           (6, 6): SHAPES[:2] + [SHAPES[3]]}
+CASES = [(lay, s) for lay, shapes in LAYOUTS.items() for s in shapes]
 
 
-def launch_table():
-    """Per launch, in the reference's layer order: the conv's state-dict prefix, its activation ('relu', 'prelu' with the
+def launch_table(l2=L2, l1=L1):
+    """OpenPose_Model(l2, l1), per launch, in the reference's layer order: the conv's state-dict prefix, its activation ('relu', 'prelu' with the
     slope key, or none), the buffers, the physical input channels in the reference's channel order, the output channel
     offset and the fp32 map a head writes (DESIGN.md 2.11)."""
-    spec = openpose_port.state_dict_spec(L2, L1)
+    spec = openpose_port.state_dict_spec(l2, l1)
     trunk = [k[:-len(".weight")] for k, s in spec.items() if k.startswith("feature_extractor.") and len(s) == 4]
     slope_of = {t: "feature_extractor.%d.weight" % (int(t.split(".")[1]) + 1) for t in trunk
                 if "feature_extractor.%d.weight" % (int(t.split(".")[1]) + 1) in spec}
@@ -49,8 +57,8 @@ def launch_table():
         T.append(dict(conv=c, act="prelu" if c in slope_of else "relu", slope=slope_of.get(c), in_buf=BUF[src],
                       in_ch=np.arange(spec[c + ".weight"][1]), out_buf=BUF[dst], off=64 if dst == "cat" else 0,
                       pool=pool, map=-1))
-    for t in range(L2 + L1):
-        branch, i = ("l2", t) if t < L2 else ("l1", t - L2)
+    for t in range(l2 + l1):
+        branch, i = ("l2", t) if t < l2 else ("l1", t - l2)
         _, inner, innerout, _ = openpose_port.stage_channels(branch, i)
         base = 384 if i == 0 else 0
         slots = np.concatenate([base + 128 * s + np.arange(inner) for s in range(3)])
@@ -72,12 +80,13 @@ def launch_table():
             T.append(dict(conv=key, act="prelu" if prelu else None,
                           slope=key[:-len(".Mconv")] + ".MPrelu.weight" if prelu else None, in_buf=BUF[src],
                           in_ch=in_ch, out_buf=BUF[dst], off=off, pool=0, map=t if li == 16 else -1))
-    assert len(T) == 1 + 11 + 17 * (L2 + L1)
+    assert len(T) == 1 + 11 + 17 * (l2 + l1)
     return T
 
 
 class Hooks:
-    def __init__(self, net):
+    def __init__(self, net, l2=L2):
+        self.l2 = l2
         self.nat = pkg_module("_native")
         self.lib = self.nat.lib()
         self.net = net
@@ -103,7 +112,7 @@ class Hooks:
         return self._read(buf, lo, img, (H // d, W // d, BUF_C[buf]), np.uint16)
 
     def stage_map(self, m, img, H, W):
-        return self._read(NUM_MAPS_BUF + m, 0, img, (38 if m < L2 else 19, H // 8, W // 8), np.float32)
+        return self._read(NUM_MAPS_BUF + m, 0, img, (38 if m < self.l2 else 19, H // 8, W // 8), np.float32)
 
 
 def _nchw(u16, ch=None):
@@ -111,10 +120,10 @@ def _nchw(u16, ch=None):
     return t if ch is None else t[:, torch.as_tensor(ch, device=REF)]
 
 
-def check_plan(hooks, sd, x_in, n, H, W, imgs, mode, label):
+def check_plan(hooks, sd, x_in, n, H, W, imgs, mode, label, l2=L2, l1=L1):
     split = mode == "bf16x3"
     planes = (0, 1) if split else (0,)
-    table = launch_table()
+    table = launch_table(l2, l1)
     fails, worst = [], {}
     before = None
     for i, t in enumerate(table):
@@ -193,18 +202,28 @@ def check_plan(hooks, sd, x_in, n, H, W, imgs, mode, label):
 
 
 @pytest.fixture(scope="module")
-def layer_net(built):
-    eng = pkg_module("engine")
-    net = eng.NativeNet.openpose(0, L2, L1)
-    sd = openpose_port.he_state_dict(L2, L1)
-    net.load_state_dict_arrays([v.numpy() for v in sd.values()])
-    return net, sd
+def layer_nets(built):
+    """One net per layout, made when a test first asks for it."""
+    nets = {}
+
+    def get(l2, l1):
+        if (l2, l1) not in nets:
+            net = pkg_module("engine").NativeNet.openpose(0, l2, l1)
+            sd = openpose_port.he_state_dict(l2, l1)
+            net.load_state_dict_arrays([v.numpy() for v in sd.values()])
+            nets.clear()            # one layout's buffers at a time
+            nets[(l2, l1)] = net, sd
+        return nets[(l2, l1)]
+    return get
 
 
 @pytest.mark.parametrize("mode", ["bf16", "bf16x3"])
-@pytest.mark.parametrize("shape,imgs", SHAPES, ids=["%dx%dx%d" % s for s, _ in SHAPES])
-def test_every_launch_matches_the_float64_reference(layer_net, shape, imgs, mode):
-    net, sd = layer_net
+@pytest.mark.parametrize("layout,shape,imgs", [(lay, s, i) for lay, (s, i) in CASES],
+                         ids=[("%dx%dx%d" % s) if lay == (L2, L1) else ("%d-%d-%dx%dx%d" % (lay + s))
+                              for lay, (s, _) in CASES])
+def test_every_launch_matches_the_float64_reference(layer_nets, layout, shape, imgs, mode):
+    l2, l1 = layout
+    net, sd = layer_nets(l2, l1)
     nat = pkg_module("_native")
     t0 = time.time()
     n, H, W = shape
@@ -212,10 +231,10 @@ def test_every_launch_matches_the_float64_reference(layer_net, shape, imgs, mode
     xd = x.cuda().contiguous()
     net.forward_ptr(xd.data_ptr(), True, n, H, W, nat.MODES[mode], [0] * 12, True, torch.cuda.current_stream().cuda_stream)
     torch.cuda.synchronize()
-    label = "%dx%dx%d" % shape
-    fails, worst = check_plan(Hooks(net), sd, x.numpy(), n, H, W, imgs, mode, label)
+    label = "OpenPose_Model(%d, %d) %dx%dx%d" % (layout + shape)
+    fails, worst = check_plan(Hooks(net, l2), sd, x.numpy(), n, H, W, imgs, mode, label, l2, l1)
     del xd
     print("\n%s %s: %d launches x %d image(s) checked in %.1f s; worst |v - r| / e per kind: %s" % (
-        label, mode, len(launch_table()), len(imgs), time.time() - t0,
+        label, mode, len(launch_table(l2, l1)), len(imgs), time.time() - t0,
         "; ".join("%s %.3f" % kv for kv in sorted(worst.items()))))
     assert not fails, "\n".join(fails[:12]) + ("\n... %d failures in all" % len(fails) if len(fails) > 12 else "")

@@ -20,7 +20,10 @@ def _spec():
         return json.load(f)
 
 
-@pytest.mark.parametrize("arch", [(4, 2), (1, 1), (5, 3)])
+LAYOUTS = [(1, 1), (1, 11), (11, 1), (2, 3), (6, 6)]      # tests/golden/openpose_<l2>_<l1>_64.npz
+
+
+@pytest.mark.parametrize("arch", [(4, 2), (1, 1), (5, 3), (1, 11), (11, 1), (2, 3), (6, 6)])
 def test_static_shape_table_equals_the_reference_state_dict(built, arch):
     ref = [(k, tuple(s)) for k, s in _spec()["%d,%d" % arch]]
     nat, eng = pkg_module("_native"), pkg_module("engine")
@@ -111,6 +114,23 @@ def test_exact_oracle_matches_the_reference_golden(built, name):
     for i, m in enumerate(saved):
         if "maps_%d" % i in g:
             np.testing.assert_allclose(m, g["maps_%d" % i], rtol=0, atol=1e-4)
+
+
+@pytest.mark.parametrize("layout", LAYOUTS, ids=["%d-%d" % lay for lay in LAYOUTS])
+def test_oracles_match_the_reference_golden_at_other_layouts(built, layout):
+    """forward and forward_exact of OpenPose_Model(l2, l1) against every saved map of the unmodified module."""
+    l2, l1 = layout
+    g = golden("openpose_%d_%d_64" % layout)
+    assert (int(g["l2"]), int(g["l1"])) == layout
+    x = torch.rand((1, 3, 64, 64), generator=torch.Generator().manual_seed(int(g["seed"]))) - 0.5
+    sd = openpose_port.he_state_dict(l2, l1)
+    with torch.no_grad():
+        saved = [t.numpy() for t in openpose_port.forward(sd, x, l2, l1)]
+    exact = openpose_port.forward_exact(sd, x.numpy(), l2, l1)
+    assert len(saved) == len(exact) == l2 + l1 == len([k for k in g.files if k.startswith("maps_")])
+    for i in range(l2 + l1):
+        np.testing.assert_allclose(saved[i], g["maps_%d" % i], rtol=0, atol=1e-5, err_msg="forward map %d" % i)
+        np.testing.assert_allclose(exact[i], g["maps_%d" % i], rtol=0, atol=1e-4, err_msg="forward_exact map %d" % i)
 
 
 def test_prelu_is_one_multiply_after_the_bias():
