@@ -32,8 +32,11 @@ namespace b2p {
 #ifdef B2P_CONV_TIMELINE
 __device__ unsigned long long g_conv_timeline[64 * kTlSlots];
 #define B2P_TL(slot) do { if (blockIdx.x < 64) g_conv_timeline[blockIdx.x * kTlSlots + (slot)] = clock64(); } while (0)
+// clocks a consumer thread spends in `stmt`, added to `acc` (slots kTlPatchWait.. of conv_tc.cuh)
+#define B2P_TL_TIME(acc, stmt) do { const long long t0_ = clock64(); stmt; acc += clock64() - t0_; } while (0)
 #else
 #define B2P_TL(slot) do { } while (0)
+#define B2P_TL_TIME(acc, stmt) stmt
 #endif
 
 namespace {
@@ -207,7 +210,15 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
         uint32_t pi = 0, pph = 0, bi = 0, bph = 0;
+#ifdef B2P_CONV_TIMELINE
+        long long tl_pw = 0, tl_bw = 0, tl_main = 0, tl_epi = 0, tl_t = 0;
+        int tl_tiles = 0;
+#endif
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+#ifdef B2P_CONV_TIMELINE
+            tl_t = clock64();
+            ++tl_tiles;
+#endif
             const TileCoord tc = decode_tile(t, a.n_tiles, a.groups, tiles_x, tiles_y);
             if (kChunk) {
 #pragma unroll
@@ -226,7 +237,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             for (int cb = 0; cb < a.cin_blocks; ++cb) {
                 for (int term = 0; term < nterms; ++term) {
                     // term 0 and 1 read the hi patch (against W_hi, W_lo), term 2 the residual patch (against W_hi)
-                    if (term != 1) mbar_wait(&patch_full[pi], pph);
+                    if (term != 1) B2P_TL_TIME(tl_pw, mbar_wait(&patch_full[pi], pph));
                     if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(2 + (cb & 1));
                     const bool release_patch = (term == nterms - 1) || (term == 1);
                     if (blk_chunks) scale = 0;
@@ -235,7 +246,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                     for (int tap0 = 0; tap0 < taps; tap0 += tps) {          // one weight stage = tps consecutive taps
                         const int cnt = taps - tap0 < tps ? taps - tap0 : tps;
                         if (row_chunks && dx == 0) scale = 0;
-                        mbar_wait(&b_full[bi], bph);
+                        B2P_TL_TIME(tl_bw, mbar_wait(&b_full[bi], bph));
                         const uint32_t b_lo = b_lo0 + bi * (b_stride >> 4);
                         for (int j = 0; j < cnt; ++j) {
                             const int p = (lh + dy) * kPatchPitch + lw + dx;     // patch pixel of this lane's A row
@@ -298,6 +309,10 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                 }
             }
             if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(5);
+#ifdef B2P_CONV_TIMELINE
+            tl_main += clock64() - tl_t;
+            tl_t = clock64();
+#endif
 
             // ---- epilogue
             const int ch_tile = tc.nt * N;                     // first channel of this n-tile within the group
@@ -328,12 +343,26 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                     out_px[hh] = a.out + (static_cast<size_t>(tc.n * Ho + yo_px[hh]) * Wo + xo) * a.out_cstride +
                                  a.out_ch_off[tc.g] + ch_tile + cq;
             }
+            // The per-channel constants of kEpC column groups at a time are loaded before any of their stores: loaded next to
+            // each group's stores, every one of the N / 8 groups waited a full load latency behind the previous group.
+            constexpr int kEpC = N / 8 < 8 ? N / 8 : 8;
 #pragma unroll
-            for (int j = 0; j < N / 8; ++j) {
-                const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + cq));
+            for (int j0 = 0; j0 < N / 8; j0 += kEpC) {
+            float2 bias2[kEpC], slope2[kPrelu ? kEpC : 1];
+            int2 wexp2[kE4m3 ? kEpC : 1];
+#pragma unroll
+            for (int j = j0; j < j0 + kEpC; ++j) {
+                bias2[j - j0] = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + cq));
+                if constexpr (kE4m3) wexp2[j - j0] = __ldg(reinterpret_cast<const int2*>(w_exp + 8 * j + cq));
+                if constexpr (kPrelu)
+                    slope2[j - j0] = __ldg(reinterpret_cast<const float2*>(a.slope + (tc.g * a.n_tiles + tc.nt) * N + 8 * j + cq));
+            }
+#pragma unroll
+            for (int j = j0; j < j0 + kEpC; ++j) {
+                const float2 b2 = bias2[j - j0];
                 float v[4];
                 if constexpr (kE4m3) {    // acc * 2^-(ea + ew) is exact: one rounding, at the bias add
-                    const int2 w2 = __ldg(reinterpret_cast<const int2*>(w_exp + 8 * j + cq));
+                    const int2 w2 = wexp2[j - j0];
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
                         v[e] = __fadd_rn(__fmul_rn(sum[4 * j + e], exp2_int(-(ea + ((e & 1) ? w2.y : w2.x)))),
@@ -341,7 +370,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                         if (a.relu) v[e] = fmaxf(v[e], 0.f);
                     }
                 } else if constexpr (kPrelu) {    // torch's prelu: one multiply, after the bias
-                    const float2 s2 = __ldg(reinterpret_cast<const float2*>(a.slope + (tc.g * a.n_tiles + tc.nt) * N + 8 * j + cq));
+                    const float2 s2 = slope2[j - j0];
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
                         const float u = (kChunk ? sum[4 * j + e] : acc[4 * j + e]) + ((e & 1) ? b2.y : b2.x);
@@ -389,6 +418,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                     }
                 }
             }
+            }
             if constexpr (kAux == TcAux::kAmax) {     // max of non-negative float bits: order-independent, so runs stay deterministic
                 amax = __reduce_max_sync(0xffffffffu, amax);
                 if (lane == 0 && amax != 0) atomicMax(a.amax_out + tc.n, amax << 16);
@@ -400,7 +430,20 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                 if (ovf) atomicOr(a.ovf_out + tc.n, 1u);
             }
             if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(7);
+#ifdef B2P_CONV_TIMELINE
+            tl_epi += clock64() - tl_t;
+#endif
         }
+#ifdef B2P_CONV_TIMELINE
+        if (warp == 4 && lane == 0 && blockIdx.x < 64) {
+            unsigned long long* s = g_conv_timeline + blockIdx.x * kTlSlots;
+            s[kTlPatchWait] = tl_pw;
+            s[kTlWeightWait] = tl_bw;
+            s[kTlMain] = tl_main;
+            s[kTlEpilogue] = tl_epi;
+            s[kTlTiles] = tl_tiles;
+        }
+#endif
     }
     if (threadIdx.x == 0) B2P_TL(9);
 }

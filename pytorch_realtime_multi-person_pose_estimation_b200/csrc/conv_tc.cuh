@@ -90,6 +90,9 @@ cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream
 #ifdef B2P_CONV_TIMELINE
 // Debug builds only (tools/conv_timeline.sh): clock64() stamps of the first 64 CTAs at the phase boundaries of conv_tc_body.
 constexpr int kTlSlots = 16;
+// Slots 10..14: clocks warp 4 (consumer) spent over all its tiles waiting on patch_full, waiting on b_full, in the main
+// loop (waits included) and in the epilogue, and its tile count.
+constexpr int kTlPatchWait = 10, kTlWeightWait = 11, kTlMain = 12, kTlEpilogue = 13, kTlTiles = 14;
 cudaError_t conv_tc_read_timeline(unsigned long long* out /*[64 * kTlSlots]*/);     // copies and clears
 #endif
 
