@@ -9,13 +9,17 @@
 //     the M = 64 rows of its wgmma (row m = pixel (h = m / 8, w = m % 8) of the half).
 //   * For each 64-channel block of the input, ONE TMA 4-D tile load brings the (16+k-1) x 16 pixel halo patch (NHWC bf16,
 //     128 B per pixel, SWIZZLE_128B, out-of-image pixels zero-filled by TMA = conv padding) into shared memory.  Every one
-//     of the k*k filter taps then reads its shifted window of that SAME patch with ldmatrix (the swizzle is undone in the
-//     address: 16-byte chunk c of patch pixel p sits at chunk c ^ (p & 7)), so the activation tile is fetched from L2
-//     once instead of k*k times.  The fragments feed wgmma with A in registers.
+//     of the k*k filter taps then reads its shifted window of that SAME patch, so the activation tile is fetched from L2
+//     once instead of k*k times.  bf16, bf16x3 and fp16 hand the window to wgmma as a shared-memory descriptor (start at
+//     patch pixel (8 wg + dy, dx), one patch row between 8-row core groups, base offset 0); fp8 loads it with ldmatrix
+//     (the swizzle undone in the address: 16-byte chunk c of patch pixel p sits at chunk c ^ (p & 7)) and converts the
+//     fragments to e4m3 for a wgmma with A in registers.
 //   * TMA 3-D loads bring the [n_tile x 64] weight slices (K-major, SWIZZLE_128B) of `tps` consecutive taps per stage into
 //     a 96 KB ring; wgmma reads them through a shared-memory descriptor.
-//   * A warpgroup issues the four k16 steps of a tap as one wgmma group and waits for it before its ldmatrix overwrites
-//     the A registers; the other warpgroup's MMAs fill the tensor cores meanwhile.
+//   * A warpgroup issues each weight stage as one wgmma group and lets it run while it waits for the previous stage's
+//     group, then releases that stage (and its patch after the patch's last stage); only a K-chunk end (bf16x3) and the
+//     tile end wait for all.  fp8 issues one group per tap and waits for it, since the next tap's conversion reuses the
+//     A registers.
 //   * The fp32 accumulators stay in registers: bias, ReLU, the optional 2x2 max-pool (vertical pair in-thread, horizontal
 //     pair through one shuffle), conversion to bf16 and NHWC stores; the stage heads additionally emit fp32 NCHW outputs.
 //   * Persistent grid (one CTA per SM), static round-robin tile schedule; warp 0 (patches) and warp 1 (weights) run
@@ -65,13 +69,11 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// wgmma of format F with A in registers: k16 on bf16 (bf16, bf16x3) or binary16 (fp16) operands, k32 on e4m3 (fp8)
-#define B2P_MMA(SHAPE)                                                        \
-    if constexpr (tc_weights(F) == TcWeights::kE4m3) SHAPE("e4m3", "32", ""); \
-    else if constexpr (tc_binary16(F)) SHAPE("f16", "16", ", 0");             \
-    else SHAPE("bf16", "16", ", 0")
+// fp8: k32 wgmma on e4m3 operands with A in registers (converted from the bf16 patch per tap)
+#define B2P_MMA(SHAPE) SHAPE("e4m3", "32", "")
 template <TcFormat F, int N>
 __device__ __forceinline__ void mma(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+    static_assert(tc_weights(F) == TcWeights::kE4m3, "the 16-bit formats read A from shared memory (mma_ss)");
     if constexpr (N == 128) { B2P_MMA(B2P_WGMMA_M64N128_RS); }
     else if constexpr (N == 64) { B2P_MMA(B2P_WGMMA_M64N64_RS); }
     else if constexpr (N == 48) { B2P_MMA(B2P_WGMMA_M64N48_RS); }
@@ -79,7 +81,29 @@ __device__ __forceinline__ void mma(float (&d)[N / 2], const uint32_t (&a)[4], u
 }
 #undef B2P_MMA
 
+// bf16, bf16x3 and fp16: k16 wgmma with A read from the halo patch through a descriptor
+#define B2P_MMA(SHAPE)                             \
+    if constexpr (tc_binary16(F)) SHAPE("f16");    \
+    else SHAPE("bf16")
+template <TcFormat F, int N>
+__device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+    if constexpr (N == 128) { B2P_MMA(B2P_WGMMA_M64N128_SS); }
+    else if constexpr (N == 64) { B2P_MMA(B2P_WGMMA_M64N64_SS); }
+    else if constexpr (N == 48) { B2P_MMA(B2P_WGMMA_M64N48_SS); }
+    else { static_assert(N == 32, "n-tile"); B2P_MMA(B2P_WGMMA_M64N32_SS); }
+}
+#undef B2P_MMA
+
 constexpr int kConsumerWarps = 8;
+
+// A consumer warp is done with weight stage b and, when p >= 0, with patch stage p: one arrive on each.
+__device__ __forceinline__ void release_stage(int b, int p, int lane, uint64_t* b_empty, uint64_t* patch_empty) {
+    __syncwarp();
+    if (lane == 0) {
+        mbar_arrive(&b_empty[b]);
+        if (p >= 0) mbar_arrive(&patch_empty[p]);
+    }
+}
 
 // F: the arithmetic format (tc_format.h).  kRagged: a.ext is set (ragged batch); a separate instantiation so that uniform
 // batches run the unmasked epilogue.
@@ -189,7 +213,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
         pdl_wait();               // (stores of this layer may overwrite what the previous layer still reads)
         const int wg = (warp >> 2) - 1;      // pixel rows 8 * wg .. 8 * wg + 7 of the tile
         const int wi = warp & 3;             // accumulator rows 16 * wi .. 16 * wi + 15 of the warpgroup
-        // ldmatrix: this lane addresses A row r (pixel (lh, lw) of the tile), 16-byte K chunk kc of each k16 step
+        // fp8's ldmatrix: this lane addresses A row r (pixel (lh, lw) of the tile), 16-byte K chunk kc of each k16 step
         const int r = (lane & 7) + ((lane >> 3) & 1) * 8;
         const int kc = lane >> 4;
         const int lh = 8 * wg + 2 * wi + (r >> 3);
@@ -201,8 +225,15 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
         const uint32_t patch0 = smem_u32(patch_smem);
         const uint64_t bdesc_hi = kE4m3 ? make_sdesc_sw64(0, 512) : make_sdesc_sw128(0, 1024);
         const uint32_t b_lo0 = (smem_u32(b_smem) & 0x3FFFFu) >> 4;
-        const bool row_chunks = kChunk && !kE4m3 && a.ksize == 7;   // bf16x3: one chunk per filter row (7x7; tps == 1) ...
-        const bool blk_chunks = kChunk && !kE4m3 && !row_chunks;    // ... or per (channel block, term); fp8: per tap
+        // The 16-bit formats' A operand, read by wgmma from the patch: row m of the warpgroup is pixel (m / 8, m % 8) of
+        // its half, so the 8-row core groups are the half's pixel rows, one patch row (SBO) apart, and the window of tap
+        // (dy, dx) starts at patch pixel (8 wg + dy, dx).  The broadcast keeps the descriptors on the uniform datapath.
+        const uint64_t adesc_hi = make_sdesc_sw128(0, kPatchPitch * 128);
+        uint32_t a_lo0 = 0;
+        if constexpr (!kE4m3)
+            a_lo0 = ((smem_u32(patch_smem) & 0x3FFFFu) >> 4) + __shfl_sync(0xffffffffu, wg, 0) * (8 * kPatchPitch * 128 >> 4);
+        // bf16x3: one K chunk per filter row (7x7; tps == 1), else per (channel block, term); fp8: per tap
+        const bool row_chunks = kChunk && !kE4m3 && a.ksize == 7;
         const int Ho = a.pool ? a.H >> 1 : a.H;
         const int Wo = a.pool ? a.W >> 1 : a.W;
         float acc[N / 2];
@@ -211,7 +242,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
         for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
         uint32_t pi = 0, pph = 0, bi = 0, bph = 0;
 #ifdef B2P_CONV_TIMELINE
-        long long tl_pw = 0, tl_bw = 0, tl_main = 0, tl_epi = 0, tl_t = 0;
+        long long tl_pw = 0, tl_bw = 0, tl_dr = 0, tl_main = 0, tl_epi = 0, tl_t = 0;
         int tl_tiles = 0;
 #endif
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
@@ -234,18 +265,76 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                 if (a.ea_out != nullptr && warp == 4 && lane == 0) a.ea_out[tc.n] = ea;
             }
             uint32_t scale = 0;       // 0: the next MMA overwrites the accumulators
+            if constexpr (!kE4m3) {
+                // One wgmma group per weight stage.  After committing it, wait_group 1 shows the previous stage's group
+                // complete, so that stage (and, after its patch's last stage, the patch) is released while this one
+                // runs.  pend_b, pend_p: the stage and patch (-1: none) whose group may still be in flight.
+                // bf16x3 drains at each K-chunk end and adds the chunk in fp32.  The chunk ends are loop exits, not
+                // branches: ptxas serialises every wgmma when the accumulators are read on a conditional path while a
+                // group may be in flight.
+                int pend_b = -1, pend_p = -1;
+                for (int cb = 0; cb < a.cin_blocks; ++cb) {
+                    for (int term = 0; term < nterms; ++term) {
+                        // term 0 and 1 read the hi patch (against W_hi, W_lo), term 2 the residual patch (against W_hi)
+                        if (term != 1) B2P_TL_TIME(tl_pw, mbar_wait(&patch_full[pi], pph));
+                        if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(2 + (cb & 1));
+                        const bool release_patch = (term == nterms - 1) || (term == 1);
+                        const uint32_t a_lo = a_lo0 + pi * (kPatchBytes >> 4);
+                        int dy = 0, dx = 0, tap0 = 0;
+                        while (tap0 < taps) {        // bf16x3: one K chunk (a 7x7 filter row, or the block) per pass
+                            do {                     // one weight stage = tps consecutive taps
+                                const int cnt = taps - tap0 < tps ? taps - tap0 : tps;
+                                B2P_TL_TIME(tl_bw, mbar_wait(&b_full[bi], bph));
+                                const uint32_t b_lo = b_lo0 + bi * (b_stride >> 4);
+                                fence_regs(acc);
+                                wgmma_fence();
+                                for (int j = 0; j < cnt; ++j) {
+                                    const uint32_t a_tap = a_lo + (dy * kPatchPitch + dx) * (128 >> 4);
+#pragma unroll
+                                    for (int k = 0; k < 4; ++k) {
+                                        mma_ss<F, N>(acc, adesc_hi | (a_tap + k * 2),
+                                                     bdesc_hi | (b_lo + j * (b_tx >> 4) + k * 2), scale);
+                                        scale = 1;
+                                    }
+                                    if (++dx == a.ksize) { dx = 0; ++dy; }
+                                }
+                                wgmma_commit();
+                                tap0 += tps;
+                                B2P_TL_TIME(tl_dr, wgmma_wait<1>());
+                                if (pend_b >= 0) release_stage(pend_b, pend_p, lane, b_empty, patch_empty);
+                                pend_b = bi;
+                                pend_p = tap0 >= taps && release_patch ? (int)pi : -1;
+                                if (++bi == nb) { bi = 0; bph ^= 1; }
+                            } while (tap0 < taps && !(row_chunks && dx == 0));
+                            if constexpr (kChunk) {
+                                B2P_TL_TIME(tl_dr, wgmma_wait<0>());
+                                fence_regs(acc);
+                                release_stage(pend_b, pend_p, lane, b_empty, patch_empty);
+                                pend_b = -1;
+#pragma unroll
+                                for (int i = 0; i < N / 2; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
+                                scale = 0;           // the next chunk starts from fresh accumulators
+                            }
+                        }
+                        if (release_patch) {
+                            if (++pi == kNumPatchStages) { pi = 0; pph ^= 1; }
+                        }
+                    }
+                }
+                B2P_TL_TIME(tl_dr, wgmma_wait<0>());     // the tile's last group, before the epilogue reads acc
+                fence_regs(acc);
+                if (pend_b >= 0) release_stage(pend_b, pend_p, lane, b_empty, patch_empty);
+            } else {
             for (int cb = 0; cb < a.cin_blocks; ++cb) {
                 for (int term = 0; term < nterms; ++term) {
                     // term 0 and 1 read the hi patch (against W_hi, W_lo), term 2 the residual patch (against W_hi)
                     if (term != 1) B2P_TL_TIME(tl_pw, mbar_wait(&patch_full[pi], pph));
                     if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(2 + (cb & 1));
                     const bool release_patch = (term == nterms - 1) || (term == 1);
-                    if (blk_chunks) scale = 0;
                     const uint32_t pbase = patch0 + pi * kPatchBytes;
                     int dy = 0, dx = 0;
                     for (int tap0 = 0; tap0 < taps; tap0 += tps) {          // one weight stage = tps consecutive taps
                         const int cnt = taps - tap0 < tps ? taps - tap0 : tps;
-                        if (row_chunks && dx == 0) scale = 0;
                         B2P_TL_TIME(tl_bw, mbar_wait(&b_full[bi], bph));
                         const uint32_t b_lo = b_lo0 + bi * (b_stride >> 4);
                         for (int j = 0; j < cnt; ++j) {
@@ -255,51 +344,30 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                             uint32_t af[4][4];
 #pragma unroll
                             for (int k = 0; k < 4; ++k) ldmatrix_x4(row_addr + (((2 * k + kc) ^ sw) << 4), af[k]);
-                            if constexpr (kE4m3) {
-                                // k32 step s takes bf16 k16 steps 2s, 2s + 1 (K order: fp8_k_to_channel)
-                                uint32_t a8[2][4];
+                            // k32 step s takes bf16 k16 steps 2s, 2s + 1 (K order: fp8_k_to_channel)
+                            uint32_t a8[2][4];
 #pragma unroll
-                                for (int s = 0; s < 2; ++s) {
-                                    a8[s][0] = bf16x4_to_e4m3x4(af[2 * s][0], af[2 * s][2], sa);
-                                    a8[s][1] = bf16x4_to_e4m3x4(af[2 * s][1], af[2 * s][3], sa);
-                                    a8[s][2] = bf16x4_to_e4m3x4(af[2 * s + 1][0], af[2 * s + 1][2], sa);
-                                    a8[s][3] = bf16x4_to_e4m3x4(af[2 * s + 1][1], af[2 * s + 1][3], sa);
-                                }
-                                fence_regs(acc);
-                                wgmma_fence();
-#pragma unroll
-                                for (int s = 0; s < 2; ++s)
-                                    mma<F, N>(acc, a8[s], bdesc_hi | (b_lo + j * (b_tx >> 4) + s * 2), s);
-                                wgmma_commit();
-                                wgmma_wait_all();
-                                fence_regs(acc);
-#pragma unroll
-                                for (int i = 0; i < N / 2; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
-                            } else {
+                            for (int s = 0; s < 2; ++s) {
+                                a8[s][0] = bf16x4_to_e4m3x4(af[2 * s][0], af[2 * s][2], sa);
+                                a8[s][1] = bf16x4_to_e4m3x4(af[2 * s][1], af[2 * s][3], sa);
+                                a8[s][2] = bf16x4_to_e4m3x4(af[2 * s + 1][0], af[2 * s + 1][2], sa);
+                                a8[s][3] = bf16x4_to_e4m3x4(af[2 * s + 1][1], af[2 * s + 1][3], sa);
+                            }
                             fence_regs(acc);
                             wgmma_fence();
 #pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                mma<F, N>(acc, af[k], bdesc_hi | (b_lo + j * (b_tx >> 4) + k * 2), scale);
-                                scale = 1;
-                            }
+                            for (int s = 0; s < 2; ++s)
+                                mma<F, N>(acc, a8[s], bdesc_hi | (b_lo + j * (b_tx >> 4) + s * 2), s);
                             wgmma_commit();
-                            wgmma_wait_all();      // the next tap's ldmatrix reuses the A registers
+                            B2P_TL_TIME(tl_dr, wgmma_wait_all());
                             fence_regs(acc);
-                            }
+#pragma unroll
+                            for (int i = 0; i < N / 2; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
                             if (++dx == a.ksize) { dx = 0; ++dy; }
                         }
                         __syncwarp();
                         if (lane == 0) mbar_arrive(&b_empty[bi]);
                         if (++bi == nb) { bi = 0; bph ^= 1; }
-                        if (row_chunks && dx == 0) {       // a filter row is complete: add the chunk in fp32
-#pragma unroll
-                            for (int i = 0; i < N / 2; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
-                        }
-                    }
-                    if (blk_chunks) {
-#pragma unroll
-                        for (int i = 0; i < N / 2; ++i) sum[i] = __fadd_rn(sum[i], acc[i]);
                     }
                     if (release_patch) {
                         __syncwarp();
@@ -307,6 +375,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                         if (++pi == kNumPatchStages) { pi = 0; pph ^= 1; }
                     }
                 }
+            }
             }
             if (wi == 0 && lane == 0 && t == (int)blockIdx.x) B2P_TL(5);
 #ifdef B2P_CONV_TIMELINE
@@ -442,6 +511,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             s[kTlMain] = tl_main;
             s[kTlEpilogue] = tl_epi;
             s[kTlTiles] = tl_tiles;
+            s[kTlDrain] = tl_dr;
         }
 #endif
     }

@@ -26,6 +26,9 @@ constexpr int kNumBStages = B2P_CONV_B_STAGES;
 #define B2P_CONV_MIN_B_STAGES 3
 #endif
 constexpr int kMinBStages = B2P_CONV_MIN_B_STAGES;     // a stage holds as many taps as still leave this many stages in the ring
+// A consumer holds the previous weight stage until the group it issues for the next one is committed (conv_tc.cu), so
+// the ring needs two stages at least: kMinBStages when a stage holds several taps, kNumBStages when it holds one.
+static_assert(kMinBStages >= 2 && kNumBStages >= 2, "conv_tc_kernel's weight ring needs at least two stages");
 constexpr int kMaxBStages = 16;       // the ring is cut into stages of the size the layer's n-tile needs (conv_tc.cu)
 constexpr int kNumPatchStages = 2;
 constexpr int kConvTcThreads = 384;   // warpgroup 0: producers (warp 0 patch TMA, warp 1 weight TMA); warpgroups 1, 2: MMA + epilogue
@@ -90,9 +93,10 @@ cudaError_t conv_tc_launch(const ConvTcArgs& a, int num_sms, cudaStream_t stream
 #ifdef B2P_CONV_TIMELINE
 // Debug builds only (tools/conv_timeline.sh): clock64() stamps of the first 64 CTAs at the phase boundaries of conv_tc_body.
 constexpr int kTlSlots = 16;
-// Slots 10..14: clocks warp 4 (consumer) spent over all its tiles waiting on patch_full, waiting on b_full, in the main
-// loop (waits included) and in the epilogue, and its tile count.
-constexpr int kTlPatchWait = 10, kTlWeightWait = 11, kTlMain = 12, kTlEpilogue = 13, kTlTiles = 14;
+// Slots 10..15: clocks warp 4 (consumer) spent over all its tiles waiting on patch_full, waiting on b_full, in the main
+// loop (waits included) and in the epilogue, its tile count, and the clocks of the main loop it spent in wgmma.wait_group
+// (waiting for issued MMAs to complete).
+constexpr int kTlPatchWait = 10, kTlWeightWait = 11, kTlMain = 12, kTlEpilogue = 13, kTlTiles = 14, kTlDrain = 15;
 cudaError_t conv_tc_read_timeline(unsigned long long* out /*[64 * kTlSlots]*/);     // copies and clears
 #endif
 

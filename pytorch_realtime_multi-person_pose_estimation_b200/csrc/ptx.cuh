@@ -87,6 +87,9 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t saddr, uint32_t (&r)[4]) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Waits until at most `kPending` of this warpgroup's committed wgmma groups are still in flight.
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
 // Keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs.
 template <int N>
 __device__ __forceinline__ void fence_regs(float (&d)[N]) {
@@ -96,12 +99,15 @@ __device__ __forceinline__ void fence_regs(float (&d)[N]) {
 
 // Shared-memory matrix descriptor (sm_90 layout), K-major, 128-byte swizzle: rows are 128 B (64 bf16) apart inside an
 // 8-row group, groups are `sbo_bytes` apart.  [0,14) addr>>4, [16,30) LBO>>4 (unused for SW128 K-major), [32,46) SBO>>4,
-// [49,52) base offset (0: the operand starts on a 1024 B boundary), [62,64) layout (1 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t saddr, uint32_t sbo_bytes) {
+// [49,52) base offset, [62,64) layout (1 = SWIZZLE_128B).  conv_tc_kernel's operands were written by TMA with the
+// swizzle of their absolute address and use base offset 0, also where they start past a 1024 B boundary
+// (tests/cuda/test_wgmma_a_desc.cu checks that rule against ldmatrix fragments).
+__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t saddr, uint32_t sbo_bytes, uint32_t base_offset = 0) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
     d |= 1ull << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
+    d |= static_cast<uint64_t>(base_offset & 7u) << 49;
     d |= 1ull << 62;
     return d;
 }
@@ -152,6 +158,53 @@ __device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t saddr, uint32_t sb
         "{%16, %17, %18, %19}, %20, p, 1, 1" TAIL ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d) \
+        : "memory")
+
+// The same with A in shared memory too: D[64 x N] (+)= A[64 x K, descriptor desc_a] * B[K x N, descriptor desc_b], for
+// the 16-bit types (TYPE "bf16" or "f16", K = 16), neither operand transposed.  Operands d (float[N / 2]), desc_a,
+// desc_b, scale_d.
+#define B2P_WGMMA_M64N128_SS(TYPE) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\t" \
+        "setp.ne.b32 p, %66, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPE "." TYPE " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, " \
+        "%64, %65, p, 1, 1, 0, 0;\n\t}\n" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d) \
+        : "memory")
+
+#define B2P_WGMMA_M64N64_SS(TYPE) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\t" \
+        "setp.ne.b32 p, %34, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32." TYPE "." TYPE " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, " \
+        "%32, %33, p, 1, 1, 0, 0;\n\t}\n" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d) \
+        : "memory")
+
+#define B2P_WGMMA_M64N48_SS(TYPE) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\t" \
+        "setp.ne.b32 p, %26, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32." TYPE "." TYPE " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, " \
+        "%24, %25, p, 1, 1, 0, 0;\n\t}\n" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]) \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d) \
+        : "memory")
+
+#define B2P_WGMMA_M64N32_SS(TYPE) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\t" \
+        "setp.ne.b32 p, %18, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32." TYPE "." TYPE " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, " \
+        "%16, %17, p, 1, 1, 0, 0;\n\t}\n" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d) \
         : "memory")
 
 // ---------------------------------------------------------------- binary16 (fp16 mode)

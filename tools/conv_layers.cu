@@ -1,7 +1,8 @@
 // Times conv_tc_kernel alone at the layer shapes of bench.py's network (batch 32, 368x368, bf16): CUDA events over 20
 // launches per layer.  Built with -DB2P_CONV_TIMELINE (tools/conv_timeline.sh) it also prints, per layer, where the first
 // consumer warp of the first 64 CTAs spends its clocks: waiting on the activation patch (patch_full), waiting on the
-// weights (b_full), the rest of the main loop (ldmatrix + MMAs) and the epilogue, averaged over those CTAs.
+// weights (b_full), waiting for issued MMAs to complete (wgmma.wait_group), the rest of the main loop (A operand set-up
+// and MMA issue) and the epilogue, averaged over those CTAs.
 // Usage on an H100:  build/conv_layers [--fmt bf16|bf16x3]
 #include <cstdio>
 #include <cstring>
@@ -93,21 +94,22 @@ int main(int argc, char** argv) {
         {   // the stamps of the last launch: per-CTA sums of the first consumer warp, averaged over the first 64 CTAs
             std::vector<unsigned long long> tl(64 * kTlSlots);
             CK(conv_tc_read_timeline(tl.data()));
-            double pw = 0, bw = 0, mn = 0, ep = 0, tot = 0, tiles = 0;
+            double pw = 0, bw = 0, dr = 0, mn = 0, ep = 0, tot = 0, tiles = 0;
             int ctas = 0;
             for (int c = 0; c < 64; ++c) {
                 const unsigned long long* s = &tl[c * kTlSlots];
                 if (s[kTlTiles] == 0) continue;
                 ++ctas;
-                pw += s[kTlPatchWait]; bw += s[kTlWeightWait]; mn += s[kTlMain]; ep += s[kTlEpilogue];
+                pw += s[kTlPatchWait]; bw += s[kTlWeightWait]; dr += s[kTlDrain]; mn += s[kTlMain]; ep += s[kTlEpilogue];
                 tot += s[kTlMain] + s[kTlEpilogue];
                 tiles += s[kTlTiles];
             }
             if (ctas > 0) {
-                pw /= ctas; bw /= ctas; mn /= ctas; ep /= ctas; tot /= ctas; tiles /= ctas;
-                printf("  clocks/CTA %.0f (%.1f tiles): patch wait %.0f (%.1f%%)  weight wait %.0f (%.1f%%)  MMA %.0f (%.1f%%)"
-                       "  epilogue %.0f (%.1f%%)\n", tot, tiles, pw, 100 * pw / tot, bw, 100 * bw / tot, mn - pw - bw,
-                       100 * (mn - pw - bw) / tot, ep, 100 * ep / tot);
+                pw /= ctas; bw /= ctas; dr /= ctas; mn /= ctas; ep /= ctas; tot /= ctas; tiles /= ctas;
+                const double rest = mn - pw - bw - dr;
+                printf("  clocks/CTA %.0f (%.1f tiles): patch wait %.0f (%.1f%%)  weight wait %.0f (%.1f%%)  MMA wait %.0f (%.1f%%)"
+                       "  A operand + issue %.0f (%.1f%%)  epilogue %.0f (%.1f%%)\n", tot, tiles, pw, 100 * pw / tot, bw,
+                       100 * bw / tot, dr, 100 * dr / tot, rest, 100 * rest / tot, ep, 100 * ep / tot);
             }
         }
 #endif

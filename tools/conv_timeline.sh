@@ -1,8 +1,8 @@
 #!/bin/bash
 # Debug aid: builds tests/cuda/test_conv_tc.cu + conv_tc.cu with -DB2P_CONV_TIMELINE (clock64() stamps of the first CTAs at the
 # phase boundaries of conv_tc_body), to be run on an H100:  build/test_conv_tc_tl | grep timeline
-# and tools/conv_layers.cu the same way (the bench's layer shapes: consumer clocks in patch waits, weight waits, MMAs and the
-# epilogue):  build/conv_layers_tl
+# and tools/conv_layers.cu the same way (the bench's layer shapes: consumer clocks in patch waits, weight waits, MMA waits,
+# the rest of the main loop and the epilogue):  build/conv_layers_tl
 # (production builds compile the stamps away).
 set -e
 cd "$(dirname "$0")/.."
