@@ -347,6 +347,23 @@ int b200pose_infer_frames(b200pose_net* net, b200pose_post* post, const b200pose
                           int mode, float thresh, int flip, void* cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3e. Drawing the persons: replaces draw_humans(frame, humans_from_rows(rows, net_w, net_h))   lib/utils/common.py
+ *     (DESIGN.md 2.12).  Draws, in place, the persons of images 0 .. n-1 of the SELECTED run (the rows
+ *     b200pose_post_get_humans returns) on uint8 HWC BGR frames packed back to back (frame i: frame_hw[2i] x
+ *     frame_hw[2i+1] x 3 bytes, the layout b200pose_net_convert_frames writes; sizes may differ).  net_hw[2i],
+ *     net_hw[2i+1]: the padded network input frame i's coordinates are in.  A part's centre is
+ *     (int(x / net_w * w + 0.5), int(y / net_h * h + 0.5)) in double precision; persons in row order, each with
+ *     cv2.circle(c, 3, CocoColors[part], thickness 3) for its parts in part order, then cv2.line(.., CocoColors[k], 3)
+ *     for the limbs k of CocoPairsRender it has, bit for bit what cv2 (OpenCV 4.13) draws (csrc/draw_core.h).
+ *     on_device = 1: device frames, asynchronous on cuda_stream; 0: host frames, staged, drawn and copied back (the
+ *     call synchronises the stream).  What a call draws is fixed when it returns: later runs and draw calls do not
+ *     change it.  n < 1 or above batch_cap or the selected run's image count, a size < 1 and no selected run are
+ *     refused, naming the field, before anything is enqueued.
+ * ---------------------------------------------------------------------------------------------------------- */
+int b200pose_post_draw(b200pose_post* post, unsigned char* frames, int on_device, int n, const int* frame_hw,
+                       const int* net_hw, void* cuda_stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

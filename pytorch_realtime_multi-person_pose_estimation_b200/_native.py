@@ -60,6 +60,7 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_post_overflow": ([vp, ci], ci),
     "b200pose_post_get_humans": ([vp, ci, vp, ci], ci),
     "b200pose_post_get_peaks": ([vp, ci, vp, ci], ci),
+    "b200pose_post_draw": ([vp, vp, ci, ci, vp, vp, vp], ci),
     "b200pose_infer": ([vp, vp, vp, ci, ci, ci, ci, ci, cf, vp], ci),
     "b200pose_infer_u8": ([vp, vp, vp, ci, ci, ci, ci, ci, cf, vp], ci),
     "b200pose_flip_merge": ([vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp], ci),

@@ -21,6 +21,7 @@
 #include "conv_misc.cuh"
 #include "conv_tc.cuh"
 #include "f16_core.h"
+#include "draw.cuh"
 #include "frames.cuh"
 #include "fp8_core.h"
 #include "postprocess.cuh"
@@ -439,6 +440,13 @@ struct b200pose_post {
     // fp16 overflow flags of the fused runs, slot = run parity: one row of 2 * batch_cap images per forward of the run (a
     // multi-scale run makes one forward per scale), copied from the net's flags behind each forward
     HostBuf<unsigned> hp_ovf[2];
+    // b200pose_post_draw: the call's images, person rows and frame table (copied from pageable memory, so a later run
+    // may reuse the pinned slot at once), its planned primitives, host frames' staging; ev_draw: the last draw is done
+    DevBuf<char> draw_job;
+    DevBuf<DrawPrim> draw_prims;
+    DevBuf<unsigned char> draw_frames;
+    Event ev_draw;
+    bool have_draw = false;
     int ovf_rows[2] = {0, 0}, ovf_imgs[2] = {0, 0};    // forwards copied, images per forward (2n with flip)
     int ovf_pending = 0, ovf_pending_imgs = 0;          // ... of the run being enqueued
     // scoring / prune settings of the runs submitted from now on (b200pose_post_set_params); they travel to the kernels
@@ -1479,7 +1487,8 @@ int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, in
     cudaError_t e = post_alloc(p->pb, batch_cap, peak_cap, human_cap, pool);
     if (e != cudaSuccess) return cuda_fail("post_alloc failed: %s", cudaGetErrorString(e));
     CU(cudaStreamCreateWithFlags(&p->s2.h, cudaStreamNonBlocking));
-    for (Event* ev : {&p->ev_limbs, &p->ev_asm, &p->ev_maps, &p->ev_fetch[0], &p->ev_fetch[1], &p->ev_ld[0], &p->ev_ld[1]})
+    for (Event* ev : {&p->ev_limbs, &p->ev_asm, &p->ev_maps, &p->ev_fetch[0], &p->ev_fetch[1], &p->ev_ld[0], &p->ev_ld[1],
+                      &p->ev_draw})
         CU(cudaEventCreateWithFlags(&ev->h, cudaEventDisableTiming));
     for (int b = 0; b < 2; ++b) {
         CU(p->hp_nh[b].alloc(batch_cap, cudaHostAllocDefault));
@@ -1705,6 +1714,73 @@ int b200pose_post_get_humans(b200pose_post* p, int img, float* out, int max_huma
     const int n = p->hp_nh[p->cur].p[img] < max_humans ? p->hp_nh[p->cur].p[img] : max_humans;
     memcpy(out, p->hp_humans[p->cur].p + (size_t)img * p->pb.human_cap * kHumanFloats, (size_t)n * kHumanFloats * sizeof(float));
     return n;
+}
+int b200pose_post_draw(b200pose_post* p, unsigned char* frames, int on_device, int n, const int* frame_hw,
+                       const int* net_hw, void* cuda_stream) {
+    if (!p) return fail("post_draw: null post");
+    if (p->cur_ticket < 0) return fail("post_draw: no run selected (b200pose_post_select or b200pose_post_sync first)");
+    if (n < 1 || n > p->pb.batch_cap) return fail("post_draw: n = %d images, must be 1 .. batch_cap %d", n, p->pb.batch_cap);
+    if (n > p->slot_n[p->cur]) return fail("post_draw: n = %d images, the selected run has %d", n, p->slot_n[p->cur]);
+    if (!frames || !frame_hw || !net_hw) return fail("post_draw: null frames, frame_hw or net_hw");
+    for (int i = 0; i < n; ++i) {
+        if (frame_hw[2 * i] < 1 || frame_hw[2 * i + 1] < 1)
+            return fail("post_draw: frame_hw of image %d is %d x %d (sizes must be >= 1)", i, frame_hw[2 * i], frame_hw[2 * i + 1]);
+        if (net_hw[2 * i] < 1 || net_hw[2 * i + 1] < 1)
+            return fail("post_draw: net_hw of image %d is %d x %d (sizes must be >= 1)", i, net_hw[2 * i], net_hw[2 * i + 1]);
+    }
+    CU(cudaSetDevice(p->device));
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    // job: images [n] | person_img [P] | rows [P][73], each part 16-byte aligned
+    const float* slot = p->hp_humans[p->cur].p;
+    std::vector<DrawImage> imgs(n);
+    long long bytes = 0;
+    int persons = 0, max_h = 0, max_w = 0;
+    for (int i = 0; i < n; ++i) {
+        const int h = frame_hw[2 * i], w = frame_hw[2 * i + 1];
+        imgs[i] = DrawImage{h, w, net_hw[2 * i], net_hw[2 * i + 1], persons, p->hp_nh[p->cur].p[i], bytes};
+        persons += imgs[i].persons;
+        bytes += 3LL * h * w;
+        max_h = h > max_h ? h : max_h;
+        max_w = w > max_w ? w : max_w;
+    }
+    auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+    const size_t o_pimg = up16(n * sizeof(DrawImage)), o_rows = o_pimg + up16(persons * sizeof(int));
+    std::vector<char> job(o_rows + (size_t)persons * kHumanFloats * sizeof(float));
+    memcpy(job.data(), imgs.data(), n * sizeof(DrawImage));
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < imgs[i].persons; ++k) {
+            const int q = imgs[i].person0 + k;
+            reinterpret_cast<int*>(job.data() + o_pimg)[q] = i;
+            memcpy(job.data() + o_rows + (size_t)q * kHumanFloats * sizeof(float),
+                   slot + ((size_t)i * p->pb.human_cap + k) * kHumanFloats, kHumanFloats * sizeof(float));
+        }
+    if (persons == 0) return 0;      // nothing to draw: the frames stay as they are
+    // the previous draw may still read the job, primitive and staging buffers (on another stream)
+    if (p->have_draw) {
+        if (job.size() > p->draw_job.n || (size_t)persons * kDrawPrimsPerPerson > p->draw_prims.n ||
+            (!on_device && (size_t)bytes > p->draw_frames.n))
+            CU(cudaEventSynchronize(p->ev_draw));
+        CU(cudaStreamWaitEvent(st, p->ev_draw, 0));
+    }
+    CU(p->draw_job.ensure(job.size()));
+    CU(p->draw_prims.ensure((size_t)persons * kDrawPrimsPerPerson));
+    CU(cudaMemcpyAsync(p->draw_job.p, job.data(), job.size(), cudaMemcpyHostToDevice, st));
+    unsigned char* d_frames = frames;
+    if (!on_device) {
+        CU(p->draw_frames.ensure((size_t)bytes));
+        d_frames = p->draw_frames.p;
+        CU(cudaMemcpyAsync(d_frames, frames, (size_t)bytes, cudaMemcpyHostToDevice, st));
+    }
+    const char* d = p->draw_job.p;
+    if (launched(draw_launch(reinterpret_cast<const DrawImage*>(d), n, reinterpret_cast<const float*>(d + o_rows),
+                             reinterpret_cast<const int*>(d + o_pimg), persons, p->draw_prims.p, max_h, max_w, d_frames, st),
+                 "draw_launch", 2))
+        return 1;
+    if (!on_device) CU(cudaMemcpyAsync(frames, d_frames, (size_t)bytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(p->ev_draw, st));
+    p->have_draw = true;
+    if (!on_device) CU(cudaStreamSynchronize(st));
+    return 0;
 }
 int b200pose_post_get_peaks(b200pose_post* p, int img, float* out, int max_peaks) {
     // valid for the LATEST run only (reads the device peak arrays, which the next run overwrites)

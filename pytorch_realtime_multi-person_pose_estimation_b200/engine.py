@@ -234,11 +234,22 @@ class NativeNet:
                                                           None), "b200pose_net_crop_with_factor")
         return (out[0] if single else out), scale, (rh, rw, 3)
 
-    def convert_frames(self, frames, format="nv12", rotate=0, stream=0):
+    def convert_frames(self, frames, format="nv12", rotate=0, stream=0, device=False):
         """Device-side cv2.rotate(cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420)) of frames as PoseEngine.infer_frames
-        takes them: a list of uint8 BGR host arrays [oh, ow, 3], `rotate` degrees clockwise."""
+        takes them: a list of uint8 BGR host arrays [oh, ow, 3], `rotate` degrees clockwise.  device=True: frames of one
+        size into a CUDA uint8 tensor [n, oh, ow, 3] instead, written asynchronously on the current stream."""
         table, keep, on_dev, sizes = frame_table(frames, format)
         outs = [rotated_size(h, w, rotate) for h, w in sizes]
+        if device:
+            import torch
+            if len(set(outs)) != 1:
+                raise nat.B200PoseError("convert_frames(device=True): the frames must share one size")
+            out = torch.empty((len(frames),) + outs[0] + (3,), dtype=torch.uint8, device="cuda:%d" % self.device_index)
+            nat.check(nat.lib().b200pose_net_convert_frames(self._h, table, len(frames), nat.FRAME_FORMATS[format],
+                                                            int(on_dev), int(rotate), ctypes.c_void_p(out.data_ptr()), 1,
+                                                            ctypes.c_void_p(torch.cuda.current_stream(out.device).cuda_stream)),
+                      "b200pose_net_convert_frames")
+            return out
         flat = np.empty(sum(h * w * 3 for h, w in outs), np.uint8)
         nat.check(nat.lib().b200pose_net_convert_frames(self._h, table, len(frames), nat.FRAME_FORMATS[format],
                                                         int(on_dev), int(rotate), ctypes.c_void_p(flat.ctypes.data), 0,
@@ -315,6 +326,17 @@ class NativePost:
                                                 n, h, w, ctypes.c_void_p(out_heat.ctypes.data),
                                                 ctypes.c_void_p(out_paf.ctypes.data), None), "b200pose_flip_merge")
         return (out_paf[0], out_heat[0]) if single else (out_paf, out_heat)
+
+    def draw(self, frames_ptr, on_device, n, frame_hw, net_hw, stream=0):
+        """Draws the persons of images 0 .. n-1 of the selected run in place on n packed uint8 HWC BGR frames
+        (b200pose_post_draw): frame_hw / net_hw are n (h, w) pairs, the frames' sizes and their network inputs'."""
+        fh = np.ascontiguousarray(frame_hw, np.int32).reshape(-1)
+        nh = np.ascontiguousarray(net_hw, np.int32).reshape(-1)
+        if len(fh) != 2 * n or len(nh) != 2 * n:
+            raise nat.B200PoseError("draw: frame_hw and net_hw need %d (h, w) pairs" % n)
+        nat.check(nat.lib().b200pose_post_draw(self._h, ctypes.c_void_p(frames_ptr), int(on_device), int(n),
+                                               ctypes.c_void_p(fh.ctypes.data), ctypes.c_void_p(nh.ctypes.data),
+                                               ctypes.c_void_p(stream)), "b200pose_post_draw")
 
     def sync(self):
         nat.check(nat.lib().b200pose_post_sync(self._h), "b200pose_post_sync")
@@ -700,6 +722,48 @@ class PoseEngine:
         if check:
             self.post.check_status(n)
         return [self.post.humans(i) for i in range(n)]
+
+    def draw_humans(self, frames, ticket=None, dest_size=368, factor=8, net_sizes=None):
+        """draw_humans(frame, humans_from_rows(rows, net_w, net_h)) for every frame of run `ticket` (default: the
+        latest), on the device, in place like draw_humans(imgcopy=False): `frames` a list of uint8 HWC BGR numpy arrays
+        (staged through the device; sizes may differ) or a CUDA uint8 tensor [n, h, w, 3] (drawn asynchronously on the
+        current stream).  net_sizes: per frame the (h, w) of the padded network input its coordinates are in; default
+        each frame's crop_geometry(h, w, dest_size, factor).  Returns `frames`."""
+        if ticket is None:
+            self.post.sync()
+        else:
+            self.post.select(ticket)
+        try:
+            import torch
+            is_tensor = isinstance(frames, torch.Tensor)
+        except ImportError:
+            is_tensor = False
+        if is_tensor:
+            if not frames.is_cuda or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+                raise nat.B200PoseError("draw_humans: expected a CUDA uint8 tensor [n, h, w, 3]")
+            if not frames.is_contiguous():
+                raise nat.B200PoseError("draw_humans: the frame tensor must be contiguous (it is drawn in place)")
+            sizes = [tuple(frames.shape[1:3])] * frames.shape[0]
+        else:
+            for f in frames:
+                if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3:
+                    raise nat.B200PoseError("draw_humans: expected uint8 HWC BGR frames")
+            sizes = [f.shape[:2] for f in frames]
+        n = len(sizes)
+        if n == 0:
+            return frames
+        if net_sizes is None:
+            net_sizes = [nat.crop_geometry(h, w, dest_size, factor)[2] for h, w in sizes]
+        if is_tensor:
+            self.post.draw(frames.data_ptr(), True, n, sizes, net_sizes, torch.cuda.current_stream(frames.device).cuda_stream)
+            return frames
+        flat = np.concatenate([np.ascontiguousarray(f).reshape(-1) for f in frames])
+        self.post.draw(flat.ctypes.data, False, n, sizes, net_sizes)
+        at = 0
+        for f in frames:
+            f[...] = flat[at:at + f.size].reshape(f.shape)
+            at += f.size
+        return frames
 
     def infer_batch(self, images, thresh=0.1, flip=False):
         """images: uint8 numpy [n,H,W,3] (BGR frames, preprocessing fused on the device), float32 numpy [n,3,H,W]

@@ -3,8 +3,11 @@
 The reference's front-ends (/root/reference/video_demo.py:85-125, demo/web_demo.py:51-71) read a frame, call
 get_outputs + paf_to_pose_cpp, draw, and only then read the next frame.  Here frames are grouped into batches and two
 batches are kept in flight: while the GPU works on batch i+1 (upload, crop_with_factor, network, post-processing - the
-fused engine), the host decodes the next frames and draws batch i.  The drawing itself is the reference's draw_humans.
+fused engine), the host decodes the next frames and draws batch i.  The drawing itself is the reference's draw_humans, or its device
+restatement (draw='device' / 'cuda', DESIGN.md 2.12).
 """
+import numpy as np
+
 from .lib.utils.common import draw_humans
 from .lib.utils.paf_to_pose import humans_from_rows
 from . import _native as nat
@@ -32,11 +35,13 @@ class PoseStream:
     PoseEngine (e.g. engine.openpose_engine's, to run OpenPose_Model); the stream then runs on that engine's net and
     post-processing, and submits batches of at most its batch_cap frames.
     frames: any iterator of uint8 BGR frames of ONE shape.  batch=1 minimises latency (camera), larger batches raise
-    throughput (files).  `draw=False` skips the rendering.
+    throughput (files).  `draw=False` skips the rendering.  draw=True draws with the reference's draw_humans on the
+    host; draw='device' yields the same numpy frames drawn on the GPU (PoseEngine.draw_humans); draw='cuda' yields the
+    drawn frames as CUDA uint8 tensors [h, w, 3] and downloads nothing but the person rows.
     format 'nv12' / 'i420' (frames as PoseEngine.infer_frames_async takes them, e.g. decoder surfaces already on the GPU)
     and rotate (degrees clockwise; nat.rotation_of maps cv2.ROTATE_* codes): the frames are converted and rotated on
-    the device; with draw=True each batch is also converted back to host BGR for the drawing, and the converted frame
-    is the one yielded."""
+    the device; with draw=True or 'device' each batch is also converted back to host BGR for the drawing, and the
+    converted frame is the one yielded; with draw='cuda' it is converted into a device tensor instead."""
 
     def __init__(self, model, frames, batch=8, preprocess='rtpose', dest_size=368, factor=8, thresh=0.1, draw=True,
                  format='bgr', rotate=None):
@@ -50,6 +55,8 @@ class PoseStream:
             self.engine = core.pose_engine(batch_cap=max(1, int(batch)))
         self.engine.net.set_preprocess(preprocess)
         self.frames, self.batch = iter(frames), max(1, int(batch))
+        if draw not in (True, False, 'device', 'cuda'):
+            raise nat.B200PoseError("PoseStream: draw must be True, False, 'device' or 'cuda', got %r" % (draw,))
         self.dest_size, self.factor, self.thresh, self.draw = dest_size, factor, thresh, draw
         self.format, self.rotate = format, int(rotate or 0)
 
@@ -64,11 +71,30 @@ class PoseStream:
     def _finish(self, ticket, batch, size):
         rows = self.engine.fetch_arrays(ticket=ticket)
         _, _, (ph, pw) = nat.crop_geometry(size[0], size[1], self.dest_size, self.factor)
-        for frame, r in zip(batch, rows):
+        if self.draw == 'device':
+            drawn = self.engine.draw_humans([f.copy() for f in batch], ticket=ticket, net_sizes=[(ph, pw)] * len(batch))
+        elif self.draw == 'cuda':
+            drawn = self._device_batch(batch)
+            self.engine.draw_humans(drawn, ticket=ticket, net_sizes=[(ph, pw)] * len(batch))
+        for i, (frame, r) in enumerate(zip(batch, rows)):
             humans = humans_from_rows(r, pw, ph)
             # draw_humans scales by the ORIGINAL frame size, like the reference front-ends (coordinates are normalised by
             # the padded network input, padding included - the same small offset the reference has)
-            yield frame, humans, (draw_humans(frame, humans, imgcopy=True) if self.draw else None)
+            if self.draw is True:
+                yield frame, humans, draw_humans(frame, humans, imgcopy=True)
+            else:
+                yield frame, humans, (drawn[i] if self.draw else None)
+
+    def _device_batch(self, batch):
+        """draw='cuda': the frames to draw on as one CUDA tensor [n, h, w, 3] (a copy: the yielded frames stay as
+        they are)."""
+        import torch
+        if isinstance(batch, torch.Tensor):
+            return batch.clone()
+        dev = "cuda:%d" % self.engine.net.device_index
+        if all(isinstance(f, torch.Tensor) for f in batch):
+            return torch.stack(list(batch)).to(dev)
+        return torch.from_numpy(np.stack(batch)).to(dev)
 
     def __iter__(self):
         pending = None
@@ -86,12 +112,17 @@ class PoseStream:
                 size = sizes.pop()
                 # host BGR frames to draw on: one more conversion launch and its download, before the submission so
                 # that its synchronisation waits only for the batch already in flight
-                shown = self.engine.net.convert_frames(batch, self.format, self.rotate) if self.draw else batch
+                if self.draw == 'cuda':
+                    shown = self.engine.net.convert_frames(batch, self.format, self.rotate, device=True)
+                elif self.draw:
+                    shown = self.engine.net.convert_frames(batch, self.format, self.rotate)
+                else:
+                    shown = batch
                 ticket = self.engine.infer_frames_async(batch, self.format, self.rotate, self.dest_size, self.factor,
                                                         self.thresh)
                 batch = shown
             if pending is not None:
                 yield from self._finish(*pending)
-            if not batch:
+            if len(batch) == 0:
                 return
             pending = (ticket, batch, size)
