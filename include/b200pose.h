@@ -364,6 +364,36 @@ int b200pose_post_draw(b200pose_post* post, unsigned char* frames, int on_device
                        const int* net_hw, void* cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3f. JPEG images: replaces cv2.imread / cv2.imdecode(buf, cv2.IMREAD_COLOR) ahead of get_outputs   (DESIGN.md 2.13)
+ *     Baseline and extended sequential Huffman streams (SOF0 / SOF1, 8-bit) with one component or three YCbCr
+ *     components sampled luma 1x1, 2x1, 2x2, 1x2 or 4x1 with chroma 1x1, restart intervals, any APPn / COM segments
+ *     and EXIF orientations 1 .. 8 are decoded on the device, bit for bit what cv2.imdecode gives (OpenCV 4.13 with
+ *     libjpeg-turbo 3.1, csrc/jpeg_core.h).  Progressive, lossless, arithmetic-coded and 12-bit streams, CMYK / YCCK,
+ *     Adobe RGB and R/G/B component ids, other sampling factors and multi-scan streams are "unsupported"; a stream
+ *     that is not a valid JPEG or whose frame has more than 2^28 pixels is "malformed".  Both are refused before
+ *     anything is enqueued, naming the image and the reason.  Damaged entropy-coded data (an invalid code, too few or
+ *     too many blocks, missing or misordered restart markers) is found on the device: it sets status bits of the image
+ *     (1 invalid code, 2 data ends early, 4 data left over, 8 restart markers) where libjpeg would warn and pad.
+ *
+ *     b200pose_jpeg_info: host only.  The oriented size h x w of the decoded frame and whether the device decodes the
+ *     stream (b200pose_last_error() holds the reason when not); returns nonzero for a malformed stream.
+ *     b200pose_net_decode_jpegs: n streams data[i] of sizes[i] bytes (host memory) -> their oriented BGR frames packed
+ *     back to back in `out` (host, or device when out_on_device); synchronises the stream and fails, naming the first
+ *     image, when an image's status is not 0.
+ *     b200pose_infer_jpegs: b200pose_infer_raw_u8* on the decoded frames - uniform when every frame has one size,
+ *     ragged otherwise, multi-scale when scales is not null; n <= batch_cap, 2n <= 1024 with flip.  The streams are
+ *     copied when the call returns.  b200pose_post_jpeg_status: the status bits of image img of the selected run (0
+ *     for runs not made from JPEG streams), -1 when img is out of range.
+ * ---------------------------------------------------------------------------------------------------------- */
+int b200pose_jpeg_info(const unsigned char* data, long long size, int* h, int* w, int* supported);
+int b200pose_net_decode_jpegs(b200pose_net* net, const unsigned char* const* data, const long long* sizes, int n,
+                              unsigned char* out, int out_on_device, void* cuda_stream);
+int b200pose_infer_jpegs(b200pose_net* net, b200pose_post* post, const unsigned char* const* data,
+                         const long long* sizes, int n, int dest_size, int factor, const double* scales, int n_scales,
+                         int mode, float thresh, int flip, void* cuda_stream);
+int b200pose_post_jpeg_status(b200pose_post* post, int img);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

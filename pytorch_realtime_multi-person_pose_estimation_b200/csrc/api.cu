@@ -23,6 +23,7 @@
 #include "f16_core.h"
 #include "draw.cuh"
 #include "frames.cuh"
+#include "jpeg.cuh"
 #include "fp8_core.h"
 #include "postprocess.cuh"
 #include "resize.cuh"
@@ -396,6 +397,11 @@ struct b200pose_net {
     // source table of the last conversion
     DevBuf<unsigned char> frame_stage;
     DevBuf<FrameSrc> d_frame_src;
+    // JPEG streams (b200pose_net_decode_jpegs, b200pose_infer_jpegs): the call's upload (descriptors, segment and chunk
+    // tables, status words, scan bytes), the unstuffed scans, the coefficients and the sample planes
+    DevBuf<char> jpeg_in;
+    DevBuf<unsigned char> jpeg_data, jpeg_planes;
+    DevBuf<short> jpeg_coef;
     // fp8 mode (DESIGN.md §2.3): amax[launch * n + image] = max |bf16| (fp32 bits) launch (0 = conv1_1) stored for the
     // image; zeroed at the start of every fp8 forward
     DevBuf<unsigned> amax;
@@ -449,6 +455,9 @@ struct b200pose_post {
     bool have_draw = false;
     int ovf_rows[2] = {0, 0}, ovf_imgs[2] = {0, 0};    // forwards copied, images per forward (2n with flip)
     int ovf_pending = 0, ovf_pending_imgs = 0;          // ... of the run being enqueued
+    // JPEG status words of a run made from JPEG streams, slot = run parity; jpeg_imgs: images copied (0: another run)
+    HostBuf<unsigned> hp_jpeg[2];
+    int jpeg_imgs[2] = {0, 0}, jpeg_pending = 0;
     // scoring / prune settings of the runs submitted from now on (b200pose_post_set_params); they travel to the kernels
     // by value, so a run in flight keeps its own
     PostParams params{DefaultPostParams::paf_thresh, DefaultPostParams::paf_samples, DefaultPostParams::paf_min_above,
@@ -1498,6 +1507,7 @@ int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, in
         CU(p->hp_humans[b].alloc((size_t)batch_cap * human_cap * kHumanFloats, cudaHostAllocMapped | cudaHostAllocPortable));
         CU(p->d_ext[b].ensure((size_t)batch_cap * 2));
         CU(p->hp_ovf[b].alloc((size_t)kMaxOvfRows * 2 * batch_cap, cudaHostAllocDefault));
+        CU(p->hp_jpeg[b].alloc(batch_cap, cudaHostAllocDefault));
     }
     *out = p.release();
     return 0;
@@ -1538,6 +1548,8 @@ static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st, 
     p->ovf_rows[b] = p->ovf_pending;
     p->ovf_imgs[b] = p->ovf_pending_imgs;
     p->ovf_pending = 0;
+    p->jpeg_imgs[b] = p->jpeg_pending;
+    p->jpeg_pending = 0;
     p->runs += 1;
     p->h_px.clear();
     return 0;
@@ -1598,6 +1610,7 @@ int b200pose_post_run(b200pose_post* p, const float* heat, const float* paf, int
     CU(cudaSetDevice(p->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     p->ovf_pending = 0;      // maps from the caller: no network ran in this run
+    p->jpeg_pending = 0;
     const float *dh = heat, *dp = paf;
     if (!on_device) {
         CU(p->d_heat.ensure((size_t)n * 19 * h * w));
@@ -1708,6 +1721,10 @@ int b200pose_post_overflow(b200pose_post* p, int img) {
     for (int k = 0; k < p->ovf_rows[b]; ++k, h += 2 * (size_t)p->pb.batch_cap)
         if (h[img] || (p->ovf_imgs[b] == 2 * n && h[n + img])) return 1;
     return 0;
+}
+int b200pose_post_jpeg_status(b200pose_post* p, int img) {
+    if (!post_ready(p, img)) return -1;
+    return img < p->jpeg_imgs[p->cur] ? (int)p->hp_jpeg[p->cur].p[img] : 0;
 }
 int b200pose_post_get_humans(b200pose_post* p, int img, float* out, int max_humans) {
     if (!post_ready(p, img)) return -1;
@@ -1904,6 +1921,7 @@ static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input,
     if (n < 1 || H < 8 || W < 8 || (H % 8) || (W % 8)) return fail("input must be [n,3,H,W] with H, W multiples of 8");
     if (int rc = check_batch(post, n)) return rc;
     post->ovf_pending = 0;
+    post->jpeg_pending = 0;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (flip) {   // the 2n batch [frames | mirrored frames] is assembled in the net's staging buffer
@@ -2144,20 +2162,155 @@ static int stage_frames(b200pose_net* net, const FrameBatch& b, int on_device, i
     return convert_frames_dev(net, b, on_device, net->raw_stage.p, st);
 }
 
+// ------------------------------------------------------------------------------------------------ JPEG streams
+constexpr long long kJpegMaxPixels = 1LL << 28;     // a frame's pixels, as for video frames
+
+// The streams of one b200pose_net_decode_jpegs / b200pose_infer_jpegs call, parsed and checked: the upload image and
+// where its tables lie, the oriented sizes [oh_0, ow_0, oh_1, ...], the packed BGR output's size, and what the device
+// buffers must hold.
+struct JpegCall {
+    int n = 0, nwork = 0;
+    std::vector<char> up;
+    size_t o_ims = 0, o_jobs = 0, o_segs = 0, o_chunk = 0, o_work = 0, o_status = 0, o_raw = 0;
+    std::vector<int> hw;
+    long long bytes = 0, data = 0, blocks = 0, planes = 0, max_blocks = 0, max_px = 0;
+    bool uniform() const {
+        for (size_t i = 2; i < hw.size(); i += 2)
+            if (hw[i] != hw[0] || hw[i + 1] != hw[1]) return false;
+        return true;
+    }
+};
+
+// Parses every stream of a call before anything is enqueued and lays out its upload.
+static int check_jpegs(const unsigned char* const* data, const long long* sizes, int n, int max_n, JpegCall* j) {
+    if (!data || !sizes) return fail("jpegs: null stream table");
+    if (n < 1 || n > max_n) return fail("jpegs: %d images (1 .. %d)", n, max_n);
+    *j = JpegCall{};
+    j->n = n;
+    std::unique_ptr<JpegParsed> P(new JpegParsed);
+    std::vector<JpegImage> ims(n);
+    std::vector<JpegUnstuffJob> jobs(n);
+    std::vector<JpegSeg> segs;
+    std::vector<unsigned> status(n);
+    std::vector<std::pair<long long, long long>> scans(n);
+    long long raw = 0, chunks = 0;
+    for (int i = 0; i < n; ++i) {
+        if (!data[i] || sizes[i] < 0) return fail("jpeg image %d: null stream or negative size", i);
+        if (!jpeg_parse(data[i], sizes[i], kJpegMaxPixels, P.get())) return fail("jpeg image %d: %s", i, P->reason);
+        if (!P->supported) return fail("jpeg image %d: %s", i, P->reason);
+        JpegImage& im = ims[i];
+        im = P->im;
+        im.out = j->bytes;
+        for (int c = 0; c < im.ncomp; ++c) {
+            JpegComp& cp = im.comp[c];
+            cp.coef = j->blocks;
+            cp.plane = j->planes;
+            j->blocks += (long long)cp.bw * cp.bh;
+            j->planes += (long long)cp.bw * cp.bh * 64;
+            j->max_blocks = std::max(j->max_blocks, (long long)cp.bw * cp.bh);
+        }
+        j->hw.push_back(im.oh);
+        j->hw.push_back(im.ow);
+        j->bytes += 3LL * im.oh * im.ow;
+        j->max_px = std::max(j->max_px, (long long)im.oh * im.ow);
+        jobs[i] = JpegUnstuffJob{raw, raw + (P->scan_end - P->scan_beg), j->data};
+        scans[i] = {P->scan_beg, P->scan_end};
+        chunks += jpeg_segments(*P, i, j->data, chunks, &segs);
+        j->data += P->seg_end.back();
+        raw += P->scan_end - P->scan_beg;
+        status[i] = P->status;
+    }
+    std::vector<int> chunk_seg;
+    std::vector<long long> work;
+    jpeg_work(segs, chunks, &chunk_seg, &work);
+    j->nwork = (int)work.size() - 1;
+    auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+    j->o_ims = 0;
+    j->o_jobs = up16(j->o_ims + n * sizeof(JpegImage));
+    j->o_segs = up16(j->o_jobs + n * sizeof(JpegUnstuffJob));
+    j->o_chunk = up16(j->o_segs + segs.size() * sizeof(JpegSeg));
+    j->o_work = up16(j->o_chunk + chunk_seg.size() * sizeof(int));
+    j->o_status = up16(j->o_work + work.size() * sizeof(long long));
+    j->o_raw = up16(j->o_status + n * sizeof(unsigned));
+    j->up.resize(j->o_raw + (size_t)raw + 16);
+    char* u = j->up.data();
+    memcpy(u + j->o_ims, ims.data(), n * sizeof(JpegImage));
+    memcpy(u + j->o_jobs, jobs.data(), n * sizeof(JpegUnstuffJob));
+    memcpy(u + j->o_segs, segs.data(), segs.size() * sizeof(JpegSeg));
+    memcpy(u + j->o_chunk, chunk_seg.data(), chunk_seg.size() * sizeof(int));
+    memcpy(u + j->o_work, work.data(), work.size() * sizeof(long long));
+    memcpy(u + j->o_status, status.data(), n * sizeof(unsigned));
+    for (int i = 0; i < n; ++i)
+        memcpy(u + j->o_raw + jobs[i].raw_beg, data[i] + scans[i].first, (size_t)(scans[i].second - scans[i].first));
+    return 0;
+}
+
+// Uploads the call's tables and scans in one copy and decodes the frames into `out` (device, j.bytes); the status
+// words are at the returned device address.
+static int decode_jpegs_dev(b200pose_net* net, const JpegCall& j, unsigned char* out, cudaStream_t st,
+                            const unsigned** d_status) {
+    CU(net->jpeg_in.ensure(j.up.size()));
+    CU(net->jpeg_data.ensure((size_t)j.data + 16));
+    CU(net->jpeg_coef.ensure((size_t)j.blocks * 64));
+    CU(net->jpeg_planes.ensure((size_t)j.planes));
+    CU(cudaMemcpyAsync(net->jpeg_in.p, j.up.data(), j.up.size(), cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(net->jpeg_coef.p, 0, (size_t)j.blocks * 64 * sizeof(short), st));
+    char* d = net->jpeg_in.p;
+    JpegBatch b;
+    b.ims = reinterpret_cast<const JpegImage*>(d + j.o_ims);
+    b.n = j.n;
+    b.jobs = reinterpret_cast<const JpegUnstuffJob*>(d + j.o_jobs);
+    b.raw = reinterpret_cast<const unsigned char*>(d + j.o_raw);
+    b.data = net->jpeg_data.p;
+    b.segs = reinterpret_cast<const JpegSeg*>(d + j.o_segs);
+    b.chunk_seg = reinterpret_cast<const int*>(d + j.o_chunk);
+    b.work = reinterpret_cast<const long long*>(d + j.o_work);
+    b.nwork = j.nwork;
+    b.coef = net->jpeg_coef.p;
+    b.planes = net->jpeg_planes.p;
+    b.out = out;
+    b.status = reinterpret_cast<unsigned*>(d + j.o_status);
+    b.max_blocks = j.max_blocks;
+    b.max_px = j.max_px;
+    *d_status = b.status;
+    return launched(jpeg_decode_launch(b, st), "jpeg_decode_launch", kJpegLaunches);
+}
+
+// The frames of j decoded into net->raw_stage, with room for their mirror images behind them when flip; the status
+// words travel to the run's slot of the post object.
+static int stage_jpegs(b200pose_net* net, b200pose_post* post, const JpegCall& j, int flip, cudaStream_t st,
+                       const unsigned char** d_raw) {
+    CU(net->raw_stage.ensure((size_t)j.bytes * (flip ? 2 : 1)));
+    *d_raw = net->raw_stage.p;
+    const unsigned* d_status;
+    if (int rc = decode_jpegs_dev(net, j, net->raw_stage.p, st, &d_status)) return rc;
+    CU(cudaMemcpyAsync(post->hp_jpeg[post->runs & 1].p, d_status, j.n * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    post->jpeg_pending = j.n;
+    return 0;
+}
+
+static const char* jpeg_status_name(unsigned s) {
+    return s & kJpegBadCode ? "an invalid Huffman code" : s & kJpegShortData ? "the data ends before the last block"
+         : s & kJpegExtraData ? "data left after the last block" : "missing or misordered restart markers";
+}
+
 // The fused inference of raw uint8 frames (b200pose_infer_raw_u8*): n frames of one size src_h x src_w, or of the
 // sizes src_hw (a ragged batch), are staged with their mirror images when flip, cropped for every scale and run
 // through the network.  scales null: one scale, base_size, post-processed as it is.  Else every scale s runs at
 // int(base_size * s) and its maps are resized (bicubic) to the grid of base_size, averaged and post-processed.
-// fb (b200pose_infer_frames): the frames are those of fb, converted into the staging buffer, instead of `images`.
+// fb (b200pose_infer_frames): the frames are those of fb, converted into the staging buffer, instead of `images`;
+// jb (b200pose_infer_jpegs): those of the JPEG streams of jb, decoded into the staging buffer.
 static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char* images, int on_device, int n,
                      int src_h, int src_w, const int* src_hw, int base_size, int factor, const double* scales,
-                     int n_scales, int mode, float thresh, int flip, void* cuda_stream, const FrameBatch* fb = nullptr) {
+                     int n_scales, int mode, float thresh, int flip, void* cuda_stream, const FrameBatch* fb = nullptr,
+                     const JpegCall* jb = nullptr) {
     if (int rc = check_infer(net, post, mode)) return rc;
-    if (!images && !fb) return fail("infer_raw: null pointer");
+    if (!images && !fb && !jb) return fail("infer_raw: null pointer");
     if (scales && (n_scales < 1 || n_scales > 16)) return fail("infer_raw: %d scales (1 .. 16)", n_scales);
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
     const bool ragged = src_hw != nullptr;
     post->ovf_pending = 0;
+    post->jpeg_pending = 0;
     // every scale's geometry first: an invalid frame size fails before anything is enqueued
     RawBatch base;
     if (scales && raw_batch(n, src_h, src_w, src_hw, base_size, factor, 0, &base)) return 1;
@@ -2175,7 +2328,8 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
     // the caller keeps a host input alive until b200pose_post_sync(), as for b200pose_infer
     const unsigned char* d_raw;
     if (int rc = fb ? stage_frames(net, *fb, on_device, flip, st, &d_raw)
-                    : stage_raw(net, images, on_device, (size_t)sc[0].raw, flip, st, &d_raw))
+                 : jb ? stage_jpegs(net, post, *jb, flip, st, &d_raw)
+                      : stage_raw(net, images, on_device, (size_t)sc[0].raw, flip, st, &d_raw))
         return rc;
     // the sources and offsets of the frame table are those of every scale
     if (ragged && upload_frames(net, sc[0].tab, st)) return 1;
@@ -2299,6 +2453,54 @@ int b200pose_infer_frames(b200pose_net* net, b200pose_post* post, const b200pose
                          thresh, flip, cuda_stream);
     return infer_raw(net, post, nullptr, on_device, n, h, w, hw, dest_size, factor, scales, n_scales, mode, thresh, flip,
                      cuda_stream, &b);
+}
+
+int b200pose_jpeg_info(const unsigned char* data, long long size, int* h, int* w, int* supported) {
+    if (!data || !h || !w || !supported) return fail("jpeg_info: null pointer");
+    std::unique_ptr<JpegParsed> P(new JpegParsed);
+    const bool ok = jpeg_parse(data, size, kJpegMaxPixels, P.get());
+    *h = P->im.oh;
+    *w = P->im.ow;
+    *supported = ok && P->supported;
+    if (!ok) return fail("jpeg: %s", P->reason);
+    if (!P->supported) fail("jpeg: %s", P->reason);
+    return 0;
+}
+
+int b200pose_net_decode_jpegs(b200pose_net* net, const unsigned char* const* data, const long long* sizes, int n,
+                              unsigned char* out, int out_on_device, void* cuda_stream) {
+    if (!net) return fail("null net");
+    if (!out) return fail("decode_jpegs: null output");
+    JpegCall j;
+    if (int rc = check_jpegs(data, sizes, n, kMaxRagged, &j)) return rc;
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    unsigned char* d_out = out;
+    if (!out_on_device) {
+        CU(net->raw_stage.ensure((size_t)j.bytes));
+        d_out = net->raw_stage.p;
+    }
+    const unsigned* d_status;
+    if (int rc = decode_jpegs_dev(net, j, d_out, st, &d_status)) return rc;
+    if (!out_on_device) CU(cudaMemcpyAsync(out, d_out, (size_t)j.bytes, cudaMemcpyDeviceToHost, st));
+    std::vector<unsigned> status(n);
+    CU(cudaMemcpyAsync(status.data(), d_status, n * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (int i = 0; i < n; ++i)
+        if (status[i]) return fail("jpeg image %d: damaged entropy-coded data: %s (status %u)", i, jpeg_status_name(status[i]), status[i]);
+    return 0;
+}
+
+int b200pose_infer_jpegs(b200pose_net* net, b200pose_post* post, const unsigned char* const* data,
+                         const long long* sizes, int n, int dest_size, int factor, const double* scales, int n_scales,
+                         int mode, float thresh, int flip, void* cuda_stream) {
+    if (int rc = check_infer(net, post, mode)) return rc;
+    if (flip && 2 * n > kMaxRagged) return fail("jpegs: %d images with flip (2n <= %d)", n, kMaxRagged);
+    JpegCall j;
+    if (int rc = check_jpegs(data, sizes, n, post->pb.batch_cap, &j)) return rc;
+    const bool uniform = j.uniform();
+    return infer_raw(net, post, nullptr, 0, n, uniform ? j.hw[0] : 0, uniform ? j.hw[1] : 0, uniform ? nullptr : j.hw.data(),
+                     dest_size, factor, scales, n_scales, mode, thresh, flip, cuda_stream, nullptr, &j);
 }
 
 // ------------------------------------------------------------------------------------------------ legacy pafprocess

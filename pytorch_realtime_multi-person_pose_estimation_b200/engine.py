@@ -127,6 +127,34 @@ def frame_table(frames, format):
     return table, keep, sides == {True}, sizes
 
 
+def _blob(b):
+    """A JPEG stream (bytes, bytearray or a 1-D uint8 numpy array) as a uint8 array whose memory the library reads."""
+    a = np.frombuffer(b, np.uint8) if isinstance(b, (bytes, bytearray, memoryview)) else np.ascontiguousarray(b)
+    if a.dtype != np.uint8 or a.ndim != 1:
+        raise nat.B200PoseError("jpeg: a stream is bytes or a 1-D uint8 array, got %s %s" % (a.dtype, a.shape))
+    return a
+
+
+def jpeg_table(blobs):
+    """(stream pointer array, size array, the arrays they point into) of b200pose_net_decode_jpegs / _infer_jpegs."""
+    arrs = [_blob(b) for b in blobs]
+    ptrs = (ctypes.c_void_p * max(1, len(arrs)))(*[a.ctypes.data for a in arrs])
+    sizes = (ctypes.c_longlong * max(1, len(arrs)))(*[a.size for a in arrs])
+    return ptrs, sizes, arrs
+
+
+def jpeg_info(blob):
+    """(h, w, supported, reason) of a JPEG stream on the host (b200pose_jpeg_info): the size of the frame
+    cv2.imdecode returns, EXIF orientation applied, and whether the device decodes it (reason: why not).  Raises for a
+    malformed stream."""
+    a = _blob(blob)
+    h, w, sup = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    nat.check(nat.lib().b200pose_jpeg_info(ctypes.c_void_p(a.ctypes.data), a.size, ctypes.byref(h), ctypes.byref(w),
+                                           ctypes.byref(sup)), "b200pose_jpeg_info")
+    reason = "" if sup.value else nat.lib().b200pose_last_error().decode()
+    return h.value, w.value, bool(sup.value), reason
+
+
 def rotated_size(h, w, rotate):
     return (w, h) if rotate in (90, 270) else (h, w)
 
@@ -260,6 +288,29 @@ class NativeNet:
             at += h * w * 3
         return res
 
+    def decode_jpegs(self, blobs, device=False, stream=0):
+        """cv2.imdecode(blob, cv2.IMREAD_COLOR) of every stream, on the device (b200pose_net_decode_jpegs): a list of
+        uint8 HWC BGR numpy frames, or with device=True of CUDA uint8 tensors [h, w, 3] (views of one buffer, written
+        on the current stream).  Raises, naming the image, for a stream the device does not decode or whose data is
+        damaged."""
+        ptrs, sizes, keep = jpeg_table(blobs)
+        shapes = [jpeg_info(b)[:2] for b in keep]
+        total = sum(h * w * 3 for h, w in shapes)
+        if device:
+            import torch
+            flat = torch.empty(max(1, total), dtype=torch.uint8, device="cuda:%d" % self.device_index)
+            ptr, stream = flat.data_ptr(), torch.cuda.current_stream(flat.device).cuda_stream
+        else:
+            flat = np.empty(max(1, total), np.uint8)
+            ptr = flat.ctypes.data
+        nat.check(nat.lib().b200pose_net_decode_jpegs(self._h, ptrs, sizes, len(keep), ctypes.c_void_p(ptr), int(device),
+                                                      ctypes.c_void_p(stream)), "b200pose_net_decode_jpegs")
+        out, at = [], 0
+        for h, w in shapes:
+            out.append(flat[at:at + h * w * 3].reshape(h, w, 3))
+            at += h * w * 3
+        return out
+
     def __del__(self):
         try:
             if self._h:
@@ -372,6 +423,13 @@ class NativePost:
         if v < 0:
             nat.check(1, "b200pose_post_overflow")
         return v == 1
+
+    def jpeg_status(self, img):
+        """Status bits of JPEG image img of the selected run (b200pose_post_jpeg_status): 0 when its data was whole."""
+        v = int(nat.lib().b200pose_post_jpeg_status(self._h, img))
+        if v < 0:
+            nat.check(1, "b200pose_post_jpeg_status")
+        return v
 
     def humans(self, img):
         """float32 [k, 73]: score, 18 x (x, y, peak score, peak id | -1)."""
@@ -573,6 +631,68 @@ class PoseEngine:
                 out[i] = humans.copy() if _arrays else humans
         return out
 
+    def infer_jpegs_async(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, stream=0):
+        """JPEG streams decoded on the device and run as infer_raw_* does on the decoded frames (b200pose_infer_jpegs):
+        uniform when every frame has one size, ragged otherwise; scales as for infer_images.  At most batch_cap
+        streams, all of which the device decodes (jpeg_info).  Returns a ticket; fetch / fetch_arrays raise, naming the
+        images, when an image's entropy-coded data is damaged.  Person coordinates refer to each decoded frame's
+        padded frame."""
+        ptrs, sizes, keep = jpeg_table(blobs)
+        shapes = [jpeg_info(b)[:2] for b in keep]
+        arr = None if scales is None else (ctypes.c_double * len(scales))(*[float(s) for s in scales])
+        nat.check(nat.lib().b200pose_infer_jpegs(self._net_h(), self.post._h, ptrs, sizes, len(keep), int(dest_size),
+                                                 int(factor), arr, 0 if scales is None else len(scales), self.mode,
+                                                 ctypes.c_float(thresh), int(bool(flip)), ctypes.c_void_p(stream)),
+                  "b200pose_infer_jpegs")
+        pads = [nat.crop_geometry(h, w, dest_size, factor)[2] for h, w in shapes]
+        if len(set(pads)) == 1:
+            t = self._remember(len(keep), pads[0][0], pads[0][1])
+        else:
+            t = self._remember(len(keep), [p[0] for p in pads], [p[1] for p in pads])
+        self._jpeg_runs = {k for k in (self.__dict__.get("_jpeg_runs") or ()) if k >= t - 1} | {t}
+        return t
+
+    def check_jpegs(self, n, names=None):
+        """Raises naming the images (names[k], default k) of the selected run whose entropy-coded data was damaged."""
+        bad = [((names[k] if names else k), s) for k, s in ((k, self.post.jpeg_status(k)) for k in range(n)) if s]
+        if bad:
+            raise nat.B200PoseError("jpeg: damaged entropy-coded data in image(s) %s (status bits: 1 invalid code, 2 data "
+                                    "ends early, 4 data left over, 8 restart markers)" % bad)
+
+    def infer_jpegs_arrays(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None):
+        """infer_jpegs, but per image the raw person rows (float32 [k, 73], pixel coordinates of the padded frame)."""
+        return self.infer_jpegs(blobs, dest_size, factor, thresh, flip, scales, _arrays=True)
+
+    def infer_jpegs(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, _arrays=False):
+        """infer_images([cv2.imdecode(b, cv2.IMREAD_COLOR) for b in blobs]) with the decoding on the device: per-image
+        human lists in input order.  Streams are grouped by plan_ragged_batches on their decoded padded sizes
+        (jpeg_info); streams the device does not decode (progressive, CMYK, ...) are decoded by cv2.imdecode and run
+        through infer_images - a frame's result does not depend on its batch.  Malformed streams raise, and so do
+        streams whose entropy-coded data is damaged, naming the image."""
+        infos = []
+        for i, b in enumerate(blobs):
+            try:
+                infos.append(jpeg_info(b))
+            except nat.B200PoseError as e:
+                raise nat.B200PoseError("infer_jpegs: image %d: %s" % (i, e)) from None
+        dev = [i for i, inf in enumerate(infos) if inf[2]]
+        out = [None] * len(blobs)
+        pads = [nat.crop_geometry(infos[i][0], infos[i][1], dest_size, factor)[2] for i in dev]
+        for part in plan_ragged_batches(pads, self.post.batch_cap):
+            idx = [dev[k] for k in part]
+            self.infer_jpegs_async([blobs[i] for i in idx], dest_size, factor, thresh, flip, scales)
+            self.post.sync()
+            self.check_jpegs(len(idx), idx)
+            for i, humans in zip(idx, self.fetch_arrays() if _arrays else self.fetch()):
+                out[i] = humans.copy() if _arrays else humans
+        rest = [i for i, inf in enumerate(infos) if not inf[2]]
+        if rest:
+            import cv2
+            frames = [cv2.imdecode(_blob(blobs[i]), cv2.IMREAD_COLOR) for i in rest]
+            for i, humans in zip(rest, self.infer_images(frames, dest_size, factor, thresh, flip, scales, _arrays)):
+                out[i] = humans
+        return out
+
     def infer_async(self, in_ptr, in_on_device, n, H, W, thresh=0.1, stream=0):
         nat.check(nat.lib().b200pose_infer(self._net_h(), self.post._h, ctypes.c_void_p(in_ptr), int(in_on_device), n, H, W,
                                            self.mode, ctypes.c_float(thresh), ctypes.c_void_p(stream)), "b200pose_infer")
@@ -702,9 +822,17 @@ class PoseEngine:
         else:
             self.post.select(ticket)
         self._check_overflow(n)
+        self._check_jpeg_run(ticket, n)
         if check:
             self.post.check_status(n)
         return [humans_to_dicts(self.post.humans(i), _at(W, i), _at(H, i)) for i in range(n)]
+
+    def _check_jpeg_run(self, ticket, n):
+        """A run made from JPEG streams (infer_jpegs_async) raises, whatever `check` says, when an image's entropy-coded
+        data was damaged: its persons are never handed back in silence."""
+        t = self.post.last_ticket() if ticket is None else ticket
+        if t in (self.__dict__.get("_jpeg_runs") or ()):
+            self.check_jpegs(n)
 
     def _check_overflow(self, n):
         if self.mode == nat.MODE_FP16:      # whatever `check` says: overflowed maps are never handed back in silence
@@ -719,6 +847,7 @@ class PoseEngine:
         else:
             self.post.select(ticket)
         self._check_overflow(n)
+        self._check_jpeg_run(ticket, n)
         if check:
             self.post.check_status(n)
         return [self.post.humans(i) for i in range(n)]
