@@ -394,6 +394,29 @@ int b200pose_infer_jpegs(b200pose_net* net, b200pose_post* post, const unsigned 
 int b200pose_post_jpeg_status(b200pose_post* post, int img);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3g. JPEG encoding: replaces cv2.imencode('.jpg', frame, [IMWRITE_JPEG_QUALITY, quality,
+ *     IMWRITE_JPEG_SAMPLING_FACTOR, sampling]) and cv2.imwrite of a .jpg name   (DESIGN.md 2.14)
+ *     Baseline streams with the standard Huffman tables, byte for byte what cv2 (OpenCV 4.13 with libjpeg-turbo 3.1)
+ *     writes: JFIF header, quality 1 .. 100 (jpeg_set_quality with baseline tables), sampling one of cv2's
+ *     IMWRITE_JPEG_SAMPLING_FACTOR values 0x221111 (4:2:0), 0x211111 (4:2:2), 0x121111 (4:4:0), 0x411111 (4:1:1) and
+ *     0x111111 (4:4:4) (csrc/jpeg_enc_core.h).
+ *
+ *     b200pose_jpeg_encode_bound: host only.  The stream bytes that always suffice for an h x w frame at this sampling
+ *     (every block at its longest codes, every byte stuffed); -1 for a size outside 1 .. 65535 or an unknown sampling.
+ *     b200pose_net_encode_jpegs: n (1 .. 1024) uint8 HWC BGR frames packed back to back (frame i: frame_hw[2i] x
+ *     frame_hw[2i+1] x 3 bytes, the layout b200pose_post_draw draws on; host, or device when frames_on_device) -> their
+ *     streams packed back to back in `out` (host, or device when out_on_device; out_cap bytes), sizes[i] (host) the
+ *     length of stream i.  Synchronises the stream (twice inside the call, to size the bit buffers and a host
+ *     output's staging from what the kernels computed, and at its end).  n, a size outside 1 .. 65535, a quality outside 1 .. 100, an
+ *     unknown sampling and an out_cap below the sum of the images' bounds are refused, naming the field, before
+ *     anything is enqueued.  One call launches 5 kernels.
+ * ---------------------------------------------------------------------------------------------------------- */
+long long b200pose_jpeg_encode_bound(int h, int w, int sampling);
+int b200pose_net_encode_jpegs(b200pose_net* net, const unsigned char* frames, int frames_on_device, const int* frame_hw,
+                              int n, int quality, int sampling, unsigned char* out, long long out_cap, int out_on_device,
+                              long long* sizes, void* cuda_stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

@@ -81,6 +81,8 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_net_decode_jpegs": ([vp, vp, vp, ci, vp, ci, vp], ci),
     "b200pose_infer_jpegs": ([vp, vp, vp, vp, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf, ci, vp], ci),
     "b200pose_post_jpeg_status": ([vp, ci], ci),
+    "b200pose_jpeg_encode_bound": ([ci, ci, ci], ctypes.c_longlong),
+    "b200pose_net_encode_jpegs": ([vp, vp, ci, vp, ci, ci, ci, vp, ctypes.c_longlong, ci, vp, vp], ci),
     "process_paf": ([ci, ci, ci, vp, ci, ci, ci, vp, ci, ci, ci, vp], ci),
     "get_num_humans": ([], ci),
     "get_part_cid": ([ci, ci], ci),
@@ -92,6 +94,8 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
 
 # b200pose_frame (include/b200pose.h 3d): pixel formats and the per-frame descriptor
 FRAME_FORMATS = {"bgr": 0, "nv12": 1, "i420": 2}
+# JPEG encoding samplings: cv2's IMWRITE_JPEG_SAMPLING_FACTOR values (b200pose_net_encode_jpegs)
+JPEG_SAMPLING = {"420": 0x221111, "422": 0x211111, "440": 0x121111, "411": 0x411111, "444": 0x111111}
 # cv2.ROTATE_90_CLOCKWISE, cv2.ROTATE_180, cv2.ROTATE_90_COUNTERCLOCKWISE -> degrees clockwise
 _CV2_ROTATIONS = {0: 90, 1: 180, 2: 270}
 

@@ -24,6 +24,7 @@
 #include "draw.cuh"
 #include "frames.cuh"
 #include "jpeg.cuh"
+#include "jpeg_enc.cuh"
 #include "fp8_core.h"
 #include "postprocess.cuh"
 #include "resize.cuh"
@@ -402,6 +403,15 @@ struct b200pose_net {
     DevBuf<char> jpeg_in;
     DevBuf<unsigned char> jpeg_data, jpeg_planes;
     DevBuf<short> jpeg_coef;
+    // JPEG encoding (b200pose_net_encode_jpegs): the call's upload (descriptors, Huffman tables) followed by the per-image
+    // bit counts and stream sizes, staged host frames, the coefficients, per-block code lengths and bit offsets, the
+    // bit buffers, and the streams of a call whose output is on the host
+    DevBuf<char> jenc_in;
+    DevBuf<unsigned char> jenc_frames, jenc_out;
+    DevBuf<short> jenc_coef;
+    DevBuf<int> jenc_acbits;
+    DevBuf<long long> jenc_off;
+    DevBuf<unsigned> jenc_words;
     // fp8 mode (DESIGN.md §2.3): amax[launch * n + image] = max |bf16| (fp32 bits) launch (0 = conv1_1) stored for the
     // image; zeroed at the start of every fp8 forward
     DevBuf<unsigned> amax;
@@ -2501,6 +2511,105 @@ int b200pose_infer_jpegs(b200pose_net* net, b200pose_post* post, const unsigned 
     const bool uniform = j.uniform();
     return infer_raw(net, post, nullptr, 0, n, uniform ? j.hw[0] : 0, uniform ? j.hw[1] : 0, uniform ? nullptr : j.hw.data(),
                      dest_size, factor, scales, n_scales, mode, thresh, flip, cuda_stream, nullptr, &j);
+}
+
+// ------------------------------------------------------------------------------------------------ JPEG encoding
+static int jenc_size_ok(int h, int w) { return h >= 1 && h <= 65535 && w >= 1 && w <= 65535; }
+
+long long b200pose_jpeg_encode_bound(int h, int w, int sampling) {
+    if (!jenc_size_ok(h, w)) return fail("jpeg_encode_bound: size %d x %d (1 .. 65535 each)", h, w), -1;
+    if (!jenc_sampling_ok(sampling)) return fail("jpeg_encode_bound: unknown sampling 0x%X", sampling), -1;
+    std::unique_ptr<JencImage> im(new JencImage);
+    jenc_image(h, w, 95, sampling, im.get());
+    return jenc_stream_bound(*im);
+}
+
+int b200pose_net_encode_jpegs(b200pose_net* net, const unsigned char* frames, int frames_on_device, const int* frame_hw,
+                              int n, int quality, int sampling, unsigned char* out, long long out_cap, int out_on_device,
+                              long long* sizes, void* cuda_stream) {
+    if (!net) return fail("null net");
+    if (!frames || !frame_hw || !out || !sizes) return fail("encode_jpegs: null pointer");
+    if (n < 1 || n > kMaxRagged) return fail("encode_jpegs: n = %d images (1 .. %d)", n, kMaxRagged);
+    if (quality < 1 || quality > 100) return fail("encode_jpegs: quality %d (1 .. 100)", quality);
+    if (!jenc_sampling_ok(sampling))
+        return fail("encode_jpegs: unknown sampling 0x%X (0x221111, 0x211111, 0x121111, 0x411111 or 0x111111)", sampling);
+    // descriptors (header and tables built once per size of the call), then the Huffman tables, and room for the
+    // per-image bit counts, stream sizes and bit-buffer offsets
+    std::vector<JencImage> ims(n);
+    std::map<std::pair<int, int>, int> first;
+    long long src = 0, blocks = 0, bound = 0, max_blocks = 0;
+    for (int i = 0; i < n; ++i) {
+        const int h = frame_hw[2 * i], w = frame_hw[2 * i + 1];
+        if (!jenc_size_ok(h, w)) return fail("encode_jpegs: image %d size %d x %d (1 .. 65535 each)", i, h, w);
+        const auto seen = first.emplace(std::make_pair(h, w), i);
+        if (seen.second) jenc_image(h, w, quality, sampling, &ims[i]);
+        else ims[i] = ims[seen.first->second];
+        ims[i].src = src;
+        ims[i].blk0 = blocks;
+        src += 3LL * h * w;
+        blocks += ims[i].blocks;
+        bound += jenc_stream_bound(ims[i]);
+        max_blocks = std::max(max_blocks, ims[i].blocks);
+    }
+    if (out_cap < bound)
+        return fail("encode_jpegs: out_cap %lld bytes, below %lld (b200pose_jpeg_encode_bound summed over the images)",
+                    out_cap, bound);
+    const size_t o_huff = n * sizeof(JencImage), o_bits = o_huff + 4 * sizeof(JencHuff);
+    const size_t o_sizes = o_bits + n * sizeof(long long), o_wbase = o_sizes + n * sizeof(long long);
+    std::vector<char> up(o_wbase + n * sizeof(long long));
+    memcpy(up.data(), ims.data(), o_huff);
+    for (int t = 0; t < 4; ++t) jenc_huff_table(t, reinterpret_cast<JencHuff*>(up.data() + o_huff) + t);
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    CU(net->jenc_in.ensure(up.size()));
+    CU(net->jenc_coef.ensure((size_t)blocks * 64));
+    CU(net->jenc_acbits.ensure((size_t)blocks));
+    CU(net->jenc_off.ensure((size_t)blocks));
+    if (!frames_on_device) CU(net->jenc_frames.ensure((size_t)src));
+    CU(cudaMemcpyAsync(net->jenc_in.p, up.data(), up.size(), cudaMemcpyHostToDevice, st));
+    if (!frames_on_device) CU(cudaMemcpyAsync(net->jenc_frames.p, frames, (size_t)src, cudaMemcpyHostToDevice, st));
+    char* d = net->jenc_in.p;
+    JencBatch b;
+    b.ims = reinterpret_cast<const JencImage*>(d);
+    b.n = n;
+    b.huff = reinterpret_cast<const JencHuff*>(d + o_huff);
+    b.frames = frames_on_device ? frames : net->jenc_frames.p;
+    b.coef = net->jenc_coef.p;
+    b.acbits = net->jenc_acbits.p;
+    b.off = net->jenc_off.p;
+    b.wbase = reinterpret_cast<const long long*>(d + o_wbase);
+    b.words = nullptr;
+    b.bits = reinterpret_cast<long long*>(d + o_bits);
+    b.sizes = reinterpret_cast<long long*>(d + o_sizes);
+    b.out = nullptr;
+    b.max_blocks = max_blocks;
+    // phase 0, then the bit buffers sized from the bit counts
+    if (int rc = launched(jpeg_encode_launch(b, 0, st), "jpeg_encode_launch", 2)) return rc;
+    std::vector<long long> got(n), wbase(n);
+    CU(cudaMemcpyAsync(got.data(), b.bits, n * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    long long words = 0;
+    for (int i = 0; i < n; ++i) {
+        wbase[i] = words;
+        words += jenc_words(got[i]);
+    }
+    CU(net->jenc_words.ensure((size_t)words));
+    b.words = net->jenc_words.p;
+    CU(cudaMemsetAsync(b.words, 0, (size_t)words * sizeof(unsigned), st));
+    CU(cudaMemcpyAsync(d + o_wbase, wbase.data(), n * sizeof(long long), cudaMemcpyHostToDevice, st));
+    // phase 1, then the output sized from the stream sizes
+    if (int rc = launched(jpeg_encode_launch(b, 1, st), "jpeg_encode_launch", 2)) return rc;
+    CU(cudaMemcpyAsync(got.data(), b.sizes, n * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    long long total = 0;
+    for (int i = 0; i < n; ++i) total += got[i];
+    if (!out_on_device) CU(net->jenc_out.ensure((size_t)total));
+    b.out = out_on_device ? out : net->jenc_out.p;
+    if (int rc = launched(jpeg_encode_launch(b, 2, st), "jpeg_encode_launch", 1)) return rc;
+    if (!out_on_device) CU(cudaMemcpyAsync(out, net->jenc_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    memcpy(sizes, got.data(), n * sizeof(long long));
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------ legacy pafprocess

@@ -155,6 +155,20 @@ def jpeg_info(blob):
     return h.value, w.value, bool(sup.value), reason
 
 
+def _packed_views(frames):
+    """A device tensor whose data pointer starts the frames packed back to back: the first frame itself when the frames
+    are contiguous and consecutive (views of one packed buffer, as b200pose_post_draw draws on), else a packed copy."""
+    import torch
+    if not frames:
+        return None
+    at = frames[0].data_ptr()
+    for f in frames:
+        if not f.is_contiguous() or f.data_ptr() != at:
+            return torch.cat([f.reshape(-1) for f in frames])
+        at += f.numel()
+    return frames[0]
+
+
 def rotated_size(h, w, rotate):
     return (w, h) if rotate in (90, 270) else (h, w)
 
@@ -310,6 +324,76 @@ class NativeNet:
             out.append(flat[at:at + h * w * 3].reshape(h, w, 3))
             at += h * w * 3
         return out
+
+    def encode_jpegs(self, frames, quality=95, sampling="420", device=False, stream=0):
+        """cv2.imencode('.jpg', frame, [IMWRITE_JPEG_QUALITY, quality, IMWRITE_JPEG_SAMPLING_FACTOR, s])[1] of every
+        frame, on the device (b200pose_net_encode_jpegs); sampling one of '420', '422', '440', '411', '444'.  frames: a
+        list of uint8 HWC BGR numpy arrays (staged through the device), a CUDA uint8 tensor [n, h, w, 3], or a list of
+        CUDA uint8 tensors [h, w, 3] of any sizes.  Returns a list of bytes, or with device=True of 1-D CUDA uint8
+        tensors (views of one buffer, written on the current stream)."""
+        if sampling not in nat.JPEG_SAMPLING:
+            raise nat.B200PoseError("encode_jpegs: unknown sampling %r (one of %s)" % (sampling, sorted(nat.JPEG_SAMPLING)))
+        try:
+            import torch
+        except ImportError:
+            torch = None
+        dev_in = torch is not None and (isinstance(frames, torch.Tensor) or any(isinstance(f, torch.Tensor) for f in frames))
+        if dev_in:
+            tensors = [frames] if isinstance(frames, torch.Tensor) else list(frames)
+            for f in tensors:
+                if not isinstance(f, torch.Tensor) or not f.is_cuda:
+                    raise nat.B200PoseError("encode_jpegs: frames are all numpy arrays or all CUDA tensors")
+                if f.device.index != self.device_index:
+                    raise nat.B200PoseError("encode_jpegs: a frame tensor is on %s, the net on cuda:%d"
+                                            % (f.device, self.device_index))
+            if isinstance(frames, torch.Tensor):
+                if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+                    raise nat.B200PoseError("encode_jpegs: expected a CUDA uint8 tensor [n, h, w, 3]")
+                sizes = [tuple(frames.shape[1:3])] * frames.shape[0]
+                flat = frames.contiguous()
+            else:
+                for f in frames:
+                    if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
+                        raise nat.B200PoseError("encode_jpegs: expected a list of CUDA uint8 tensors [h, w, 3]")
+                sizes = [tuple(f.shape[:2]) for f in frames]
+                flat = _packed_views(frames)
+            src = flat.data_ptr() if flat is not None else 0
+        else:
+            arrs = [np.ascontiguousarray(f) for f in frames]
+            for a in arrs:
+                if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+                    raise nat.B200PoseError("encode_jpegs: expected uint8 HWC BGR frames")
+            sizes = [a.shape[:2] for a in arrs]
+            flat = np.concatenate([a.reshape(-1) for a in arrs]) if arrs else None
+            src = flat.ctypes.data if flat is not None else 0
+        n = len(sizes)
+        if n == 0:
+            return []
+        code = nat.JPEG_SAMPLING[sampling]
+        cap = 0
+        for h, w in sizes:
+            b = int(nat.lib().b200pose_jpeg_encode_bound(int(h), int(w), code))
+            if b < 0:
+                nat.check(1, "b200pose_jpeg_encode_bound")
+            cap += b
+        if dev_in or device:
+            stream = torch.cuda.current_stream(torch.device("cuda", self.device_index)).cuda_stream
+        out = (torch.empty(cap, dtype=torch.uint8, device="cuda:%d" % self.device_index) if device
+               else np.empty(cap, np.uint8))
+        hw = (ctypes.c_int * (2 * n))(*[int(v) for s in sizes for v in s])
+        lens = (ctypes.c_longlong * n)()
+        nat.check(nat.lib().b200pose_net_encode_jpegs(self._h, ctypes.c_void_p(src), int(dev_in), hw, n, int(quality), code,
+                                                      ctypes.c_void_p(out.data_ptr() if device else out.ctypes.data), cap,
+                                                      int(device), lens, ctypes.c_void_p(stream)),
+                  "b200pose_net_encode_jpegs")
+        total = sum(lens)
+        if device:      # the bound-sized buffer goes back to the allocator; the views keep only the streams
+            out = out[:total].clone()
+        res, at = [], 0
+        for k in lens:
+            res.append(out[at:at + k] if device else out[at:at + k].tobytes())
+            at += k
+        return res
 
     def __del__(self):
         try:
@@ -851,6 +935,10 @@ class PoseEngine:
         if check:
             self.post.check_status(n)
         return [self.post.humans(i) for i in range(n)]
+
+    def encode_jpegs(self, frames, quality=95, sampling="420", device=False, stream=0):
+        """NativeNet.encode_jpegs on this engine's device: cv2.imencode('.jpg', ...) of every frame, on the GPU."""
+        return self.net.encode_jpegs(frames, quality, sampling, device, stream)
 
     def draw_humans(self, frames, ticket=None, dest_size=368, factor=8, net_sizes=None):
         """draw_humans(frame, humans_from_rows(rows, net_w, net_h)) for every frame of run `ticket` (default: the

@@ -108,16 +108,57 @@ def eval_coco(outputs, annFile, imgIds):
 EVAL_BATCH = 32      # images per device batch of the batched evaluation loop
 
 
-def _humans_batched(core, images, preprocess):
+def is_jpeg_name(name):
+    return os.path.splitext(name)[1].lower() in (".jpg", ".jpeg")
+
+
+def write_vis_device(post, net, frames, net_hw, paths, keep):
+    """cv2.imwrite(paths[k], draw_humans(frames[k], humans)) for the frames k in `keep`, on the device: the frames are
+    uploaded once into a packed buffer, the persons of the post object's selected run (frame i: image i of the run,
+    coordinates of a network input net_hw[i]) are drawn on it in place (b200pose_post_draw), and the kept frames are
+    encoded from the same buffer at cv2.imwrite's JPEG defaults, quality 95 and 4:2:0 (b200pose_net_encode_jpegs).  The
+    host frames are left as they are."""
+    dev = torch.from_numpy(np.concatenate([np.ascontiguousarray(f).reshape(-1) for f in frames]))
+    dev = dev.to("cuda:%d" % net.device_index)
+    sizes = [f.shape[:2] for f in frames]
+    post.draw(dev.data_ptr(), True, len(frames), sizes, net_hw, torch.cuda.current_stream(dev.device).cuda_stream)
+    views, at = [], 0
+    for h, w in sizes:
+        views.append(dev[at:at + h * w * 3].view(h, w, 3))
+        at += h * w * 3
+    for k, blob in zip(keep, net.encode_jpegs([views[k] for k in keep], 95, "420")):
+        with open(paths[k], "wb") as f:
+            f.write(blob)
+
+
+def _humans_batched(core, images, preprocess, vis_paths=None):
     """images (raw BGR frames of mixed sizes) -> per image (humans, heat-map shape): one fused device pass per ragged
     batch of frames of different sizes (crop_with_factor, normalisation, network, NMS, PAF matching, assembly - nothing but the person rows comes back)
-    instead of get_outputs + paf_to_pose_cpp per image.  Same kernels, same arithmetic: identical persons."""
+    instead of get_outputs + paf_to_pose_cpp per image.  Same kernels, same arithmetic: identical persons.
+    vis_paths: per image its visualisation file; those named .jpg / .jpeg are drawn, encoded and written on the device
+    here (write_vis_device), one ragged batch after the other, the others are left to the caller."""
     from .. import _native as nat
+    from ..engine import plan_ragged_batches
     from ..lib.utils.paf_to_pose import humans_from_rows
     eng = core.pose_engine(batch_cap=EVAL_BATCH)
     eng.net.set_preprocess(preprocess)
-    rows = eng.infer_images_arrays(images, cfg.DATASET.IMAGE_SIZE, cfg.MODEL.DOWNSAMPLE,
-                                   float(np.float32(cfg.TEST.THRESH_HEATMAP)))
+    args = (cfg.DATASET.IMAGE_SIZE, cfg.MODEL.DOWNSAMPLE, float(np.float32(cfg.TEST.THRESH_HEATMAP)))
+    jpeg = [bool(vis_paths) and is_jpeg_name(vis_paths[i]) for i in range(len(images))]
+    if not any(jpeg):
+        rows = eng.infer_images_arrays(images, *args)
+    else:
+        # the ragged batches infer_images_arrays would run, one call each, so that each batch's run is the selected
+        # one when its frames are drawn; a batch planned again on its own frames stays one batch
+        pads = [nat.crop_geometry(im.shape[0], im.shape[1], args[0], args[1])[2] for im in images]
+        rows = [None] * len(images)
+        for part in plan_ragged_batches(pads, eng.post.batch_cap):
+            sub = [images[i] for i in part]
+            for i, r in zip(part, eng.infer_images_arrays(sub, *args)):
+                rows[i] = r
+            keep = [k for k, i in enumerate(part) if jpeg[i]]
+            if keep:
+                eng.post.sync()
+                write_vis_device(eng.post, eng.net, sub, [pads[i] for i in part], [vis_paths[i] for i in part], keep)
     out = []
     for img, r in zip(images, rows):
         scale, _, (ph, pw) = nat.crop_geometry(img.shape[0], img.shape[1], cfg.DATASET.IMAGE_SIZE, cfg.MODEL.DOWNSAMPLE)
@@ -129,7 +170,9 @@ def run_eval(image_dir, anno_file, vis_dir, model, preprocess):
     """coco_eval.py:245-283: every person image of the annotation file -> get_outputs -> paf_to_pose_cpp ->
     visualisation written to vis_dir -> COCO records -> mAP.  With a model from this package's get_model() the images
     are processed EVAL_BATCH at a time by the fused batched engine (SURVEY.md 8f rank 3); any other module takes the
-    reference's image-by-image sequence.  Records, visualisations and printed progress are the same either way."""
+    reference's image-by-image sequence; its visualisations with a .jpg / .jpeg name are then drawn and encoded on the
+    device, byte for byte cv2.imwrite(draw_humans(...)).  Records, visualisations and printed progress are the same
+    either way."""
     COCO, _ = _pycocotools()
     coco = COCO(anno_file)
     img_ids = coco.getImgIds(catIds=coco.getCatIds(catNms=['person']))
@@ -143,7 +186,7 @@ def run_eval(image_dir, anno_file, vis_dir, model, preprocess):
         names = [coco.loadImgs(img_id)[0]['file_name'] for img_id in chunk]
         images = [cv2.imread(os.path.join(image_dir, name)) for name in names]
         if batched:
-            results = _humans_batched(core, images, preprocess)
+            results = _humans_batched(core, images, preprocess, [os.path.join(vis_dir, name) for name in names])
         else:
             results = []
             for ori in images:
@@ -153,7 +196,8 @@ def run_eval(image_dir, anno_file, vis_dir, model, preprocess):
             i = c0 + k
             if i % 10 == 0 and i != 0:
                 print("Processed {} images".format(i))
-            cv2.imwrite(os.path.join(vis_dir, name), draw_humans(ori, humans))
+            if not (batched and is_jpeg_name(name)):      # .jpg / .jpeg: written on the device by _humans_batched
+                cv2.imwrite(os.path.join(vis_dir, name), draw_humans(ori, humans))
             upsample_keypoints = (hm_shape[0] * cfg.MODEL.DOWNSAMPLE / scale_img,
                                   hm_shape[1] * cfg.MODEL.DOWNSAMPLE / scale_img)
             append_result(img_id, humans, upsample_keypoints, outputs)
