@@ -25,6 +25,7 @@
 //   * Persistent grid (one CTA per SM), static round-robin tile schedule; warp 0 (patches) and warp 1 (weights) run
 //     ahead of the consumers through mbarrier rings and prefetch the next tile's operands during the epilogue.
 #include <cstdio>
+#include <type_traits>
 
 #include "conv_tc.cuh"
 #include "fp8_core.h"
@@ -415,10 +416,17 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
             // The per-channel constants of kEpC column groups at a time are loaded before any of their stores: loaded next to
             // each group's stores, every one of the N / 8 groups waited a full load latency behind the previous group.
             constexpr int kEpC = N / 8 < 8 ? N / 8 : 8;
+            // The column groups are unrolled, so their code is the largest part of the kernel, and every tile runs it once,
+            // after the main loop has taken the instruction caches.  Only the stage heads write fp32 maps and only bf16x3
+            // has a residual plane, so those paths are compiled into a separate copy (kF32) or only into the bf16x3
+            // kernels: the copy a launch runs holds none of the stores it never makes (DESIGN.md §6, *Epilogue code*).
+            auto columns = [&](auto f32_tag) {
+            constexpr bool kF32 = decltype(f32_tag)::value;
 #pragma unroll
             for (int j0 = 0; j0 < N / 8; j0 += kEpC) {
-            float2 bias2[kEpC], slope2[kPrelu ? kEpC : 1];
-            int2 wexp2[kE4m3 ? kEpC : 1];
+            float2 bias2[kEpC];
+            [[maybe_unused]] float2 slope2[kPrelu ? kEpC : 1];
+            [[maybe_unused]] int2 wexp2[kE4m3 ? kEpC : 1];
 #pragma unroll
             for (int j = j0; j < j0 + kEpC; ++j) {
                 bias2[j - j0] = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + cq));
@@ -474,13 +482,15 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                         } else {
                             *reinterpret_cast<uint32_t*>(out_px[hh] + 8 * j) = pack_bf16x2(lo, hi);
                         }
-                        if (a.out_lo != nullptr) {      // bf16x3: residual plane v - bf16(v)
-                            __nv_bfloat16* dlo = a.out_lo + (out_px[hh] - a.out) + 8 * j;
-                            *reinterpret_cast<uint32_t*>(dlo) =
-                                pack_bf16x2(lo - __bfloat162float(__float2bfloat16_rn(lo)), hi - __bfloat162float(__float2bfloat16_rn(hi)));
+                        if constexpr (tc_planes(F) == 2) {
+                            if (a.out_lo != nullptr) {      // bf16x3: residual plane v - bf16(v)
+                                __nv_bfloat16* dlo = a.out_lo + (out_px[hh] - a.out) + 8 * j;
+                                *reinterpret_cast<uint32_t*>(dlo) = pack_bf16x2(lo - __bfloat162float(__float2bfloat16_rn(lo)),
+                                                                                hi - __bfloat162float(__float2bfloat16_rn(hi)));
+                            }
                         }
                     }
-                    if (of32 != nullptr) {
+                    if constexpr (kF32) {
                         const int c = ch_tile + 8 * j + cq;
                         if (c < f32_ch) of32[(static_cast<size_t>(tc.n * f32_ch + c) * Ho + yo_px[hh]) * Wo + xo] = lo;
                         if (c + 1 < f32_ch) of32[(static_cast<size_t>(tc.n * f32_ch + c + 1) * Ho + yo_px[hh]) * Wo + xo] = hi;
@@ -488,6 +498,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcArgs& a) {
                 }
             }
             }
+            };
+            if (of32 != nullptr) columns(std::true_type{});
+            else columns(std::false_type{});
             if constexpr (kAux == TcAux::kAmax) {     // max of non-negative float bits: order-independent, so runs stay deterministic
                 amax = __reduce_max_sync(0xffffffffu, amax);
                 if (lane == 0 && amax != 0) atomicMax(a.amax_out + tc.n, amax << 16);
