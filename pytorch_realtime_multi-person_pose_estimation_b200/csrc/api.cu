@@ -73,41 +73,6 @@ const bool kPoolAfter[12] = {false, true, false, true, false, false, false, true
 constexpr int kPaf = 38, kHeat = 19, kFeat = 128, kCat = kPaf + kHeat + kFeat;
 
 constexpr int kStages = 6;     // refinement stages of the network; a forward may stop after any of them
-int stage_num_layers(int stage) { return stage == 1 ? 5 : 7; }
-ConvSpec stage_layer(int stage, int branch, int li) {
-    const int outc = branch == 0 ? kPaf : kHeat;
-    if (stage == 1) {
-        if (li < 3) return {128, 128, 3};
-        if (li == 3) return {128, 512, 1};
-        return {512, outc, 1};
-    }
-    if (li == 0) return {kCat, 128, 7};
-    if (li < 5) return {128, 128, 7};
-    if (li == 5) return {128, 128, 1};
-    return {128, outc, 1};
-}
-// conv index in state_dict order: trunk 0..11, then branch 0 stages 1..6, then branch 1 stages 1..6
-int conv_index(int stage, int branch, int li) {
-    int idx = 12;
-    for (int b = 0; b < 2; ++b)
-        for (int s = 1; s <= 6; ++s) {
-            if (b == branch && s == stage) return idx + li;
-            idx += stage_num_layers(s);
-        }
-    return -1;
-}
-constexpr int kNumConvs = 12 + 2 * (5 + 5 * 7);   // 92
-ConvSpec conv_spec(int ci) {
-    if (ci < 12) return kTrunk[ci];
-    int idx = 12;
-    for (int b = 0; b < 2; ++b)
-        for (int s = 1; s <= 6; ++s) {
-            const int nl = stage_num_layers(s);
-            if (ci < idx + nl) return stage_layer(s, b, ci - idx);
-            idx += nl;
-        }
-    return {0, 0, 0};
-}
 // physical channel of the bf16 concat buffer [paf 0..37, pad, heat 40..58, pad, feat 64..191] for reference
 // concat channel c of torch.cat([paf, heat, feat], 1) (rtpose_vgg.py:165)
 int cat_phys(int c) { return c < kPaf ? c : (c < kPaf + kHeat ? c + 2 : c + 7); }
@@ -119,9 +84,8 @@ int cat_phys(int c) { return c < kPaf ? c : (c < kPaf + kHeat ? c + 2 : c + 7); 
 // a 1x1 Mconv6 and the 1x1 head Mconv7; every conv but Mconv7 is followed by a PReLU.  Stage inputs: the features (L2
 // stage 1), cat[features, paf] (L2 stages >= 2, L1 stage 1), cat[features, heat, paf] (L1 stages >= 2).
 enum Nonlin { kNoAct, kRelu, kPrelu };
-constexpr int kOpMaxStages = 12, kOpStageConvs = 17;
+constexpr int kOpMaxStages = 12;
 bool op_valid(int l2, int l1) { return l2 >= 1 && l1 >= 1 && l2 + l1 <= kOpMaxStages; }
-int op_num_convs(int l2, int l1) { return 12 + kOpStageConvs * (l2 + l1); }
 struct OpStage {
     bool paf, first;                  // PAF (L2) stage; first stage of its branch (96 inner channels)
     int in, inner, innerout, out;     // StageBlock's channels
@@ -130,44 +94,6 @@ OpStage op_stage(int l2, int t) {
     const bool paf = t < l2, first = t == 0 || t == l2;
     const int in = t == 0 ? kFeat : (paf || first ? kFeat + kPaf : kFeat + kHeat + kPaf);
     return {paf, first, in, first ? 96 : 128, first ? 256 : 512, paf ? kPaf : kHeat};
-}
-// conv ci in state_dict order: trunk 0..11, then 17 per stage (Mconv1_0 .. Mconv5_2, Mconv6, Mconv7)
-struct OpConv { ConvSpec s; Nonlin act; };
-OpConv op_conv(int l2, int ci) {
-    if (ci < 12) return {kTrunk[ci], ci >= 9 ? kPrelu : kRelu};
-    const int t = (ci - 12) / kOpStageConvs, li = (ci - 12) % kOpStageConvs;
-    const OpStage g = op_stage(l2, t);
-    if (li == 16) return {{g.innerout, g.out, 1}, kNoAct};
-    if (li == 15) return {{3 * g.inner, g.innerout, 1}, kPrelu};
-    return {{li % 3 ? g.inner : (li == 0 ? g.in : 3 * g.inner), g.inner, 3}, kPrelu};
-}
-// state_dict tensor `index` of OpenPose_Model(l2, l1): conv *ci, *kind 0 = weight, 1 = bias, 2 = PReLU slope (each conv's
-// tensors in that order).  False when out of range.
-bool op_tensor(int l2, int l1, int index, int* ci, int* kind) {
-    for (int c = 0; c < op_num_convs(l2, l1); ++c) {
-        const int nt = op_conv(l2, c).act == kPrelu ? 3 : 2;
-        if (index < nt) {
-            *ci = c;
-            *kind = index;
-            return index >= 0;
-        }
-        index -= nt;
-    }
-    return false;
-}
-int op_num_tensors(int l2, int l1) {
-    int n = 0;
-    for (int c = 0; c < op_num_convs(l2, l1); ++c) n += op_conv(l2, c).act == kPrelu ? 3 : 2;
-    return n;
-}
-int op_tensor_shape(int l2, int l1, int index, long dims[4]) {
-    int ci, kind;
-    if (!op_valid(l2, l1) || !op_tensor(l2, l1, index, &ci, &kind)) return -1;
-    const ConvSpec s = op_conv(l2, ci).s;
-    dims[0] = s.cout;
-    if (kind != 0) return 1;
-    dims[1] = s.cin; dims[2] = s.ks; dims[3] = s.ks;
-    return 4;
 }
 
 // Input channel permutation of a tensor-core layer: reference channel c of its input -> channel of the buffer it reads.
@@ -303,24 +229,154 @@ const Wiring kStageWiring[7] = {     // stages 2 .. 6
     {BRA,   0,  128,  BRB,   {0, 128}, {128, 128}},
     {BRB,   0,  128,  CAT,   {0, 40},  {40, 24}, true},
 };
-// OpenPose_Model (DESIGN §2.11): bra and brb hold 768 channels, six 128-channel slots: a dense block's three outputs go to
+// ---------------------------------------------------------------- the architecture of a net
+// A conv in state_dict order and the nonlinearity after it.  Its tensors are the weight, the bias and, for a PReLU
+// conv, the slopes.
+struct ArchConv { ConvSpec s; Nonlin act; };
+
+// One tensor-core launch, in launch order (conv1_1 runs on CUDA cores before them).  Its ReLU or PReLU is its convs'.
+struct ArchLayer {
+    int stage;                // 0 = the trunk; a forward of k stages runs the layers of stages 0 .. k
+    std::vector<int> convs;   // conv per group
+    int n_tile, pool;
+    InPerm perm;
+    Wiring wiring;
+    int map0;                 // stage head: the fp32 map group 0 writes (group 1: map0 + 1); -1 otherwise
+};
+
+// Everything the runtime knows about a net's architecture, built once when the net is created.
+struct NetArch {
+    std::string name;                   // as the refusals print it
+    int l2 = 0, l1 = 0;                 // OpenPose_Model's L2 / L1 stage counts; 0 for rtpose
+    int stages = 0;                     // refinement stages; a net runs all of them unless set_stages asks for fewer
+    std::vector<ArchConv> convs;        // state_dict order
+    std::vector<ArchLayer> layers;      // launch order
+    int act_c[kNumAct];                 // channels per pixel of each activation buffer
+    bool zero_pads[kNumAct] = {};       // buffers with pad lanes no launch writes: zeroed when a plan is built
+    // channels of each stage map (outputs[] entries, saved_for_loss order): rtpose [paf_1, heat_1, ..., paf_6, heat_6];
+    // OpenPose_Model [paf_1 .. paf_l2, heat_1 .. heat_l1]
+    int map_ch[12];
+    // by stage count k, for every k a forward of the net may run: the stage maps 0 .. maps-1 it writes and, among
+    // them, the final PAF and heat map
+    struct { int maps, paf, heat; } out[kOpMaxStages + 1] = {};
+};
+
+// The trunk of both architectures: rtpose's twelve convs, PReLU after those from prelu_from on, and the eleven
+// tensor-core layers of conv1_2 .. conv4_4_CPM.
+NetArch trunk_arch(int prelu_from) {
+    NetArch a;
+    for (int i = 0; i < 12; ++i) a.convs.push_back({kTrunk[i], i >= prelu_from ? kPrelu : kRelu});
+    for (int i = 1; i < 12; ++i)
+        a.layers.push_back({0, {i}, std::min(kTrunk[i].cout, 128), kPoolAfter[i], kPermNone, kTrunkWiring[i - 1], -1});
+    memcpy(a.act_c, kActC, sizeof(kActC));
+    a.zero_pads[CAT] = true;
+    return a;
+}
+
+// rtpose (rtpose_vgg.py:69-127): state_dict order is the trunk, then branch 0 (PAF) stages 1 .. 6, then branch 1
+// (heat map) stages 1 .. 6.  Each layer of a stage runs both branches as one two-group launch.
+NetArch rtpose_arch() {
+    NetArch a = trunk_arch(12);
+    a.name = "rtpose";
+    a.stages = kStages;
+    int first[2][kStages + 1];      // conv of layer 0 of branch b, stage s
+    for (int b = 0; b < 2; ++b)
+        for (int s = 1; s <= kStages; ++s) {
+            const int outc = b == 0 ? kPaf : kHeat;
+            const std::vector<ConvSpec> convs = s == 1
+                ? std::vector<ConvSpec>{{128, 128, 3}, {128, 128, 3}, {128, 128, 3}, {128, 512, 1}, {512, outc, 1}}
+                : std::vector<ConvSpec>{{kCat, 128, 7}, {128, 128, 7}, {128, 128, 7}, {128, 128, 7}, {128, 128, 7},
+                                        {128, 128, 1}, {128, outc, 1}};
+            first[b][s] = (int)a.convs.size();
+            for (const ConvSpec& c : convs) a.convs.push_back({c, kRelu});
+            a.convs.back().act = kNoAct;      // the head
+        }
+    for (int s = 1; s <= kStages; ++s)
+        for (int li = 0; li < (s == 1 ? 5 : 7); ++li) {
+            const Wiring& wr = (s == 1 ? kStage1Wiring : kStageWiring)[li];
+            a.layers.push_back({s, {first[0][s] + li, first[1][s] + li}, wr.maps ? 48 : 128, 0,
+                                s > 1 && li == 0 ? kPermRtposeCat : kPermNone, wr, wr.maps ? 2 * (s - 1) : -1});
+        }
+    for (int i = 0; i < 12; ++i) a.map_ch[i] = i % 2 == 0 ? kPaf : kHeat;
+    for (int k = 1; k <= kStages; ++k) a.out[k] = {2 * k, 2 * k - 2, 2 * k - 1};
+    return a;
+}
+
+// OpenPose_Model(l2, l1): state_dict order is the trunk, then 17 convs per stage (Mconv1_0 .. Mconv5_2, Mconv6, Mconv7),
+// one launch each; stage t writes map t.  n-tiles: 48 for the 96-channel convs (two tiles, no pad lanes), 128 for the
+// others; the heads 64 (PAF: zero rows 38..63 store +0 over the heat slot) and 32 (heat map).
+// DESIGN §2.11: bra and brb hold 768 channels, six 128-channel slots: a dense block's three outputs go to
 // slots 0, 1, 2 (stages of 128 inner channels) or 3, 4, 5 (the 96-channel first stage of each branch: lanes 96..127 of
 // those slots are never written and stay +0).  Blocks 1, 3, 5 write bra, blocks 2, 4 brb: Mconv{b}_0 reads all three
 // slots of the other buffer, _1 reads slot 0 and writes slot 1, _2 reads slot 1 and writes slot 2.  Mconv6 writes br512
 // (512 channels).  The PAF heads store 64 lanes at channel 0 of the concat buffer - PAF, then +0 from zero rows and bias
 // over the heat slot and the pad lanes, so that an L2 stage >= 2 or L1 stage 1, which reads the heat slot against zero
 // weights, never reads an earlier forward's values; the heat-map heads store the 24 lanes from channel 40.
-constexpr int kOpActBr = 768, kOpActBr512 = 512;
-Wiring op_wiring(int l2, int t, int li) {
-    const OpStage g = op_stage(l2, t);
-    const int base = g.first ? 384 : 0, store = g.inner == 96 ? 48 : 128;
-    if (li == 16) return g.paf ? Wiring{BR512, 0, 0, CAT, {0, 0}, {64, 0}, true} : Wiring{BR512, 0, 0, CAT, {40, 0}, {24, 0}, true};
-    if (li == 15) return {BRA, base, 0, BR512, {0, 0}, {128, 0}};
-    const int b = li / 3, j = li % 3;
-    const int cur = b % 2 ? BRB : BRA, prev = b % 2 ? BRA : BRB;
-    if (li == 0) return {CAT, t == 0 ? 64 : 0, 0, cur, {base, 0}, {store, 0}};
-    if (j == 0) return {prev, base, 0, cur, {base, 0}, {store, 0}};
-    return {cur, base + 128 * (j - 1), 0, cur, {base + 128 * j, 0}, {store, 0}};
+NetArch openpose_arch(int l2, int l1) {
+    NetArch a = trunk_arch(9);
+    a.name = "OpenPose_Model(" + std::to_string(l2) + ", " + std::to_string(l1) + ")";
+    a.l2 = l2;
+    a.l1 = l1;
+    a.stages = l2 + l1;
+    auto add = [&](ConvSpec s, Nonlin act, ArchLayer l) {      // a conv and its launch
+        l.convs = {(int)a.convs.size()};
+        a.convs.push_back({s, act});
+        a.layers.push_back(l);
+    };
+    for (int t = 0; t < l2 + l1; ++t) {
+        const OpStage g = op_stage(l2, t);
+        const int base = g.first ? 384 : 0, n = g.inner == 96 ? 48 : 128;     // first slot; n-tile and lanes stored
+        for (int b = 0; b < 5; ++b) {      // Mconv{b + 1}_{0,1,2}
+            const int cur = b % 2 ? BRB : BRA, prev = b % 2 ? BRA : BRB;
+            if (b == 0)
+                add({g.in, g.inner, 3}, kPrelu, {t + 1, {}, n, 0, t == 0 ? kPermNone : (g.paf || g.first ? kPermFeatPaf : kPermFeatHeatPaf),
+                                                 {CAT, t == 0 ? 64 : 0, 0, cur, {base, 0}, {n, 0}}, -1});
+            else
+                add({3 * g.inner, g.inner, 3}, kPrelu, {t + 1, {}, n, 0, kPermSlots, {prev, base, 0, cur, {base, 0}, {n, 0}}, -1});
+            for (int j = 1; j < 3; ++j)
+                add({g.inner, g.inner, 3}, kPrelu,
+                    {t + 1, {}, n, 0, kPermNone, {cur, base + 128 * (j - 1), 0, cur, {base + 128 * j, 0}, {n, 0}}, -1});
+        }
+        add({3 * g.inner, g.innerout, 1}, kPrelu, {t + 1, {}, 128, 0, kPermSlots, {BRA, base, 0, BR512, {0, 0}, {128, 0}}, -1});
+        add({g.innerout, g.out, 1}, kNoAct,
+            {t + 1, {}, g.paf ? 64 : 32, 0, kPermNone, {BR512, 0, 0, CAT, {g.paf ? 0 : 40, 0}, {g.paf ? 64 : 24, 0}, true}, t});
+    }
+    a.act_c[BRA] = a.act_c[BRB] = 768;
+    a.act_c[BR512] = 512;
+    a.zero_pads[BRA] = a.zero_pads[BRB] = true;     // the 96-channel dense-block slots
+    for (int i = 0; i < 12; ++i) a.map_ch[i] = i < l2 ? kPaf : kHeat;
+    a.out[l2 + l1] = {l2 + l1, l2 - 1, l2 + l1 - 1};
+    return a;
+}
+
+// state_dict tensor `index` of architecture a: conv *ci, *kind 0 = weight, 1 = bias, 2 = PReLU slope.  False when out of
+// range.
+bool arch_tensor(const NetArch& a, int index, int* ci, int* kind) {
+    if (index < 0) return false;
+    for (int c = 0; c < (int)a.convs.size(); ++c) {
+        const int nt = a.convs[c].act == kPrelu ? 3 : 2;
+        if (index < nt) {
+            *ci = c;
+            *kind = index;
+            return true;
+        }
+        index -= nt;
+    }
+    return false;
+}
+int arch_num_tensors(const NetArch& a) {
+    int n = 0;
+    for (const ArchConv& c : a.convs) n += c.act == kPrelu ? 3 : 2;
+    return n;
+}
+int arch_tensor_shape(const NetArch& a, int index, long dims[4]) {
+    int ci, kind;
+    if (!arch_tensor(a, index, &ci, &kind)) return -1;
+    const ConvSpec s = a.convs[ci].s;
+    dims[0] = s.cout;
+    if (kind != 0) return 1;
+    dims[1] = s.cin; dims[2] = s.ks; dims[3] = s.ks;
+    return 4;
 }
 
 struct PlanLaunch {
@@ -358,14 +414,13 @@ struct LastForward {
 
 struct b200pose_net {
     int device = 0, num_sms = 0;
-    // architecture, fixed at creation: OpenPose_Model(l2, l1) (b200pose_net_create_openpose), or rtpose when l2 == 0
-    int l2 = 0, l1 = 0;
+    // architecture, fixed at creation: rtpose, or OpenPose_Model(l2, l1) (b200pose_net_create_openpose)
+    NetArch arch;
     bool finalized = false;
     std::vector<std::vector<float>> host_w, host_b, host_slope;   // per conv (slope: PReLU convs only)
     std::vector<bool> have;                                        // per tensor
     std::vector<DevBuf<float>> d_w, d_b, d_slope;      // per conv, fp32 OIHW (parity mode, conv1_1) and PReLU slopes
-    // tensor-core layers: trunk 1..11 -> tc[0..10]; stage 1: tc[11..15]; stage t>=2: tc[16 + (t-2)*7 + li]
-    std::vector<TcLayer> tc;
+    std::vector<TcLayer> tc;                           // per layer of arch
     // Plans of the last 32 keys are kept, so that alternating shapes (multi-scale, mixed frame sizes) do not re-encode
     // up to 51 tensor maps and synchronise the stream.  `plan` is the one the last tensor-core forward selected.
     std::list<Plan> plans;
@@ -478,37 +533,12 @@ struct b200pose_post {
 
 namespace {
 
-bool is_openpose(const b200pose_net* net) { return net->l2 > 0; }
-ConvSpec net_conv(const b200pose_net* net, int ci) { return is_openpose(net) ? op_conv(net->l2, ci).s : conv_spec(ci); }
-int net_num_convs(const b200pose_net* net) { return is_openpose(net) ? op_num_convs(net->l2, net->l1) : kNumConvs; }
-int net_num_tensors(const b200pose_net* net) {
-    return is_openpose(net) ? op_num_tensors(net->l2, net->l1) : B200POSE_NUM_TENSORS;
-}
-// "OpenPose_Model(l2, l1)" or "rtpose": the refusals name the net's architecture
-std::string arch_name(const b200pose_net* net) {
-    return is_openpose(net) ? "OpenPose_Model(" + std::to_string(net->l2) + ", " + std::to_string(net->l1) + ")" : "rtpose";
-}
-// Stage maps a forward of the net writes (outputs[] entries, saved_for_loss order) and the channels of map i: rtpose
-// [paf_1, heat_1, ..., paf_k, heat_k]; OpenPose_Model [paf_1 .. paf_l2, heat_1 .. heat_l1].
-int net_num_maps(const b200pose_net* net, int stages) { return is_openpose(net) ? net->l2 + net->l1 : 2 * stages; }
-int map_ch(const b200pose_net* net, int i) {
-    return (is_openpose(net) ? i < net->l2 : i % 2 == 0) ? kPaf : kHeat;
-}
-// channels per pixel of activation buffer i
-int act_c(const b200pose_net* net, int i) {
-    if (is_openpose(net) && (i == BRA || i == BRB)) return kOpActBr;
-    if (is_openpose(net) && i == BR512) return kOpActBr512;
-    return kActC[i];
-}
+bool is_openpose(const b200pose_net* net) { return net->arch.l2 > 0; }
 
 // The final maps of the last forward: the PAF and heatmap of its last stage (OpenPose_Model: of its last L2 and L1
 // stages).
-const float* last_paf(const b200pose_net* net) {
-    return net->out_f32[is_openpose(net) ? net->l2 - 1 : 2 * net->last.stages - 2].p;
-}
-const float* last_heat(const b200pose_net* net) {
-    return net->out_f32[is_openpose(net) ? net->l2 + net->l1 - 1 : 2 * net->last.stages - 1].p;
-}
+const float* last_paf(const b200pose_net* net) { return net->out_f32[net->arch.out[net->last.stages].paf].p; }
+const float* last_heat(const b200pose_net* net) { return net->out_f32[net->arch.out[net->last.stages].heat].p; }
 
 // Calls row(g, o, r, w) for output channel o of every group g of layer L (packed row r = g * cout_pad + o), w its fp32
 // weights in packed order [tap][cin_pad]: input channels at their physical channel of the buffer the layer reads
@@ -517,7 +547,7 @@ template <class F> void for_each_weight_row(const b200pose_net* net, const TcLay
     const int taps = L.ks * L.ks, cin_pad = L.cin_blocks * 64, cout_pad = L.n_tiles * L.n_tile;
     std::vector<float> w((size_t)taps * cin_pad);
     for (int g = 0; g < L.groups; ++g) {
-        const ConvSpec s = net_conv(net, L.convs[g]);
+        const ConvSpec s = net->arch.convs[L.convs[g]].s;
         const std::vector<float>& hw = net->host_w[L.convs[g]];
         for (int o = 0; o < s.cout; ++o) {
             std::fill(w.begin(), w.end(), 0.f);
@@ -529,18 +559,17 @@ template <class F> void for_each_weight_row(const b200pose_net* net, const TcLay
     }
 }
 
-// The layer of the convs conv_ids (one per group), before any weights are packed.  Its input is 192 channels of the
-// concat buffer (the concat permutations), three 128-channel slots (kPermSlots) or the conv's input channels rounded up to
-// 64.  prelu: the convs' PReLU replaces `relu`.
-TcLayer make_tc_layer(const b200pose_net* net, const std::vector<int>& conv_ids, int n_tile, InPerm perm, int relu,
-                      int pool, bool prelu = false) {
-    const ConvSpec sp = net_conv(net, conv_ids[0]);
-    const int cin_pad = perm == kPermSlots ? 3 * 128 : (perm != kPermNone ? 192 : (sp.cin + 63) / 64 * 64);
-    const int cout_pad = ((sp.cout + n_tile - 1) / n_tile) * n_tile;
+// The tensor-core layer of arch layer l, before any weights are packed.  Its input is 192 channels of the concat buffer
+// (the concat permutations), three 128-channel slots (kPermSlots) or the conv's input channels rounded up to 64.
+TcLayer make_tc_layer(const NetArch& arch, const ArchLayer& l) {
+    const ArchConv& c0 = arch.convs[l.convs[0]];
+    const ConvSpec sp = c0.s;
+    const int cin_pad = l.perm == kPermSlots ? 3 * 128 : (l.perm != kPermNone ? 192 : (sp.cin + 63) / 64 * 64);
+    const int cout_pad = ((sp.cout + l.n_tile - 1) / l.n_tile) * l.n_tile;
     TcLayer L;
-    L.ks = sp.ks; L.cin_blocks = cin_pad / 64; L.groups = (int)conv_ids.size(); L.n_tile = n_tile; L.n_tiles = cout_pad / n_tile;
-    L.relu = relu; L.pool = pool; L.prelu = prelu; L.convs = conv_ids; L.perm = perm; L.slot = sp.cin / 3;
-    for (int c : conv_ids) L.macs_per_pixel += (double)net_conv(net, c).cin * net_conv(net, c).cout * sp.ks * sp.ks;
+    L.ks = sp.ks; L.cin_blocks = cin_pad / 64; L.groups = (int)l.convs.size(); L.n_tile = l.n_tile; L.n_tiles = cout_pad / l.n_tile;
+    L.relu = c0.act == kRelu; L.pool = l.pool; L.prelu = c0.act == kPrelu; L.convs = l.convs; L.perm = l.perm; L.slot = sp.cin / 3;
+    for (int c : l.convs) L.macs_per_pixel += (double)arch.convs[c].s.cin * arch.convs[c].s.cout * sp.ks * sp.ks;
     return L;
 }
 
@@ -692,14 +721,14 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         a.ea_out = net->ea.p + (size_t)slot * n;
     }
     if (tc_aux(p.fmt) == TcAux::kOverflow) a.ovf_out = net->ovf.p;
-    a.out = net->act[wr.out].p; a.out_cstride = act_c(net, wr.out);
+    a.out = net->act[wr.out].p; a.out_cstride = net->arch.act_c[wr.out];
     a.out_ch_off[0] = wr.out_off[0]; a.out_ch_off[1] = wr.out_off[1];
     a.store_ch[0] = wr.store[0]; a.store_ch[1] = wr.store[1];
     const int f32[2] = {wr.maps ? map0 : -1, wr.maps && L.groups == 2 ? map0 + 1 : -1};
     for (int g = 0; g < 2; ++g)
         if (f32[g] >= 0) {
             a.out_f32[g] = net->out_f32[f32[g]].p;
-            a.f32_ch[g] = map_ch(net, f32[g]);
+            a.f32_ch[g] = net->arch.map_ch[f32[g]];
         }
     // small batches (the 46 x 46 layers fill less than half of the SMs with 16 x 16 tiles): chain the layers with programmatic
     // dependent launches; the first tensor-core layer follows conv1_1, which does not signal.  small_plan gets this
@@ -712,7 +741,7 @@ int add_plan(const b200pose_net* net, Plan& p, const TcLayer& L, const Wiring& w
         in_lo = net->act_lo[wr.in].p;
         a.out_lo = net->act_lo[wr.out].p;
     }
-    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, act_c(net, wr.in), L.w[(int)tc_weights(p.fmt)].p, in_lo);
+    cudaError_t e = conv_tc_make_maps(a, net->act[wr.in].p, net->arch.act_c[wr.in], L.w[(int)tc_weights(p.fmt)].p, in_lo);
     if (e != cudaSuccess) return cuda_fail("conv_tc_make_maps failed: %s", cudaGetErrorString(e));
     p.launches.push_back({a, 2.0 * n * H * W * L.macs_per_pixel, wr.in, wr.out, {f32[0], f32[1]}});
     return 0;
@@ -737,17 +766,18 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
     const size_t px = (size_t)p.n * p.H * p.W;
     for (int plane = 0; plane < tc_planes(p.fmt); ++plane) {
         DevBuf<__nv_bfloat16>* bufs = plane ? net->act_lo : net->act;
-        for (int i = 0; i < kNumAct; ++i) CU(bufs[i].ensure(px / (kActDiv[i] * kActDiv[i]) * act_c(net, i)));
-        // pad lanes of the concat buffer must read as zero; on the caller's stream (a non-blocking stream is not ordered
+        for (int i = 0; i < kNumAct; ++i) CU(bufs[i].ensure(px / (kActDiv[i] * kActDiv[i]) * net->arch.act_c[i]));
+        // pad lanes no launch writes must read as zero; on the caller's stream (a non-blocking stream is not ordered
         // against the legacy default stream a plain cudaMemset would use)
-        CU(cudaMemsetAsync(bufs[CAT].p, 0, px / 64 * kActC[CAT] * 2, st));
-        if (is_openpose(net))     // ... and those of the 96-channel dense-block slots
-            for (int i : {BRA, BRB}) CU(cudaMemsetAsync(bufs[i].p, 0, px / 64 * act_c(net, i) * 2, st));
+        for (int i = 0; i < kNumAct; ++i)
+            if (net->arch.zero_pads[i])
+                CU(cudaMemsetAsync(bufs[i].p, 0, px / (kActDiv[i] * kActDiv[i]) * net->arch.act_c[i] * 2, st));
     }
-    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * map_ch(net, i)));
-    if (tc_aux(p.fmt) == TcAux::kAmax) {     // rows for six stages whatever p.stages: plans of every stage count share them
-        CU(net->amax.ensure((size_t)(1 + 51) * p.n));
-        CU(net->ea.ensure((size_t)(1 + 51) * p.n));
+    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px / 64 * net->arch.map_ch[i]));
+    if (tc_aux(p.fmt) == TcAux::kAmax) {     // rows for every layer whatever p.stages: plans of every stage count share them
+        const size_t rows = 1 + net->arch.layers.size();
+        CU(net->amax.ensure(rows * p.n));
+        CU(net->ea.ensure(rows * p.n));
     }
     if (tc_aux(p.fmt) == TcAux::kOverflow) CU(net->ovf.ensure((size_t)p.n));
     if (tc_binary16(p.fmt))
@@ -760,24 +790,12 @@ int build_plan_tc(b200pose_net* net, Plan& p, cudaStream_t st) {
     int writer[kNumAct], cat_head = -1;
     for (int& w : writer) w = -1;
     writer[T1] = 0;
-    auto add = [&](const TcLayer& L, const Wiring& wr, int map0) {
+    for (size_t k = 0; k < net->tc.size() && net->arch.layers[k].stage <= p.stages; ++k) {
+        const Wiring& wr = net->arch.layers[k].wiring;
         const int ws[2] = {writer[wr.in], wr.in == CAT && wr.in_base == 0 ? cat_head : -1};
-        if (add_plan(net, p, L, wr, map0, ws)) return 1;
+        if (add_plan(net, p, net->tc[k], wr, net->arch.layers[k].map0, ws)) return 1;
         if (wr.out == CAT && wr.maps) cat_head = (int)p.launches.size();
         else writer[wr.out] = (int)p.launches.size();
-        return 0;
-    };
-    int k = 0;
-    for (const Wiring& wr : kTrunkWiring)
-        if (add(net->tc[k++], wr, 0)) return 1;
-    if (is_openpose(net)) {      // every stage, one after the other; stage t writes map t
-        for (int t = 0; t < net->l2 + net->l1; ++t)
-            for (int li = 0; li < kOpStageConvs; ++li)
-                if (add(net->tc[k++], op_wiring(net->l2, t, li), t)) return 1;
-    } else {
-        for (int s = 1; s <= p.stages; ++s)
-            for (int li = 0; li < stage_num_layers(s); ++li)
-                if (add(net->tc[k++], (s == 1 ? kStage1Wiring : kStageWiring)[li], 2 * (s - 1))) return 1;
     }
     p.buffers = plan_buffers(net, p.fmt);
     return 0;
@@ -879,6 +897,14 @@ int forward_tc(b200pose_net* net, const void* d_in, int in_u8, int n, int H, int
     return 0;
 }
 
+// The convs of group g of stage s's tensor-core layers, in launch order.
+std::vector<int> stage_convs(const NetArch& a, int s, int g) {
+    std::vector<int> v;
+    for (const ArchLayer& l : a.layers)
+        if (l.stage == s) v.push_back(l.convs[g]);
+    return v;
+}
+
 int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int stages, cudaStream_t st,
                  const int* ext) {
     const size_t px1 = (size_t)n * H * W;
@@ -887,7 +913,8 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
     CU(net->f_in.ensure(px1 * 3));
     CU(net->f_a.ensure(px1 * 64)); CU(net->f_b.ensure(px1 * 64));
     CU(net->f_cat.ensure(px8 * kCat)); CU(net->f_x.ensure(px8 * 512)); CU(net->f_y.ensure(px8 * 512));
-    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px8 * map_ch(net, i)));
+    for (int i = 0; i < 12; ++i) CU(net->out_f32[i].ensure(px8 * net->arch.map_ch[i]));
+    const NetArch& arch = net->arch;
     const bool op = is_openpose(net);
     if (op) { CU(net->f_cat3.ensure(px8 * kCat)); CU(net->f_z.ensure(px8 * 512)); }
     CU(nchw_to_nhwc_f32_launch(d_in, net->f_in.p, n, 3, H, W, 3, 0, st));
@@ -896,14 +923,13 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
     int cur_c = 3, ch = H, cw = W;
     float* ping = net->f_a.p;
     float* pong = net->f_b.p;
-    // relu: the conv's ReLU (rtpose); a conv with PReLU slopes applies those instead
     auto conv = [&](int ci, const float* in, int in_cs, int in_off, float* out, int out_cs, int out_off, int hh, int ww,
-                    int relu, float* nchw) -> int {
-        const ConvSpec s = net_conv(net, ci);
+                    float* nchw) -> int {
+        const ConvSpec s = arch.convs[ci].s;
         ConvF32Args a;
         a.in = in; a.in_cstride = in_cs; a.in_ch_off = in_off; a.w = net->d_w[ci].p; a.bias = net->d_b[ci].p;
         a.out = out; a.out_cstride = out_cs; a.out_ch_off = out_off; a.out_nchw = nchw;
-        a.n_img = n; a.H = hh; a.W = ww; a.cin = s.cin; a.cout = s.cout; a.ks = s.ks; a.relu = relu;
+        a.n_img = n; a.H = hh; a.W = ww; a.cin = s.cin; a.cout = s.cout; a.ks = s.ks; a.relu = arch.convs[ci].act == kRelu;
         a.slope = net->d_slope[ci].p;
         a.ext = ext;
         a.ext_shift = 0;
@@ -919,7 +945,7 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
         // OpenPose_Model: the features go to cat[features, paf] at channel 0, and through f_z (NCHW) into
         // cat[features, heat, paf]
         const int cat_cs = op ? kFeat + kPaf : kCat, cat_off = op ? 0 : kPaf + kHeat;
-        if (conv(i, cur, cur_c, 0, dst, last ? cat_cs : s.cout, last ? cat_off : 0, ch, cw, 1, last && op ? net->f_z.p : nullptr))
+        if (conv(i, cur, cur_c, 0, dst, last ? cat_cs : s.cout, last ? cat_off : 0, ch, cw, last && op ? net->f_z.p : nullptr))
             return 1;
         cur = dst; cur_c = s.cout;
         std::swap(ping, pong);
@@ -937,9 +963,10 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
         constexpr int kCat2 = kFeat + kPaf, kCat3 = kFeat + kHeat + kPaf;
         CU(nchw_to_nhwc_f32_launch(net->f_z.p, net->f_cat3.p, n, kFeat, h, w, kCat3, 0, st));
         ++g_launches;
-        for (int t = 0; t < net->l2 + net->l1; ++t) {
-            const OpStage g = op_stage(net->l2, t);
-            const int ci0 = 12 + kOpStageConvs * t, cs = 3 * g.inner;
+        for (int t = 0; t < arch.stages; ++t) {
+            const OpStage g = op_stage(arch.l2, t);
+            const std::vector<int> ci = stage_convs(arch, t + 1, 0);
+            const int cs = 3 * g.inner;
             float* blk[2] = {net->f_x.p, net->f_y.p};
             for (int li = 0; li < 15; ++li) {
                 const int b = li / 3, j = li % 3;
@@ -947,23 +974,23 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
                 int rc;
                 if (li == 0) {
                     const bool three = !g.paf && !g.first;
-                    rc = conv(ci0, three ? net->f_cat3.p : net->f_cat.p, three ? kCat3 : kCat2, 0, dst, cs, 0, h, w, 0, nullptr);
+                    rc = conv(ci[0], three ? net->f_cat3.p : net->f_cat.p, three ? kCat3 : kCat2, 0, dst, cs, 0, h, w, nullptr);
                 } else if (j == 0) {
-                    rc = conv(ci0 + li, blk[(b + 1) % 2], cs, 0, dst, cs, 0, h, w, 0, nullptr);
+                    rc = conv(ci[li], blk[(b + 1) % 2], cs, 0, dst, cs, 0, h, w, nullptr);
                 } else {
-                    rc = conv(ci0 + li, dst, cs, (j - 1) * g.inner, dst, cs, j * g.inner, h, w, 0, nullptr);
+                    rc = conv(ci[li], dst, cs, (j - 1) * g.inner, dst, cs, j * g.inner, h, w, nullptr);
                 }
                 if (rc) return 1;
             }
-            if (conv(ci0 + 15, net->f_x.p, cs, 0, net->f_z.p, g.innerout, 0, h, w, 0, nullptr)) return 1;
-            if (conv(ci0 + 16, net->f_z.p, g.innerout, 0, net->f_y.p, g.out, 0, h, w, 0, net->out_f32[t].p)) return 1;
+            if (conv(ci[15], net->f_x.p, cs, 0, net->f_z.p, g.innerout, 0, h, w, nullptr)) return 1;
+            if (conv(ci[16], net->f_z.p, g.innerout, 0, net->f_y.p, g.out, 0, h, w, net->out_f32[t].p)) return 1;
             // the next stages' inputs: an L2 head's PAF into cat[features, paf] (and the last one into
             // cat[features, heat, paf]), an L1 head's heat map into cat[features, heat, paf]
             if (g.paf) {
                 CU(nchw_to_nhwc_f32_launch(net->out_f32[t].p, net->f_cat.p, n, kPaf, h, w, kCat2, kFeat, st));
                 ++g_launches;
             }
-            if (t == net->l2 - 1 || !g.paf) {
+            if (t == arch.l2 - 1 || !g.paf) {
                 CU(nchw_to_nhwc_f32_launch(net->out_f32[t].p, net->f_cat3.p, n, g.out, h, w, kCat3,
                                            g.paf ? kFeat + kHeat : kFeat, st));
                 ++g_launches;
@@ -973,18 +1000,19 @@ int forward_fp32(b200pose_net* net, const float* d_in, int n, int H, int W, int 
     }
     for (int s = 1; s <= stages; ++s)
         for (int b = 0; b < 2; ++b) {
-            const int nl = stage_num_layers(s);
+            const std::vector<int> ci = stage_convs(arch, s, b);
+            const int nl = (int)ci.size();
             const float* in = net->f_cat.p;
             int in_cs = kCat, in_off = (s == 1) ? kPaf + kHeat : 0;
             float* bufs[2] = {net->f_x.p, net->f_y.p};
             for (int li = 0; li < nl; ++li) {
-                const ConvSpec sp = stage_layer(s, b, li);
+                const ConvSpec sp = arch.convs[ci[li]].s;
                 const bool lastl = (li == nl - 1);
                 float* nchw = lastl ? net->out_f32[2 * (s - 1) + b].p : nullptr;
                 // last layer output goes to a scratch slice; the concat for the next stage is written after both
                 // branches are done (the other branch still reads f_cat)
                 float* dst = bufs[li & 1];
-                if (conv(conv_index(s, b, li), in, in_cs, in_off, dst, sp.cout, 0, h, w, lastl ? 0 : 1, nchw)) return 1;
+                if (conv(ci[li], in, in_cs, in_off, dst, sp.cout, 0, h, w, nchw)) return 1;
                 in = dst; in_cs = sp.cout; in_off = 0;
             }
             if (b == 1 && s < stages) {
@@ -1005,23 +1033,19 @@ int b200pose_version(void) { return 100; }
 long b200pose_launch_count(void) { return g_launches.load(); }
 
 int b200pose_net_tensor_shape(int index, long dims[4]) {
-    if (index < 0 || index >= B200POSE_NUM_TENSORS) return -1;
-    const ConvSpec s = conv_spec(index / 2);
-    if (index % 2 == 0) { dims[0] = s.cout; dims[1] = s.cin; dims[2] = s.ks; dims[3] = s.ks; return 4; }
-    dims[0] = s.cout;
-    return 1;
+    static const NetArch rtpose = rtpose_arch();
+    return arch_tensor_shape(rtpose, index, dims);
 }
 
 int b200pose_openpose_num_tensors(int l2_stages, int l1_stages) {
-    return op_valid(l2_stages, l1_stages) ? op_num_tensors(l2_stages, l1_stages) : -1;
+    return op_valid(l2_stages, l1_stages) ? arch_num_tensors(openpose_arch(l2_stages, l1_stages)) : -1;
 }
 
 int b200pose_openpose_tensor_shape(int l2_stages, int l1_stages, int index, long dims[4]) {
-    return op_tensor_shape(l2_stages, l1_stages, index, dims);
+    return op_valid(l2_stages, l1_stages) ? arch_tensor_shape(openpose_arch(l2_stages, l1_stages), index, dims) : -1;
 }
 
-// A net of architecture OpenPose_Model(l2, l1), or rtpose when l2 == 0.
-static int net_create(b200pose_net** out, int cuda_device, int l2, int l1) {
+static int net_create(b200pose_net** out, int cuda_device, NetArch arch) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return cuda_fail("b200pose: no CUDA device available (this library has no CPU fallback)");
@@ -1033,30 +1057,29 @@ static int net_create(b200pose_net** out, int cuda_device, int l2, int l1) {
     b200pose_net* net = new b200pose_net();
     net->device = cuda_device;
     net->num_sms = prop.multiProcessorCount;
-    net->l2 = l2;
-    net->l1 = l1;
-    if (l2 > 0) net->stages = l2 + l1;     // the plan and graph keys' stage count: all of them, always
-    const int nc = net_num_convs(net);
+    net->arch = std::move(arch);
+    net->stages = net->arch.stages;
+    const int nc = (int)net->arch.convs.size();
     net->host_w.resize(nc);
     net->host_b.resize(nc);
     net->host_slope.resize(nc);
     net->d_w.resize(nc);
     net->d_b.resize(nc);
     net->d_slope.resize(nc);
-    net->have.assign(net_num_tensors(net), false);
+    net->have.assign(arch_num_tensors(net->arch), false);
     const char* gr = getenv("B200POSE_GRAPH");
     net->use_graph = !(gr && gr[0] == '0');
     *out = net;
     return 0;
 }
 
-int b200pose_net_create(b200pose_net** out, int cuda_device) { return net_create(out, cuda_device, 0, 0); }
+int b200pose_net_create(b200pose_net** out, int cuda_device) { return net_create(out, cuda_device, rtpose_arch()); }
 
 int b200pose_net_create_openpose(b200pose_net** out, int cuda_device, int l2_stages, int l1_stages) {
     if (!op_valid(l2_stages, l1_stages))
         return fail("OpenPose_Model(%d, %d): stages must be l2 >= 1, l1 >= 1, l2 + l1 <= %d", l2_stages, l1_stages,
                     kOpMaxStages);
-    return net_create(out, cuda_device, l2_stages, l1_stages);
+    return net_create(out, cuda_device, openpose_arch(l2_stages, l1_stages));
 }
 
 void b200pose_net_destroy(b200pose_net* net) {
@@ -1068,15 +1091,14 @@ void b200pose_net_destroy(b200pose_net* net) {
 int b200pose_net_set_tensor(b200pose_net* net, int index, const float* host_data, long count) {
     if (!net || !host_data) return fail("set_tensor: null pointer");
     long dims[4];
-    const bool op = is_openpose(net);
-    const int nd = op ? op_tensor_shape(net->l2, net->l1, index, dims) : b200pose_net_tensor_shape(index, dims);
-    const std::string who = op ? arch_name(net) + ": " : "";
+    const int nd = arch_tensor_shape(net->arch, index, dims);
+    const std::string who = is_openpose(net) ? net->arch.name + ": " : "";
     if (nd < 0) return fail("%stensor index %d out of range", who.c_str(), index);
     long expect = 1;
     for (int i = 0; i < nd; ++i) expect *= dims[i];
     if (count != expect) return fail("%stensor %d: got %ld elements, expected %ld", who.c_str(), index, count, expect);
-    int ci = index / 2, kind = index % 2;
-    if (op) op_tensor(net->l2, net->l1, index, &ci, &kind);
+    int ci, kind;
+    arch_tensor(net->arch, index, &ci, &kind);
     std::vector<float>& dst = kind == 0 ? net->host_w[ci] : (kind == 1 ? net->host_b[ci] : net->host_slope[ci]);
     dst.assign(host_data, host_data + count);
     net->have[index] = true;
@@ -1087,9 +1109,9 @@ int b200pose_net_set_tensor(b200pose_net* net, int index, const float* host_data
 int b200pose_net_finalize(b200pose_net* net) {
     if (!net) return fail("null net");
     CU(cudaSetDevice(net->device));
-    for (int i = 0; i < net_num_tensors(net); ++i)
+    for (int i = 0; i < (int)net->have.size(); ++i)
         if (!net->have[i]) return fail("state_dict tensor %d was never set", i);
-    for (int i = 0; i < net_num_convs(net); ++i) {
+    for (size_t i = 0; i < net->arch.convs.size(); ++i) {
         // freed first, not reused: cudaFree synchronises the device, so a forward in flight on another stream has
         // stopped reading the weights before the synchronous copies below overwrite them
         net->d_w[i].release();
@@ -1104,38 +1126,7 @@ int b200pose_net_finalize(b200pose_net* net) {
             CU(cudaMemcpy(net->d_slope[i].p, net->host_slope[i].data(), net->host_slope[i].size() * 4, cudaMemcpyHostToDevice));
     }
     net->tc.clear();
-    if (is_openpose(net)) {
-        for (int i = 1; i < 12; ++i) {
-            const ConvSpec s = kTrunk[i];
-            const bool prelu = op_conv(net->l2, i).act == kPrelu;
-            net->tc.push_back(make_tc_layer(net, {i}, s.cout < 128 ? s.cout : 128, kPermNone, !prelu, kPoolAfter[i], prelu));
-        }
-        // n-tiles: 48 for the 96-channel convs (two tiles, no pad lanes), 128 for the others; the heads 64 (PAF: zero rows
-        // 38..63 store +0 over the heat slot) and 32 (heat map)
-        for (int t = 0; t < net->l2 + net->l1; ++t) {
-            const OpStage g = op_stage(net->l2, t);
-            for (int li = 0; li < kOpStageConvs; ++li) {
-                const int ci = 12 + kOpStageConvs * t + li;
-                const int n_tile = li == 16 ? (g.paf ? 64 : 32) : (li < 15 && g.inner == 96 ? 48 : 128);
-                InPerm perm = kPermNone;
-                if (li == 0 && t > 0) perm = g.paf || g.first ? kPermFeatPaf : kPermFeatHeatPaf;
-                else if (li == 15 || (li > 0 && li % 3 == 0)) perm = kPermSlots;
-                net->tc.push_back(make_tc_layer(net, {ci}, n_tile, perm, 0, 0, op_conv(net->l2, ci).act == kPrelu));
-            }
-        }
-    } else {
-        for (int i = 1; i < 12; ++i) {
-            const ConvSpec s = kTrunk[i];
-            net->tc.push_back(make_tc_layer(net, {i}, s.cout < 128 ? s.cout : 128, kPermNone, 1, kPoolAfter[i]));
-        }
-        for (int li = 0; li < 5; ++li)
-            net->tc.push_back(make_tc_layer(net, {conv_index(1, 0, li), conv_index(1, 1, li)}, li == 4 ? 48 : 128, kPermNone,
-                                            li != 4, 0));
-        for (int st = 2; st <= 6; ++st)
-            for (int li = 0; li < 7; ++li)
-                net->tc.push_back(make_tc_layer(net, {conv_index(st, 0, li), conv_index(st, 1, li)}, li == 6 ? 48 : 128,
-                                                li == 0 ? kPermRtposeCat : kPermNone, li != 6, 0));
-    }
+    for (const ArchLayer& l : net->arch.layers) net->tc.push_back(make_tc_layer(net->arch, l));
     for (TcLayer& L : net->tc)
         if (ensure_packed(net, L, TcFormat::kBf16)) return 1;
     net->last = LastForward();
@@ -1149,10 +1140,10 @@ int b200pose_net_finalize(b200pose_net* net) {
 // Entries of outputs[12] for stages the net does not run must be NULL: a caller must not read a map no stage wrote as if
 // it were fresh.
 static int check_outputs(const b200pose_net* net, float* const* outputs) {
-    for (int i = net_num_maps(net, net->stages); outputs && i < 12; ++i)
+    for (int i = net->arch.out[net->stages].maps; outputs && i < 12; ++i)
         if (outputs[i]) {
             if (is_openpose(net))
-                return fail("outputs[%d] must be NULL: %s writes %d maps", i, arch_name(net).c_str(), net->l2 + net->l1);
+                return fail("outputs[%d] must be NULL: %s writes %d maps", i, net->arch.name.c_str(), net->arch.out[net->stages].maps);
             return fail("outputs[%d] must be NULL: the net runs %d stage(s), stage %d does not run", i, net->stages, i / 2 + 1);
         }
     return 0;
@@ -1162,7 +1153,7 @@ static int check_outputs(const b200pose_net* net, float* const* outputs) {
 // rtpose's launch list) are refused before anything is enqueued.
 static int check_mode(const b200pose_net* net, int mode) {
     if (is_openpose(net) && (mode == B200POSE_MODE_FP8 || mode == B200POSE_MODE_FP16))
-        return fail("%s runs modes bf16, bf16x3 and fp32, not %s", arch_name(net).c_str(),
+        return fail("%s runs modes bf16, bf16x3 and fp32, not %s", net->arch.name.c_str(),
                     mode == B200POSE_MODE_FP8 ? "fp8" : "fp16");
     return 0;
 }
@@ -1210,9 +1201,9 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
     net->last = LastForward{n, H, W, mode == B200POSE_MODE_FP32, fmt, stages, d_in, first_u8, ext};
     if (outputs) {
         const size_t px8 = (size_t)n * (H / 8) * (W / 8);
-        for (int i = 0; i < net_num_maps(net, stages); ++i)
+        for (int i = 0; i < net->arch.out[stages].maps; ++i)
             if (outputs[i])
-                CU(cudaMemcpyAsync(outputs[i], net->out_f32[i].p, px8 * map_ch(net, i) * 4,
+                CU(cudaMemcpyAsync(outputs[i], net->out_f32[i].p, px8 * net->arch.map_ch[i] * 4,
                                    outputs_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
     }
     if (sync_host && (!input_on_device || (outputs && !outputs_on_device))) CU(cudaStreamSynchronize(st));
@@ -1339,7 +1330,7 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess) {
 int b200pose_net_set_stages(b200pose_net* net, int stages) {
     if (!net) return fail("null net");
     if (is_openpose(net))
-        return fail("%s: the stage count is the architecture's (set at b200pose_net_create_openpose)", arch_name(net).c_str());
+        return fail("%s: the stage count is the architecture's (set at b200pose_net_create_openpose)", net->arch.name.c_str());
     if (stages < 1 || stages > kStages) return fail("stages must be 1 .. %d, got %d", kStages, stages);
     net->stages = stages;
     return 0;
@@ -1414,7 +1405,7 @@ int b200pose_net_debug_launch(b200pose_net* net, int i, int* fields, int cap) {
     } else {
         const PlanLaunch& l = p.launches[i - 1];
         const ConvTcArgs& a = l.a;
-        f[0] = l.in; f[1] = act_c(net, l.in); f[2] = a.in_ch_base; f[3] = a.in_ch_group_stride;
+        f[0] = l.in; f[1] = net->arch.act_c[l.in]; f[2] = a.in_ch_base; f[3] = a.in_ch_group_stride;
         f[4] = l.out; f[5] = a.out_cstride; f[6] = a.out_ch_off[0]; f[7] = a.out_ch_off[1];
         f[8] = a.store_ch[0]; f[9] = a.store_ch[1];
         f[10] = a.H; f[11] = a.W; f[12] = a.ksize; f[13] = a.cin_blocks; f[14] = a.groups; f[15] = a.n_tile;
@@ -1435,13 +1426,13 @@ int b200pose_net_debug_read(b200pose_net* net, int buf, int lo_plane, int img0, 
     size_t per = 0;
     if (buf >= 0 && buf < kNumAct) {
         if (lo_plane && tc_planes(net->plan->fmt) < 2) return fail("debug_read: residual planes exist in bf16x3 mode only");
-        per = (size_t)(H / kActDiv[buf]) * (W / kActDiv[buf]) * act_c(net, buf) * 2;
+        per = (size_t)(H / kActDiv[buf]) * (W / kActDiv[buf]) * net->arch.act_c[buf] * 2;
         src = reinterpret_cast<const char*>((lo_plane ? net->act_lo : net->act)[buf].p);
     } else if (buf >= kNumAct && buf < kNumAct + 12 && !lo_plane) {
         const int m = buf - kNumAct;
-        if (m >= net_num_maps(net, net->last.stages))
+        if (m >= net->arch.out[net->last.stages].maps)
             return fail("debug_read: stage map %d was not written by the last forward (%d stages)", m, net->last.stages);
-        per =(size_t)(H / 8) * (W / 8) * map_ch(net, m) * 4;
+        per =(size_t)(H / 8) * (W / 8) * net->arch.map_ch[m] * 4;
         src = reinterpret_cast<const char*>(net->out_f32[m].p);
     } else {
         return fail("debug_read: no buffer %d (plane %d)", buf, lo_plane);
