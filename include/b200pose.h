@@ -417,6 +417,26 @@ int b200pose_net_encode_jpegs(b200pose_net* net, const unsigned char* frames, in
                               long long* sizes, void* cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3h. PNG encoding: replaces cv2.imencode('.png', frame) and cv2.imwrite of a .png name   (DESIGN.md 2.15)
+ *     Byte for byte what cv2 (OpenCV 4.13 with libpng 1.6 and zlib 1.3) writes at its defaults: 8-bit RGB, no
+ *     interlace, every row Sub-filtered, zlib level 1 with strategy Z_RLE, IDAT chunks of 8 192 bytes, no ancillary
+ *     chunks (csrc/png_enc_core.h).  The call takes no encoder parameters.
+ *
+ *     b200pose_png_encode_bound: host only.  The file bytes that always suffice for an h x w frame (every deflate
+ *     block stored, plus the framing); -1 for a size outside 1 .. 65535.
+ *     b200pose_net_encode_pngs: n (1 .. 1024) uint8 HWC BGR frames packed back to back (frame i: frame_hw[2i] x
+ *     frame_hw[2i+1] x 3 bytes, the layout b200pose_post_draw draws on; host, or device when frames_on_device) -> their
+ *     PNG files packed back to back in `out` (host, or device when out_on_device; out_cap bytes), sizes[i] (host) the
+ *     length of file i.  Synchronises the stream (once inside the call, to size the deflate words and the output from
+ *     what the kernels computed, and at its end).  n, a size outside 1 .. 65535 and an out_cap below the sum of the
+ *     images' bounds are refused, naming the field, before anything is enqueued.  One call launches 9 kernels.
+ * ---------------------------------------------------------------------------------------------------------- */
+long long b200pose_png_encode_bound(int h, int w);
+int b200pose_net_encode_pngs(b200pose_net* net, const unsigned char* frames, int frames_on_device, const int* frame_hw,
+                             int n, unsigned char* out, long long out_cap, int out_on_device, long long* sizes,
+                             void* cuda_stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

@@ -83,6 +83,8 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_post_jpeg_status": ([vp, ci], ci),
     "b200pose_jpeg_encode_bound": ([ci, ci, ci], ctypes.c_longlong),
     "b200pose_net_encode_jpegs": ([vp, vp, ci, vp, ci, ci, ci, vp, ctypes.c_longlong, ci, vp, vp], ci),
+    "b200pose_png_encode_bound": ([ci, ci], ctypes.c_longlong),
+    "b200pose_net_encode_pngs": ([vp, vp, ci, vp, ci, vp, ctypes.c_longlong, ci, vp, vp], ci),
     "process_paf": ([ci, ci, ci, vp, ci, ci, ci, vp, ci, ci, ci, vp], ci),
     "get_num_humans": ([], ci),
     "get_part_cid": ([ci, ci], ci),

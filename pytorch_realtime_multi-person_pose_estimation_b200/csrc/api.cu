@@ -25,6 +25,7 @@
 #include "frames.cuh"
 #include "jpeg.cuh"
 #include "jpeg_enc.cuh"
+#include "png_enc.cuh"
 #include "fp8_core.h"
 #include "postprocess.cuh"
 #include "resize.cuh"
@@ -467,6 +468,15 @@ struct b200pose_net {
     DevBuf<int> jenc_acbits;
     DevBuf<long long> jenc_off;
     DevBuf<unsigned> jenc_words;
+    // PNG encoding (b200pose_net_encode_pngs): the call's upload (descriptors, per-image results, deflate word offsets),
+    // staged host frames, the filtered bytes, the tile table, the symbols, the blocks, the deflate words, and the files
+    // of a call whose output is on the host
+    DevBuf<char> penc_in;
+    DevBuf<unsigned char> penc_frames, penc_filt, penc_out;
+    DevBuf<long long> penc_tiles;
+    DevBuf<unsigned short> penc_sym;
+    DevBuf<PngBlock> penc_blocks;
+    DevBuf<unsigned> penc_words;
     // fp8 mode (DESIGN.md §2.3): amax[launch * n + image] = max |bf16| (fp32 bits) launch (0 = conv1_1) stored for the
     // image; zeroed at the start of every fp8 forward
     DevBuf<unsigned> amax;
@@ -2600,6 +2610,107 @@ int b200pose_net_encode_jpegs(b200pose_net* net, const unsigned char* frames, in
     if (!out_on_device) CU(cudaMemcpyAsync(out, net->jenc_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     memcpy(sizes, got.data(), n * sizeof(long long));
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ PNG encoding
+long long b200pose_png_encode_bound(int h, int w) {
+    if (!jenc_size_ok(h, w)) return fail("png_encode_bound: size %d x %d (1 .. 65535 each)", h, w), -1;
+    return png_stream_bound(h, w);
+}
+
+int b200pose_net_encode_pngs(b200pose_net* net, const unsigned char* frames, int frames_on_device, const int* frame_hw,
+                             int n, unsigned char* out, long long out_cap, int out_on_device, long long* sizes,
+                             void* cuda_stream) {
+    if (!net) return fail("null net");
+    if (!frames || !frame_hw || !out || !sizes) return fail("encode_pngs: null pointer");
+    if (n < 1 || n > kMaxRagged) return fail("encode_pngs: n = %d images (1 .. %d)", n, kMaxRagged);
+    // descriptors, then the per-image results (zeroed) and room for the deflate word offsets
+    std::vector<PngImage> ims(n);
+    long long src = 0, filt = 0, tiles = 0, blocks = 0, bound = 0, max_tiles = 0, max_blocks = 0;
+    for (int i = 0; i < n; ++i) {
+        const int h = frame_hw[2 * i], w = frame_hw[2 * i + 1];
+        if (!jenc_size_ok(h, w)) return fail("encode_pngs: image %d size %d x %d (1 .. 65535 each)", i, h, w);
+        PngImage& im = ims[i];
+        im.h = h;
+        im.w = w;
+        im.n = (long long)h * (3LL * w + 1);
+        im.src = src;
+        im.f0 = filt;
+        im.tile0 = tiles;
+        im.blk0 = blocks;
+        im.tiles = (int)((im.n + kPngTile - 1) / kPngTile);
+        im.max_blocks = (int)png_blocks(im.n);
+        png_zlib_header(im.n, im.zhdr);
+        src += 3LL * h * w;
+        filt += (im.n + 15) & ~15LL;
+        tiles += im.tiles;
+        blocks += im.max_blocks;
+        bound += png_stream_bound(h, w);
+        max_tiles = std::max(max_tiles, (long long)im.tiles);
+        max_blocks = std::max(max_blocks, (long long)im.max_blocks);
+    }
+    if (out_cap < bound)
+        return fail("encode_pngs: out_cap %lld bytes, below %lld (b200pose_png_encode_bound summed over the images)",
+                    out_cap, bound);
+    const size_t o_outs = n * sizeof(PngImage), o_wbase = o_outs + n * sizeof(PngImageOut);
+    std::vector<char> up(o_wbase + n * sizeof(long long), 0);
+    memcpy(up.data(), ims.data(), o_outs);
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    CU(net->penc_in.ensure(up.size()));
+    CU(net->penc_filt.ensure((size_t)filt));
+    CU(net->penc_sym.ensure((size_t)filt));
+    CU(net->penc_tiles.ensure((size_t)tiles * 6));
+    CU(net->penc_blocks.ensure((size_t)blocks));
+    if (!frames_on_device) CU(net->penc_frames.ensure((size_t)src));
+    CU(cudaMemcpyAsync(net->penc_in.p, up.data(), up.size(), cudaMemcpyHostToDevice, st));
+    if (!frames_on_device) CU(cudaMemcpyAsync(net->penc_frames.p, frames, (size_t)src, cudaMemcpyHostToDevice, st));
+    char* d = net->penc_in.p;
+    long long* t = net->penc_tiles.p;
+    PngBatch b;
+    b.ims = reinterpret_cast<const PngImage*>(d);
+    b.n = n;
+    b.frames = frames_on_device ? frames : net->penc_frames.p;
+    b.filt = net->penc_filt.p;
+    b.tfirst = t;
+    b.tlast = t + tiles;
+    b.tstart = t + 2 * tiles;
+    b.tend = t + 3 * tiles;
+    b.tcount = t + 4 * tiles;
+    b.tbase = t + 5 * tiles;
+    b.sym = net->penc_sym.p;
+    b.blocks = net->penc_blocks.p;
+    b.outs = reinterpret_cast<PngImageOut*>(d + o_outs);
+    b.wbase = reinterpret_cast<const long long*>(d + o_wbase);
+    b.words = nullptr;
+    b.out = nullptr;
+    b.max_tiles = max_tiles;
+    b.max_blocks = max_blocks;
+    b.max_chunks = 0;
+    // phase 0, then the deflate words and the output sized from what it found
+    if (int rc = launched(png_encode_launch(b, 0, st), "png_encode_launch", 7)) return rc;
+    std::vector<PngImageOut> got(n);
+    CU(cudaMemcpyAsync(got.data(), b.outs, n * sizeof(PngImageOut), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    std::vector<long long> wbase(n);
+    long long words = 0, total = 0;
+    for (int i = 0; i < n; ++i) {
+        wbase[i] = words;
+        words += got[i].bits / 32 + 2;
+        total += got[i].size;
+        b.max_chunks = std::max(b.max_chunks, (long long)got[i].chunks);
+    }
+    CU(net->penc_words.ensure((size_t)words));
+    b.words = net->penc_words.p;
+    CU(cudaMemsetAsync(b.words, 0, (size_t)words * sizeof(unsigned), st));
+    CU(cudaMemcpyAsync(d + o_wbase, wbase.data(), n * sizeof(long long), cudaMemcpyHostToDevice, st));
+    if (!out_on_device) CU(net->penc_out.ensure((size_t)total));
+    b.out = out_on_device ? out : net->penc_out.p;
+    if (int rc = launched(png_encode_launch(b, 1, st), "png_encode_launch", 2)) return rc;
+    if (!out_on_device) CU(cudaMemcpyAsync(out, net->penc_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (int i = 0; i < n; ++i) sizes[i] = got[i].size;
     return 0;
 }
 

@@ -325,14 +325,10 @@ class NativeNet:
             at += h * w * 3
         return out
 
-    def encode_jpegs(self, frames, quality=95, sampling="420", device=False, stream=0):
-        """cv2.imencode('.jpg', frame, [IMWRITE_JPEG_QUALITY, quality, IMWRITE_JPEG_SAMPLING_FACTOR, s])[1] of every
-        frame, on the device (b200pose_net_encode_jpegs); sampling one of '420', '422', '440', '411', '444'.  frames: a
-        list of uint8 HWC BGR numpy arrays (staged through the device), a CUDA uint8 tensor [n, h, w, 3], or a list of
-        CUDA uint8 tensors [h, w, 3] of any sizes.  Returns a list of bytes, or with device=True of 1-D CUDA uint8
-        tensors (views of one buffer, written on the current stream)."""
-        if sampling not in nat.JPEG_SAMPLING:
-            raise nat.B200PoseError("encode_jpegs: unknown sampling %r (one of %s)" % (sampling, sorted(nat.JPEG_SAMPLING)))
+    def _frames_to_encode(self, frames, what):
+        """The frames of an encode call as (frame pointer, on device, [(h, w)], buffer that keeps the pointer valid):
+        a list of uint8 HWC BGR numpy arrays (packed on the host), a CUDA uint8 tensor [n, h, w, 3], or a list of CUDA
+        uint8 tensors [h, w, 3] on the net's device (packed unless they are consecutive views of one buffer)."""
         try:
             import torch
         except ImportError:
@@ -342,19 +338,19 @@ class NativeNet:
             tensors = [frames] if isinstance(frames, torch.Tensor) else list(frames)
             for f in tensors:
                 if not isinstance(f, torch.Tensor) or not f.is_cuda:
-                    raise nat.B200PoseError("encode_jpegs: frames are all numpy arrays or all CUDA tensors")
+                    raise nat.B200PoseError("%s: frames are all numpy arrays or all CUDA tensors" % what)
                 if f.device.index != self.device_index:
-                    raise nat.B200PoseError("encode_jpegs: a frame tensor is on %s, the net on cuda:%d"
-                                            % (f.device, self.device_index))
+                    raise nat.B200PoseError("%s: a frame tensor is on %s, the net on cuda:%d"
+                                            % (what, f.device, self.device_index))
             if isinstance(frames, torch.Tensor):
                 if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
-                    raise nat.B200PoseError("encode_jpegs: expected a CUDA uint8 tensor [n, h, w, 3]")
+                    raise nat.B200PoseError("%s: expected a CUDA uint8 tensor [n, h, w, 3]" % what)
                 sizes = [tuple(frames.shape[1:3])] * frames.shape[0]
                 flat = frames.contiguous()
             else:
                 for f in frames:
                     if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
-                        raise nat.B200PoseError("encode_jpegs: expected a list of CUDA uint8 tensors [h, w, 3]")
+                        raise nat.B200PoseError("%s: expected a list of CUDA uint8 tensors [h, w, 3]" % what)
                 sizes = [tuple(f.shape[:2]) for f in frames]
                 flat = _packed_views(frames)
             src = flat.data_ptr() if flat is not None else 0
@@ -362,30 +358,37 @@ class NativeNet:
             arrs = [np.ascontiguousarray(f) for f in frames]
             for a in arrs:
                 if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
-                    raise nat.B200PoseError("encode_jpegs: expected uint8 HWC BGR frames")
+                    raise nat.B200PoseError("%s: expected uint8 HWC BGR frames" % what)
             sizes = [a.shape[:2] for a in arrs]
             flat = np.concatenate([a.reshape(-1) for a in arrs]) if arrs else None
             src = flat.ctypes.data if flat is not None else 0
+        return src, dev_in, sizes, flat
+
+    def _encode(self, frames, what, bound, call, device, stream):
+        """The streams of an encode call `what` (the entry point's name without b200pose_net_): bound(h, w) gives
+        each frame's capacity, call(src, on_device, hw, n, out, cap, out_on_device, lens, stream) runs the entry point.  A list of bytes, or with device=True of 1-D CUDA uint8
+        tensors (views of one buffer, written on the current stream)."""
+        src, dev_in, sizes, flat = self._frames_to_encode(frames, what)
         n = len(sizes)
         if n == 0:
             return []
-        code = nat.JPEG_SAMPLING[sampling]
         cap = 0
         for h, w in sizes:
-            b = int(nat.lib().b200pose_jpeg_encode_bound(int(h), int(w), code))
+            b = int(bound(int(h), int(w)))
             if b < 0:
-                nat.check(1, "b200pose_jpeg_encode_bound")
+                nat.check(1, "b200pose_%s_encode_bound" % what[len("encode_"):-1])
             cap += b
         if dev_in or device:
+            import torch
             stream = torch.cuda.current_stream(torch.device("cuda", self.device_index)).cuda_stream
-        out = (torch.empty(cap, dtype=torch.uint8, device="cuda:%d" % self.device_index) if device
-               else np.empty(cap, np.uint8))
+            out = (torch.empty(cap, dtype=torch.uint8, device="cuda:%d" % self.device_index) if device
+                   else np.empty(cap, np.uint8))
+        else:
+            out = np.empty(cap, np.uint8)
         hw = (ctypes.c_int * (2 * n))(*[int(v) for s in sizes for v in s])
         lens = (ctypes.c_longlong * n)()
-        nat.check(nat.lib().b200pose_net_encode_jpegs(self._h, ctypes.c_void_p(src), int(dev_in), hw, n, int(quality), code,
-                                                      ctypes.c_void_p(out.data_ptr() if device else out.ctypes.data), cap,
-                                                      int(device), lens, ctypes.c_void_p(stream)),
-                  "b200pose_net_encode_jpegs")
+        nat.check(call(ctypes.c_void_p(src), int(dev_in), hw, n, ctypes.c_void_p(out.data_ptr() if device else out.ctypes.data),
+                       cap, int(device), lens, ctypes.c_void_p(stream)), "b200pose_net_" + what)
         total = sum(lens)
         if device:      # the bound-sized buffer goes back to the allocator; the views keep only the streams
             out = out[:total].clone()
@@ -394,6 +397,31 @@ class NativeNet:
             res.append(out[at:at + k] if device else out[at:at + k].tobytes())
             at += k
         return res
+
+    def encode_jpegs(self, frames, quality=95, sampling="420", device=False, stream=0):
+        """cv2.imencode('.jpg', frame, [IMWRITE_JPEG_QUALITY, quality, IMWRITE_JPEG_SAMPLING_FACTOR, s])[1] of every
+        frame, on the device (b200pose_net_encode_jpegs); sampling one of '420', '422', '440', '411', '444'.  frames: a
+        list of uint8 HWC BGR numpy arrays (staged through the device), a CUDA uint8 tensor [n, h, w, 3], or a list of
+        CUDA uint8 tensors [h, w, 3] of any sizes.  Returns a list of bytes, or with device=True of 1-D CUDA uint8
+        tensors (views of one buffer, written on the current stream)."""
+        if sampling not in nat.JPEG_SAMPLING:
+            raise nat.B200PoseError("encode_jpegs: unknown sampling %r (one of %s)" % (sampling, sorted(nat.JPEG_SAMPLING)))
+        code, L = nat.JPEG_SAMPLING[sampling], nat.lib()
+        return self._encode(frames, "encode_jpegs", lambda h, w: L.b200pose_jpeg_encode_bound(h, w, code),
+                            lambda src, dev_in, hw, n, out, cap, dev_out, lens, st: L.b200pose_net_encode_jpegs(
+                                self._h, src, dev_in, hw, n, int(quality), code, out, cap, dev_out, lens, st),
+                            device, stream)
+
+    def encode_pngs(self, frames, device=False, stream=0):
+        """cv2.imencode('.png', frame)[1] of every frame, on the device (b200pose_net_encode_pngs).  frames: a list of
+        uint8 HWC BGR numpy arrays (staged through the device), a CUDA uint8 tensor [n, h, w, 3], or a list of CUDA
+        uint8 tensors [h, w, 3] of any sizes.  Returns a list of bytes, or with device=True of 1-D CUDA uint8 tensors
+        (views of one buffer, written on the current stream)."""
+        L = nat.lib()
+        return self._encode(frames, "encode_pngs", L.b200pose_png_encode_bound,
+                            lambda src, dev_in, hw, n, out, cap, dev_out, lens, st: L.b200pose_net_encode_pngs(
+                                self._h, src, dev_in, hw, n, out, cap, dev_out, lens, st),
+                            device, stream)
 
     def __del__(self):
         try:
@@ -939,6 +967,10 @@ class PoseEngine:
     def encode_jpegs(self, frames, quality=95, sampling="420", device=False, stream=0):
         """NativeNet.encode_jpegs on this engine's device: cv2.imencode('.jpg', ...) of every frame, on the GPU."""
         return self.net.encode_jpegs(frames, quality, sampling, device, stream)
+
+    def encode_pngs(self, frames, device=False, stream=0):
+        """NativeNet.encode_pngs on this engine's device: cv2.imencode('.png', frame) of every frame, on the GPU."""
+        return self.net.encode_pngs(frames, device, stream)
 
     def draw_humans(self, frames, ticket=None, dest_size=368, factor=8, net_sizes=None):
         """draw_humans(frame, humans_from_rows(rows, net_w, net_h)) for every frame of run `ticket` (default: the
