@@ -210,6 +210,18 @@ int b200pose_post_debug(b200pose_post* post, unsigned long long* out, int n, int
 /* Test hook: sorts n 64-bit candidate keys (high word = ~score bits, low word = pair index) on the device with the
  * product's sorting kernels - libstdc++'s std::sort order (pafprocess.cpp:97), ties included.  Host pointers. */
 int b200pose_post_debug_sort(b200pose_post* post, const unsigned long long* keys, int n, unsigned long long* out);
+/* Test hook: the grids of the two work-queue kernels of PAF scoring and sorting (limb_score_kernel, range_sort_kernel),
+ * for every run of this post object submitted after the call (b200pose_post_run, the fused b200pose_infer* entry points)
+ * and for b200pose_post_debug_sort.  Both kernels take their work from a global cursor, so their results do not depend
+ * on the grid; this lets a test check that.  0 restores a default (score: SMs x 6; sort: min(n x 19, SMs x 3), and
+ * SMs x 3 for debug_sort).  A value below 0 or above 65535 is refused with an error naming it, and the grids stay as
+ * they were. */
+int b200pose_post_set_grids(b200pose_post* post, int score_blocks, int sort_blocks);
+/* Test hook: the connections the greedy matcher (pafprocess.cpp:98-124) chose for limb `limb` of image `img` of the
+ * latest run, in the order it chose them: peak indices a (part limb[0]) and b (part limb[1]) within their parts, and
+ * the candidate score.  Waits for the run, copies at most cap entries to the host arrays and returns the count;
+ * -1 on error. */
+int b200pose_post_debug_connections(b200pose_post* post, int img, int limb, int* a, int* b, float* s, int cap);
 /* Test hook: waits for the device, then copies the first heat_floats / paf_floats floats of the maps the last flip or
  * multi-scale run averaged and post-processed (NCHW fp32; a ragged run's at its canvas pitch) to host memory. */
 int b200pose_post_debug_maps(b200pose_post* post, float* heat, long heat_floats, float* paf, long paf_floats);

@@ -50,6 +50,21 @@ class _PafProcess:
         return self._process(*peaks.shape, peaks.ctypes.data_as(_FP), *heat.shape, heat.ctypes.data_as(_FP),
                              *paf.shape, paf.ctypes.data_as(_FP))
 
+    def connections(self, limb):
+        """(a int32 [k], b int32 [k], score float32 [k]): the connections the last call chose for `limb`, in the order
+        of its greedy loop (pafprocess.cpp:98-124), a and b peak indices within the limb's two parts.  The port only."""
+        L = self._lib
+        L.port_get_connection.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_int),
+                                          ctypes.POINTER(ctypes.c_int), _FP]
+        L.port_get_connection.restype = None
+        k = L.port_get_num_connections(int(limb))
+        a, b, s = np.zeros(k, np.int32), np.zeros(k, np.int32), np.zeros(k, np.float32)
+        ia, ib, fs = ctypes.c_int(), ctypes.c_int(), ctypes.c_float()
+        for i in range(k):
+            L.port_get_connection(int(limb), i, ctypes.byref(ia), ctypes.byref(ib), ctypes.byref(fs))
+            a[i], b[i], s[i] = ia.value, ib.value, fs.value
+        return a, b, s
+
     def humans(self, num_parts=18):
         """[(score, {part: (x, y, peak_score, cid)})] in subset order."""
         out = []

@@ -39,6 +39,9 @@ static float* g_rows = NULL;  /* [n_rows][20] */
 static int g_nrows = 0;
 static Peak* g_line = NULL;
 static int g_nline = 0;
+/* the connections of the last port_process_paf call per limb, in the order the greedy loop chose them (getters only) */
+static Conn* g_conn[NUM_LIMB];
+static int g_nconn[NUM_LIMB];
 
 /* std::sort(candidates.begin(), candidates.end(), comp_candidate) (pafprocess.cpp:97, comp = a.score > b.score).
  * The order of candidates with EXACTLY equal score is whatever the standard library's algorithm leaves; such
@@ -287,7 +290,11 @@ int port_process_paf(int p1, int p2, int p3, const float* peaks, int h1, int h2,
         memcpy(g_rows + 20 * g_nrows++, rows + 20 * r, sizeof(float) * 20);
     }
     free(rows); free(alive);
-    for (int l = 0; l < NUM_LIMB; ++l) free(conns[l]);
+    for (int l = 0; l < NUM_LIMB; ++l) {         /* kept for the connection getters */
+        free(g_conn[l]);
+        g_conn[l] = conns[l];
+        g_nconn[l] = n_conn[l];
+    }
     for (int p = 0; p < NUM_PART; ++p) free(by_part[p]);
     return 0;
 }
@@ -298,3 +305,10 @@ float port_get_score(int human) { return g_rows[human * 20 + 18] / g_rows[human 
 int port_get_part_x(int cid) { return g_line[cid].x; }
 int port_get_part_y(int cid) { return g_line[cid].y; }
 float port_get_part_score(int cid) { return g_line[cid].score; }
+/* connection k of limb `limb` (pafprocess.cpp:113-119): peak indices within the limb's two parts and the score */
+int port_get_num_connections(int limb) { return g_nconn[limb]; }
+void port_get_connection(int limb, int k, int* a, int* b, float* score) {
+    *a = g_conn[limb][k].pid1;
+    *b = g_conn[limb][k].pid2;
+    *score = g_conn[limb][k].score;
+}

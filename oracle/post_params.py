@@ -12,6 +12,8 @@ import ctypes
 import os
 import subprocess
 
+import numpy as np
+
 from .pafprocess_oracle import _PafProcess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -58,6 +60,16 @@ class _Port(_PafProcess):
         f.restype = ctypes.c_int
         bound = self.params
         self._process = lambda *a: f(*a, ctypes.byref(bound))
+
+    def connections(self, limb):
+        """As the port's, from the (limb, a, b, score) quads port_process_paf_params records."""
+        L = self._lib
+        L.port_params_num_conns.restype = ctypes.c_long
+        L.port_params_conns.restype = ctypes.POINTER(ctypes.c_float)
+        n = int(L.port_params_num_conns())
+        q = np.ctypeslib.as_array(L.port_params_conns(), (n, 4)).copy() if n else np.zeros((0, 4), np.float32)
+        q = q[q[:, 0] == limb]
+        return q[:, 1].astype(np.int32), q[:, 2].astype(np.int32), np.ascontiguousarray(q[:, 3])
 
 
 def port_path():

@@ -54,6 +54,8 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_post_debug": ([vp, vp, ci, ci], ci),
     "b200pose_post_status_accum": ([vp, ci], ci),
     "b200pose_post_debug_sort": ([vp, vp, ci, vp], ci),
+    "b200pose_post_set_grids": ([vp, ci, ci], ci),
+    "b200pose_post_debug_connections": ([vp, ci, ci, vp, vp, vp, ci], ci),
     "b200pose_post_debug_maps": ([vp, vp, cl, vp, cl], ci),
     "b200pose_post_num_humans": ([vp, ci], ci),
     "b200pose_post_status": ([vp, ci], ci),

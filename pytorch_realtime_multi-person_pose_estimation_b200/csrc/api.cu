@@ -537,6 +537,9 @@ struct b200pose_post {
     // by value, so a run in flight keeps its own
     PostParams params{DefaultPostParams::paf_thresh, DefaultPostParams::paf_samples, DefaultPostParams::paf_min_above,
                       DefaultPostParams::min_parts, DefaultPostParams::min_person_score};
+    // grids of limb_score_kernel / range_sort_kernel for the runs submitted from now on, 0 = the defaults
+    // (b200pose_post_set_grids, a test hook: the results never depend on them)
+    int score_blocks = 0, sort_blocks = 0;
     // the second stream's work still reads the buffers; post_free is null-safe (post_alloc zeroes pb first)
     ~b200pose_post() { if (s2) cudaStreamSynchronize(s2); post_free(pb); }
 };
@@ -1601,12 +1604,14 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
     if (layout == 0) {
         e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, (long)h * w, w, 1, h, w, thresh, ps, ext);
         if (launched(e, "post_peaks")) return 1;
-        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps, ext, prm);
+        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps, ext, prm,
+                       p->score_blocks, p->sort_blocks);
     } else {
         if (ext) return fail("post_run: ragged batches need the planar (layout 0) maps");
         e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, 1, (long)w * 19, 19, h, w, thresh, ps);
         if (launched(e, "post_peaks")) return 1;
-        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * 8, w, h, ps, nullptr, prm);
+        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * 8, w, h, ps, nullptr, prm,
+                       p->score_blocks, p->sort_blocks);
     }
     if (launched(e, "post_limbs")) return 1;
     CU(cudaEventRecord(p->ev_ld[slot], ps));
@@ -1660,6 +1665,17 @@ int b200pose_post_get_params(b200pose_post* p, b200pose_post_params* out) {
     return 0;
 }
 
+int b200pose_post_set_grids(b200pose_post* p, int score_blocks, int sort_blocks) {
+    if (!p) return fail("null post");
+    if (score_blocks < 0 || score_blocks > 65535)
+        return fail("post_set_grids: score_blocks %d is outside 0 .. 65535", score_blocks);
+    if (sort_blocks < 0 || sort_blocks > 65535)
+        return fail("post_set_grids: sort_blocks %d is outside 0 .. 65535", sort_blocks);
+    p->score_blocks = score_blocks;
+    p->sort_blocks = sort_blocks;
+    return 0;
+}
+
 long b200pose_post_last_ticket(b200pose_post* p) { return p ? p->runs - 1 : -1; }
 
 int b200pose_post_select(b200pose_post* p, long ticket) {
@@ -1697,7 +1713,27 @@ int b200pose_post_debug_sort(b200pose_post* p, const unsigned long long* keys, i
     if (!p || !keys || !out) return fail("debug_sort: null pointer");
     CU(cudaSetDevice(p->device));
     CU(cudaStreamSynchronize(p->s2));
-    return launched(post_debug_sort(p->pb, keys, n, out, nullptr), "post_debug_sort", 2);
+    return launched(post_debug_sort(p->pb, keys, n, out, nullptr, p->sort_blocks), "post_debug_sort", 2);
+}
+
+int b200pose_post_debug_connections(b200pose_post* p, int img, int limb, int* a, int* b, float* s, int cap) {
+    // valid for the LATEST run only (reads the device connection lists, which the next run overwrites); a count can be
+    // 1, so errors return -1
+    if (!p || !a || !b || !s) return -fail("debug_connections: null pointer");
+    if (p->runs == 0) return -fail("debug_connections: no run submitted");
+    if (b200pose_post_select(p, p->runs - 1)) return -1;
+    if (img < 0 || img >= p->slot_n[p->cur] || limb < 0 || limb >= kNumLimb || cap < 0)
+        return -fail("debug_connections: image %d of %d, limb %d, cap %d", img, p->slot_n[p->cur], limb, cap);
+    const PostBuffers& pb = p->pb;
+    const long li = (long)img * kNumLimb + limb;
+    int cnt = 0;
+    cudaError_t e = cudaMemcpy(&cnt, pb.conn_cnt + li, sizeof(int), cudaMemcpyDeviceToHost);
+    const size_t k = (size_t)(cnt < cap ? cnt : cap);
+    if (e == cudaSuccess && k > 0) e = cudaMemcpy(a, pb.conn_a + li * pb.peak_cap, k * sizeof(int), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && k > 0) e = cudaMemcpy(b, pb.conn_b + li * pb.peak_cap, k * sizeof(int), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && k > 0) e = cudaMemcpy(s, pb.conn_s + li * pb.peak_cap, k * sizeof(float), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) return -cuda_fail("debug_connections: %s", cudaGetErrorString(e));
+    return cnt;
 }
 
 int b200pose_post_debug(b200pose_post* p, unsigned long long* out, int n, int reset) {

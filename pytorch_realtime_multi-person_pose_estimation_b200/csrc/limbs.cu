@@ -812,7 +812,8 @@ __global__ void __launch_bounds__(kGreedyThreads) limb_greedy_kernel(PostBuffers
     } while (0)
 
 cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long p_img, long p_ch, long p_y, long p_x,
-                       int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext, const PostParams* prm) {
+                       int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext, const PostParams* prm,
+                       int score_blocks, int sort_blocks) {
     if (batch > pb.batch_cap) return cudaErrorInvalidValue;
     if (pb.cand_smem_cap != kS) return cudaErrorInvalidValue;
     PafView pv{paf, p_ch, p_y, p_x, shift};
@@ -828,20 +829,21 @@ cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long 
     int dev = 0, sms = 132;
     B2P_TRY(cudaGetDevice(&dev));
     B2P_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    if (score_blocks == 0) score_blocks = sms * 6;
     if (!prm) {
         B2P_TRY(optin_score.ensure(limb_score_kernel<DefaultPostParams>, smem));
-        limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
-                                                               ext, DefaultPostParams{});
+        limb_score_kernel<<<score_blocks, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
+                                                                  ext, DefaultPostParams{});
     } else {
         B2P_TRY(optin_score_p.ensure(limb_score_kernel<PostParams>, smem));
-        limb_score_kernel<<<sms * 6, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
-                                                               ext, *prm);
+        limb_score_kernel<<<score_blocks, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
+                                                                  ext, *prm);
     }
     B2P_TRY(cudaGetLastError());
     limb_gather_kernel<<<dim3(batch, kNumLimb), kGatherThreads, 0, s>>>(pb);
     B2P_TRY(cudaGetLastError());
     B2P_TRY(optin_sort.ensure(range_sort_kernel, sizeof(SortSmem)));
-    const int sort_blocks = batch * kNumLimb < sms * 3 ? batch * kNumLimb : sms * 3;
+    if (sort_blocks == 0) sort_blocks = batch * kNumLimb < sms * 3 ? batch * kNumLimb : sms * 3;
     range_sort_kernel<<<sort_blocks, kSortThreads, sizeof(SortSmem), s>>>(pb);
     B2P_TRY(cudaGetLastError());
     limb_greedy_kernel<<<dim3(batch, kNumLimb), kGreedyThreads, 0, s>>>(pb);
@@ -851,7 +853,7 @@ cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long 
 // Test hook: exact std::sort of `n` host keys through the product's sorting stages (limb_gather_kernel's global-memory
 // partitions + range_sort_kernel), as if they were the candidates of limb 0 of image 0.
 cudaError_t post_debug_sort(const PostBuffers& pb, const unsigned long long* keys, int n, unsigned long long* out,
-                            cudaStream_t s) {
+                            cudaStream_t s, int sort_blocks) {
     if (n < 1 || (long long)n + 2 > pb.pool_cap / 2) return cudaErrorInvalidValue;
     const int nchunks = (n + kChunkPairs - 1) / kChunkPairs;
     if (nchunks > pb.work_cap) return cudaErrorInvalidValue;
@@ -870,9 +872,15 @@ cudaError_t post_debug_sort(const PostBuffers& pb, const unsigned long long* key
     B2P_TRY(cudaMemcpyAsync(pb.pool, keys, (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, s));
     limb_gather_kernel<<<dim3(1, kNumLimb), kGatherThreads, 0, s>>>(pb);
     B2P_TRY(cudaGetLastError());
+    if (sort_blocks == 0) {
+        int dev = 0, sms = 132;
+        B2P_TRY(cudaGetDevice(&dev));
+        B2P_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        sort_blocks = sms * 3;
+    }
     static DynSmemOptIn optin_sort;
     B2P_TRY(optin_sort.ensure(range_sort_kernel, sizeof(SortSmem)));
-    range_sort_kernel<<<132 * 3, kSortThreads, sizeof(SortSmem), s>>>(pb);
+    range_sort_kernel<<<sort_blocks, kSortThreads, sizeof(SortSmem), s>>>(pb);
     B2P_TRY(cudaGetLastError());
     B2P_TRY(cudaMemcpyAsync(out, pb.pool + pb.pool_cap / 2, (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);

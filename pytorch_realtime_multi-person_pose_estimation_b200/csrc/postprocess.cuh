@@ -85,12 +85,15 @@ cudaError_t post_peaks(const PostBuffers& pb, int batch, const float* heat, long
 // paf: fp32 view per image: base + img*p_img, strides (p_ch, p_y, p_x), shift (3: low-res, 0: already upsampled).
 // ext (ragged batch) or null: h_up of image i is its own padded height ext[2 i].
 // prm: the scoring settings, copied into the launch; null = the reference's constants (the DefaultPostParams kernel).
+// score_blocks / sort_blocks: the grids of the two work-queue kernels, limb_score_kernel and range_sort_kernel; 0 = the
+// defaults (SMs x 6, and min(batch x 19, SMs x 3)).  Results do not depend on them (b200pose_post_set_grids).
 cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long p_img, long p_ch, long p_y,
                                     long p_x, int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext = nullptr,
-                                    const PostParams* prm = nullptr);
+                                    const PostParams* prm = nullptr, int score_blocks = 0, int sort_blocks = 0);
 // Test hook (limbs.cu): exact std::sort of n host keys through the global-memory partition + shared-memory range kernels.
+// sort_blocks: range_sort_kernel's grid, 0 = SMs x 3.
 cudaError_t post_debug_sort(const PostBuffers& pb, const unsigned long long* keys, int n, unsigned long long* out,
-                            cudaStream_t s);
+                            cudaStream_t s, int sort_blocks = 0);
 // Person assembly of the connections post_limbs() left in `pb`.  Small footprint (128 threads, human_cap*4 B smem per
 // image): it can run on a second stream next to the convolutions of the following batch.
 // prm: the prune settings, as for post_limbs.

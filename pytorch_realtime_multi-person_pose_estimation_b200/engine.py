@@ -463,6 +463,29 @@ class NativePost:
         nat.check(nat.lib().b200pose_post_get_params(self._h, ctypes.byref(q)), "b200pose_post_get_params")
         return q.as_dict()
 
+    def set_grids(self, score_blocks=0, sort_blocks=0):
+        """Test hook: the grids of the PAF scoring and range sorting kernels for the runs submitted from now on (fused
+        runs and debug_sort included); 0 restores a default.  The results never depend on them.  A value outside
+        0 .. 65535 raises B200PoseError naming it and leaves the grids unchanged."""
+        for name, v in (("score_blocks", score_blocks), ("sort_blocks", sort_blocks)):
+            if int(v) != v or not -2 ** 31 <= v < 2 ** 31:      # ctypes would wrap
+                raise nat.B200PoseError("set_grids: %s must be a 32-bit integer, got %r" % (name, v))
+        nat.check(nat.lib().b200pose_post_set_grids(self._h, int(score_blocks), int(sort_blocks)),
+                  "b200pose_post_set_grids")
+
+    def connections(self, img, limb):
+        """Test hook: (a int32 [k], b int32 [k], score float32 [k]), the connections the greedy matcher chose for limb
+        `limb` of image `img` of the latest run, in its order; a and b index the peaks of the limb's two parts."""
+        L = nat.lib()
+        a = np.empty(self.peak_cap, np.int32)
+        b = np.empty(self.peak_cap, np.int32)
+        s = np.empty(self.peak_cap, np.float32)
+        k = int(L.b200pose_post_debug_connections(self._h, int(img), int(limb), a.ctypes.data, b.ctypes.data,
+                                                   s.ctypes.data, self.peak_cap))
+        if k < 0:
+            nat.check(1, "b200pose_post_debug_connections")
+        return a[:k].copy(), b[:k].copy(), s[:k].copy()
+
     def run(self, heat_ptr, paf_ptr, on_device, layout, n, h, w, thresh, stream=0):
         nat.check(nat.lib().b200pose_post_run(self._h, ctypes.c_void_p(heat_ptr), ctypes.c_void_p(paf_ptr), int(on_device),
                                               layout, n, h, w, ctypes.c_float(thresh), ctypes.c_void_p(stream)),
