@@ -449,7 +449,7 @@ struct b200pose_net {
     // Allocated once for kMaxRagged images and never moved, so that plans and captured graphs stay valid across mixes;
     // rewritten on the stream before each ragged forward.
     DevBuf<int> d_ext;
-    DevBuf<RaggedFrame> d_frames;      // per-frame source geometry of the last ragged crop
+    DevBuf<RaggedFrame> d_frames;      // frame table (per-frame source geometry) of the last crop or uint8 mirror
     // video frames (b200pose_net_convert_frames, b200pose_infer_frames): the planes of host frames, packed, and the
     // source table of the last conversion
     DevBuf<unsigned char> frame_stage;
@@ -1268,7 +1268,8 @@ constexpr int kMaxOvfRows = 16;
 
 // A batch of raw uint8 frames packed back to back, cropped for one destination size: frame table (flip: the mirrored
 // frames follow the originals, in the staging buffer and in both tables), padded extents and canvas, the frames' total
-// and largest size in bytes.  A uniform batch (frames of one size) keeps `ext` empty: its kernels get no extents table.
+// and largest size in bytes.  A uniform batch (frames of one size) keeps `ext` empty: its forward and post-processing get
+// no extents table.
 struct RawBatch {
     std::vector<RaggedFrame> tab;
     std::vector<int> ext;
@@ -1277,16 +1278,14 @@ struct RawBatch {
     bool ragged() const { return !ext.empty(); }
 };
 
-// Crops the nimg frames of c (sources at d_raw; ragged: frame table already in net->d_frames) into net->in_stage_u8
-// and runs the forward pass on them.
+// Crops the nimg frames of c (sources at d_raw; frame table already in net->d_frames) into net->in_stage_u8 and runs
+// the forward pass on them.
 static int crop_and_forward(b200pose_net* net, const unsigned char* d_raw, int nimg, const RawBatch& c, int mode,
                             cudaStream_t st, float* const* outputs = nullptr, int outputs_on_device = 1,
                             bool sync_host = false) {
     CU(net->in_stage_u8.ensure((size_t)nimg * c.Hc * c.Wc * 3));
-    const RaggedFrame& f = c.tab[0];
-    cudaError_t e = c.ragged() ? ragged_frames_launch(d_raw, net->d_frames.p, nimg, net->in_stage_u8.p, c.Hc, c.Wc, st)
-                               : crop_with_factor_launch(d_raw, net->in_stage_u8.p, nimg, f.src_h, f.src_w, f.g, st);
-    if (launched(e, c.ragged() ? "ragged_frames_launch" : "crop_with_factor_launch")) return 1;
+    if (launched(crop_frames_launch(d_raw, net->d_frames.p, nimg, net->in_stage_u8.p, c.Hc, c.Wc, st), "crop_frames_launch"))
+        return 1;
     if (c.ragged() && upload_ext(net, c.ext, st)) return 1;
     return net_forward_impl(net, net->in_stage_u8.p, 1, 1, nimg, c.Hc, c.Wc, mode, outputs, outputs_on_device, st,
                             sync_host, c.ragged() ? net->d_ext.p : nullptr);
@@ -1978,7 +1977,10 @@ static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input,
         if (in_u8) {
             CU(net->in_stage_u8.ensure(2 * elems));
             CU(cudaMemcpyAsync(net->in_stage_u8.p, input, elems, kind, st));
-            e = tta_mirror_u8hwc(net->in_stage_u8.p, net->in_stage_u8.p + elems, n, H, W, st);
+            std::vector<RaggedFrame> tab(n);       // already cropped frames: the geometry is unused
+            for (int i = 0; i < n; ++i) tab[i] = RaggedFrame{(long long)i * H * W * 3, H, W, CropGeom{}};
+            if (int rc = upload_frames(net, tab, st)) return rc;
+            e = tta_mirror_frames(net->in_stage_u8.p, net->in_stage_u8.p + elems, net->d_frames.p, n, (long)H * W * 3, st);
             input = net->in_stage_u8.p;
         } else {
             CU(net->in_stage.ensure(2 * elems));
@@ -2016,6 +2018,7 @@ int b200pose_infer_u8_flip(b200pose_net* net, b200pose_post* post, const unsigne
 // ------------------------------------------------------------------------------------------------ crop_with_factor
 static int crop_check(int n, int src_h, int src_w, int dest_size, int factor, CropGeom* g) {
     if (n < 1 || src_h < 1 || src_w < 1 || dest_size < 1) return fail("crop_with_factor: bad shape");
+    if (n > 65535) return fail("crop_with_factor: %d images (at most 65535)", n);
     if (factor < 8 || factor % 8) return fail("crop_with_factor: factor must be a multiple of 8 (the network's stride)");
     *g = crop_geometry(src_h, src_w, dest_size, factor);
     if (g->res_h < 1 || g->res_w < 1) return fail("crop_with_factor: the resized frame would be empty");
@@ -2052,7 +2055,10 @@ int b200pose_net_crop_with_factor(b200pose_net* net, const unsigned char* images
         CU(net->in_stage_u8.ensure(outb));
         d_out = net->in_stage_u8.p;
     }
-    if (launched(crop_with_factor_launch(d_in, d_out, n, src_h, src_w, g, st), "crop_with_factor_launch")) return 1;
+    std::vector<RaggedFrame> tab(n);
+    for (int i = 0; i < n; ++i) tab[i] = RaggedFrame{(long long)i * src_h * src_w * 3, src_h, src_w, g};
+    if (int rc = upload_frames(net, tab, st)) return rc;
+    if (launched(crop_frames_launch(d_in, net->d_frames.p, n, d_out, g.pad_h, g.pad_w, st), "crop_frames_launch")) return 1;
     if (!out_on_device) CU(cudaMemcpyAsync(out, d_out, outb, cudaMemcpyDeviceToHost, st));
     if (!images_on_device || !out_on_device) CU(cudaStreamSynchronize(st));
     return 0;
@@ -2366,9 +2372,10 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
     for (int k = 0; k < (int)sc.size(); ++k) {
         const int dest = scales ? (int)((double)base_size * scales[k]) : base_size;       // Python: int(base_size * s)
         if (int rc = raw_batch(n, src_h, src_w, src_hw, dest, factor, flip, &sc[k])) return rc;
-        for (int i = 0; i < n && scales && ragged; ++i)
-            rz.push_back(ragged_resize(sc[k].ext[2 * i] / 8, sc[k].ext[2 * i + 1] / 8, base.ext[2 * i] / 8,
-                                       base.ext[2 * i + 1] / 8));
+        for (int i = 0; i < n && scales; ++i) {
+            const CropGeom &g = sc[k].tab[i].g, &g1 = base.tab[i].g;
+            rz.push_back(ragged_resize(g.pad_h / 8, g.pad_w / 8, g1.pad_h / 8, g1.pad_w / 8));
+        }
     }
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
@@ -2379,12 +2386,11 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
                       : stage_raw(net, images, on_device, (size_t)sc[0].raw, flip, st, &d_raw))
         return rc;
     // the sources and offsets of the frame table are those of every scale
-    if (ragged && upload_frames(net, sc[0].tab, st)) return 1;
+    if (upload_frames(net, sc[0].tab, st)) return 1;
     if (flip) {      // mirrored RAW frames, so that the padding of both orientations ends up on the right, as for the reference
         unsigned char* mirror = net->raw_stage.p + sc[0].raw;
-        cudaError_t e = ragged ? tta_mirror_u8hwc_ragged(net->raw_stage.p, mirror, net->d_frames.p, n, (long)sc[0].max_bytes, st)
-                               : tta_mirror_u8hwc(net->raw_stage.p, mirror, n, src_h, src_w, st);
-        if (launched(e, "tta_mirror")) return 1;
+        if (launched(tta_mirror_frames(net->raw_stage.p, mirror, net->d_frames.p, n, (long)sc[0].max_bytes, st), "tta_mirror"))
+            return 1;
     }
     const int nimg = flip ? 2 * n : n;
     if (!scales) {
@@ -2395,15 +2401,15 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
     if (ragged) {
         CU(post->ms_ext.ensure(base.ext.size()));
         CU(cudaMemcpyAsync(post->ms_ext.p, base.ext.data(), base.ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-        CU(post->ms_resize.ensure(rz.size()));
-        CU(cudaMemcpyAsync(post->ms_resize.p, rz.data(), rz.size() * sizeof(RaggedResize), cudaMemcpyHostToDevice, st));
     }
+    CU(post->ms_resize.ensure(rz.size()));
+    CU(cudaMemcpyAsync(post->ms_resize.p, rz.data(), rz.size() * sizeof(RaggedResize), cudaMemcpyHostToDevice, st));
     const int h1 = base.Hc / 8, w1 = base.Wc / 8;
     CU(post->d_heat.ensure((size_t)n * kHeat * h1 * w1));
     CU(post->d_paf.ensure((size_t)n * kPaf * h1 * w1));
     for (int k = 0; k < n_scales; ++k) {
         const RawBatch& c = sc[k];
-        if (ragged && k > 0 && upload_frames(net, c.tab, st)) return 1;
+        if (k > 0 && upload_frames(net, c.tab, st)) return 1;
         if (int rc = crop_and_forward(net, d_raw, nimg, c, mode, st)) return rc;
         if (int rc = stash_overflow(net, post, nimg, st)) return rc;
         const int h = c.Hc / 8, w = c.Wc / 8;
@@ -2416,17 +2422,9 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
             s_paf = post->tta_out.p + eh;
         }
         const float div = (k == n_scales - 1) ? (float)n_scales : 0.f;
-        cudaError_t e;
-        if (ragged) {
-            const RaggedResize* f = post->ms_resize.p + (size_t)k * n;
-            e = resize_cubic_accum_ragged_launch(s_heat, post->d_heat.p, f, n, kHeat, h, w, h1, w1, k == 0, div, st);
-            if (e == cudaSuccess)
-                e = resize_cubic_accum_ragged_launch(s_paf, post->d_paf.p, f, n, kPaf, h, w, h1, w1, k == 0, div, st);
-        } else {
-            e = resize_cubic_accum_launch(s_heat, post->d_heat.p, (long)n * kHeat, h, w, h1, w1, k == 0, div, st);
-            if (e == cudaSuccess)
-                e = resize_cubic_accum_launch(s_paf, post->d_paf.p, (long)n * kPaf, h, w, h1, w1, k == 0, div, st);
-        }
+        const RaggedResize* f = post->ms_resize.p + (size_t)k * n;
+        cudaError_t e = resize_cubic_accum_launch(s_heat, post->d_heat.p, f, n, kHeat, h, w, h1, w1, k == 0, div, st);
+        if (e == cudaSuccess) e = resize_cubic_accum_launch(s_paf, post->d_paf.p, f, n, kPaf, h, w, h1, w1, k == 0, div, st);
         if (launched(e, "resize_cubic_accum", 2)) return 1;
     }
     // the net's extents table now holds the last scale's: post-processing reads the base extents

@@ -9,22 +9,11 @@ namespace {
 
 constexpr int kThreads = 256;
 
-__global__ void __launch_bounds__(kThreads) mirror_u8hwc_kernel(const unsigned char* __restrict__ in,
-                                                                unsigned char* __restrict__ out, long rows, int W) {
-    // one thread per output byte; row = (image, y)
-    const long total = rows * W * 3;
-    for (long i = blockIdx.x * (long)kThreads + threadIdx.x; i < total; i += (long)gridDim.x * kThreads) {
-        const long row = i / (W * 3);
-        const int r = (int)(i - row * (W * 3));
-        const int x = r / 3, ch = r - 3 * x;
-        out[i] = in[row * (W * 3) + (W - 1 - x) * 3 + ch];
-    }
-}
-
-// ragged batch: frame blockIdx.y (src_h x src_w pixels at byte offset off) mirrored within its own width into out + off
-__global__ void __launch_bounds__(kThreads) mirror_u8hwc_ragged_kernel(const unsigned char* __restrict__ in,
-                                                                       unsigned char* __restrict__ out,
-                                                                       const RaggedFrame* __restrict__ frames) {
+// frame blockIdx.y (src_h x src_w pixels at byte offset off) mirrored within its own width into out + off; one thread
+// per output byte
+__global__ void __launch_bounds__(kThreads) mirror_frames_kernel(const unsigned char* __restrict__ in,
+                                                                 unsigned char* __restrict__ out,
+                                                                 const RaggedFrame* __restrict__ frames) {
     const RaggedFrame f = frames[blockIdx.y];
     const int W = f.src_w;
     const long total = (long)f.src_h * W * 3;
@@ -82,20 +71,14 @@ int grid_for(long total) {
 
 }  // namespace
 
-cudaError_t tta_mirror_u8hwc(const unsigned char* in, unsigned char* out, int n, int H, int W, cudaStream_t s) {
-    const long rows = (long)n * H;
-    mirror_u8hwc_kernel<<<grid_for(rows * W * 3), kThreads, 0, s>>>(in, out, rows, W);
-    return cudaGetLastError();
-}
-
-cudaError_t tta_mirror_u8hwc_ragged(const unsigned char* in, unsigned char* out, const RaggedFrame* frames, int n,
-                                    long max_frame_bytes, cudaStream_t s) {
+cudaError_t tta_mirror_frames(const unsigned char* in, unsigned char* out, const RaggedFrame* frames, int n,
+                              long max_frame_bytes, cudaStream_t s) {
     if (n < 1 || n > 65535) return cudaErrorInvalidValue;
     long bx = (max_frame_bytes + kThreads - 1) / kThreads;
     const long cap = (132L * 8 + n - 1) / n;
     if (bx > cap) bx = cap;
     if (bx < 1) bx = 1;
-    mirror_u8hwc_ragged_kernel<<<dim3((unsigned)bx, (unsigned)n), kThreads, 0, s>>>(in, out, frames);
+    mirror_frames_kernel<<<dim3((unsigned)bx, (unsigned)n), kThreads, 0, s>>>(in, out, frames);
     return cudaGetLastError();
 }
 

@@ -8,12 +8,10 @@
 
 namespace b2p {
 
-// out[i, y, x, :] = in[i, y, W-1-x, :]   uint8 HWC frames (3 channels)
-cudaError_t tta_mirror_u8hwc(const unsigned char* in, unsigned char* out, int n, int H, int W, cudaStream_t s);
-// ragged batch: frame i (frames[i].src_h x frames[i].src_w, HWC at byte offset frames[i].off) mirrored from in + off into
-// out + off; max_frame_bytes = the largest frame's size
-cudaError_t tta_mirror_u8hwc_ragged(const unsigned char* in, unsigned char* out, const RaggedFrame* frames, int n,
-                                    long max_frame_bytes, cudaStream_t s);
+// uint8 HWC frames (3 channels): frame i (H = frames[i].src_h, W = frames[i].src_w, at byte offset off = frames[i].off)
+// out[off + (y, x, :)] = in[off + (y, W-1-x, :)]; max_frame_bytes = the largest frame's size
+cudaError_t tta_mirror_frames(const unsigned char* in, unsigned char* out, const RaggedFrame* frames, int n,
+                              long max_frame_bytes, cudaStream_t s);
 // out[i, c, y, x] = in[i, c, y, W-1-x]   fp32 planes; `planes` = n * channels
 cudaError_t tta_mirror_f32(const float* in, float* out, long planes, int H, int W, cudaStream_t s);
 // out(img, c, y, x) = (normal(img, c, y, x) +/- flipped(img, swap[c], y, w-1-x)) / 2 for `channels` = 19 (heat) or 38

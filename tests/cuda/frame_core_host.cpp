@@ -24,7 +24,7 @@ static FrameSrc frame_src(const unsigned char* const* planes, const int* pitch, 
 }
 
 // planes[3] / pitch[3] of one stored h x w frame of format fmt -> out [oh, ow, 3] rotated by rot degrees clockwise;
-// mirror: then out(y, x) = rotated(y, ow - 1 - x), what tta_mirror_u8hwc makes of it.
+// mirror: then out(y, x) = rotated(y, ow - 1 - x), what tta_mirror_frames makes of it.
 extern "C" int core_convert_frame(const unsigned char* const* planes, const int* pitch, int h, int w, int fmt, int rot,
                                   int mirror, unsigned char* out) {
     const FrameSrc f = frame_src(planes, pitch, h, w);

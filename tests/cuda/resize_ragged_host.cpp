@@ -1,5 +1,5 @@
 // Host build of the ragged bicubic resize (csrc/resize_core.h: ragged_resize, rs_cubic_ragged_at), walked over a whole
-// destination canvas exactly as resize_cubic_accum_ragged_kernel walks it (one plane, no running sum).
+// destination canvas exactly as resize_cubic_accum_kernel walks it (one plane, no running sum).
 #include "../../pytorch_realtime_multi-person_pose_estimation_b200/csrc/resize_core.h"
 
 using namespace b2p;

@@ -138,7 +138,7 @@ def ragged_core(tmp_path_factory):
 
 
 def test_ragged_cubic_resize_core_on_host_matches_each_frame_resized_alone(built, ragged_core):
-    """csrc/resize_core.h ragged_resize / rs_cubic_ragged_at (what resize_cubic_accum_ragged_kernel calls), compiled for
+    """csrc/resize_core.h ragged_resize / rs_cubic_ragged_at (what resize_cubic_accum_kernel calls), compiled for
     the host: each frame of a mixed canvas resized from its own extent at scale s to its own base grid equals the
     oracle's resize_cubic of that frame alone, bit for bit, for the four scale ratios; the taps never read the canvas
     outside the frame (filled with NaN here), and every element outside a frame's base extent is +0."""
@@ -166,11 +166,11 @@ def test_ragged_cubic_resize_core_on_host_matches_each_frame_resized_alone(built
             assert (outside.view(np.int32) == 0).all(), (s, i)
 
 
-def test_ragged_resize_kernel_does_not_spill(built):
+def test_resize_cubic_accum_kernel_does_not_spill(built):
     r = subprocess.run([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17",
                         "-Xptxas", "-v", "-c", os.path.join(CSRC, "resize.cu"), "-o", os.devnull],
                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-2000:]
     bodies = [body for fn, body in re.findall(r"Compiling entry function '(\S+)' for 'sm_90a'(.*?)(?=Compiling entry|\Z)",
-                                              r.stdout, re.S) if "resize_cubic_accum_ragged_kernel" in fn]
+                                              r.stdout, re.S) if "resize_cubic_accum_kernel" in fn]
     assert len(bodies) == 1 and "0 bytes spill stores, 0 bytes spill loads" in bodies[0], r.stdout[-2000:]
