@@ -449,6 +449,31 @@ int b200pose_net_encode_pngs(b200pose_net* net, const unsigned char* frames, int
                              void* cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3i. COCO keypoint evaluation: replaces pycocotools' COCOeval(cocoGt, cocoDt, 'keypoints') .evaluate() and
+ *     .accumulate() with default Params   (DESIGN.md 2.16, csrc/coco_eval_core.h)
+ *     The caller has done loadRes and _prepare: the gts and detections are grouped into (category, image) units that
+ *     have at least one of either, units ordered by category index (0 .. n_cats - 1, the sorted category ids) and
+ *     within a category by ascending image id.  Unit u: category unit_cat[u], gts unit_gt0[u] .. unit_gt0[u+1] - 1 in
+ *     the gt file's order, detections unit_dt0[u] .. unit_dt0[u+1] - 1 in the result list's order.
+ *     Per gt: gt_id (non-zero, all different), gt_kpt [51] (x, y, v per part), gt_box [5] (bbox x, y, w, h, then the
+ *     annotation's area), gt_crowd (iscrowd) and gt_ignore (_prepare's flag: iscrowd or num_keypoints == 0).  Per
+ *     detection: dt_kpt [51] and dt_score.  thr: iouThrs [10] then recThrs [101], each ascending.
+ *     Out (host): precision [10][101][n_cats][3] and recall [10][n_cats][3] (pycocotools' eval['precision'] and
+ *     eval['recall'] without the maxDets axis; area ranges all, medium, large).  oks (host, may be null): each unit's
+ *     computeOks block [min(nd, 20)][ng] back to back in unit order, oks_cap doubles; oks_count (may be null) gets
+ *     the block sizes' sum.
+ *     Runs on `device` in a stream of its own and synchronises it.  Non-finite values, a keypoint count other than
+ *     51, gt id 0 or a repeated gt id, units out of order, and counts above the limits (1024 gts and 1024 detections
+ *     per unit, 2^24 gts or detections per call, 2^18 detections after the cut to 20 per unit, 1024 categories) are
+ *     refused, naming the argument, before anything is enqueued.  One call launches 4 kernels.
+ * ---------------------------------------------------------------------------------------------------------- */
+int b200pose_coco_kpt_eval(int device, int n_units, int n_cats, const int* unit_cat, const int* unit_gt0,
+                           const int* unit_dt0, const long long* gt_id, const double* gt_kpt, int gt_kpt_len,
+                           const double* gt_box, const unsigned char* gt_crowd, const unsigned char* gt_ignore,
+                           const double* dt_kpt, int dt_kpt_len, const double* dt_score, const double* thr,
+                           double* precision, double* recall, double* oks, long long oks_cap, long long* oks_count);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

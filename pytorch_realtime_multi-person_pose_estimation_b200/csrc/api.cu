@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/b200pose.h"
+#include "coco_eval.cuh"
 #include "conv_misc.cuh"
 #include "conv_tc.cuh"
 #include "f16_core.h"
@@ -2745,6 +2746,134 @@ int b200pose_net_encode_pngs(b200pose_net* net, const unsigned char* frames, int
     if (!out_on_device) CU(cudaMemcpyAsync(out, net->penc_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     for (int i = 0; i < n; ++i) sizes[i] = got[i].size;
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ COCO keypoint evaluation
+int b200pose_coco_kpt_eval(int device, int n_units, int n_cats, const int* unit_cat, const int* unit_gt0,
+                           const int* unit_dt0, const long long* gt_id, const double* gt_kpt, int gt_kpt_len,
+                           const double* gt_box, const unsigned char* gt_crowd, const unsigned char* gt_ignore,
+                           const double* dt_kpt, int dt_kpt_len, const double* dt_score, const double* thr,
+                           double* precision, double* recall, double* oks, long long oks_cap, long long* oks_count) {
+    if (n_units < 0) return fail("coco_kpt_eval: n_units = %d", n_units);
+    if (n_cats < 1 || n_cats > kCocoMaxCats) return fail("coco_kpt_eval: n_cats = %d (1 .. %d)", n_cats, kCocoMaxCats);
+    if ((n_units && (!unit_cat || !unit_gt0 || !unit_dt0)) || !thr || !precision || !recall)
+        return fail("coco_kpt_eval: null pointer");
+    if (gt_kpt_len != kCocoKpt) return fail("coco_kpt_eval: gt_kpt_len = %d (keypoints are 51 values)", gt_kpt_len);
+    if (dt_kpt_len != kCocoKpt) return fail("coco_kpt_eval: dt_kpt_len = %d (keypoints are 51 values)", dt_kpt_len);
+    for (int i = 0; i < kCocoIouThrs + kCocoRecThrs; ++i) {
+        if (!std::isfinite(thr[i])) return fail("coco_kpt_eval: thr[%d] is not finite", i);
+        if (i != 0 && i != kCocoIouThrs && thr[i] < thr[i - 1]) return fail("coco_kpt_eval: thr[%d] not ascending", i);
+    }
+    const int G = n_units ? unit_gt0[n_units] : 0, D = n_units ? unit_dt0[n_units] : 0;
+    if (n_units && (unit_gt0[0] != 0 || unit_dt0[0] != 0)) return fail("coco_kpt_eval: unit_gt0[0] / unit_dt0[0] not 0");
+    if (G > kCocoMaxTotal) return fail("coco_kpt_eval: %d gts (at most %d)", G, kCocoMaxTotal);
+    if (D > kCocoMaxTotal) return fail("coco_kpt_eval: %d detections (at most %d)", D, kCocoMaxTotal);
+    if ((G && (!gt_id || !gt_kpt || !gt_box || !gt_crowd || !gt_ignore)) || (D && (!dt_kpt || !dt_score)))
+        return fail("coco_kpt_eval: null pointer");
+    // units, kept detections and OKS blocks
+    std::vector<CocoUnit> units(n_units);
+    std::vector<int> cat_k0(n_cats + 1, 0);
+    int kept = 0;
+    long long oks_n = 0;
+    for (int u = 0; u < n_units; ++u) {
+        CocoUnit& x = units[u];
+        x.cat = unit_cat[u];
+        if (x.cat < 0 || x.cat >= n_cats) return fail("coco_kpt_eval: unit_cat[%d] = %d (0 .. %d)", u, x.cat, n_cats - 1);
+        if (u && x.cat < units[u - 1].cat) return fail("coco_kpt_eval: unit_cat[%d] below the unit before", u);
+        x.g0 = unit_gt0[u];
+        x.ng = unit_gt0[u + 1] - x.g0;
+        x.d0 = unit_dt0[u];
+        x.nd = unit_dt0[u + 1] - x.d0;
+        if (x.ng < 0 || x.ng > kCocoMaxUnitGts) return fail("coco_kpt_eval: unit_gt0: unit %d has %d gts (0 .. %d)", u, x.ng, kCocoMaxUnitGts);
+        if (x.nd < 0 || x.nd > kCocoMaxUnitDets)
+            return fail("coco_kpt_eval: unit_dt0: unit %d has %d detections (0 .. %d)", u, x.nd, kCocoMaxUnitDets);
+        x.nk = std::min(x.nd, kCocoMaxDets);
+        x.k0 = kept;
+        x.o0 = oks_n;
+        kept += x.nk;
+        oks_n += (long long)x.nk * x.ng;
+        if (kept > kCocoMaxKept) return fail("coco_kpt_eval: more than %d detections after the cut to 20 per unit", kCocoMaxKept);
+        cat_k0[x.cat + 1] = kept;
+    }
+    for (int c = 1; c <= n_cats; ++c) cat_k0[c] = std::max(cat_k0[c], cat_k0[c - 1]);
+    if (oks && oks_cap < oks_n) return fail("coco_kpt_eval: oks_cap %lld doubles, below %lld", oks_cap, oks_n);
+    std::set<long long> ids;
+    for (int g = 0; g < G; ++g) {
+        if (gt_id[g] == 0) return fail("coco_kpt_eval: gt_id[%d] is 0 (a match is marked by the gt id)", g);
+        if (!ids.insert(gt_id[g]).second) return fail("coco_kpt_eval: gt_id[%d] = %lld repeats an earlier gt", g, gt_id[g]);
+        for (int k = 0; k < kCocoKpt; ++k)
+            if (!std::isfinite(gt_kpt[(size_t)g * kCocoKpt + k])) return fail("coco_kpt_eval: gt_kpt of gt %d is not finite", g);
+        for (int k = 0; k < 5; ++k)
+            if (!std::isfinite(gt_box[(size_t)g * 5 + k])) return fail("coco_kpt_eval: gt_box of gt %d is not finite", g);
+    }
+    for (int d = 0; d < D; ++d) {
+        if (!std::isfinite(dt_score[d])) return fail("coco_kpt_eval: dt_score[%d] is not finite", d);
+        for (int k = 0; k < kCocoKpt; ++k)
+            if (!std::isfinite(dt_kpt[(size_t)d * kCocoKpt + k])) return fail("coco_kpt_eval: dt_kpt of detection %d is not finite", d);
+    }
+    // one upload: units, category offsets, gts, detections, thresholds; then the device's own arrays
+    auto align = [](size_t o) { return (o + 255) & ~(size_t)255; };
+    size_t at = 0;
+    auto take = [&](size_t bytes) { const size_t o = at; at = align(at + bytes); return o; };
+    const size_t o_units = take(n_units * sizeof(CocoUnit)), o_catk = take((n_cats + 1) * sizeof(int));
+    const size_t o_gkpt = take((size_t)G * kCocoKpt * 8), o_gbox = take((size_t)G * 5 * 8), o_gflag = take(G);
+    const size_t o_dkpt = take((size_t)D * kCocoKpt * 8), o_dsc = take((size_t)D * 8);
+    const size_t o_thr = take((kCocoIouThrs + kCocoRecThrs) * 8), up_bytes = at;
+    const size_t o_npig = take((size_t)n_cats * kCocoAreas * 4), o_kscore = take((size_t)kept * 8);
+    const size_t o_karea = take((size_t)kept * 8), o_kcat = take((size_t)kept * 4), o_oks = take((size_t)oks_n * 8);
+    const size_t o_state = take((size_t)kCocoAreas * kCocoIouThrs * kept), o_order = take((size_t)kept * 4);
+    const size_t n_prec = (size_t)kCocoIouThrs * kCocoRecThrs * n_cats * kCocoAreas;
+    const size_t n_rec = (size_t)kCocoIouThrs * n_cats * kCocoAreas;
+    const size_t o_prec = take(n_prec * 8), o_rec = take(n_rec * 8);
+    std::vector<char> up(up_bytes, 0);
+    memcpy(up.data() + o_units, units.data(), n_units * sizeof(CocoUnit));
+    memcpy(up.data() + o_catk, cat_k0.data(), (n_cats + 1) * sizeof(int));
+    if (G) {
+        memcpy(up.data() + o_gkpt, gt_kpt, (size_t)G * kCocoKpt * 8);
+        memcpy(up.data() + o_gbox, gt_box, (size_t)G * 5 * 8);
+        for (int g = 0; g < G; ++g) up[o_gflag + g] = (char)((gt_crowd[g] ? 1 : 0) | (gt_ignore[g] ? 2 : 0));
+    }
+    if (D) {
+        memcpy(up.data() + o_dkpt, dt_kpt, (size_t)D * kCocoKpt * 8);
+        memcpy(up.data() + o_dsc, dt_score, (size_t)D * 8);
+    }
+    memcpy(up.data() + o_thr, thr, (kCocoIouThrs + kCocoRecThrs) * 8);
+    CU(cudaSetDevice(device));
+    Stream st;
+    CU(cudaStreamCreateWithFlags(&st.h, cudaStreamNonBlocking));
+    DevBuf<char> buf;
+    CU(buf.ensure(at));
+    char* d = buf.p;
+    CU(cudaMemcpyAsync(d, up.data(), up_bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(d + o_npig, 0, (size_t)n_cats * kCocoAreas * 4, st));
+    CocoBatch b;
+    b.units = reinterpret_cast<const CocoUnit*>(d + o_units);
+    b.n_units = n_units;
+    b.n_cats = n_cats;
+    b.cat_k0 = reinterpret_cast<const int*>(d + o_catk);
+    b.gt_kpt = reinterpret_cast<const double*>(d + o_gkpt);
+    b.gt_box = reinterpret_cast<const double*>(d + o_gbox);
+    b.gt_flag = reinterpret_cast<const unsigned char*>(d + o_gflag);
+    b.dt_kpt = reinterpret_cast<const double*>(d + o_dkpt);
+    b.dt_score = reinterpret_cast<const double*>(d + o_dsc);
+    b.thr = reinterpret_cast<const double*>(d + o_thr);
+    b.kept = kept;
+    b.k_score = reinterpret_cast<double*>(d + o_kscore);
+    b.k_area = reinterpret_cast<double*>(d + o_karea);
+    b.k_cat = reinterpret_cast<int*>(d + o_kcat);
+    b.oks = reinterpret_cast<double*>(d + o_oks);
+    b.state = reinterpret_cast<unsigned char*>(d + o_state);
+    b.order = reinterpret_cast<int*>(d + o_order);
+    b.npig = reinterpret_cast<int*>(d + o_npig);
+    b.precision = reinterpret_cast<double*>(d + o_prec);
+    b.recall = reinterpret_cast<double*>(d + o_rec);
+    if (int rc = launched(coco_eval_launch(b, st), "coco_eval_launch", kCocoLaunches)) return rc;
+    CU(cudaMemcpyAsync(precision, b.precision, n_prec * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(recall, b.recall, n_rec * 8, cudaMemcpyDeviceToHost, st));
+    if (oks && oks_n) CU(cudaMemcpyAsync(oks, b.oks, (size_t)oks_n * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (oks_count) *oks_count = oks_n;
     return 0;
 }
 

@@ -1113,3 +1113,134 @@ def openpose_engine(state_dict, l2_stages=4, l1_stages=2, device_index=0, mode="
     net = NativeNet.openpose(device_index, l2_stages, l1_stages)
     net.load_state_dict_arrays(arrays)
     return PoseEngine.from_net(net, mode=mode, **engine_kwargs)
+
+
+# COCOeval's default Params for keypoints (pycocotools 2.0), as numpy computes them: iouThrs[8] is 0.8999999999999999
+COCO_IOU_THRS = np.linspace(.5, 0.95, 10)
+COCO_REC_THRS = np.linspace(.0, 1.00, 101)
+COCO_AREA_LABELS = ("all", "medium", "large")
+COCO_MAX_DETS = 20
+
+
+class CocoKeypointEval:
+    """Result of coco_keypoint_eval: COCOeval's eval['precision'] [10, 101, K, 3, 1], eval['recall'] [10, K, 3, 1] and
+    stats [10] (AP and AR at IoU .50:.95, .50, .75, medium, large), K the gt file's sorted category ids `cat_ids`.
+    oks: with export_oks, computeOks per (image id, category id) unit that has a gt and a detection."""
+
+    def __init__(self, precision, recall, cat_ids, oks=None):
+        self.precision, self.recall, self.cat_ids, self.oks = precision, recall, cat_ids, oks
+        self.stats = np.zeros((10,))
+        self._lines = []
+        for n, (ap, thr, area) in enumerate((a, t, r) for a in (1, 0) for t, r in ((None, "all"), (.5, "all"), (.75, "all"),
+                                                                                     (None, "medium"), (None, "large"))):
+            # COCOeval._summarize: the mean over the entries > -1 is numpy's, whose summation order the stats follow
+            s = self.precision if ap else self.recall
+            if thr is not None:
+                s = s[np.where(thr == COCO_IOU_THRS)[0]]
+            aind = [COCO_AREA_LABELS.index(area)]
+            s = s[:, :, :, aind, 0] if ap else s[:, :, aind, 0]
+            self.stats[n] = -1 if len(s[s > -1]) == 0 else np.mean(s[s > -1])
+            iou = "{:0.2f}:{:0.2f}".format(COCO_IOU_THRS[0], COCO_IOU_THRS[-1]) if thr is None else "{:0.2f}".format(thr)
+            self._lines.append(" {:<18} {} @[ IoU={:<9} | area={:>6s} | maxDets={:>3d} ] = {:0.3f}".format(
+                "Average Precision" if ap else "Average Recall", "(AP)" if ap else "(AR)", iou, area, COCO_MAX_DETS,
+                self.stats[n]))
+
+    def summarize(self):
+        """Prints COCOeval.summarize()'s ten lines for keypoints and returns them."""
+        for line in self._lines:
+            print(line)
+        return list(self._lines)
+
+
+def _coco_kpt(rec, what):
+    kp = rec.get("keypoints")
+    if kp is None or len(kp) != 51:
+        raise nat.B200PoseError("coco_keypoint_eval: %s: keypoints has %s values, not 51"
+                                % (what, "no" if kp is None else len(kp)))
+    return kp
+
+
+def coco_pack(gt_dataset, results, img_ids):
+    """loadRes and _prepare of coco_keypoint_eval on the host: the (category, image) units with a gt or a detection, in
+    the order b200pose_coco_kpt_eval takes them, and their packed arrays (a dict)."""
+    if not isinstance(gt_dataset, dict):
+        import json
+        with open(gt_dataset) as f:
+            gt_dataset = json.load(f)
+    results = list(results)
+    if not results:
+        raise nat.B200PoseError("coco_keypoint_eval: results is empty (pycocotools' loadRes fails on it too)")
+    gt_imgs = {im["id"] for im in gt_dataset["images"]}
+    for i, r in enumerate(results):
+        if r["image_id"] not in gt_imgs:
+            raise nat.B200PoseError("coco_keypoint_eval: results[%d]: image_id %r is not in the gt file" % (i, r["image_id"]))
+    imgs = np.unique(np.asarray(img_ids)).tolist()
+    if not imgs:
+        raise nat.B200PoseError("coco_keypoint_eval: img_ids is empty")
+    cat_ids = sorted(c["id"] for c in gt_dataset["categories"])
+    if not cat_ids:
+        raise nat.B200PoseError("coco_keypoint_eval: the gt file has no categories")
+    cat_pos = {c: k for k, c in enumerate(cat_ids)}
+    img_pos = {i: n for n, i in enumerate(imgs)}
+    units = {}        # (category index, image index) -> (gts in file order, detections in result order)
+    for ann in gt_dataset["annotations"]:
+        if ann["image_id"] in img_pos and ann["category_id"] in cat_pos:
+            units.setdefault((cat_pos[ann["category_id"]], img_pos[ann["image_id"]]), ([], []))[0].append(ann)
+    for r in results:
+        if r["image_id"] in img_pos and r["category_id"] in cat_pos:
+            units.setdefault((cat_pos[r["category_id"]], img_pos[r["image_id"]]), ([], []))[1].append(r)
+    keys = sorted(units)
+    gts = [g for k in keys for g in units[k][0]]
+    dts = [d for k in keys for d in units[k][1]]
+    return {
+        "cat_ids": cat_ids,
+        "units": [(imgs[k[1]], cat_ids[k[0]], len(units[k][0]), len(units[k][1])) for k in keys],
+        "unit_cat": np.array([k[0] for k in keys], np.int32),
+        "unit_gt0": np.cumsum([0] + [len(units[k][0]) for k in keys]).astype(np.int32),
+        "unit_dt0": np.cumsum([0] + [len(units[k][1]) for k in keys]).astype(np.int32),
+        "gt_id": np.array([g["id"] for g in gts], np.int64),
+        "gt_kpt": np.array([_coco_kpt(g, "gt annotation %r" % g["id"]) for g in gts], np.float64).reshape(-1, 51),
+        "gt_box": np.array([list(g["bbox"]) + [g["area"]] for g in gts], np.float64).reshape(-1, 5),
+        "gt_crowd": np.array([bool(g.get("iscrowd", 0)) for g in gts], np.uint8),
+        # _prepare: ignore = iscrowd (a gt's own 'ignore' is overwritten), then num_keypoints == 0 (the field)
+        "gt_ignore": np.array([bool(g.get("iscrowd", 0)) or g["num_keypoints"] == 0 for g in gts], np.uint8),
+        "dt_kpt": np.array([_coco_kpt(d, "result for image %r" % d["image_id"]) for d in dts], np.float64).reshape(-1, 51),
+        "dt_score": np.array([d["score"] for d in dts], np.float64),
+        "thr": np.concatenate([COCO_IOU_THRS, COCO_REC_THRS]),
+    }
+
+
+def coco_oks_blocks(pk, oks):
+    """The flat OKS export of b200pose_coco_kpt_eval -> {(image id, category id): [min(nd, 20), ng]} for the units
+    that have a gt and a detection."""
+    blocks, at = {}, 0
+    for img, cat, ng, nd in pk["units"]:
+        nk = min(nd, COCO_MAX_DETS)
+        if ng and nk:
+            blocks[img, cat] = oks[at:at + nk * ng].reshape(nk, ng)
+        at += nk * ng
+    return blocks
+
+
+def coco_keypoint_eval(gt_dataset, results, img_ids, device_index=0, export_oks=False):
+    """pycocotools' COCOeval(COCO(gt), COCO(gt).loadRes(results), 'keypoints') with params.imgIds = img_ids, then
+    evaluate(), accumulate() and summarize() (DESIGN.md 2.16).  gt_dataset: the parsed person_keypoints JSON, or its
+    path; results: COCO keypoint records (image_id, category_id, keypoints [51], score).  loadRes and _prepare run here
+    (coco_pack); OKS, matching and accumulation are one device call (b200pose_coco_kpt_eval).  Returns a
+    CocoKeypointEval.  Refused: an empty result list and a result for an image the gt file does not have (pycocotools
+    fails on both), keypoint lists not 51 long, and whatever the device call refuses (non-finite values, gt id 0 or
+    repeated, limits)."""
+    pk = coco_pack(gt_dataset, results, img_ids)
+    K = len(pk["cat_ids"])
+    precision = np.empty((10, 101, K, 3), np.float64)
+    recall = np.empty((10, K, 3), np.float64)
+    n_oks = sum(min(nd, COCO_MAX_DETS) * ng for _, _, ng, nd in pk["units"])
+    oks = np.empty(max(n_oks, 1), np.float64) if export_oks else None
+    p = lambda a: None if a is None or a.size == 0 else a.ctypes.data
+    nat.check(nat.lib().b200pose_coco_kpt_eval(
+        int(device_index), len(pk["units"]), K, p(pk["unit_cat"]), p(pk["unit_gt0"]), p(pk["unit_dt0"]), p(pk["gt_id"]),
+        p(pk["gt_kpt"]), 51, p(pk["gt_box"]), p(pk["gt_crowd"]), p(pk["gt_ignore"]), p(pk["dt_kpt"]), 51,
+        p(pk["dt_score"]), p(pk["thr"]), p(precision), p(recall), p(oks), oks.size if export_oks else 0,
+        None), "b200pose_coco_kpt_eval")
+    blocks = coco_oks_blocks(pk, oks) if export_oks else None
+    return CocoKeypointEval(precision[..., None], recall[..., None], pk["cat_ids"], blocks)

@@ -1,7 +1,8 @@
 """Drop-in for /root/reference/evaluate/coco_eval.py: the inference glue `get_outputs` (:80-114) and
 `handle_paf_and_heat` (:197-242), and the evaluation loop around it (SURVEY.md 8f rank 3): `append_result` (:117-154),
-`eval_coco` (:56-76), `run_eval` (:245-283).  pycocotools is imported when the evaluation loop is used (it is absent
-from the build image); the network and the post-processing run on the GPU through libb200pose.so.
+`eval_coco` (:56-76), `run_eval` (:245-283).  pycocotools scores the evaluation loop where it can be imported;
+elsewhere its COCOeval for keypoints runs on the device (engine.coco_keypoint_eval).  The network and the
+post-processing run on the GPU through libb200pose.so.
 Unlike the reference this module does not parse sys.argv at import; `cfg` is the shared lib.config node."""
 import json
 import os
@@ -89,8 +90,48 @@ def _pycocotools():
     return COCO, COCOeval
 
 
+class _CocoIndex:
+    """The part of pycocotools' COCO index run_eval uses, from the parsed annotation file: getCatIds(catNms=...),
+    getImgIds(catIds=...) (in the order of list(set(...)), as pycocotools returns them) and loadImgs."""
+
+    def __init__(self, anno_file):
+        with open(anno_file) as f:
+            self.dataset = json.load(f)
+        self.imgs = {im["id"]: im for im in self.dataset["images"]}
+        self.cat_imgs = {}
+        for ann in self.dataset["annotations"]:
+            self.cat_imgs.setdefault(ann["category_id"], []).append(ann["image_id"])
+
+    def getCatIds(self, catNms):
+        return [c["id"] for c in self.dataset["categories"] if c["name"] in catNms]
+
+    def getImgIds(self, catIds):
+        ids = set()
+        for i, c in enumerate(catIds):
+            ids = set(self.cat_imgs.get(c, [])) if i == 0 else ids & set(self.cat_imgs.get(c, []))
+        return list(ids)
+
+    def loadImgs(self, img_id):
+        return [self.imgs[img_id]]
+
+
+def _have_pycocotools():
+    try:
+        _pycocotools()
+    except ImportError:
+        return False
+    return True
+
+
 def eval_coco(outputs, annFile, imgIds):
-    """coco_eval.py:56-76: keypoint mAP of `outputs` with pycocotools (through a temporary results.json)."""
+    """coco_eval.py:56-76: keypoint mAP of `outputs` with pycocotools (through a temporary results.json).  Where
+    pycocotools cannot be imported, the same COCOeval for keypoints runs on the device
+    (engine.coco_keypoint_eval, DESIGN.md 2.16): same stats, same printed summary, no results.json."""
+    if not _have_pycocotools():
+        from ..engine import coco_keypoint_eval
+        ev = coco_keypoint_eval(annFile, outputs, imgIds)
+        ev.summarize()
+        return ev.stats[0]
     COCO, COCOeval = _pycocotools()
     with open('results.json', 'w') as f:
         json.dump(outputs, f)
@@ -172,9 +213,8 @@ def run_eval(image_dir, anno_file, vis_dir, model, preprocess):
     are processed EVAL_BATCH at a time by the fused batched engine (SURVEY.md 8f rank 3); any other module takes the
     reference's image-by-image sequence; its visualisations with a .jpg / .jpeg name are then drawn and encoded on the
     device, byte for byte cv2.imwrite(draw_humans(...)).  Records, visualisations and printed progress are the same
-    either way."""
-    COCO, _ = _pycocotools()
-    coco = COCO(anno_file)
+    either way.  Without pycocotools the annotation file is indexed here and eval_coco scores on the device."""
+    coco = _pycocotools()[0](anno_file) if _have_pycocotools() else _CocoIndex(anno_file)
     img_ids = coco.getImgIds(catIds=coco.getCatIds(catNms=['person']))
     print("Total number of validation images {}".format(len(img_ids)))
     outputs = []
