@@ -474,6 +474,38 @@ int b200pose_coco_kpt_eval(int device, int n_units, int n_cats, const int* unit_
                            double* precision, double* recall, double* oks, long long oks_cap, long long* oks_count);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3j. PNG images: replaces cv2.imread / cv2.imdecode(buf, cv2.IMREAD_COLOR) of PNG streams ahead of get_outputs
+ *     (DESIGN.md 2.17)
+ *     Every colour type and bit depth, Adam7 interlacing, any ancillary chunks and eXIf orientations 1 .. 8 are
+ *     decoded on the device, bit for bit what cv2.imdecode gives (OpenCV 4.13 with libpng 1.6 and zlib 1.3,
+ *     csrc/png_core.h): 8-bit BGR, 16-bit samples stripped to their high byte, gray below 8 bits replicated, palette
+ *     entries past PLTE black, alpha dropped.  APNG streams (acTL) are "unsupported".  A bad signature or IHDR, a
+ *     chunk running past the end, no IDAT, non-consecutive IDATs, no IEND, a palette image without PLTE, a CRC error
+ *     on a critical chunk other than IDAT, an unknown critical chunk and a frame of more than 2^28 pixels (or a side
+ *     beyond libpng's 1 000 000) are "malformed".  Both are refused before anything is enqueued, naming the image and
+ *     the reason.  Damage inside the image data is found on the device and sets status bits of the image: 1 invalid
+ *     deflate data, 2 data ends early, 4 Adler-32 mismatch, 8 IDAT CRC error, 16 invalid filter type - exactly the
+ *     streams for which cv2.imdecode returns None.
+ *
+ *     b200pose_png_info: host only.  The oriented size h x w of the decoded frame and whether the device decodes the
+ *     stream (b200pose_last_error() holds the reason when not); returns nonzero for a malformed stream.
+ *     b200pose_net_decode_pngs: n streams data[i] of sizes[i] bytes (host memory) -> their oriented BGR frames packed
+ *     back to back in `out` (host, or device when out_on_device); synchronises the stream and fails, naming the first
+ *     image, when an image's status is not 0.  One call launches 4 kernels.
+ *     b200pose_infer_pngs: b200pose_infer_raw_u8* on the decoded frames - uniform when every frame has one size,
+ *     ragged otherwise, multi-scale when scales is not null; n <= batch_cap, 2n <= 1024 with flip.  The streams are
+ *     copied when the call returns.  b200pose_post_png_status: the status bits of image img of the selected run (0
+ *     for runs not made from PNG streams), -1 when img is out of range.
+ * ---------------------------------------------------------------------------------------------------------- */
+int b200pose_png_info(const unsigned char* data, long long size, int* h, int* w, int* supported);
+int b200pose_net_decode_pngs(b200pose_net* net, const unsigned char* const* data, const long long* sizes, int n,
+                             unsigned char* out, int out_on_device, void* cuda_stream);
+int b200pose_infer_pngs(b200pose_net* net, b200pose_post* post, const unsigned char* const* data,
+                        const long long* sizes, int n, int dest_size, int factor, const double* scales, int n_scales,
+                        int mode, float thresh, int flip, void* cuda_stream);
+int b200pose_post_png_status(b200pose_post* post, int img);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

@@ -83,6 +83,10 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_net_decode_jpegs": ([vp, vp, vp, ci, vp, ci, vp], ci),
     "b200pose_infer_jpegs": ([vp, vp, vp, vp, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf, ci, vp], ci),
     "b200pose_post_jpeg_status": ([vp, ci], ci),
+    "b200pose_png_info": ([vp, ctypes.c_longlong, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)], ci),
+    "b200pose_net_decode_pngs": ([vp, vp, vp, ci, vp, ci, vp], ci),
+    "b200pose_infer_pngs": ([vp, vp, vp, vp, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf, ci, vp], ci),
+    "b200pose_post_png_status": ([vp, ci], ci),
     "b200pose_jpeg_encode_bound": ([ci, ci, ci], ctypes.c_longlong),
     "b200pose_net_encode_jpegs": ([vp, vp, ci, vp, ci, ci, ci, vp, ctypes.c_longlong, ci, vp, vp], ci),
     "b200pose_png_encode_bound": ([ci, ci], ctypes.c_longlong),

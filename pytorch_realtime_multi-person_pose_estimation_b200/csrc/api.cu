@@ -27,6 +27,7 @@
 #include "jpeg.cuh"
 #include "jpeg_enc.cuh"
 #include "png_enc.cuh"
+#include "png.cuh"
 #include "fp8_core.h"
 #include "postprocess.cuh"
 #include "resize.cuh"
@@ -478,6 +479,10 @@ struct b200pose_net {
     DevBuf<unsigned short> penc_sym;
     DevBuf<PngBlock> penc_blocks;
     DevBuf<unsigned> penc_words;
+    // PNG streams (b200pose_net_decode_pngs, b200pose_infer_pngs): the call's upload (descriptors, IDAT table, status
+    // words, IDAT chunks), the gathered zlib streams and the inflated rows
+    DevBuf<char> png_in;
+    DevBuf<unsigned char> png_zlib, png_rows;
     // fp8 mode (DESIGN.md §2.3): amax[launch * n + image] = max |bf16| (fp32 bits) launch (0 = conv1_1) stored for the
     // image; zeroed at the start of every fp8 forward
     DevBuf<unsigned> amax;
@@ -534,6 +539,9 @@ struct b200pose_post {
     // JPEG status words of a run made from JPEG streams, slot = run parity; jpeg_imgs: images copied (0: another run)
     HostBuf<unsigned> hp_jpeg[2];
     int jpeg_imgs[2] = {0, 0}, jpeg_pending = 0;
+    // the same for a run made from PNG streams
+    HostBuf<unsigned> hp_png[2];
+    int png_imgs[2] = {0, 0}, png_pending = 0;
     // scoring / prune settings of the runs submitted from now on (b200pose_post_set_params); they travel to the kernels
     // by value, so a run in flight keeps its own
     PostParams params{DefaultPostParams::paf_thresh, DefaultPostParams::paf_samples, DefaultPostParams::paf_min_above,
@@ -1522,6 +1530,7 @@ int b200pose_post_create(b200pose_post** out, int cuda_device, int batch_cap, in
         CU(p->d_ext[b].ensure((size_t)batch_cap * 2));
         CU(p->hp_ovf[b].alloc((size_t)kMaxOvfRows * 2 * batch_cap, cudaHostAllocDefault));
         CU(p->hp_jpeg[b].alloc(batch_cap, cudaHostAllocDefault));
+        CU(p->hp_png[b].alloc(batch_cap, cudaHostAllocDefault));
     }
     *out = p.release();
     return 0;
@@ -1564,6 +1573,8 @@ static int enqueue_assemble_and_fetch(b200pose_post* p, int n, cudaStream_t st, 
     p->ovf_pending = 0;
     p->jpeg_imgs[b] = p->jpeg_pending;
     p->jpeg_pending = 0;
+    p->png_imgs[b] = p->png_pending;
+    p->png_pending = 0;
     p->runs += 1;
     p->h_px.clear();
     return 0;
@@ -1627,6 +1638,7 @@ int b200pose_post_run(b200pose_post* p, const float* heat, const float* paf, int
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     p->ovf_pending = 0;      // maps from the caller: no network ran in this run
     p->jpeg_pending = 0;
+    p->png_pending = 0;
     const float *dh = heat, *dp = paf;
     if (!on_device) {
         CU(p->d_heat.ensure((size_t)n * 19 * h * w));
@@ -1772,6 +1784,10 @@ int b200pose_post_overflow(b200pose_post* p, int img) {
 int b200pose_post_jpeg_status(b200pose_post* p, int img) {
     if (!post_ready(p, img)) return -1;
     return img < p->jpeg_imgs[p->cur] ? (int)p->hp_jpeg[p->cur].p[img] : 0;
+}
+int b200pose_post_png_status(b200pose_post* p, int img) {
+    if (!post_ready(p, img)) return -1;
+    return img < p->png_imgs[p->cur] ? (int)p->hp_png[p->cur].p[img] : 0;
 }
 int b200pose_post_get_humans(b200pose_post* p, int img, float* out, int max_humans) {
     if (!post_ready(p, img)) return -1;
@@ -1969,6 +1985,7 @@ static int infer_impl(b200pose_net* net, b200pose_post* post, const void* input,
     if (int rc = check_batch(post, n)) return rc;
     post->ovf_pending = 0;
     post->jpeg_pending = 0;
+    post->png_pending = 0;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (flip) {   // the 2n batch [frames | mirrored frames] is assembled in the net's staging buffer
@@ -2348,23 +2365,139 @@ static const char* jpeg_status_name(unsigned s) {
          : s & kJpegExtraData ? "data left after the last block" : "missing or misordered restart markers";
 }
 
+// ------------------------------------------------------------------------------------------------ PNG streams
+// The streams of one b200pose_net_decode_pngs / b200pose_infer_pngs call, parsed and checked: the upload image and
+// where its tables lie, the oriented sizes [oh_0, ow_0, oh_1, ...], the packed BGR output's size, and what the device
+// buffers must hold.
+struct PngCall {
+    int n = 0, nidat = 0;
+    std::vector<char> up;
+    size_t o_ims = 0, o_idat = 0, o_status = 0, o_raw = 0;
+    std::vector<int> hw;
+    long long bytes = 0, zlib = 0, rows = 0, max_px = 0;
+    bool uniform() const {
+        for (size_t i = 2; i < hw.size(); i += 2)
+            if (hw[i] != hw[0] || hw[i + 1] != hw[1]) return false;
+        return true;
+    }
+};
+
+// Parses every stream of a call before anything is enqueued and lays out its upload: per image the bytes from its
+// first IDAT chunk's type to its last one's data, which hold every IDAT chunk's type and data.
+static int check_pngs(const unsigned char* const* data, const long long* sizes, int n, int max_n, PngCall* j) {
+    if (!data || !sizes) return fail("pngs: null stream table");
+    if (n < 1 || n > max_n) return fail("pngs: %d images (1 .. %d)", n, max_n);
+    *j = PngCall{};
+    j->n = n;
+    std::unique_ptr<PngParsed> P(new PngParsed);
+    std::vector<PngDecImage> ims(n);
+    std::vector<PngIdat> idat;
+    std::vector<std::pair<long long, long long>> spans(n);
+    long long raw = 0;
+    for (int i = 0; i < n; ++i) {
+        if (!data[i] || sizes[i] < 0) return fail("png image %d: null stream or negative size", i);
+        if (!png_parse(data[i], sizes[i], kJpegMaxPixels, P.get())) return fail("png image %d: %s", i, P->reason);
+        if (!P->supported) return fail("png image %d: %s", i, P->reason);
+        PngDecImage& im = ims[i];
+        im = P->im;
+        im.out = j->bytes;
+        im.z0 = j->zlib;
+        im.zlen = P->zlen;
+        im.f0 = j->rows;
+        im.idat0 = (int)idat.size();
+        im.nidat = (int)P->idat.size();
+        const long long beg = P->idat.front().src, end = P->idat.back().src + 4 + P->idat.back().len;
+        for (PngIdat c : P->idat) {
+            c.img = i;
+            c.src += raw - beg;
+            idat.push_back(c);
+        }
+        spans[i] = {beg, end};
+        raw += end - beg;
+        j->zlib += P->zlen;
+        j->rows += im.flen;
+        j->hw.push_back(im.oh);
+        j->hw.push_back(im.ow);
+        j->bytes += 3LL * im.oh * im.ow;
+        j->max_px = std::max(j->max_px, (long long)im.oh * im.ow);
+    }
+    j->nidat = (int)idat.size();
+    auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+    j->o_ims = 0;
+    j->o_idat = up16(j->o_ims + n * sizeof(PngDecImage));
+    j->o_status = up16(j->o_idat + idat.size() * sizeof(PngIdat));
+    j->o_raw = up16(j->o_status + n * sizeof(unsigned));
+    j->up.assign(j->o_raw + (size_t)raw + 16, 0);
+    char* u = j->up.data();
+    memcpy(u + j->o_ims, ims.data(), n * sizeof(PngDecImage));
+    memcpy(u + j->o_idat, idat.data(), idat.size() * sizeof(PngIdat));
+    for (long long at = 0, i = 0; i < n; at += spans[i].second - spans[i].first, ++i)
+        memcpy(u + j->o_raw + at, data[i] + spans[i].first, (size_t)(spans[i].second - spans[i].first));
+    return 0;
+}
+
+// Uploads the call's tables and chunks in one copy and decodes the frames into `out` (device, j.bytes); the status
+// words are at the returned device address.
+static int decode_pngs_dev(b200pose_net* net, const PngCall& j, unsigned char* out, cudaStream_t st,
+                           const unsigned** d_status) {
+    CU(net->png_in.ensure(j.up.size()));
+    CU(net->png_zlib.ensure((size_t)j.zlib + 16));
+    CU(net->png_rows.ensure((size_t)j.rows + 16));
+    CU(cudaMemcpyAsync(net->png_in.p, j.up.data(), j.up.size(), cudaMemcpyHostToDevice, st));
+    char* d = net->png_in.p;
+    PngDecBatch b;
+    b.ims = reinterpret_cast<const PngDecImage*>(d + j.o_ims);
+    b.n = j.n;
+    b.idat = reinterpret_cast<const PngIdat*>(d + j.o_idat);
+    b.nidat = j.nidat;
+    b.raw = reinterpret_cast<const unsigned char*>(d + j.o_raw);
+    b.zlib = net->png_zlib.p;
+    b.rows = net->png_rows.p;
+    b.out = out;
+    b.status = reinterpret_cast<unsigned*>(d + j.o_status);
+    b.max_px = j.max_px;
+    *d_status = b.status;
+    return launched(png_decode_launch(b, st), "png_decode_launch", kPngLaunches);
+}
+
+// The frames of j decoded into net->raw_stage, with room for their mirror images behind them when flip; the status
+// words travel to the run's slot of the post object.
+static int stage_pngs(b200pose_net* net, b200pose_post* post, const PngCall& j, int flip, cudaStream_t st,
+                      const unsigned char** d_raw) {
+    CU(net->raw_stage.ensure((size_t)j.bytes * (flip ? 2 : 1)));
+    *d_raw = net->raw_stage.p;
+    const unsigned* d_status;
+    if (int rc = decode_pngs_dev(net, j, net->raw_stage.p, st, &d_status)) return rc;
+    CU(cudaMemcpyAsync(post->hp_png[post->runs & 1].p, d_status, j.n * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    post->png_pending = j.n;
+    return 0;
+}
+
+static const char* png_status_name(unsigned s) {
+    return s & kPngBadCrc ? "a CRC error in an IDAT chunk" : s & kPngBadDeflate ? "invalid deflate data"
+         : s & kPngShortData ? "the image data ends early" : s & kPngBadAdler ? "an Adler-32 mismatch"
+         : "an invalid filter type";
+}
+
 // The fused inference of raw uint8 frames (b200pose_infer_raw_u8*): n frames of one size src_h x src_w, or of the
 // sizes src_hw (a ragged batch), are staged with their mirror images when flip, cropped for every scale and run
 // through the network.  scales null: one scale, base_size, post-processed as it is.  Else every scale s runs at
 // int(base_size * s) and its maps are resized (bicubic) to the grid of base_size, averaged and post-processed.
 // fb (b200pose_infer_frames): the frames are those of fb, converted into the staging buffer, instead of `images`;
-// jb (b200pose_infer_jpegs): those of the JPEG streams of jb, decoded into the staging buffer.
+// jb (b200pose_infer_jpegs): those of the JPEG streams of jb, decoded into the staging buffer; pc
+// (b200pose_infer_pngs): those of the PNG streams of pc.
 static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char* images, int on_device, int n,
                      int src_h, int src_w, const int* src_hw, int base_size, int factor, const double* scales,
                      int n_scales, int mode, float thresh, int flip, void* cuda_stream, const FrameBatch* fb = nullptr,
-                     const JpegCall* jb = nullptr) {
+                     const JpegCall* jb = nullptr, const PngCall* pc = nullptr) {
     if (int rc = check_infer(net, post, mode)) return rc;
-    if (!images && !fb && !jb) return fail("infer_raw: null pointer");
+    if (!images && !fb && !jb && !pc) return fail("infer_raw: null pointer");
     if (scales && (n_scales < 1 || n_scales > 16)) return fail("infer_raw: %d scales (1 .. 16)", n_scales);
     if (n < 1 || n > post->pb.batch_cap) return fail("batch %d outside 1 .. post batch_cap %d", n, post->pb.batch_cap);
     const bool ragged = src_hw != nullptr;
     post->ovf_pending = 0;
     post->jpeg_pending = 0;
+    post->png_pending = 0;
     // every scale's geometry first: an invalid frame size fails before anything is enqueued
     RawBatch base;
     if (scales && raw_batch(n, src_h, src_w, src_hw, base_size, factor, 0, &base)) return 1;
@@ -2384,6 +2517,7 @@ static int infer_raw(b200pose_net* net, b200pose_post* post, const unsigned char
     const unsigned char* d_raw;
     if (int rc = fb ? stage_frames(net, *fb, on_device, flip, st, &d_raw)
                  : jb ? stage_jpegs(net, post, *jb, flip, st, &d_raw)
+                 : pc ? stage_pngs(net, post, *pc, flip, st, &d_raw)
                       : stage_raw(net, images, on_device, (size_t)sc[0].raw, flip, st, &d_raw))
         return rc;
     // the sources and offsets of the frame table are those of every scale
@@ -2547,6 +2681,54 @@ int b200pose_infer_jpegs(b200pose_net* net, b200pose_post* post, const unsigned 
     const bool uniform = j.uniform();
     return infer_raw(net, post, nullptr, 0, n, uniform ? j.hw[0] : 0, uniform ? j.hw[1] : 0, uniform ? nullptr : j.hw.data(),
                      dest_size, factor, scales, n_scales, mode, thresh, flip, cuda_stream, nullptr, &j);
+}
+
+int b200pose_png_info(const unsigned char* data, long long size, int* h, int* w, int* supported) {
+    if (!data || !h || !w || !supported) return fail("png_info: null pointer");
+    std::unique_ptr<PngParsed> P(new PngParsed);
+    const bool ok = png_parse(data, size, kJpegMaxPixels, P.get());
+    *h = P->im.oh;
+    *w = P->im.ow;
+    *supported = ok && P->supported;
+    if (!ok) return fail("png: %s", P->reason);
+    if (!P->supported) fail("png: %s", P->reason);
+    return 0;
+}
+
+int b200pose_net_decode_pngs(b200pose_net* net, const unsigned char* const* data, const long long* sizes, int n,
+                             unsigned char* out, int out_on_device, void* cuda_stream) {
+    if (!net) return fail("null net");
+    if (!out) return fail("decode_pngs: null output");
+    PngCall j;
+    if (int rc = check_pngs(data, sizes, n, kMaxRagged, &j)) return rc;
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    unsigned char* d_out = out;
+    if (!out_on_device) {
+        CU(net->raw_stage.ensure((size_t)j.bytes));
+        d_out = net->raw_stage.p;
+    }
+    const unsigned* d_status;
+    if (int rc = decode_pngs_dev(net, j, d_out, st, &d_status)) return rc;
+    if (!out_on_device) CU(cudaMemcpyAsync(out, d_out, (size_t)j.bytes, cudaMemcpyDeviceToHost, st));
+    std::vector<unsigned> status(n);
+    CU(cudaMemcpyAsync(status.data(), d_status, n * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (int i = 0; i < n; ++i)
+        if (status[i]) return fail("png image %d: damaged image data: %s (status %u)", i, png_status_name(status[i]), status[i]);
+    return 0;
+}
+
+int b200pose_infer_pngs(b200pose_net* net, b200pose_post* post, const unsigned char* const* data,
+                        const long long* sizes, int n, int dest_size, int factor, const double* scales, int n_scales,
+                        int mode, float thresh, int flip, void* cuda_stream) {
+    if (int rc = check_infer(net, post, mode)) return rc;
+    if (flip && 2 * n > kMaxRagged) return fail("pngs: %d images with flip (2n <= %d)", n, kMaxRagged);
+    PngCall j;
+    if (int rc = check_pngs(data, sizes, n, post->pb.batch_cap, &j)) return rc;
+    const bool uniform = j.uniform();
+    return infer_raw(net, post, nullptr, 0, n, uniform ? j.hw[0] : 0, uniform ? j.hw[1] : 0, uniform ? nullptr : j.hw.data(),
+                     dest_size, factor, scales, n_scales, mode, thresh, flip, cuda_stream, nullptr, nullptr, &j);
 }
 
 // ------------------------------------------------------------------------------------------------ JPEG encoding

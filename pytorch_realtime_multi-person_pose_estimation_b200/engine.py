@@ -127,32 +127,50 @@ def frame_table(frames, format):
     return table, keep, sides == {True}, sizes
 
 
-def _blob(b):
-    """A JPEG stream (bytes, bytearray or a 1-D uint8 numpy array) as a uint8 array whose memory the library reads."""
+def _blob(b, codec="jpeg"):
+    """A JPEG or PNG stream (bytes, bytearray or a 1-D uint8 numpy array) as a uint8 array whose memory the library
+    reads."""
     a = np.frombuffer(b, np.uint8) if isinstance(b, (bytes, bytearray, memoryview)) else np.ascontiguousarray(b)
     if a.dtype != np.uint8 or a.ndim != 1:
-        raise nat.B200PoseError("jpeg: a stream is bytes or a 1-D uint8 array, got %s %s" % (a.dtype, a.shape))
+        raise nat.B200PoseError("%s: a stream is bytes or a 1-D uint8 array, got %s %s" % (codec, a.dtype, a.shape))
     return a
 
 
-def jpeg_table(blobs):
+def jpeg_table(blobs, codec="jpeg"):
     """(stream pointer array, size array, the arrays they point into) of b200pose_net_decode_jpegs / _infer_jpegs."""
-    arrs = [_blob(b) for b in blobs]
+    arrs = [_blob(b, codec) for b in blobs]
     ptrs = (ctypes.c_void_p * max(1, len(arrs)))(*[a.ctypes.data for a in arrs])
     sizes = (ctypes.c_longlong * max(1, len(arrs)))(*[a.size for a in arrs])
     return ptrs, sizes, arrs
+
+
+def png_table(blobs):
+    """(stream pointer array, size array, the arrays they point into) of b200pose_net_decode_pngs / _infer_pngs."""
+    return jpeg_table(blobs, "png")
+
+
+def _stream_info(blob, codec):
+    a = _blob(blob, codec)
+    h, w, sup = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    name = "b200pose_%s_info" % codec
+    nat.check(getattr(nat.lib(), name)(ctypes.c_void_p(a.ctypes.data), a.size, ctypes.byref(h), ctypes.byref(w),
+                                       ctypes.byref(sup)), name)
+    reason = "" if sup.value else nat.lib().b200pose_last_error().decode()
+    return h.value, w.value, bool(sup.value), reason
 
 
 def jpeg_info(blob):
     """(h, w, supported, reason) of a JPEG stream on the host (b200pose_jpeg_info): the size of the frame
     cv2.imdecode returns, EXIF orientation applied, and whether the device decodes it (reason: why not).  Raises for a
     malformed stream."""
-    a = _blob(blob)
-    h, w, sup = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    nat.check(nat.lib().b200pose_jpeg_info(ctypes.c_void_p(a.ctypes.data), a.size, ctypes.byref(h), ctypes.byref(w),
-                                           ctypes.byref(sup)), "b200pose_jpeg_info")
-    reason = "" if sup.value else nat.lib().b200pose_last_error().decode()
-    return h.value, w.value, bool(sup.value), reason
+    return _stream_info(blob, "jpeg")
+
+
+def png_info(blob):
+    """(h, w, supported, reason) of a PNG stream on the host (b200pose_png_info): the size of the frame cv2.imdecode
+    returns, eXIf orientation applied, and whether the device decodes it (APNG: not).  Raises for a malformed
+    stream."""
+    return _stream_info(blob, "png")
 
 
 def _packed_views(frames):
@@ -307,8 +325,17 @@ class NativeNet:
         uint8 HWC BGR numpy frames, or with device=True of CUDA uint8 tensors [h, w, 3] (views of one buffer, written
         on the current stream).  Raises, naming the image, for a stream the device does not decode or whose data is
         damaged."""
-        ptrs, sizes, keep = jpeg_table(blobs)
-        shapes = [jpeg_info(b)[:2] for b in keep]
+        return self._decode(blobs, "jpeg", device, stream)
+
+    def decode_pngs(self, blobs, device=False, stream=0):
+        """cv2.imdecode(blob, cv2.IMREAD_COLOR) of every PNG stream, on the device (b200pose_net_decode_pngs), as
+        decode_jpegs returns them.  Raises, naming the image, for a stream the device does not decode (APNG) or whose
+        image data is damaged (where cv2.imdecode returns None)."""
+        return self._decode(blobs, "png", device, stream)
+
+    def _decode(self, blobs, codec, device, stream):
+        ptrs, sizes, keep = jpeg_table(blobs, codec)
+        shapes = [_stream_info(b, codec)[:2] for b in keep]
         total = sum(h * w * 3 for h, w in shapes)
         if device:
             import torch
@@ -317,8 +344,9 @@ class NativeNet:
         else:
             flat = np.empty(max(1, total), np.uint8)
             ptr = flat.ctypes.data
-        nat.check(nat.lib().b200pose_net_decode_jpegs(self._h, ptrs, sizes, len(keep), ctypes.c_void_p(ptr), int(device),
-                                                      ctypes.c_void_p(stream)), "b200pose_net_decode_jpegs")
+        name = "b200pose_net_decode_%ss" % codec
+        nat.check(getattr(nat.lib(), name)(self._h, ptrs, sizes, len(keep), ctypes.c_void_p(ptr), int(device),
+                                           ctypes.c_void_p(stream)), name)
         out, at = [], 0
         for h, w in shapes:
             out.append(flat[at:at + h * w * 3].reshape(h, w, 3))
@@ -566,6 +594,13 @@ class NativePost:
             nat.check(1, "b200pose_post_jpeg_status")
         return v
 
+    def png_status(self, img):
+        """Status bits of PNG image img of the selected run (b200pose_post_png_status): 0 when its data was whole."""
+        v = int(nat.lib().b200pose_post_png_status(self._h, img))
+        if v < 0:
+            nat.check(1, "b200pose_post_png_status")
+        return v
+
     def humans(self, img):
         """float32 [k, 73]: score, 18 x (x, y, peak score, peak id | -1)."""
         L = nat.lib()
@@ -772,19 +807,29 @@ class PoseEngine:
         streams, all of which the device decodes (jpeg_info).  Returns a ticket; fetch / fetch_arrays raise, naming the
         images, when an image's entropy-coded data is damaged.  Person coordinates refer to each decoded frame's
         padded frame."""
-        ptrs, sizes, keep = jpeg_table(blobs)
-        shapes = [jpeg_info(b)[:2] for b in keep]
+        return self._infer_streams_async("jpeg", blobs, dest_size, factor, thresh, flip, scales, stream)
+
+    def infer_pngs_async(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, stream=0):
+        """PNG streams decoded on the device and run as infer_jpegs_async runs JPEG streams (b200pose_infer_pngs): at
+        most batch_cap streams, all of which the device decodes (png_info).  Returns a ticket; fetch / fetch_arrays
+        raise, naming the images, when an image's data is damaged (where cv2.imdecode returns None)."""
+        return self._infer_streams_async("png", blobs, dest_size, factor, thresh, flip, scales, stream)
+
+    def _infer_streams_async(self, codec, blobs, dest_size, factor, thresh, flip, scales, stream):
+        ptrs, sizes, keep = jpeg_table(blobs, codec)
+        shapes = [_stream_info(b, codec)[:2] for b in keep]
         arr = None if scales is None else (ctypes.c_double * len(scales))(*[float(s) for s in scales])
-        nat.check(nat.lib().b200pose_infer_jpegs(self._net_h(), self.post._h, ptrs, sizes, len(keep), int(dest_size),
-                                                 int(factor), arr, 0 if scales is None else len(scales), self.mode,
-                                                 ctypes.c_float(thresh), int(bool(flip)), ctypes.c_void_p(stream)),
-                  "b200pose_infer_jpegs")
+        name = "b200pose_infer_%ss" % codec
+        nat.check(getattr(nat.lib(), name)(self._net_h(), self.post._h, ptrs, sizes, len(keep), int(dest_size),
+                                           int(factor), arr, 0 if scales is None else len(scales), self.mode,
+                                           ctypes.c_float(thresh), int(bool(flip)), ctypes.c_void_p(stream)), name)
         pads = [nat.crop_geometry(h, w, dest_size, factor)[2] for h, w in shapes]
         if len(set(pads)) == 1:
             t = self._remember(len(keep), pads[0][0], pads[0][1])
         else:
             t = self._remember(len(keep), [p[0] for p in pads], [p[1] for p in pads])
-        self._jpeg_runs = {k for k in (self.__dict__.get("_jpeg_runs") or ()) if k >= t - 1} | {t}
+        runs = "_%s_runs" % codec
+        setattr(self, runs, {k for k in (self.__dict__.get(runs) or ()) if k >= t - 1} | {t})
         return t
 
     def check_jpegs(self, n, names=None):
@@ -793,6 +838,13 @@ class PoseEngine:
         if bad:
             raise nat.B200PoseError("jpeg: damaged entropy-coded data in image(s) %s (status bits: 1 invalid code, 2 data "
                                     "ends early, 4 data left over, 8 restart markers)" % bad)
+
+    def check_pngs(self, n, names=None):
+        """Raises naming the images (names[k], default k) of the selected run whose PNG image data was damaged."""
+        bad = [((names[k] if names else k), s) for k, s in ((k, self.post.png_status(k)) for k in range(n)) if s]
+        if bad:
+            raise nat.B200PoseError("png: damaged image data in image(s) %s (status bits: 1 invalid deflate data, 2 data "
+                                    "ends early, 4 Adler-32 mismatch, 8 IDAT CRC error, 16 invalid filter type)" % bad)
 
     def infer_jpegs_arrays(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None):
         """infer_jpegs, but per image the raw person rows (float32 [k, 73], pixel coordinates of the padded frame)."""
@@ -804,26 +856,40 @@ class PoseEngine:
         (jpeg_info); streams the device does not decode (progressive, CMYK, ...) are decoded by cv2.imdecode and run
         through infer_images - a frame's result does not depend on its batch.  Malformed streams raise, and so do
         streams whose entropy-coded data is damaged, naming the image."""
+        return self._infer_streams("jpeg", blobs, dest_size, factor, thresh, flip, scales, _arrays)
+
+    def infer_pngs_arrays(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None):
+        """infer_pngs, but per image the raw person rows (float32 [k, 73], pixel coordinates of the padded frame)."""
+        return self.infer_pngs(blobs, dest_size, factor, thresh, flip, scales, _arrays=True)
+
+    def infer_pngs(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, _arrays=False):
+        """infer_images([cv2.imdecode(b, cv2.IMREAD_COLOR) for b in blobs]) with the PNG decoding on the device, as
+        infer_jpegs does for JPEG streams: batches by plan_ragged_batches on the decoded padded sizes (png_info), APNG
+        streams decoded by cv2.imdecode and run through infer_images.  Malformed streams raise, and so do streams whose
+        image data is damaged, naming the image."""
+        return self._infer_streams("png", blobs, dest_size, factor, thresh, flip, scales, _arrays)
+
+    def _infer_streams(self, codec, blobs, dest_size, factor, thresh, flip, scales, _arrays):
         infos = []
         for i, b in enumerate(blobs):
             try:
-                infos.append(jpeg_info(b))
+                infos.append(_stream_info(b, codec))
             except nat.B200PoseError as e:
-                raise nat.B200PoseError("infer_jpegs: image %d: %s" % (i, e)) from None
+                raise nat.B200PoseError("infer_%ss: image %d: %s" % (codec, i, e)) from None
         dev = [i for i, inf in enumerate(infos) if inf[2]]
         out = [None] * len(blobs)
         pads = [nat.crop_geometry(infos[i][0], infos[i][1], dest_size, factor)[2] for i in dev]
         for part in plan_ragged_batches(pads, self.post.batch_cap):
             idx = [dev[k] for k in part]
-            self.infer_jpegs_async([blobs[i] for i in idx], dest_size, factor, thresh, flip, scales)
+            self._infer_streams_async(codec, [blobs[i] for i in idx], dest_size, factor, thresh, flip, scales, 0)
             self.post.sync()
-            self.check_jpegs(len(idx), idx)
+            (self.check_jpegs if codec == "jpeg" else self.check_pngs)(len(idx), idx)
             for i, humans in zip(idx, self.fetch_arrays() if _arrays else self.fetch()):
                 out[i] = humans.copy() if _arrays else humans
         rest = [i for i, inf in enumerate(infos) if not inf[2]]
         if rest:
             import cv2
-            frames = [cv2.imdecode(_blob(blobs[i]), cv2.IMREAD_COLOR) for i in rest]
+            frames = [cv2.imdecode(_blob(blobs[i], codec), cv2.IMREAD_COLOR) for i in rest]
             for i, humans in zip(rest, self.infer_images(frames, dest_size, factor, thresh, flip, scales, _arrays)):
                 out[i] = humans
         return out
@@ -963,11 +1029,13 @@ class PoseEngine:
         return [humans_to_dicts(self.post.humans(i), _at(W, i), _at(H, i)) for i in range(n)]
 
     def _check_jpeg_run(self, ticket, n):
-        """A run made from JPEG streams (infer_jpegs_async) raises, whatever `check` says, when an image's entropy-coded
-        data was damaged: its persons are never handed back in silence."""
+        """A run made from JPEG or PNG streams (infer_jpegs_async, infer_pngs_async) raises, whatever `check` says, when
+        an image's data was damaged: its persons are never handed back in silence."""
         t = self.post.last_ticket() if ticket is None else ticket
         if t in (self.__dict__.get("_jpeg_runs") or ()):
             self.check_jpegs(n)
+        if t in (self.__dict__.get("_png_runs") or ()):
+            self.check_pngs(n)
 
     def _check_overflow(self, n):
         if self.mode == nat.MODE_FP16:      # whatever `check` says: overflowed maps are never handed back in silence
