@@ -195,6 +195,27 @@ typedef struct b200pose_post_params {
 int b200pose_post_default_params(b200pose_post_params* out);
 int b200pose_post_set_params(b200pose_post* post, const b200pose_post_params* p);
 int b200pose_post_get_params(b200pose_post* post, b200pose_post_params* out);
+/* Peak refinement (NMS, lib/utils/paf_to_pose.py:67-145) and the up-sampling factor f from the maps to the peaks.
+ *   B200POSE_REFINE_CUBIC       : the clipped 5x5 window around each peak, cv2.resize(INTER_CUBIC) by f, first arg-max;
+ *                                 position f * window origin + arg-max, score the value there (the default)
+ *   B200POSE_REFINE_CUBIC_GAUSS : as CUBIC, the resized patch first smoothed by scipy.ndimage.gaussian_filter(sigma=3)
+ *                                 (bool_gaussian_filt=True); the score is the smoothed value
+ *   B200POSE_REFINE_NONE        : no refinement (bool_refine_center=False): position (p + 0.5) f - 0.5 truncated to an
+ *                                 int as pafprocess does, score the low-resolution map value
+ *   b200pose_post_set_refine : the mode of the runs submitted after the call (b200pose_post_run, _run_scaled and every
+ *                              fused entry point); each run keeps its own.  An invalid mode is refused and the setting
+ *                              stays as it was
+ *   b200pose_post_get_refine : the mode the next run will use, < 0 on error
+ *   b200pose_post_run_scaled : b200pose_post_run with the factor as an argument, 1 .. 16; b200pose_post_run is this call
+ *                              with 8.  PAF scoring reads the maps at (y / f, x / f) and h * f, w * f must not exceed
+ *                              16384.  Fused runs always use 8, the network's stride. */
+#define B200POSE_REFINE_NONE 0
+#define B200POSE_REFINE_CUBIC 1
+#define B200POSE_REFINE_CUBIC_GAUSS 2
+int b200pose_post_set_refine(b200pose_post* post, int mode);
+int b200pose_post_get_refine(b200pose_post* post);
+int b200pose_post_run_scaled(b200pose_post* post, const float* heat, const float* paf, int on_device, int layout, int n,
+                             int h, int w, int upsample, float thresh, void* cuda_stream);
 /* Every run copies its results (person rows, counts, status) to pinned host memory by itself, on a second stream right
  * after the person assembly, into one of two slots (run parity) - so a caller may submit run i+1 before reading run i
  * (at most two runs in flight).  The getters below read the selected slot.

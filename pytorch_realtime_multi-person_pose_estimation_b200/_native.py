@@ -45,6 +45,9 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_post_create": ([ctypes.POINTER(vp), ci, ci, ci, ci], ci),
     "b200pose_post_destroy": ([vp], None),
     "b200pose_post_run": ([vp, vp, vp, ci, ci, ci, ci, ci, cf, vp], ci),
+    "b200pose_post_run_scaled": ([vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp], ci),
+    "b200pose_post_set_refine": ([vp, ci], ci),
+    "b200pose_post_get_refine": ([vp], ci),
     "b200pose_post_sync": ([vp], ci),
     "b200pose_post_default_params": ([vp], ci),
     "b200pose_post_set_params": ([vp, vp], ci),

@@ -30,6 +30,7 @@
 #include "png.cuh"
 #include "fp8_core.h"
 #include "postprocess.cuh"
+#include "refine_core.h"
 #include "resize.cuh"
 #include "tta.cuh"
 
@@ -549,6 +550,8 @@ struct b200pose_post {
     // grids of limb_score_kernel / range_sort_kernel for the runs submitted from now on, 0 = the defaults
     // (b200pose_post_set_grids, a test hook: the results never depend on them)
     int score_blocks = 0, sort_blocks = 0;
+    // peak refinement of the runs submitted from now on (b200pose_post_set_refine), passed to the kernels by value
+    int refine = B200POSE_REFINE_CUBIC;
     // the second stream's work still reads the buffers; post_free is null-safe (post_alloc zeroes pb first)
     ~b200pose_post() { if (s2) cudaStreamSynchronize(s2); post_free(pb); }
 };
@@ -1586,9 +1589,14 @@ static int check_batch(const b200pose_post* p, int n) {
 }
 
 // ext: device extents table of a ragged batch (h x w is then its canvas at the maps' resolution), or null
+// up: the factor from the maps to the peak coordinates (8 for every fused run)
 static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_paf, int layout, int n, int h, int w,
-                        float thresh, cudaStream_t st, const int* ext = nullptr) {
+                        float thresh, cudaStream_t st, const int* ext = nullptr, int up = 8) {
     if (int rc = check_batch(p, n)) return rc;
+    if (up < 1 || up > kMaxUpsample) return fail("post_run: upsample must be 1 .. %d, got %d", kMaxUpsample, up);
+    if ((long)h * up > kMaxUpCoord || (long)w * up > kMaxUpCoord)
+        return fail("post_run: maps of %d x %d at upsample %d give %ld x %ld pixels, above %d", h, w, up, (long)h * up,
+                    (long)w * up, kMaxUpCoord);
     const int slot = (int)(p->runs & 1);
     if (p->have_ld[slot]) CU(cudaStreamWaitEvent(st, p->ev_ld[slot], 0));   // run i-2 is done with this slot
     if (ext) {
@@ -1613,16 +1621,16 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
     cudaError_t e;
     const PostParams* prm = run_params(p);
     if (layout == 0) {
-        e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, (long)h * w, w, 1, h, w, thresh, ps, ext);
+        e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, (long)h * w, w, 1, h, w, thresh, ps, ext, up, p->refine);
         if (launched(e, "post_peaks")) return 1;
-        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * 8, w, h, ps, ext, prm,
-                       p->score_blocks, p->sort_blocks);
+        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, (long)h * w, w, 1, 3, h * up, w, h, ps, ext, prm,
+                       p->score_blocks, p->sort_blocks, up);
     } else {
         if (ext) return fail("post_run: ragged batches need the planar (layout 0) maps");
-        e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, 1, (long)w * 19, 19, h, w, thresh, ps);
+        e = post_peaks(p->pb, n, d_heat, (long)19 * h * w, 1, (long)w * 19, 19, h, w, thresh, ps, nullptr, up, p->refine);
         if (launched(e, "post_peaks")) return 1;
-        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * 8, w, h, ps, nullptr, prm,
-                       p->score_blocks, p->sort_blocks);
+        e = post_limbs(p->pb, n, d_paf, (long)38 * h * w, 1, (long)w * 38, 38, 3, h * up, w, h, ps, nullptr, prm,
+                       p->score_blocks, p->sort_blocks, up);
     }
     if (launched(e, "post_limbs")) return 1;
     CU(cudaEventRecord(p->ev_ld[slot], ps));
@@ -1633,7 +1641,17 @@ static int post_run_dev(b200pose_post* p, const float* d_heat, const float* d_pa
 
 int b200pose_post_run(b200pose_post* p, const float* heat, const float* paf, int on_device, int layout, int n, int h,
                       int w, float thresh, void* cuda_stream) {
+    return b200pose_post_run_scaled(p, heat, paf, on_device, layout, n, h, w, 8, thresh, cuda_stream);
+}
+
+int b200pose_post_run_scaled(b200pose_post* p, const float* heat, const float* paf, int on_device, int layout, int n,
+                             int h, int w, int upsample, float thresh, void* cuda_stream) {
     if (!p) return fail("null post");
+    if (upsample < 1 || upsample > kMaxUpsample)
+        return fail("post_run: upsample must be 1 .. %d, got %d", kMaxUpsample, upsample);
+    if ((long)h * upsample > kMaxUpCoord || (long)w * upsample > kMaxUpCoord)
+        return fail("post_run: maps of %d x %d at upsample %d give %ld x %ld pixels, above %d", h, w, upsample,
+                    (long)h * upsample, (long)w * upsample, kMaxUpCoord);
     CU(cudaSetDevice(p->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     p->ovf_pending = 0;      // maps from the caller: no network ran in this run
@@ -1647,7 +1665,21 @@ int b200pose_post_run(b200pose_post* p, const float* heat, const float* paf, int
         CU(cudaMemcpyAsync(p->d_paf.p, paf, (size_t)n * 38 * h * w * 4, cudaMemcpyHostToDevice, st));
         dh = p->d_heat.p; dp = p->d_paf.p;
     }
-    return post_run_dev(p, dh, dp, layout, n, h, w, thresh, st);
+    return post_run_dev(p, dh, dp, layout, n, h, w, thresh, st, nullptr, upsample);
+}
+
+int b200pose_post_set_refine(b200pose_post* p, int mode) {
+    if (!p) return fail("null post");
+    if (mode < B200POSE_REFINE_NONE || mode > B200POSE_REFINE_CUBIC_GAUSS)
+        return fail("post_set_refine: mode must be %d (none), %d (cubic) or %d (cubic+gauss), got %d", B200POSE_REFINE_NONE,
+                    B200POSE_REFINE_CUBIC, B200POSE_REFINE_CUBIC_GAUSS, mode);
+    p->refine = mode;
+    return 0;
+}
+
+int b200pose_post_get_refine(b200pose_post* p) {
+    if (!p) return fail("null post");
+    return p->refine;
 }
 
 int b200pose_post_default_params(b200pose_post_params* out) {

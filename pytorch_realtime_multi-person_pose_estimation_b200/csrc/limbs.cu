@@ -164,9 +164,22 @@ struct PlanePaf {          // the limb's two PAF planes in shared memory: channe
     __device__ __forceinline__ float at(int c, int y, int x) const { return pl[c * hw + (y >> 3) * lw + (x >> 3)]; }
 };
 
+// the same planes read at any integer factor (UpIndex: a shift for powers of two, a division otherwise)
+struct PlanePafF {
+    const float* pl;
+    int lw, hw;
+    UpIndex up;
+    __device__ __forceinline__ float at(int c, int y, int x) const { return pl[c * hw + up(y) * lw + up(x)]; }
+};
+__device__ __forceinline__ PlanePaf plane_paf(const float* pl, int lw, int hw, const PafView&) { return PlanePaf{pl, lw, hw}; }
+__device__ __forceinline__ PlanePafF plane_paf(const float* pl, int lw, int hw, const PafViewF& v) {
+    return PlanePafF{pl, lw, hw, v.up};
+}
+
 // Prm: DefaultPostParams (the instantiation of default runs) or PostParams (run-time settings, post_limbs)
-template <class Prm>
-__global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers pb, PafView paf0, long p_img, int h_up0,
+// View: PafView (factor 8, or the legacy up-sampled maps; the instantiations of default runs) or PafViewF (any factor)
+template <class Prm, class View = PafView>
+__global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers pb, View paf0, long p_img, int h_up0,
                                                                    int lw, int lh, int paf_in_smem, int n_limbs,
                                                                    const int* __restrict__ ext, Prm prm) {
     extern __shared__ float s_planes[];
@@ -202,7 +215,7 @@ __global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers p
         const int pa = c_lparts[limb][0], pbp = c_lparts[limb][1];
         const int c1 = c_lpaf[limb][0], c2 = c_lpaf[limb][1];
         const int h_up = ext ? __ldg(ext + 2 * img) : h_up0;     // ragged batch: the image's own padded height
-        PafView paf = paf0;
+        View paf = paf0;
         paf.base += img * p_img;
         if (paf_in_smem && staged != li) {
             __syncthreads();                 // every warp is done with the planes of the previous limb
@@ -231,7 +244,7 @@ __global__ void __launch_bounds__(kScoreThreads) limb_score_kernel(PostBuffers p
             unsigned long long* dst = pb.pool + pl.region + start;
             long p = start + lane;
             int a = (int)(p / nb), b = (int)(p - (long)a * nb);
-            const PlanePaf pp{s_planes, lw, hw};
+            const auto pp = plane_paf(s_planes, lw, hw, paf);
 #pragma unroll 1
             for (int it = 0; it < kSubPairs / 32; ++it, p += 32) {
                 float sc = 0.f;
@@ -813,10 +826,13 @@ __global__ void __launch_bounds__(kGreedyThreads) limb_greedy_kernel(PostBuffers
 
 cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long p_img, long p_ch, long p_y, long p_x,
                        int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext, const PostParams* prm,
-                       int score_blocks, int sort_blocks) {
+                       int score_blocks, int sort_blocks, int up) {
     if (batch > pb.batch_cap) return cudaErrorInvalidValue;
     if (pb.cand_smem_cap != kS) return cudaErrorInvalidValue;
+    if (up < 1 || up > 16 || (shift == 3 && up != 8 && ext)) return cudaErrorInvalidValue;
+    const bool any_up = shift == 3 && up != 8;
     PafView pv{paf, p_ch, p_y, p_x, shift};
+    const PafViewF pvf{paf, p_ch, p_y, p_x, up_index(up)};
     limb_plan_kernel<<<1, 1024, 0, s>>>(pb, batch);
     B2P_TRY(cudaGetLastError());
     int in_smem = 0;
@@ -830,7 +846,16 @@ cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long 
     B2P_TRY(cudaGetDevice(&dev));
     B2P_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     if (score_blocks == 0) score_blocks = sms * 6;
-    if (!prm) {
+    static DynSmemOptIn optin_score_f, optin_score_fp;
+    if (any_up && !prm) {
+        B2P_TRY(optin_score_f.ensure(limb_score_kernel<DefaultPostParams, PafViewF>, smem));
+        limb_score_kernel<<<score_blocks, kScoreThreads, smem, s>>>(pb, pvf, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
+                                                                  ext, DefaultPostParams{});
+    } else if (any_up) {
+        B2P_TRY(optin_score_fp.ensure(limb_score_kernel<PostParams, PafViewF>, smem));
+        limb_score_kernel<<<score_blocks, kScoreThreads, smem, s>>>(pb, pvf, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
+                                                                  ext, *prm);
+    } else if (!prm) {
         B2P_TRY(optin_score.ensure(limb_score_kernel<DefaultPostParams>, smem));
         limb_score_kernel<<<score_blocks, kScoreThreads, smem, s>>>(pb, pv, p_img, h_up, lw, lh, in_smem, batch * kNumLimb,
                                                                   ext, DefaultPostParams{});

@@ -52,6 +52,25 @@ struct PafView {
     B2P_HD float at(int c, int y, int x) const { return base[c * sc + (long)(y >> shift) * sy + (long)(x >> shift) * sx]; }
 };
 
+// Up-sampled coordinate -> low-resolution index at an integer factor f: cv2.resize(INTER_NEAREST) by f reads source
+// pixel x // f (checked for f = 1 .. 16).  A shift when f is a power of two, a division otherwise.
+struct UpIndex {
+    int f, shift;     // shift < 0: divide by f
+    B2P_HD int operator()(int v) const { return shift >= 0 ? v >> shift : v / f; }
+};
+inline UpIndex up_index(int f) {
+    int sh = 0;
+    while ((1 << sh) < f) ++sh;
+    return UpIndex{f, (1 << sh) == f ? sh : -1};
+}
+// PafView at any factor (the kernels of default runs keep PafView and its shift of 3)
+struct PafViewF {
+    const float* base;
+    long sc, sy, sx;
+    UpIndex up;
+    B2P_HD float at(int c, int y, int x) const { return base[c * sc + (long)up(y) * sy + (long)up(x) * sx]; }
+};
+
 // roundpaf (pafprocess.cpp:240-242) is `(int)(v + 0.5)` evaluated in DOUBLE.  For 0 <= v <= 16384 the single-precision
 // form gives the same integer for every float except v = 0x1.fffffep-2 (largest float below 0.5, where v + 0.5f rounds
 // up to 1.0f) - checked exhaustively over all 1.18e9 floats of that range - so one compare keeps it exact while avoiding

@@ -8,6 +8,7 @@
 
 #include "host_util.h"
 #include "postprocess.cuh"
+#include "refine_core.h"
 
 namespace b2p {
 
@@ -99,6 +100,9 @@ __device__ __forceinline__ void refine_interior_slots(const float* plane, int w,
     }
 }
 
+// kRefine8: the fused x8 cubic refinement below (the default run); false: stop after the compaction, leaving the
+// low-resolution peaks and their map values for refine_kernel (any factor, any refinement mode).
+template <bool kRefine8>
 __global__ void __launch_bounds__(kPeakThreads, 512 / kPeakThreads) peaks_kernel(PostBuffers pb, const float* __restrict__ heat, long h_img,
                                                              long h_ch, long h_y, long h_x, int h_max, int w_max, float thresh,
                                                              const int* __restrict__ ext) {
@@ -158,6 +162,10 @@ __global__ void __launch_bounds__(kPeakThreads, 512 / kPeakThreads) peaks_kernel
         n = cap;
     }
     if (tid == 0) pb.counts[img * kNumPart + part] = n;
+    if (!kRefine8) {
+        for (int pk = tid; pk < n; pk += kPeakThreads) ps[pk] = plane[py[pk] * w + px[pk]];
+        return;
+    }
 
     // refinement: 5x5 window (clipped) -> x8 bicubic (separable, OpenCV's operation order) -> first arg-max.
     // Peaks whose window is not clipped (all but the two outermost rows / columns of the map) take the fast path: FOUR
@@ -271,6 +279,85 @@ __global__ void __launch_bounds__(kPeakThreads, 512 / kPeakThreads) peaks_kernel
             px[pk] = 8 * x_min + ax;     // == (x+0.5)*8-0.5 + (ax - ((x-x_min+0.5)*8-0.5)), paf_to_pose.py:126-139
             py[pk] = 8 * y_min + ay;
             ps[pk] = best;
+        }
+    }
+}
+
+// ------------------------------------------------------------------ refinement at any factor / mode
+// One warp per peak of (part, image) = (blockIdx.y, blockIdx.z), after peaks_kernel<false>: the window goes to shared
+// memory, then (cubic) the up-sampled patch is evaluated element by element straight into the arg-max, or (cubic+gauss)
+// it is written to `up`, the axis-0 pass to `tmp` and the axis-1 pass feeds the arg-max.  Lanes visit their row-major
+// indices in increasing order, so a strict compare per lane and rf_better across lanes give the first maximum.
+constexpr int kRefineWinFloats = 32;
+
+__global__ void __launch_bounds__(256) refine_kernel(PostBuffers pb, const float* __restrict__ heat, long h_img, long h_ch,
+                                                     long h_y, long h_x, int h_max, int w_max, const int* __restrict__ ext,
+                                                     int f, int mode) {
+    extern __shared__ float sm_r[];
+    const int part = blockIdx.y, img = blockIdx.z;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    const int h = ext ? __ldg(ext + 2 * img) / f : h_max, w = ext ? __ldg(ext + 2 * img + 1) / f : w_max;
+    const int cap = pb.peak_cap;
+    const int n = pb.counts[img * kNumPart + part];
+    int* px = pb.peak_x + ((long)img * kNumPart + part) * cap;
+    int* py = pb.peak_y + ((long)img * kNumPart + part) * cap;
+    float* ps = pb.peak_s + ((long)img * kNumPart + part) * cap;
+    const int area = (2 * kRefineWin + 1) * (2 * kRefineWin + 1) * f * f;
+    float* win = sm_r + (long)warp * (kRefineWinFloats + (mode == kRefineCubicGauss ? 2 * area : 0));
+    float* up = win + kRefineWinFloats;
+    float* tmp = up + area;
+    const float* src = heat + img * h_img + part * h_ch;
+    for (int pk = blockIdx.x * nwarps + warp; pk < n; pk += gridDim.x * nwarps) {
+        const int x = px[pk], y = py[pk];
+        __syncwarp();
+        if (mode == kRefineNone) {      // score: the map value peaks_kernel<false> left
+            if (lane == 0) { px[pk] = rf_unrefined_coord(x, f); py[pk] = rf_unrefined_coord(y, f); }
+            continue;
+        }
+        const RefineWin rw = rf_window(x, y, h, w);
+        if (lane < rw.pw * rw.ph) {
+            const int r = lane / rw.pw, c = lane - r * rw.pw;
+            win[lane] = src[(long)(rw.y0 + r) * h_y + (long)(rw.x0 + c) * h_x];
+        }
+        __syncwarp();
+        const int W = rw.pw * f, HW = rw.ph * f * W;
+        float bv = -INFINITY;
+        int bi = 0x7fffffff;
+        if (mode == kRefineCubic) {
+            for (int i = lane; i < HW; i += 32) {
+                const int Y = i / W, X = i - Y * W;
+                const float v = rf_up_at(win, rw.pw, rw.ph, rw.pw, f, Y, X);
+                if (v > bv) { bv = v; bi = i; }
+            }
+        } else {
+            const int H = rw.ph * f;
+            for (int i = lane; i < HW; i += 32) {
+                const int Y = i / W, X = i - Y * W;
+                up[i] = rf_up_at(win, rw.pw, rw.ph, rw.pw, f, Y, X);
+            }
+            __syncwarp();
+            for (int i = lane; i < HW; i += 32) {
+                const int Y = i / W, X = i - Y * W;
+                tmp[i] = rf_gauss_at(up + X, W, H, Y);          // axis 0
+            }
+            __syncwarp();
+            for (int i = lane; i < HW; i += 32) {
+                const int Y = i / W, X = i - Y * W;
+                const float v = rf_gauss_at(tmp + Y * W, 1, W, X);     // axis 1
+                if (v > bv) { bv = v; bi = i; }
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (rf_better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+        }
+        if (lane == 0) {
+            const int ay = bi / W, ax = bi - ay * W;
+            px[pk] = f * rw.x0 + ax;     // == (x+0.5)f-0.5 + (ax - ((x-x0+0.5)f-0.5)), paf_to_pose.py:129-140
+            py[pk] = f * rw.y0 + ay;
+            ps[pk] = bv;
         }
     }
 }
@@ -454,14 +541,31 @@ void post_free(PostBuffers& pb) {
 }
 
 cudaError_t post_peaks(const PostBuffers& pb, int batch, const float* heat, long h_img, long h_ch, long h_y, long h_x,
-                       int h, int w, float thresh, cudaStream_t s, const int* ext) {
+                       int h, int w, float thresh, cudaStream_t s, const int* ext, int up, int refine) {
     if (batch > pb.batch_cap) return cudaErrorInvalidValue;
+    if (up < 1 || up > kMaxUpsample || refine < kRefineNone || refine > kRefineCubicGauss) return cudaErrorInvalidValue;
+    if ((long)h * up > kMaxUpCoord || (long)w * up > kMaxUpCoord || (ext && up != 8)) return cudaErrorInvalidValue;
     const size_t smem = ((size_t)h * w + (kPeakThreads / 32) * 5 * kHorStride) * sizeof(float);
     if (smem > 200 * 1024) return cudaErrorInvalidValue;
-    static DynSmemOptIn optin;
-    B2P_TRY(optin.ensure(peaks_kernel, smem));
     B2P_TRY(cudaMemsetAsync(pb.status, 0, batch * sizeof(int), s));
-    peaks_kernel<<<dim3(kNumPart, batch), kPeakThreads, smem, s>>>(pb, heat, h_img, h_ch, h_y, h_x, h, w, thresh, ext);
+    if (up == 8 && refine == kRefineCubic) {
+        static DynSmemOptIn optin;
+        B2P_TRY(optin.ensure(peaks_kernel<true>, smem));
+        peaks_kernel<true><<<dim3(kNumPart, batch), kPeakThreads, smem, s>>>(pb, heat, h_img, h_ch, h_y, h_x, h, w, thresh, ext);
+        return cudaGetLastError();
+    }
+    static DynSmemOptIn optin_det, optin_ref;
+    B2P_TRY(optin_det.ensure(peaks_kernel<false>, smem));
+    peaks_kernel<false><<<dim3(kNumPart, batch), kPeakThreads, smem, s>>>(pb, heat, h_img, h_ch, h_y, h_x, h, w, thresh, ext);
+    B2P_TRY(cudaGetLastError());
+    // warps per block: as many as fit 96 KB of patches (one at f = 16 with the Gaussian's second buffer)
+    const size_t per_warp = (kRefineWinFloats + (refine == kRefineCubicGauss ? 2 * 25 * up * up : 0)) * sizeof(float);
+    int nw = (int)(96 * 1024 / per_warp);
+    nw = nw < 1 ? 1 : (nw > 8 ? 8 : nw);
+    const int gx = (pb.peak_cap + nw - 1) / nw < 4 ? (pb.peak_cap + nw - 1) / nw : 4;
+    B2P_TRY(optin_ref.ensure(refine_kernel, nw * per_warp));
+    refine_kernel<<<dim3(gx, kNumPart, batch), 32 * nw, nw * per_warp, s>>>(pb, heat, h_img, h_ch, h_y, h_x, h, w, ext, up,
+                                                                            refine);
     return cudaGetLastError();
 }
 

@@ -80,16 +80,20 @@ void post_free(PostBuffers& pb);
 
 // heat: fp32, value(img, part, y, x) = heat[img*h_img + part*h_ch + y*h_y + x*h_x]; low-res (h x w).
 // ext (ragged batch, DESIGN.md §1) or null: image i covers only (ext[2 i] / 8) x (ext[2 i + 1] / 8) of the h x w canvas.
+// up: the up-sampling factor 1 .. 16 (8 with ext), h * up and w * up at most 16384; refine: a RefineMode (refine_core.h).
+// up = 8 with kRefineCubic runs the fused x8 kernel; every other setting runs NMS alone, then refine_kernel per peak.
 cudaError_t post_peaks(const PostBuffers& pb, int batch, const float* heat, long h_img, long h_ch, long h_y, long h_x,
-                       int h, int w, float thresh, cudaStream_t s, const int* ext = nullptr);
+                       int h, int w, float thresh, cudaStream_t s, const int* ext = nullptr, int up = 8, int refine = 1);
 // paf: fp32 view per image: base + img*p_img, strides (p_ch, p_y, p_x), shift (3: low-res, 0: already upsampled).
+// up: with shift 3, the factor from the maps to the peak coordinates (8: the default kernels, else 1 .. 16).
 // ext (ragged batch) or null: h_up of image i is its own padded height ext[2 i].
 // prm: the scoring settings, copied into the launch; null = the reference's constants (the DefaultPostParams kernel).
 // score_blocks / sort_blocks: the grids of the two work-queue kernels, limb_score_kernel and range_sort_kernel; 0 = the
 // defaults (SMs x 6, and min(batch x 19, SMs x 3)).  Results do not depend on them (b200pose_post_set_grids).
 cudaError_t post_limbs(const PostBuffers& pb, int batch, const float* paf, long p_img, long p_ch, long p_y,
                                     long p_x, int shift, int h_up, int lw, int lh, cudaStream_t s, const int* ext = nullptr,
-                                    const PostParams* prm = nullptr, int score_blocks = 0, int sort_blocks = 0);
+                                    const PostParams* prm = nullptr, int score_blocks = 0, int sort_blocks = 0,
+                                    int up = 8);
 // Test hook (limbs.cu): exact std::sort of n host keys through the global-memory partition + shared-memory range kernels.
 // sort_blocks: range_sort_kernel's grid, 0 = SMs x 3.
 cudaError_t post_debug_sort(const PostBuffers& pb, const unsigned long long* keys, int n, unsigned long long* out,

@@ -460,6 +460,10 @@ class NativeNet:
             pass
 
 
+# NativePost.set_refine's modes -> B200POSE_REFINE_* (include/b200pose.h)
+REFINE_MODES = {"none": 0, "cubic": 1, "gauss": 2}
+
+
 class NativePost:
     """Owns a b200pose_post handle (fused NMS + PAF scoring + matching + assembly)."""
 
@@ -514,10 +518,31 @@ class NativePost:
             nat.check(1, "b200pose_post_debug_connections")
         return a[:k].copy(), b[:k].copy(), s[:k].copy()
 
-    def run(self, heat_ptr, paf_ptr, on_device, layout, n, h, w, thresh, stream=0):
-        nat.check(nat.lib().b200pose_post_run(self._h, ctypes.c_void_p(heat_ptr), ctypes.c_void_p(paf_ptr), int(on_device),
-                                              layout, n, h, w, ctypes.c_float(thresh), ctypes.c_void_p(stream)),
-                  "b200pose_post_run")
+    def set_refine(self, mode):
+        """Peak refinement of the runs submitted from now on (fused runs included), include/b200pose.h section 2:
+        'cubic' (the default: x f bicubic patch, first arg-max), 'gauss' (the patch smoothed by gaussian_filter(sigma=3)
+        first) or 'none' (the low-resolution peak, rescaled).  Runs already submitted keep theirs.  Anything else raises
+        B200PoseError and leaves the mode unchanged."""
+        if mode not in REFINE_MODES:
+            raise nat.B200PoseError("set_refine: mode must be one of %s, got %r" % (", ".join(map(repr, REFINE_MODES)), mode))
+        nat.check(nat.lib().b200pose_post_set_refine(self._h, REFINE_MODES[mode]), "b200pose_post_set_refine")
+
+    def refine(self):
+        """The refinement mode the next run uses ('cubic', 'gauss' or 'none')."""
+        m = int(nat.lib().b200pose_post_get_refine(self._h))
+        if m < 0:
+            nat.check(1, "b200pose_post_get_refine")
+        return {v: k for k, v in REFINE_MODES.items()}[m]
+
+    def run(self, heat_ptr, paf_ptr, on_device, layout, n, h, w, thresh, stream=0, upsample=8):
+        """Post-processing of n maps (h x w, low resolution).  upsample: the integer factor 1 .. 16 from the maps to the
+        peak and person coordinates (MODEL.DOWNSAMPLE); h * upsample and w * upsample must not exceed 16384."""
+        if isinstance(upsample, bool) or int(upsample) != upsample or not 1 <= upsample <= 16:
+            raise nat.B200PoseError("run: upsample must be an integer 1 .. 16, got %r" % (upsample,))
+        nat.check(nat.lib().b200pose_post_run_scaled(self._h, ctypes.c_void_p(heat_ptr), ctypes.c_void_p(paf_ptr),
+                                                     int(on_device), layout, n, h, w, int(upsample), ctypes.c_float(thresh),
+                                                     ctypes.c_void_p(stream)),
+                  "b200pose_post_run_scaled")
 
     def flip_merge(self, normal_heat, flipped_heat, normal_paf, flipped_paf, layout=1):
         """Device-side handle_paf_and_heat (evaluate/coco_eval.py:197-242) on host float32 arrays.
@@ -670,12 +695,15 @@ class PoseEngine:
     OpenPose_Model net (NativeNet.openpose) the count is the architecture's: `stages` must stay None, and modes fp8 /
     fp16 are refused here.  `post_params`: the
     post-processing settings of the submissions (a dict of NativePost.set_params' fields; None: the reference's
-    constants), changed later with set_post_params."""
+    constants), changed later with set_post_params.  `refine`: the peak refinement of the submissions ('cubic',
+    'gauss' or 'none', NativePost.set_refine), changed later with set_refine."""
 
     stages = 6
 
     def __init__(self, state_arrays, device_index=0, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, net=None,
-                 stages=None, post_params=None):
+                 stages=None, post_params=None, refine="cubic"):
+        if refine not in REFINE_MODES:      # before any allocation
+            raise nat.B200PoseError("refine must be one of %s, got %r" % (", ".join(map(repr, REFINE_MODES)), refine))
         if net is None:
             net = NativeNet(device_index)
             net.load_state_dict_arrays(state_arrays)
@@ -694,6 +722,7 @@ class PoseEngine:
         self.post = NativePost(device_index, batch_cap, peak_cap, human_cap)
         if post_params:
             self.post.set_params(**post_params)
+        self.post.set_refine(refine)
         self.mode = nat.MODES[mode]
         self.device_index = device_index
         self._shapes = {}
@@ -710,6 +739,11 @@ class PoseEngine:
         """Post-processing settings of the following submissions (a dict such as post_params_from_cfg's, and / or
         fields; see NativePost.set_params).  Runs already submitted keep theirs."""
         self.post.set_params(**dict(params or {}, **fields))
+
+    def set_refine(self, mode):
+        """Peak refinement of the following submissions ('cubic', 'gauss' or 'none'; see NativePost.set_refine).  Runs
+        already submitted keep theirs."""
+        self.post.set_refine(mode)
 
     def _remember(self, n, H, W):
         """Shape of the run just submitted, kept per ticket (two runs may be in flight with different batch sizes or
@@ -732,10 +766,11 @@ class PoseEngine:
         return self._shapes[ticket]
 
     @classmethod
-    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=None, post_params=None):
+    def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=None, post_params=None,
+                 refine="cubic"):
         """An engine around an existing NativeNet (e.g. the one a get_model() module already packed its weights into)."""
         return cls(None, net.device_index, mode, batch_cap, peak_cap, human_cap, net=net, stages=stages,
-                   post_params=post_params)
+                   post_params=post_params, refine=refine)
 
     def submit_images(self, images, dest_size=368, factor=8, thresh=0.1, flip=False):
         """Asynchronous half of infer_images for frames of ONE shape (a video stream): returns a ticket; the frames must

@@ -1,7 +1,7 @@
 """Drop-in for the live post-processing entry points of /root/reference/lib/utils/paf_to_pose.py:
-`NMS` (:67-145) and `paf_to_pose_cpp` (:372-406).  Both run on the GPU through libb200pose.so; the x8
-nearest-neighbour up-sampling of the maps (:382-385, 31 MB per image in the reference) is never materialised -
-the kernels read the low-resolution maps at (y >> 3, x >> 3), which is the same value."""
+`NMS` (:67-145) and `paf_to_pose_cpp` (:372-406).  Both run on the GPU through libb200pose.so; the xf
+nearest-neighbour up-sampling of the maps (:382-385, 31 MB per image at f = 8 in the reference) is never materialised -
+the kernels read the low-resolution maps at (y // f, x // f), which is the same value."""
 import numpy as np
 
 from ... import _native as nat
@@ -21,30 +21,48 @@ def _post(device_index=None, peak_cap=2048, human_cap=2048):
     return _posts[idx]
 
 
-def _run(heatmaps, pafs, config):
-    if config.MODEL.DOWNSAMPLE != 8:
-        raise ValueError("the H100 path supports MODEL.DOWNSAMPLE == 8 only")
+def _factor(f):
+    """The integer up-sampling factor 1 .. 16 that f stands for, or None."""
+    if isinstance(f, (bool, np.bool_)) or not isinstance(f, (int, float, np.integer, np.floating)):
+        return None
+    return int(f) if f == int(f) and 1 <= f <= 16 else None
+
+
+def _run(heatmaps, pafs, config, upsample, refine):
     heat = np.ascontiguousarray(heatmaps, dtype=np.float32)
     paf = np.ascontiguousarray(pafs, dtype=np.float32)
     if heat.ndim != 3 or heat.shape[2] != 19 or paf.shape[:2] != heat.shape[:2] or paf.shape[2] != 38:
         raise ValueError("expected heatmaps [h,w,19] and pafs [h,w,38]")
     post = _post()
     h, w = heat.shape[:2]
-    post.run(heat.ctypes.data, paf.ctypes.data, False, 1, 1, h, w, float(np.float32(config.TEST.THRESH_HEATMAP)))
+    post.set_refine(refine)
+    post.run(heat.ctypes.data, paf.ctypes.data, False, 1, 1, h, w, float(np.float32(config.TEST.THRESH_HEATMAP)),
+             upsample=upsample)
     post.sync()
     post.check_status(1)
     return post, h, w
 
 
 def NMS(heatmaps, upsampFactor=1., bool_refine_center=True, bool_gaussian_filt=False, config=None):
-    """Returns, per joint type, an array (k, 4) of (x, y, score, id) like paf_to_pose.py:67-145
-    (refine branch, no Gaussian filtering - the configuration paf_to_pose_cpp uses)."""
-    if not bool_refine_center or bool_gaussian_filt or upsampFactor != 8:
-        raise NotImplementedError("only NMS(..., upsampFactor=8, bool_refine_center=True, bool_gaussian_filt=False)")
+    """Returns, per joint type, an array (k, 4) of (x, y, score, id) like paf_to_pose.py:67-145, for an integer
+    upsampFactor 1 .. 16 and every refinement: the bicubic patch (bool_refine_center), smoothed first with
+    gaussian_filter(sigma=3) (bool_gaussian_filt), or none at all (bool_refine_center=False: the Gaussian flag is then
+    ignored, as in the reference)."""
+    f = _factor(upsampFactor)
+    if f is None:
+        raise NotImplementedError("NMS: upsampFactor must be an integer 1 .. 16, got %r" % (upsampFactor,))
+    refine = ("gauss" if bool_gaussian_filt else "cubic") if bool_refine_center else "none"
     pafs = np.zeros(heatmaps.shape[:2] + (38,), np.float32)
-    post, _, _ = _run(heatmaps, pafs, config)
+    post, _, _ = _run(heatmaps, pafs, config, f, refine)
     peaks = post.peaks(0)
-    return [peaks[peaks[:, 4] == j][:, :4].astype(np.float64) for j in range(config.MODEL.NUM_KEYPOINTS)]
+    out = []
+    for j in range(config.MODEL.NUM_KEYPOINTS):
+        pj = peaks[peaks[:, 4] == j][:, :4].astype(np.float64)
+        if refine == "none":
+            # the device keeps pafprocess's int position f p + (f - 1) // 2; NMS reports (p + 0.5) f - 0.5 itself
+            pj[:, :2] = (pj[:, :2] // f + 0.5) * f - 0.5
+        out.append(pj)
+    return out
 
 
 def humans_from_rows(rows, W, H, num_keypoints=18):
@@ -66,6 +84,10 @@ def humans_from_rows(rows, W, H, num_keypoints=18):
 
 
 def paf_to_pose_cpp(heatmaps, pafs, config):
-    post, h, w = _run(heatmaps, pafs, config)
-    W, H = w * config.MODEL.DOWNSAMPLE, h * config.MODEL.DOWNSAMPLE
-    return humans_from_rows(post.humans(0), W, H, config.MODEL.NUM_KEYPOINTS)
+    """paf_to_pose.py:372-406 at any integer cfg.MODEL.DOWNSAMPLE f from 1 to 16: NMS at that factor, PAF scoring on the
+    xf nearest-up-sampled maps, coordinates divided by w f and h f."""
+    f = _factor(config.MODEL.DOWNSAMPLE)
+    if f is None:
+        raise ValueError("paf_to_pose_cpp: MODEL.DOWNSAMPLE must be an integer 1 .. 16, got %r" % (config.MODEL.DOWNSAMPLE,))
+    post, h, w = _run(heatmaps, pafs, config, f, "cubic")
+    return humans_from_rows(post.humans(0), w * f, h * f, config.MODEL.NUM_KEYPOINTS)
