@@ -417,8 +417,21 @@ int b200pose_post_draw(b200pose_post* post, unsigned char* frames, int on_device
  *     ragged otherwise, multi-scale when scales is not null; n <= batch_cap, 2n <= 1024 with flip.  The streams are
  *     copied when the call returns.  b200pose_post_jpeg_status: the status bits of image img of the selected run (0
  *     for runs not made from JPEG streams), -1 when img is out of range.
+ *
+ *     Progressive streams (SOF2, DESIGN.md 2.18), opt-in per net: b200pose_net_set_jpeg_progressive(net, 1) makes
+ *     b200pose_net_decode_jpegs and b200pose_infer_jpegs on that net decode progressive Huffman streams with 8-bit
+ *     samples and the sampling set above too, bit for bit cv2.imdecode, up to 256 scans per image.  Default 0: they
+ *     are refused as "unsupported: progressive (SOF2)".  Still refused as unsupported with the switch on: streams in
+ *     which some component has unknown bits among zig-zag coefficients 0 .. 9 after its last scan (libjpeg smooths
+ *     those blocks), bogus progressions (libjpeg only warns), undefined Huffman tables.  A scan that is not a valid
+ *     progression (where libjpeg stops with JERR_BAD_PROGRESSION and cv2.imdecode returns None) is malformed.  Damaged
+ *     entropy data sets the status bits above.  b200pose_net_get_jpeg_progressive: the switch (0 / 1), -1 for a null
+ *     net.  b200pose_jpeg_info_ex: b200pose_jpeg_info with the switch given (b200pose_jpeg_info: 0).
  * ---------------------------------------------------------------------------------------------------------- */
 int b200pose_jpeg_info(const unsigned char* data, long long size, int* h, int* w, int* supported);
+int b200pose_jpeg_info_ex(const unsigned char* data, long long size, int progressive, int* h, int* w, int* supported);
+int b200pose_net_set_jpeg_progressive(b200pose_net* net, int on);
+int b200pose_net_get_jpeg_progressive(b200pose_net* net);
 int b200pose_net_decode_jpegs(b200pose_net* net, const unsigned char* const* data, const long long* sizes, int n,
                               unsigned char* out, int out_on_device, void* cuda_stream);
 int b200pose_infer_jpegs(b200pose_net* net, b200pose_post* post, const unsigned char* const* data,

@@ -83,6 +83,9 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_infer_frames": ([vp, vp, vp, ci, ci, ci, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf, ci, vp],
                               ci),
     "b200pose_jpeg_info": ([vp, ctypes.c_longlong, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)], ci),
+    "b200pose_jpeg_info_ex": ([vp, ctypes.c_longlong, ci, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)], ci),
+    "b200pose_net_set_jpeg_progressive": ([vp, ci], ci),
+    "b200pose_net_get_jpeg_progressive": ([vp], ci),
     "b200pose_net_decode_jpegs": ([vp, vp, vp, ci, vp, ci, vp], ci),
     "b200pose_infer_jpegs": ([vp, vp, vp, vp, ci, ci, ci, ctypes.POINTER(ctypes.c_double), ci, ci, cf, ci, vp], ci),
     "b200pose_post_jpeg_status": ([vp, ci], ci),

@@ -447,6 +447,7 @@ struct b200pose_net {
     DevBuf<unsigned char> in_stage_u8;
     int preprocess = 1;                // normalisation fused into the uint8 entry points (preprocess_core.h; 1 = rtpose)
     int stages = kStages;              // refinement stages every later forward runs (b200pose_net_set_stages)
+    bool jpeg_progressive = false;     // the JPEG calls decode progressive streams (b200pose_net_set_jpeg_progressive)
     DevBuf<unsigned char> raw_stage;   // raw (un-resized) frames of b200pose_*crop* / b200pose_infer_raw_u8
     // Ragged batches (DESIGN.md §1): the extents table [H_0, W_0, H_1, W_1, ...] every kernel of a ragged forward reads.
     // Allocated once for kMaxRagged images and never moved, so that plans and captured graphs stay valid across mixes;
@@ -1349,6 +1350,17 @@ int b200pose_net_set_preprocess(b200pose_net* net, int preprocess) {
     if (preprocess < 1 || preprocess > 4) return fail("preprocess must be 1 (rtpose), 2 (vgg), 3 (inception) or 4 (ssd)");
     net->preprocess = preprocess;
     return 0;
+}
+
+int b200pose_net_set_jpeg_progressive(b200pose_net* net, int on) {
+    if (!net) return fail("null net");
+    net->jpeg_progressive = on != 0;
+    return 0;
+}
+
+int b200pose_net_get_jpeg_progressive(b200pose_net* net) {
+    if (!net) return fail("null net"), -1;
+    return net->jpeg_progressive ? 1 : 0;
 }
 
 int b200pose_net_set_stages(b200pose_net* net, int stages) {
@@ -2272,9 +2284,10 @@ constexpr long long kJpegMaxPixels = 1LL << 28;     // a frame's pixels, as for 
 // where its tables lie, the oriented sizes [oh_0, ow_0, oh_1, ...], the packed BGR output's size, and what the device
 // buffers must hold.
 struct JpegCall {
-    int n = 0, nwork = 0;
+    int n = 0, nwork = 0, njobs = 0, nprog = 0;
     std::vector<char> up;
-    size_t o_ims = 0, o_jobs = 0, o_segs = 0, o_chunk = 0, o_work = 0, o_status = 0, o_raw = 0;
+    size_t o_ims = 0, o_jobs = 0, o_segs = 0, o_chunk = 0, o_work = 0, o_status = 0, o_raw = 0, o_prog = 0, o_scans = 0,
+           o_pseg = 0;
     std::vector<int> hw;
     long long bytes = 0, data = 0, blocks = 0, planes = 0, max_blocks = 0, max_px = 0;
     bool uniform() const {
@@ -2284,22 +2297,27 @@ struct JpegCall {
     }
 };
 
-// Parses every stream of a call before anything is enqueued and lays out its upload.
-static int check_jpegs(const unsigned char* const* data, const long long* sizes, int n, int max_n, JpegCall* j) {
+// Parses every stream of a call before anything is enqueued and lays out its upload.  progressive: progressive
+// streams are decoded too (b200pose_net_set_jpeg_progressive); each of their scans is an unstuffing job of its own.
+static int check_jpegs(const unsigned char* const* data, const long long* sizes, int n, int max_n, JpegCall* j,
+                       bool progressive) {
     if (!data || !sizes) return fail("jpegs: null stream table");
     if (n < 1 || n > max_n) return fail("jpegs: %d images (1 .. %d)", n, max_n);
     *j = JpegCall{};
     j->n = n;
     std::unique_ptr<JpegParsed> P(new JpegParsed);
     std::vector<JpegImage> ims(n);
-    std::vector<JpegUnstuffJob> jobs(n);
-    std::vector<JpegSeg> segs;
+    std::vector<JpegUnstuffJob> jobs;
+    std::vector<JpegSeg> segs, psegs;
+    std::vector<JpegProgImage> progs;
+    std::vector<JpegScan> pscans;
     std::vector<unsigned> status(n);
-    std::vector<std::pair<long long, long long>> scans(n);
+    std::vector<std::pair<long long, long long>> scans;      // per job, its bytes of the stream
+    std::vector<int> job_img;
     long long raw = 0, chunks = 0;
     for (int i = 0; i < n; ++i) {
         if (!data[i] || sizes[i] < 0) return fail("jpeg image %d: null stream or negative size", i);
-        if (!jpeg_parse(data[i], sizes[i], kJpegMaxPixels, P.get())) return fail("jpeg image %d: %s", i, P->reason);
+        if (!jpeg_parse(data[i], sizes[i], kJpegMaxPixels, P.get(), progressive)) return fail("jpeg image %d: %s", i, P->reason);
         if (!P->supported) return fail("jpeg image %d: %s", i, P->reason);
         JpegImage& im = ims[i];
         im = P->im;
@@ -2316,35 +2334,59 @@ static int check_jpegs(const unsigned char* const* data, const long long* sizes,
         j->hw.push_back(im.ow);
         j->bytes += 3LL * im.oh * im.ow;
         j->max_px = std::max(j->max_px, (long long)im.oh * im.ow);
-        jobs[i] = JpegUnstuffJob{raw, raw + (P->scan_end - P->scan_beg), j->data};
-        scans[i] = {P->scan_beg, P->scan_end};
+        status[i] = P->status;
+        if (P->progressive) {      // each scan's unstuffed data gets room for its raw bytes
+            std::vector<long long> base;
+            for (size_t s = 0; s < P->scans.size(); ++s) {
+                const long long b = P->scan_raw[2 * s], e = P->scan_raw[2 * s + 1];
+                jobs.push_back(JpegUnstuffJob{raw, raw + (e - b), j->data});
+                scans.push_back({b, e});
+                job_img.push_back(i);
+                base.push_back(j->data);
+                j->data += e - b;
+                raw += e - b;
+            }
+            progs.push_back(JpegProgImage{i, (int)pscans.size(), (int)P->scans.size()});
+            jpeg_prog_segments(*P, i, base.data(), &pscans, &psegs);
+            continue;
+        }
+        jobs.push_back(JpegUnstuffJob{raw, raw + (P->scan_end - P->scan_beg), j->data});
+        scans.push_back({P->scan_beg, P->scan_end});
+        job_img.push_back(i);
         chunks += jpeg_segments(*P, i, j->data, chunks, &segs);
         j->data += P->seg_end.back();
         raw += P->scan_end - P->scan_beg;
-        status[i] = P->status;
     }
     std::vector<int> chunk_seg;
     std::vector<long long> work;
     jpeg_work(segs, chunks, &chunk_seg, &work);
     j->nwork = (int)work.size() - 1;
+    j->njobs = (int)jobs.size();
+    j->nprog = (int)progs.size();
     auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
     j->o_ims = 0;
     j->o_jobs = up16(j->o_ims + n * sizeof(JpegImage));
-    j->o_segs = up16(j->o_jobs + n * sizeof(JpegUnstuffJob));
+    j->o_segs = up16(j->o_jobs + jobs.size() * sizeof(JpegUnstuffJob));
     j->o_chunk = up16(j->o_segs + segs.size() * sizeof(JpegSeg));
     j->o_work = up16(j->o_chunk + chunk_seg.size() * sizeof(int));
     j->o_status = up16(j->o_work + work.size() * sizeof(long long));
-    j->o_raw = up16(j->o_status + n * sizeof(unsigned));
+    j->o_prog = up16(j->o_status + n * sizeof(unsigned));
+    j->o_scans = up16(j->o_prog + progs.size() * sizeof(JpegProgImage));
+    j->o_pseg = up16(j->o_scans + pscans.size() * sizeof(JpegScan));
+    j->o_raw = up16(j->o_pseg + psegs.size() * sizeof(JpegSeg));
     j->up.resize(j->o_raw + (size_t)raw + 16);
     char* u = j->up.data();
     memcpy(u + j->o_ims, ims.data(), n * sizeof(JpegImage));
-    memcpy(u + j->o_jobs, jobs.data(), n * sizeof(JpegUnstuffJob));
+    memcpy(u + j->o_jobs, jobs.data(), jobs.size() * sizeof(JpegUnstuffJob));
     memcpy(u + j->o_segs, segs.data(), segs.size() * sizeof(JpegSeg));
     memcpy(u + j->o_chunk, chunk_seg.data(), chunk_seg.size() * sizeof(int));
     memcpy(u + j->o_work, work.data(), work.size() * sizeof(long long));
     memcpy(u + j->o_status, status.data(), n * sizeof(unsigned));
-    for (int i = 0; i < n; ++i)
-        memcpy(u + j->o_raw + jobs[i].raw_beg, data[i] + scans[i].first, (size_t)(scans[i].second - scans[i].first));
+    memcpy(u + j->o_prog, progs.data(), progs.size() * sizeof(JpegProgImage));
+    memcpy(u + j->o_scans, pscans.data(), pscans.size() * sizeof(JpegScan));
+    memcpy(u + j->o_pseg, psegs.data(), psegs.size() * sizeof(JpegSeg));
+    for (size_t k = 0; k < jobs.size(); ++k)
+        memcpy(u + j->o_raw + jobs[k].raw_beg, data[job_img[k]] + scans[k].first, (size_t)(scans[k].second - scans[k].first));
     return 0;
 }
 
@@ -2375,8 +2417,13 @@ static int decode_jpegs_dev(b200pose_net* net, const JpegCall& j, unsigned char*
     b.status = reinterpret_cast<unsigned*>(d + j.o_status);
     b.max_blocks = j.max_blocks;
     b.max_px = j.max_px;
+    b.njobs = j.njobs;
+    b.prog = reinterpret_cast<const JpegProgImage*>(d + j.o_prog);
+    b.nprog = j.nprog;
+    b.scans = reinterpret_cast<const JpegScan*>(d + j.o_scans);
+    b.pseg = reinterpret_cast<const JpegSeg*>(d + j.o_pseg);
     *d_status = b.status;
-    return launched(jpeg_decode_launch(b, st), "jpeg_decode_launch", kJpegLaunches);
+    return launched(jpeg_decode_launch(b, st), "jpeg_decode_launch", jpeg_decode_launches(b));
 }
 
 // The frames of j decoded into net->raw_stage, with room for their mirror images behind them when flip; the status
@@ -2668,9 +2715,13 @@ int b200pose_infer_frames(b200pose_net* net, b200pose_post* post, const b200pose
 }
 
 int b200pose_jpeg_info(const unsigned char* data, long long size, int* h, int* w, int* supported) {
+    return b200pose_jpeg_info_ex(data, size, 0, h, w, supported);
+}
+
+int b200pose_jpeg_info_ex(const unsigned char* data, long long size, int progressive, int* h, int* w, int* supported) {
     if (!data || !h || !w || !supported) return fail("jpeg_info: null pointer");
     std::unique_ptr<JpegParsed> P(new JpegParsed);
-    const bool ok = jpeg_parse(data, size, kJpegMaxPixels, P.get());
+    const bool ok = jpeg_parse(data, size, kJpegMaxPixels, P.get(), progressive != 0);
     *h = P->im.oh;
     *w = P->im.ow;
     *supported = ok && P->supported;
@@ -2684,7 +2735,7 @@ int b200pose_net_decode_jpegs(b200pose_net* net, const unsigned char* const* dat
     if (!net) return fail("null net");
     if (!out) return fail("decode_jpegs: null output");
     JpegCall j;
-    if (int rc = check_jpegs(data, sizes, n, kMaxRagged, &j)) return rc;
+    if (int rc = check_jpegs(data, sizes, n, kMaxRagged, &j, net->jpeg_progressive)) return rc;
     CU(cudaSetDevice(net->device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     unsigned char* d_out = out;
@@ -2709,7 +2760,7 @@ int b200pose_infer_jpegs(b200pose_net* net, b200pose_post* post, const unsigned 
     if (int rc = check_infer(net, post, mode)) return rc;
     if (flip && 2 * n > kMaxRagged) return fail("jpegs: %d images with flip (2n <= %d)", n, kMaxRagged);
     JpegCall j;
-    if (int rc = check_jpegs(data, sizes, n, post->pb.batch_cap, &j)) return rc;
+    if (int rc = check_jpegs(data, sizes, n, post->pb.batch_cap, &j, net->jpeg_progressive)) return rc;
     const bool uniform = j.uniform();
     return infer_raw(net, post, nullptr, 0, n, uniform ? j.hw[0] : 0, uniform ? j.hw[1] : 0, uniform ? nullptr : j.hw.data(),
                      dest_size, factor, scales, n_scales, mode, thresh, flip, cuda_stream, nullptr, &j);

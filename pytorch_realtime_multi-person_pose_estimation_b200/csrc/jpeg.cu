@@ -12,6 +12,12 @@
 //     interval (a segmented scan in 32-bit ints, stored as 16-bit coefficients as jdhuff.c does).
 //  4. IDCT: one thread per 8 x 8 block into the component's sample plane.
 //  5. colour: one thread per output pixel - upsampling, YCbCr -> BGR and orientation - into the packed output.
+// Progressive images (DESIGN.md 2.18) are unstuffed per scan by the same kernel, skip steps 2 and 3 (the DC kernel's
+// prefix sums run before their coefficients are written, over zeros) and are decoded by jpeg_prog_kernel between
+// steps 3 and 4: one CTA per image walks its scans in stream order, each scan's restart segments spread over the
+// threads, each segment decoded serially by jdphuff.c's loop (refinement scans consume bits by the coefficients of
+// earlier scans, so they cannot be self-synchronised as the Huffman kernel's chunks are).  Launches whose grid would be
+// empty (no baseline image) are skipped.
 #include "jpeg.cuh"
 
 namespace b2p {
@@ -206,6 +212,25 @@ __global__ void __launch_bounds__(kThreads) jpeg_color_kernel(const JpegImage* _
     }
 }
 
+constexpr int kProgThreads = 128;
+
+__global__ void __launch_bounds__(kProgThreads) jpeg_prog_kernel(const JpegImage* __restrict__ ims,
+                                                                 const JpegProgImage* __restrict__ prog,
+                                                                 const JpegScan* __restrict__ scans,
+                                                                 const JpegSeg* __restrict__ segs,
+                                                                 const unsigned char* __restrict__ data, short* coef,
+                                                                 unsigned* status) {
+    const JpegProgImage pi = prog[blockIdx.x];
+    const JpegImage& im = ims[pi.img];
+    unsigned bad = 0;
+    for (int s = pi.scan0; s < pi.scan0 + pi.nscans; ++s) {
+        const JpegScan& sc = scans[s];
+        for (int k = threadIdx.x; k < sc.nseg; k += kProgThreads) bad |= jp_prog_segment(im, sc, segs[sc.seg0 + k], data, coef);
+        __syncthreads();
+    }
+    if (bad) atomicOr(status + pi.img, bad);
+}
+
 unsigned grid_for(long long items, int n) {
     long long bx = (items + kThreads - 1) / kThreads;
     const long long cap = (132LL * 8 + n - 1) / n;      // about one wave of 8 blocks per SM over the whole batch
@@ -215,11 +240,21 @@ unsigned grid_for(long long items, int n) {
 
 }  // namespace
 
+int jpeg_decode_launches(const JpegBatch& b) {
+    return b.nprog == 0 ? kJpegLaunches : b.nwork > 0 ? kJpegProgLaunches : kJpegProgOnlyLaunches;
+}
+
 cudaError_t jpeg_decode_launch(const JpegBatch& b, cudaStream_t s) {
-    if (b.n < 1 || b.n > 65535 || b.nwork < 1 || b.max_px < 1 || b.max_blocks < 1) return cudaErrorInvalidValue;
-    jpeg_unstuff_kernel<<<b.n, kThreads, 0, s>>>(b.jobs, b.raw, b.data);
-    jpeg_huff_kernel<<<b.nwork, kThreads, 0, s>>>(b.ims, b.segs, b.chunk_seg, b.work, b.data, b.coef, b.status);
-    jpeg_dc_kernel<<<dim3(b.n, 3), kThreads, 0, s>>>(b.ims, b.coef);
+    if (b.n < 1 || b.n > 65535 || b.nwork < (b.nprog ? 0 : 1) || b.max_px < 1 || b.max_blocks < 1 || b.nprog < 0 ||
+        b.nprog > b.n || b.njobs < 1)
+        return cudaErrorInvalidValue;
+    jpeg_unstuff_kernel<<<b.njobs, kThreads, 0, s>>>(b.jobs, b.raw, b.data);
+    if (b.nwork > 0) {
+        jpeg_huff_kernel<<<b.nwork, kThreads, 0, s>>>(b.ims, b.segs, b.chunk_seg, b.work, b.data, b.coef, b.status);
+        jpeg_dc_kernel<<<dim3(b.n, 3), kThreads, 0, s>>>(b.ims, b.coef);
+    }
+    if (b.nprog > 0)
+        jpeg_prog_kernel<<<b.nprog, kProgThreads, 0, s>>>(b.ims, b.prog, b.scans, b.pseg, b.data, b.coef, b.status);
     jpeg_idct_kernel<<<dim3(grid_for(b.max_blocks, 3 * b.n), b.n, 3), kThreads, 0, s>>>(b.ims, b.coef, b.planes);
     jpeg_color_kernel<<<dim3(grid_for(b.max_px, b.n), b.n), kThreads, 0, s>>>(b.ims, b.planes, b.out);
     return cudaGetLastError();

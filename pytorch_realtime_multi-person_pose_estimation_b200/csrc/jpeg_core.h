@@ -15,6 +15,8 @@
 //  * OpenCV's EXIF orientation (ExifReader + ApplyExifOrientation): the first orientation entry of IFD0 among the APP1
 //    segments that begin "Exif\0\0" (a TIFF header from byte 6), mapped through frame_core.h's rotation plus a mirror
 //    for 2, 4, 5 and 7.
+// Progressive (SOF2) streams are parsed scan by scan when jpeg_parse's `progressive` is set, and their scans decoded as
+// jdphuff.c does into the same coefficient buffer (DESIGN.md 2.18); the steps above then run unchanged.
 // The parse (host only) validates every length, table and dimension; streams the device does not decode are reported
 // as unsupported with the reason.  The decode steps are the functions the kernels of jpeg.cu run, and the host build of
 // the tests (tests/cuda/jpeg_core_host.cpp) runs them in the same order.
@@ -342,6 +344,154 @@ B2P_JP_HD short* jp_dc_block(const JpegImage& im, short* coef, int c, long long 
     return coef + (cp.coef + by * cp.bw + bx) * 64;
 }
 
+// ---------------------------------------------------------------------------------------------- progressive scans
+// Progressive (SOF2) streams, jdphuff.c restated (DESIGN.md 2.18).  Every scan is decoded into the same coefficient
+// buffer in stream order; the IDCT, upsampling and colour steps above then run unchanged.  A scan's unit is a block
+// of its one component (component's own ceil(dw / 8) x ceil(dh / 8) blocks in raster order, not the MCU-padded plane)
+// or, for an interleaved DC scan, an MCU of the frame; its restart interval counts units.
+constexpr int kJpegMaxScans = 256;      // scans per image; more are refused as unsupported
+
+// One scan of a progressive image (device-resident).  DC first scans decode component k of the scan with huff[k], AC
+// first and refinement scans with huff[0]; DC refinement scans read no table.
+struct JpegScan {
+    int ncomp, comp[3];          // frame components of the scan, in frame order
+    int ss, se, ah, al;          // spectral band and successive-approximation bits
+    int units, restart;          // units of the scan; units per segment (0: one segment)
+    int seg0, nseg;              // its segments in the batch's segment table (JpegSeg::mcu0 / mcus count units)
+    JpegHuff huff[3];
+};
+
+// One progressive image of a decode batch: JpegImage img of the batch, its scans scan0 .. scan0 + nscans - 1.
+struct JpegProgImage {
+    int img, scan0, nscans;
+};
+
+// The next n (0 .. 16) bits at bit *p of the segment, advancing *p.
+B2P_JP_HD unsigned jp_getbits(const unsigned char* d, long long nbytes, long long* p, int n) {
+    if (n == 0) return 0;
+    const unsigned v = jp_peek32(d, nbytes, *p) >> (32 - n);
+    *p += n;
+    return v;
+}
+
+// The block of unit u of scan sc holding its k-th block (k < the unit's blocks), and the scan component it belongs to.
+B2P_JP_HD short* jp_prog_block(const JpegImage& im, const JpegScan& sc, short* coef, long long u, int k, int* ci) {
+    if (sc.ncomp == 1) {
+        const JpegComp& cp = im.comp[sc.comp[0]];
+        const long long wb = (cp.dw + 7) / 8;
+        *ci = 0;
+        return coef + (cp.coef + (u / wb) * cp.bw + u % wb) * 64;
+    }
+    int c = 0;
+    for (;; ++c) {
+        const int per = im.comp[sc.comp[c]].h * im.comp[sc.comp[c]].v;
+        if (k < per) break;
+        k -= per;
+    }
+    const JpegComp& cp = im.comp[sc.comp[c]];
+    *ci = c;
+    const long long bx = (u % im.mcux) * cp.h + k % cp.h, by = (u / im.mcux) * cp.v + k / cp.h;
+    return coef + (cp.coef + by * cp.bw + bx) * 64;
+}
+
+// jdphuff.c's decode_mcu_AC_refine for one block: correction bits for the band's nonzero coefficients passed over,
+// new coefficients +-p1 at the r-th zero-history position, EOB runs.  16-bit JCOEF arithmetic.
+B2P_JP_HD bool jp_ac_refine(const JpegImage& im, const JpegScan& sc, short* blk, const unsigned char* d, long long nbytes,
+                            long long* p, int* eobrun) {
+    const int p1 = 1 << sc.al, m1 = (int)(~0u << sc.al);
+    int k = sc.ss;
+    if (*eobrun == 0) {
+        for (; k <= sc.se; ++k) {
+            int len;
+            const int rs = jp_huff(sc.huff[0], jp_peek32(d, nbytes, *p), &len);
+            if (len == 0) return false;
+            *p += len;
+            int r = rs >> 4, s = rs & 15;
+            if (s) {
+                s = jp_getbits(d, nbytes, p, 1) ? p1 : m1;       // a size other than 1: libjpeg warns, reads one bit
+            } else if (r != 15) {
+                *eobrun = (1 << r) + (int)jp_getbits(d, nbytes, p, r);
+                break;
+            }
+            do {
+                short* c = blk + im.zz[k];
+                if (*c != 0) {
+                    if (jp_getbits(d, nbytes, p, 1) && (*c & p1) == 0) *c = (short)(*c >= 0 ? *c + p1 : *c + m1);
+                } else if (--r < 0) {
+                    break;
+                }
+                ++k;
+            } while (k <= sc.se);
+            if (s) blk[im.zz[k]] = (short)s;
+        }
+    }
+    if (*eobrun > 0) {
+        for (; k <= sc.se; ++k) {
+            short* c = blk + im.zz[k];
+            if (*c != 0 && jp_getbits(d, nbytes, p, 1) && (*c & p1) == 0) *c = (short)(*c >= 0 ? *c + p1 : *c + m1);
+        }
+        --*eobrun;
+    }
+    return true;
+}
+
+// Decodes segment sg of scan sc of image im (unstuffed bytes [sg.beg, sg.end) of data) into coef, as libjpeg's loop
+// runs it from a restart: DC predictors and EOBRUN start at 0.  Returns the kJpeg* status bits it found.
+B2P_JP_HD unsigned jp_prog_segment(const JpegImage& im, const JpegScan& sc, const JpegSeg& sg, const unsigned char* data,
+                                   short* coef) {
+    const unsigned char* d = data + sg.beg;
+    const long long nbytes = sg.end - sg.beg, bits = nbytes * 8;
+    long long p = 0;
+    int pred[3] = {0, 0, 0}, eobrun = 0;
+    int bpu = 1;                 // blocks per unit
+    if (sc.ncomp > 1) {
+        bpu = 0;
+        for (int c = 0; c < sc.ncomp; ++c) bpu += im.comp[sc.comp[c]].h * im.comp[sc.comp[c]].v;
+    }
+    for (long long u = sg.mcu0; u < (long long)sg.mcu0 + sg.mcus; ++u) {
+        for (int k = 0; k < bpu; ++k) {
+            int ci;
+            short* blk = jp_prog_block(im, sc, coef, u, k, &ci);
+            if (sc.ss == 0 && sc.ah == 0) {              // DC first
+                int len;
+                const int t = jp_huff(sc.huff[ci], jp_peek32(d, nbytes, p), &len);
+                if (len == 0 || t > 15) return kJpegBadCode;
+                p += len;
+                pred[ci] += jp_extend(jp_getbits(d, nbytes, &p, t), t);
+                blk[0] = (short)(int)((unsigned)pred[ci] << sc.al);
+            } else if (sc.ss == 0) {                     // DC refinement
+                if (jp_getbits(d, nbytes, &p, 1)) blk[0] = (short)(blk[0] | (1 << sc.al));
+            } else if (sc.ah == 0) {                     // AC first
+                if (eobrun > 0) {
+                    --eobrun;
+                    continue;
+                }
+                for (int j = sc.ss; j <= sc.se; ++j) {
+                    int len;
+                    const int rs = jp_huff(sc.huff[0], jp_peek32(d, nbytes, p), &len);
+                    if (len == 0) return kJpegBadCode;
+                    p += len;
+                    const int r = rs >> 4, s = rs & 15;
+                    if (s) {
+                        j += r;
+                        blk[im.zz[j]] = (short)(int)((unsigned)jp_extend(jp_getbits(d, nbytes, &p, s), s) << sc.al);
+                    } else if (r == 15) {
+                        j += 15;
+                    } else {
+                        eobrun = (1 << r) + (int)jp_getbits(d, nbytes, &p, r) - 1;
+                        break;
+                    }
+                }
+            } else if (!jp_ac_refine(im, sc, blk, d, nbytes, &p, &eobrun)) {
+                return kJpegBadCode;
+            }
+        }
+        if (p > bits) return kJpegShortData;
+    }
+    if (bits - p >= 8) return kJpegExtraData;
+    return 0;
+}
+
 }  // namespace b2p
 
 // ================================================================================================ host-side parse
@@ -396,6 +546,14 @@ struct JpegParsed {
     unsigned status = 0;           // what the marker walk found: kJpegBadRestart
     long long scan_beg = 0, scan_end = 0;                  // the scan's bytes [scan_beg, scan_end) of the stream
     std::vector<long long> seg_beg, seg_end;              // per segment, unstuffed bytes from the scan's start
+    // Progressive streams (jpeg_parse's `progressive`): every scan with its tables, and its bytes [scan_raw[2s],
+    // scan_raw[2s + 1]) of the stream; seg_beg / seg_end then hold the segments of all scans one after another, each in
+    // unstuffed bytes from its own scan's start (JpegScan::seg0, nseg).  bits[c][k]: the Al of the last scan that
+    // coded zig-zag coefficient k of component c (-1: none did), libjpeg's coef_bits.
+    bool progressive = false;
+    std::vector<JpegScan> scans;
+    std::vector<long long> scan_raw;
+    int bits[3][64];
 };
 
 inline bool jp_fail(JpegParsed* P, const char* fmt, ...) {
@@ -432,9 +590,170 @@ inline bool jpeg_build_huff(const unsigned char* counts, const unsigned char* va
     return true;
 }
 
+// The entropy-coded data of a scan from byte beg: every 0xFF is a stuffed byte (FF 00), a restart marker (RSTn, ending
+// a segment) or the marker after the scan; fill bytes (more 0xFF) may precede any of them.  Appends each segment's
+// unstuffed [begin, end) from beg to sb / se and ORs kJpegBadRestart into *status for a misnumbered restart marker.
+// Returns where the scan ends (the marker's first 0xFF, or n); *code: the marker after the scan (-1: none).
+inline long long jpeg_scan_walk(const unsigned char* d, long long n, long long beg, std::vector<long long>* sb,
+                                std::vector<long long>* se, unsigned* status, int* code) {
+    long long dropped = 0, pos = beg, rst = 0, end = n;     // dropped: the bytes unstuffing removes
+    *code = -1;
+    sb->push_back(0);
+    while (pos < n) {
+        const void* f = memchr(d + pos, 0xFF, (size_t)(n - pos));
+        if (!f) break;
+        const long long a = (const unsigned char*)f - d;
+        long long j = a + 1;
+        while (j < n && d[j] == 0xFF) ++j;
+        if (j >= n) {
+            end = a;
+            break;
+        }
+        const int c = d[j];
+        pos = j + 1;
+        if (c == 0x00) {
+            dropped += j - a;
+        } else if (c >= 0xD0 && c <= 0xD7) {
+            if (c != 0xD0 + (rst & 7)) *status |= kJpegBadRestart;
+            ++rst;
+            se->push_back(a - beg - dropped);
+            dropped += j - a + 1;
+            sb->push_back(j + 1 - beg - dropped);
+        } else {
+            *code = c;
+            end = a;
+            break;
+        }
+    }
+    se->push_back(end - beg - dropped);
+    return end;
+}
+
+// One SOS of a progressive stream (payload s, ns components): the scan's checks, tables and progression, appended to
+// P->scans.  Returns false for a malformed scan (reason set), true otherwise (P->reason set: unsupported).
+struct JpegProgTables {
+    const int (*qt)[64];
+    const unsigned char (*counts)[16];
+    const unsigned char (*vals)[256];
+    const int* nvals;
+    int qt_have, huff_have, restart;
+    const int *ids, *tq;
+    bool latched[3];
+};
+
+inline bool jp_prog_sos(JpegParsed* P, const unsigned char* s, int ns, JpegProgTables& T) {
+    JpegImage& im = P->im;
+    const int nf = im.ncomp;
+    const int Ss = s[1 + 2 * ns], Se = s[2 + 2 * ns], Ah = s[3 + 2 * ns] >> 4, Al = s[3 + 2 * ns] & 15;
+    const int scan = (int)P->scans.size();
+    // jdphuff.c start_pass_phuff_decoder's JERR_BAD_PROGRESSION: cv2.imdecode returns None
+    const bool dc = Ss == 0;
+    if ((dc && Se != 0) || (!dc && (Ss > Se || Se > 63 || ns != 1)) || (Ah != 0 && Al != Ah - 1) || Al > 13)
+        return jp_fail(P, "malformed scan %d: Ss %d, Se %d, Ah %d, Al %d with %d components is not a valid progression",
+                       scan, Ss, Se, Ah, Al, ns);
+    if (scan >= kJpegMaxScans) return jp_unsupported(P, "more than 256 scans");
+    P->scans.emplace_back();
+    JpegScan& sc = P->scans.back();
+    memset(&sc, 0, sizeof(sc));
+    sc.ncomp = ns;
+    sc.ss = Ss;
+    sc.se = Se;
+    sc.ah = Ah;
+    sc.al = Al;
+    int prev = -1;
+    for (int k = 0; k < ns; ++k) {
+        int c = 0;
+        while (c < nf && T.ids[c] != s[1 + 2 * k]) ++c;
+        if (c == nf || c <= prev) return jp_unsupported(P, "scan components not in the frame's order");
+        prev = c;
+        sc.comp[k] = c;
+        if (!T.latched[c]) {     // latch_quant_tables: a component keeps the table it had at its first scan
+            if (!(T.qt_have >> T.tq[c] & 1)) return jp_fail(P, "malformed header: component %d has no quantisation table", c);
+            memcpy(im.qt[c], T.qt[T.tq[c]], sizeof(im.qt[c]));
+            T.latched[c] = true;
+        }
+        const int td = s[2 + 2 * k] >> 4, ta = s[2 + 2 * k] & 15;
+        if (dc && Ah == 0) {     // DC refinement reads no table
+            if (td > 3) return jp_fail(P, "malformed header: SOS DC table id %d", td);
+            if (!(T.huff_have >> td & 1)) return jp_unsupported(P, "a scan with an undefined Huffman table");
+            if (!jpeg_build_huff(T.counts[td], T.vals[td], T.nvals[td], true, &sc.huff[k]))
+                return jp_fail(P, "malformed header: Huffman table DC %d is not a valid code", td);
+        } else if (!dc) {
+            if (ta > 3) return jp_fail(P, "malformed header: SOS AC table id %d", ta);
+            if (!(T.huff_have >> (4 + ta) & 1)) return jp_unsupported(P, "a scan with an undefined Huffman table");
+            if (!jpeg_build_huff(T.counts[4 + ta], T.vals[4 + ta], T.nvals[4 + ta], false, &sc.huff[0]))
+                return jp_fail(P, "malformed header: Huffman table AC %d is not a valid code", ta);
+        }
+        // libjpeg only warns about a bogus progression (JWRN_BOGUS_PROGRESSION) and decodes on: left to cv2
+        int* bits = P->bits[c];
+        if (!dc && bits[0] < 0) return jp_unsupported(P, "a bogus progression (an AC scan before the component's DC)");
+        for (int q = Ss; q <= Se; ++q) {
+            if (Ah != (bits[q] < 0 ? 0 : bits[q]))
+                return jp_unsupported(P, "a bogus progression (Ah differs from the bits already coded)");
+            bits[q] = Al;
+        }
+    }
+    if (ns == 1) {
+        const JpegComp& cp = im.comp[sc.comp[0]];
+        sc.units = ((cp.dw + 7) / 8) * ((cp.dh + 7) / 8);
+    } else {
+        sc.units = im.mcux * im.mcuy;
+    }
+    sc.restart = T.restart;
+    return true;
+}
+
+// The frame geometry of a JpegImage: sizes, MCUs, per component its sampling, planes and downsampled size, and the
+// blocks of an interleaved MCU.
+inline void jpeg_geometry(JpegImage* im, int h, int w, int nf, const int* hs, const int* vs) {
+    for (int k = 0; k < 80; ++k) im->zz[k] = (unsigned char)jp_natural(k);
+    im->h = h;
+    im->w = w;
+    im->ncomp = nf;
+    im->hmax = nf == 3 ? hs[0] : 1;
+    im->vmax = nf == 3 ? vs[0] : 1;
+    im->mcux = (im->w + 8 * im->hmax - 1) / (8 * im->hmax);
+    im->mcuy = (im->h + 8 * im->vmax - 1) / (8 * im->vmax);
+    im->bpm = 0;
+    for (int c = 0; c < nf; ++c) {
+        JpegComp& cp = im->comp[c];
+        cp.h = nf == 3 ? hs[c] : 1;
+        cp.v = nf == 3 ? vs[c] : 1;
+        cp.bw = im->mcux * cp.h;
+        cp.bh = im->mcuy * cp.v;
+        cp.dw = (int)(((long long)im->w * cp.h + im->hmax - 1) / im->hmax);
+        cp.dh = (int)(((long long)im->h * cp.v + im->vmax - 1) / im->vmax);
+        for (int y = 0; y < cp.v; ++y)
+            for (int x = 0; x < cp.h; ++x, ++im->bpm) {
+                im->mcu_comp[im->bpm] = c;
+                im->mcu_bx[im->bpm] = x;
+                im->mcu_by[im->bpm] = y;
+            }
+    }
+}
+
+// The entropy-coded data of the progressive scan just parsed (P->scans.back()), from byte *i: its bytes, segments and
+// restart status.  *i becomes the scan's end; returns false when the data ends there (no marker follows).
+inline bool jpeg_prog_walk(const unsigned char* d, long long n, long long* i, JpegParsed* P) {
+    JpegScan& sc = P->scans.back();
+    sc.seg0 = (int)P->seg_beg.size();
+    int code;
+    const long long end = jpeg_scan_walk(d, n, *i, &P->seg_beg, &P->seg_end, &P->status, &code);
+    const long long found = (long long)P->seg_beg.size() - sc.seg0;
+    const long long expect = sc.restart ? (sc.units + (long long)sc.restart - 1) / sc.restart : 1;
+    if (found != expect) P->status |= kJpegBadRestart;
+    sc.nseg = (int)(found < expect ? found : expect);
+    P->scan_raw.push_back(*i);
+    P->scan_raw.push_back(end);
+    *i = end;
+    return code >= 0;
+}
+
 // Parses a whole stream: the headers up to the scan, then the scan's markers.  Returns false for a malformed stream
 // (reason set); else P->supported tells whether the device decodes it (reason: why not).  max_pixels bounds h * w.
-inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels, JpegParsed* P) {
+// progressive: progressive (SOF2) streams with 8-bit samples are parsed scan by scan (DESIGN.md 2.18) instead of being
+// refused as unsupported.
+inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels, JpegParsed* P, bool progressive = false) {
     *P = JpegParsed{};
     if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return jp_fail(P, "not a JPEG stream (no SOI marker)");
     struct Tables {
@@ -446,13 +765,20 @@ inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels
     bool jfif = false, exif_found = false;
     int ids[4] = {0}, hs[4] = {0}, vs[4] = {0}, tq[4] = {0};
     long long i = 2;
+    JpegProgTables PT{T.qt, T.counts, T.vals, T.nvals, 0, 0, 0, ids, tq, {false, false, false}};
     for (;;) {
+        // between the scans of a progressive stream, the end of the data stands for EOI (libjpeg's fill_input_buffer)
+        if (P->progressive && i >= n) break;
         if (i >= n || d[i] != 0xFF) return jp_fail(P, "malformed header: no marker at byte %lld", i);
         while (i < n && d[i] == 0xFF) ++i;
+        if (P->progressive && i >= n) break;
         if (i >= n) return jp_fail(P, "malformed header: the stream ends before the scan");
         const int m = d[i++];
+        if (P->progressive && m == 0xD9) break;
         if (m == 0xD8 || m == 0xD9) return jp_fail(P, "malformed header: marker 0xFF%02X before the scan", m);
         if ((m >= 0xD0 && m <= 0xD7) || m == 0x01) continue;        // parameterless markers
+        if (P->progressive && (i + 2 > n || i + ((d[i] << 8) | d[i + 1]) > n))
+            return jp_unsupported(P, "a marker segment cut off between scans");
         if (i + 2 > n) return jp_fail(P, "malformed header: the stream ends in marker 0xFF%02X", m);
         const long long len = (d[i] << 8) | d[i + 1];
         if (len < 2 || i + len > n) return jp_fail(P, "malformed header: segment 0xFF%02X of length %lld runs past the data", m, len);
@@ -523,6 +849,15 @@ inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels
             if (sof < 0) return jp_fail(P, "malformed header: SOS before SOF");
             const int ns = sl >= 1 ? s[0] : 0;
             if (ns < 1 || ns > 4 || sl != 4 + 2 * ns) return jp_fail(P, "malformed header: SOS segment of %lld bytes", sl);
+            if (P->progressive) {      // a later scan of a progressive stream
+                PT.qt_have = qt_have;
+                PT.huff_have = huff_have;
+                PT.restart = restart;
+                if (!jp_prog_sos(P, s, ns, PT)) return false;
+                if (P->reason[0]) return true;
+                if (!jpeg_prog_walk(d, n, &i, P)) break;
+                continue;
+            }
             P->scan_beg = i;
             if (P->h < 1 || (long long)P->h * P->w > max_pixels)
                 return jp_fail(P, "%d x %d pixels: a frame has 1 .. %lld pixels", P->h, P->w, max_pixels);
@@ -530,7 +865,8 @@ inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels
             fr_rotated_size(P->h, P->w, P->im.rot, &P->im.oh, &P->im.ow);
             char why[96];
             why[0] = 0;
-            if (sof == 0xC2 || sof == 0xC6) snprintf(why, sizeof(why), "progressive (SOF%d)", sof - 0xC0);
+            const bool prog = progressive && sof == 0xC2;
+            if ((sof == 0xC2 && !prog) || sof == 0xC6) snprintf(why, sizeof(why), "progressive (SOF%d)", sof - 0xC0);
             else if (sof == 0xC3 || sof == 0xC7) snprintf(why, sizeof(why), "lossless (SOF%d)", sof - 0xC0);
             else if (sof >= 0xC9) snprintf(why, sizeof(why), "arithmetic-coded (SOF%d)", sof - 0xC0);
             else if (sof == 0xC5) snprintf(why, sizeof(why), "hierarchical (SOF5)");
@@ -545,8 +881,20 @@ inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels
             if (nf == 3 && (!(hv == 11 || hv == 21 || hv == 22 || hv == 12 || hv == 41) || hs[1] != 1 || vs[1] != 1 ||
                             hs[2] != 1 || vs[2] != 1))
                 return jp_unsupported(P, "sampling other than luma 1x1, 2x1, 2x2, 1x2 or 4x1 with chroma 1x1");
-            if (ns != nf) return jp_unsupported(P, "a scan without every component (multi-scan sequential)");
             JpegImage& im = P->im;
+            if (prog) {                // the first scan of a progressive stream
+                jpeg_geometry(&im, P->h, P->w, nf, hs, vs);
+                P->progressive = true;
+                memset(P->bits, 0xFF, sizeof(P->bits));
+                PT.qt_have = qt_have;
+                PT.huff_have = huff_have;
+                PT.restart = restart;
+                if (!jp_prog_sos(P, s, ns, PT)) return false;
+                if (P->reason[0]) return true;
+                if (!jpeg_prog_walk(d, n, &i, P)) break;
+                continue;
+            }
+            if (ns != nf) return jp_unsupported(P, "a scan without every component (multi-scan sequential)");
             for (int c = 0; c < ns; ++c) {
                 const int td = s[2 + 2 * c] >> 4, ta = s[2 + 2 * c] & 15;
                 if (s[1 + 2 * c] != ids[c]) return jp_unsupported(P, "scan components in another order than the frame's");
@@ -561,31 +909,8 @@ inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels
                     return jp_fail(P, "malformed header: Huffman table DC %d / AC %d is not a valid code", td, ta);
                 memcpy(im.qt[c], T.qt[tq[c]], sizeof(im.qt[c]));
             }
-            for (int k = 0; k < 80; ++k) im.zz[k] = (unsigned char)jp_natural(k);
-            im.h = P->h;
-            im.w = P->w;
-            im.ncomp = nf;
+            jpeg_geometry(&im, P->h, P->w, nf, hs, vs);
             im.restart = restart;
-            im.hmax = nf == 3 ? hs[0] : 1;
-            im.vmax = nf == 3 ? vs[0] : 1;
-            im.mcux = (im.w + 8 * im.hmax - 1) / (8 * im.hmax);
-            im.mcuy = (im.h + 8 * im.vmax - 1) / (8 * im.vmax);
-            im.bpm = 0;
-            for (int c = 0; c < nf; ++c) {
-                JpegComp& cp = im.comp[c];
-                cp.h = nf == 3 ? hs[c] : 1;
-                cp.v = nf == 3 ? vs[c] : 1;
-                cp.bw = im.mcux * cp.h;
-                cp.bh = im.mcuy * cp.v;
-                cp.dw = (int)(((long long)im.w * cp.h + im.hmax - 1) / im.hmax);
-                cp.dh = (int)(((long long)im.h * cp.v + im.vmax - 1) / im.vmax);
-                for (int y = 0; y < cp.v; ++y)
-                    for (int x = 0; x < cp.h; ++x, ++im.bpm) {
-                        im.mcu_comp[im.bpm] = c;
-                        im.mcu_bx[im.bpm] = x;
-                        im.mcu_by[im.bpm] = y;
-                    }
-            }
             break;
         } else if (m == 0xDC || (m >= 0xE2 && m <= 0xEF) || m == 0xFE) {
             // DNL, other APPn, COM: skipped
@@ -593,40 +918,27 @@ inline bool jpeg_parse(const unsigned char* d, long long n, long long max_pixels
             return jp_fail(P, "malformed header: unknown marker 0xFF%02X", m);
         }
     }
-    // The scan: every 0xFF is a stuffed byte (FF 00), a restart marker (RSTn, ending a segment) or the marker after the
-    // scan; fill bytes (more 0xFF) may precede any of them.  `dropped` counts the bytes unstuffing removes.
+    if (P->progressive) {
+        // jdcoefct.c's block smoothing changes the output where bits of zig-zag coefficients 0 .. 9 are still unknown
+        // after the last scan; such streams are left to cv2
+        for (int c = 0; c < P->im.ncomp; ++c)
+            for (int k = 0; k < 10; ++k)
+                if (P->bits[c][k] != 0) {
+                    char why[120];
+                    snprintf(why, sizeof(why), "an incomplete progression (component %d, zig-zag coefficient %d: %s), "
+                             "which libjpeg smooths", c, k, P->bits[c][k] < 0 ? "never coded" : "low bits not coded");
+                    return jp_unsupported(P, why);
+                }
+        P->scan_beg = P->scan_raw.front();
+        P->scan_end = P->scan_raw.back();
+        P->supported = true;
+        return true;
+    }
     const long long mcus = (long long)P->im.mcux * P->im.mcuy;
     const long long expect = P->im.restart ? (mcus + P->im.restart - 1) / P->im.restart : 1;
-    long long dropped = 0, pos = P->scan_beg, rst = 0;
-    P->scan_end = n;
-    P->seg_beg.push_back(0);
-    while (pos < n) {
-        const void* f = memchr(d + pos, 0xFF, (size_t)(n - pos));
-        if (!f) break;
-        const long long a = (const unsigned char*)f - d;
-        long long j = a + 1;
-        while (j < n && d[j] == 0xFF) ++j;
-        if (j >= n) {
-            P->scan_end = a;
-            break;
-        }
-        const int code = d[j];
-        pos = j + 1;
-        if (code == 0x00) {
-            dropped += j - a;
-        } else if (code >= 0xD0 && code <= 0xD7) {
-            if (code != 0xD0 + (rst & 7)) P->status |= kJpegBadRestart;
-            ++rst;
-            P->seg_end.push_back(a - P->scan_beg - dropped);
-            dropped += j - a + 1;
-            P->seg_beg.push_back(j + 1 - P->scan_beg - dropped);
-        } else {
-            if (code == 0xDA) return jp_unsupported(P, "more than one scan");
-            P->scan_end = a;
-            break;
-        }
-    }
-    P->seg_end.push_back(P->scan_end - P->scan_beg - dropped);
+    int code;
+    P->scan_end = jpeg_scan_walk(d, n, P->scan_beg, &P->seg_beg, &P->seg_end, &P->status, &code);
+    if (code == 0xDA) return jp_unsupported(P, "more than one scan");
     if ((long long)P->seg_beg.size() != expect) P->status |= kJpegBadRestart;
     P->supported = true;
     return true;
@@ -652,6 +964,28 @@ inline long long jpeg_segments(const JpegParsed& P, int img, long long base, lon
         out->push_back(s);
     }
     return chunks;
+}
+
+// The scans of one parsed progressive image appended to *scans and their segments to *segs as JpegSeg entries (units
+// by the scan's restart interval), scan s's unstuffed data starting at scan_base[s]; seg0 indexes *segs.
+inline void jpeg_prog_segments(const JpegParsed& P, int img, const long long* scan_base, std::vector<JpegScan>* scans,
+                               std::vector<JpegSeg>* segs) {
+    for (size_t s = 0; s < P.scans.size(); ++s) {
+        JpegScan sc = P.scans[s];
+        const long long per = sc.restart ? sc.restart : sc.units;
+        const int first = sc.seg0;
+        sc.seg0 = (int)segs->size();
+        for (int k = 0; k < sc.nseg; ++k) {
+            JpegSeg g{};
+            g.img = img;
+            g.mcu0 = (int)(k * per);
+            g.mcus = (int)(sc.units - g.mcu0 < per ? sc.units - g.mcu0 : per);
+            g.beg = scan_base[s] + P.seg_beg[first + k];
+            g.end = scan_base[s] + P.seg_end[first + k];
+            segs->push_back(g);
+        }
+        scans->push_back(sc);
+    }
 }
 
 // The Huffman kernel's work for segments holding `chunks` chunks in all: the segment of every chunk, and runs of whole

@@ -149,21 +149,28 @@ def png_table(blobs):
     return jpeg_table(blobs, "png")
 
 
-def _stream_info(blob, codec):
+def _stream_info(blob, codec, progressive=False):
     a = _blob(blob, codec)
     h, w, sup = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    name = "b200pose_%s_info" % codec
-    nat.check(getattr(nat.lib(), name)(ctypes.c_void_p(a.ctypes.data), a.size, ctypes.byref(h), ctypes.byref(w),
-                                       ctypes.byref(sup)), name)
+    if progressive:
+        name = "b200pose_jpeg_info_ex"
+        rc = nat.lib().b200pose_jpeg_info_ex(ctypes.c_void_p(a.ctypes.data), a.size, 1, ctypes.byref(h), ctypes.byref(w),
+                                             ctypes.byref(sup))
+    else:
+        name = "b200pose_%s_info" % codec
+        rc = getattr(nat.lib(), name)(ctypes.c_void_p(a.ctypes.data), a.size, ctypes.byref(h), ctypes.byref(w),
+                                      ctypes.byref(sup))
+    nat.check(rc, name)
     reason = "" if sup.value else nat.lib().b200pose_last_error().decode()
     return h.value, w.value, bool(sup.value), reason
 
 
-def jpeg_info(blob):
+def jpeg_info(blob, progressive=False):
     """(h, w, supported, reason) of a JPEG stream on the host (b200pose_jpeg_info): the size of the frame
     cv2.imdecode returns, EXIF orientation applied, and whether the device decodes it (reason: why not).  Raises for a
-    malformed stream."""
-    return _stream_info(blob, "jpeg")
+    malformed stream.  progressive: whether a net decoding progressive streams (NativeNet.set_jpeg_progressive) would
+    (b200pose_jpeg_info_ex)."""
+    return _stream_info(blob, "jpeg", progressive)
 
 
 def png_info(blob):
@@ -235,6 +242,18 @@ class NativeNet:
         if name not in nat.PREPROCESS:
             raise nat.B200PoseError("unknown preprocess %r (expected one of %s)" % (name, sorted(nat.PREPROCESS)))
         nat.check(nat.lib().b200pose_net_set_preprocess(self._h, nat.PREPROCESS[name]), "b200pose_net_set_preprocess")
+
+    def set_jpeg_progressive(self, on):
+        """Whether decode_jpegs and PoseEngine.infer_jpegs* on this net decode progressive (SOF2) streams on the device
+        (b200pose_net_set_jpeg_progressive; default off: they are refused as unsupported)."""
+        nat.check(nat.lib().b200pose_net_set_jpeg_progressive(self._h, int(bool(on))), "b200pose_net_set_jpeg_progressive")
+
+    @property
+    def jpeg_progressive(self):
+        v = nat.lib().b200pose_net_get_jpeg_progressive(self._h)
+        if v < 0:
+            nat.check(1, "b200pose_net_get_jpeg_progressive")
+        return bool(v)
 
     def set_stages(self, k):
         """Refinement stages every later forward runs: the trunk, stage 1 and stages 2 .. k (1 <= k <= 6, default 6).
@@ -335,7 +354,8 @@ class NativeNet:
 
     def _decode(self, blobs, codec, device, stream):
         ptrs, sizes, keep = jpeg_table(blobs, codec)
-        shapes = [_stream_info(b, codec)[:2] for b in keep]
+        prog = codec == "jpeg" and self.jpeg_progressive
+        shapes = [_stream_info(b, codec, prog)[:2] for b in keep]
         total = sum(h * w * 3 for h, w in shapes)
         if device:
             import torch
@@ -696,12 +716,14 @@ class PoseEngine:
     fp16 are refused here.  `post_params`: the
     post-processing settings of the submissions (a dict of NativePost.set_params' fields; None: the reference's
     constants), changed later with set_post_params.  `refine`: the peak refinement of the submissions ('cubic',
-    'gauss' or 'none', NativePost.set_refine), changed later with set_refine."""
+    'gauss' or 'none', NativePost.set_refine), changed later with set_refine.  `jpeg_progressive`: whether the JPEG
+    entry points decode progressive streams on the device (NativeNet.set_jpeg_progressive, set on the net before each
+    JPEG submission), changed later with set_jpeg_progressive."""
 
     stages = 6
 
     def __init__(self, state_arrays, device_index=0, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, net=None,
-                 stages=None, post_params=None, refine="cubic"):
+                 stages=None, post_params=None, refine="cubic", jpeg_progressive=False):
         if refine not in REFINE_MODES:      # before any allocation
             raise nat.B200PoseError("refine must be one of %s, got %r" % (", ".join(map(repr, REFINE_MODES)), refine))
         if net is None:
@@ -725,6 +747,7 @@ class PoseEngine:
         self.post.set_refine(refine)
         self.mode = nat.MODES[mode]
         self.device_index = device_index
+        self.jpeg_progressive = bool(jpeg_progressive)
         self._shapes = {}
         self._last = None
 
@@ -744,6 +767,11 @@ class PoseEngine:
         """Peak refinement of the following submissions ('cubic', 'gauss' or 'none'; see NativePost.set_refine).  Runs
         already submitted keep theirs."""
         self.post.set_refine(mode)
+
+    def set_jpeg_progressive(self, on):
+        """Whether the following JPEG submissions decode progressive (SOF2) streams on the device; off, infer_jpegs
+        decodes them with cv2.imdecode and infer_jpegs_async refuses them."""
+        self.jpeg_progressive = bool(on)
 
     def _remember(self, n, H, W):
         """Shape of the run just submitted, kept per ticket (two runs may be in flight with different batch sizes or
@@ -767,10 +795,10 @@ class PoseEngine:
 
     @classmethod
     def from_net(cls, net, mode="bf16", batch_cap=32, peak_cap=1024, human_cap=1024, stages=None, post_params=None,
-                 refine="cubic"):
+                 refine="cubic", jpeg_progressive=False):
         """An engine around an existing NativeNet (e.g. the one a get_model() module already packed its weights into)."""
         return cls(None, net.device_index, mode, batch_cap, peak_cap, human_cap, net=net, stages=stages,
-                   post_params=post_params, refine=refine)
+                   post_params=post_params, refine=refine, jpeg_progressive=jpeg_progressive)
 
     def submit_images(self, images, dest_size=368, factor=8, thresh=0.1, flip=False):
         """Asynchronous half of infer_images for frames of ONE shape (a video stream): returns a ticket; the frames must
@@ -839,7 +867,8 @@ class PoseEngine:
     def infer_jpegs_async(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, stream=0):
         """JPEG streams decoded on the device and run as infer_raw_* does on the decoded frames (b200pose_infer_jpegs):
         uniform when every frame has one size, ragged otherwise; scales as for infer_images.  At most batch_cap
-        streams, all of which the device decodes (jpeg_info).  Returns a ticket; fetch / fetch_arrays raise, naming the
+        streams, all of which the device decodes (jpeg_info, progressive streams too when jpeg_progressive is on).
+        Returns a ticket; fetch / fetch_arrays raise, naming the
         images, when an image's entropy-coded data is damaged.  Person coordinates refer to each decoded frame's
         padded frame."""
         return self._infer_streams_async("jpeg", blobs, dest_size, factor, thresh, flip, scales, stream)
@@ -850,9 +879,20 @@ class PoseEngine:
         raise, naming the images, when an image's data is damaged (where cv2.imdecode returns None)."""
         return self._infer_streams_async("png", blobs, dest_size, factor, thresh, flip, scales, stream)
 
+    def _progressive(self, codec):
+        """Whether this engine's submissions of `codec` streams decode progressive JPEG: the net's switch is set to the
+        engine's before each JPEG submission, as the stage count is (engines may share a net)."""
+        if codec != "jpeg":
+            return False
+        prog = bool(self.__dict__.get("jpeg_progressive", False))
+        if self.net.jpeg_progressive != prog:
+            self.net.set_jpeg_progressive(prog)
+        return prog
+
     def _infer_streams_async(self, codec, blobs, dest_size, factor, thresh, flip, scales, stream):
         ptrs, sizes, keep = jpeg_table(blobs, codec)
-        shapes = [_stream_info(b, codec)[:2] for b in keep]
+        prog = self._progressive(codec)
+        shapes = [_stream_info(b, codec, prog)[:2] for b in keep]
         arr = None if scales is None else (ctypes.c_double * len(scales))(*[float(s) for s in scales])
         name = "b200pose_infer_%ss" % codec
         nat.check(getattr(nat.lib(), name)(self._net_h(), self.post._h, ptrs, sizes, len(keep), int(dest_size),
@@ -888,7 +928,8 @@ class PoseEngine:
     def infer_jpegs(self, blobs, dest_size=368, factor=8, thresh=0.1, flip=False, scales=None, _arrays=False):
         """infer_images([cv2.imdecode(b, cv2.IMREAD_COLOR) for b in blobs]) with the decoding on the device: per-image
         human lists in input order.  Streams are grouped by plan_ragged_batches on their decoded padded sizes
-        (jpeg_info); streams the device does not decode (progressive, CMYK, ...) are decoded by cv2.imdecode and run
+        (jpeg_info); streams the device does not decode (CMYK, progressive unless jpeg_progressive is on, ...) are
+        decoded by cv2.imdecode and run
         through infer_images - a frame's result does not depend on its batch.  Malformed streams raise, and so do
         streams whose entropy-coded data is damaged, naming the image."""
         return self._infer_streams("jpeg", blobs, dest_size, factor, thresh, flip, scales, _arrays)
@@ -906,9 +947,10 @@ class PoseEngine:
 
     def _infer_streams(self, codec, blobs, dest_size, factor, thresh, flip, scales, _arrays):
         infos = []
+        prog = self._progressive(codec)
         for i, b in enumerate(blobs):
             try:
-                infos.append(_stream_info(b, codec))
+                infos.append(_stream_info(b, codec, prog))
             except nat.B200PoseError as e:
                 raise nat.B200PoseError("infer_%ss: image %d: %s" % (codec, i, e)) from None
         dev = [i for i, inf in enumerate(infos) if inf[2]]

@@ -37,7 +37,8 @@ def card():
     return r.stdout.strip().split("\n")[0]
 
 
-def collection(seed=7):
+def collection(seed=7, progressive=False):
+    """96 seeded JPEG streams of bench_mixed.py's shapes; progressive: written progressive by cv2 instead."""
     import cv2
     rng = np.random.default_rng(seed)
     blobs = []
@@ -53,7 +54,8 @@ def collection(seed=7):
         r = rng.random()
         sf = 0x221111 if r < 0.8 else (0x111111 if r < 0.9 else 0x211111)
         ok, buf = cv2.imencode(".jpg", img, [cv2.IMWRITE_JPEG_QUALITY, int(rng.integers(75, 96)),
-                                            cv2.IMWRITE_JPEG_SAMPLING_FACTOR, sf])
+                                            cv2.IMWRITE_JPEG_SAMPLING_FACTOR, sf,
+                                            cv2.IMWRITE_JPEG_PROGRESSIVE, int(progressive)])
         blobs.append(buf.tobytes())
     return blobs
 
