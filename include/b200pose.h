@@ -540,6 +540,37 @@ int b200pose_infer_pngs(b200pose_net* net, b200pose_post* post, const unsigned c
 int b200pose_post_png_status(b200pose_post* post, int img);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3k. Training targets and stage losses: replace CocoKeypoints.get_ground_truth (lib/datasets/datasets.py:259-308) +
+ *     transpose((2, 0, 1)).astype(float32), and get_loss's MSEs (train/train_VGG19.py:143-174)   (DESIGN.md 2.19)
+ *   b200pose_ground_truth: keypoints (host) [sum persons][17][3] float32, COCO order, the persons of image 0 first;
+ *     persons[n] per image; hw[2n] = (input_y, input_x) per image.  Writes heat [n][19][canvas_h][canvas_w] and
+ *     paf [n][38][canvas_h][canvas_w] float32 (device pointers), asynchronously on cuda_stream: image i fills the
+ *     top-left int(input_y / 8) x int(input_x / 8) of its slot, bit for bit the reference's maps, +0 outside.  The
+ *     stage maps' own layout, ragged batches included (canvas = max H_i / 8, max W_i / 8).  An image without persons
+ *     gets zero PAFs and a background of 1.0 (the reference raises IndexError there).  Refused, naming the argument,
+ *     before anything is enqueued: n outside 1 .. 1024, persons outside 0 .. 256 per image, a side outside 8 .. 8192,
+ *     non-finite keypoints, a canvas below an image's grid or above 1024 x 1024 cells.  heat and paf both NULL: the arguments are checked and
+ *     nothing else happens.  One call: one upload and 2 kernels.
+ *   b200pose_net_last_forward: what the net's last forward ran (any entry point): info[4] = n images, canvas H, canvas
+ *     W (input pixels) and the stage maps it wrote (2k for k rtpose stages, l2 + l1 for OpenPose_Model); hw (may be
+ *     NULL; hw_cap >= 2n) gets each image's extent {H_i, W_i}, the canvas for a uniform forward.  Later set_stages calls
+ *     do not change it.  No forward yet: refused.
+ *   b200pose_net_stage_losses: for the net's last forward (n images, canvas Hc x Wc, k stages or an OpenPose_Model's
+ *     maps), with heat / paf its targets in the layout above at the forward's canvas (device pointers), writes on
+ *     cuda_stream sums[n][maps] (double, device; `maps` must be the count b200pose_net_last_forward reports, anything
+ *     else is refused): per (image, stage map in saved_for_loss order) the float64 sum of the
+ *     float32 (pred - target)^2 over the image's own (H_i / 8) x (W_i / 8) cells, the PAF maps against paf and the heat
+ *     maps against heat; and extrema[n][4] (float, device): max and min of the final heat map's channels 0 .. 17, then
+ *     max and min of the final PAF map, over the image's own cells.  The sums are added in a fixed order without
+ *     atomics: they depend on neither the canvas nor the other images.  One kernel.  No forward yet: refused.
+ * ---------------------------------------------------------------------------------------------------------- */
+int b200pose_ground_truth(int device, const float* keypoints, const int* persons, const int* hw, int n, float* heat,
+                          float* paf, int canvas_h, int canvas_w, void* cuda_stream);
+int b200pose_net_last_forward(b200pose_net* net, int* info, int* hw, int hw_cap);
+int b200pose_net_stage_losses(b200pose_net* net, const float* heat, const float* paf, double* sums, int maps,
+                              float* extrema, void* cuda_stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

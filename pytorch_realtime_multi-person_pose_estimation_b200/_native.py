@@ -99,6 +99,9 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_net_encode_pngs": ([vp, vp, ci, vp, ci, vp, ctypes.c_longlong, ci, vp, vp], ci),
     "b200pose_coco_kpt_eval": ([ci, ci, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp,
                                 ctypes.c_longlong, vp], ci),
+    "b200pose_ground_truth": ([ci, vp, vp, vp, ci, vp, vp, ci, ci, vp], ci),
+    "b200pose_net_last_forward": ([vp, vp, vp, ci], ci),
+    "b200pose_net_stage_losses": ([vp, vp, vp, vp, ci, vp, vp], ci),
     "process_paf": ([ci, ci, ci, vp, ci, ci, ci, vp, ci, ci, ci, vp], ci),
     "get_num_humans": ([], ci),
     "get_part_cid": ([ci, ci], ci),

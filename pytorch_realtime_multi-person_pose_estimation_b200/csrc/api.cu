@@ -24,6 +24,7 @@
 #include "f16_core.h"
 #include "draw.cuh"
 #include "frames.cuh"
+#include "gt.cuh"
 #include "jpeg.cuh"
 #include "jpeg_enc.cuh"
 #include "png_enc.cuh"
@@ -412,6 +413,7 @@ struct LastForward {
     const void* in = nullptr;    // device input
     int in_u8 = 0;               // normalisation of a uint8 input fused into conv1_1 (0: fp32 input)
     const int* ext = nullptr;    // extents table of a ragged forward, null: uniform
+    std::vector<int> ext_host;   // ... and its host copy {H_0, W_0, ...} (empty: uniform)
 };
 
 }  // namespace
@@ -453,6 +455,7 @@ struct b200pose_net {
     // Allocated once for kMaxRagged images and never moved, so that plans and captured graphs stay valid across mixes;
     // rewritten on the stream before each ragged forward.
     DevBuf<int> d_ext;
+    std::vector<int> ext_host;     // what upload_ext last wrote into d_ext
     DevBuf<RaggedFrame> d_frames;      // frame table (per-frame source geometry) of the last crop or uint8 mirror
     // video frames (b200pose_net_convert_frames, b200pose_infer_frames): the planes of host frames, packed, and the
     // source table of the last conversion
@@ -1224,7 +1227,8 @@ static int net_forward_impl(b200pose_net* net, const void* input, int in_u8, int
         rc = forward_tc(net, d_in, first_u8, n, H, W, fmt, stages, st, ext);
     }
     if (rc) return rc;
-    net->last = LastForward{n, H, W, mode == B200POSE_MODE_FP32, fmt, stages, d_in, first_u8, ext};
+    net->last = LastForward{n, H, W, mode == B200POSE_MODE_FP32, fmt, stages, d_in, first_u8, ext,
+                            ext ? net->ext_host : std::vector<int>()};
     if (outputs) {
         const size_t px8 = (size_t)n * (H / 8) * (W / 8);
         for (int i = 0; i < net->arch.out[stages].maps; ++i)
@@ -1267,6 +1271,7 @@ static int ragged_canvas(int n, const int* hw, int* Hc, int* Wc) {
 static int upload_ext(b200pose_net* net, const std::vector<int>& ext, cudaStream_t st) {
     CU(net->d_ext.ensure((size_t)kMaxRagged * 2));
     CU(cudaMemcpyAsync(net->d_ext.p, ext.data(), ext.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    net->ext_host = ext;
     return 0;
 }
 
@@ -3140,6 +3145,111 @@ int b200pose_coco_kpt_eval(int device, int n_units, int n_cats, const int* unit_
     CU(cudaStreamSynchronize(st));
     if (oks_count) *oks_count = oks_n;
     return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ training targets, stage losses
+int b200pose_ground_truth(int device, const float* keypoints, const int* persons, const int* hw, int n, float* heat,
+                          float* paf, int canvas_h, int canvas_w, void* cuda_stream) {
+    if (n < 1 || n > kGtMaxImages) return fail("ground_truth: %d images (1 .. %d)", n, kGtMaxImages);
+    if (!persons || !hw) return fail("ground_truth: null persons / sizes");
+    long long total = 0;
+    int gh_max = 0, gw_max = 0;
+    for (int i = 0; i < n; ++i) {
+        if (persons[i] < 0 || persons[i] > kGtMaxPersons)
+            return fail("ground_truth: persons of image %d = %d (0 .. %d)", i, persons[i], kGtMaxPersons);
+        if (hw[2 * i] < kGtStride || hw[2 * i] > kGtMaxSize || hw[2 * i + 1] < kGtStride || hw[2 * i + 1] > kGtMaxSize)
+            return fail("ground_truth: sizes of image %d = %d x %d (each side %d .. %d)", i, hw[2 * i], hw[2 * i + 1],
+                        kGtStride, kGtMaxSize);
+        total += persons[i];
+        gh_max = std::max(gh_max, gt_grid(hw[2 * i]));
+        gw_max = std::max(gw_max, gt_grid(hw[2 * i + 1]));
+    }
+    if (total && !keypoints) return fail("ground_truth: null keypoints");
+    for (long long k = 0; k < total * kGtCocoParts * 3; ++k)
+        if (!std::isfinite(keypoints[k]))
+            return fail("ground_truth: keypoints of person %lld (of the call) are not finite", k / (kGtCocoParts * 3));
+    if (canvas_h < gh_max || canvas_w < gw_max)
+        return fail("ground_truth: canvas %d x %d below the largest grid %d x %d", canvas_h, canvas_w, gh_max, gw_max);
+    if (canvas_h > kGtMaxSize / kGtStride || canvas_w > kGtMaxSize / kGtStride)
+        return fail("ground_truth: canvas %d x %d above %d x %d cells", canvas_h, canvas_w, kGtMaxSize / kGtStride,
+                    kGtMaxSize / kGtStride);
+    if (!heat && !paf) return 0;      // arguments checked, nothing to write
+    if (!heat || !paf) return fail("ground_truth: null heat / paf");
+    // one upload: the images, then every person's 18 joints (add_neck, our_order, remove_illegal_joint on the host)
+    const size_t o_joints = ((size_t)n * sizeof(GtImage) + 255) & ~(size_t)255;
+    std::vector<char> up(o_joints + (size_t)total * kGtParts * 3 * sizeof(float));
+    GtImage* im = reinterpret_cast<GtImage*>(up.data());
+    float* jo = reinterpret_cast<float*>(up.data() + o_joints);
+    for (int i = 0, j0 = 0; i < n; j0 += persons[i++]) {
+        im[i] = {j0, persons[i], gt_grid(hw[2 * i]), gt_grid(hw[2 * i + 1])};
+        for (int p = j0; p < j0 + persons[i]; ++p)
+            gt_person_joints(keypoints + (size_t)p * kGtCocoParts * 3, hw[2 * i + 1], hw[2 * i], jo + (size_t)p * kGtParts * 3);
+    }
+    CU(cudaSetDevice(device));
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    void* d = nullptr;
+    CU(cudaMallocAsync(&d, up.size(), st));
+    GtBatch b;
+    b.images = reinterpret_cast<const GtImage*>(d);
+    b.joints = reinterpret_cast<const float*>(static_cast<char*>(d) + o_joints);
+    b.n = n;
+    b.ch = canvas_h;
+    b.cw = canvas_w;
+    b.heat = heat;
+    b.paf = paf;
+    cudaError_t e = cudaMemcpyAsync(d, up.data(), up.size(), cudaMemcpyHostToDevice, st);
+    int rc = e != cudaSuccess ? cuda_fail("ground_truth: upload: %s", cudaGetErrorString(e))
+                              : launched(gt_launch(b, st), "gt_launch", kGtLaunches);
+    cudaError_t ef = cudaFreeAsync(d, st);
+    if (!rc && ef != cudaSuccess) rc = cuda_fail("ground_truth: cudaFreeAsync: %s", cudaGetErrorString(ef));
+    return rc;
+}
+
+int b200pose_net_last_forward(b200pose_net* net, int* info, int* hw, int hw_cap) {
+    if (!net || net->last.n == 0) return fail("last_forward: no forward has run");
+    if (!info) return fail("last_forward: null info");
+    const LastForward& l = net->last;
+    info[0] = l.n;
+    info[1] = l.H;
+    info[2] = l.W;
+    info[3] = net->arch.out[l.stages].maps;
+    if (hw) {
+        if (hw_cap < 2 * l.n) return fail("last_forward: hw_cap %d below 2 x %d images", hw_cap, l.n);
+        for (int i = 0; i < l.n; ++i) {
+            hw[2 * i] = l.ext_host.empty() ? l.H : l.ext_host[2 * i];
+            hw[2 * i + 1] = l.ext_host.empty() ? l.W : l.ext_host[2 * i + 1];
+        }
+    }
+    return 0;
+}
+
+int b200pose_net_stage_losses(b200pose_net* net, const float* heat, const float* paf, double* sums, int maps,
+                              float* extrema, void* cuda_stream) {
+    if (!net || net->last.n == 0) return fail("stage_losses: no forward has run");
+    if (!heat || !paf) return fail("stage_losses: null heat / paf targets");
+    if (!sums || !extrema) return fail("stage_losses: null sums / extrema");
+    const auto& out = net->arch.out[net->last.stages];
+    if (maps != out.maps)
+        return fail("stage_losses: maps = %d, but the last forward wrote %d stage maps (sums is [n][%d])", maps, out.maps,
+                    out.maps);
+    GtLossBatch b;
+    b.n_maps = out.maps;
+    for (int m = 0; m < kGtMaxMaps; ++m) {
+        b.maps[m] = m < out.maps ? net->out_f32[m].p : nullptr;
+        b.ch[m] = m < out.maps ? net->arch.map_ch[m] : 0;
+    }
+    b.n = net->last.n;
+    b.mh = net->last.H / 8;
+    b.mw = net->last.W / 8;
+    b.ext = net->last.ext;
+    b.last_paf = out.paf;
+    b.last_heat = out.heat;
+    b.heat = heat;
+    b.paf = paf;
+    b.sums = sums;
+    b.extrema = extrema;
+    CU(cudaSetDevice(net->device));
+    return launched(gt_stage_loss_launch(b, static_cast<cudaStream_t>(cuda_stream)), "gt_stage_loss_launch");
 }
 
 // ------------------------------------------------------------------------------------------------ legacy pafprocess

@@ -198,6 +198,52 @@ def rotated_size(h, w, rotate):
     return (w, h) if rotate in (90, 270) else (h, w)
 
 
+GT_MAX_IMAGES, GT_MAX_PERSONS = 1024, 256      # b200pose_ground_truth's capacities
+
+
+def ground_truth(keypoints_per_image, sizes, device_index=0, canvas=None):
+    """CocoKeypoints.get_ground_truth (lib/datasets/datasets.py:259-308) + transpose((2, 0, 1)).astype(float32) for a
+    batch of images, on the device, bit for bit the reference's maps (DESIGN.md 2.19).  keypoints_per_image[i]: the
+    image's annotations' keypoints, [P_i, 17, 3] (or [P_i, 51]) in COCO order, as float32 after transforms.Normalize;
+    sizes[i] = (input_y, input_x).  Returns CUDA float32 tensors heat [n, 19, gh, gw] and paf [n, 38, gh, gw] on
+    cuda:device_index, written on its current stream, at the canvas grid (max int(input_y / 8), max int(input_x / 8)),
+    or `canvas` = (gh, gw) if given: image i fills the top-left of its slot, +0 outside.  An image without persons gets
+    zero PAFs and a background of 1 (the reference raises IndexError)."""
+    import torch
+    kps = [np.ascontiguousarray(k, dtype=np.float32).reshape(-1, 17, 3) for k in keypoints_per_image]
+    hw = np.ascontiguousarray(np.asarray(sizes, dtype=np.int64).reshape(-1, 2).astype(np.int32))
+    if len(kps) != len(hw):
+        raise nat.B200PoseError("ground_truth: %d keypoint arrays for %d sizes" % (len(kps), len(hw)))
+    n = len(hw)
+    table = np.ascontiguousarray(np.concatenate(kps) if n else np.zeros((0, 17, 3), np.float32))
+    counts = np.array([len(k) for k in kps], np.int32)
+    gh, gw = canvas or ((int(hw[:, 0].max()) // 8, int(hw[:, 1].max()) // 8) if n else (0, 0))
+    L = nat.lib()
+    args = (table.ctypes.data, counts.ctypes.data, hw.ctypes.data, n)
+    nat.check(L.b200pose_ground_truth(int(device_index), *args, None, None, gh, gw, None), "b200pose_ground_truth")
+    dev = torch.device("cuda", int(device_index))
+    heat = torch.empty((n, 19, gh, gw), dtype=torch.float32, device=dev)
+    paf = torch.empty((n, 38, gh, gw), dtype=torch.float32, device=dev)
+    nat.check(L.b200pose_ground_truth(int(device_index), *args, ctypes.c_void_p(heat.data_ptr()),
+                                      ctypes.c_void_p(paf.data_ptr()), gh, gw,
+                                      ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "b200pose_ground_truth")
+    return heat, paf
+
+
+def _loss_dict(names_flags, sums, extrema, cells):
+    """get_loss's saved_for_log from per-map squared-error sums over `cells` cells per channel and per-image extrema."""
+    from collections import OrderedDict
+    names, is_paf = names_flags
+    out = OrderedDict()
+    for name, s, p in zip(names, sums, is_paf):
+        out[name] = float(s) / ((38 if p else 19) * cells)
+    out["total_loss"] = float(sum(out[k] for k in names))
+    ext = np.asarray(extrema, np.float32).reshape(-1, 4)
+    out["max_ht"], out["min_ht"] = float(ext[:, 0].max()), float(ext[:, 1].min())
+    out["max_paf"], out["min_paf"] = float(ext[:, 2].max()), float(ext[:, 3].min())
+    return out
+
+
 class NativeNet:
     """Owns a b200pose_net handle on one CUDA device: the rtpose VGG19 network, or OpenPose_Model(l2, l1) for a net
     made by NativeNet.openpose."""
@@ -283,6 +329,65 @@ class NativeNet:
         nat.check(nat.lib().b200pose_net_forward_ragged_u8(self._h, ctypes.c_void_p(in_ptr), int(in_on_device), len(shapes),
                                                            hw, mode, arr, int(out_on_device), ctypes.c_void_p(stream)),
                   "b200pose_net_forward_ragged_u8")
+
+    def stage_map_names(self, maps=None):
+        """Names of `maps` stage maps in saved_for_loss order, as get_loss logs them: loss_stage{j}_L1 (PAF) and
+        loss_stage{j}_L2 (heat) for rtpose's stages j; loss_paf_{t} / loss_heat_{t} after OpenPose_Model's outputs
+        paf_1 .. paf_l2, heat_1 .. heat_l1.  maps=None: the maps the net's next forward writes (its stage setting).
+        Returns (names, is_paf flags)."""
+        if self.openpose_stages is not None:
+            l2, l1 = self.openpose_stages
+            return (["loss_paf_%d" % t for t in range(1, l2 + 1)] + ["loss_heat_%d" % t for t in range(1, l1 + 1)],
+                    [True] * l2 + [False] * l1)
+        k = self.__dict__.get("_stages", 6) if maps is None else int(maps) // 2
+        return ["loss_stage%d_L%d" % (j, b) for j in range(1, k + 1) for b in (1, 2)], [True, False] * k
+
+    def last_forward(self):
+        """What the net's last forward ran, whichever entry point ran it (b200pose_net_last_forward): (n, canvas H,
+        canvas W, stage maps written, [(H_i, W_i)] per image).  A later set_stages does not change it."""
+        L = nat.lib()
+        info = (ctypes.c_int * 4)()
+        if L.b200pose_net_last_forward(self._h, info, None, 0):
+            nat.check(1, "b200pose_net_last_forward")
+        n = info[0]
+        hw = (ctypes.c_int * (2 * n))()
+        nat.check(L.b200pose_net_last_forward(self._h, info, hw, 2 * n), "b200pose_net_last_forward")
+        return n, info[1], info[2], info[3], [(hw[2 * i], hw[2 * i + 1]) for i in range(n)]
+
+    def stage_loss_sums(self, heat, paf):
+        """Device half of stage_losses for the last forward, targets heat [n, 19, Hc/8, Wc/8] / paf [n, 38, Hc/8, Wc/8]
+        CUDA float32 tensors at its canvas (as ground_truth makes them): (sums float64 [n, maps], extrema float32
+        [n, 4], cells per image, (names, is_paf)).  The map count and the frames' extents are the last forward's own, as
+        the library reports them."""
+        import torch
+        L = nat.lib()
+        if L.b200pose_net_last_forward(self._h, (ctypes.c_int * 4)(), None, 0):
+            nat.check(L.b200pose_net_stage_losses(self._h, None, None, None, 0, None, None), "b200pose_net_stage_losses")
+        n, H, W, maps, extents = self.last_forward()
+        h, w = H // 8, W // 8
+        for name, t, c in (("heat", heat, 19), ("paf", paf, 38)):
+            if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
+                    or tuple(t.shape) != (n, c, h, w)):
+                raise nat.B200PoseError("stage_losses: %s must be a contiguous CUDA float32 tensor [%d, %d, %d, %d] (the "
+                                        "last forward's maps), got %s" % (name, n, c, h, w, getattr(t, "shape", type(t))))
+        dev = heat.device
+        sums = torch.empty((n, maps), dtype=torch.float64, device=dev)
+        ext = torch.empty((n, 4), dtype=torch.float32, device=dev)
+        nat.check(L.b200pose_net_stage_losses(self._h, ctypes.c_void_p(heat.data_ptr()), ctypes.c_void_p(paf.data_ptr()),
+                                              ctypes.c_void_p(sums.data_ptr()), maps, ctypes.c_void_p(ext.data_ptr()),
+                                              ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                  "b200pose_net_stage_losses")
+        return (sums.cpu().numpy(), ext.cpu().numpy(), [(a // 8) * (b // 8) for a, b in extents],
+                self.stage_map_names(maps))
+
+    def stage_losses(self, heat, paf):
+        """get_loss (train/train_VGG19.py:143-174) for the last forward against targets heat / paf (ground_truth's
+        tensors at the forward's canvas): an OrderedDict of each stage map's MSE (nn.MSELoss's mean over all cells of the
+        batch; a ragged frame counts its own cells only), keyed as get_loss's saved_for_log for the maps that forward
+        wrote (stage_map_names), then total_loss (their sum), max_ht, min_ht (the final heat map's channels 0 .. 17),
+        max_paf and min_paf."""
+        sums, ext, cells, names = self.stage_loss_sums(heat, paf)
+        return _loss_dict(names, sums.sum(0), ext, sum(cells))
 
     def overflow(self, n, stream=0):
         """Per image of the last forward (n = its batch): True if the fp16 mode overflowed binary16 for it.  Waits for
@@ -1091,6 +1196,62 @@ class PoseEngine:
             for i, humans in zip(part, self.fetch_arrays() if _arrays else self.fetch()):
                 out[i] = humans.copy() if _arrays else humans
         return out
+
+    def validation_loss(self, images, keypoints, dest_size=368, factor=8):
+        """A deterministic validate() (train/train_VGG19.py:233-278) over images of any sizes: get_loss's MSEs as dataset
+        means (each stage map's squared-error sum over all images, divided by all their cells), keyed as stage_losses
+        keys them, with total_loss and the extrema over the whole set.  This is the inference geometry, not the
+        reference's validation protocol, which draws a random flip, crop and colour jitter per image: each frame is
+        crop_with_factor(image, dest_size, factor)-ed on the device (resize to dest_size on its long side, pad to a
+        multiple of factor) and runs through the net in this engine's mode and the net's normalisation, in ragged
+        batches of at most batch_cap frames.  keypoints[i]: image i's annotations' keypoints [P_i, 17, 3] in its source
+        pixels, mapped as RescaleRelative.scale maps them, (k + 0.5) * s - 0.5 in float32 with s the resized over the
+        source size per axis; the targets are ground_truth's at each padded frame's size."""
+        import torch
+        if len(images) != len(keypoints):
+            raise nat.B200PoseError("validation_loss: %d images but %d keypoint arrays" % (len(images), len(keypoints)))
+        if not len(images):
+            raise nat.B200PoseError("validation_loss: images is empty")
+        for im in images:
+            if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+                raise nat.B200PoseError("validation_loss: expected uint8 [h,w,3] frames")
+        h_net = self._net_h()
+        L = nat.lib()
+        dev = torch.device("cuda", self.device_index)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        geo = [nat.crop_geometry(im.shape[0], im.shape[1], dest_size, factor) for im in images]
+        sums, extrema, cells, names = 0.0, [], 0, None
+        for part in plan_ragged_batches([g[2] for g in geo], self.post.batch_cap):
+            # the part's sources in one upload; each frame cropped on the device straight into the packed batch
+            src = torch.from_numpy(np.concatenate([np.ascontiguousarray(images[i]).ravel() for i in part])).to(dev)
+            shapes = [geo[i][2] for i in part]
+            batch = torch.empty(sum(h * w * 3 for h, w in shapes), dtype=torch.uint8, device=dev)
+            s_at, b_at, kps = 0, 0, []
+            for i, (ph, pw) in zip(part, shapes):
+                sh, sw = images[i].shape[:2]
+                nat.check(L.b200pose_net_crop_with_factor(h_net, ctypes.c_void_p(src.data_ptr() + s_at), 1, 1, sh, sw,
+                                                          int(dest_size), int(factor),
+                                                          ctypes.c_void_p(batch.data_ptr() + b_at), 1,
+                                                          ctypes.c_void_p(stream)), "b200pose_net_crop_with_factor")
+                s_at += sh * sw * 3
+                b_at += ph * pw * 3
+                (rh, rw) = geo[i][1]
+                k = np.array(keypoints[i], dtype=np.float32).reshape(-1, 17, 3)
+                for ax, sc in ((0, rw / sw), (1, rh / sh)):
+                    k[:, :, ax] = (k[:, :, ax] + np.float32(0.5)) * np.float32(sc) - np.float32(0.5)
+                kps.append(k)
+            if len(set(shapes)) == 1:
+                self.net.forward_u8_ptr(batch.data_ptr(), True, len(part), shapes[0][0], shapes[0][1], self.mode,
+                                        [None] * 12, True, stream)
+            else:
+                self.net.forward_ragged_u8_ptr(batch.data_ptr(), True, shapes, self.mode, [None] * 12, True, stream)
+            canvas = (max(h for h, _ in shapes) // 8, max(w for _, w in shapes) // 8)
+            heat, paf = ground_truth(kps, shapes, self.device_index, canvas)
+            s, e, c, names = self.net.stage_loss_sums(heat, paf)
+            sums = sums + s.sum(0)
+            extrema.append(e)
+            cells += sum(c)
+        return _loss_dict(names, sums, np.concatenate(extrema), cells)
 
     def fetch(self, check=True, ticket=None):
         """Results of run `ticket` (default: the latest).  Up to two runs may be in flight: submit i+1, then fetch i."""
