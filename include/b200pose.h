@@ -571,6 +571,35 @@ int b200pose_net_stage_losses(b200pose_net* net, const float* heat, const float*
                               float* extrema, void* cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3l. Training batches: replace the reference loader's per-sample image path, preprocess = Normalize,
+ *     RandomApply(HFlip, 0.5), RescaleRelative (Pillow BICUBIC), Crop(edge), CenterPad(edge) (train/train_VGG19.py:124-130,
+ *     lib/datasets/transforms.py), then image_transform_train = ColorJitter(0.1, 0.1, 0.1, 0.1), a JPEG quality-50
+ *     round trip, RandomGrayscale(0.01), ToTensor + Normalize (transforms.py:53-65), and mask_valid_area
+ *     (lib/datasets/utils.py:36-54)   (DESIGN.md 2.20)
+ *   b200pose_net_augment: frames: n uint8 BGR frames packed back to back (host, or device with frames_on_device),
+ *     hw[2n] = (h, w) each; params[n][B200POSE_AUG_PARAMS] the draws of each sample, as engine.augment_params makes
+ *     them: hflip, resized w, resized h, crop x, crop y, ColorJitter's order (4 fn ids), brightness, contrast,
+ *     saturation and hue factors, jpeg, grayscale, and the mask bounds x0, y0, x1, y1 (columns < x0 or >= x1 and rows
+ *     < y0 or >= y1 become 0).  Writes out_f32 [n][3][edge][edge] (RGB, normalised, masked) and, unless out_u8 is
+ *     NULL, out_u8 [n][edge][edge][3] (the BGR image ToTensor receives), bit for bit the reference's tensors; device
+ *     pointers with out_on_device (written asynchronously on cuda_stream unless a sample drew the JPEG round trip,
+ *     which waits for the encoded streams), else host pointers and the call waits.  Refused, naming the argument,
+ *     before anything is enqueued: n outside 1 .. 1024, a side outside 2 .. 8192, an edge not a multiple of 8 or
+ *     outside 8 .. 1024, and a params record that does not fit its source (non-integers, a resized size outside
+ *     side / 2 .. side, a crop outside the resized image, an order that is not a permutation, a negative factor or a
+ *     hue outside -0.5 .. 0.5, flags other than 0 / 1, mask bounds outside 0 .. edge).  4 kernels, plus
+ *     b200pose_net_encode_jpegs' and b200pose_net_decode_jpegs' when any sample drew the JPEG round trip.
+ *   b200pose_ground_truth_f64: b200pose_ground_truth for float64 keypoints (a flipped sample's, as horizontal_swap_coco
+ *     returns them): add_neck and the joint centres in float64.  The same checks, layout and launches.
+ * ---------------------------------------------------------------------------------------------------------- */
+#define B200POSE_AUG_PARAMS 19
+int b200pose_net_augment(b200pose_net* net, const unsigned char* frames, int frames_on_device, int n, const int* hw,
+                         const double* params, int edge, float* out_f32, unsigned char* out_u8, int out_on_device,
+                         void* cuda_stream);
+int b200pose_ground_truth_f64(int device, const double* keypoints, const int* persons, const int* hw, int n,
+                              float* heat, float* paf, int canvas_h, int canvas_w, void* cuda_stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Legacy SWIG surface of lib/pafprocess (pafprocess.h:53-59, pafprocess.i:14): same names, same argument
  *    meaning; state is kept in a process-global context exactly like the reference's file-scope globals
  *    (pafprocess.cpp:12-13).  peaks [p1,p2,5] rows (x, y, score, id, part) sorted by part as paf_to_pose_cpp

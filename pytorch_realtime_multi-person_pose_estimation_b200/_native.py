@@ -100,6 +100,8 @@ _SIGNATURES = {      # every exported symbol: (argtypes, restype)
     "b200pose_coco_kpt_eval": ([ci, ci, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp,
                                 ctypes.c_longlong, vp], ci),
     "b200pose_ground_truth": ([ci, vp, vp, vp, ci, vp, vp, ci, ci, vp], ci),
+    "b200pose_ground_truth_f64": ([ci, vp, vp, vp, ci, vp, vp, ci, ci, vp], ci),
+    "b200pose_net_augment": ([vp, vp, ci, ci, vp, vp, ci, vp, vp, ci, vp], ci),
     "b200pose_net_last_forward": ([vp, vp, vp, ci], ci),
     "b200pose_net_stage_losses": ([vp, vp, vp, vp, ci, vp, vp], ci),
     "process_paf": ([ci, ci, ci, vp, ci, ci, ci, vp, ci, ci, ci, vp], ci),

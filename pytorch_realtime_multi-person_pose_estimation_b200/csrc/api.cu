@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/b200pose.h"
+#include "aug.cuh"
 #include "coco_eval.cuh"
 #include "conv_misc.cuh"
 #include "conv_tc.cuh"
@@ -488,6 +489,11 @@ struct b200pose_net {
     // words, IDAT chunks), the gathered zlib streams and the inflated rows
     DevBuf<char> png_in;
     DevBuf<unsigned char> png_zlib, png_rows;
+    // training batches (b200pose_net_augment): the sample table and L sums, staged host frames, the horizontal passes,
+    // the jittered images, the images of the JPEG round trip, and the outputs of a call whose outputs are on the host
+    DevBuf<char> aug_in;
+    DevBuf<unsigned char> aug_src, aug_tmp, aug_px, aug_jpeg, aug_u8;
+    DevBuf<float> aug_out;
     // fp8 mode (DESIGN.md §2.3): amax[launch * n + image] = max |bf16| (fp32 bits) launch (0 = conv1_1) stored for the
     // image; zeroed at the start of every fp8 forward
     DevBuf<unsigned> amax;
@@ -3147,9 +3153,14 @@ int b200pose_coco_kpt_eval(int device, int n_units, int n_cats, const int* unit_
     return 0;
 }
 
+}  // extern "C"
+
 // ------------------------------------------------------------------------------------------------ training targets, stage losses
-int b200pose_ground_truth(int device, const float* keypoints, const int* persons, const int* hw, int n, float* heat,
-                          float* paf, int canvas_h, int canvas_w, void* cuda_stream) {
+namespace {
+// b200pose_ground_truth with keypoints of type T (float32, or float64 after a flip)
+template <class T>
+int ground_truth_impl(int device, const T* keypoints, const int* persons, const int* hw, int n, float* heat, float* paf,
+                      int canvas_h, int canvas_w, void* cuda_stream) {
     if (n < 1 || n > kGtMaxImages) return fail("ground_truth: %d images (1 .. %d)", n, kGtMaxImages);
     if (!persons || !hw) return fail("ground_truth: null persons / sizes");
     long long total = 0;
@@ -3177,9 +3188,9 @@ int b200pose_ground_truth(int device, const float* keypoints, const int* persons
     if (!heat || !paf) return fail("ground_truth: null heat / paf");
     // one upload: the images, then every person's 18 joints (add_neck, our_order, remove_illegal_joint on the host)
     const size_t o_joints = ((size_t)n * sizeof(GtImage) + 255) & ~(size_t)255;
-    std::vector<char> up(o_joints + (size_t)total * kGtParts * 3 * sizeof(float));
+    std::vector<char> up(o_joints + (size_t)total * kGtParts * 3 * sizeof(T));
     GtImage* im = reinterpret_cast<GtImage*>(up.data());
-    float* jo = reinterpret_cast<float*>(up.data() + o_joints);
+    T* jo = reinterpret_cast<T*>(up.data() + o_joints);
     for (int i = 0, j0 = 0; i < n; j0 += persons[i++]) {
         im[i] = {j0, persons[i], gt_grid(hw[2 * i]), gt_grid(hw[2 * i + 1])};
         for (int p = j0; p < j0 + persons[i]; ++p)
@@ -3191,7 +3202,8 @@ int b200pose_ground_truth(int device, const float* keypoints, const int* persons
     CU(cudaMallocAsync(&d, up.size(), st));
     GtBatch b;
     b.images = reinterpret_cast<const GtImage*>(d);
-    b.joints = reinterpret_cast<const float*>(static_cast<char*>(d) + o_joints);
+    b.joints = static_cast<char*>(d) + o_joints;
+    b.f64 = sizeof(T) == 8;
     b.n = n;
     b.ch = canvas_h;
     b.cw = canvas_w;
@@ -3203,6 +3215,157 @@ int b200pose_ground_truth(int device, const float* keypoints, const int* persons
     cudaError_t ef = cudaFreeAsync(d, st);
     if (!rc && ef != cudaSuccess) rc = cuda_fail("ground_truth: cudaFreeAsync: %s", cudaGetErrorString(ef));
     return rc;
+}
+}  // namespace
+
+extern "C" {
+int b200pose_ground_truth(int device, const float* keypoints, const int* persons, const int* hw, int n, float* heat,
+                          float* paf, int canvas_h, int canvas_w, void* cuda_stream) {
+    return ground_truth_impl(device, keypoints, persons, hw, n, heat, paf, canvas_h, canvas_w, cuda_stream);
+}
+
+int b200pose_ground_truth_f64(int device, const double* keypoints, const int* persons, const int* hw, int n,
+                              float* heat, float* paf, int canvas_h, int canvas_w, void* cuda_stream) {
+    return ground_truth_impl(device, keypoints, persons, hw, n, heat, paf, canvas_h, canvas_w, cuda_stream);
+}
+
+// ------------------------------------------------------------------------------------------------ training batches
+int b200pose_net_augment(b200pose_net* net, const unsigned char* frames, int frames_on_device, int n, const int* hw,
+                         const double* params, int edge, float* out_f32, unsigned char* out_u8, int out_on_device,
+                         void* cuda_stream) {
+    if (!net) return fail("null net");
+    if (n < 1 || n > kAugMaxImages) return fail("augment: n = %d images (1 .. %d)", n, kAugMaxImages);
+    if (!frames || !hw || !params || !out_f32) return fail("augment: null frames / hw / params / out_f32");
+    if (edge % 8 || edge < kAugMinEdge || edge > kAugMaxEdge)
+        return fail("augment: edge %d (a multiple of 8, %d .. %d)", edge, kAugMinEdge, kAugMaxEdge);
+    std::vector<AugImage> im(n);
+    std::vector<int> jpeg;
+    long long src_bytes = 0, tmp_bytes = 0;
+    int max_tmp = 0;
+    for (int i = 0; i < n; ++i) {
+        const int h = hw[2 * i], w = hw[2 * i + 1];
+        if (h < kAugMinSide || h > kAugMaxSide || w < kAugMinSide || w > kAugMaxSide)
+            return fail("augment: size of image %d = %d x %d (each side %d .. %d)", i, h, w, kAugMinSide, kAugMaxSide);
+        const double* p = params + (size_t)i * B200POSE_AUG_PARAMS;
+        for (int k = 0; k < B200POSE_AUG_PARAMS; ++k)
+            if (!std::isfinite(p[k]) || ((k < 9 || k > 12) && p[k] != std::floor(p[k])) || std::fabs(p[k]) > 1e6)
+                return fail("augment: params[%d][%d] = %g (finite; an integer except the factors)", i, k, p[k]);
+        AugImage& a = im[i];
+        a.h = h;
+        a.w = w;
+        a.flip = (int)p[0];
+        a.rw = (int)p[1];
+        a.rh = (int)p[2];
+        a.x0 = (int)p[3];
+        a.y0 = (int)p[4];
+        const int jp = (int)p[13];
+        a.gray = (int)p[14];
+        a.mx0 = (int)p[15];
+        a.my0 = (int)p[16];
+        a.mx1 = (int)p[17];
+        a.my1 = (int)p[18];
+        if ((a.flip | jp | a.gray) & ~1) return fail("augment: image %d: hflip, jpeg, grayscale must be 0 or 1", i);
+        if (a.rw < w / 2 || a.rw > w || a.rh < h / 2 || a.rh > h || a.rw < 1 || a.rh < 1)
+            return fail("augment: image %d: resized %d x %d outside %d x %d .. %d x %d", i, a.rh, a.rw, h / 2, w / 2, h, w);
+        if (a.x0 < 0 || a.x0 > std::max(0, a.rw - edge) || a.y0 < 0 || a.y0 > std::max(0, a.rh - edge))
+            return fail("augment: image %d: crop (%d, %d) outside the resized %d x %d image", i, a.x0, a.y0, a.rh, a.rw);
+        unsigned seen = 0;
+        for (int o = 0; o < 4; ++o) {
+            const int op = (int)p[5 + o];
+            if (op < 0 || op > 3 || (seen >> op & 1)) return fail("augment: image %d: order is not a permutation of 0 .. 3", i);
+            seen |= 1u << op;
+            a.order[o] = op;
+        }
+        for (int k = 0; k < 3; ++k) {
+            if (p[9 + k] < 0) return fail("augment: image %d: factor %d = %g is negative", i, k, p[9 + k]);
+            a.f[k] = p[9 + k];
+        }
+        a.f[3] = 0.0;
+        if (p[12] < -0.5 || p[12] > 0.5) return fail("augment: image %d: hue %g outside -0.5 .. 0.5", i, p[12]);
+        a.dh = (int)(p[12] * 255.0) & 255;      // np.int32(hue * 255).astype(uint8)
+        if (a.mx0 < 0 || a.mx0 > a.mx1 || a.mx1 > edge || a.my0 < 0 || a.my0 > a.my1 || a.my1 > edge)
+            return fail("augment: image %d: mask (%d, %d) .. (%d, %d) outside 0 .. %d", i, a.mx0, a.my0, a.mx1, a.my1, edge);
+        a.cw = std::min(edge, a.rw - a.x0);
+        a.ch = std::min(edge, a.rh - a.y0);
+        a.left = (edge - a.cw) / 2;
+        a.top = (edge - a.ch) / 2;
+        int32_t k[kAugMaxTaps];
+        int first, last;
+        aug_taps(h, a.rh, a.y0, &first, k);
+        const int cnt = aug_taps(h, a.rh, a.y0 + a.ch - 1, &last, k);
+        a.r0 = first;
+        a.rows = last + cnt - first;
+        a.src = src_bytes;
+        a.tmp = tmp_bytes;
+        src_bytes += (long long)h * w * 3;
+        tmp_bytes += (long long)a.rows * a.cw * 3;
+        max_tmp = std::max(max_tmp, a.rows * a.cw);
+        if (jp) jpeg.push_back(i);
+    }
+    CU(cudaSetDevice(net->device));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    const size_t frame = (size_t)edge * edge * 3, o_sum = ((size_t)n * sizeof(AugImage) + 255) & ~(size_t)255;
+    CU(net->aug_in.ensure(o_sum + (size_t)n * 8));
+    AugBatch b;
+    b.images = reinterpret_cast<const AugImage*>(net->aug_in.p);
+    b.lsum = reinterpret_cast<unsigned long long*>(net->aug_in.p + o_sum);
+    b.src = frames;
+    if (!frames_on_device) {
+        CU(net->aug_src.ensure((size_t)src_bytes));
+        CU(cudaMemcpyAsync(net->aug_src.p, frames, (size_t)src_bytes, cudaMemcpyHostToDevice, st));
+        b.src = net->aug_src.p;
+    }
+    CU(net->aug_tmp.ensure((size_t)tmp_bytes));
+    CU(net->aug_px.ensure((size_t)n * frame));
+    b.tmp = net->aug_tmp.p;
+    b.px = net->aug_px.p;
+    b.out = out_f32;
+    b.out_u8 = out_u8;
+    if (!out_on_device) {
+        CU(net->aug_out.ensure((size_t)n * frame));
+        b.out = net->aug_out.p;
+        if (out_u8) {
+            CU(net->aug_u8.ensure((size_t)n * frame));
+            b.out_u8 = net->aug_u8.p;
+        }
+    }
+    b.n = n;
+    b.edge = edge;
+    b.max_tmp_px = max_tmp;
+    CU(cudaMemcpyAsync(net->aug_in.p, im.data(), (size_t)n * sizeof(AugImage), cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(b.lsum, 0, (size_t)n * 8, st));
+    if (int rc = launched(aug_jitter_launch(b, st), "aug_jitter_launch", kAugLaunchesJitter)) return rc;
+    if (!jpeg.empty()) {
+        // jpeg_compression_augmentation: Pillow's save(quality=50) + Image.open equal cv2.imencode(q=50, 4:2:0) +
+        // cv2.imdecode, which the device encoder and decoder reproduce.  The sampled images go through them packed.
+        const int nj = (int)jpeg.size();
+        CU(net->aug_jpeg.ensure((size_t)nj * frame));
+        for (int k = 0; k < nj; ++k)
+            CU(cudaMemcpyAsync(net->aug_jpeg.p + k * frame, net->aug_px.p + jpeg[k] * frame, frame,
+                               cudaMemcpyDeviceToDevice, st));
+        const int sampling = 0x221111;
+        const long long bound = b200pose_jpeg_encode_bound(edge, edge, sampling);
+        if (bound < 0) return 1;
+        std::vector<unsigned char> streams((size_t)bound * nj);
+        std::vector<long long> lens(nj);
+        std::vector<int> jhw(2 * nj, edge);
+        if (int rc = b200pose_net_encode_jpegs(net, net->aug_jpeg.p, 1, jhw.data(), nj, 50, sampling, streams.data(),
+                                               bound * nj, 0, lens.data(), st))
+            return rc;
+        std::vector<const unsigned char*> ptrs(nj);
+        for (int k = 0, at = 0; k < nj; at += (int)lens[k++]) ptrs[k] = streams.data() + at;
+        if (int rc = b200pose_net_decode_jpegs(net, ptrs.data(), lens.data(), nj, net->aug_jpeg.p, 1, st)) return rc;
+        for (int k = 0; k < nj; ++k)
+            CU(cudaMemcpyAsync(net->aug_px.p + jpeg[k] * frame, net->aug_jpeg.p + k * frame, frame,
+                               cudaMemcpyDeviceToDevice, st));
+    }
+    if (int rc = launched(aug_finish_launch(b, st), "aug_finish_launch", kAugLaunchesFinish)) return rc;
+    if (!out_on_device) {
+        CU(cudaMemcpyAsync(out_f32, b.out, (size_t)n * frame * 4, cudaMemcpyDeviceToHost, st));
+        if (out_u8) CU(cudaMemcpyAsync(out_u8, b.out_u8, (size_t)n * frame, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+    }
+    return 0;
 }
 
 int b200pose_net_last_forward(b200pose_net* net, int* info, int* hw, int hw_cap) {

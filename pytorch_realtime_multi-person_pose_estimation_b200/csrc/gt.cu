@@ -1,50 +1,9 @@
-// COCO training targets and stage losses on the device (gt.cuh; arithmetic in gt_core.h, DESIGN.md 2.19).
+// COCO training targets and stage losses on the device (gt.cuh, whose kernels this file instantiates for float32
+// joints; arithmetic in gt_core.h, DESIGN.md 2.19).
 #include "gt.cuh"
 
 namespace b2p {
 namespace {
-
-constexpr int kThreads = 128;
-
-// One thread per (image, canvas cell): the 18 part channels, each over the image's persons in order, then the
-// background from their maximum.  Cells outside the image's grid get +0 in every channel.
-__global__ void __launch_bounds__(kThreads) gt_heat_kernel(GtBatch b) {
-    const long long plane = (long long)b.ch * b.cw;
-    const long long t = (long long)blockIdx.x * kThreads + threadIdx.x;
-    if (t >= plane * b.n) return;
-    const int i = (int)(t / plane);
-    const long long at = t - (long long)i * plane;
-    const int y = (int)(at / b.cw), x = (int)(at - (long long)y * b.cw);
-    const GtImage im = b.images[i];
-    const bool in = y < im.gh && x < im.gw;
-    const float* jo = b.joints + (size_t)im.j0 * kGtParts * 3;
-    float* out = b.heat + (size_t)i * kGtHeat * plane + at;
-    double mx = 0.0;
-    for (int c = 0; c < kGtParts; ++c) {
-        const double v = in ? gt_heat_part(jo, im.np, c, x, y) : 0.0;
-        mx = v > mx ? v : mx;
-        out[c * plane] = __double2float_rn(v);
-    }
-    out[kGtParts * plane] = in ? __double2float_rn(gt_background(mx)) : 0.0f;
-}
-
-// One thread per (image, limb, canvas cell): the limb's x and y channels over the image's persons in order.
-__global__ void __launch_bounds__(kThreads) gt_paf_kernel(GtBatch b) {
-    const long long plane = (long long)b.ch * b.cw;
-    const long long t = (long long)blockIdx.x * kThreads + threadIdx.x;
-    if (t >= plane * b.n * kGtLimbs) return;
-    const long long il = t / plane;
-    const int i = (int)(il / kGtLimbs), l = (int)(il - (long long)i * kGtLimbs);
-    const long long at = t - il * plane;
-    const int y = (int)(at / b.cw), x = (int)(at - (long long)y * b.cw);
-    const GtImage im = b.images[i];
-    double vx = 0.0, vy = 0.0;
-    const bool in = y < im.gh && x < im.gw;
-    if (in) gt_paf_limb(b.joints + (size_t)im.j0 * kGtParts * 3, im.np, l, im.gw, im.gh, x, y, &vx, &vy);
-    float* out = b.paf + ((size_t)i * kGtPaf + 2 * l) * plane + at;
-    out[0] = in ? __double2float_rn(vx) : 0.0f;
-    out[plane] = in ? __double2float_rn(vy) : 0.0f;
-}
 
 // NaN-propagating max / min, as torch.max / torch.min
 __device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
@@ -105,14 +64,7 @@ __global__ void __launch_bounds__(kGtLossThreads) gt_stage_loss_kernel(GtLossBat
 
 }  // namespace
 
-cudaError_t gt_launch(const GtBatch& b, cudaStream_t s) {
-    const long long cells = (long long)b.n * b.ch * b.cw;
-    gt_heat_kernel<<<(unsigned)((cells + kThreads - 1) / kThreads), kThreads, 0, s>>>(b);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    gt_paf_kernel<<<(unsigned)((cells * kGtLimbs + kThreads - 1) / kThreads), kThreads, 0, s>>>(b);
-    return cudaGetLastError();
-}
+cudaError_t gt_launch(const GtBatch& b, cudaStream_t s) { return b.f64 ? gt_launch_f64(b, s) : gt_launch_t<float>(b, s); }
 
 cudaError_t gt_stage_loss_launch(const GtLossBatch& b, cudaStream_t s) {
     gt_stage_loss_kernel<<<dim3(b.n_maps, b.n), kGtLossThreads, 0, s>>>(b);

@@ -1,8 +1,8 @@
 // COCO training targets, host/device shared core: what CocoKeypoints.get_ground_truth (lib/datasets/datasets.py:259-308,
 // with add_neck :227-257 and remove_illegal_joint :216-225) builds with putGaussianMaps (lib/datasets/heatmap.py:20-36)
 // and putVecMaps (lib/datasets/paf.py:18-68), restated (DESIGN.md 2.19):
-//  * gt_person_joints: per person the 17 COCO keypoints (float32, as transforms.Normalize leaves them) gain the neck
-//    (r_shoulder + l_shoulder) / 2 in float32, visibility 2 if both are 2 else their product, np.round (half to even) on
+//  * gt_person_joints: per person the 17 COCO keypoints (float32, as transforms.Normalize leaves them, or float64 after
+//    transforms.HFlip) gain the neck (r_shoulder + l_shoulder) / 2 in that dtype, visibility 2 if both are 2 else their product, np.round (half to even) on
 //    x, y and v; reordered to the 18-part order; a joint at x >= input_x, x < 0, y >= input_y or y < 0 becomes (-1, -1, 0);
 //  * heat maps (gt_heat_term): per part, persons in annotation order, += exp(-d2 / 2 / sigma / sigma) where the exponent
 //    is <= 4.6052, clamped to 1 after each person; background max(1 - max over the 18 parts, 0);
@@ -91,24 +91,29 @@ B2P_GT_HD double gt_exp(double x) {
     return GT_MUL(e, two_k);
 }
 
-// add_neck + our_order + remove_illegal_joint of one person: kp [17][3] float32 -> j [18][3] float32.  input_x /
-// input_y: the image's width and height.
-B2P_GT_HD void gt_person_joints(const float* kp, int input_x, int input_y, float* j) {
-    const float* rs = kp + 3 * 6;
-    const float* ls = kp + 3 * 5;
-    float neck[3];
-    for (int t = 0; t < 2; ++t) neck[t] = (rs[t] + ls[t]) / 2.0f;
-    neck[2] = (rs[2] == 2.0f && ls[2] == 2.0f) ? 2.0f : rs[2] * ls[2];
-    for (int t = 0; t < 3; ++t) neck[t] = rintf(neck[t]);      // np.round: half to even
-    const float fx = (float)input_x, fy = (float)input_y;
+// np.round (half to even) in the keypoints' own precision
+B2P_GT_HD float gt_round(float v) { return rintf(v); }
+B2P_GT_HD double gt_round(double v) { return GT_RINT(v); }
+
+// add_neck + our_order + remove_illegal_joint of one person: kp [17][3] -> j [18][3], in the keypoints' dtype T: float32
+// as transforms.Normalize leaves them, float64 after HFlip (horizontal_swap_coco returns float64, and every later step
+// keeps it).  input_x / input_y: the image's width and height.
+template <class T> B2P_GT_HD void gt_person_joints(const T* kp, int input_x, int input_y, T* j) {
+    const T* rs = kp + 3 * 6;
+    const T* ls = kp + 3 * 5;
+    T neck[3];
+    for (int t = 0; t < 2; ++t) neck[t] = (rs[t] + ls[t]) / (T)2;
+    neck[2] = (rs[2] == (T)2 && ls[2] == (T)2) ? (T)2 : rs[2] * ls[2];
+    for (int t = 0; t < 3; ++t) neck[t] = gt_round(neck[t]);
+    const T fx = (T)input_x, fy = (T)input_y;
     for (int p = 0; p < kGtParts; ++p) {
         const int s = gt_source_part(p);
-        const float* src = s == kGtCocoParts ? neck : kp + 3 * s;
-        const float x = src[0], y = src[1];
+        const T* src = s == kGtCocoParts ? neck : kp + 3 * s;
+        const T x = src[0], y = src[1];
         if (x >= fx || x < 0.0f || y >= fy || y < 0.0f) {
-            j[3 * p] = -1.0f;
-            j[3 * p + 1] = -1.0f;
-            j[3 * p + 2] = 0.0f;
+            j[3 * p] = (T)-1;
+            j[3 * p + 1] = (T)-1;
+            j[3 * p + 2] = (T)0;
         } else {
             j[3 * p] = x;
             j[3 * p + 1] = y;
@@ -118,7 +123,7 @@ B2P_GT_HD void gt_person_joints(const float* kp, int input_x, int input_y, float
 }
 
 // putGaussianMaps' term of a joint at (cx, cy) for grid cell (gx, gy): exp(-exponent) where exponent <= 4.6052, else 0.
-B2P_GT_HD double gt_heat_term(float cx, float cy, int gx, int gy) {
+template <class T> B2P_GT_HD double gt_heat_term(T cx, T cy, int gx, int gy) {
     const double start = kGtStride / 2.0 - 0.5;
     const double dx = GT_SUB(GT_ADD((double)(gx * kGtStride), start), (double)cx);
     const double dy = GT_SUB(GT_ADD((double)(gy * kGtStride), start), (double)cy);
@@ -129,10 +134,10 @@ B2P_GT_HD double gt_heat_term(float cx, float cy, int gx, int gy) {
 
 // Heat-map channel p (0 .. 17) at cell (gx, gy) over np persons' joints [np][18][3]: accumulated in order, clamped to
 // 1 after each person.
-B2P_GT_HD double gt_heat_part(const float* joints, int np, int p, int gx, int gy) {
+template <class T> B2P_GT_HD double gt_heat_part(const T* joints, int np, int p, int gx, int gy) {
     double acc = 0.0;
     for (int i = 0; i < np; ++i) {
-        const float* jo = joints + (i * kGtParts + p) * 3;
+        const T* jo = joints + (i * kGtParts + p) * 3;
         if (jo[2] > 0.5f) {
             acc = GT_ADD(acc, gt_heat_term(jo[0], jo[1], gx, gy));
             if (acc > 1.0) acc = 1.0;
@@ -155,7 +160,7 @@ struct GtLimb {
 
 // putVecMaps' set-up for joints ja, jb ([3] each): false when either is not visible (v <= 0.5) or the limb has zero
 // length, which putVecMaps skips without touching the maps.
-B2P_GT_HD bool gt_limb_setup(const float* ja, const float* jb, int grid_x, int grid_y, GtLimb* L) {
+template <class T> B2P_GT_HD bool gt_limb_setup(const T* ja, const T* jb, int grid_x, int grid_y, GtLimb* L) {
     if (!(ja[2] > 0.5f && jb[2] > 0.5f)) return false;
     const double ax = GT_DIV((double)ja[0], (double)kGtStride), ay = GT_DIV((double)ja[1], (double)kGtStride);
     const double bx = GT_DIV((double)jb[0], (double)kGtStride), by = GT_DIV((double)jb[1], (double)kGtStride);
@@ -199,8 +204,8 @@ B2P_GT_HD void gt_paf_step(const GtLimb& L, int gx, int gy, double& vx, double& 
 }
 
 // PAF channels 2l, 2l + 1 of limb l at cell (gx, gy) over np persons' joints [np][18][3], persons in order.
-B2P_GT_HD void gt_paf_limb(const float* joints, int np, int l, int grid_x, int grid_y, int gx, int gy, double* vx,
-                           double* vy) {
+template <class T>
+B2P_GT_HD void gt_paf_limb(const T* joints, int np, int l, int grid_x, int grid_y, int gx, int gy, double* vx, double* vy) {
     double x = 0.0, y = 0.0;
     int count = 0;
     const int a = gt_limb_a(l), b = gt_limb_b(l);

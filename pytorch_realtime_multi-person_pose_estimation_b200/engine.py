@@ -201,33 +201,125 @@ def rotated_size(h, w, rotate):
 GT_MAX_IMAGES, GT_MAX_PERSONS = 1024, 256      # b200pose_ground_truth's capacities
 
 
-def ground_truth(keypoints_per_image, sizes, device_index=0, canvas=None):
+def ground_truth(keypoints_per_image, sizes, device_index=0, canvas=None, float64=False):
     """CocoKeypoints.get_ground_truth (lib/datasets/datasets.py:259-308) + transpose((2, 0, 1)).astype(float32) for a
     batch of images, on the device, bit for bit the reference's maps (DESIGN.md 2.19).  keypoints_per_image[i]: the
     image's annotations' keypoints, [P_i, 17, 3] (or [P_i, 51]) in COCO order, as float32 after transforms.Normalize;
     sizes[i] = (input_y, input_x).  Returns CUDA float32 tensors heat [n, 19, gh, gw] and paf [n, 38, gh, gw] on
     cuda:device_index, written on its current stream, at the canvas grid (max int(input_y / 8), max int(input_x / 8)),
     or `canvas` = (gh, gw) if given: image i fills the top-left of its slot, +0 outside.  An image without persons gets
-    zero PAFs and a background of 1 (the reference raises IndexError)."""
+    zero PAFs and a background of 1 (the reference raises IndexError).  float64=True: the keypoints are float64, as
+    they are after transforms.HFlip (augment_keypoints), and add_neck and the joint centres run in float64
+    (b200pose_ground_truth_f64)."""
     import torch
-    kps = [np.ascontiguousarray(k, dtype=np.float32).reshape(-1, 17, 3) for k in keypoints_per_image]
+    dt = np.float64 if float64 else np.float32
+    kps = [np.ascontiguousarray(k, dtype=dt).reshape(-1, 17, 3) for k in keypoints_per_image]
     hw = np.ascontiguousarray(np.asarray(sizes, dtype=np.int64).reshape(-1, 2).astype(np.int32))
     if len(kps) != len(hw):
         raise nat.B200PoseError("ground_truth: %d keypoint arrays for %d sizes" % (len(kps), len(hw)))
     n = len(hw)
-    table = np.ascontiguousarray(np.concatenate(kps) if n else np.zeros((0, 17, 3), np.float32))
+    table = np.ascontiguousarray(np.concatenate(kps) if n else np.zeros((0, 17, 3), dt))
     counts = np.array([len(k) for k in kps], np.int32)
     gh, gw = canvas or ((int(hw[:, 0].max()) // 8, int(hw[:, 1].max()) // 8) if n else (0, 0))
     L = nat.lib()
+    name = "b200pose_ground_truth_f64" if float64 else "b200pose_ground_truth"
+    call = getattr(L, name)
     args = (table.ctypes.data, counts.ctypes.data, hw.ctypes.data, n)
-    nat.check(L.b200pose_ground_truth(int(device_index), *args, None, None, gh, gw, None), "b200pose_ground_truth")
+    nat.check(call(int(device_index), *args, None, None, gh, gw, None), name)
     dev = torch.device("cuda", int(device_index))
     heat = torch.empty((n, 19, gh, gw), dtype=torch.float32, device=dev)
     paf = torch.empty((n, 38, gh, gw), dtype=torch.float32, device=dev)
-    nat.check(L.b200pose_ground_truth(int(device_index), *args, ctypes.c_void_p(heat.data_ptr()),
-                                      ctypes.c_void_p(paf.data_ptr()), gh, gw,
-                                      ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "b200pose_ground_truth")
+    nat.check(call(int(device_index), *args, ctypes.c_void_p(heat.data_ptr()), ctypes.c_void_p(paf.data_ptr()), gh, gw,
+                   ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), name)
     return heat, paf
+
+
+# ------------------------------------------------------------------------------------ training batches (DESIGN.md 2.20)
+AUG_PARAMS = 19          # B200POSE_AUG_PARAMS: doubles per sample of b200pose_net_augment
+AUG_PAD = (124, 116, 104)
+# horizontal_swap_coco (lib/datasets/utils.py:8-21): target index of each COCO keypoint after a flip
+COCO_HFLIP = (0, 2, 1, 4, 3, 6, 5, 8, 7, 10, 9, 12, 11, 14, 13, 16, 15)
+
+
+def augment_params(sizes, generator=None, edge=368):
+    """The random draws of the reference's training loader (train/train_VGG19.py:124-130 preprocess, then
+    lib/datasets/transforms.py:53-65 image_transform_train) for images of sizes[i] = (h, w), one sample after the other
+    in the reference's order: RandomApply(HFlip, 0.5), RescaleRelative, Crop(edge) (x, then y, each only when the
+    resized side exceeds edge), CenterPad(edge), ColorJitter.get_params (randperm(4), then brightness, contrast,
+    saturation and hue factors), RandomApply(jpeg_compression_augmentation, 0.1) and RandomGrayscale(0.01).
+    generator=None draws from torch's global generator, as the reference does.  Returns one dict per sample; its
+    'valid_area' is meta['valid_area'] computed in float64 as Crop and CenterPad compute it, and 'mask' the bounds
+    (x0, y0, x1, y1) mask_valid_area (lib/datasets/utils.py:36-54) derives from it."""
+    import math
+    import torch
+    g = {} if generator is None else {"generator": generator}
+    edge = int(edge)
+    out = []
+    for h, w in sizes:
+        h, w = int(h), int(w)
+        flip = not float(torch.rand(1, **g).item()) > 0.5
+        factor = 0.5 + torch.rand(1, **g).item() * (1.0 - 0.5)
+        rw, rh = int(w * factor), int(h * factor)
+        xs, ys = rw / w, rh / h
+        va = np.array((0.0, 0.0, w, h))
+        if flip:
+            va[0] = -(va[0] + va[2]) + w
+        va[:2] *= (xs, ys)
+        va[2:] *= (xs, ys)
+        pad = int(edge / 2.0)
+        x0 = y0 = 0
+        if rw > edge:
+            x0 = torch.clamp(torch.randint(-pad, rw - edge + pad, (1,), **g), min=0, max=rw - edge).item()
+        if rh > edge:
+            y0 = torch.clamp(torch.randint(-pad, rh - edge + pad, (1,), **g), min=0, max=rh - edge).item()
+        cw, ch = min(edge, rw - x0), min(edge, rh - y0)
+        ltrb = np.array((x0, y0, x0 + cw, y0 + ch))
+        va[:2] = np.maximum(0.0, va[:2] - ltrb[:2])
+        va[2:] = np.maximum(0.0, va[2:] - ltrb[:2])
+        va[2:] = np.minimum(va[2:], ltrb[2:] - ltrb[:2])
+        left, top = int((edge - cw) / 2.0), int((edge - ch) / 2.0)
+        va[:2] += (left, top)
+        order = [int(v) for v in torch.randperm(4, **g)]
+        fb, fc, fs = (float(torch.empty(1).uniform_(0.9, 1.1, **g)) for _ in range(3))
+        fh = float(torch.empty(1).uniform_(-0.1, 0.1, **g))
+        jpeg = not 0.1 < torch.rand(1, **g)
+        gray = bool(torch.rand(1, **g) < 0.01)
+        mask = (int(va[0]) if va[0] >= 1.0 else 0, int(va[1]) if va[1] >= 1.0 else 0,
+                min(int(math.ceil(va[0] + va[2])), edge), min(int(math.ceil(va[1] + va[3])), edge))
+        out.append({"size": (h, w), "edge": edge, "hflip": flip, "scale_factor": factor, "resized": (rw, rh),
+                    "scale": (xs, ys), "crop": (x0, y0), "cropped": (cw, ch), "pad": (left, top),
+                    "valid_area": va, "order": order, "factors": (fb, fc, fs, fh), "jpeg": bool(jpeg), "gray": gray,
+                    "mask": mask})
+    return out
+
+
+def augment_table(params):
+    """augment_params' records as b200pose_net_augment's params [n][AUG_PARAMS] (float64)."""
+    t = np.zeros((len(params), AUG_PARAMS), np.float64)
+    for i, p in enumerate(params):
+        t[i] = ([p["hflip"], p["resized"][0], p["resized"][1], p["crop"][0], p["crop"][1]] + list(p["order"])
+                + list(p["factors"]) + [p["jpeg"], p["gray"]] + list(p["mask"]))
+    return t
+
+
+def augment_keypoints(keypoints, params):
+    """Each image's keypoints [P, 17, 3] (COCO order, source pixels) through the preprocess steps of its record, as the
+    reference maps them: float32 throughout (transforms.Normalize) for a sample without a flip; for a flipped one, the
+    flip in float32, then horizontal_swap_coco's float64 copy, and every later step in float64."""
+    out = []
+    for k, p in zip(keypoints, params):
+        k = np.array(k, dtype=np.float32).reshape(-1, 17, 3)
+        if p["hflip"]:
+            k[:, :, 0] = -k[:, :, 0] - 1.0 + p["size"][1]
+            swapped = np.zeros(k.shape)
+            swapped[:, list(COCO_HFLIP)] = k
+            k = swapped
+        for ax in (0, 1):
+            k[:, :, ax] = (k[:, :, ax] + 0.5) * p["scale"][ax] - 0.5
+            k[:, :, ax] -= p["crop"][ax]
+            k[:, :, ax] += p["pad"][ax]
+        out.append(k)
+    return out
 
 
 def _loss_dict(names_flags, sums, extrema, cells):
@@ -575,6 +667,35 @@ class NativeNet:
                             lambda src, dev_in, hw, n, out, cap, dev_out, lens, st: L.b200pose_net_encode_pngs(
                                 self._h, src, dev_in, hw, n, out, cap, dev_out, lens, st),
                             device, stream)
+
+    def augment(self, frames, params, edge=368, uint8=False):
+        """The reference loader's image path for each frame (b200pose_net_augment, DESIGN.md 2.20): the preprocess and
+        image_transform_train draws of params[i] (augment_params' records) applied to uint8 BGR frames of any sizes (a
+        list of numpy arrays, or of CUDA uint8 tensors [h, w, 3] on the net's device), then mask_valid_area.  Returns a
+        CUDA float32 tensor [n, 3, edge, edge] (RGB, normalised), written on the current stream, and with uint8=True
+        also the uint8 BGR images ToTensor receives [n, edge, edge, 3]."""
+        import torch
+        src, dev_in, sizes, flat = self._frames_to_encode(frames, "augment")
+        n = len(sizes)
+        if n != len(params):
+            raise nat.B200PoseError("augment: %d frames but %d params records" % (n, len(params)))
+        for (h, w), p in zip(sizes, params):
+            if tuple(p["size"]) != (int(h), int(w)) or int(p["edge"]) != int(edge):
+                raise nat.B200PoseError("augment: a params record for %s at edge %d, given a %d x %d frame at edge %d"
+                                        % (tuple(p["size"]), p["edge"], h, w, edge))
+        table = augment_table(params)
+        hw = np.array([int(v) for s in sizes for v in s], np.int32)
+        dev = torch.device("cuda", self.device_index)
+        E = int(edge)
+        out = torch.empty((n, 3, E, E), dtype=torch.float32, device=dev)
+        u8 = torch.empty((n, E, E, 3), dtype=torch.uint8, device=dev) if uint8 else None
+        nat.check(nat.lib().b200pose_net_augment(self._h, ctypes.c_void_p(src), int(dev_in), n, hw.ctypes.data,
+                                                 table.ctypes.data, E, ctypes.c_void_p(out.data_ptr()),
+                                                 ctypes.c_void_p(u8.data_ptr() if uint8 else None), 1,
+                                                 ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                  "b200pose_net_augment")
+        del flat
+        return (out, u8) if uint8 else out
 
     def __del__(self):
         try:
@@ -1247,6 +1368,60 @@ class PoseEngine:
                 self.net.forward_ragged_u8_ptr(batch.data_ptr(), True, shapes, self.mode, [None] * 12, True, stream)
             canvas = (max(h for h, _ in shapes) // 8, max(w for _, w in shapes) // 8)
             heat, paf = ground_truth(kps, shapes, self.device_index, canvas)
+            s, e, c, names = self.net.stage_loss_sums(heat, paf)
+            sums = sums + s.sum(0)
+            extrema.append(e)
+            cells += sum(c)
+        return _loss_dict(names, sums, np.concatenate(extrema), cells)
+
+    def training_batch(self, images, keypoints, generator=None, edge=368, params=None):
+        """One collated batch of the reference's training loader (CocoKeypoints.__getitem__ with preprocess =
+        Normalize, RandomApply(HFlip), RescaleRelative, Crop(edge), CenterPad(edge), image_transform_train,
+        mask_valid_area and get_ground_truth at input_x = input_y = edge; DESIGN.md 2.20) for uint8 BGR frames
+        images[i] and their annotations' keypoints [P_i, 17, 3] (COCO order, source pixels), drawing from `generator`
+        (None: torch's global generator) sample after sample as augment_params does, or from `params` if given.
+        Returns CUDA float32 tensors (images [B, 3, edge, edge], heat [B, 19, edge / 8, edge / 8],
+        paf [B, 38, edge / 8, edge / 8]) on the current stream.  Flipped samples' targets come from float64 keypoints."""
+        import torch
+        if len(images) != len(keypoints):
+            raise nat.B200PoseError("training_batch: %d images but %d keypoint arrays" % (len(images), len(keypoints)))
+        if not len(images):
+            raise nat.B200PoseError("training_batch: images is empty")
+        if params is None:
+            params = augment_params([im.shape[:2] for im in images], generator, edge)
+        x = self.net.augment(images, params, edge)
+        kps = augment_keypoints(keypoints, params)
+        g = int(edge) // 8
+        dev = torch.device("cuda", self.device_index)
+        heat = torch.empty((len(images), 19, g, g), dtype=torch.float32, device=dev)
+        paf = torch.empty((len(images), 38, g, g), dtype=torch.float32, device=dev)
+        for f64 in (False, True):
+            idx = [i for i, p in enumerate(params) if p["hflip"] == f64]
+            if idx:
+                h, p = ground_truth([kps[i] for i in idx], [(edge, edge)] * len(idx), self.device_index, (g, g), f64)
+                heat[idx], paf[idx] = h, p
+        return x, heat, paf
+
+    def augmented_validation_loss(self, images, keypoints, generator=None, edge=368):
+        """validate() (train/train_VGG19.py:233-278) under the reference's own protocol: every image through
+        training_batch (random flip, rescale, crop, pad, colour jitter, JPEG, grayscale drawn from `generator`, or torch's
+        global generator), in batches of at most batch_cap, the float batch through the net in this engine's mode, and
+        the stage losses against the batch's targets.  Returns validation_loss's dict: dataset-mean MSEs per stage map,
+        total_loss and the extrema over the whole set."""
+        import torch
+        if len(images) != len(keypoints):
+            raise nat.B200PoseError("augmented_validation_loss: %d images but %d keypoint arrays"
+                                    % (len(images), len(keypoints)))
+        if not len(images):
+            raise nat.B200PoseError("augmented_validation_loss: images is empty")
+        stream = torch.cuda.current_stream(torch.device("cuda", self.device_index)).cuda_stream
+        cap = self.post.batch_cap
+        sums, extrema, cells, names = 0.0, [], 0, None
+        for at in range(0, len(images), cap):
+            x, heat, paf = self.training_batch(images[at:at + cap], keypoints[at:at + cap], generator, edge)
+            self._net_h()
+            self.net.forward_ptr(x.data_ptr(), True, x.shape[0], int(edge), int(edge), self.mode, [None] * 12, True,
+                                 stream)
             s, e, c, names = self.net.stage_loss_sums(heat, paf)
             sums = sums + s.sum(0)
             extrema.append(e)
